@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py — STEGO correspondence-distillation training step on B200 (BASELINE.json metric).
+"""bench.py — STEGO correspondence-distillation training step on H100 (BASELINE.json metric).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--config c1|c2|c3|c4] [--impl ours|reference|torch-eager]
+                    [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 ... bench.py --gpus N ...
 
 A "step" is one full training step of the hot path on one synthetic batch per GPU: 2x frozen DINO ViT
@@ -13,16 +14,20 @@ One JSON line on rank 0:
   e2e        same metric through the public API with pinned-host inputs copied H2D and the loss read back
              D2H inside the timed region, every step
   roofline   the dominant kernel of the step, timed live with CUDA events; achieved = algorithmic FLOPs/launch
-             / measured duration; peak from MEASURED_PEAKS.json (burst figure: kernel timed alone)
+             / measured duration; peak from MEASURED_PEAKS.json, else the H100 SXM data-sheet figure
   corr_roofline  the named correlation+loss kernel against BOTH the bf16 tensor peak and the HBM peak
   cpu_baseline   the oracle port (CPU restatement of the reference, oracle/stego_oracle.py) on the host cores,
                  bounded sample
-  sustained      the same device-resident loop run for >= 5 s with its own clock record
-`--impl reference` times the reference's CPU path alone (rank 0 only; the REAL reference classes from baseline/_ref
-through oracle/lightning_harness.py when that copy is present — `cpu_baseline.kind` "reference" — else the oracle port)
-and prints the same line shape.  `--impl torch-eager` runs the unmodified reference modules.py / vision_transformer.py /
-training_step text in PyTorch eager ON THE GPU (fp32 defaults and bf16 autocast) plus the library kernels (cuBLAS
-GEMMs, SDPA) at the step's shapes: the "reference PyTorch path on B200" comparator (SURVEY.md §2.2, BASELINE.md §5).
+  sustained      with --sustain-seconds S > 0: the same device-resident loop run for >= S s with its own clock record
+Every timed loop runs exactly --steps steps after its warm-up.  `--dump-outputs DIR` writes, after the timed loop, what
+its last step returned to the caller: the loss and the logged loss terms, and the trainable parameters and their
+gradients after that step, as DIR/<name>.npy (float32).  Inputs, initial weights and random draws are seeded, so two
+builds run with the same arguments can be compared output for output.
+`--impl reference` times the reference's CPU path alone (rank 0 only; the REAL reference classes from the checkout
+$STEGO_REFERENCE_SRC names, through oracle/lightning_harness.py, when it is set — `cpu_baseline.kind` "reference" —
+else the oracle port) and prints the same line shape.  `--impl torch-eager` runs the unmodified reference modules.py /
+vision_transformer.py / training_step text in PyTorch eager ON THE GPU (fp32 defaults and bf16 autocast) plus the library
+kernels (cuBLAS GEMMs, SDPA) at the step's shapes: the "reference PyTorch path" comparator (SURVEY.md §2.2, BASELINE.md §5).
 """
 from __future__ import annotations
 
@@ -58,7 +63,8 @@ def load_peaks():
         d = json.load(open(p))
         return dict(hbm=d["hbm_gbs"], tf_burst=d["bf16_tflops"], tf_sust=d.get("bf16_tflops_sustained", d["bf16_tflops"]),
                     source="measured (MEASURED_PEAKS.json)")
-    return dict(hbm=6650.0, tf_burst=1590.0, tf_sust=1400.0, source="fallback (B200_PROFILING.md)")
+    # not measured: NVIDIA's H100 SXM data sheet (3.35 TB/s HBM3, 989 TFLOP/s dense BF16 at up to 700 W)
+    return dict(hbm=3350.0, tf_burst=989.0, tf_sust=989.0, source="H100 SXM data sheet (dense BF16, 700 W), not measured")
 
 
 # ----------------------------------------------------------------------------------------------------
@@ -84,7 +90,7 @@ def step_flops_per_image(model_type, res):
 
 
 # ----------------------------------------------------------------------------------------------------
-# clocks sampling (B200_PROFILING.md recipe)
+# clocks sampling (nvidia-smi queries while the timed loop runs)
 # ----------------------------------------------------------------------------------------------------
 class ClockSampler:
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
@@ -205,8 +211,8 @@ def time_cpu(model_type, res, batch, steps, warmup, budget_s=150.0):
 
 def reference_step_fn(model_type, res, batch, device, autocast=False):
     """One training step of the REAL reference (src/train_segmentation.py:112-245 over src/modules.py and
-    src/dino/vision_transformer.py, all unmodified, from baseline/_ref) behind the stub-Lightning harness.  Returns
-    step() or None when the reference copy is not present."""
+    src/dino/vision_transformer.py, all unmodified, from $STEGO_REFERENCE_SRC) behind the stub-Lightning harness.  Returns
+    step() or None when no reference checkout is named."""
     sys.path.insert(0, os.path.join(ROOT, "oracle"))
     import lightning_harness as H
     if not H.available():
@@ -276,7 +282,7 @@ def time_reference_cpu(model_type, res, batch, steps, warmup, budget_s=150.0):
 
 
 def run_torch_eager(args, cfgd, workload):
-    """The reference PyTorch path on the B200: unmodified reference modules in eager mode (what PyTorch 2.11 dispatches
+    """The reference PyTorch path on the GPU: unmodified reference modules in eager mode (what PyTorch 2.11 dispatches
     — cuBLAS / cuDNN / ATen), fp32 (PyTorch defaults: TF32 off for matmul) and under bf16 autocast, plus the library
     kernels at the step's GEMM / attention shapes.  One JSON line; `value` is the bf16-autocast images/s."""
     import torch.nn.functional as F
@@ -288,7 +294,7 @@ def run_torch_eager(args, cfgd, workload):
         try:
             step = reference_step_fn(model_type, res, B, dev, autocast=ac)
             if step is None:
-                print(json.dumps({"impl": "torch-eager", "unavailable": "baseline/_ref (reference copy) not present"}))
+                print(json.dumps({"impl": "torch-eager", "unavailable": "no reference checkout (STEGO_REFERENCE_SRC)"}))
                 return
             for _ in range(max(args.warmup, 3)):
                 step()
@@ -336,7 +342,7 @@ def run_torch_eager(args, cfgd, workload):
         "dtype": "bf16 autocast (value) / fp32", "data": "synthetic",
         "config": {"workload": workload, "global_batch": B, "parallelism": "dp1",
                    "what": "unmodified reference modules.py + dino/vision_transformer.py + training_step text "
-                           "(baseline/_ref) in PyTorch eager on the B200"},
+                           "($STEGO_REFERENCE_SRC) in PyTorch eager on the GPU"},
         "modes": out, "library_kernels": lib}))
 
 
@@ -351,7 +357,7 @@ def time_kernel(fn, iters=10, flush=None):
     tot = 0.0
     for _ in range(iters):
         if flush is not None:
-            flush.add_(1.0)  # > L2 (126 MB) write: evicts the previous iteration's working set
+            flush.add_(1.0)  # 256 MB write (H100 L2: 50 MB): evicts the previous iteration's working set
         s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         s.record()
         fn()
@@ -402,8 +408,8 @@ def kernel_rooflines(cfgd, peaks, dev):
     out["attention"] = dict(ms=ms, tflops=fl / ms / 1e9, gbs=(M * 4 * E * 2) / ms / 1e6, flops=fl, bytes=M * 4 * E * 2,
                             launches_per_step=12)
     # head-dim-64 attention needs one exponential per 256 tensor flops; MUFU.EX2 issues 16 / clk / SM, so the exponentials
-    # alone cap the kernel at 4096 flop/clk/SM, half the nominal tensor rate (profiles/r2_attention_v3.md).  Tile-padded count: 128-row query
-    # tiles x 64-key tiles, what the kernel actually evaluates.
+    # alone cap the kernel at 4096 flop/clk/SM.  Tile-padded count: 128-row query tiles x 64-key tiles, what the kernel
+    # actually evaluates.
     n_exp = float(B2 * heads) * (-(-N // 128) * 128) * (-(-N // 64) * 64)
     sm_count = torch.cuda.get_device_properties(dev).multi_processor_count
     out["attention"]["exp_per_launch"] = n_exp
@@ -452,7 +458,7 @@ def kernel_rooflines(cfgd, peaks, dev):
 # points per image; S = h w is its plotting script's use of the same einsum, src/plot_dino_correspondence.py:45,49)
 # ----------------------------------------------------------------------------------------------------
 def run_corr_sweep(args):
-    """`tensor_correlation` (einsum nchw,ncij->nhwij) as one batched tcgen05 GEMM launch, S x S x E per image, for S from
+    """`tensor_correlation` (einsum nchw,ncij->nhwij) as one batched wgmma GEMM launch, S x S x E per image, for S from
     the reference's 121 sampled points up to the full feature map of c1 / c2 / c3.  TFLOP/s are ALGORITHMIC (2 S^2 E per
     image) against the measured bf16 peak; `split3` is the fp32-input path (bf16 hi/lo split: 3x the tensor work for
     ~2^-16 relative error), `bf16` the single pass on bf16 features (what the frozen backbone emits)."""
@@ -572,7 +578,6 @@ def run_c4(args, rank, world, local):
         return ms.item()
 
     run(args.warmup, False)
-    model.check_update_health()  # N > 1: every rank made every peer-memory rendezvous of the warm-up
     sampler = ClockSampler(local)
     if rank == 0:
         sampler.start()
@@ -640,7 +645,7 @@ def run_c4(args, rank, world, local):
             "warmup": args.warmup, "ms_per_step": ms_dev / args.steps, "higher_is_better": True, "scaling": "weak",
             "vs_baseline": None, "dtype": "f32", "data": "synthetic",
             "config": {"workload": workload, "global_batch": B * world, "parallelism": f"dp{world}",
-                       "l2": "each step writes 1.8 GB of outputs (> 126 MB L2); no explicit flush"},
+                       "l2": "each step writes 1.8 GB of outputs (H100 L2: 50 MB); no explicit flush"},
             "e2e": {"value": frames / (ms_e2e / 1e3), "unit": "frames/s", "h2d_bytes_per_step": B * h * w * C * 4,
                     "d2h_bytes_per_step": 2 * B * H * W, "ms_per_step": ms_e2e / args.steps},
             "gpu_launches": int(launches), "clocks": clocks,
@@ -666,6 +671,28 @@ def run_c4(args, rank, world, local):
         dist.destroy_process_group()
 
 
+def dump_step_outputs(out_dir, model, loss):
+    """What one training step hands its caller: the returned loss, the logged loss terms and the trainable parameters
+    and their gradients after the step (the update is flushed first)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    model.flush()
+    arrays = {"loss": loss.detach().reshape(1)}
+    arrays.update({"logged." + k.replace("/", "."): (v if torch.is_tensor(v) else torch.tensor(float(v))).reshape(1)
+                   for k, v in model.logged.items()})
+    for name, p in model.named_parameters():
+        if p.requires_grad:
+            arrays["param." + name] = p.detach()
+            if p.grad is not None:
+                arrays["grad." + name] = p.grad.detach()
+    total = 0
+    for name, t in arrays.items():
+        a = t.float().cpu().numpy()
+        total += a.nbytes
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+    assert total <= 64 << 20, total
+
+
 # ----------------------------------------------------------------------------------------------------
 def main():
     ap = argparse.ArgumentParser()
@@ -676,7 +703,9 @@ def main():
     ap.add_argument("--exchange", default="p2p", choices=["p2p", "nccl"],
                     help="N > 1: fused peer-memory all-reduce + Adam (default) or NCCL all-reduce + Adam launches")
     ap.add_argument("--impl", default="ours", choices=["ours", "reference", "torch-eager"])
-    ap.add_argument("--sustain-seconds", type=float, default=5.0, help="length of the extra sustained-clock run (0 = skip)")
+    ap.add_argument("--sustain-seconds", type=float, default=0.0, help="length of an extra sustained-clock run (0 = skip)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write what the last timed step computed as DIR/<name>.npy")
     ap.add_argument("--batch", type=int, default=None, help="override the per-GPU batch")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-kernel-rooflines", action="store_true")
@@ -703,7 +732,7 @@ def main():
 
     if args.impl == "reference":
         # the reference's own CPU implementation of the path, rank 0 only, bounded sample per step: the REAL reference
-        # (baseline/_ref through the stub-Lightning harness) when that copy travelled with the repo, else the oracle port
+        # (through the stub-Lightning harness) when a reference checkout is named, else the oracle port
         if rank != 0:
             return
         os.environ["CUDA_VISIBLE_DEVICES"] = ""  # a CPU arm: the reference's unconditional .cuda() must not find a GPU
@@ -714,7 +743,7 @@ def main():
             kind, sample_b = "port", 2
             r = time_cpu(model_type, res, sample_b, max(1, args.steps), max(1, min(args.warmup, 2)))
         v, dt, cores, nst = r
-        what = ("the reference's own LitUnsupervisedSegmenter.training_step (baseline/_ref, unmodified, stub Lightning base)"
+        what = ("the reference's own LitUnsupervisedSegmenter.training_step (unmodified, stub Lightning base)"
                 if kind == "reference" else "the oracle port")
         print(json.dumps({
             "impl": "reference", "metric": "train-step images/sec", "value": v, "unit": "images/s", "n_gpus": args.gpus,
@@ -778,6 +807,8 @@ def main():
 
     host_ms = [0.0]
 
+    last = {}
+
     def run(nsteps, e2e, hb=None):
         barrier()
         s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -812,7 +843,7 @@ def main():
         else:
             t_host = time.perf_counter()
             for i in range(nsteps):
-                model.training_step(batch, i)
+                last["loss"] = model.training_step(batch, i)
             host_ms[0] = (time.perf_counter() - t_host) * 1e3 / max(nsteps, 1)  # CPU time to ENQUEUE one step
         model.flush()  # the last step's parameter update (side stream) belongs to the timed region too
         e.record()
@@ -829,6 +860,8 @@ def main():
         sampler.start()
     l0 = _lib.launch_count()
     ms_dev = run(args.steps, False)
+    if args.dump_outputs and rank == 0:
+        dump_step_outputs(args.dump_outputs, model, last["loss"])
     host_enqueue_ms = host_ms[0]
     launches = _lib.launch_count() - l0
     clocks = sampler.stop() if rank == 0 else None
@@ -880,7 +913,7 @@ def main():
                                 "all-reduce fused into Adam over NVLink peer memory (csrc/p2p_update.cu), on the side stream under "
                                 "the next step's backbone" if getattr(model, "_peer", None) is not None else
                                 "NCCL all-reduce + 3 Adam launches on the side stream"),
-                   "l2": "per-step working set (>5 GB of activations) exceeds the 126 MB L2; no explicit flush between steps"},
+                   "l2": "per-step working set (>5 GB of activations) exceeds the 50 MB L2; no explicit flush between steps"},
         "e2e": {"value": e2e_value, "unit": "images/s", "h2d_bytes_per_step": h2d_of(host_compact), "d2h_bytes_per_step": 4,
                 "ms_per_step": ms_e2e / args.steps,
                 "inputs": "LitUnsupervisedSegmenter.training_step with pinned-host bf16 images + uint8 labels (255 = "
@@ -904,18 +937,8 @@ def main():
         dom = max((k for k in ks if "tflops" in ks[k] and k != "corr_loss_fwd" and not k.startswith("diag_")),
                   key=lambda k: ks[k]["share_of_step"])
         d = ks[dom]
-        traffic = None
-        traffic_src = None
-        tpath = os.path.join(ROOT, "profiles", "ncu_traffic_r2.json")
-        if os.path.exists(tpath):
-            # dram__bytes_read.sum + dram__bytes_write.sum per launch from the committed `ncu --set full` capture of
-            # THIS build's kernels at these shapes (a profiler cannot run inside the timed region); see `traffic_source`
-            tj = json.load(open(tpath))
-            if tj.get("config") == args.config and not args.batch:
-                traffic = tj["bytes_per_launch"].get(dom)
-                traffic_src = tj.get("source")
         line["roofline"] = {"kernel": dom, "bound": "tensor", "achieved": d["tflops"], "peak": peaks["tf_burst"],
-                            "unit": "TFLOP/s", "frac": d["tflops"] / peaks["tf_burst"], "traffic": traffic, "traffic_source": traffic_src,
+                            "unit": "TFLOP/s", "frac": d["tflops"] / peaks["tf_burst"], "traffic": None,
                             "algorithmic_bytes_per_launch": d["bytes"],
                             "algorithmic_flops_per_launch": d["flops"], "ms_per_launch": d["ms"],
                             "share_of_step": d["share_of_step"], "peak_source": peaks["source"] + ", burst"}
@@ -925,7 +948,7 @@ def main():
             line["roofline"]["mufu"] = {"exp_per_launch": d["exp_per_launch"], "achieved_gexp_s": d["exp_rate_gexp_s"],
                                         "peak_gexp_s": mufu_peak, "frac": d["exp_rate_gexp_s"] / mufu_peak,
                                         "note": "head_dim 64: 256 tensor flop per exponential, so the MUFU pipe caps this kernel at "
-                                                "4096 flop/clk/SM (1.19 PFLOP/s at 1965 MHz, half the nominal tensor rate); frac here = share of that second ceiling"}
+                                                "4096 flop/clk/SM; frac here = share of that second ceiling"}
         c = ks["corr_loss_fwd"]
         line["corr_roofline"] = {"kernel": "corr_loss_fwd (fd+cd einsums + loss reduction, 7 calls x B images)",
                                  "ms_per_launch": c["ms"], "achieved_tflops": c["tflops"],
@@ -935,8 +958,8 @@ def main():
         line["kernels"] = {k: {kk: (round(vv, 4) if isinstance(vv, float) else vv) for kk, vv in v.items()
                                if kk in ("ms", "tflops", "gbs", "share_of_step")} for k, v in ks.items()}
     if not args.no_cpu_baseline and world == 1:  # the CPU arm is reported at N = 1 only
-        # the reference's own training_step on the host cores when its copy travelled with the repo (baseline/_ref, made by
-        # __graft_entry__.build()); the oracle port otherwise
+        # the reference's own training_step on the host cores when a reference checkout is named ($STEGO_REFERENCE_SRC);
+        # the oracle port otherwise
         sample_b = {"c1": 4, "c2": 2, "c3": 1}.get(args.config, 2)
         try:
             r = time_reference_cpu(model_type, res, sample_b, 2, 0, budget_s=30.0)
@@ -947,7 +970,7 @@ def main():
             v, dt, cores, nst = r
             line["cpu_baseline"] = {"value": v, "unit": "images/s", "cores": cores, "kind": "reference",
                                     "sample": f"{nst} steps of batch {sample_b} of the {args.config} workload: the reference's "
-                                              f"LitUnsupervisedSegmenter.training_step (baseline/_ref, unmodified; Lightning / "
+                                              f"LitUnsupervisedSegmenter.training_step ($STEGO_REFERENCE_SRC, unmodified; Lightning / "
                                               f"Hydra stubbed) on {cores} host threads"}
         else:
             v, dt, cores, nst = time_cpu(model_type, res, 2, 3, 1, budget_s=30.0)

@@ -1,10 +1,10 @@
 /*
- * stego_b200 — C-ABI of the B200-native STEGO correspondence-distillation hot path.
+ * stego_b200 — C-ABI of the H100-native STEGO correspondence-distillation hot path.
  *
  * This header is the drop-in boundary.  The reference (mhamilton723/STEGO) has no FFI layer: its
  * hot path is Python over torch ops in src/modules.py / src/dino/vision_transformer.py /
  * src/train_segmentation.py.  Each entry point below replaces the torch-op sequence cited next to
- * it (reference file:line) with hand-written sm_100a kernels; stego_b200/modules.py binds them with
+ * it (reference file:line) with hand-written sm_90a kernels; stego_b200/modules.py binds them with
  * ctypes behind the reference's own class / function names (see INTEGRATION.md).
  *
  * Conventions
@@ -34,7 +34,7 @@ STEGO_API const char* stego_last_error(void);
 STEGO_API long long stego_launch_count(void);
 
 /* ------------------------------------------------------------------------------------------------
- * Dense contraction (tcgen05 + TMA + TMEM):
+ * Dense contraction (wgmma + TMA + mbarrier):
  *     out[M,N] = act(A . B^T + bias[N]) + residual
  * replaces nn.Linear / 1x1 Conv2d calls of the path:
  *   src/dino/vision_transformer.py:80,88 (qkv, proj), :58-62 (fc1+GELU, fc2), :127-131 (patch embed),
@@ -85,7 +85,7 @@ STEGO_API int stego_layernorm_bf16(const float* x, const float* gamma, const flo
 STEGO_API int stego_layernorm_gap(const float* x, const float* gamma, const float* beta, float* out, int B, int ntok,
                                   int E, float eps, void* stream);
 /* Attention.forward (:78-90) without the projections: softmax(q k^T / sqrt(64)) v, fused (flash-style) on
- * tcgen05; qkv [B][N][3E] bf16 packed q|k|v with heads contiguous inside each third, out [B][N][E] bf16. */
+ * wgmma; qkv [B][N][3E] bf16 packed q|k|v with heads contiguous inside each third, out [B][N][E] bf16. */
 STEGO_API int stego_attention_fwd(const void* qkv, void* out, int B, int N, int E, int heads, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
@@ -107,7 +107,7 @@ STEGO_API int stego_sample_norm_fwd(const void* src, const void* src_pos, int sr
                                     const float* coords2, const long long* perms, void* tiles, int B, int C,
                                     int Cpad, int H, int W, int feature_samples, int nslots, int perms_are_raw_randperm,
                                     void* stream);
-/* helper (:325-347) for all calls at once: fd and cd einsums on tcgen05 (bf16 hi/lo split, fp32 accumulate),
+/* helper (:325-347) for all calls at once: fd and cd einsums on wgmma (bf16 hi/lo split, fp32 accumulate),
  * pointwise centring, clamp, shift, product and reduction.  slot_of_call / shifts are HOST arrays.
  * partials: scratch [ncalls][B][8]; stats: out [ncalls][4] = {mean loss, mean cd, old_mean, mean of centred fd}.
  * Optional (may be null): cd_out / fdc_out / loss_out [ncalls][B][S][S] (loss_out needs the other two). */
@@ -124,7 +124,8 @@ STEGO_API int stego_corr_loss_bwd(const void* feat_tiles, const void* code_tiles
                                   const float* shifts_host, int pointwise, int zero_clamp, int stabilize,
                                   const float* stats, const float* gscale, const float* gelem, const float* gcd,
                                   float* dtiles, void* stream);
-/* Backward of norm + sample for the code tensors: scatter-adds into dcode / dcode_pos (same strides as code). */
+/* Backward of norm + sample for the code tensors: adds into dcode / dcode_pos (same strides as code); every element is
+ * written once, in a fixed order (no atomics). */
 STEGO_API int stego_sample_norm_bwd(const float* code, const float* code_pos, long long stride_b, long long stride_c,
                                     long long stride_y, long long stride_x, const float* coords1,
                                     const float* coords2, const long long* perms, const float* dtiles, float* dcode,
@@ -212,7 +213,7 @@ STEGO_API int stego_eval_probes(const float* code, const float* code_flip, long 
 /* ------------------------------------------------------------------------------------------------
  * k-nearest-neighbour descriptors (SURVEY.md 8(f) rank 1; src/precompute_knns.py:15-21, 83-96):
  *   normed = F.normalize(feats, dim=1);  sims = einsum("nf,mf->nm", normed, normed);  idx = topk(sims, k)[1]
- * fused: the [n][n] similarity matrix is never materialised (tcgen05 tiles in TMEM, bf16 hi/lo split = 3 passes,
+ * fused: the [n][n] similarity matrix is never materialised (wgmma tiles in registers, bf16 hi/lo split = 3 passes,
  * per-row running top-k in the epilogue).  feats: fp32 [n][E] (un-normalised, e.g. GAP-pooled ViT features),
  * E a multiple of 64, 1 <= k <= 32.  planes_scratch: 2*n*E bf16 (16-byte aligned).  idx_out: int64 [n][k], sorted by
  * descending similarity (ties: lower index first; a row is its own nearest neighbour, as in the reference);

@@ -1,6 +1,6 @@
 """CPU oracle for the dense-CRF stage of the eval path (reference: src/crf.py:22-45 -> pydensecrf).  TEST INFRASTRUCTURE ONLY.
 
-Parity status: **UNPINNED**.  The arithmetic lives in a third-party dependency that is neither vendored in /root/reference nor
+Parity status: **UNPINNED**.  The arithmetic lives in a third-party dependency that is neither vendored in the reference nor
 installed here: `pydensecrf` (listed unpinned in environment.yml:34; the demo notebook installs
 `git+https://github.com/lucasb-eyer/pydensecrf.git`, i.e. master, which wraps Philipp Kraehenbuehl's densecrf C++:
 densecrf.cpp, pairwise.cpp, permutohedral.cpp).  This file restates that PUBLISHED algorithm in numpy —

@@ -3,14 +3,13 @@ Lightning / Hydra / torchmetrics / matplotlib installed.  TEST INFRASTRUCTURE ON
 
 What it is for
   * the drop-in check SURVEY.md §7.3(9) asks for: the reference `training_step` text executed over
-    `stego_b200.modules` (`from modules import *` resolves to the B200 package) — `modules_impl="stego_b200"`;
+    `stego_b200.modules` (`from modules import *` resolves to the stego_b200 package) — `modules_impl="stego_b200"`;
   * the "reference PyTorch path" comparator: the same class over the reference's own `modules.py`
-    (`modules_impl="reference"`) on the B200 (PyTorch eager, fp32 or bf16 autocast) and on the host CPU.
+    (`modules_impl="reference"`) in PyTorch eager, on the GPU (fp32 or bf16 autocast) or on the host CPU;
+  * the reference side of the golden fixtures (oracle/make_golden.py).
 
 Nothing here is product code and nothing under stego_b200/ imports it.  The reference sources are never copied
-into the repository: they are read at run time from `baseline/_ref/src` (a git-ignored verbatim copy made by
-`__graft_entry__.build()` in the build container; it travels to the GPU box with the snapshot) or, in the build
-container only, from /root/reference/src.
+into the repository: they are read at run time from the checkout $STEGO_REFERENCE_SRC names (its `src` directory).
 
 The stubs replace exactly the third-party names `train_segmentation.py` imports (`:1-16`):
   utils.*            -> nn, F, torch, np, os, join, plt + no-op UnsupervisedMetrics / colormaps / resize / one_hot_feats
@@ -35,14 +34,11 @@ import torch.nn.functional as F
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(_HERE)
-_CANDIDATES = [os.path.join(ROOT, "baseline", "_ref", "src"), "/root/reference/src"]
 
 
 def reference_src() -> Optional[str]:
-    for c in _CANDIDATES:
-        if os.path.isfile(os.path.join(c, "train_segmentation.py")):
-            return c
-    return None
+    c = os.environ.get("STEGO_REFERENCE_SRC", "")
+    return c if c and os.path.isfile(os.path.join(c, "train_segmentation.py")) else None
 
 
 def available() -> bool:
@@ -156,7 +152,7 @@ def _stub_misc():
 
 
 def _stego_modules_shim():
-    """`modules` as the B200 package: what `from modules import *` sees when stego_b200 replaces src/modules.py."""
+    """`modules` as the stego_b200 package: what `from modules import *` sees when stego_b200 replaces src/modules.py."""
     if ROOT not in sys.path:
         sys.path.insert(0, ROOT)
     import stego_b200.modules as ours
@@ -181,8 +177,7 @@ def load_reference_segmenter(modules_impl: str = "reference"):
     The module objects are private to this call (sys.modules is restored), so both flavours can coexist."""
     src = reference_src()
     if src is None:
-        raise RuntimeError("reference sources not found (baseline/_ref/src is made by __graft_entry__.build() in the "
-                           "build container)")
+        raise RuntimeError("reference sources not found: set STEGO_REFERENCE_SRC to the reference's src directory")
     saved = {k: sys.modules.get(k) for k in _OWNED}
     saved_path = list(sys.path)
     try:

@@ -6,7 +6,7 @@ eb4d6b5).  It exists so that tests/, __graft_entry__.smoke() and bench.py's cpu_
 imports it, and it must never be used as (or behind) the product path.
 
 Parity status: PINNED.  The reference has no tests or golden vectors of its own (SURVEY.md §4.1),
-but it is importable in the build container, so this restatement is checked function-by-function
+but it is importable without a GPU, so this restatement is checked function-by-function
 against the real reference code by oracle/check_against_reference.py, and the golden fixtures under
 tests/golden/ were produced by the reference itself (oracle/make_golden.py).
 

@@ -1,4 +1,4 @@
-"""Correctness + timing of the fused attention kernel at the bench shapes (run on the GPU box).
+"""Correctness + timing of the fused attention kernel at the bench shapes (needs an H100).
     python profiles/attn_bench.py [--check-only]
 Prints rel-L2 error vs fp32 torch for edge shapes and µs / TFLOP/s (algorithmic flops 4*N^2*64 per head-image) for
 c1 (64 x 6 x 785), c2 (64 x 12 x 1601), c3 (32 x 12 x 3137); L2 flushed between launches."""

@@ -1,7 +1,7 @@
-"""Build libstego_b200.so (sm_100a) in-tree with nvcc.
+"""Build libstego_b200.so (sm_90a) in-tree with nvcc.
 
 The shared library is the drop-in boundary (C-ABI, see include/stego_b200.h). It is built in-tree so
-the artefact travels with the repo snapshot to the GPU box; it is git-ignored.
+the package imports straight from the source tree; the library is git-ignored.
 """
 from __future__ import annotations
 
@@ -17,9 +17,9 @@ OBJ = os.path.join(CSRC, "_obj")
 LIB = os.path.join(HERE, "libstego_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-I", os.path.join(HERE, "..", "include"),
-] + os.environ.get("STEGO_NVCC_DEFS", "").split()  # e.g. -DSTEGO_ATT_TRACE for profiles/attn_trace.py (diagnostic build)
+] + os.environ.get("STEGO_NVCC_DEFS", "").split()  # extra -D flags for diagnostic builds
 
 
 def _sources():

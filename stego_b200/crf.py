@@ -2,7 +2,7 @@
 hands every frame to pydensecrf on a pool of CPU processes (src/eval_segmentation.py:52-54,118,133-135).
 
 Same parameters (src/crf.py:13-19) and the same preparation of image and unaries (src/crf.py:23-33); the mean-field
-inference with permutohedral-lattice filtering runs as the sm_100a kernels of csrc/crf.cu.  pydensecrf itself is a
+inference with permutohedral-lattice filtering runs as the sm_90a kernels of csrc/crf.cu.  pydensecrf itself is a
 third-party dependency that is not part of the reference tree, so parity of this stage is UNPINNED: the kernels follow
 the published densecrf algorithm and are tested against its CPU restatement oracle/crf_oracle.py (DESIGN.md).
 No CPU fallback: CUDA tensors only.

@@ -1,29 +1,22 @@
-// Fused multi-head self-attention forward for the frozen DINO ViT (sm_100a, tcgen05 + TMA + TMEM).
+// Fused multi-head self-attention forward for the frozen DINO ViT (sm_90a, wgmma + TMA + mbarrier).
 //
 // Reference: src/dino/vision_transformer.py:78-90 (Attention.forward):
 //     attn = softmax(q k^T * head_dim^-0.5);  x = attn v
 // The reference materialises the [B, heads, N, N] fp32 score tensor three times per layer; here it
-// never leaves the SM: S = Q K^T accumulates in TMEM, softmax runs out of TMEM in registers,
-// P (bf16) goes through swizzled shared memory straight back into the tensor core for P V.
+// never leaves the SM: S = Q K^T accumulates in registers (wgmma, both operands in shared memory), the online
+// softmax runs on those registers, and P (bf16) feeds the P V wgmma straight from registers (no shared-memory round
+// trip: the accumulator fragment of S is the A-operand fragment of P V).
 //
-// One CTA per (128-query tile, head, image), head_dim = 64, 320 threads:
-//   warp 0      TMA producer: Q tile and the first K/V stages before the CTA-wide sync, then a 4-stage ring of
-//               64-key (K,V) tiles
-//   warp 1      MMA issuer (whole warp in uniform control flow, one elected lane): S_j = Q K_j^T (128x64x64) two
-//               tiles ahead of O += P_j V_j (128x64x64)
-//   warps 2..5  softmax warpgroup 0  (KV tiles 0,2,4,..)   } each thread owns one query row, keeps its own
-//   warps 6..9  softmax warpgroup 1  (KV tiles 1,3,5,..)   } reference max / running sum
-// O accumulates IN TMEM across a warpgroup's KV tiles (tcgen05.mma accumulate), so the softmax warps never wait
-// for P V inside the loop.  The running max is updated lazily (FA4-style): the reference max only moves when the
-// new row max exceeds it by more than 2^8, and only then is O rescaled in TMEM (tcgen05.ld -> scale ->
-// tcgen05.st); otherwise P = exp2(s - m_ref) is at most 256, harmless in bf16 / fp32.
-// The two warpgroups work on alternate KV tiles (S, P, O are double buffered) and are merged once at the
-// end (split-KV combine, both accumulators read straight from TMEM), so there is no cross-warpgroup dependency inside
-// the loop; the [128 x 64] output tile is staged in the idle P tile and leaves as two TMA bulk stores.
-// Two CTAs per SM (112 KB of shared memory, 256 TMEM columns each).
+// One CTA per (128-query tile, head, image), head_dim = 64, 288 threads:
+//   warps 0..3  MMA/softmax warpgroup 0 (query rows 0..63 of the tile)
+//   warps 4..7  MMA/softmax warpgroup 1 (query rows 64..127)
+//   warp 8      TMA producer: the Q tile, then a 4-stage ring of 64-key (K, V) tiles shared by both warpgroups
+// Each warpgroup keeps its rows' running max / sum and O (64 x 64 fp32) in registers; the [64 x 64] output tile is
+// staged in the warpgroup's (then idle) half of the Q tile and leaves as one TMA bulk store.
+// Two CTAs per SM (80 KB of shared memory each).
 // Input is the packed qkv GEMM output [B, N, 3E] bf16 (q | k | v, head-major inside each), read through
 // ONE 3-D tensor map; rows past N (ragged last tile: N = hw + 1 is never a multiple of 128) are
-// zero-filled by TMA and masked to -inf in the softmax.
+// zero-filled by TMA, masked to -inf in the softmax and clipped from the output store.
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -35,106 +28,20 @@ constexpr int ATT_BQ = 128;
 constexpr int ATT_BKV = 64;   // 64-key tiles: 6 % padding waste at N = 785 (128-key tiles waste 14 %), half the smem
 constexpr int ATT_D = 64;
 constexpr int ATT_STAGES = 4;
-constexpr int ATT_THREADS = 320;
-constexpr uint32_t ATT_TMEM_COLS = 256;  // S: 2 x 64, O: 2 x 64 -> two CTAs fit the 512 columns of an SM
+constexpr int ATT_THREADS = 288;
 
 constexpr uint32_t ATT_Q_BYTES = 128 * 64 * 2;   // 16 KB [128 q][64 d]
 constexpr uint32_t ATT_KV_BYTES = 64 * 64 * 2;   // 8 KB  [64 kv][64 d]
-constexpr uint32_t ATT_P_BYTES = 128 * 64 * 2;   // 16 KB [128 q][64 kv]
 constexpr uint32_t ATT_SMEM_Q = 0;
 constexpr uint32_t ATT_SMEM_KV = ATT_Q_BYTES;                                   // stages x (K,V)
-constexpr uint32_t ATT_SMEM_P = ATT_SMEM_KV + ATT_STAGES * 2 * ATT_KV_BYTES;    // one P tile per warpgroup
-constexpr uint32_t ATT_SMEM_ML = ATT_SMEM_Q;  // m,l of WG1 (2 x 128 floats) reuse the Q tile once every S has been issued
-constexpr uint32_t ATT_SMEM_BAR = ATT_SMEM_P + 2 * ATT_P_BYTES;
-constexpr uint32_t ATT_SMEM_TOTAL = ATT_SMEM_BAR + 256;  // 112.25 KB: two CTAs per SM (<= 113 KB each)
-
-// Diagnostic build only (-DSTEGO_ATT_TRACE, see profiles/attn_trace.py): lane 0 of every warp of a few CTAs stamps
-// (globaltimer, event id) pairs into a global buffer so the pipeline of one CTA can be drawn as a timeline.  The
-// default build contains none of this.
-#ifdef STEGO_ATT_TRACE
-constexpr int ATT_TRACE_EVENTS = 256;   // per warp
-constexpr int ATT_TRACE_SLOTS = 8;      // traced CTAs
-static unsigned long long* g_att_trace = nullptr;
-static int g_att_trace_every = 0;
-#define ATT_TRACE(ev) att_trace_event(p, warp, lane, (ev), trace_seq)
-#else
-#define ATT_TRACE(ev) ((void)0)
-#endif
-
-// Phase-isolation switches (profiles/attn_phases.py) exist only in a -DSTEGO_DIAG build; the default build folds them to
-// constants (no getenv on the launch path, no diag branches in the kernel).
-#ifdef STEGO_DIAG
-#define ATT_DIAG(p, bit) (((p).diag & (bit)) != 0)
-#else
-#define ATT_DIAG(p, bit) false
-#endif
-
-// Round-2 scheduling experiments, kept as compile-time knobs, BOTH OFF in the shipped build because both measured slower
-// (profiles/r2_attention_v3.md; c1 / c2 / c3 in us: shipped 135.1 / 776 / 1330):
-//   ATT_LATE_OWAIT  1: the wait for the previous P V of this warpgroup (P buffer free, O stable) moves from BEFORE the
-//                   exponentials to AFTER them, the packed bf16 P row held in registers meanwhile, to hide the
-//                   tcgen05.mma + commit + mbarrier round trip under the MUFU work: 146.2 / 846 / 1443 (the burst of
-//                   eight 16-byte shared-memory stores behind the wait and the extra spills cost more than the wait).
-//   ATT_POLY        1..4: that many of every four packed pairs take exp2 on the FMA pipe (Cody-Waite split + minimax
-//                   cubic, 7.5e-5 relative error, 50x below the bf16 rounding of P) instead of MUFU.EX2:
-//                   146.5 / 852 / 1449 (1 of 4), 147.8 / 872 / 1508 (2 of 4) — the softmax warps are bound by their
-//                   dependent issue chain, not by the MUFU pipe, so extra FMA-pipe instructions only lengthen it.
-#ifndef ATT_LATE_OWAIT
-#define ATT_LATE_OWAIT 0
-#endif
-#ifndef ATT_POLY
-#define ATT_POLY 0
-#endif
-
-// exp2 of a packed pair on the FMA pipe.  a <= ~2^4 (lazy max), clamped at -125 (2^-125: harmless, no exponent wrap).
-// t = a + 1.5*2^23 holds round(a) in its low mantissa bits; f = a - round(a) in [-0.5, 0.5]; 2^f by a minimax cubic;
-// the integer part is added straight into the exponent field: bits(p) + (bits(t) << 23).
-__device__ __forceinline__ void ex2_poly_x2(uint64_t a2, float& e0, float& e1) {
-  float a0, a1;
-  unpack_f32x2(a2, a0, a1);
-  a0 = fmaxf(a0, -125.f);
-  a1 = fmaxf(a1, -125.f);
-  const uint64_t a = pack_f32x2(a0, a1);
-  const uint64_t t = add_f32x2(a, pack_f32x2(12582912.f, 12582912.f));
-  const uint64_t r = add_f32x2(t, pack_f32x2(-12582912.f, -12582912.f));
-  const uint64_t f = fma_f32x2(r, pack_f32x2(-1.f, -1.f), a);
-  uint64_t q = fma_f32x2(f, pack_f32x2(0.0551716685f, 0.0551716685f), pack_f32x2(0.242611125f, 0.242611125f));
-  q = fma_f32x2(q, f, pack_f32x2(0.693260968f, 0.693260968f));
-  q = fma_f32x2(q, f, pack_f32x2(0.999928057f, 0.999928057f));
-  float p0, p1, t0, t1;
-  unpack_f32x2(q, p0, p1);
-  unpack_f32x2(t, t0, t1);
-  e0 = __uint_as_float(__float_as_uint(p0) + (__float_as_uint(t0) << 23));
-  e1 = __uint_as_float(__float_as_uint(p1) + (__float_as_uint(t1) << 23));
-}
+constexpr uint32_t ATT_SMEM_BAR = ATT_SMEM_KV + ATT_STAGES * 2 * ATT_KV_BYTES;
+constexpr uint32_t ATT_SMEM_TOTAL = ATT_SMEM_BAR + 128;
 
 struct AttnParams {
-#ifdef STEGO_ATT_TRACE
-  unsigned long long* trace;  // [SLOTS][10 warps][EVENTS][2]
-  int trace_every;            // CTA with linear id i is traced into slot i / every if i % every == 0
-#endif
-  bf16* out;   // [B*N][E] bf16 (heads concatenated, like .transpose(1,2).reshape(B,N,C))
   int N;       // tokens per image
   int E;       // embed dim = heads * 64
   float scale_log2e;  // head_dim^-0.5 * log2(e)
-  int s_ahead;        // how many KV tiles S = QK^T is issued ahead of P V (1 or 2)
-  int diag;           // STEGO_ATT_DIAG phase-timing flags (results garbage): 1 skip softmax math, 2 skip MMAs, 4 skip TMA,
-                      // 8 no KV tiles at all (prologue + merge + store only), 16 skip the output stores
 };
-
-#ifdef STEGO_ATT_TRACE
-__device__ __forceinline__ void att_trace_event(const AttnParams& p, int warp, int lane, int ev, int& seq) {
-  if (lane != 0 || p.trace == nullptr || p.trace_every <= 0) return;
-  const int cta = (blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x;
-  if (cta % p.trace_every != 0) return;
-  const int slot = cta / p.trace_every;
-  if (slot >= ATT_TRACE_SLOTS || seq >= ATT_TRACE_EVENTS) return;
-  unsigned long long* e = p.trace + ((static_cast<size_t>(slot) * 10 + warp) * ATT_TRACE_EVENTS + seq) * 2;
-  e[0] = globaltimer_ns();
-  e[1] = static_cast<unsigned long long>(ev) | (static_cast<unsigned long long>(cta) << 32);
-  ++seq;
-}
-#endif
 
 __global__ void __launch_bounds__(ATT_THREADS, 2)
 attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant__ CUtensorMap tmOut, AttnParams p) {
@@ -146,369 +53,146 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_con
   uint64_t* q_full = bars;                        // [1]
   uint64_t* kv_full = bars + 1;                   // [STAGES]
   uint64_t* kv_empty = kv_full + ATT_STAGES;      // [STAGES]
-  uint64_t* s_full = kv_empty + ATT_STAGES;       // [2]
-  uint64_t* s_empty = s_full + 2;                 // [2]
-  uint64_t* p_full = s_empty + 2;                 // [2]
-  uint64_t* o_full = p_full + 2;                  // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(o_full + 2);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-#ifdef STEGO_ATT_TRACE
-  int trace_seq = 0;
-#endif
-  ATT_TRACE(1);  // CTA start
   const int q0 = blockIdx.x * ATT_BQ;
   const int head = blockIdx.y;
   const int img = blockIdx.z;
-  const int nkv = ATT_DIAG(p, 8) ? 0 : (p.N + ATT_BKV - 1) / ATT_BKV;
+  const int nkv = (p.N + ATT_BKV - 1) / ATT_BKV;
 
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmQKV);
-    tma_prefetch_desc(&tmOut);
+  if (threadIdx.x == 0) {
     mbar_init(q_full, 1);
     for (int s = 0; s < ATT_STAGES; ++s) {
       mbar_init(&kv_full[s], 1);
-      mbar_init(&kv_empty[s], 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(&s_full[b], 1);
-      mbar_init(&s_empty[b], 4);
-      mbar_init(&p_full[b], 4);
-      mbar_init(&o_full[b], 1);
+      mbar_init(&kv_empty[s], 2);  // one arrive per warpgroup
     }
     fence_barrier_init();
-    // Q and the first K/V stages are requested BEFORE the CTA-wide sync / TMEM allocation: their L2/HBM latency
-    // overlaps the rest of the prologue (the barriers they signal were initialised by this very thread)
-    if (!ATT_DIAG(p, 4)) {
-    mbar_arrive_expect_tx(q_full, ATT_Q_BYTES);
-    tma_load_3d(smem + ATT_SMEM_Q, &tmQKV, q_full, head * ATT_D, q0, img);
-    tma_load_3d(smem + ATT_SMEM_Q + ATT_Q_BYTES / 2, &tmQKV, q_full, head * ATT_D, q0 + 64, img);
-    for (int j = 0; j < ATT_STAGES && j < nkv; ++j) {
-      uint8_t* sk = smem + ATT_SMEM_KV + j * 2 * ATT_KV_BYTES;
-      mbar_arrive_expect_tx(&kv_full[j], 2 * ATT_KV_BYTES);
-      tma_load_3d(sk, &tmQKV, &kv_full[j], p.E + head * ATT_D, j * ATT_BKV, img);
-      tma_load_3d(sk + ATT_KV_BYTES, &tmQKV, &kv_full[j], 2 * p.E + head * ATT_D, j * ATT_BKV, img);
-    }
-    }
   }
-  if (warp == 1) tmem_alloc<ATT_TMEM_COLS>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  ATT_TRACE(2);  // prologue done (barriers, TMEM, CTA-wide sync)
-  const uint32_t TM_S = tmem_base;         // S[b] at + b*64
-  const uint32_t TM_O = tmem_base + 128;   // O[b] at + b*64
 
-  if (warp == 0) {
+  if (warp == 8) {
     // ===================== TMA producer =====================
-    if (lane == 0 && !ATT_DIAG(p, 4)) {
-      uint32_t stage = 0, phase = 1;  // tiles 0..STAGES-1 were requested in the prologue
-      for (int j = ATT_STAGES; j < nkv; ++j) {
+    if (lane == 0) {
+      tma_prefetch_desc(&tmQKV);
+      tma_prefetch_desc(&tmOut);
+      mbar_arrive_expect_tx(q_full, ATT_Q_BYTES);
+      tma_load_3d(smem + ATT_SMEM_Q, &tmQKV, q_full, head * ATT_D, q0, img);
+      tma_load_3d(smem + ATT_SMEM_Q + ATT_Q_BYTES / 2, &tmQKV, q_full, head * ATT_D, q0 + 64, img);
+      uint32_t stage = 0, phase = 0;
+      for (int j = 0; j < nkv; ++j) {
         mbar_wait(&kv_empty[stage], phase ^ 1u);
         uint8_t* sk = smem + ATT_SMEM_KV + stage * 2 * ATT_KV_BYTES;
-        uint8_t* sv = sk + ATT_KV_BYTES;
         mbar_arrive_expect_tx(&kv_full[stage], 2 * ATT_KV_BYTES);
         tma_load_3d(sk, &tmQKV, &kv_full[stage], p.E + head * ATT_D, j * ATT_BKV, img);
-        tma_load_3d(sv, &tmQKV, &kv_full[stage], 2 * p.E + head * ATT_D, j * ATT_BKV, img);
-        ATT_TRACE(140 + j);  // K/V tile j requested
+        tma_load_3d(sk + ATT_KV_BYTES, &tmQKV, &kv_full[stage], 2 * p.E + head * ATT_D, j * ATT_BKV, img);
         if (++stage == ATT_STAGES) { stage = 0; phase ^= 1u; }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    // The whole warp walks the schedule (warp-uniform control flow keeps the descriptors in uniform registers; from
-    // inside an `if (lane == 0)` region every tcgen05.mma was preceded by ~17 instructions of per-thread descriptor
-    // rebuilding behind an ELECT/R2UR loop) and one elected lane issues.
-    constexpr uint32_t IDESC_S = make_idesc_bf16(128, ATT_BKV, 0, 0);  // Q (K-major) x K (K-major)
-    constexpr uint32_t IDESC_O = make_idesc_bf16(128, 64, 0, 1);       // P (K-major) x V (MN-major: d contiguous)
-    constexpr uint32_t DESC_HI = smem_desc_hi_sw128(1024);
-    const uint32_t tm_s = __shfl_sync(0xffffffffu, TM_S, 0);
-    const uint32_t tm_o = __shfl_sync(0xffffffffu, TM_O, 0);
-    const uint32_t q_lo = smem_desc_lo(smem_u32(smem + ATT_SMEM_Q), 16);
-    const uint32_t k_lo0 = smem_desc_lo(smem_u32(smem + ATT_SMEM_KV), 16);
-    const uint32_t v_lo0 = smem_desc_lo(smem_u32(smem + ATT_SMEM_KV + ATT_KV_BYTES), 8192);
-    const uint32_t p_lo0 = smem_desc_lo(smem_u32(smem + ATT_SMEM_P), 16);
-    if (!ATT_DIAG(p, 4)) mbar_wait(q_full, 0);
-    tc_fence_after();
-    auto issue_pv = [&](int i) {
-      const uint32_t b = static_cast<uint32_t>(i & 1);
-      const uint32_t it = static_cast<uint32_t>(i >> 1);
-      const uint32_t stage_i = static_cast<uint32_t>(i % ATT_STAGES);
-      mbar_wait(&p_full[b], it & 1u);  // P written (and O rescaled, if needed) by warpgroup b
-      tc_fence_after();
-      const uint32_t p_lo = p_lo0 + b * (ATT_P_BYTES >> 4);
-      const uint32_t v_lo = v_lo0 + stage_i * ((2 * ATT_KV_BYTES) >> 4);
-      if (elect_one()) {
-#pragma unroll
-        for (uint32_t kk = 0; kk < (ATT_DIAG(p, 2) ? 0u : ATT_BKV / 16); ++kk)  // accumulate over this warpgroup's tiles
-          umma_bf16(tm_o + b * 64, smem_desc_join(p_lo + kk * 2, DESC_HI), smem_desc_join(v_lo + kk * (2048u >> 4), DESC_HI),
-                    IDESC_O, (it > 0 || kk > 0) ? 1u : 0u);
-        umma_commit(&o_full[b]);
-        umma_commit(&kv_empty[stage_i]);  // K_i and V_i are no longer needed
-      }
-      __syncwarp();
-      ATT_TRACE(40 + i);  // P_i V_i issued
-    };
-    // S runs two tiles ahead of P V: the S buffer of tile j+2 is free as soon as the softmax warpgroup holds the
-    // scores of tile j in registers (early s_empty), so S_{j+2} is issued BEFORE the blocking wait for P_j and is
-    // ready when that warpgroup comes back.  (Blocking try_wait on purpose: a polling loop on this warp steals
-    // issue slots from the softmax warps of its SM sub-partition.)
-    auto issue_s = [&](int j) {
-      const uint32_t b = static_cast<uint32_t>(j & 1);
-      const uint32_t it = static_cast<uint32_t>(j >> 1);
-      const uint32_t stage = static_cast<uint32_t>(j % ATT_STAGES);
-      const uint32_t phase = static_cast<uint32_t>((j / ATT_STAGES) & 1);
-      if (!ATT_DIAG(p, 4)) mbar_wait(&kv_full[stage], phase);
-      mbar_wait(&s_empty[b], (it & 1u) ^ 1u);
-      tc_fence_after();
-      const uint32_t k_lo = k_lo0 + stage * ((2 * ATT_KV_BYTES) >> 4);
-      if (elect_one()) {
-#pragma unroll
-        for (uint32_t k = 0; k < (ATT_DIAG(p, 2) ? 0u : ATT_D / 16); ++k)
-          umma_bf16(tm_s + b * ATT_BKV, smem_desc_join(q_lo + k * 2, DESC_HI), smem_desc_join(k_lo + k * 2, DESC_HI), IDESC_S,
-                    k > 0 ? 1u : 0u);
-        umma_commit(&s_full[b]);
-      }
-      __syncwarp();
-      ATT_TRACE(10 + j);  // S_j issued
-    };
-    const int ahead = p.s_ahead;
-    for (int j = 0; j < ahead && j < nkv; ++j) issue_s(j);
-    for (int j = 0; j < nkv; ++j) {
-      if (j + ahead < nkv) issue_s(j + ahead);
-      issue_pv(j);
-    }
-  } else {
-    // ===================== softmax warpgroups =====================
-    const int wg = (warp - 2) >> 2;  // 0 or 1
-    const int quarter = warp & 3;    // TMEM lane quarter accessible to this warp
-    const int r = quarter * 32 + lane;  // query row inside the tile
-    const uint32_t lane_off = static_cast<uint32_t>(quarter * 32) << 16;
-    uint8_t* sp = smem + ATT_SMEM_P + wg * ATT_P_BYTES;
-    const bool warp_has_rows = (q0 + quarter * 32) < p.N;
-    float m_run = -INFINITY, l_run = 0.f;  // m_run: reference max the exponentials are taken against
-    const float c = p.scale_log2e;
-    const uint32_t to = TM_O + wg * 64 + lane_off;
-
-    uint32_t it = 0;
-    for (int j = wg; j < nkv; j += 2, ++it) {
-      const int valid = p.N - j * ATT_BKV;  // number of real keys in this tile (>= 1)
-      mbar_wait(&s_full[wg], it & 1u);
-      tc_fence_after();
-      ATT_TRACE(70 + j);  // S_j visible to this warp
-      if (!warp_has_rows || ATT_DIAG(p, 1)) {
-        // ragged last query tile (N = hw + 1): this warp's 32 rows are all padding — keep the barrier protocol,
-        // skip the loads / exponentials / stores (their P rows and O rows are never read back)
-        if (lane == 0) mbar_arrive(&s_empty[wg]);
-        if (it > 0) mbar_wait(&o_full[wg], (it - 1u) & 1u);
-        if (lane == 0) mbar_arrive(&p_full[wg]);
-        continue;
-      }
-      const uint32_t ts = TM_S + wg * ATT_BKV + lane_off;
-      // the whole 64-key score row comes out of TMEM once and stays in registers for max, exp and packing
-      uint32_t v[2][32];
-      tmem_ld32(ts, v[0]);
-      tmem_ld32(ts + 32, v[1]);
-      tmem_ld_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&s_empty[wg]);  // S buffer is free for the MMA warp as soon as it is in registers
-      float mx = -INFINITY;
-      if (valid >= ATT_BKV) {
-        float mxb = -INFINITY;  // two independent FMNMX3 chains (one per 32-column half): half the dependent latency
-#pragma unroll
-        for (int t = 0; t < 32; ++t) {
-          mx = fmaxf(mx, __uint_as_float(v[0][t]));
-          mxb = fmaxf(mxb, __uint_as_float(v[1][t]));
-        }
-        mx = fmaxf(mx, mxb);
-      } else {
-#pragma unroll
-        for (int h = 0; h < 2; ++h)
-#pragma unroll
-          for (int t = 0; t < 32; ++t)
-            if (h * 32 + t < valid) mx = fmaxf(mx, __uint_as_float(v[h][t]));
-      }
-      // lazy reference-max update: move it only on the first tile or when it is off by more than 2^8
-      const bool first = (it == 0);
-      const bool move = first || ((mx - m_run) * c > 8.0f);
-      float alpha = 1.0f;
-      if (move) {
-        alpha = first ? 0.0f : ex2_approx((m_run - mx) * c);
-        m_run = mx;
-        l_run *= alpha;
-      }
-      // P V of this warpgroup's previous tile must have retired before P is overwritten or O is touched
-      auto wait_prev_pv = [&]() {
-        if (!first) {
-          mbar_wait(&o_full[wg], (it - 1u) & 1u);
-          tc_fence_after();
-          if (__any_sync(0xffffffffu, move)) {
-#pragma unroll 1
-            for (int h = 0; h < ATT_D / 8; ++h) {  // rare path: 8 columns at a time keeps the register budget
-              uint32_t o[8];
-              tmem_ld8(to + h * 8, o);
-              tmem_ld_wait();
-#pragma unroll
-              for (int t = 0; t < 8; ++t) o[t] = __float_as_uint(__uint_as_float(o[t]) * alpha);
-              tmem_st8(to + h * 8, o);
-            }
-            tmem_st_wait();
-          }
-        }
-      };
-      if (!ATT_LATE_OWAIT || valid < ATT_BKV) wait_prev_pv();
-      const float mc = m_run * c;
-      // p = exp2(s*c - m*c), row sum, bf16 P tile into swizzled smem (8 keys = one 16-byte chunk at a time).
-      // Full tiles (all but the last) take the select-free path: a per-element mask costs an ISETP + FSEL each.
-      float rs = 0.f;
-      if (valid >= ATT_BKV) {
-        // packed fp32x2 FMA / ADD: the scale-and-shift and the row sum take half the issue slots of the scalar form
-        const uint64_t c2 = pack_f32x2(c, c), nmc2 = pack_f32x2(-mc, -mc);
-        uint64_t rs2a = 0ull, rs2b = 0ull;  // two independent (0.f, 0.f) accumulators
-        uint8_t* prow = sp + r * 128;
-        const uint32_t rx = (static_cast<uint32_t>(r) & 7u) << 4;
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-#pragma unroll
-          for (int g = 0; g < 4; ++g) {
-#pragma unroll
-            for (int t = 0; t < 4; ++t) {
-              const uint64_t s2 = pack_f32x2(__uint_as_float(v[h][8 * g + 2 * t]), __uint_as_float(v[h][8 * g + 2 * t + 1]));
-              const uint64_t a2 = fma_f32x2(s2, c2, nmc2);
-              float e0, e1;
-              if (t < ATT_POLY) {
-                ex2_poly_x2(a2, e0, e1);
-              } else {
-                float a0, a1;
-                unpack_f32x2(a2, a0, a1);
-                e0 = ex2_approx(a0);
-                e1 = ex2_approx(a1);
-              }
-              // the packed bf16 pair replaces the first of the two score registers it came from (no second array)
-              v[h][8 * g + 2 * t] = pack_bf16x2(e0, e1);
-              if (t & 1) rs2b = add_f32x2(rs2b, pack_f32x2(e0, e1));
-              else rs2a = add_f32x2(rs2a, pack_f32x2(e0, e1));
-            }
-            if (!ATT_LATE_OWAIT)
-              *reinterpret_cast<uint4*>(prow + ((static_cast<uint32_t>(h * 4 + g) << 4) ^ rx)) =
-                  make_uint4(v[h][8 * g], v[h][8 * g + 2], v[h][8 * g + 4], v[h][8 * g + 6]);
-          }
-        }
-        if (ATT_LATE_OWAIT) {
-          wait_prev_pv();
-#pragma unroll
-          for (int h = 0; h < 2; ++h)
-#pragma unroll
-            for (int g = 0; g < 4; ++g)
-              *reinterpret_cast<uint4*>(prow + ((static_cast<uint32_t>(h * 4 + g) << 4) ^ rx)) =
-                  make_uint4(v[h][8 * g], v[h][8 * g + 2], v[h][8 * g + 4], v[h][8 * g + 6]);
-        }
-        float s0, s1;
-        unpack_f32x2(add_f32x2(rs2a, rs2b), s0, s1);
-        rs = s0 + s1;
-      } else {
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-#pragma unroll
-          for (int g = 0; g < 4; ++g) {
-            float e[8];
-#pragma unroll
-            for (int t = 0; t < 8; ++t) {
-              const float x = ex2_approx(fmaf(__uint_as_float(v[h][8 * g + t]), c, -mc));
-              e[t] = (h * 32 + 8 * g + t < valid) ? x : 0.f;
-            }
-            uint4 w;
-            w.x = pack_bf16x2(e[0], e[1]);
-            w.y = pack_bf16x2(e[2], e[3]);
-            w.z = pack_bf16x2(e[4], e[5]);
-            w.w = pack_bf16x2(e[6], e[7]);
-            *reinterpret_cast<uint4*>(sp + sw128_offset(r, h * 4 + g)) = w;
-            rs += ((e[0] + e[1]) + (e[2] + e[3])) + ((e[4] + e[5]) + (e[6] + e[7]));
-          }
-        }
-      }
-      l_run += rs;
-      tc_fence_before();
-      fence_proxy_async_smem();  // generic-proxy smem writes -> visible to the tensor-core (async) proxy
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&p_full[wg]);
-      ATT_TRACE(100 + j);  // P_j stored, p_full signalled
-    }
-    ATT_TRACE(130);  // KV loop done
-    // ---- combine the two warpgroups (split-KV merge) and write the output ----
-    // Both O accumulators live in the SAME TMEM lanes (rows), 64 columns apart, so warpgroup 0 reads both
-    // straight out of TMEM; only m and l of warpgroup 1 travel through shared memory.
-    float* ml = reinterpret_cast<float*>(smem + ATT_SMEM_ML);  // [2][128]
-    if (wg == 1) {
-      // ml aliases the Q tile: every S = Q K^T must have retired first.  tcgen05.commit covers all earlier MMAs of
-      // the issuing thread, and every S is issued before this warpgroup's last P V, so its o_full is sufficient
-      // (with no tile of its own — a single KV tile — wait for S_0 instead).
-      if (it > 0) mbar_wait(&o_full[1], (it - 1u) & 1u);
-      else if (!ATT_DIAG(p, 8)) mbar_wait(&s_full[0], 0);
-      ml[r] = m_run;
-      ml[128 + r] = l_run;
-    }
-    asm volatile("bar.sync 1, 256;\n" ::: "memory");  // the 8 softmax warps only
-    if (wg == 0) {
-      const uint32_t it1 = static_cast<uint32_t>(nkv / 2);  // tiles warpgroup 1 processed (it = tiles of WG0 >= 1)
-      if (it > 0) mbar_wait(&o_full[0], (it - 1u) & 1u);
-      if (it1 > 0) mbar_wait(&o_full[1], (it1 - 1u) & 1u);
-      tc_fence_after();
-      const float m1 = ml[r], l1 = ml[128 + r];
-      const float m = fmaxf(m_run, m1);
-      const float a0 = ex2_approx((m_run - m) * c);
-      const float a1 = (it1 == 0 || m1 == -INFINITY) ? 0.f : ex2_approx((m1 - m) * c);
-      const float inv = 1.0f / (l_run * a0 + l1 * a1);
-      const float s0 = a0 * inv, s1 = a1 * inv;
-      // The [128 q][64 d] bf16 output tile is staged in this warpgroup's (now idle) P tile and leaves as two TMA bulk
-      // stores: one thread per row writing 8 x 16 B straight to global cost 1024 LSU wavefronts per CTA (14 of the
-      // kernel's ~150 us with nothing else running, profiles/r1_attn_phases_before.md); rows >= N are clipped by the map.
-      uint8_t* stage_row = sp + r * 128;
-      const uint32_t rx = (static_cast<uint32_t>(r) & 7u) << 4;
-#pragma unroll 1
-      for (int h = 0; h < 2; ++h) {
-        uint32_t v0[32], v1[32];
-        tmem_ld32(TM_O + lane_off + h * 32, v0);
-        tmem_ld32(TM_O + 64 + lane_off + h * 32, v1);  // never-written columns if it1 == 0: multiplied by s1 = 0
-        tmem_ld_wait();
-        {
-#pragma unroll
-          for (int g = 0; g < 4; ++g) {
-            float y[8];
-#pragma unroll
-            for (int t = 0; t < 8; ++t) {
-              const float b1 = (it1 > 0) ? __uint_as_float(v1[8 * g + t]) : 0.f;
-              y[t] = __uint_as_float(v0[8 * g + t]) * s0 + b1 * s1;
-            }
-            uint4 w;
-            w.x = pack_bf16x2(y[0], y[1]);
-            w.y = pack_bf16x2(y[2], y[3]);
-            w.z = pack_bf16x2(y[4], y[5]);
-            w.w = pack_bf16x2(y[6], y[7]);
-            *reinterpret_cast<uint4*>(stage_row + ((static_cast<uint32_t>(h * 4 + g) << 4) ^ rx)) = w;
-          }
-        }
-      }
-      fence_proxy_async_smem();
-      asm volatile("bar.sync 2, 128;\n" ::: "memory");  // warpgroup 0 only: the whole tile is staged
-      if (warp == 2 && lane == 0 && !ATT_DIAG(p, 16)) {
-        tma_store_3d(sp, &tmOut, head * ATT_D, q0, img);
-        tma_store_3d(sp + 64 * 128, &tmOut, head * ATT_D, q0 + 64, img);
-        tma_commit_group();
-        tma_wait_group_read<0>();  // the staging tile must outlive the bulk stores
-      }
-    }
+    return;
   }
 
-  ATT_TRACE(131);  // role finished (merge + store done for warpgroup 0)
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<ATT_TMEM_COLS>(tmem_base);
+  // ===================== MMA / softmax warpgroups =====================
+  const int wg = warp >> 2;
+  const int wq = warp & 3;
+  const bool leader = (threadIdx.x & 127) == 0;
+  const float c = p.scale_log2e;
+  constexpr uint32_t DESC_HI = smem_desc_hi_sw128(1024);
+  uint8_t* sq = smem + ATT_SMEM_Q + wg * (ATT_Q_BYTES / 2);  // this warpgroup's 64 query rows
+  const uint32_t q_lo = smem_desc_lo(smem_u32(sq), 16);
+  const uint32_t k_lo0 = smem_desc_lo(smem_u32(smem + ATT_SMEM_KV), 16);
+  const uint32_t v_lo0 = smem_desc_lo(smem_u32(smem + ATT_SMEM_KV + ATT_KV_BYTES), 8192);
+  // accumulator fragment: rows wq*16 + lane/4 (+8 for h = 1), columns 8 i + 2 (lane % 4) + {0, 1}
+  float o[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) o[i] = 0.f;
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};  // l_run: this thread's partial row sums
+  mbar_wait(q_full, 0);
+  uint32_t stage = 0, phase = 0;
+  for (int j = 0; j < nkv; ++j) {
+    mbar_wait(&kv_full[stage], phase);
+    const uint32_t k_lo = k_lo0 + stage * ((2 * ATT_KV_BYTES) >> 4);
+    const uint32_t v_lo = v_lo0 + stage * ((2 * ATT_KV_BYTES) >> 4);
+    float s[32];
+    wgmma_fence();
+#pragma unroll
+    for (uint32_t k = 0; k < ATT_D / 16; ++k)
+      wgmma_ss<64, 0, 0>(s, smem_desc_join(q_lo + k * 2, DESC_HI), smem_desc_join(k_lo + k * 2, DESC_HI), k > 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_operands(s);
+    const int valid = p.N - j * ATT_BKV;  // number of real keys in this tile (>= 1)
+    if (valid < ATT_BKV) {
+#pragma unroll
+      for (int i = 0; i < 32; ++i)
+        if (8 * (i >> 2) + 2 * (lane & 3) + (i & 1) >= valid) s[i] = -INFINITY;
+    }
+    float alpha[2], mc[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float mx = -INFINITY;
+#pragma unroll
+      for (int i = 0; i < 8; ++i) mx = fmaxf(mx, fmaxf(s[4 * i + 2 * h], s[4 * i + 2 * h + 1]));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      const float m_new = fmaxf(m_run[h], mx);
+      alpha[h] = ex2_approx((m_run[h] - m_new) * c);  // 0 on the first tile (m_run = -inf)
+      m_run[h] = m_new;
+      mc[h] = m_new * c;
+    }
+    // P = exp2(s c - m c) packed to bf16 in the A-operand fragment of the P V wgmma: k16 slice kk of P is
+    // accumulator columns 16 kk .. 16 kk + 15, i.e. n8 groups 2 kk (regs 0, 1) and 2 kk + 1 (regs 2, 3)
+    uint32_t a[4][4];
+    float rs[2] = {0.f, 0.f};
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const float e0 = ex2_approx(fmaf(s[4 * i + 2 * h], c, -mc[h]));
+        const float e1 = ex2_approx(fmaf(s[4 * i + 2 * h + 1], c, -mc[h]));
+        rs[h] += e0 + e1;
+        a[i >> 1][(i & 1) * 2 + h] = pack_bf16x2(e0, e1);
+      }
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) l_run[h] = l_run[h] * alpha[h] + rs[h];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) o[i] *= alpha[(i >> 1) & 1];
+    wgmma_fence();
+#pragma unroll
+    for (uint32_t kk = 0; kk < ATT_BKV / 16; ++kk)
+      wgmma_rs_n64<1>(o, a[kk], smem_desc_join(v_lo + kk * (2048u >> 4), DESC_HI), 1u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_operands(o);
+    if (leader) mbar_arrive(&kv_empty[stage]);  // K_j and V_j are no longer needed by this warpgroup
+    if (++stage == ATT_STAGES) { stage = 0; phase ^= 1u; }
+  }
+  // normalise and stage the [64 q][64 d] bf16 tile in this warpgroup's half of the Q tile (its last reader, the final
+  // S wgmma, has retired), 128B-swizzled like the output tensor map; rows >= N are clipped by the map
+  float inv[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float l = l_run[h];
+    l += __shfl_xor_sync(0xffffffffu, l, 1);
+    l += __shfl_xor_sync(0xffffffffu, l, 2);
+    inv[h] = __fdividef(1.0f, l);
+  }
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const uint32_t r = static_cast<uint32_t>(wq * 16 + (lane >> 2) + 8 * h);
+      const uint32_t off = sw128_offset(r, static_cast<uint32_t>(i)) + 4u * static_cast<uint32_t>(lane & 3);
+      *reinterpret_cast<uint32_t*>(sq + off) = pack_bf16x2(o[4 * i + 2 * h] * inv[h], o[4 * i + 2 * h + 1] * inv[h]);
+    }
+  }
+  fence_proxy_async_smem();
+  asm volatile("bar.sync %0, 128;\n" ::"r"(wg + 1) : "memory");  // this warpgroup's tile is staged
+  if (leader) {
+    tma_store_3d(sq, &tmOut, head * ATT_D, q0 + wg * 64, img);
+    tma_commit_group();
+    tma_wait_group_read<0>();  // the staging tile must outlive the bulk store
   }
 }
 
@@ -541,33 +225,11 @@ extern "C" int stego_attention_fwd(const void* qkv, void* out, int B, int N, int
     configured = true;
   }
   AttnParams p;
-  p.out = reinterpret_cast<bf16*>(out);
   p.N = N;
   p.E = E;
   p.scale_log2e = 0.125f * 1.4426950408889634f;
-  p.s_ahead = 2;
-  p.diag = 0;
-#ifdef STEGO_ATT_TRACE
-  p.trace = g_att_trace;
-  p.trace_every = g_att_trace_every;
-#endif
-#ifdef STEGO_DIAG
-  {
-    const char* dg = getenv("STEGO_ATT_DIAG");  // read every call (profiles/attn_phases.py toggles it)
-    p.diag = dg ? atoi(dg) : 0;
-  }
-#endif
   dim3 grid((N + ATT_BQ - 1) / ATT_BQ, heads, B);
   attention_fwd_kernel<<<grid, ATT_THREADS, ATT_SMEM_TOTAL, stream>>>(tm, tmo, p);
   STEGO_CHECK_LAUNCH("attention_fwd_kernel");
   return STEGO_OK;
 }
-
-#ifdef STEGO_ATT_TRACE
-// Diagnostic build only: buffer of ATT_TRACE_SLOTS * 10 * ATT_TRACE_EVENTS * 2 u64 (zero it first); every-th CTA is traced.
-extern "C" int stego_attention_set_trace(unsigned long long* buf, int every) {
-  g_att_trace = buf;
-  g_att_trace_every = every;
-  return STEGO_OK;
-}
-#endif

@@ -1,9 +1,9 @@
-// Shared sm_100a device primitives for the STEGO hot path kernels:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (UMMA + TMEM) wrappers as inline PTX,
-// UMMA shared-memory / instruction descriptor builders and warp reductions.
+// Shared sm_90a device primitives for the STEGO hot path kernels:
+// mbarrier, TMA (cp.async.bulk.tensor), wgmma wrappers as inline PTX,
+// wgmma shared-memory descriptor builders and warp reductions.
 //
-// Everything here is written for sm_100a only (compile with
-//   -gencode arch=compute_100a,code=sm_100a).
+// Everything here is written for sm_90a only (compile with
+//   -gencode arch=compute_90a,code=sm_90a).
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -22,16 +22,6 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
 __device__ __forceinline__ uint32_t lane_id() { return threadIdx.x & 31u; }
-
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred = 0;
-  asm volatile(
-      "{\n\t.reg .pred P1;\n\t"
-      "elect.sync _|P1, 0xffffffff;\n\t"
-      "selp.b32 %0, 1, 0, P1;\n\t}\n"
-      : "=r"(pred));
-  return pred != 0;
-}
 
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
@@ -64,9 +54,8 @@ __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t by
                : "memory");
 }
 __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
-  // with a suspend-time hint the thread really sleeps until the phase completes (or the hint expires): without it
-  // try_wait came back every few hundred cycles and the retry loops of waiting warps executed ~20 % of all instructions
-  // of the attention kernel (ncu source counters: 1.8 M YIELD iterations), competing with the warps doing the work
+  // with a suspend-time hint the thread really sleeps until the phase completes (or the hint expires) instead of
+  // spinning in a retry loop that competes for issue slots with the warps doing the work
   uint32_t ok;
   asm volatile(
       "{\n\t.reg .pred P1;\n\t"
@@ -101,10 +90,11 @@ __device__ __forceinline__ uint64_t globaltimer_ns() {
   return t;
 }
 // Blocking wait with a watchdog: if a pipeline bug deadlocks the CTA we trap (launch error on the
-// host) instead of hanging the device.
+// host) instead of hanging the device.  No printf here: a function call anywhere in a kernel makes ptxas serialize
+// every wgmma of it.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  // non-blocking probe first: try_wait is a potentially-suspending instruction and costs ~200 cycles even when the phase
-  // completed long ago (clock64 stamps, profiles/r2_attn_trace.md); most waits of a well-fed pipeline end right here
+  // non-blocking probe first: try_wait is a potentially-suspending instruction; most waits of a well-fed pipeline end
+  // right here
   if (mbar_test_wait(bar, parity)) return;
   if (mbar_try_wait(bar, parity)) return;
   // try_wait suspends the thread by itself (up to its 1 ms hint); consult the global timer only every 64 retries.
@@ -116,8 +106,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
       if (t0 == 0) {
         t0 = now;
       } else if (now - t0 > STEGO_MBAR_TIMEOUT_NS) {
-        printf("stego_b200: mbarrier wait timed out (block %d,%d,%d thread %d bar %u parity %u)\n", blockIdx.x,
-               blockIdx.y, blockIdx.z, threadIdx.x, smem_u32(bar), parity);
         __trap();
       }
     }
@@ -153,34 +141,6 @@ __device__ __forceinline__ void tma_prefetch_l2_2d(const CUtensorMap* m, int c0,
                : "memory");
 }
 
-// multicast variant: the box lands at the same CTA-relative smem offset in every CTA of `cta_mask` and performs
-// complete_tx on the mbarrier at the same offset in each of them
-__device__ __forceinline__ void tma_load_2d_multicast(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
-                                                      uint16_t cta_mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
-      " [%0], [%1, {%3, %4}], [%2], %5;\n" ::"r"(smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(cta_mask)
-      : "memory");
-}
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;\n" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;\n" ::: "memory");
-}
-// tcgen05.commit arriving on the mbarrier at the same offset in every CTA of `cta_mask`
-__device__ __forceinline__ void umma_commit_multicast(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;\n" ::"r"(
-          smem_u32(bar)),
-      "h"(cta_mask)
-      : "memory");
-}
-
 // smem -> global tile store / fp32 reduce-add (bulk async group completion)
 __device__ __forceinline__ void tma_store_2d(const void* smem_src, const CUtensorMap* m, int c0, int c1) {
   asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];\n" ::"l"(
@@ -200,12 +160,6 @@ __device__ __forceinline__ void tma_reduce_add_2d(const void* smem_src, const CU
                "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
                : "memory");
 }
-__device__ __forceinline__ void tma_reduce_add_3d(const void* smem_src, const CUtensorMap* m, int c0, int c1, int c2) {
-  asm volatile("cp.reduce.async.bulk.tensor.3d.global.shared::cta.add.bulk_group [%0, {%2, %3, %4}], [%1];\n" ::"l"(
-                   reinterpret_cast<uint64_t>(m)),
-               "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2)
-               : "memory");
-}
 __device__ __forceinline__ void tma_commit_group() { asm volatile("cp.async.bulk.commit_group;\n" ::: "memory"); }
 template <int kPending>
 __device__ __forceinline__ void tma_wait_group_read() {
@@ -213,109 +167,75 @@ __device__ __forceinline__ void tma_wait_group_read() {
 }
 
 // ----------------------------------------------------------------------------------------------
-// tcgen05 / TMEM
+// wgmma (warpgroup MMA): four consecutive warps (a warpgroup, first warp index a multiple of 4) issue together; the
+// fp32 accumulator of an m64nNk16 lives in registers, N/2 per thread.  Fragment layout of accumulator register
+// d[4 c + e] of thread t (warp w = (t / 32) % 4, lane l): row 16 w + l / 4 + 8 (e >= 2), column 8 c + 2 (l % 4) + (e & 1).
 // ----------------------------------------------------------------------------------------------
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_slot) {
-  static_assert(kCols == 32 || kCols == 64 || kCols == 128 || kCols == 256 || kCols == 512, "pow2 >= 32");
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(smem_u32(smem_slot)),
-               "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n" ::: "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;\n" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;\n" ::: "memory"); }
+template <int kPending>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;\n" ::"n"(kPending) : "memory");
 }
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_dealloc(uint32_t tmem_base) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" ::"r"(tmem_base), "n"(kCols) : "memory");
+// keeps the compiler from moving accumulator reads / writes across the asynchronous wgmma window
+template <int kN>
+__device__ __forceinline__ void fence_operands(float (&d)[kN]) {
+#pragma unroll
+  for (int i = 0; i < kN; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem], bf16 inputs, fp32 accumulate. Issued by ONE thread.
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                          uint32_t accumulate) {
+
+// D (+)= A[smem] * B[smem] (kTransA / kTransB: 0 = K-major, 1 = MN-major operand), and D (+)= A[registers] * B[smem]
+// with the A fragment in the accumulator layout of an m64n16 tile packed to bf16 pairs (wgmma_rs_n64).
+template <int kTransA, int kTransB>
+__device__ __forceinline__ void wgmma_ss_n64(float (&d)[32], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, %35, %36;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(desc_a), "l"(desc_b), "r"(accumulate), "n"(kTransA), "n"(kTransB));
 }
-// D[tmem] (+)= A[tmem] * B[smem]: the A operand (M = 128 rows = the 128 TMEM lanes, K-major, two bf16 per 32-bit
-// column, 8 columns per UMMA_K = 16) is read from tensor memory — used for O += P V with P written by the softmax
-// warps straight into TMEM (no shared-memory round trip).  Issued by ONE thread.
-__device__ __forceinline__ void umma_bf16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc,
-                                             uint32_t accumulate) {
+
+template <int kTransA, int kTransB>
+__device__ __forceinline__ void wgmma_ss_n128(float (&d)[64], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, %67, %68;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(desc_a), "l"(desc_b), "r"(accumulate), "n"(kTransA), "n"(kTransB));
 }
-// Arrive on an mbarrier once all previously issued tcgen05.mma of this thread have completed.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n" ::"r"(smem_u32(bar))
-               : "memory");
-}
-// TMEM -> registers: this warp's 32 lanes (lane = accumulator row), 32 consecutive fp32 columns.
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
+
+template <int kTransA, int kTransB>
+__device__ __forceinline__ void wgmma_ss_n256(float (&d)[128], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, %128, %129, p, 1, 1, %131, %132;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(desc_a), "l"(desc_b), "r"(accumulate), "n"(kTransA), "n"(kTransB));
 }
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
+
+template <int kTransB>
+__device__ __forceinline__ void wgmma_rs_n64(float (&d)[32], const uint32_t (&a)[4], uint64_t desc_b, uint32_t accumulate) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, %38;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(accumulate), "n"(kTransB));
 }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory"); }
-// registers -> TMEM (same 32x32b shape as tmem_ld32)
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};\n" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]),
-      "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]),
-      "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
+
+template <int N, int kTransA, int kTransB>
+__device__ __forceinline__ void wgmma_ss(float (&d)[N / 2], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
+  static_assert(N == 64 || N == 128 || N == 256, "wgmma_ss: N must be 64, 128 or 256");
+  if constexpr (N == 64) wgmma_ss_n64<kTransA, kTransB>(d, desc_a, desc_b, accumulate);
+  else if constexpr (N == 128) wgmma_ss_n128<kTransA, kTransB>(d, desc_a, desc_b, accumulate);
+  else wgmma_ss_n256<kTransA, kTransB>(d, desc_a, desc_b, accumulate);
 }
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};\n" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-// 8-column variants (rare paths that must stay light on registers)
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, uint32_t (&r)[8]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];\n"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const uint32_t (&r)[8]) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};\n" ::"r"(taddr),
-               "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-               : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;\n" ::: "memory"); }
+
+// register budget hand-over between the producer and the MMA warpgroups (setmaxnreg)
+template <uint32_t kRegs>
+__device__ __forceinline__ void warpgroup_reg_alloc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;\n" ::"n"(kRegs)); }
+template <uint32_t kRegs>
+__device__ __forceinline__ void warpgroup_reg_dealloc() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;\n" ::"n"(kRegs)); }
+
 // single-instruction 2^x (MUFU.EX2, flush-to-zero): exp2f() adds denormal range handling we do not need
 __device__ __forceinline__ float ex2_approx(float x) {
   float y;
@@ -331,58 +251,37 @@ __device__ __forceinline__ float ex2_approx_v(float x) {
 }
 
 // ----------------------------------------------------------------------------------------------
-// UMMA descriptors (see cute/arch/mma_sm100_desc.hpp for the bit layout this follows)
+// wgmma shared-memory matrix descriptors (sm_90 GMMA layout)
 // ----------------------------------------------------------------------------------------------
-// Shared-memory matrix descriptor, SWIZZLE_128B, sm_100 version field = 1.
 //   start address  bits [0,14)   (>>4)
 //   LBO            bits [16,30)  (>>4)
 //   SBO            bits [32,46)  (>>4)
-//   version        bits [46,48)  = 1
-//   layout type    bits [61,64)  = 2 (SWIZZLE_128B)
+//   base offset    bits [49,52)  = 0 (every tile is 1024-byte aligned)
+//   layout type    bits [62,64)  = 1 (SWIZZLE_128B)
 // K-major operand tile ([rows][64 bf16] = 128 B per row, 8-row swizzle atoms of 1024 B):
-//   SBO = 1024 B (next 8-row group), LBO unused.
+//   SBO = 1024 B (next 8-row group), LBO unused; the next k16 slice starts 32 B further.
 // MN-major operand tile ([k rows][64 bf16 along M/N] per 64-wide block):
-//   SBO = 1024 B (next group of 8 k rows), LBO = byte distance between 64-element M/N blocks.
-__device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes,
-                                                         uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
-  d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;
-  d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
-  return d;
-}
-// The same descriptor split into its two 32-bit words: the high word is a compile-time constant and the low word is
-// (address >> 4) | LBO field, so stepping through a tile (next UMMA_K slice, next pipeline stage) is ONE integer add
-// on the low word instead of re-deriving all fields (the MMA-issuing thread is a serial bottleneck otherwise).
+//   SBO = 1024 B (next group of 8 k rows), LBO = byte distance between 64-element M/N blocks; next k16 slice: +2048 B.
+// The descriptor is kept as two 32-bit words: the high word is a compile-time constant and the low word is
+// (address >> 4) | LBO field, so stepping through a tile (next k slice, next pipeline stage) is ONE integer add.
 // Valid while the address stays below 256 KB (14-bit field), which holds for shared memory.
 __device__ __forceinline__ uint32_t smem_desc_lo(uint32_t smem_addr, uint32_t lbo_bytes) {
   return ((smem_addr & 0x3FFFFu) >> 4) | (((lbo_bytes >> 4) & 0x3FFFu) << 16);
 }
 __host__ __device__ constexpr uint32_t smem_desc_hi_sw128(uint32_t sbo_bytes) {
-  return ((sbo_bytes >> 4) & 0x3FFFu) | (1u << 14) | (2u << 29);
+  return ((sbo_bytes >> 4) & 0x3FFFu) | (1u << 30);
 }
 __device__ __forceinline__ uint64_t smem_desc_join(uint32_t lo, uint32_t hi) {
   return (static_cast<uint64_t>(hi) << 32) | lo;
 }
 
-// Instruction descriptor for kind::f16 with BF16 A/B and FP32 accumulator.
-//   c_format [4,6)=1 (F32); a_format [7,10)=1 (BF16); b_format [10,13)=1 (BF16)
-//   a_major bit 15, b_major bit 16 (0 = K-major, 1 = MN-major); n>>3 at [17,23); m>>4 at [24,29)
-__host__ __device__ constexpr uint32_t make_idesc_bf16(uint32_t m, uint32_t n, uint32_t a_mn_major,
-                                                       uint32_t b_mn_major) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (a_mn_major << 15) | (b_mn_major << 16) | ((n >> 3) << 17) |
-         ((m >> 4) << 24);
-}
-
 // Byte offset of element (row, 16-byte chunk) inside a [rows][128 B] SWIZZLE_128B tile whose base is
-// 1024-byte aligned (the layout TMA writes with CU_TENSOR_MAP_SWIZZLE_128B and UMMA expects).
+// 1024-byte aligned (the layout TMA writes with CU_TENSOR_MAP_SWIZZLE_128B and wgmma expects).
 __device__ __forceinline__ uint32_t sw128_offset(uint32_t row, uint32_t chunk16) {
   return row * 128u + ((chunk16 ^ (row & 7u)) << 4);
 }
 
-// Packed fp32x2 arithmetic (sm_100: two fp32 lanes per instruction on the FMA pipe)
+// fp32 pairs carried in one 64-bit register (two independent round-to-nearest fp32 operations per helper)
 __device__ __forceinline__ uint64_t pack_f32x2(float lo, float hi) {
   uint64_t r;
   asm("mov.b64 %0, {%1, %2};\n" : "=l"(r) : "f"(lo), "f"(hi));
@@ -392,14 +291,19 @@ __device__ __forceinline__ void unpack_f32x2(uint64_t v, float& lo, float& hi) {
   asm("mov.b64 {%0, %1}, %2;\n" : "=f"(lo), "=f"(hi) : "l"(v));
 }
 __device__ __forceinline__ uint64_t fma_f32x2(uint64_t a, uint64_t b, uint64_t c) {
-  uint64_t d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;\n" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
+  float a0, a1, b0, b1, c0, c1;
+  unpack_f32x2(a, a0, a1); unpack_f32x2(b, b0, b1); unpack_f32x2(c, c0, c1);
+  return pack_f32x2(__fmaf_rn(a0, b0, c0), __fmaf_rn(a1, b1, c1));
 }
 __device__ __forceinline__ uint64_t add_f32x2(uint64_t a, uint64_t b) {
-  uint64_t d;
-  asm("add.rn.f32x2 %0, %1, %2;\n" : "=l"(d) : "l"(a), "l"(b));
-  return d;
+  float a0, a1, b0, b1;
+  unpack_f32x2(a, a0, a1); unpack_f32x2(b, b0, b1);
+  return pack_f32x2(__fadd_rn(a0, b0), __fadd_rn(a1, b1));
+}
+__device__ __forceinline__ uint64_t mul_f32x2(uint64_t a, uint64_t b) {
+  float a0, a1, b0, b1;
+  unpack_f32x2(a, a0, a1); unpack_f32x2(b, b0, b1);
+  return pack_f32x2(__fmul_rn(a0, b0), __fmul_rn(a1, b1));
 }
 
 // bf16 pack helpers

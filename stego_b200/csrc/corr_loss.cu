@@ -1,5 +1,5 @@
-// Fused feature-correspondence loss for STEGO (sm_100a): sampling + L2-norm, the tensor_correlation
-// einsum on tcgen05, the centre/shift/clamp/product reduction, and the full backward.
+// Fused feature-correspondence loss for STEGO (sm_90a): sampling + L2-norm, the tensor_correlation
+// einsum on wgmma, the centre/shift/clamp/product reduction, and the full backward.
 //
 // Reference: src/modules.py
 //   :275-276 norm, :283-284 tensor_correlation (einsum nchw,ncij->nhwij), :287-288 sample (grid_sample),
@@ -11,17 +11,19 @@
 //                       L2-normalise over channels in fp32, write [128][C] operand tiles as a bf16 hi/lo SPLIT
 //                       (x = hi + lo).  The einsum is then three bf16 tensor-core passes
 //                       hi.hi + lo.hi + hi.lo, i.e. ~2^-16 relative accuracy with fp32 accumulation.
-//   2. corr_fwd       : one CTA per (image, call): TMA-staged tiles -> tcgen05.mma -> fd and cd accumulators in
-//                       TMEM (128 columns each); epilogue straight out of TMEM: row means (pointwise centring),
-//                       clamp, shift, product, five partial sums per CTA (no atomics, deterministic).
+//   2. corr_fwd       : one CTA per (image, call): TMA-staged tiles -> wgmma -> fd and cd accumulators in the
+//                       registers of two warpgroups (64 rows each); epilogue straight on the accumulator fragments: row
+//                       means (pointwise centring), clamp, shift, product, five partial sums per CTA (no atomics,
+//                       deterministic).
 //                       The batch-global `old_mean` enters the loss linearly, so it is applied in the finish step.
 //   3. corr_finish    : per call: old_mean, loss mean, cd mean.
-//   4. corr_bwd       : recomputes fd, cd (cheaper than stashing them), forms G = dL/dcd in registers, writes it
-//                       as a swizzled bf16 hi/lo tile to smem and runs the two backward GEMMs on the tensor core
+//   4. corr_bwd       : recomputes fd, cd (cheaper than stashing them), forms G = dL/dfd in registers, writes it
+//                       as a swizzled bf16 hi/lo tile to smem and runs the two backward GEMMs on the tensor cores
 //                       from the SAME smem image:  dA = G . Bc (G as K-major A) and dB = G^T . Ac (G as MN-major A);
 //                       the code tiles Ac/Bc stay resident in smem from the forward part and are reused as
 //                       MN-major B operands.  Results are accumulated into per-slot gradient tiles.
-//   5. sample_norm_bwd: normalisation backward + grid_sample backward (4-tap scatter-add into d_code).
+//   5. sample_norm_bwd: normalisation backward + grid_sample backward (per-pixel gather of the 4-tap contributions
+//                       into d_code, fixed order, no atomics).
 #include "common.cuh"
 #include "host_util.h"
 
@@ -268,7 +270,7 @@ struct CorrParams {
   int D;                // real code channels (<= CL_CODE_PAD)
 };
 
-constexpr int CL_THREADS = 192;
+constexpr int CL_THREADS = 384;  // two MMA warpgroups (rows 0..63 / 64..127 of the tile) + the TMA producer warpgroup
 constexpr uint32_t CL_TILE = 128 * 64 * 2;  // 16 KB
 
 __device__ __forceinline__ uint32_t tile_row(int plane, int slot, int b, int nslots, int B) {
@@ -281,6 +283,8 @@ __device__ __forceinline__ void split_pass(int pass, int& pa, int& pb) {
   pb = (pass == 2) ? 1 : 0;
 }
 
+// Forward: one CTA per (image, call).  Backward: one CTA per image walking the calls in order, so that every gradient
+// tile element has ONE writer and is accumulated in a fixed order (bit-reproducible run to run).
 template <bool kBackward>
 __global__ void __launch_bounds__(CL_THREADS, 1)
 corr_kernel(const __grid_constant__ CUtensorMap tmF, const __grid_constant__ CUtensorMap tmC, CorrParams p) {
@@ -290,7 +294,6 @@ corr_kernel(const __grid_constant__ CUtensorMap tmF, const __grid_constant__ CUt
   constexpr uint32_t CODE_BYTES = 8 * CL_TILE;  // Ac: [plane][kb] 4 tiles, Bc: 4 tiles
   constexpr uint32_t OFF_CODE = RING_BYTES;
   constexpr uint32_t OFF_BAR = OFF_CODE + CODE_BYTES;
-  constexpr uint32_t TMEM_COLS = kBackward ? 512 : 256;
 
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -298,280 +301,252 @@ corr_kernel(const __grid_constant__ CUtensorMap tmF, const __grid_constant__ CUt
   uint64_t* full_bar = bars;              // [kRing]
   uint64_t* empty_bar = bars + kRing;     // [kRing]
   uint64_t* code_full = empty_bar + kRing;  // [1]
-  uint64_t* acc_full = code_full + 1;       // [1]
-  uint64_t* g_full = acc_full + 1;          // [1] (backward)
-  uint64_t* d_full = g_full + 1;            // [1] (backward)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(d_full + 1);
-  float* red = reinterpret_cast<float*>(tmem_slot + 4);  // [4 warps][8]
+  uint64_t* call_done = code_full + 1;      // [1] backward: ring (G) and code tiles of the call are no longer read
+  float* red = reinterpret_cast<float*>(call_done + 1);  // [8 warps][8]
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int b = blockIdx.x;
-  const int call = blockIdx.y;
-  const int slotB = p.slot_of_call[call];
+  const int call_begin = kBackward ? 0 : static_cast<int>(blockIdx.y);
+  const int call_end = kBackward ? p.ncalls : call_begin + 1;
   const int nkb_f = p.E / 64;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmF);
     tma_prefetch_desc(&tmC);
-    for (int s = 0; s < kRing; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
+    for (int s = 0; s < kRing; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 2); }
     mbar_init(code_full, 1);
-    mbar_init(acc_full, 1);
-    mbar_init(g_full, 4);
-    mbar_init(d_full, 1);
+    mbar_init(call_done, 2);
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<TMEM_COLS>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t TM_FD = tmem_base, TM_CD = tmem_base + 128, TM_DA = tmem_base + 256, TM_DB = tmem_base + 384;
 
-  if (warp == 0) {
-    if (lane == 0) {
-      // code tiles first (small, resident): Ac planes then Bc planes, 2 k-blocks each
-      mbar_arrive_expect_tx(code_full, CODE_BYTES);
-      for (int pl = 0; pl < 2; ++pl)
-        for (int kb = 0; kb < 2; ++kb) {
-          tma_load_2d(smem + OFF_CODE + (pl * 2 + kb) * CL_TILE, &tmC, code_full, kb * 64,
-                      tile_row(pl, 0, b, p.nslots, p.B));
-          tma_load_2d(smem + OFF_CODE + (4 + pl * 2 + kb) * CL_TILE, &tmC, code_full, kb * 64,
-                      tile_row(pl, slotB, b, p.nslots, p.B));
-        }
+  if (warp >= 8) {
+    warpgroup_reg_dealloc<40>();
+    if (warp == 8 && lane == 0) {
       uint32_t stage = 0, phase = 0;
-      for (int pass = 0; pass < 3; ++pass) {
-        int pa, pb;
-        split_pass(pass, pa, pb);
-        for (int kb = 0; kb < nkb_f; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1u);
-          uint8_t* sa = smem + stage * 2 * CL_TILE;
-          mbar_arrive_expect_tx(&full_bar[stage], 2 * CL_TILE);
-          tma_load_2d(sa, &tmF, &full_bar[stage], kb * 64, tile_row(pa, 0, b, p.nslots, p.B));
-          tma_load_2d(sa + CL_TILE, &tmF, &full_bar[stage], kb * 64, tile_row(pb, slotB, b, p.nslots, p.B));
-          if (++stage == kRing) { stage = 0; phase ^= 1u; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // MMA issuer: the whole warp walks the schedule (uniform control flow -> descriptors in uniform registers), one
-    // elected lane issues.  All descriptors are base-low-word + constant steps (see smem_desc_lo).
-    {
-      constexpr uint32_t IDESC_KK = make_idesc_bf16(128, 128, 0, 0);
-      constexpr uint32_t DESC_HI = smem_desc_hi_sw128(1024);
-      constexpr uint32_t TILE16 = CL_TILE >> 4;
-      const uint32_t tmem_u = __shfl_sync(0xffffffffu, tmem_base, 0);
-      const uint32_t tm_fd = tmem_u, tm_cd = tmem_u + 128, tm_da = tmem_u + 256, tm_db = tmem_u + 384;
-      const uint32_t ring_lo = smem_desc_lo(smem_u32(smem), 16);
-      uint32_t stage = 0, phase = 0;
-      // fd = An_f . Bn_f^T  (3 split passes over E)
-      for (int pass = 0; pass < 3; ++pass) {
-        for (int kb = 0; kb < nkb_f; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t a_lo = ring_lo + stage * 2 * TILE16;
-          if (elect_one()) {
-#pragma unroll
-            for (uint32_t k = 0; k < 4; ++k)
-              umma_bf16(tm_fd, smem_desc_join(a_lo + 2 * k, DESC_HI), smem_desc_join(a_lo + TILE16 + 2 * k, DESC_HI), IDESC_KK,
-                        (pass | kb | static_cast<int>(k)) ? 1u : 0u);
-            umma_commit(&empty_bar[stage]);
+      for (int call = call_begin; call < call_end; ++call) {
+        const int slotB = p.slot_of_call[call];
+        if (call > call_begin) mbar_wait(call_done, static_cast<uint32_t>(call - call_begin - 1) & 1u);
+        // code tiles first (small, resident): Ac planes then Bc planes, 2 k-blocks each
+        mbar_arrive_expect_tx(code_full, CODE_BYTES);
+        for (int pl = 0; pl < 2; ++pl)
+          for (int kb = 0; kb < 2; ++kb) {
+            tma_load_2d(smem + OFF_CODE + (pl * 2 + kb) * CL_TILE, &tmC, code_full, kb * 64,
+                        tile_row(pl, 0, b, p.nslots, p.B));
+            tma_load_2d(smem + OFF_CODE + (4 + pl * 2 + kb) * CL_TILE, &tmC, code_full, kb * 64,
+                        tile_row(pl, slotB, b, p.nslots, p.B));
           }
-          __syncwarp();
-          if (++stage == kRing) { stage = 0; phase ^= 1u; }
-        }
-      }
-      // cd = An_c . Bn_c^T from the resident code tiles
-      mbar_wait(code_full, 0);
-      tc_fence_after();
-      const uint32_t code_lo = smem_desc_lo(smem_u32(smem + OFF_CODE), 16);
-      if (elect_one()) {
-#pragma unroll
         for (int pass = 0; pass < 3; ++pass) {
           int pa, pb;
           split_pass(pass, pa, pb);
-#pragma unroll
-          for (int kb = 0; kb < 2; ++kb) {
-            const uint32_t a_lo = code_lo + (pa * 2 + kb) * TILE16;
-            const uint32_t b_lo = code_lo + (4 + pb * 2 + kb) * TILE16;
-#pragma unroll
-            for (uint32_t k = 0; k < 4; ++k)
-              umma_bf16(tm_cd, smem_desc_join(a_lo + 2 * k, DESC_HI), smem_desc_join(b_lo + 2 * k, DESC_HI), IDESC_KK,
-                        (pass | kb | static_cast<int>(k)) ? 1u : 0u);
+          for (int kb = 0; kb < nkb_f; ++kb) {
+            mbar_wait(&empty_bar[stage], phase ^ 1u);
+            uint8_t* sa = smem + stage * 2 * CL_TILE;
+            mbar_arrive_expect_tx(&full_bar[stage], 2 * CL_TILE);
+            tma_load_2d(sa, &tmF, &full_bar[stage], kb * 64, tile_row(pa, 0, b, p.nslots, p.B));
+            tma_load_2d(sa + CL_TILE, &tmF, &full_bar[stage], kb * 64, tile_row(pb, slotB, b, p.nslots, p.B));
+            if (++stage == kRing) { stage = 0; phase ^= 1u; }
           }
         }
-        umma_commit(acc_full);
       }
-      __syncwarp();
-      if (kBackward) {
-        // G (bf16 hi/lo, [i][j] swizzled K-major image) is written by the epilogue warps into the ring area.
-        mbar_wait(g_full, 0);
-        tc_fence_after();
-        constexpr uint32_t IDESC_K_MN = make_idesc_bf16(128, 128, 0, 1);   // A K-major, B MN-major
-        constexpr uint32_t IDESC_MN_MN = make_idesc_bf16(128, 128, 1, 1);  // A MN-major, B MN-major
-        // MN-major operands: LBO = CL_TILE (64-wide blocks 16 KB apart); G planes: hi at +0, lo at +32 KB
-        const uint32_t g_k_lo = ring_lo;                                          // G as K-major A operand
-        const uint32_t g_mn_lo = smem_desc_lo(smem_u32(smem), CL_TILE);           // G^T as MN-major A operand
-        const uint32_t code_mn_lo = smem_desc_lo(smem_u32(smem + OFF_CODE), CL_TILE);
-        if (elect_one()) {
+    }
+    return;
+  }
+
+  // ===================== MMA warpgroups: rows 64 mwg .. 64 mwg + 63 of fd / cd =====================
+  warpgroup_reg_alloc<232>();
+  const int mwg = warp >> 2;
+  const int wq = warp & 3;
+  const bool leader = (threadIdx.x & 127) == 0;
+  constexpr uint32_t DESC_HI = smem_desc_hi_sw128(1024);
+  constexpr uint32_t TILE16 = CL_TILE >> 4;
+  constexpr uint32_t HALF16 = (CL_TILE / 2) >> 4;  // rows 64.. of a [128][64] K-major tile
+  const uint32_t ring_lo = smem_desc_lo(smem_u32(smem), 16);
+  const uint32_t code_lo = smem_desc_lo(smem_u32(smem + OFF_CODE), 16);
+  // this thread's accumulator fragment: rows i = 64 mwg + 16 wq + lane / 4 (+ 8 for h = 1), columns
+  // j = 8 n + 2 (lane % 4) + {0, 1}
+  const int S = p.S;
+  const int i_top = mwg * 64 + wq * 16 + (lane >> 2);
+  const int j_base = 2 * (lane & 3);
+  uint32_t stage = 0, phase = 0;
+  for (int call = call_begin; call < call_end; ++call) {
+    const int slotB = p.slot_of_call[call];
+    const uint32_t it = static_cast<uint32_t>(call - call_begin);
+    float fd[64], cd[64];
 #pragma unroll
-          for (int pass = 0; pass < 3; ++pass) {
-            int pg, pc;
-            split_pass(pass, pg, pc);
-            const uint32_t g_off = pg * 2 * TILE16;
-            const uint32_t bc_lo = code_mn_lo + (4 + pc * 2) * TILE16;  // Bc plane: c-blocks 16 KB apart, rows = j
-            const uint32_t ac_lo = code_mn_lo + (pc * 2) * TILE16;      // Ac plane: rows = i
+    for (int t = 0; t < 64; ++t) { fd[t] = 0.f; cd[t] = 0.f; }
+    {
+      // fd = An_f . Bn_f^T  (3 split passes over E)
+      uint32_t prev = 0;
+      for (int ks = 0; ks < 3 * nkb_f; ++ks) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t a_lo = ring_lo + stage * 2 * TILE16;
+        fence_operands(fd);
+        wgmma_fence();
 #pragma unroll
-            for (uint32_t kk = 0; kk < 8; ++kk) {
-              // dA[i][c] += sum_j G[i][j] Bc[j][c]: A = G K-major (k = j), B = Bc MN-major (n = c contiguous)
-              umma_bf16(tm_da, smem_desc_join(g_k_lo + g_off + (kk >> 2) * TILE16 + (kk & 3) * 2, DESC_HI),
-                        smem_desc_join(bc_lo + kk * (2048u >> 4), DESC_HI), IDESC_K_MN, (pass | static_cast<int>(kk)) ? 1u : 0u);
-            }
+        for (uint32_t k = 0; k < 4; ++k)
+          wgmma_ss<128, 0, 0>(fd, smem_desc_join(a_lo + mwg * HALF16 + 2 * k, DESC_HI),
+                              smem_desc_join(a_lo + TILE16 + 2 * k, DESC_HI), 1u);
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (ks > 0 && leader) mbar_arrive(&empty_bar[prev]);
+        prev = stage;
+        if (++stage == kRing) { stage = 0; phase ^= 1u; }
+      }
+      // cd = An_c . Bn_c^T from the resident code tiles
+      mbar_wait(code_full, it & 1u);
+      wgmma_fence();
 #pragma unroll
-            for (uint32_t kk = 0; kk < 8; ++kk) {
-              // dB[j][c] += sum_i G[i][j] Ac[i][c]: A = G^T as MN-major (m = j contiguous, k = i rows)
-              umma_bf16(tm_db, smem_desc_join(g_mn_lo + g_off + kk * (2048u >> 4), DESC_HI),
-                        smem_desc_join(ac_lo + kk * (2048u >> 4), DESC_HI), IDESC_MN_MN, (pass | static_cast<int>(kk)) ? 1u : 0u);
-            }
-          }
-          umma_commit(d_full);
+      for (int pass = 0; pass < 3; ++pass) {
+        int pa, pb;
+        split_pass(pass, pa, pb);
+#pragma unroll
+        for (int kb = 0; kb < 2; ++kb) {
+          const uint32_t a_lo = code_lo + (pa * 2 + kb) * TILE16 + mwg * HALF16;
+          const uint32_t b_lo = code_lo + (4 + pb * 2 + kb) * TILE16;
+#pragma unroll
+          for (uint32_t k = 0; k < 4; ++k)
+            wgmma_ss<128, 0, 0>(cd, smem_desc_join(a_lo + 2 * k, DESC_HI), smem_desc_join(b_lo + 2 * k, DESC_HI), 1u);
         }
-        __syncwarp();
       }
+      wgmma_commit();
+      wgmma_wait<0>();
+      fence_operands(fd);
+      fence_operands(cd);
+      if (leader) mbar_arrive(&empty_bar[prev]);
     }
-  } else {
-    // ===================== epilogue warps =====================
-    const int quarter = warp & 3;
-    const int i = quarter * 32 + lane;  // sample row
-    const uint32_t lane_off = static_cast<uint32_t>(quarter * 32) << 16;
-    const int S = p.S;
-    const bool row_ok = i < S;
-    mbar_wait(acc_full, 0);
-    tc_fence_after();
-    // pass 1: row sum of fd over the valid columns
-    float rsum = 0.f;
-#pragma unroll 1
-    for (int ch = 0; ch < 4; ++ch) {
-      uint32_t v[32];
-      tmem_ld32(TM_FD + lane_off + ch * 32, v);
-      tmem_ld_wait();
+
+    // ===================== epilogue on the accumulator fragments =====================
+    // pass 1: row sums of fd over the valid columns (the four lanes of a row hold disjoint columns)
+    float rsum[2] = {0.f, 0.f};
 #pragma unroll
-      for (int t = 0; t < 32; ++t)
-        if (ch * 32 + t < S) rsum += __uint_as_float(v[t]);
+    for (int t = 0; t < 64; ++t)
+      if (8 * (t >> 2) + j_base + (t & 1) < S) rsum[(t >> 1) & 1] += fd[t];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      rsum[h] += __shfl_xor_sync(0xffffffffu, rsum[h], 1);
+      rsum[h] += __shfl_xor_sync(0xffffffffu, rsum[h], 2);
     }
-    const float rmean = p.pointwise ? rsum / static_cast<float>(S) : 0.f;
     const float shift = p.shift[call];
-    float P1 = 0.f, P2 = 0.f, P3 = row_ok ? rsum : 0.f, P4 = 0.f, P5 = 0.f;
     float offset = 0.f, gs = 0.f;
     if (kBackward) {
       const float* st = p.stats + call * 4;
       offset = p.pointwise ? (st[2] - st[3]) : 0.f;  // old_mean - mean(centred fd)
       gs = p.gscale[call] / (static_cast<float>(p.B) * S * S);
     }
-    const size_t eoff = ((static_cast<size_t>(call) * p.B + b) * S + i) * S;
-#pragma unroll 1
-    for (int ch = 0; ch < 4; ++ch) {
-      uint32_t vf[32], vc[32];
-      tmem_ld32(TM_FD + lane_off + ch * 32, vf);
-      tmem_ld32(TM_CD + lane_off + ch * 32, vc);
-      tmem_ld_wait();
-      float g[32];
+    float P1 = 0.f, P2 = 0.f, P3 = 0.f, P4 = 0.f, P5 = 0.f;
+    if (!kBackward && (lane & 3) == 0) {  // each row's sum once
+      if (i_top < S) P3 += rsum[0];
+      if (i_top + 8 < S) P3 += rsum[1];
+    }
 #pragma unroll
-      for (int t = 0; t < 32; ++t) {
-        const int j = ch * 32 + t;
-        const bool ok = row_ok && j < S;
-        const float fdc = __uint_as_float(vf[t]) - rmean;
-        const float cd = __uint_as_float(vc[t]);
-        if (!kBackward) {
-          if (ok) {
-            const float cl = fminf(fmaxf(cd, p.clamp_lo), p.clamp_hi);
-            P1 += cl * (fdc - shift);
-            P2 += cl;
-            P4 += fdc;
-            P5 += cd;
-            if (p.cd_out) p.cd_out[eoff + j] = cd;
-            if (p.fdc_out) p.fdc_out[eoff + j] = fdc;
-          }
-        } else {
-          float gv = 0.f;
-          if (ok) {
-            float up = gs;
-            if (p.gelem) up += p.gelem[eoff + j];
-            const bool pass_grad = (cd >= p.clamp_lo) && (cd <= p.clamp_hi);
-            gv = pass_grad ? -up * (fdc + offset - shift) : 0.f;
-            if (p.gcd) gv += p.gcd[eoff + j];
-          }
-          g[t] = gv;
+    for (int t = 0; t < 64; ++t) {
+      const int h = (t >> 1) & 1;
+      const int i = i_top + 8 * h;
+      const int j = 8 * (t >> 2) + j_base + (t & 1);
+      const bool ok = i < S && j < S;
+      const float rmean = p.pointwise ? rsum[h] / static_cast<float>(S) : 0.f;
+      const float fdc = fd[t] - rmean;
+      const float cdv = cd[t];
+      const size_t e = ((static_cast<size_t>(call) * p.B + b) * S + i) * S + j;
+      if (!kBackward) {
+        if (ok) {
+          const float cl = fminf(fmaxf(cdv, p.clamp_lo), p.clamp_hi);
+          P1 += cl * (fdc - shift);
+          P2 += cl;
+          P4 += fdc;
+          P5 += cdv;
+          if (p.cd_out) p.cd_out[e] = cdv;
+          if (p.fdc_out) p.fdc_out[e] = fdc;
         }
-      }
-      if (kBackward) {
-        // G[i][j] -> smem (ring area, free: every feature MMA has retired before acc_full fired)
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          uint4 wh, wl;
-          float h[8];
-#pragma unroll
-          for (int t = 0; t < 8; ++t) h[t] = __bfloat162float(__float2bfloat16_rn(g[8 * q + t]));
-          wh.x = pack_bf16x2(h[0], h[1]); wh.y = pack_bf16x2(h[2], h[3]);
-          wh.z = pack_bf16x2(h[4], h[5]); wh.w = pack_bf16x2(h[6], h[7]);
-          wl.x = pack_bf16x2(g[8 * q + 0] - h[0], g[8 * q + 1] - h[1]);
-          wl.y = pack_bf16x2(g[8 * q + 2] - h[2], g[8 * q + 3] - h[3]);
-          wl.z = pack_bf16x2(g[8 * q + 4] - h[4], g[8 * q + 5] - h[5]);
-          wl.w = pack_bf16x2(g[8 * q + 6] - h[6], g[8 * q + 7] - h[7]);
-          const uint32_t o = (ch >> 1) * CL_TILE + sw128_offset(i, (ch & 1) * 4 + q);
-          *reinterpret_cast<uint4*>(smem + o) = wh;
-          *reinterpret_cast<uint4*>(smem + 2 * CL_TILE + o) = wl;
+      } else {
+        float gv = 0.f;
+        if (ok) {
+          float up = gs;
+          if (p.gelem) up += p.gelem[e];
+          const bool pass_grad = (cdv >= p.clamp_lo) && (cdv <= p.clamp_hi);
+          gv = pass_grad ? -up * (fdc + offset - shift) : 0.f;
+          if (p.gcd) gv += p.gcd[e];
         }
+        fd[t] = gv;  // G in place of fd
       }
     }
     if (!kBackward) {
       // deterministic block reduction of the five partial sums
       P1 = warp_sum(P1); P2 = warp_sum(P2); P3 = warp_sum(P3); P4 = warp_sum(P4); P5 = warp_sum(P5);
       if (lane == 0) {
-        float* r = red + quarter * 8;
+        float* r = red + warp * 8;
         r[0] = P1; r[1] = P2; r[2] = P3; r[3] = P4; r[4] = P5;
       }
-      asm volatile("bar.sync 1, 128;\n" ::: "memory");
-      if (warp == 2 && lane < 5) {
-        const float tot = red[lane] + red[8 + lane] + red[16 + lane] + red[24 + lane];
+      asm volatile("bar.sync 1, 256;\n" ::: "memory");
+      if (warp == 0 && lane < 5) {
+        float tot = 0.f;
+#pragma unroll
+        for (int w = 0; w < 8; ++w) tot += red[w * 8 + lane];
         p.partials[(static_cast<size_t>(call) * p.B + b) * 8 + lane] = tot;
       }
-    } else {
-      tc_fence_before();
-      fence_proxy_async_smem();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(g_full);
-      mbar_wait(d_full, 0);
-      tc_fence_after();
-      // dA -> slot 0, dB -> slot of this call (slot 0 again for the intra call: code is on both GEMM sides)
-      float* dA = p.dtiles + ((static_cast<size_t>(0) * p.B + b) * CL_ROWS + i) * CL_DT_LD;
-      float* dB = p.dtiles + ((static_cast<size_t>(slotB) * p.B + b) * CL_ROWS + i) * CL_DT_LD;
-#pragma unroll 1
-      for (int ch = 0; ch < 3; ++ch) {  // 96 >= D columns
-        if (ch * 32 >= p.D) break;
-        uint32_t va[32], vb[32];
-        tmem_ld32(TM_DA + lane_off + ch * 32, va);
-        tmem_ld32(TM_DB + lane_off + ch * 32, vb);
-        tmem_ld_wait();
-        if (row_ok) {
+      return;
+    }
+    // ---- backward: G[i][j] as a bf16 hi/lo split into the ring area ([j block][i][64 j], 128B-swizzled K-major image,
+    //      hi plane at +0, lo plane at +2 tiles).  Both warpgroups' feature MMAs must have retired first.
+    asm volatile("bar.sync 1, 256;\n" ::: "memory");
 #pragma unroll
-          for (int t = 0; t < 32; ++t) {
-            const int c = ch * 32 + t;
-            if (c < p.D) {
-              atomicAdd(dA + c, __uint_as_float(va[t]));
-              atomicAdd(dB + c, __uint_as_float(vb[t]));
-            }
-          }
-        }
+    for (int t = 0; t < 64; t += 2) {
+      const int i = i_top + 8 * ((t >> 1) & 1);
+      const int j = 8 * (t >> 2) + j_base;
+      const float h0 = __bfloat162float(__float2bfloat16_rn(fd[t]));
+      const float h1 = __bfloat162float(__float2bfloat16_rn(fd[t + 1]));
+      const uint32_t o = (j >> 6) * CL_TILE + sw128_offset(i, (j & 63) >> 3) + (j & 7) * 2;
+      *reinterpret_cast<uint32_t*>(smem + o) = pack_bf16x2(h0, h1);
+      *reinterpret_cast<uint32_t*>(smem + 2 * CL_TILE + o) = pack_bf16x2(fd[t] - h0, fd[t + 1] - h1);
+    }
+    fence_proxy_async_smem();  // generic-proxy smem writes -> visible to the tensor cores
+    asm volatile("bar.sync 1, 256;\n" ::: "memory");
+    {
+      // dA[i][c] += sum_j G[i][j] Bc[j][c]: A = G K-major (k = j), B = Bc MN-major (n = c contiguous), rows i of this
+      // warpgroup (accumulated in cd).  dB[j][c] += sum_i G[i][j] Ac[i][c]: A = G^T MN-major (m = j: the j block of this
+      // warpgroup, k = i), accumulated in fd.  MN-major operands: LBO = CL_TILE (64-wide blocks 16 KB apart).
+      const uint32_t g_k_lo = ring_lo + mwg * HALF16;
+      const uint32_t g_mn_lo = smem_desc_lo(smem_u32(smem), CL_TILE) + mwg * TILE16;
+      const uint32_t code_mn_lo = smem_desc_lo(smem_u32(smem + OFF_CODE), CL_TILE);
+#pragma unroll
+      for (int t = 0; t < 64; ++t) { cd[t] = 0.f; fd[t] = 0.f; }
+      wgmma_fence();
+#pragma unroll
+      for (int pass = 0; pass < 3; ++pass) {
+        int pg, pc;
+        split_pass(pass, pg, pc);
+        const uint32_t g_off = pg * 2 * TILE16;
+        const uint32_t bc_lo = code_mn_lo + (4 + pc * 2) * TILE16;  // Bc plane: c-blocks 16 KB apart, rows = j
+        const uint32_t ac_lo = code_mn_lo + (pc * 2) * TILE16;      // Ac plane: rows = i
+#pragma unroll
+        for (uint32_t kk = 0; kk < 8; ++kk)
+          wgmma_ss<128, 0, 1>(cd, smem_desc_join(g_k_lo + g_off + (kk >> 2) * TILE16 + (kk & 3) * 2, DESC_HI),
+                              smem_desc_join(bc_lo + kk * (2048u >> 4), DESC_HI), 1u);
+#pragma unroll
+        for (uint32_t kk = 0; kk < 8; ++kk)
+          wgmma_ss<128, 1, 1>(fd, smem_desc_join(g_mn_lo + g_off + kk * (2048u >> 4), DESC_HI),
+                              smem_desc_join(ac_lo + kk * (2048u >> 4), DESC_HI), 1u);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      fence_operands(cd);
+      fence_operands(fd);
+    }
+    if (leader) mbar_arrive(call_done);  // the producer may refill the ring and the code tiles
+    // dA -> slot 0, dB -> slot of this call (slot 0 again for the intra call: code is on both GEMM sides).  This CTA
+    // owns image b, and each element belongs to one thread: plain read-modify-write in call order.  Rows >= S carry
+    // zero gradients and are skipped.
+#pragma unroll
+    for (int t = 0; t < 64; ++t) {
+      const int r = i_top + 8 * ((t >> 1) & 1);
+      const int c = 8 * (t >> 2) + j_base + (t & 1);
+      if (r < S && c < p.D) {
+        p.dtiles[((static_cast<size_t>(0) * p.B + b) * CL_ROWS + r) * CL_DT_LD + c] += cd[t];
+        p.dtiles[((static_cast<size_t>(slotB) * p.B + b) * CL_ROWS + r) * CL_DT_LD + c] += fd[t];
       }
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<TMEM_COLS>(tmem_base);
   }
 }
 
@@ -614,7 +589,9 @@ __global__ void corr_loss_elems_kernel(const float* __restrict__ cd, const float
 }
 
 // ---------------------------------------------------------------------------------------------
-// 5. normalisation + grid_sample backward: one warp per (slot, image, sample)
+// 5. normalisation + grid_sample backward, as a gather: one warp per destination pixel (of code or code_pos) visits
+//    every (slot, image, sample) whose bilinear taps reach that pixel, in a fixed order, and writes its channels once —
+//    no atomics, so the code gradient is bit-reproducible run to run.
 // ---------------------------------------------------------------------------------------------
 struct SampleBwdParams {
   SampleParams f;        // forward description of the code sampling (src = code, src_pos = code_pos)
@@ -623,21 +600,11 @@ struct SampleBwdParams {
   float* dsrc_pos;
 };
 
+// d/dv of the normalised sample v/||v|| for (slot, b, s), lane-owned channels lane + 32 k
 template <int NV>
-__global__ void __launch_bounds__(256)
-sample_norm_bwd_kernel(SampleBwdParams q) {
+__device__ __forceinline__ void sample_dv(const SampleBwdParams& q, int slot, int b, int s, const Taps& t,
+                                          const float* src, int img, int lane, float (&dv)[NV]) {
   const SampleParams& p = q.f;
-  const int warp_global = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  const int lane = threadIdx.x & 31;
-  const int total = p.nslots * p.B * p.S;
-  if (warp_global >= total) return;
-  const int s = warp_global % p.S;
-  const int b = (warp_global / p.S) % p.B;
-  const int slot = warp_global / (p.S * p.B);
-  const void* src; const float* cscale; const float* coords; int img;
-  slot_source(p, slot, b, src, cscale, coords, img);
-  float* dsrc = (slot == 1) ? q.dsrc_pos : q.dsrc;
-  const Taps t = make_taps(coords, b, s, p.fs, p.H, p.W);
   auto off = [&](int pix) { return static_cast<long long>(pix / p.W) * p.sy + static_cast<long long>(pix % p.W) * p.sx; };
   const long long o00 = off(t.i00), o01 = off(t.i01), o10 = off(t.i10), o11 = off(t.i11);
   const long long base = static_cast<long long>(img) * p.sb;
@@ -649,7 +616,7 @@ sample_norm_bwd_kernel(SampleBwdParams q) {
     const int c = lane + 32 * k;
     float val = 0.f, gg = 0.f;
     if (c < p.C) {
-      const float* qf = reinterpret_cast<const float*>(src) + base + static_cast<long long>(c) * p.sc;
+      const float* qf = src + base + static_cast<long long>(c) * p.sc;
       val = qf[o00] * t.w00;
       val += qf[o01] * t.w01;
       val += qf[o10] * t.w10;
@@ -665,20 +632,75 @@ sample_norm_bwd_kernel(SampleBwdParams q) {
   const float nrm = sqrtf(ss);
 #pragma unroll
   for (int k = 0; k < NV; ++k) {
-    const int c = lane + 32 * k;
-    if (c >= p.C) continue;
-    float dv;
     if (nrm > p.eps) {
       const float inv = 1.0f / nrm;
-      dv = (gr[k] - v[k] * (dot * inv * inv)) * inv;  // d/dv of v/||v||
+      dv[k] = (gr[k] - v[k] * (dot * inv * inv)) * inv;  // d/dv of v/||v||
     } else {
-      dv = gr[k] / p.eps;
+      dv[k] = gr[k] / p.eps;
     }
-    float* d = dsrc + base + static_cast<long long>(c) * p.sc;
-    if (t.w00 != 0.f) atomicAdd(d + o00, dv * t.w00);
-    if (t.w01 != 0.f) atomicAdd(d + o01, dv * t.w01);
-    if (t.w10 != 0.f) atomicAdd(d + o10, dv * t.w10);
-    if (t.w11 != 0.f) atomicAdd(d + o11, dv * t.w11);
+  }
+}
+
+template <int NV>
+__global__ void __launch_bounds__(256)
+sample_norm_bwd_kernel(SampleBwdParams q) {
+  const SampleParams& p = q.f;
+  const int warp_global = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  const int HW = p.H * p.W;
+  if (warp_global >= 2 * p.B * HW) return;
+  const bool pos = warp_global >= p.B * HW;  // destination: code_pos (slot 1 only) or code (slot 0 and slots >= 2)
+  const int dst_img = (warp_global % (p.B * HW)) / HW;
+  const int pix = warp_global % HW;
+  float acc[NV];
+#pragma unroll
+  for (int k = 0; k < NV; ++k) acc[k] = 0.f;
+  for (int slot = 0; slot < p.nslots; ++slot) {
+    if ((slot == 1) != pos) continue;
+    for (int b0 = 0; b0 < p.B; b0 += 32) {
+      // the images (slot, b0 + lane) sample from, tested 32 at a time; then the hits in ascending b
+      int lane_img = -1;
+      if (b0 + lane < p.B) {
+        const void* src_l; const float* cscale_l; const float* coords_l;
+        slot_source(p, slot, b0 + lane, src_l, cscale_l, coords_l, lane_img);
+      }
+      uint32_t bhits = __ballot_sync(0xffffffffu, lane_img == dst_img);
+      while (bhits) {
+        const int b = b0 + __ffs(bhits) - 1;
+        bhits &= bhits - 1;
+        const void* src; const float* cscale; const float* coords; int img;
+        slot_source(p, slot, b, src, cscale, coords, img);
+        for (int s0 = 0; s0 < p.S; s0 += 32) {
+          const int s = s0 + lane;
+          float w = 0.f;
+          Taps t;
+          if (s < p.S) {
+            t = make_taps(coords, b, s, p.fs, p.H, p.W);
+            // at most one tap with a non-zero weight lands on a given pixel (a clamped duplicate tap has weight 0)
+            w = (t.i00 == pix && t.w00 != 0.f) ? t.w00 : (t.i01 == pix && t.w01 != 0.f) ? t.w01
+              : (t.i10 == pix && t.w10 != 0.f) ? t.w10 : (t.i11 == pix && t.w11 != 0.f) ? t.w11 : 0.f;
+          }
+          uint32_t hits = __ballot_sync(0xffffffffu, w != 0.f);
+          while (hits) {  // samples in ascending order
+            const int src_lane = __ffs(hits) - 1;
+            hits &= hits - 1;
+            const float wm = __shfl_sync(0xffffffffu, w, src_lane);
+            const Taps tm = make_taps(coords, b, s0 + src_lane, p.fs, p.H, p.W);
+            float dv[NV];
+            sample_dv<NV>(q, slot, b, s0 + src_lane, tm, reinterpret_cast<const float*>(src), img, lane, dv);
+#pragma unroll
+            for (int k = 0; k < NV; ++k) acc[k] += dv[k] * wm;
+          }
+        }
+      }
+    }
+  }
+  float* d = (pos ? q.dsrc_pos : q.dsrc) + static_cast<long long>(dst_img) * p.sb +
+             static_cast<long long>(pix / p.W) * p.sy + static_cast<long long>(pix % p.W) * p.sx;
+#pragma unroll
+  for (int k = 0; k < NV; ++k) {
+    const int c = lane + 32 * k;
+    if (c < p.C) d[static_cast<long long>(c) * p.sc] += acc[k];
   }
 }
 
@@ -788,6 +810,7 @@ template <bool kBwd>
 static int launch_corr(const CUtensorMap& tmF, const CUtensorMap& tmC, const CorrParams& p, cudaStream_t stream) {
   constexpr int kRing = kBwd ? 2 : 3;
   constexpr size_t smem = size_t(kRing) * 2 * CL_TILE + 8 * CL_TILE + 512 + 1024;
+  static_assert(smem <= 232448, "exceeds the 227 KB of shared memory a CTA can opt into");
   auto kern = corr_kernel<kBwd>;
   static bool configured = false;
   if (!configured) {
@@ -795,7 +818,7 @@ static int launch_corr(const CUtensorMap& tmF, const CUtensorMap& tmC, const Cor
     if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(corr)");
     configured = true;
   }
-  kern<<<dim3(p.B, p.ncalls), CL_THREADS, smem, stream>>>(tmF, tmC, p);
+  kern<<<dim3(p.B, kBwd ? 1 : p.ncalls), CL_THREADS, smem, stream>>>(tmF, tmC, p);
   STEGO_CHECK_LAUNCH("corr_kernel");
   return STEGO_OK;
 }
@@ -861,7 +884,7 @@ extern "C" int stego_sample_norm_bwd(const float* code, const float* code_pos, l
   if (rc != STEGO_OK) return rc;
   q.f.perms_raw = perms_are_raw_randperm;
   q.dtiles = dtiles; q.dsrc = dcode; q.dsrc_pos = dcode_pos;
-  const int warps = nslots * B * q.f.S;
+  const int warps = 2 * B * H * W;
   sample_norm_bwd_kernel<3><<<(warps + 7) / 8, 256, 0, stream>>>(q);
   STEGO_CHECK_LAUNCH("sample_norm_bwd_kernel");
   return STEGO_OK;

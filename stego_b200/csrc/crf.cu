@@ -5,7 +5,7 @@
 //     d = DenseCRF2D(w, h, c); d.setUnaryEnergy(-log softmax);
 //     d.addPairwiseGaussian(sxy=1, compat=3); d.addPairwiseBilateral(sxy=67, srgb=3, rgbim, compat=4); Q = d.inference(10)
 // i.e. mean-field inference in a fully connected CRF (Kraehenbuehl & Koltun 2011) whose two Gaussian kernels are applied
-// with the permutohedral lattice (Adams et al. 2010).  pydensecrf is third-party C++ that is not in /root/reference; the
+// with the permutohedral lattice (Adams et al. 2010).  pydensecrf is third-party C++ that is not in the reference; the
 // algorithm below follows its published sources (densecrf.cpp / pairwise.cpp / permutohedral.cpp) as restated by
 // oracle/crf_oracle.py — parity with the reference's CRF stage is UNPINNED (DESIGN.md), the CUDA path is tested against
 // that restatement.

@@ -38,16 +38,10 @@ __device__ __forceinline__ float gelu_erf_poly(float x) {
   return 0.5f * x * (1.0f + copysignf(e, x));
 }
 
-// bf16-output GELU, eight elements in lock-step as four packed fp32x2 lanes (FFMA2 / FMUL2: two fp32 results per
-// issue slot), ~8 instructions per element instead of 13:
+// bf16-output GELU, eight elements in lock-step as four fp32 pairs, ~8 instructions per element instead of 13:
 //   erf(|x|/sqrt2) = xc * Q(xc^2), xc = min(|x|, 3.2*sqrt2), Q of degree 8 (minimax fit, |abs err| < 4.3e-5 in
 //   fp32 evaluation — two orders of magnitude below the bf16 rounding of the result), and
 //   gelu(x) = 0.5 x (1 + sign(x) erf(|x|/sqrt2)) = h + |h| * e with h = x/2.
-__device__ __forceinline__ uint64_t mul_f32x2(uint64_t a, uint64_t b) {
-  uint64_t d;
-  asm("mul.rn.f32x2 %0, %1, %2;\n" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
 __device__ __forceinline__ void gelu_erf_poly8(float* x) {
   uint64_t xc[4], u[4], q[4];
 #pragma unroll
@@ -73,121 +67,6 @@ __device__ __forceinline__ void gelu_erf_poly8(float* x) {
     const float h0 = 0.5f * x[2 * j], h1 = 0.5f * x[2 * j + 1];
     const uint64_t r = fma_f32x2(pack_f32x2(fabsf(h0), fabsf(h1)), e, pack_f32x2(h0, h1));
     unpack_f32x2(r, x[2 * j], x[2 * j + 1]);
-  }
-}
-
-}  // namespace stego
-
-namespace stego {
-
-// TMA epilogue of one accumulator tile, executed by ONE epilogue warp for its 32 TMEM lanes (rows) and every second
-// column group (`half` selects which): TMEM -> registers (bias / activation) -> 128B-swizzled staging tile in shared
-// memory -> one bulk tensor store (or fp32 reduce-add into the in-place residual) per 32-row x 128-byte tile.
-// Shared by the 1-CTA and 2-CTA GEMM kernels; edges are clipped by the tensor map.
-struct EpiArgs {
-  const float* bias;  // [N] or null
-  int act;            // 0 none, 1 GELU(erf), 2 ReLU
-  int out_bf16;
-  int reduce_add;     // fp32 only: cp.reduce.async.bulk.add instead of a plain store (x += ...)
-  int N;
-};
-
-template <int BN, uint32_t kEpiBufs, int kParts>
-__device__ __forceinline__ void epilogue_tma_tile(const CUtensorMap* tmO, const EpiArgs& p, uint32_t taddr, uint8_t* buf0,
-                                                  uint32_t& epi_groups, int part, int lane, int col_tile0, int row_base,
-                                                  int batch_idx) {
-  // kParts warps share one TMEM lane quarter and take every kParts-th column group.  32 accumulator columns are in
-  // registers at a time (the kernel runs 18 warps: 112 registers per thread).
-  if (p.out_bf16) {
-#pragma unroll 1
-    for (int c = part; c < BN / 64; c += kParts) {
-      const int col0 = col_tile0 + c * 64;
-      if (col0 >= p.N) break;
-      uint8_t* buf = buf0 + (epi_groups & (kEpiBufs - 1u)) * 4096;
-      if (lane == 0) tma_wait_group_read<kEpiBufs - 1>();  // the store that last read this staging tile is done
-      __syncwarp();
-#pragma unroll 1
-      for (int hh = 0; hh < 2; ++hh) {
-        uint32_t v[32];
-        tmem_ld32(taddr + c * 64 + hh * 32, v);
-        tmem_ld_wait();
-        const int cb = col0 + hh * 32;
-        float x[32];
-#pragma unroll
-        for (int j = 0; j < 32; ++j) x[j] = __uint_as_float(v[j]);
-        if (p.bias != nullptr && cb < p.N) {
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const float4 b4 = __ldg(reinterpret_cast<const float4*>(p.bias + cb) + j);
-            x[4 * j + 0] += b4.x; x[4 * j + 1] += b4.y; x[4 * j + 2] += b4.z; x[4 * j + 3] += b4.w;
-          }
-        }
-        if (p.act == 1) {
-#pragma unroll
-          for (int j = 0; j < 32; j += 8) gelu_erf_poly8(x + j);
-        } else if (p.act == 2) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) x[j] = fmaxf(x[j], 0.0f);
-        }
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          uint4 w;
-          w.x = pack_bf16x2(x[8 * j + 0], x[8 * j + 1]);
-          w.y = pack_bf16x2(x[8 * j + 2], x[8 * j + 3]);
-          w.z = pack_bf16x2(x[8 * j + 4], x[8 * j + 5]);
-          w.w = pack_bf16x2(x[8 * j + 6], x[8 * j + 7]);
-          *reinterpret_cast<uint4*>(buf + sw128_offset(lane, hh * 4 + j)) = w;
-        }
-      }
-      fence_proxy_async_smem();
-      __syncwarp();
-      if (lane == 0) {
-        tma_store_3d(buf, tmO, col0, row_base, batch_idx);
-        tma_commit_group();
-      }
-      ++epi_groups;
-    }
-  } else {
-#pragma unroll 1
-    for (int c = part; c < BN / 32; c += kParts) {
-      const int col0 = col_tile0 + c * 32;
-      if (col0 >= p.N) break;
-      uint32_t v[32];
-      tmem_ld32(taddr + c * 32, v);
-      uint8_t* buf = buf0 + (epi_groups & (kEpiBufs - 1u)) * 4096;
-      if (lane == 0) tma_wait_group_read<kEpiBufs - 1>();
-      __syncwarp();
-      tmem_ld_wait();
-      float x[32];
-#pragma unroll
-      for (int j = 0; j < 32; ++j) x[j] = __uint_as_float(v[j]);
-      if (p.bias != nullptr) {  // (callers only route N % 32 != 0 here without a bias: the store clips, a bias load would not)
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const float4 b4 = __ldg(reinterpret_cast<const float4*>(p.bias + col0) + j);
-          x[4 * j + 0] += b4.x; x[4 * j + 1] += b4.y; x[4 * j + 2] += b4.z; x[4 * j + 3] += b4.w;
-        }
-      }
-      if (p.act == 1) {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) x[j] = gelu_erf(x[j]);
-      } else if (p.act == 2) {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) x[j] = fmaxf(x[j], 0.0f);
-      }
-#pragma unroll
-      for (int j = 0; j < 8; ++j)
-        *reinterpret_cast<float4*>(buf + sw128_offset(lane, j)) =
-            make_float4(x[4 * j + 0], x[4 * j + 1], x[4 * j + 2], x[4 * j + 3]);
-      fence_proxy_async_smem();
-      __syncwarp();
-      if (lane == 0) {
-        if (p.reduce_add) tma_reduce_add_3d(buf, tmO, col0, row_base, batch_idx);
-        else tma_store_3d(buf, tmO, col0, row_base, batch_idx);
-        tma_commit_group();
-      }
-      ++epi_groups;
-    }
   }
 }
 

@@ -1,4 +1,4 @@
-// tcgen05 / TMA / TMEM GEMM for the STEGO hot path (sm_100a).
+// wgmma / TMA / mbarrier GEMM for the STEGO hot path (sm_90a).
 //
 //   out[M,N] = act(A[M,K] . B[N,K]^T + bias[N]) + residual[M,N]
 //
@@ -8,10 +8,11 @@
 //   * segmentation head (reference: src/modules.py:73-81 cluster1/cluster2 1x1 convs) forward,
 //     dgrad (B operand MN-major) and wgrad (both operands MN-major, split-K + fp32 atomics).
 //
-// Structure: persistent CTAs (one per SM), 320 threads:
-//   warp 0      TMA producer   (cp.async.bulk.tensor -> 128B-swizzled smem ring, mbarrier expect_tx)
-//   warp 1      MMA issuer     (one elected lane issues tcgen05.mma, accumulators in TMEM, 2 buffers)
-//   warps 2..9  epilogue       (tcgen05.ld TMEM->regs, bias/GELU/ReLU/residual, smem transpose, coalesced stores)
+// Structure: persistent CTAs (one per SM), 384 threads = three warpgroups:
+//   warpgroup 0     TMA producer (one thread: cp.async.bulk.tensor -> 128B-swizzled smem ring, mbarrier expect_tx)
+//   warpgroups 1,2  MMA + epilogue, rows 0..63 and 64..127 of the 128 x BN tile: wgmma with both operands in shared
+//                   memory, fp32 accumulators in registers (BN / 2 per thread), then bias / GELU / ReLU / residual and
+//                   the stores straight from the accumulator registers.
 // Operand tiles are 128 x 64 (A) and BN x 64 (B) bf16; accumulation fp32.
 #include <stdlib.h>
 
@@ -23,19 +24,7 @@ namespace stego {
 
 constexpr int GEMM_BM = 128;
 constexpr int GEMM_BK = 64;
-// warp 0 TMA, warp 1 MMA, then 8 epilogue warps (two per TMEM lane quarter).  16 epilogue warps (four per quarter)
-// were measured: the epilogue alone got 10-15 % faster but the whole kernel 8-12 % slower (qkv 55 -> 60 us, fc1 81 -> 91):
-// the extra warps compete with the TMA-fed mainloop for shared-memory bandwidth (profiles/r1_gemm_phases.md).
-__host__ __device__ constexpr int gemm_epi_warps(int BN) { return BN == 384 ? 8 : 8; }
-__host__ __device__ constexpr int gemm_threads(int BN) { return 64 + 32 * gemm_epi_warps(BN); }
-
-// Phase-isolation switches (profiles/gemm_phases.py) exist only in a -DSTEGO_DIAG build; the default build folds them
-// to constants (no getenv on the launch path, no diag branches in the kernel).
-#ifdef STEGO_DIAG
-#define GEMM_DIAG(p, bit) (((p).diag & (bit)) != 0)
-#else
-#define GEMM_DIAG(p, bit) false
-#endif
+constexpr int GEMM_THREADS = 384;
 
 struct GemmParams {
   int M, N, K;        // logical GEMM sizes; K is the reduction length
@@ -50,54 +39,123 @@ struct GemmParams {
   int ldr;
   int row_div;        // >0: patch-embed mode: out_row = r + r/row_div + 1, residual row = r % row_div + 1
   int atomic;         // 1: fp32 atomicAdd into out (split-K)
-  int vec_ok;         // host-verified 16-byte alignment of out/residual rows
-  int fast_epi;       // coalesced smem-transpose epilogue usable (aligned, N % 32 == 0 tiles, plain row mapping)
-  int tma_epi;        // 1: epilogue tiles leave through TMA stores; 2: TMA fp32 reduce-add (in-place residual)
+  int vec_ok;         // host-verified alignment for paired (8-byte fp32 / 4-byte bf16) accesses of out / residual / bias
   int batch;          // independent GEMMs of the same shape (third tensor-map dimension); 1 = plain GEMM
   long long out_bs;   // element stride between the outputs / residuals of consecutive batch entries
   long long res_bs;
-  int diag;           // -DSTEGO_DIAG builds only: STEGO_GEMM_DIAG bit flags for phase timing (results are garbage):
-                      // 1 skip the epilogue work, 2 skip the MMAs, 4 skip the TMA loads
 };
 
+// Epilogue of one warpgroup's 64 x BN accumulator, straight from the wgmma fragment: each thread holds rows
+// row_top and row_top + 8, and column pairs 8 c + 2 (lane % 4) + {0, 1}.
+template <int BN>
+__device__ __forceinline__ void gemm_epilogue(float (&acc)[BN / 2], const GemmParams& p, int row_top, int col_base,
+                                              int tb) {
+  void* const outp = p.out_bf16 ? static_cast<void*>(reinterpret_cast<bf16*>(p.out) + tb * p.out_bs)
+                                : static_cast<void*>(reinterpret_cast<float*>(p.out) + tb * p.out_bs);
+  const float* const resp = p.residual ? p.residual + tb * p.res_bs : nullptr;
+  if (p.bias != nullptr) {
+#pragma unroll
+    for (int c = 0; c < BN / 8; ++c) {
+      const int col = col_base + 8 * c;
+      float b0 = 0.f, b1 = 0.f;
+      if (col + 1 < p.N && p.vec_ok) {
+        const float2 b2 = __ldg(reinterpret_cast<const float2*>(p.bias + col));
+        b0 = b2.x; b1 = b2.y;
+      } else {
+        if (col < p.N) b0 = __ldg(p.bias + col);
+        if (col + 1 < p.N) b1 = __ldg(p.bias + col + 1);
+      }
+      acc[4 * c + 0] += b0; acc[4 * c + 1] += b1;
+      acc[4 * c + 2] += b0; acc[4 * c + 3] += b1;
+    }
+  }
+  if (p.act == 1) {
+    // bf16 outputs take the MUFU-free polynomial (error far below the bf16 rounding), fp32 outputs the A-S erf
+    if (p.out_bf16) {
+#pragma unroll
+      for (int j = 0; j < BN / 2; j += 8) gelu_erf_poly8(acc + j);
+    } else {
+#pragma unroll
+      for (int j = 0; j < BN / 2; ++j) acc[j] = gelu_erf(acc[j]);
+    }
+  } else if (p.act == 2) {
+#pragma unroll
+    for (int j = 0; j < BN / 2; ++j) acc[j] = fmaxf(acc[j], 0.0f);
+  }
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int row = row_top + 8 * h;
+    if (row >= p.M) continue;
+    int out_row = row, res_row = row;
+    if (p.row_div > 0) {
+      out_row = row + row / p.row_div + 1;
+      res_row = row % p.row_div + 1;
+    }
+    const size_t obase = static_cast<size_t>(out_row) * p.ldo;
+    const size_t rbase = static_cast<size_t>(res_row) * p.ldr;
+#pragma unroll
+    for (int c = 0; c < BN / 8; ++c) {
+      const int col = col_base + 8 * c;
+      if (col >= p.N) break;
+      const bool two = col + 1 < p.N;
+      float x0 = acc[4 * c + 2 * h], x1 = acc[4 * c + 2 * h + 1];
+      if (p.atomic) {
+        float* o = reinterpret_cast<float*>(outp) + obase + col;
+        atomicAdd(o, x0);
+        if (two) atomicAdd(o + 1, x1);
+        continue;
+      }
+      const bool vec = two && p.vec_ok;
+      if (resp != nullptr) {
+        if (vec) {
+          const float2 r = *reinterpret_cast<const float2*>(resp + rbase + col);
+          x0 += r.x; x1 += r.y;
+        } else {
+          x0 += resp[rbase + col];
+          if (two) x1 += resp[rbase + col + 1];
+        }
+      }
+      if (p.out_bf16) {
+        bf16* o = reinterpret_cast<bf16*>(outp) + obase + col;
+        if (vec) {
+          *reinterpret_cast<uint32_t*>(o) = pack_bf16x2(x0, x1);
+        } else {
+          o[0] = __float2bfloat16_rn(x0);
+          if (two) o[1] = __float2bfloat16_rn(x1);
+        }
+      } else {
+        float* o = reinterpret_cast<float*>(outp) + obase + col;
+        if (vec) {
+          *reinterpret_cast<float2*>(o) = make_float2(x0, x1);
+        } else {
+          o[0] = x0;
+          if (two) o[1] = x1;
+        }
+      }
+    }
+  }
+}
+
 template <int BN, int kStages, bool A_MN, bool B_MN>
-__global__ void __launch_bounds__(gemm_threads(BN), 1)
-gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                 const __grid_constant__ CUtensorMap tmO, GemmParams p) {
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, GemmParams p) {
   constexpr uint32_t A_BYTES = GEMM_BM * GEMM_BK * 2;  // 16 KB
   constexpr uint32_t B_BYTES = BN * GEMM_BK * 2;
   constexpr uint32_t STAGE_BYTES = A_BYTES + B_BYTES;
-  // BN = 128 / 256: two accumulator buffers (epilogue of tile i overlaps the MMAs of tile i+1).
-  // BN = 384 (a whole E = 384 row block per CTA: A is read ONCE instead of three times): one 384-column
-  // accumulator (TMEM has 512 columns), two MMAs per k-step (N = 256 + 128), single epilogue staging tile.
-  static_assert(BN == 128 || BN == 192 || BN == 256 || BN == 384, "BN must be 128, 192, 256 or 384");
-  constexpr uint32_t kAccBufs = (BN == 384) ? 1u : 2u;
-  constexpr int kEpiWarps = gemm_epi_warps(BN);
-  constexpr int kParts = kEpiWarps / 4;      // warps sharing one TMEM lane quarter
-  constexpr uint32_t kEpiBufs = (BN == 384) ? 1u : 2u;  // staging tiles per epilogue warp
-  constexpr uint32_t TMEM_COLS = (BN == 128) ? 256u : 512u;
-  constexpr uint32_t N0 = (BN == 384) ? 256u : static_cast<uint32_t>(BN);  // first MMA of a k-step
-  constexpr uint32_t IDESC = make_idesc_bf16(GEMM_BM, N0, A_MN ? 1u : 0u, B_MN ? 1u : 0u);
-  constexpr uint32_t IDESC_TAIL = make_idesc_bf16(GEMM_BM, 128, A_MN ? 1u : 0u, B_MN ? 1u : 0u);
-  static_assert(BN != 384 || (!A_MN && !B_MN), "384-wide tiles are K-major only");
-  static_assert(BN != 192 || (!A_MN && !B_MN), "192-wide tiles are K-major only");
-  constexpr int kBBox = (BN % 128 == 0) ? 128 : 64;           // non-cluster K-major B box rows (192 = 3 x 64)
+  static_assert(BN == 128 || BN == 256, "BN must be 128 or 256");
+  static_assert(BN == 128 || (!A_MN && !B_MN), "256-wide tiles are K-major only");
+  constexpr int kBBox = 128;  // K-major B box rows
 
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  constexpr uint32_t EPI_BYTES = kEpiWarps * kEpiBufs * 4096;  // 32-row x 128-byte staging tiles per epilogue warp
-  uint8_t* epi_smem = smem + kStages * STAGE_BYTES;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kStages * STAGE_BYTES + EPI_BYTES);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kStages * STAGE_BYTES);
   uint64_t* empty_bar = full_bar + kStages;
-  uint64_t* tfull_bar = empty_bar + kStages;  // [2]
-  uint64_t* tempty_bar = tfull_bar + 2;       // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 2);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
+  const int wg = warp >> 2;  // 0 producer, 1..2 MMA warpgroups
 
-  const int tiles_m_real = (p.M + GEMM_BM - 1) / GEMM_BM;
-  const int tiles_m = tiles_m_real;
+  const int tiles_m = (p.M + GEMM_BM - 1) / GEMM_BM;
   const int tiles_n = (p.N + BN - 1) / BN;
   const int num_kb = (p.K + GEMM_BK - 1) / GEMM_BK;  // K tail: TMA zero-fills out-of-bounds
   const int tiles_per_batch = tiles_m * tiles_n * p.splits;
@@ -105,29 +163,21 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   const int sched_start = static_cast<int>(blockIdx.x);
   const int sched_step = static_cast<int>(gridDim.x);
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-    if (p.tma_epi) tma_prefetch_desc(&tmO);
     for (int s = 0; s < kStages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&tfull_bar[s], 1);
-      mbar_init(&tempty_bar[s], kEpiWarps);  // one arrive per epilogue warp
+      mbar_init(&empty_bar[s], 2);  // one arrive per MMA warpgroup
     }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<TMEM_COLS>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (wg == 0) {
     // ===================== TMA producer =====================
-    if (lane == 0 && !GEMM_DIAG(p, 4)) {
+    warpgroup_reg_dealloc<40>();
+    if (threadIdx.x == 0) {
       uint32_t stage = 0, phase = 0;
       for (int t = sched_start; t < total_tiles; t += sched_step) {
         const int tb = t / tiles_per_batch, tl = t % tiles_per_batch;
@@ -161,321 +211,57 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    // The WHOLE warp walks the pipeline (warp-uniform control flow keeps addresses / descriptors in uniform registers)
-    // and one elected lane issues the tcgen05 instructions.  Issuing from inside an `if (lane == 0)` region made the
-    // compiler rebuild every descriptor from per-thread registers behind an ELECT/R2UR loop: ~70 dependent
-    // instructions per k-step, which — not the tensor pipe, TMA or L2 — set the 0.65 us k-step time of every variant.
-    uint32_t stage = 0, phase = 0;
-    uint32_t acc = 0, acc_phase = 0;
-    const uint32_t tmem_u = __shfl_sync(0xffffffffu, tmem_base, 0);
-    constexpr uint32_t DESC_HI = smem_desc_hi_sw128(1024);
-    constexpr uint32_t A_KSTEP = A_MN ? (2048u >> 4) : (32u >> 4);  // low-word step per UMMA_K = 16
-    constexpr uint32_t B_KSTEP = B_MN ? (2048u >> 4) : (32u >> 4);
-    const uint32_t a_lo0 = smem_desc_lo(smem_u32(smem), A_MN ? 8192u : 16u);
-    const uint32_t b_lo0 = smem_desc_lo(smem_u32(smem) + A_BYTES, B_MN ? 8192u : 16u);
-    for (int t = sched_start; t < total_tiles; t += sched_step) {
-      const int split = (t % tiles_per_batch) % p.splits;
-      const int kb0 = split * p.kb_per_split;
-      const int kb1 = min(num_kb, kb0 + p.kb_per_split);
-      mbar_wait(&tempty_bar[acc], acc_phase ^ 1u);
-      tc_fence_after();
-      const uint32_t tmem_d = tmem_u + acc * (TMEM_COLS / kAccBufs);
-      for (int kb = kb0; kb < kb1; ++kb) {
-        if (!GEMM_DIAG(p, 4)) mbar_wait(&full_bar[stage], phase);
-        tc_fence_after();
-        const uint32_t a_lo = a_lo0 + stage * (STAGE_BYTES >> 4);
-        const uint32_t b_lo = b_lo0 + stage * (STAGE_BYTES >> 4);
-        if (elect_one()) {
-#pragma unroll
-          for (uint32_t k = 0; k < (GEMM_DIAG(p, 2) ? 0u : GEMM_BK / 16); ++k) {
-            const uint64_t da = smem_desc_join(a_lo + k * A_KSTEP, DESC_HI);
-            umma_bf16(tmem_d, da, smem_desc_join(b_lo + k * B_KSTEP, DESC_HI), IDESC, (kb > kb0 || k > 0) ? 1u : 0u);
-            if (BN == 384)  // columns 256..383 of the accumulator <- B rows 256..383
-              umma_bf16(tmem_d + 256, da, smem_desc_join(b_lo + ((256u * 128u) >> 4) + k * B_KSTEP, DESC_HI), IDESC_TAIL,
-                        (kb > kb0 || k > 0) ? 1u : 0u);
-          }
-          umma_commit(&empty_bar[stage]);  // smem slot reusable once these MMAs retire
-        }
-        __syncwarp();
-        if (++stage == kStages) { stage = 0; phase ^= 1u; }
-      }
-      if (elect_one()) umma_commit(&tfull_bar[acc]);  // accumulator complete -> epilogue
-      __syncwarp();
-      if (++acc == kAccBufs) { acc = 0; acc_phase ^= 1u; }
-    }
   } else {
-    // ===================== epilogue warps (2..9) =====================
-    const int quarter = warp & 3;        // TMEM lane quarter this warp may read
-    const int half = (warp - 2) >> 2;    // the kParts warps of a quarter take alternate column groups
-    uint32_t acc = 0, acc_phase = 0;
-    uint32_t epi_groups = 0;  // bulk-store groups this warp has committed (selects the staging tile)
+    // ===================== MMA warpgroups =====================
+    warpgroup_reg_alloc<232>();
+    const int mwg = wg - 1;  // rows 64 * mwg .. of every tile
+    // K-major A: rows 64.. start 64 x 128 B further; MN-major A: the second 64-wide M block, also 8 KB further
+    constexpr uint32_t DESC_HI = smem_desc_hi_sw128(1024);
+    constexpr uint32_t A_KSTEP = A_MN ? (2048u >> 4) : (32u >> 4);  // low-word step per k16 slice
+    constexpr uint32_t B_KSTEP = B_MN ? (2048u >> 4) : (32u >> 4);
+    const uint32_t a_lo0 = smem_desc_lo(smem_u32(smem) + mwg * 8192u, 8192u);
+    const uint32_t b_lo0 = smem_desc_lo(smem_u32(smem) + A_BYTES, 8192u);
+    const bool leader = (threadIdx.x & 127) == 0;
+    uint32_t stage = 0, phase = 0;
+    float acc[BN / 2];
     for (int t = sched_start; t < total_tiles; t += sched_step) {
       const int tb = t / tiles_per_batch, tl = t % tiles_per_batch;
+      const int split = tl % p.splits;
       const int tn = (tl / p.splits) % tiles_n;
       const int tm = tl / (p.splits * tiles_n);
-      // batch entry of this tile: outputs / residuals of consecutive entries are out_bs / res_bs elements apart
-      void* const outp = p.out_bf16 ? static_cast<void*>(reinterpret_cast<bf16*>(p.out) + tb * p.out_bs)
-                                    : static_cast<void*>(reinterpret_cast<float*>(p.out) + tb * p.out_bs);
-      const float* const resp = p.residual ? p.residual + tb * p.res_bs : nullptr;
-      if (p.fast_epi && !p.tma_epi && resp != nullptr) {
-        // pull this warp's slice of the residual tile towards L2 while the MMAs of the tile are still running
-        const int prow = tm * GEMM_BM + quarter * 32 + lane;
-        if (prow < p.M) {
-          for (int c = half; c < BN / 32; c += kParts) {
-            const int pc = tn * BN + c * 32;
-            if (pc < p.N)
-              asm volatile("prefetch.global.L2 [%0];\n" ::"l"(resp + static_cast<size_t>(prow) * p.ldr + pc));
-          }
-        }
+      const int kb0 = split * p.kb_per_split;
+      const int kb1 = min(num_kb, kb0 + p.kb_per_split);
+#pragma unroll
+      for (int j = 0; j < BN / 2; ++j) acc[j] = 0.f;
+      uint32_t prev_stage = 0;
+      for (int kb = kb0; kb < kb1; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t a_lo = a_lo0 + stage * (STAGE_BYTES >> 4);
+        const uint32_t b_lo = b_lo0 + stage * (STAGE_BYTES >> 4);
+        fence_operands(acc);
+        wgmma_fence();
+#pragma unroll
+        for (uint32_t k = 0; k < GEMM_BK / 16; ++k)
+          wgmma_ss<BN, A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, smem_desc_join(a_lo + k * A_KSTEP, DESC_HI),
+                                                  smem_desc_join(b_lo + k * B_KSTEP, DESC_HI), 1u);
+        wgmma_commit();
+        wgmma_wait<1>();  // the previous k-block's MMAs have retired: its smem slot is reusable
+        if (kb > kb0 && leader) mbar_arrive(&empty_bar[prev_stage]);
+        prev_stage = stage;
+        if (++stage == kStages) { stage = 0; phase ^= 1u; }
       }
-      mbar_wait(&tfull_bar[acc], acc_phase);
-      tc_fence_after();
-      if (GEMM_DIAG(p, 1)) {
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&tempty_bar[acc]);
-        if (++acc == kAccBufs) { acc = 0; acc_phase ^= 1u; }
-        continue;
-      }
-      const int row = tm * GEMM_BM + quarter * 32 + lane;
-      const bool row_ok = row < p.M;
-      int out_row = row, res_row = row;
-      if (p.row_div > 0) {
-        out_row = row + row / p.row_div + 1;
-        res_row = row % p.row_div + 1;
-      }
-      const uint32_t taddr = tmem_base + acc * (TMEM_COLS / kAccBufs) + (static_cast<uint32_t>(quarter * 32) << 16);
-      if (p.tma_epi) {
-        // ---- TMA epilogue: TMEM -> regs (bias/act) -> swizzled smem staging tile -> ONE bulk tensor store (or fp32
-        //      reduce-add for the in-place residual update x += ...) per 32 x 128-byte tile.  No global load/store
-        //      instructions, edges clipped by the tensor map (epilogue.cuh).
-        EpiArgs ea;
-        ea.bias = p.bias; ea.act = p.act; ea.out_bf16 = p.out_bf16; ea.reduce_add = (p.tma_epi == 2); ea.N = p.N;
-        epilogue_tma_tile<BN, kEpiBufs, kParts>(&tmO, ea, taddr, epi_smem + (warp - 2) * (kEpiBufs * 4096), epi_groups, half,
-                                                lane, tn * BN, tm * GEMM_BM + quarter * 32, tb);
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&tempty_bar[acc]);
-        if (++acc == kAccBufs) { acc = 0; acc_phase ^= 1u; }
-        continue;
-      }
-      if (p.fast_epi) {
-        // ---- coalesced epilogue: TMEM -> regs (bias/act) -> per-warp swizzled smem transpose -> 128-byte row
-        //      segments: every global load/store instruction covers 4 full rows x 128 B.
-        uint8_t* buf = epi_smem + (warp - 2) * 4096;
-        const int row_base = tm * GEMM_BM + quarter * 32;
-        const int rsub = lane >> 3, chunk = lane & 7;
-        if (p.out_bf16) {
-#pragma unroll 1
-          for (int c = half; c < BN / 64; c += kParts) {
-            const int col0 = tn * BN + c * 64;
-            if (col0 >= p.N) break;
-            uint32_t v0[32], v1[32];
-            tmem_ld32(taddr + c * 64, v0);
-            tmem_ld32(taddr + c * 64 + 32, v1);
-            tmem_ld_wait();
-#pragma unroll
-            for (int hh = 0; hh < 2; ++hh) {
-              uint32_t* v = hh ? v1 : v0;
-              const int cb = col0 + hh * 32;
-              float x[32];
-#pragma unroll
-              for (int j = 0; j < 32; ++j) x[j] = __uint_as_float(v[j]);
-              if (p.bias != nullptr && cb < p.N) {
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                  const float4 b4 = __ldg(reinterpret_cast<const float4*>(p.bias + cb) + j);
-                  x[4 * j + 0] += b4.x; x[4 * j + 1] += b4.y; x[4 * j + 2] += b4.z; x[4 * j + 3] += b4.w;
-                }
-              }
-              if (p.act == 1) {
-#pragma unroll
-                for (int j = 0; j < 32; j += 8) gelu_erf_poly8(x + j);
-              } else if (p.act == 2) {
-#pragma unroll
-                for (int j = 0; j < 32; ++j) x[j] = fmaxf(x[j], 0.0f);
-              }
-#pragma unroll
-              for (int j = 0; j < 4; ++j) {
-                uint4 w;
-                w.x = pack_bf16x2(x[8 * j + 0], x[8 * j + 1]);
-                w.y = pack_bf16x2(x[8 * j + 2], x[8 * j + 3]);
-                w.z = pack_bf16x2(x[8 * j + 4], x[8 * j + 5]);
-                w.w = pack_bf16x2(x[8 * j + 6], x[8 * j + 7]);
-                *reinterpret_cast<uint4*>(buf + sw128_offset(lane, hh * 4 + j)) = w;
-              }
-            }
-            __syncwarp();
-            const int col = col0 + chunk * 8;
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              const int r = i * 4 + rsub;
-              const int grow = row_base + r;
-              if (grow < p.M && col < p.N) {
-                const uint4 w = *reinterpret_cast<const uint4*>(buf + sw128_offset(r, chunk));
-                *reinterpret_cast<uint4*>(reinterpret_cast<bf16*>(outp) + static_cast<size_t>(grow) * p.ldo + col) = w;
-              }
-            }
-            __syncwarp();
-          }
-        } else {
-#pragma unroll 1
-          for (int c = half; c < BN / 32; c += kParts) {
-            const int col0 = tn * BN + c * 32;
-            if (col0 >= p.N) break;
-            const int col = col0 + chunk * 4;
-            // all residual loads first (out may alias residual: the compiler cannot hoist loads over the stores,
-            // so issuing them together is what keeps 8 x 512 B per warp in flight instead of one)
-            float4 rr[8];
-            if (resp != nullptr) {
-#pragma unroll
-              for (int i = 0; i < 8; ++i) {
-                const int grow = row_base + i * 4 + rsub;
-                rr[i] = (grow < p.M && col < p.N)
-                            ? *reinterpret_cast<const float4*>(resp + static_cast<size_t>(grow) * p.ldr + col)
-                            : make_float4(0.f, 0.f, 0.f, 0.f);
-              }
-            } else {
-#pragma unroll
-              for (int i = 0; i < 8; ++i) rr[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-            }
-            uint32_t v[32];
-            tmem_ld32(taddr + c * 32, v);
-            tmem_ld_wait();
-            float x[32];
-#pragma unroll
-            for (int j = 0; j < 32; ++j) x[j] = __uint_as_float(v[j]);
-            if (p.bias != nullptr) {
-#pragma unroll
-              for (int j = 0; j < 8; ++j) {
-                const float4 b4 = __ldg(reinterpret_cast<const float4*>(p.bias + col0) + j);
-                x[4 * j + 0] += b4.x; x[4 * j + 1] += b4.y; x[4 * j + 2] += b4.z; x[4 * j + 3] += b4.w;
-              }
-            }
-            if (p.act == 1) {
-#pragma unroll
-              for (int j = 0; j < 32; ++j) x[j] = gelu_erf(x[j]);
-            } else if (p.act == 2) {
-#pragma unroll
-              for (int j = 0; j < 32; ++j) x[j] = fmaxf(x[j], 0.0f);
-            }
-#pragma unroll
-            for (int j = 0; j < 8; ++j)
-              *reinterpret_cast<float4*>(buf + sw128_offset(lane, j)) =
-                  make_float4(x[4 * j + 0], x[4 * j + 1], x[4 * j + 2], x[4 * j + 3]);
-            __syncwarp();
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              const int r = i * 4 + rsub;
-              const int grow = row_base + r;
-              if (grow < p.M && col < p.N) {
-                float4 y = *reinterpret_cast<const float4*>(buf + sw128_offset(r, chunk));
-                y.x += rr[i].x; y.y += rr[i].y; y.z += rr[i].z; y.w += rr[i].w;
-                *reinterpret_cast<float4*>(reinterpret_cast<float*>(outp) + static_cast<size_t>(grow) * p.ldo + col) = y;
-              }
-            }
-            __syncwarp();
-          }
-        }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&tempty_bar[acc]);
-        if (++acc == kAccBufs) { acc = 0; acc_phase ^= 1u; }
-        continue;
-      }
-#pragma unroll 1
-      for (int c = half; c < BN / 32; c += kParts) {
-        const int col0 = tn * BN + c * 32;
-        if (col0 >= p.N) break;  // warp-uniform
-        uint32_t v[32];
-        __syncwarp();  // tcgen05.ld is .sync.aligned: reconverge lanes that skipped the previous store
-        tmem_ld32(taddr + c * 32, v);
-        tmem_ld_wait();
-        if (!row_ok) continue;
-        float x[32];
-#pragma unroll
-        for (int j = 0; j < 32; ++j) x[j] = __uint_as_float(v[j]);
-        const bool full = (col0 + 32 <= p.N);
-        if (p.bias != nullptr) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j)
-            if (full || col0 + j < p.N) x[j] += __ldg(p.bias + col0 + j);
-        }
-        if (p.act == 1) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) x[j] = gelu_erf(x[j]);
-        } else if (p.act == 2) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) x[j] = fmaxf(x[j], 0.0f);
-        }
-        if (p.atomic) {
-          float* o = reinterpret_cast<float*>(outp) + static_cast<size_t>(out_row) * p.ldo + col0;
-#pragma unroll
-          for (int j = 0; j < 32; ++j)
-            if (full || col0 + j < p.N) atomicAdd(o + j, x[j]);
-          continue;
-        }
-        if (full && p.vec_ok) {
-          if (resp != nullptr) {
-            const float4* r4 = reinterpret_cast<const float4*>(resp + static_cast<size_t>(res_row) * p.ldr + col0);
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              const float4 r = r4[j];
-              x[4 * j + 0] += r.x; x[4 * j + 1] += r.y; x[4 * j + 2] += r.z; x[4 * j + 3] += r.w;
-            }
-          }
-          if (p.out_bf16) {
-            uint4* o = reinterpret_cast<uint4*>(reinterpret_cast<bf16*>(outp) + static_cast<size_t>(out_row) * p.ldo + col0);
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              uint4 w;
-              w.x = pack_bf16x2(x[8 * j + 0], x[8 * j + 1]);
-              w.y = pack_bf16x2(x[8 * j + 2], x[8 * j + 3]);
-              w.z = pack_bf16x2(x[8 * j + 4], x[8 * j + 5]);
-              w.w = pack_bf16x2(x[8 * j + 6], x[8 * j + 7]);
-              o[j] = w;
-            }
-          } else {
-            float4* o = reinterpret_cast<float4*>(reinterpret_cast<float*>(outp) + static_cast<size_t>(out_row) * p.ldo + col0);
-#pragma unroll
-            for (int j = 0; j < 8; ++j) o[j] = make_float4(x[4 * j + 0], x[4 * j + 1], x[4 * j + 2], x[4 * j + 3]);
-          }
-        } else {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            if (col0 + j < p.N) {
-              float y = x[j];
-              if (resp != nullptr) y += resp[static_cast<size_t>(res_row) * p.ldr + col0 + j];
-              if (p.out_bf16)
-                reinterpret_cast<bf16*>(outp)[static_cast<size_t>(out_row) * p.ldo + col0 + j] = __float2bfloat16_rn(y);
-              else
-                reinterpret_cast<float*>(outp)[static_cast<size_t>(out_row) * p.ldo + col0 + j] = y;
-            }
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty_bar[acc]);
-      if (++acc == kAccBufs) { acc = 0; acc_phase ^= 1u; }
+      wgmma_wait<0>();
+      fence_operands(acc);
+      if (kb1 > kb0 && leader) mbar_arrive(&empty_bar[prev_stage]);
+      const int wq = (threadIdx.x >> 5) & 3;
+      gemm_epilogue<BN>(acc, p, tm * GEMM_BM + mwg * 64 + wq * 16 + (lane >> 2), tn * BN + 2 * (lane & 3), tb);
     }
-  }
-
-  if (p.tma_epi && warp >= 2 && lane == 0) tma_wait_group_read<0>();  // staging smem must outlive the bulk stores
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<TMEM_COLS>(tmem_base);
   }
 }
 
 template <int BN, int kStages, bool A_MN, bool B_MN>
-static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmO, const GemmParams& p,
-                       cudaStream_t stream) {
-  constexpr size_t smem = size_t(kStages) * (GEMM_BM * GEMM_BK * 2 + BN * GEMM_BK * 2) + gemm_epi_warps(BN) * (BN == 384 ? 1 : 2) * 4096 + 1024 + 256;
+static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, cudaStream_t stream) {
+  constexpr size_t smem = size_t(kStages) * (GEMM_BM * GEMM_BK * 2 + BN * GEMM_BK * 2) + 1024 + 256;
   static_assert(smem <= 232448, "exceeds the 227 KB of shared memory a CTA can opt into");
   auto kern = gemm_bf16_kernel<BN, kStages, A_MN, B_MN>;
   static bool configured = false;
@@ -488,7 +274,7 @@ static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUt
   const int tiles_n = (p.N + BN - 1) / BN;
   const int tiles = tiles_m * tiles_n * p.splits * p.batch;
   const int grid = tiles < num_sms() ? tiles : num_sms();
-  kern<<<grid, gemm_threads(BN), smem, stream>>>(tmA, tmB, tmO, p);
+  kern<<<grid, GEMM_THREADS, smem, stream>>>(tmA, tmB, p);
   STEGO_CHECK_LAUNCH("gemm_bf16_kernel launch");
   return STEGO_OK;
 }
@@ -533,43 +319,15 @@ static int gemm_impl(const void* A, int lda, long long a_bs, int a_mn_major, con
   p.row_div = row_div; p.atomic = atomic_out;
   p.batch = batch; p.out_bs = out_bs; p.res_bs = res_bs;
   const size_t esz = out_bf16 ? 2 : 4;
-  p.vec_ok = ((reinterpret_cast<uintptr_t>(out) & 15u) == 0) && ((size_t(ldo) * esz) % 16 == 0) &&
-             (residual == nullptr || (((reinterpret_cast<uintptr_t>(residual) & 15u) == 0) && (size_t(ldr) * 4) % 16 == 0));
+  const size_t pair = 2 * esz;  // paired accesses: two consecutive elements
+  p.vec_ok = ((reinterpret_cast<uintptr_t>(out) % pair) == 0) && (ldo % 2 == 0) && (out_bs % 2 == 0) &&
+             (residual == nullptr || ((reinterpret_cast<uintptr_t>(residual) % 8) == 0 && ldr % 2 == 0 && res_bs % 2 == 0)) &&
+             (bias == nullptr || (reinterpret_cast<uintptr_t>(bias) % 8) == 0);
+  // Tile shape: 128 x 256 for wide-N K-major linears (qkv: N = 3E, fc1: N = 4E; halves the A re-reads from L2),
+  // 128 x 128 for everything else (incl. MN-major operands and split-K).
+  const bool wide = !a_mn_major && !b_mn_major && splits == 1 && N >= 1024;
 
-  // the coalesced epilogue handles whole 32-column (fp32) / 64-column (bf16) groups: N % 32 == 0, bias 16B-aligned
-  p.fast_epi = p.vec_ok && !atomic_out && row_div == 0 && (N % 32 == 0) &&
-               (bias == nullptr || (reinterpret_cast<uintptr_t>(bias) & 15u) == 0) &&
-               !(out_bf16 && residual != nullptr);
-  // TMA epilogue: plain store for outputs without a residual; fp32 reduce-add when the residual IS the output
-  // (the in-place x += ... of the transformer blocks) — then the epilogue issues no global loads at all.
-  // Without a bias the TMA store also covers N % 32 != 0 (the tensor map clips the last column group), which is what
-  // the dense correlation (N = h w = 784, 1600, 3136) needs.
-  const bool tma_ragged_ok = p.vec_ok && !atomic_out && row_div == 0 && bias == nullptr && residual == nullptr &&
-                             (out_bs * static_cast<long long>(esz)) % 16 == 0;
-  p.tma_epi = 0;
-  if ((p.fast_epi || tma_ragged_ok) && !b_mn_major && !a_mn_major && (out_bs * static_cast<long long>(esz)) % 16 == 0) {
-    if (residual == nullptr) p.tma_epi = 1;
-    else if (!out_bf16 && residual == out && ldr == ldo && res_bs == out_bs) p.tma_epi = 2;
-  }
-  p.diag = 0;
-#ifdef STEGO_DIAG
-  {
-    const char* e = getenv("STEGO_GEMM_DIAG");  // read every call: profiles/gemm_phases.py toggles it between timings
-    p.diag = e ? atoi(e) : 0;
-  }
-#endif
-  // Tile shape (the kernel launched below fixes the B box of the tensor map, so it is decided first):
-  //   128 x 256  wide-N linears (fc1: N >= 1024): halves the A re-reads from L2
-  //   128 x 192  N = 1152 (qkv): six exact tiles instead of 4.5 of 256; two accumulator buffers, 4 stages
-  //   128 x 384  N = 384 / 768 with K >= 1024 (fc2): each A row block is read once; single accumulator
-  //   128 x 128  everything else (incl. MN-major operands, split-K, non-TMA epilogues)
-  // The 192 / 384 kernels only exist with the TMA epilogue; anything else falls back to 128-wide tiles.
-  const bool k_major = !a_mn_major && !b_mn_major && splits == 1;
-  const bool use_192 = k_major && p.tma_epi && N == 1152;
-  const bool use_384 = k_major && p.tma_epi && !use_192 && N % 384 == 0 && N <= 768 && K >= 1024;
-  const bool wide = k_major && !use_192 && !use_384 && N >= 1024;
-
-  CUtensorMap tmA, tmB, tmO;
+  CUtensorMap tmA, tmB;
   int rc;
   {
     // K-major: tensor is [batch][M][K] (inner = K). MN-major: tensor is [batch][K][M] (inner = M).
@@ -581,25 +339,14 @@ static int gemm_impl(const void* A, int lda, long long a_bs, int a_mn_major, con
   {
     uint64_t dims[3] = {b_mn_major ? (uint64_t)N : (uint64_t)K, b_mn_major ? (uint64_t)K : (uint64_t)N, (uint64_t)batch};
     uint64_t str[2] = {(uint64_t)ldb * 2, (uint64_t)b_bs * 2};
-    uint32_t box[3] = {64, (b_mn_major || use_192) ? 64u : 128u, 1};  // rows per B box: must match the kernel's kBBox
+    uint32_t box[3] = {64, b_mn_major ? 64u : 128u, 1};  // rows per B box: must match the kernel's kBBox
     if ((rc = make_tmap_bf16(&tmB, B, 3, dims, str, box)) != STEGO_OK) return rc;
   }
-  if (p.tma_epi) {
-    uint64_t dims[3] = {(uint64_t)N, (uint64_t)M, (uint64_t)batch};
-    uint64_t str[2] = {(uint64_t)ldo * esz, (uint64_t)out_bs * esz};
-    uint32_t box[3] = {out_bf16 ? 64u : 32u, 32u, 1};
-    rc = out_bf16 ? make_tmap_bf16(&tmO, out, 3, dims, str, box) : make_tmap_f32(&tmO, out, 3, dims, str, box);
-    if (rc != STEGO_OK) return rc;
-  } else {
-    tmO = tmA;  // unused
-  }
-  if (use_192) return launch_gemm<192, 4, false, false>(tmA, tmB, tmO, p, stream);
-  if (use_384) return launch_gemm<384, 3, false, false>(tmA, tmB, tmO, p, stream);
-  if (wide) return launch_gemm<256, 3, false, false>(tmA, tmB, tmO, p, stream);
-  if (!a_mn_major && !b_mn_major) return launch_gemm<128, 5, false, false>(tmA, tmB, tmO, p, stream);
-  if (!a_mn_major && b_mn_major) return launch_gemm<128, 5, false, true>(tmA, tmB, tmO, p, stream);
-  if (a_mn_major && b_mn_major) return launch_gemm<128, 5, true, true>(tmA, tmB, tmO, p, stream);
-  return launch_gemm<128, 5, true, false>(tmA, tmB, tmO, p, stream);
+  if (wide) return launch_gemm<256, 4, false, false>(tmA, tmB, p, stream);
+  if (!a_mn_major && !b_mn_major) return launch_gemm<128, 6, false, false>(tmA, tmB, p, stream);
+  if (!a_mn_major && b_mn_major) return launch_gemm<128, 6, false, true>(tmA, tmB, p, stream);
+  if (a_mn_major && b_mn_major) return launch_gemm<128, 6, true, true>(tmA, tmB, p, stream);
+  return launch_gemm<128, 6, true, false>(tmA, tmB, p, stream);
 }
 
 // C-ABI: see include/stego_b200.h for the contract.

@@ -1,10 +1,10 @@
-// Elementwise / reduction helpers around the segmentation-head GEMMs (sm_100a, HBM-bound).
+// Elementwise / reduction helpers around the segmentation-head GEMMs (sm_90a, HBM-bound).
 //
 // Reference: src/modules.py:108-118 (DinoFeaturizer.forward tail):
 //     code = cluster1(dropout(f)) + cluster2(dropout(f));  return dropout(f), code
 // The three Dropout2d calls each draw an independent [B,C,1,1] Bernoulli noise; here one pass over the
 // frozen features applies all three masks (the reference re-reads the feature map three times).
-// The 1x1 convs themselves run on the tcgen05 GEMM (gemm.cu); this file supplies what sits between
+// The 1x1 convs themselves run on the wgmma GEMM (gemm.cu); this file supplies what sits between
 // GEMMs in forward and backward: mask application, fp32->bf16 operand packing, ReLU backward and the
 // bias-gradient column sums, and the fused Adam update (torch.optim.Adam semantics,
 // src/train_segmentation.py:373-383).

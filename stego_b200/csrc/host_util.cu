@@ -29,8 +29,8 @@ int num_sms() {
   static int cached = 0;
   if (cached == 0) {
     int dev = 0, n = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) return 148;
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) return 148;
+    if (cudaGetDevice(&dev) != cudaSuccess) return 132;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) return 132;
     cached = n;
   }
   return cached;
@@ -96,10 +96,6 @@ static int make_tmap(CUtensorMapDataType dtype, CUtensorMap* out, const void* ba
 int make_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims,
                    const uint64_t* strides_bytes, const uint32_t* box) {
   return make_tmap(CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, out, base, rank, dims, strides_bytes, box);
-}
-int make_tmap_f32(CUtensorMap* out, const void* base, int rank, const uint64_t* dims,
-                  const uint64_t* strides_bytes, const uint32_t* box) {
-  return make_tmap(CU_TENSOR_MAP_DATA_TYPE_FLOAT32, out, base, rank, dims, strides_bytes, box);
 }
 
 }  // namespace stego

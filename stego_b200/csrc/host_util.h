@@ -24,9 +24,6 @@ void count_launch();  // bumps the library-wide kernel launch counter (stego_lau
 //   dims[i], box[i]: element counts, innermost first; strides_bytes[i]: byte stride of dim i+1.
 int make_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims,
                    const uint64_t* strides_bytes, const uint32_t* box);
-// same for fp32 elements (epilogue TMA store / reduce-add of fp32 outputs)
-int make_tmap_f32(CUtensorMap* out, const void* base, int rank, const uint64_t* dims,
-                  const uint64_t* strides_bytes, const uint32_t* box);
 
 #define STEGO_CHECK_ARG(cond, ...)       \
   do {                                   \

@@ -4,28 +4,31 @@
 // Reference: src/precompute_knns.py:15-21 (get_feats: F.normalize(model(img).mean([2, 3]), dim=1)) and :83-96
 //     pairwise_sims = torch.einsum("nf,mf->nm", batch_feats, normed_feats);  all_nns.append(torch.topk(pairwise_sims, 30)[1])
 // The reference materialises an [n/16, n] fp32 similarity slab per batch on the host (n = 118 K for COCO: 3.5 GB per
-// slab, 14 G similarities in total).  Here the similarity tile never leaves the SM: S = F F^T accumulates in TMEM
-// (bf16 hi/lo split, three tcgen05 passes = ~2^-16 relative accuracy, enough to rank neighbours), and each epilogue
-// thread (= one TMEM lane = one query row) keeps its running top-k in a sorted private list, compared against a
-// register threshold (an insert happens ~k ln(n/k) times per row, everything else is one FSETP per similarity).
+// slab, 14 G similarities in total).  Here the similarity tile never leaves the SM: S = F F^T accumulates in registers
+// (bf16 hi/lo split, three wgmma passes = ~2^-16 relative accuracy, enough to rank neighbours), is staged transposed in
+// shared memory, and two scan threads per query row (one per half of the key tile) keep a running top-k in a sorted
+// private list, compared against a register threshold (an insert happens ~k ln(n/k) times per row, everything else
+// is one FSETP per similarity).  The two lists of a row are merged once per row block.
 //
 //   knn_prep_kernel   : fp32 [n][E] -> L2-normalise (eps 1e-12 like F.normalize) -> bf16 hi / lo planes [2][n][E]
-//   knn_topk_kernel   : persistent CTAs, one 128-row query block at a time against all 256-column key tiles
-//       warp 0      TMA producer (A = query rows, B = key rows, both from the same planes tensor, 4-stage ring)
-//       warp 1      MMA issuer (warp-uniform, elected lane): 3 passes (hi.hi, hi.lo, lo.hi) x E/64 k-blocks per tile,
-//                   two 256-column accumulators so the scan of tile t overlaps the MMAs of tile t+1
-//       warps 2..5  scan: tcgen05.ld 32 columns at a time, threshold test, sorted insert; after the last tile the
-//                   row's k indices (descending similarity, ties -> lower index first) are written as int64
+//   knn_topk_kernel   : persistent CTAs, one 128-row query block at a time against all 128-column key tiles
+//       warpgroups 0,1  wgmma for query rows 0..63 / 64..127: 3 passes (hi.hi, hi.lo, lo.hi) x E/64 k-blocks per tile,
+//                       then the scan of those rows; after the last tile the row's k indices (descending similarity,
+//                       ties -> lower index first) are written as int64
+//       warpgroup 2     TMA producer (A = query rows, B = key rows, both from the same planes tensor, 3-stage ring)
 #include "common.cuh"
 #include "host_util.h"
 
 namespace stego {
 
-constexpr int KNN_BM = 128, KNN_BN = 256, KNN_BK = 64, KNN_STAGES = 4, KNN_THREADS = 192, KNN_MAXK = 32;
+constexpr int KNN_BM = 128, KNN_BN = 128, KNN_BK = 64, KNN_STAGES = 3, KNN_THREADS = 384, KNN_MAXK = 32;
 constexpr uint32_t KNN_A_BYTES = KNN_BM * KNN_BK * 2;   // 16 KB
-constexpr uint32_t KNN_B_BYTES = KNN_BN * KNN_BK * 2;   // 32 KB
+constexpr uint32_t KNN_B_BYTES = KNN_BN * KNN_BK * 2;   // 16 KB
 constexpr uint32_t KNN_STAGE_BYTES = KNN_A_BYTES + KNN_B_BYTES;
-constexpr size_t KNN_SMEM = size_t(KNN_STAGES) * KNN_STAGE_BYTES + 1024 + 256;
+constexpr int KNN_ST_LD = KNN_BM + 4;                   // transposed score tile [key col][query row], padded
+constexpr uint32_t KNN_ST_BYTES = KNN_BN * KNN_ST_LD * 4;
+constexpr uint32_t KNN_MERGE_BYTES = KNN_BM * KNN_MAXK * 8;  // second-half lists: [row][k] value + index
+constexpr size_t KNN_SMEM = size_t(KNN_STAGES) * KNN_STAGE_BYTES + KNN_ST_BYTES + KNN_MERGE_BYTES + 1024 + 256;
 
 struct KnnParams {
   int n, E, k;
@@ -56,11 +59,11 @@ __global__ void __launch_bounds__(KNN_THREADS, 1)
 knn_topk_kernel(const __grid_constant__ CUtensorMap tmF, KnnParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + KNN_STAGES * KNN_STAGE_BYTES);
+  float* st = reinterpret_cast<float*>(smem + KNN_STAGES * KNN_STAGE_BYTES);
+  float* merge_v = reinterpret_cast<float*>(smem + KNN_STAGES * KNN_STAGE_BYTES + KNN_ST_BYTES);
+  int* merge_i = reinterpret_cast<int*>(merge_v + KNN_BM * KNN_MAXK);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + KNN_STAGES * KNN_STAGE_BYTES + KNN_ST_BYTES + KNN_MERGE_BYTES);
   uint64_t* empty_bar = full_bar + KNN_STAGES;
-  uint64_t* tfull_bar = empty_bar + KNN_STAGES;  // [2]
-  uint64_t* tempty_bar = tfull_bar + 2;          // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 2);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -69,27 +72,20 @@ knn_topk_kernel(const __grid_constant__ CUtensorMap tmF, KnnParams p) {
   const int nkb = p.E / KNN_BK;
   const int ksteps = 3 * nkb;  // pass 0: A hi x B hi, pass 1: A hi x B lo, pass 2: A lo x B hi
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmF);
     for (int s = 0; s < KNN_STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&tfull_bar[s], 1);
-      mbar_init(&tempty_bar[s], 4);
+      mbar_init(&empty_bar[s], 2);  // one arrive per MMA warpgroup
     }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<512>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp >= 8) {
     // ===================== TMA producer =====================
-    if (lane == 0) {
+    warpgroup_reg_dealloc<40>();
+    if (warp == 8 && lane == 0) {
       uint32_t stage = 0, phase = 0;
       for (int rb = blockIdx.x; rb < row_blocks; rb += gridDim.x) {
         for (int ct = 0; ct < col_tiles; ++ct) {
@@ -102,105 +98,114 @@ knn_topk_kernel(const __grid_constant__ CUtensorMap tmF, KnnParams p) {
             mbar_arrive_expect_tx(&full_bar[stage], KNN_STAGE_BYTES);
             tma_load_3d(sa, &tmF, &full_bar[stage], kb * KNN_BK, rb * KNN_BM, pa);
             tma_load_3d(sb, &tmF, &full_bar[stage], kb * KNN_BK, ct * KNN_BN, pb);
-            tma_load_3d(sb + 16384, &tmF, &full_bar[stage], kb * KNN_BK, ct * KNN_BN + 128, pb);
             if (++stage == KNN_STAGES) { stage = 0; phase ^= 1u; }
           }
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (whole warp, one elected lane) =====================
-    uint32_t stage = 0, phase = 0, acc = 0, acc_phase = 0;
-    const uint32_t tmem_u = __shfl_sync(0xffffffffu, tmem_base, 0);
-    constexpr uint32_t IDESC = make_idesc_bf16(KNN_BM, KNN_BN, 0, 0);
-    constexpr uint32_t DESC_HI = smem_desc_hi_sw128(1024);
-    const uint32_t a_lo0 = smem_desc_lo(smem_u32(smem), 16);
-    const uint32_t b_lo0 = smem_desc_lo(smem_u32(smem) + KNN_A_BYTES, 16);
-    for (int rb = blockIdx.x; rb < row_blocks; rb += gridDim.x) {
-      for (int ct = 0; ct < col_tiles; ++ct) {
-        mbar_wait(&tempty_bar[acc], acc_phase ^ 1u);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_u + acc * KNN_BN;
-        for (int ks = 0; ks < ksteps; ++ks) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t a_lo = a_lo0 + stage * (KNN_STAGE_BYTES >> 4);
-          const uint32_t b_lo = b_lo0 + stage * (KNN_STAGE_BYTES >> 4);
-          if (elect_one()) {
-#pragma unroll
-            for (uint32_t k = 0; k < KNN_BK / 16; ++k)
-              umma_bf16(tmem_d, smem_desc_join(a_lo + 2 * k, DESC_HI), smem_desc_join(b_lo + 2 * k, DESC_HI), IDESC,
-                        (ks > 0 || k > 0) ? 1u : 0u);
-            umma_commit(&empty_bar[stage]);
-          }
-          __syncwarp();
-          if (++stage == KNN_STAGES) { stage = 0; phase ^= 1u; }
-        }
-        if (elect_one()) umma_commit(&tfull_bar[acc]);
-        __syncwarp();
-        if (++acc == 2) { acc = 0; acc_phase ^= 1u; }
-      }
-    }
-  } else {
-    // ===================== scan warps (2..5): one query row per thread =====================
-    const int quarter = warp & 3;
-    const uint32_t lane_off = static_cast<uint32_t>(quarter * 32) << 16;
-    uint32_t acc = 0, acc_phase = 0;
-    const int k = p.k;
-    float tv[KNN_MAXK];  // sorted descending; dynamic indexing -> local memory (touched only on inserts)
-    int ti[KNN_MAXK];
-    for (int rb = blockIdx.x; rb < row_blocks; rb += gridDim.x) {
-      const int row = rb * KNN_BM + quarter * 32 + lane;
-#pragma unroll 1
-      for (int i = 0; i < KNN_MAXK; ++i) { tv[i] = -INFINITY; ti[i] = -1; }
-      float thr = -INFINITY;  // similarity of the current k-th neighbour
-      for (int ct = 0; ct < col_tiles; ++ct) {
-        mbar_wait(&tfull_bar[acc], acc_phase);
-        tc_fence_after();
-        const uint32_t taddr = tmem_base + acc * KNN_BN + lane_off;
-        const int col0 = ct * KNN_BN;
-#pragma unroll 1
-        for (int c = 0; c < KNN_BN / 32; ++c) {
-          if (col0 + c * 32 >= p.n) break;  // warp-uniform: key rows past n are zero-filled padding
-          uint32_t v[32];
-          tmem_ld32(taddr + c * 32, v);
-          tmem_ld_wait();
-#pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            const float s = __uint_as_float(v[j]);
-            const int col = col0 + c * 32 + j;
-            if (s > thr && col < p.n) {
-              int pos = k - 1;
-              while (pos > 0 && tv[pos - 1] < s) {  // strict: earlier (lower) columns stay ahead on ties
-                tv[pos] = tv[pos - 1];
-                ti[pos] = ti[pos - 1];
-                --pos;
-              }
-              tv[pos] = s;
-              ti[pos] = col;
-              thr = tv[k - 1];
-            }
-          }
-        }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&tempty_bar[acc]);
-        if (++acc == 2) { acc = 0; acc_phase ^= 1u; }
-      }
-      if (row < p.n) {
-        for (int i = 0; i < k; ++i) {
-          p.idx_out[static_cast<size_t>(row) * k + i] = ti[i];
-          if (p.val_out) p.val_out[static_cast<size_t>(row) * k + i] = tv[i];
-        }
-      }
-    }
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<512>(tmem_base);
+  // ===================== MMA + scan warpgroups =====================
+  warpgroup_reg_alloc<232>();
+  const int mwg = warp >> 2;
+  const int t128 = threadIdx.x & 127;
+  const bool leader = t128 == 0;
+  const int wq = warp & 3;
+  constexpr uint32_t DESC_HI = smem_desc_hi_sw128(1024);
+  const uint32_t a_lo0 = smem_desc_lo(smem_u32(smem) + mwg * (KNN_A_BYTES / 2), 16);
+  const uint32_t b_lo0 = smem_desc_lo(smem_u32(smem) + KNN_A_BYTES, 16);
+  // scan role: query row `srow` of the tile, key columns [64 half, 64 half + 64) of every key tile
+  const int srow = mwg * 64 + (t128 & 63);
+  const int half = t128 >> 6;
+  const int k = p.k;
+  uint32_t stage = 0, phase = 0;
+  float tv[KNN_MAXK];  // sorted descending; dynamic indexing -> local memory (touched only on inserts)
+  int ti[KNN_MAXK];
+  float acc[KNN_BN / 2];
+  for (int rb = blockIdx.x; rb < row_blocks; rb += gridDim.x) {
+#pragma unroll 1
+    for (int i = 0; i < KNN_MAXK; ++i) { tv[i] = -INFINITY; ti[i] = -1; }
+    float thr = -INFINITY;  // similarity of the current k-th neighbour
+    for (int ct = 0; ct < col_tiles; ++ct) {
+#pragma unroll
+      for (int j = 0; j < KNN_BN / 2; ++j) acc[j] = 0.f;
+      uint32_t prev = 0;
+      for (int ks = 0; ks < ksteps; ++ks) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t a_lo = a_lo0 + stage * (KNN_STAGE_BYTES >> 4);
+        const uint32_t b_lo = b_lo0 + stage * (KNN_STAGE_BYTES >> 4);
+        fence_operands(acc);
+        wgmma_fence();
+#pragma unroll
+        for (uint32_t kk = 0; kk < KNN_BK / 16; ++kk)
+          wgmma_ss<KNN_BN, 0, 0>(acc, smem_desc_join(a_lo + 2 * kk, DESC_HI), smem_desc_join(b_lo + 2 * kk, DESC_HI), 1u);
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (ks > 0 && leader) mbar_arrive(&empty_bar[prev]);
+        prev = stage;
+        if (++stage == KNN_STAGES) { stage = 0; phase ^= 1u; }
+      }
+      wgmma_wait<0>();
+      fence_operands(acc);
+      if (leader) mbar_arrive(&empty_bar[prev]);
+      // stage the tile transposed (bank-conflict-free both ways); this warpgroup's previous scan must be over
+      asm volatile("bar.sync %0, 128;\n" ::"r"(1 + mwg) : "memory");
+#pragma unroll
+      for (int t = 0; t < KNN_BN / 2; ++t) {
+        const int r = mwg * 64 + wq * 16 + (lane >> 2) + 8 * ((t >> 1) & 1);
+        const int col = 8 * (t >> 2) + 2 * (lane & 3) + (t & 1);
+        st[col * KNN_ST_LD + r] = acc[t];
+      }
+      asm volatile("bar.sync %0, 128;\n" ::"r"(1 + mwg) : "memory");
+      const int col0 = ct * KNN_BN + half * 64;
+#pragma unroll 1
+      for (int c = 0; c < 64; c += 32) {
+        if (col0 + c >= p.n) break;  // warp-uniform: key rows past n are zero-filled padding
+        float v[32];
+#pragma unroll
+        for (int j = 0; j < 32; ++j) v[j] = st[(half * 64 + c + j) * KNN_ST_LD + srow];
+#pragma unroll
+        for (int j = 0; j < 32; ++j) {
+          const float s = v[j];
+          const int col = col0 + c + j;
+          if (s > thr && col < p.n) {
+            int pos = k - 1;
+            while (pos > 0 && tv[pos - 1] < s) {  // strict: earlier (lower) columns stay ahead on ties
+              tv[pos] = tv[pos - 1];
+              ti[pos] = ti[pos - 1];
+              --pos;
+            }
+            tv[pos] = s;
+            ti[pos] = col;
+            thr = tv[k - 1];
+          }
+        }
+      }
+    }
+    // merge the two half lists of every row: (value desc, index asc), the order a single scan would produce
+    if (half == 1) {
+      for (int i = 0; i < k; ++i) {
+        merge_v[srow * KNN_MAXK + i] = tv[i];
+        merge_i[srow * KNN_MAXK + i] = ti[i];
+      }
+    }
+    asm volatile("bar.sync %0, 128;\n" ::"r"(1 + mwg) : "memory");
+    const int row = rb * KNN_BM + srow;
+    if (half == 0 && row < p.n) {
+      int ia = 0, ib = 0;
+      for (int i = 0; i < k; ++i) {
+        const float vb = merge_v[srow * KNN_MAXK + ib];
+        const int xb = merge_i[srow * KNN_MAXK + ib];
+        const bool take_a = tv[ia] > vb || (tv[ia] == vb && ti[ia] >= 0 && (xb < 0 || ti[ia] < xb));
+        const float v = take_a ? tv[ia] : vb;
+        const int x = take_a ? ti[ia] : xb;
+        if (take_a) ++ia; else ++ib;
+        p.idx_out[static_cast<size_t>(row) * k + i] = x;
+        if (p.val_out) p.val_out[static_cast<size_t>(row) * k + i] = v;
+      }
+    }
+    asm volatile("bar.sync %0, 128;\n" ::"r"(1 + mwg) : "memory");  // merge buffer free for the next row block
   }
 }
 
@@ -221,7 +226,7 @@ extern "C" int stego_knn_topk(const float* feats, int n, int E, int k, void* pla
   CUtensorMap tm;
   uint64_t dims[3] = {(uint64_t)E, (uint64_t)n, 2};
   uint64_t str[2] = {(uint64_t)E * 2, (uint64_t)n * E * 2};
-  uint32_t box[3] = {64, 128, 1};
+  uint32_t box[3] = {64, 128, 1};  // KNN_BM = KNN_BN = 128 rows
   int rc = make_tmap_bf16(&tm, planes_scratch, 3, dims, str, box);
   if (rc != STEGO_OK) return rc;
   static bool configured = false;

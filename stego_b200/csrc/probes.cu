@@ -1,4 +1,4 @@
-// Probe heads of the STEGO training / eval step (sm_100a; HBM-bound, fp32 arithmetic):
+// Probe heads of the STEGO training / eval step (sm_90a; HBM-bound, fp32 arithmetic):
 //
 //   ClusterLookup            src/modules.py:134-161   cosine similarity to n_classes centroids,
 //                                                     argmax one-hot / softmax(alpha.) / log_softmax(alpha.), loss

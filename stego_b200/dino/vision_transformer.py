@@ -1,8 +1,8 @@
-"""Frozen DINO ViT forward on B200: same constructor / parameter names / entry points as the reference
+"""Frozen DINO ViT forward on H100: same constructor / parameter names / entry points as the reference
 `src/dino/vision_transformer.py` (so DINO and STEGO checkpoints load unchanged), but the forward pass is
-a fixed sequence of hand-written sm_100a kernels called through the C-ABI:
+a fixed sequence of hand-written sm_90a kernels called through the C-ABI:
 
-    patchify -> tcgen05 GEMM (+bias +pos-embed, cls rows) ->
+    patchify -> wgmma GEMM (+bias +pos-embed, cls rows) ->
     12 x [ LayerNorm -> qkv GEMM -> fused attention -> proj GEMM (+residual, in place) ->
            LayerNorm -> fc1 GEMM (+GELU) -> fc2 GEMM (+residual, in place) ] -> LayerNorm
 
@@ -185,7 +185,7 @@ class VisionTransformer(nn.Module):
         """Returns (x, qkv_last): x = fp32 residual stream [B*N, E] after the last block (before the
         final norm); qkv_last = packed bf16 [B*N, 3E] of the last block if requested."""
         if not img.is_cuda:
-            raise RuntimeError("stego_b200: the DINO ViT forward only exists as sm_100a kernels (no CPU fallback)")
+            raise RuntimeError("stego_b200: the DINO ViT forward only exists as sm_90a kernels (no CPU fallback)")
         w = self._prepared()
         # bf16 images are taken as they are (patchify rounds fp32 images to bf16 anyway: same operand bits)
         img = (img if img.dtype == torch.bfloat16 else img.float()).contiguous()

@@ -231,8 +231,8 @@ class FusedStep:
         c1.bias.grad.copy_(ws.db_pad[:D])
 
         def splits_for(out_rows, out_cols):
-            # split-K so that tiles x splits fills ONE wave of the persistent GEMM (one CTA per SM): 3 x 49 = 147 and
-            # 9 x 16 = 144 CTAs on 148 SMs (64 splits made 192 / 297 CTAs = 2 and 3 rounds of a 148-CTA grid)
+            # split-K so that tiles x splits fills ONE wave of the persistent GEMM (one CTA per SM): at most num_sms
+            # CTAs (more splits would make a second round of the grid)
             tiles = ((out_rows + 127) // 128) * ((out_cols + 127) // 128)
             return max(1, min(M // 512, ws.num_sms // tiles))
         ops.gemm(ws.dyb, ws.x1, c1.weight.grad.view(D, E), M=D, N=E, K=M, a_mn=True, b_mn=True,

@@ -1,9 +1,9 @@
 """Drop-in for the reference `src/modules.py` (mhamilton723/STEGO): same public names, constructor
 arguments, forward signatures, parameter names and return tuples — with the hot path running on
-hand-written sm_100a kernels through libstego_b200.so (include/stego_b200.h).
+hand-written sm_90a kernels through libstego_b200.so (include/stego_b200.h).
 
 Hot path (CUDA kernels, no CPU / eager fallback):
-    DinoFeaturizer               modules.py:17-118    frozen DINO ViT + 1x1-conv head (tcgen05 GEMMs, fused attention)
+    DinoFeaturizer               modules.py:17-118    frozen DINO ViT + 1x1-conv head (wgmma GEMMs, fused attention)
     ContrastiveCorrelationLoss   modules.py:314-398   fused sample/norm/einsum/loss + backward
     ClusterLookup                modules.py:134-161   fused cosine-sim / argmax / softmax probe
     norm, tensor_correlation, sample, super_perm  modules.py:275-295
@@ -54,7 +54,7 @@ def average_norm(t):
 
 def tensor_correlation(a, b):
     """modules.py:283-284: einsum nchw,ncij->nhwij — one [hw, C] x [C, ij] GEMM per image, all images in ONE launch of
-    the batched tcgen05 GEMM.  fp32 inputs are split into bf16 hi + lo parts and the three significant products are
+    the batched wgmma GEMM.  fp32 inputs are split into bf16 hi + lo parts and the three significant products are
     folded into the K axis: [hi | lo | hi] . [hi | hi | lo]^T = hi.hi + lo.hi + hi.lo (fp32 accumulate, ~2^-16
     relative instead of bf16's 2^-9); bf16 inputs take a single pass.  Off-device there is no implementation."""
     if not (a.is_cuda and b.is_cuda):
@@ -80,7 +80,7 @@ def tensor_correlation(a, b):
 
     A = operand(a, h * w, ("hi", "lo", "hi"))
     Bm = operand(b, i * j, ("hi", "hi", "lo"))
-    ld = _round_up(i * j, 4)  # 16-byte rows for the TMA store of the fp32 result
+    ld = _round_up(i * j, 4)  # 16-byte rows: the GEMM epilogue stores fp32 pairs
     out = torch.empty(n, h * w, ld, dtype=torch.float32, device=a.device)
     ops.gemm_batched(A, Bm, out[:, :, :i * j])
     return out[:, :, :i * j].reshape(n, h, w, i, j) if ld == i * j else out[:, :, :i * j].contiguous().reshape(n, h, w, i, j)
@@ -125,7 +125,7 @@ class LambdaLayer(nn.Module):
 
 
 # ==================================================================================================
-# segmentation head (cluster1 + cluster2) as one autograd node over tcgen05 GEMMs
+# segmentation head (cluster1 + cluster2) as one autograd node over wgmma GEMMs
 # ==================================================================================================
 class _HeadFn(torch.autograd.Function):
     """code = conv1x1(E->D)(f*m1) + conv1x1(E->D)(relu(conv1x1(E->E)(f*m2)))   (modules.py:108-111)

@@ -19,7 +19,7 @@ def gemm(a: torch.Tensor, b: torch.Tensor, out: torch.Tensor, *, M: int, N: int,
          a_mn: bool = False, b_mn: bool = False, bias: Optional[torch.Tensor] = None, act: int = ACT_NONE,
          residual: Optional[torch.Tensor] = None, row_div: int = 0, splits: int = 1,
          atomic: bool = False) -> torch.Tensor:
-    """out[M,N] = act(A.B^T + bias) + residual on tcgen05 (see include/stego_b200.h: stego_gemm_bf16)."""
+    """out[M,N] = act(A.B^T + bias) + residual on wgmma (see include/stego_b200.h: stego_gemm_bf16)."""
     _lib.require_cuda(a, b, out, bias, residual)
     assert a.dtype == torch.bfloat16 and b.dtype == torch.bfloat16
     assert a.dim() == 2 and b.dim() == 2 and out.dim() == 2
@@ -87,7 +87,7 @@ def layernorm(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, out: tor
 
 
 def attention(qkv: torch.Tensor, out: torch.Tensor, B: int, N: int, E: int, heads: int) -> torch.Tensor:
-    """Fused softmax(q k^T / 8) v on tcgen05 (stego_attention_fwd). qkv [B*N, 3E] bf16, out [B*N, E] bf16."""
+    """Fused softmax(q k^T / 8) v on wgmma (stego_attention_fwd). qkv [B*N, 3E] bf16, out [B*N, E] bf16."""
     _lib.require_cuda(qkv, out)
     assert qkv.dtype == torch.bfloat16 and qkv.is_contiguous() and out.dtype == torch.bfloat16 and out.is_contiguous()
     _lib.check(_lib.load().stego_attention_fwd(_lib.ptr(qkv), _lib.ptr(out), B, N, E, heads, _lib.stream()),

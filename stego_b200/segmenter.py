@@ -1,5 +1,5 @@
 """`LitUnsupervisedSegmenter` — the training-step orchestration of the reference
-(src/train_segmentation.py:53-383) re-hosted on the fused sm_100a path, without a Lightning dependency.
+(src/train_segmentation.py:53-383) re-hosted on the fused sm_90a path, without a Lightning dependency.
 
 Same constructor `(n_classes, cfg)`, attribute names (`net`, `linear_probe`, `cluster_probe`,
 `train_cluster_probe`, `decoder`, `contrastive_corr_loss_fn`, ...), `forward`, `training_step(batch,

@@ -1,7 +1,7 @@
 """Shared helpers of the GPU parity tests: the oracle stepping the same trainable parameters as the CUDA path.
 
 The oracle (oracle/stego_oracle.py) is plain torch and device-agnostic: `odev="cuda"` runs the very same functions in
-fp32 on the GPU with TF32 disabled (cuBLAS / cuDNN fp32 kernels — "the reference PyTorch path" on the B200), which makes
+fp32 on the GPU with TF32 disabled (cuBLAS / cuDNN fp32 kernels — "the reference PyTorch path" on the GPU), which makes
 the BASELINE.json full-size configurations a seconds-long check; `odev="cpu"` is the CPU oracle.
 """
 import json
@@ -142,8 +142,10 @@ def oracle_vit_feats(sd, imgs, arch, odev, chunk=8):
 
 
 def record(name, payload):
-    """Keep a machine-readable copy of what a parity test measured (gpurun_out/ comes back from the GPU box)."""
-    d = os.path.join(ROOT, "gpurun_out")
+    """Keep a machine-readable copy of what a parity test measured, in $STEGO_PARITY_DIR when that is set."""
+    d = os.environ.get("STEGO_PARITY_DIR")
+    if not d:
+        return
     os.makedirs(d, exist_ok=True)
     with open(os.path.join(d, f"parity_{name}.json"), "w") as fh:
         json.dump(payload, fh, indent=1, sort_keys=True)

@@ -1,4 +1,4 @@
-"""Fused correspondence loss (sample+norm tiles, tcgen05 einsum, loss reduction, backward) vs the oracle.
+"""Fused correspondence loss (sample+norm tiles, wgmma einsum, loss reduction, backward) vs the oracle.
 
 Tolerances: the CUDA path computes the einsum as a bf16 hi/lo split (~2^-16 relative) with fp32
 accumulation, so losses / cd / gradients are compared at 1e-4 relative (well inside the 1e-3 bar of

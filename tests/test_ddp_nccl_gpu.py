@@ -1,6 +1,6 @@
 """2-GPU run of the data-parallel CUDA training step against shard-and-average (see tests/ddp_nccl_worker.py), once with the
 fused peer-memory exchange (the default) and once with the NCCL fallback.
-Needs two visible GPUs (`gpurun --gpus 2`); skipped on a single-GPU box.  The log is kept in gpurun_out/."""
+Needs two visible GPUs; skipped on a single-GPU machine.  With $STEGO_PARITY_DIR set, the workers' log is kept there."""
 import json
 import os
 import subprocess
@@ -24,9 +24,10 @@ def test_ddp_step_matches_shard_and_average(cuda_dev, exchange):
            "127.0.0.1", "--master-port", str(port), os.path.join(ROOT, "tests", "ddp_nccl_worker.py")]
     env = dict(os.environ, STEGO_TEST_P2P="1" if exchange == "p2p" else "0")
     r = subprocess.run(cmd, capture_output=True, text=True, timeout=900, cwd=ROOT, env=env)
-    os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-    with open(os.path.join(ROOT, "gpurun_out", f"ddp_{exchange}_parity.log"), "w") as fh:
-        fh.write(r.stdout + "\n---- stderr ----\n" + r.stderr[-4000:])
+    if os.environ.get("STEGO_PARITY_DIR"):
+        os.makedirs(os.environ["STEGO_PARITY_DIR"], exist_ok=True)
+        with open(os.path.join(os.environ["STEGO_PARITY_DIR"], f"ddp_{exchange}_parity.log"), "w") as fh:
+            fh.write(r.stdout + "\n---- stderr ----\n" + r.stderr[-4000:])
     lines = [json.loads(l.split(" ", 1)[1]) for l in r.stdout.splitlines() if l.startswith("DDP_NCCL_RESULT ")]
     assert r.returncode == 0, r.stdout[-2000:] + r.stderr[-2000:]
     assert len(lines) == world and all(l["ok"] and l["exchange"] == exchange for l in lines)

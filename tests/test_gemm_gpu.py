@@ -1,4 +1,4 @@
-"""tcgen05 GEMM (stego_gemm_bf16) against a plain PyTorch fp32 reference on bf16-rounded operands."""
+"""wgmma GEMM (stego_gemm_bf16) against a plain PyTorch fp32 reference on bf16-rounded operands."""
 import pytest
 import torch
 
@@ -131,9 +131,9 @@ def test_gemm_bad_args_raise(cuda_dev):
 
 @pytest.mark.parametrize("mode", ["residual_other", "bf16_out_residual", "atomic", "bias_misaligned"])
 def test_gemm_n1152_without_tma_epilogue(cuda_dev, mode):
-    """N = 1152 normally takes the 128x192 tile, which only exists with the TMA epilogue.  Calls that cannot use that
-    epilogue (residual != out, bf16 output + residual, atomic output, misaligned bias) must pick a tile whose
-    tensor-map box matches the kernel actually launched (a mismatch hangs on the stage barrier)."""
+    """N = 1152 (the ViT-B qkv width) takes the wide 128x256 tile with a ragged last column tile; every epilogue
+    variant (residual != out, bf16 output + residual, atomic output, misaligned bias) must clip it correctly and the
+    tensor-map box must match the kernel actually launched (a mismatch hangs on the stage barrier)."""
     from stego_b200 import ops
     torch.manual_seed(11)
     M, N, K = 300, 1152, 384
