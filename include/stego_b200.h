@@ -132,6 +132,39 @@ STEGO_API int stego_sample_norm_bwd(const float* code, const float* code_pos, lo
                                     float* dcode_pos, int B, int C, int H, int W, int feature_samples, int nslots,
                                     int perms_are_raw_randperm, void* stream);
 
+/* Multi-tile counterparts of the four calls above for feature_samples 1..64 (S = fs^2 up to 4096 points; the
+ * training path uses them for fs >= 12, where S exceeds one 128-row tile).  Tiles hold R = ceil(S / 128) * 128 rows
+ * per (plane, slot, image): operand tiles bf16 [2][nslots][B][R][Cpad], gradient tiles fp32 [nslots][B][R][72].
+ * The fd / cd einsums run per 128x128 (row tile, column tile) block on wgmma, with the same bf16 hi/lo split and fp32
+ * accumulation; every reduction runs in a fixed order (no atomics), so results are bit-reproducible run to run. */
+STEGO_API int stego_sample_norm_tiled_fwd(const void* src, const void* src_pos, int src_is_bf16, long long stride_b,
+                                          long long stride_c, long long stride_y, long long stride_x,
+                                          const float* chan_scale, const float* chan_scale_pos, const float* coords1,
+                                          const float* coords2, const long long* perms, void* tiles, int B, int C,
+                                          int Cpad, int H, int W, int feature_samples, int nslots,
+                                          int perms_are_raw_randperm, void* stream);
+/* row_partials: scratch [ncalls][B][R / 128][R][4] (per-row, per-column-tile sums of fd, clamp(cd) * fd, clamp(cd),
+ * cd); row_means: out [ncalls][B][R], the pointwise row means of fd (0 when !pointwise), needed by the backward;
+ * stats / cd_out / fdc_out / loss_out as for stego_corr_loss_fwd (fdc_out is centred with the row means). */
+STEGO_API int stego_corr_loss_tiled_fwd(const void* feat_tiles, const void* code_tiles, int B, int feature_samples,
+                                        int E, int D, int nslots, int ncalls, const int* slot_of_call_host,
+                                        const float* shifts_host, int pointwise, int zero_clamp, int stabilize,
+                                        float* row_partials, float* row_means, float* stats, float* cd_out,
+                                        float* fdc_out, float* loss_out, void* stream);
+/* dtiles: fp32 [nslots][B][R][72], zero on entry.  Two passes recompute fd / cd per block: dB (all slots) then dA
+ * (slot 0), each with one CTA owning its output rows. */
+STEGO_API int stego_corr_loss_tiled_bwd(const void* feat_tiles, const void* code_tiles, int B, int feature_samples,
+                                        int E, int D, int nslots, int ncalls, const int* slot_of_call_host,
+                                        const float* shifts_host, int pointwise, int zero_clamp, int stabilize,
+                                        const float* stats, const float* row_means, const float* gscale,
+                                        const float* gelem, const float* gcd, float* dtiles, void* stream);
+STEGO_API int stego_sample_norm_tiled_bwd(const float* code, const float* code_pos, long long stride_b,
+                                          long long stride_c, long long stride_y, long long stride_x,
+                                          const float* coords1, const float* coords2, const long long* perms,
+                                          const float* dtiles, float* dcode, float* dcode_pos, int B, int C, int H,
+                                          int W, int feature_samples, int nslots, int perms_are_raw_randperm,
+                                          void* stream);
+
 /* ------------------------------------------------------------------------------------------------
  * Segmentation head glue (reference: src/modules.py:73-81, 108-118) and optimiser
  * ---------------------------------------------------------------------------------------------- */

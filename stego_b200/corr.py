@@ -16,6 +16,7 @@ from . import _lib
 CODE_PAD = 128   # code channels are zero-padded to two 64-wide k-blocks in the operand tiles
 TILE_ROWS = 128  # feature_samples^2 <= 128
 DT_LD = 72       # row stride of the gradient tiles
+MAX_TILED_FS = 64  # the multi-tile kernels take feature_samples up to 64 (S = 4096 points per image)
 
 
 def _i32(vals: Sequence[int]):
@@ -41,38 +42,71 @@ def _zeros_strided_like(t: torch.Tensor) -> torch.Tensor:
     return torch.as_strided(buf, t.size(), t.stride())
 
 
+def _describe(spec, cfg, n_neg: Optional[int]) -> None:
+    spec.fs = int(cfg.feature_samples)
+    spec.n_neg = int(cfg.neg_samples if n_neg is None else n_neg)
+    spec.pointwise = bool(cfg.pointwise)
+    spec.zero_clamp = bool(cfg.zero_clamp)
+    spec.stabilize = bool(cfg.stabalize)
+    spec.nslots = 2 + spec.n_neg
+    spec.ncalls = 2 + spec.n_neg
+    # call 0: intra (A vs A), call 1: inter (A vs pos), calls 2..: negatives (A vs img[perm_i])
+    spec.slot_of_call = [0, 1] + [2 + i for i in range(spec.n_neg)]
+    spec.shifts = [float(cfg.pos_intra_shift), float(cfg.pos_inter_shift)] + [float(cfg.neg_inter_shift)] * spec.n_neg
+
+
 class LossSpec:
-    """Static description of one ContrastiveCorrelationLoss evaluation (which calls, which shifts)."""
+    """Static description of one ContrastiveCorrelationLoss evaluation (which calls, which shifts) for the
+    single-tile kernels: all S = feature_samples^2 <= 128 points of an image in one 128-row tile."""
+    tiled = False
+    rows = TILE_ROWS  # operand / gradient tile rows per (slot, image)
 
     def __init__(self, cfg, n_neg: Optional[int] = None):
-        self.fs = int(cfg.feature_samples)
-        self.n_neg = int(cfg.neg_samples if n_neg is None else n_neg)
-        self.pointwise = bool(cfg.pointwise)
-        self.zero_clamp = bool(cfg.zero_clamp)
-        self.stabilize = bool(cfg.stabalize)
-        self.nslots = 2 + self.n_neg
-        self.ncalls = 2 + self.n_neg
-        # call 0: intra (A vs A), call 1: inter (A vs pos), calls 2..: negatives (A vs img[perm_i])
-        self.slot_of_call = [0, 1] + [2 + i for i in range(self.n_neg)]
-        self.shifts = [float(cfg.pos_intra_shift), float(cfg.pos_inter_shift)] + [float(cfg.neg_inter_shift)] * self.n_neg
+        _describe(self, cfg, n_neg)
         if self.fs * self.fs > TILE_ROWS:
             raise RuntimeError(f"stego_b200: feature_samples={self.fs} exceeds the 128-row tile (max 11)")
+
+
+class TiledLossSpec:
+    """The same description for the multi-tile kernels: S points padded to whole 128-row tiles (`rows`), the fd / cd
+    blocks computed per (row tile, column tile).  Any feature_samples up to MAX_TILED_FS."""
+    tiled = True
+
+    def __init__(self, cfg, n_neg: Optional[int] = None):
+        _describe(self, cfg, n_neg)
+        if not 1 <= self.fs <= MAX_TILED_FS:
+            raise RuntimeError(f"stego_b200: feature_samples={self.fs} is outside the supported range "
+                               f"1..{MAX_TILED_FS}")
+        S = self.fs * self.fs
+        self.rows = (S + TILE_ROWS - 1) // TILE_ROWS * TILE_ROWS
+        self.n_tiles = self.rows // TILE_ROWS
+
+
+def make_spec(cfg, n_neg: Optional[int] = None):
+    """The loss implementation for cfg.feature_samples: the single-tile kernels up to 11 (S <= 128), the multi-tile
+    kernels from 12 to MAX_TILED_FS; above that a RuntimeError."""
+    fs = int(cfg.feature_samples)
+    if fs * fs <= TILE_ROWS:
+        return LossSpec(cfg, n_neg)
+    return TiledLossSpec(cfg, n_neg)
 
 
 def build_tiles(src: torch.Tensor, src_pos: torch.Tensor, coords1: torch.Tensor, coords2: torch.Tensor,
                 perms: Optional[torch.Tensor], spec: LossSpec, c_pad: int,
                 chan_scale: Optional[torch.Tensor] = None, chan_scale_pos: Optional[torch.Tensor] = None,
                 raw_perms: bool = False) -> torch.Tensor:
-    """sample + norm for every slot -> bf16 hi/lo tiles [2][nslots][B][128][c_pad]."""
+    """sample + norm for every slot -> bf16 hi/lo tiles [2][nslots][B][spec.rows][c_pad]."""
     B, C, H, W = src.shape
     src_pos = _same_layout(src, src_pos)
-    tiles = torch.empty(2, spec.nslots, B, TILE_ROWS, c_pad, dtype=torch.bfloat16, device=src.device)
+    tiles = torch.empty(2, spec.nslots, B, spec.rows, c_pad, dtype=torch.bfloat16, device=src.device)
     sb, sc, sy, sx = src.stride()
-    rc = _lib.load().stego_sample_norm_fwd(
-        _lib.ptr(src), _lib.ptr(src_pos), int(src.dtype == torch.bfloat16), sb, sc, sy, sx,
-        _lib.ptr(chan_scale), _lib.ptr(chan_scale_pos), _lib.ptr(coords1), _lib.ptr(coords2), _lib.ptr(perms),
-        _lib.ptr(tiles), B, C, c_pad, H, W, spec.fs, spec.nslots, int(raw_perms), _lib.stream())
-    _lib.check(rc, "stego_sample_norm_fwd")
+    lib = _lib.load()
+    fn, name = ((lib.stego_sample_norm_tiled_fwd, "stego_sample_norm_tiled_fwd") if spec.tiled
+                else (lib.stego_sample_norm_fwd, "stego_sample_norm_fwd"))
+    rc = fn(_lib.ptr(src), _lib.ptr(src_pos), int(src.dtype == torch.bfloat16), sb, sc, sy, sx,
+            _lib.ptr(chan_scale), _lib.ptr(chan_scale_pos), _lib.ptr(coords1), _lib.ptr(coords2), _lib.ptr(perms),
+            _lib.ptr(tiles), B, C, c_pad, H, W, spec.fs, spec.nslots, int(raw_perms), _lib.stream())
+    _lib.check(rc, name)
     return tiles
 
 
@@ -129,7 +163,6 @@ class _CorrLossFn(torch.autograd.Function):
         ctiles = build_tiles(code_f, code_pos_f, coords1, coords2, perms_t, spec, CODE_PAD, raw_perms=raw_perms)
         ctx.raw_perms = bool(raw_perms)
         S = spec.fs * spec.fs
-        partials = torch.empty(spec.ncalls, B, 8, dtype=torch.float32, device=dev)
         stats = torch.empty(spec.ncalls, 4, dtype=torch.float32, device=dev)
         cd = fdc = elems = None
         if want_elems:
@@ -137,16 +170,27 @@ class _CorrLossFn(torch.autograd.Function):
             fdc = torch.empty_like(cd)
             elems = torch.empty_like(cd)
         soc, shf = _i32(spec.slot_of_call), _f32(spec.shifts)
-        rc = _lib.load().stego_corr_loss_fwd(
-            _lib.ptr(ftiles), _lib.ptr(ctiles), B, spec.fs, E, D, spec.nslots, spec.ncalls, soc, shf,
-            int(spec.pointwise), int(spec.zero_clamp), int(spec.stabilize), _lib.ptr(partials), _lib.ptr(stats),
-            _lib.ptr(cd), _lib.ptr(fdc), _lib.ptr(elems), _lib.stream())
-        _lib.check(rc, "stego_corr_loss_fwd")
+        if spec.tiled:
+            partials = torch.empty(spec.ncalls, B, spec.n_tiles, spec.rows, 4, dtype=torch.float32, device=dev)
+            row_means = torch.empty(spec.ncalls, B, spec.rows, dtype=torch.float32, device=dev)
+            rc = _lib.load().stego_corr_loss_tiled_fwd(
+                _lib.ptr(ftiles), _lib.ptr(ctiles), B, spec.fs, E, D, spec.nslots, spec.ncalls, soc, shf,
+                int(spec.pointwise), int(spec.zero_clamp), int(spec.stabilize), _lib.ptr(partials),
+                _lib.ptr(row_means), _lib.ptr(stats), _lib.ptr(cd), _lib.ptr(fdc), _lib.ptr(elems), _lib.stream())
+            _lib.check(rc, "stego_corr_loss_tiled_fwd")
+        else:
+            partials = torch.empty(spec.ncalls, B, 8, dtype=torch.float32, device=dev)
+            row_means = torch.empty(0, device=dev)
+            rc = _lib.load().stego_corr_loss_fwd(
+                _lib.ptr(ftiles), _lib.ptr(ctiles), B, spec.fs, E, D, spec.nslots, spec.ncalls, soc, shf,
+                int(spec.pointwise), int(spec.zero_clamp), int(spec.stabilize), _lib.ptr(partials), _lib.ptr(stats),
+                _lib.ptr(cd), _lib.ptr(fdc), _lib.ptr(elems), _lib.stream())
+            _lib.check(rc, "stego_corr_loss_fwd")
         ctx.spec = spec
         ctx.dims = (B, E, D, H, W)
         ctx.code_dtype = (code.dtype, code_pos.dtype if code_pos is not None else code.dtype)
         ctx.save_for_backward(ftiles, ctiles, stats, code_f, code_pos_f, coords1, coords2,
-                              perms_t if perms_t is not None else torch.empty(0, device=dev))
+                              perms_t if perms_t is not None else torch.empty(0, device=dev), row_means)
         losses = stats[:, 0].clone()
         cd_means = stats[:, 1].clone()
         ctx.mark_non_differentiable(cd_means)
@@ -158,19 +202,27 @@ class _CorrLossFn(torch.autograd.Function):
     def backward(ctx, g_losses, _g_cd_means, g_cd, g_elems):
         spec: LossSpec = ctx.spec
         B, E, D, H, W = ctx.dims
-        ftiles, ctiles, stats, code_f, code_pos_f, coords1, coords2, perms_t = ctx.saved_tensors
+        ftiles, ctiles, stats, code_f, code_pos_f, coords1, coords2, perms_t, row_means = ctx.saved_tensors
         perms_arg = perms_t if spec.n_neg > 0 else None
         dev = code_f.device
         gscale = (g_losses if g_losses is not None else torch.zeros(spec.ncalls, device=dev)).to(torch.float32).contiguous()
         gel = g_elems.to(torch.float32).contiguous() if g_elems is not None else None
         gcd = g_cd.to(torch.float32).contiguous() if g_cd is not None else None
-        dtiles = torch.zeros(spec.nslots, B, TILE_ROWS, DT_LD, dtype=torch.float32, device=dev)
+        dtiles = torch.zeros(spec.nslots, B, spec.rows, DT_LD, dtype=torch.float32, device=dev)
         soc, shf = _i32(spec.slot_of_call), _f32(spec.shifts)
-        rc = _lib.load().stego_corr_loss_bwd(
-            _lib.ptr(ftiles), _lib.ptr(ctiles), B, spec.fs, E, D, spec.nslots, spec.ncalls, soc, shf,
-            int(spec.pointwise), int(spec.zero_clamp), int(spec.stabilize), _lib.ptr(stats), _lib.ptr(gscale),
-            _lib.ptr(gel), _lib.ptr(gcd), _lib.ptr(dtiles), _lib.stream())
-        _lib.check(rc, "stego_corr_loss_bwd")
+        lib = _lib.load()
+        if spec.tiled:
+            rc = lib.stego_corr_loss_tiled_bwd(
+                _lib.ptr(ftiles), _lib.ptr(ctiles), B, spec.fs, E, D, spec.nslots, spec.ncalls, soc, shf,
+                int(spec.pointwise), int(spec.zero_clamp), int(spec.stabilize), _lib.ptr(stats), _lib.ptr(row_means),
+                _lib.ptr(gscale), _lib.ptr(gel), _lib.ptr(gcd), _lib.ptr(dtiles), _lib.stream())
+            _lib.check(rc, "stego_corr_loss_tiled_bwd")
+        else:
+            rc = lib.stego_corr_loss_bwd(
+                _lib.ptr(ftiles), _lib.ptr(ctiles), B, spec.fs, E, D, spec.nslots, spec.ncalls, soc, shf,
+                int(spec.pointwise), int(spec.zero_clamp), int(spec.stabilize), _lib.ptr(stats), _lib.ptr(gscale),
+                _lib.ptr(gel), _lib.ptr(gcd), _lib.ptr(dtiles), _lib.stream())
+            _lib.check(rc, "stego_corr_loss_bwd")
         if ctx.pair:
             # code_f / code_pos_f are the two halves of one tensor: one zero-filled buffer with its layout
             full_size = (2 * B,) + tuple(code_f.shape[1:])
@@ -180,11 +232,12 @@ class _CorrLossFn(torch.autograd.Function):
             dcode = _zeros_strided_like(code_f)
             dcode_pos = _zeros_strided_like(code_f)
         sb, sc, sy, sx = code_f.stride()
-        rc = _lib.load().stego_sample_norm_bwd(
-            _lib.ptr(code_f), _lib.ptr(code_pos_f), sb, sc, sy, sx, _lib.ptr(coords1), _lib.ptr(coords2),
-            _lib.ptr(perms_arg), _lib.ptr(dtiles), _lib.ptr(dcode), _lib.ptr(dcode_pos), B, D, H, W, spec.fs,
-            spec.nslots, int(ctx.raw_perms), _lib.stream())
-        _lib.check(rc, "stego_sample_norm_bwd")
+        fn, name = ((lib.stego_sample_norm_tiled_bwd, "stego_sample_norm_tiled_bwd") if spec.tiled
+                    else (lib.stego_sample_norm_bwd, "stego_sample_norm_bwd"))
+        rc = fn(_lib.ptr(code_f), _lib.ptr(code_pos_f), sb, sc, sy, sx, _lib.ptr(coords1), _lib.ptr(coords2),
+                _lib.ptr(perms_arg), _lib.ptr(dtiles), _lib.ptr(dcode), _lib.ptr(dcode_pos), B, D, H, W, spec.fs,
+                spec.nslots, int(ctx.raw_perms), _lib.stream())
+        _lib.check(rc, name)
         d0, d1 = ctx.code_dtype
         if ctx.pair:
             return (dall.to(d0), None) + (None,) * 11
@@ -196,6 +249,7 @@ def corr_loss(feats, feats_pos, code, code_pos, coords1, coords2, perms, spec: L
     """raw_perms=True: `perms` holds the raw torch.randperm draws and the sampling kernel applies super_perm's
     fix-up itself (saves the eq/add/remainder launches of modules.super_perm).
     pair=True: `code` holds code ++ code_pos ([2B, D, h, w], one head pass) and `code_pos` is None.
+    spec: a LossSpec (single-tile kernels) or a TiledLossSpec (multi-tile kernels); make_spec picks by feature_samples.
     Returns (losses[ncalls], cd_means[ncalls], cd[ncalls,B,S,S]|None, loss_elems|None).
     losses[k] is the mean of helper call k (0 intra, 1 inter, 2.. negatives); differentiable wrt code/code_pos."""
     return _CorrLossFn.apply(code, code_pos, feats, feats_pos, coords1, coords2, perms, spec, want_elems,

@@ -53,6 +53,14 @@ struct SampleParams {
   float eps;
 };
 
+// Rows per (plane, slot, image) of the operand and gradient tiles: one 128-row tile for the single-tile kernels
+// (S <= 128), S rounded up to whole 128-row tiles for the multi-tile ones.
+template <bool kTiled>
+__host__ __device__ __forceinline__ int tile_rows(int S) {
+  if constexpr (kTiled) return (S + CL_ROWS - 1) / CL_ROWS * CL_ROWS;
+  else return CL_ROWS;
+}
+
 struct Taps {
   int i00, i01, i10, i11;      // pixel offsets (y*W + x), clamped in-bounds
   float w00, w01, w10, w11;    // nw, ne, sw, se weights (0 for out-of-bounds taps)
@@ -97,18 +105,19 @@ __device__ __forceinline__ void slot_source(const SampleParams& p, int slot, int
 }
 
 // One warp per tile row. Generic strides / dtypes; each lane owns channels lane, lane+32, ...
-template <int NV>  // NV = Cpad / 32
+template <int NV, bool kTiled = false>  // NV = Cpad / 32
 __global__ void __launch_bounds__(256)
 sample_norm_kernel(SampleParams p) {
+  const int R = tile_rows<kTiled>(p.S);
   const int warp_global = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
-  const int total = p.nslots * p.B * CL_ROWS;
+  const int total = p.nslots * p.B * R;
   if (warp_global >= total) return;
-  const int s = warp_global % CL_ROWS;
-  const int b = (warp_global / CL_ROWS) % p.B;
-  const int slot = warp_global / (CL_ROWS * p.B);
-  const size_t plane = static_cast<size_t>(p.nslots) * p.B * CL_ROWS * p.Cpad;
-  bf16* hi = p.tiles + (static_cast<size_t>(slot) * p.B + b) * CL_ROWS * p.Cpad + static_cast<size_t>(s) * p.Cpad;
+  const int s = warp_global % R;
+  const int b = (warp_global / R) % p.B;
+  const int slot = warp_global / (R * p.B);
+  const size_t plane = static_cast<size_t>(p.nslots) * p.B * R * p.Cpad;
+  bf16* hi = p.tiles + (static_cast<size_t>(slot) * p.B + b) * R * p.Cpad + static_cast<size_t>(s) * p.Cpad;
   bf16* lo = hi + plane;
   float v[NV];
   if (s >= p.S) {
@@ -163,18 +172,19 @@ sample_norm_kernel(SampleParams p) {
 // Vectorised variant for the layout the training step uses: bf16 source, channel stride 1 (tokens-major),
 // C % 8 == 0, Cpad == C.  Each lane owns 8 consecutive channels per step: four 16-byte tap loads, two 16-byte tile
 // stores (hi, lo) — 8x fewer memory instructions than the generic kernel.
-template <int NI>  // NI = ceil(C / 256)
+template <int NI, bool kTiled = false>  // NI = ceil(C / 256)
 __global__ void __launch_bounds__(256)
 sample_norm_vec8_kernel(SampleParams p) {
+  const int R = tile_rows<kTiled>(p.S);
   const int warp_global = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
-  const int total = p.nslots * p.B * CL_ROWS;
+  const int total = p.nslots * p.B * R;
   if (warp_global >= total) return;
-  const int s = warp_global % CL_ROWS;
-  const int b = (warp_global / CL_ROWS) % p.B;
-  const int slot = warp_global / (CL_ROWS * p.B);
-  const size_t plane = static_cast<size_t>(p.nslots) * p.B * CL_ROWS * p.Cpad;
-  bf16* hi = p.tiles + (static_cast<size_t>(slot) * p.B + b) * CL_ROWS * p.Cpad + static_cast<size_t>(s) * p.Cpad;
+  const int s = warp_global % R;
+  const int b = (warp_global / R) % p.B;
+  const int slot = warp_global / (R * p.B);
+  const size_t plane = static_cast<size_t>(p.nslots) * p.B * R * p.Cpad;
+  bf16* hi = p.tiles + (static_cast<size_t>(slot) * p.B + b) * R * p.Cpad + static_cast<size_t>(s) * p.Cpad;
   bf16* lo = hi + plane;
   if (s >= p.S) {
 #pragma unroll
@@ -589,26 +599,398 @@ __global__ void corr_loss_elems_kernel(const float* __restrict__ cd, const float
 }
 
 // ---------------------------------------------------------------------------------------------
+// Multi-tile variant for S > 128 (feature_samples 12 .. CT_MAX_FS).  The operand tiles hold R = tile_rows<true>(S)
+// rows per (plane, slot, image), i.e. nT = R / 128 row tiles.  A work unit is one 128x128 (row tile rt, column tile
+// ct) block of fd / cd for one (image, call), computed exactly like corr_kernel computes its single tile.
+//   forward  : one CTA per (image, call, rt, ct).  The loss is linear in the row mean m_i of fd,
+//                sum_j cl_ij (fd_ij - m_i - shift) = sum_j cl_ij fd_ij - (m_i + shift) sum_j cl_ij,
+//              so each unit emits per-row partials over its columns (sum fd, sum cl fd, sum cl, sum cd) without knowing
+//              m_i; corr_tiled_finish_kernel reduces them over the column tiles in a fixed order (fp64) into the row
+//              means and the per-call stats.
+//   backward : recomputes fd / cd per unit and forms G = dL/dfd as in corr_kernel.  dA = G . Bc sums over column tiles
+//              and dB = G^T . Ac over row tiles, so each has its own pass in which ONE CTA owns the output rows and walks
+//              the units in a fixed order: kMode 1 = CTA per (image, rt) walking (call, ct) -> dA rows rt of slot 0;
+//              kMode 2 = CTA per (image, ct) walking (call, rt) -> dB rows ct of each call's slot.  No atomics: the
+//              gradient tiles are bit-reproducible run to run.
+// ---------------------------------------------------------------------------------------------
+constexpr int CT_MAX_FS = 64;
+
+struct TiledParams {
+  int B, S, R, nT, E, D, nslots, ncalls;
+  int slot_of_call[CL_MAX_CALLS];
+  float shift[CL_MAX_CALLS];
+  int pointwise;
+  float clamp_lo, clamp_hi;
+  // forward outputs
+  float* rowpart;        // [ncalls][B][nT (column tile)][R][4]: sum fd, sum cl*fd, sum cl, sum cd over the tile's columns
+  float* cd_out;         // optional [ncalls][B][S][S]
+  float* fd_out;         // optional [ncalls][B][S][S]: raw fd here, centred in place by corr_tiled_elems_kernel
+  // backward inputs
+  const float* stats;    // [ncalls][4] as for corr_kernel
+  const float* rowmean;  // [ncalls][B][R]: the pointwise row means of fd (0 when !pointwise)
+  const float* gscale;
+  const float* gelem;
+  const float* gcd;
+  float* dtiles;         // [nslots][B][R][CL_DT_LD] fp32, zero-initialised by the caller
+};
+
+__device__ __forceinline__ uint32_t tiled_row(int plane, int slot, int b, int tile, const TiledParams& p) {
+  return static_cast<uint32_t>(((plane * p.nslots + slot) * p.B + b) * p.R + tile * CL_ROWS);
+}
+
+// unit u of this CTA -> (call, row tile, column tile)
+template <int kMode>
+__device__ __forceinline__ void tiled_unit(const TiledParams& p, int u, int& call, int& rt, int& ct) {
+  if constexpr (kMode == 0) {
+    call = blockIdx.y; rt = blockIdx.z / p.nT; ct = blockIdx.z % p.nT;
+  } else if constexpr (kMode == 1) {
+    call = u / p.nT; ct = u % p.nT; rt = blockIdx.y;
+  } else {
+    call = u / p.nT; rt = u % p.nT; ct = blockIdx.y;
+  }
+}
+
+template <int kMode>
+__global__ void __launch_bounds__(CL_THREADS, 1)
+corr_tiled_kernel(const __grid_constant__ CUtensorMap tmF, const __grid_constant__ CUtensorMap tmC, TiledParams p) {
+  constexpr bool kBackward = kMode != 0;
+  constexpr int kRing = kBackward ? 2 : 3;
+  constexpr uint32_t RING_BYTES = kRing * 2 * CL_TILE;
+  constexpr uint32_t CODE_BYTES = 8 * CL_TILE;  // Ac: [plane][kb] 4 tiles, Bc: 4 tiles
+  constexpr uint32_t OFF_CODE = RING_BYTES;
+  constexpr uint32_t OFF_BAR = OFF_CODE + CODE_BYTES;
+
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + OFF_BAR);
+  uint64_t* full_bar = bars;
+  uint64_t* empty_bar = bars + kRing;
+  uint64_t* code_full = empty_bar + kRing;
+  uint64_t* unit_done = code_full + 1;  // backward: ring (G) and code tiles of the unit are no longer read
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const int b = blockIdx.x;
+  const int nunits = kBackward ? p.ncalls * p.nT : 1;
+  const int nkb_f = p.E / 64;
+
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmF);
+    tma_prefetch_desc(&tmC);
+    for (int s = 0; s < kRing; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 2); }
+    mbar_init(code_full, 1);
+    mbar_init(unit_done, 2);
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  if (warp >= 8) {
+    warpgroup_reg_dealloc<40>();
+    if (warp == 8 && lane == 0) {
+      uint32_t stage = 0, phase = 0;
+      for (int u = 0; u < nunits; ++u) {
+        int call, rt, ct;
+        tiled_unit<kMode>(p, u, call, rt, ct);
+        const int slotB = p.slot_of_call[call];
+        if (u > 0) mbar_wait(unit_done, static_cast<uint32_t>(u - 1) & 1u);
+        mbar_arrive_expect_tx(code_full, CODE_BYTES);
+        for (int pl = 0; pl < 2; ++pl)
+          for (int kb = 0; kb < 2; ++kb) {
+            tma_load_2d(smem + OFF_CODE + (pl * 2 + kb) * CL_TILE, &tmC, code_full, kb * 64, tiled_row(pl, 0, b, rt, p));
+            tma_load_2d(smem + OFF_CODE + (4 + pl * 2 + kb) * CL_TILE, &tmC, code_full, kb * 64,
+                        tiled_row(pl, slotB, b, ct, p));
+          }
+        for (int pass = 0; pass < 3; ++pass) {
+          int pa, pb;
+          split_pass(pass, pa, pb);
+          for (int kb = 0; kb < nkb_f; ++kb) {
+            mbar_wait(&empty_bar[stage], phase ^ 1u);
+            uint8_t* sa = smem + stage * 2 * CL_TILE;
+            mbar_arrive_expect_tx(&full_bar[stage], 2 * CL_TILE);
+            tma_load_2d(sa, &tmF, &full_bar[stage], kb * 64, tiled_row(pa, 0, b, rt, p));
+            tma_load_2d(sa + CL_TILE, &tmF, &full_bar[stage], kb * 64, tiled_row(pb, slotB, b, ct, p));
+            if (++stage == kRing) { stage = 0; phase ^= 1u; }
+          }
+        }
+      }
+    }
+    return;
+  }
+
+  // ===================== MMA warpgroups: rows 64 mwg .. 64 mwg + 63 of the unit's fd / cd block =====================
+  warpgroup_reg_alloc<232>();
+  const int mwg = warp >> 2;
+  const int wq = warp & 3;
+  const bool leader = (threadIdx.x & 127) == 0;
+  constexpr uint32_t DESC_HI = smem_desc_hi_sw128(1024);
+  constexpr uint32_t TILE16 = CL_TILE >> 4;
+  constexpr uint32_t HALF16 = (CL_TILE / 2) >> 4;
+  const uint32_t ring_lo = smem_desc_lo(smem_u32(smem), 16);
+  const uint32_t code_lo = smem_desc_lo(smem_u32(smem + OFF_CODE), 16);
+  const int S = p.S;
+  const int i_loc = mwg * 64 + wq * 16 + (lane >> 2);  // tile-local row of fragment half 0 (+8 for half 1)
+  const int j_base = 2 * (lane & 3);
+  uint32_t stage = 0, phase = 0;
+  for (int u = 0; u < nunits; ++u) {
+    int call, rt, ct;
+    tiled_unit<kMode>(p, u, call, rt, ct);
+    const int slotB = p.slot_of_call[call];
+    float fd[64], cd[64];
+#pragma unroll
+    for (int t = 0; t < 64; ++t) { fd[t] = 0.f; cd[t] = 0.f; }
+    {
+      uint32_t prev = 0;
+      for (int ks = 0; ks < 3 * nkb_f; ++ks) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t a_lo = ring_lo + stage * 2 * TILE16;
+        fence_operands(fd);
+        wgmma_fence();
+#pragma unroll
+        for (uint32_t k = 0; k < 4; ++k)
+          wgmma_ss<128, 0, 0>(fd, smem_desc_join(a_lo + mwg * HALF16 + 2 * k, DESC_HI),
+                              smem_desc_join(a_lo + TILE16 + 2 * k, DESC_HI), 1u);
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (ks > 0 && leader) mbar_arrive(&empty_bar[prev]);
+        prev = stage;
+        if (++stage == kRing) { stage = 0; phase ^= 1u; }
+      }
+      mbar_wait(code_full, static_cast<uint32_t>(u) & 1u);
+      wgmma_fence();
+#pragma unroll
+      for (int pass = 0; pass < 3; ++pass) {
+        int pa, pb;
+        split_pass(pass, pa, pb);
+#pragma unroll
+        for (int kb = 0; kb < 2; ++kb) {
+          const uint32_t a_lo = code_lo + (pa * 2 + kb) * TILE16 + mwg * HALF16;
+          const uint32_t b_lo = code_lo + (4 + pb * 2 + kb) * TILE16;
+#pragma unroll
+          for (uint32_t k = 0; k < 4; ++k)
+            wgmma_ss<128, 0, 0>(cd, smem_desc_join(a_lo + 2 * k, DESC_HI), smem_desc_join(b_lo + 2 * k, DESC_HI), 1u);
+        }
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      fence_operands(fd);
+      fence_operands(cd);
+      if (leader) mbar_arrive(&empty_bar[prev]);
+    }
+
+    const int i0 = rt * CL_ROWS + i_loc;  // global rows of fragment halves 0 / 1: i0, i0 + 8
+    const int j0 = ct * CL_ROWS + j_base;
+    if constexpr (!kBackward) {
+      // per-row partials over this tile's valid columns; the four lanes of a quad hold disjoint columns of a row
+      float r_fd[2] = {0.f, 0.f}, r_clfd[2] = {0.f, 0.f}, r_cl[2] = {0.f, 0.f}, r_cd[2] = {0.f, 0.f};
+#pragma unroll
+      for (int t = 0; t < 64; ++t) {
+        const int h = (t >> 1) & 1;
+        const int i = i0 + 8 * h;
+        const int j = j0 + 8 * (t >> 2) + (t & 1);
+        if (i < S && j < S) {
+          const float cl = fminf(fmaxf(cd[t], p.clamp_lo), p.clamp_hi);
+          r_fd[h] += fd[t];
+          r_clfd[h] += cl * fd[t];
+          r_cl[h] += cl;
+          r_cd[h] += cd[t];
+          const size_t e = ((static_cast<size_t>(call) * p.B + b) * S + i) * S + j;
+          if (p.cd_out) p.cd_out[e] = cd[t];
+          if (p.fd_out) p.fd_out[e] = fd[t];
+        }
+      }
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+#pragma unroll
+        for (int o = 1; o <= 2; o <<= 1) {
+          r_fd[h] += __shfl_xor_sync(0xffffffffu, r_fd[h], o);
+          r_clfd[h] += __shfl_xor_sync(0xffffffffu, r_clfd[h], o);
+          r_cl[h] += __shfl_xor_sync(0xffffffffu, r_cl[h], o);
+          r_cd[h] += __shfl_xor_sync(0xffffffffu, r_cd[h], o);
+        }
+        const int i = i0 + 8 * h;
+        if ((lane & 3) == 0 && i < S)
+          *reinterpret_cast<float4*>(p.rowpart + (((static_cast<size_t>(call) * p.B + b) * p.nT + ct) * p.R + i) * 4) =
+              make_float4(r_fd[h], r_clfd[h], r_cl[h], r_cd[h]);
+      }
+      return;
+    } else {
+      const float* st = p.stats + call * 4;
+      const float offset = p.pointwise ? (st[2] - st[3]) : 0.f;  // old_mean - mean(centred fd)
+      const float gs = p.gscale[call] / (static_cast<float>(p.B) * S * S);
+      const float shift = p.shift[call];
+      float rmean[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int i = i0 + 8 * h;
+        rmean[h] = i < S ? p.rowmean[(static_cast<size_t>(call) * p.B + b) * p.R + i] : 0.f;
+      }
+#pragma unroll
+      for (int t = 0; t < 64; ++t) {
+        const int h = (t >> 1) & 1;
+        const int i = i0 + 8 * h;
+        const int j = j0 + 8 * (t >> 2) + (t & 1);
+        float gv = 0.f;
+        if (i < S && j < S) {
+          const size_t e = ((static_cast<size_t>(call) * p.B + b) * S + i) * S + j;
+          const float cdv = cd[t];
+          float up = gs;
+          if (p.gelem) up += p.gelem[e];
+          const bool pass_grad = (cdv >= p.clamp_lo) && (cdv <= p.clamp_hi);
+          gv = pass_grad ? -up * (fd[t] - rmean[h] + offset - shift) : 0.f;
+          if (p.gcd) gv += p.gcd[e];
+        }
+        fd[t] = gv;
+      }
+    }
+    // ---- backward: G as a swizzled bf16 hi/lo image in the ring area, exactly as corr_kernel stages it
+    asm volatile("bar.sync 1, 256;\n" ::: "memory");
+#pragma unroll
+    for (int t = 0; t < 64; t += 2) {
+      const int i = i_loc + 8 * ((t >> 1) & 1);
+      const int j = 8 * (t >> 2) + j_base;
+      const float h0 = __bfloat162float(__float2bfloat16_rn(fd[t]));
+      const float h1 = __bfloat162float(__float2bfloat16_rn(fd[t + 1]));
+      const uint32_t o = (j >> 6) * CL_TILE + sw128_offset(i, (j & 63) >> 3) + (j & 7) * 2;
+      *reinterpret_cast<uint32_t*>(smem + o) = pack_bf16x2(h0, h1);
+      *reinterpret_cast<uint32_t*>(smem + 2 * CL_TILE + o) = pack_bf16x2(fd[t] - h0, fd[t + 1] - h1);
+    }
+    fence_proxy_async_smem();
+    asm volatile("bar.sync 1, 256;\n" ::: "memory");
+    {
+      const uint32_t code_mn_lo = smem_desc_lo(smem_u32(smem + OFF_CODE), CL_TILE);
+#pragma unroll
+      for (int t = 0; t < 64; ++t) cd[t] = 0.f;
+      wgmma_fence();
+#pragma unroll
+      for (int pass = 0; pass < 3; ++pass) {
+        int pg, pc;
+        split_pass(pass, pg, pc);
+        const uint32_t g_off = pg * 2 * TILE16;
+        if constexpr (kMode == 1) {
+          // dA[i][c] = sum_j G[i][j] Bc[j][c]: G K-major (k = j), Bc MN-major
+          const uint32_t g_k_lo = ring_lo + mwg * HALF16;
+          const uint32_t bc_lo = code_mn_lo + (4 + pc * 2) * TILE16;
+#pragma unroll
+          for (uint32_t kk = 0; kk < 8; ++kk)
+            wgmma_ss<128, 0, 1>(cd, smem_desc_join(g_k_lo + g_off + (kk >> 2) * TILE16 + (kk & 3) * 2, DESC_HI),
+                                smem_desc_join(bc_lo + kk * (2048u >> 4), DESC_HI), 1u);
+        } else {
+          // dB[j][c] = sum_i G[i][j] Ac[i][c]: G^T MN-major (m = j block of this warpgroup, k = i), Ac MN-major
+          const uint32_t g_mn_lo = smem_desc_lo(smem_u32(smem), CL_TILE) + mwg * TILE16;
+          const uint32_t ac_lo = code_mn_lo + (pc * 2) * TILE16;
+#pragma unroll
+          for (uint32_t kk = 0; kk < 8; ++kk)
+            wgmma_ss<128, 1, 1>(cd, smem_desc_join(g_mn_lo + g_off + kk * (2048u >> 4), DESC_HI),
+                                smem_desc_join(ac_lo + kk * (2048u >> 4), DESC_HI), 1u);
+        }
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      fence_operands(cd);
+    }
+    if (leader) mbar_arrive(unit_done);
+    // kMode 1: rows i of tile rt of slot 0; kMode 2: rows j of tile ct of the call's slot.  One owner CTA per row,
+    // units in a fixed order: plain read-modify-write.
+    const int slot_out = kMode == 1 ? 0 : slotB;
+    const int row0 = (kMode == 1 ? rt : ct) * CL_ROWS + i_loc;
+    float* dt = p.dtiles + (static_cast<size_t>(slot_out) * p.B + b) * p.R * CL_DT_LD;
+#pragma unroll
+    for (int t = 0; t < 64; ++t) {
+      const int r = row0 + 8 * ((t >> 1) & 1);
+      const int c = 8 * (t >> 2) + j_base + (t & 1);
+      if (r < S && c < p.D) dt[static_cast<size_t>(r) * CL_DT_LD + c] += cd[t];
+    }
+  }
+}
+
+// Per call: row means and stats from the per-row partials, fp64, every sum in a fixed order.
+constexpr int CT_FINISH_THREADS = 256;
+__global__ void __launch_bounds__(CT_FINISH_THREADS)
+corr_tiled_finish_kernel(TiledParams p, float* __restrict__ rowmean, float* __restrict__ stats) {
+  const int call = blockIdx.x;
+  const int S = p.S;
+  const double shift = p.shift[call];
+  // acc: 0 sum cl (fd - m - shift), 1 sum cl, 2 sum fd, 3 sum (fd - m), 4 sum cd
+  double acc[5] = {0, 0, 0, 0, 0};
+  for (int r = threadIdx.x; r < p.B * S; r += CT_FINISH_THREADS) {
+    const int b = r / S, i = r % S;
+    double s_fd = 0, s_clfd = 0, s_cl = 0, s_cd = 0;
+    const float* rp = p.rowpart + ((static_cast<size_t>(call) * p.B + b) * p.nT * p.R + i) * 4;
+    for (int ct = 0; ct < p.nT; ++ct) {
+      const float4 v = *reinterpret_cast<const float4*>(rp + static_cast<size_t>(ct) * p.R * 4);
+      s_fd += v.x; s_clfd += v.y; s_cl += v.z; s_cd += v.w;
+    }
+    const float m = p.pointwise ? static_cast<float>(s_fd / S) : 0.f;
+    rowmean[(static_cast<size_t>(call) * p.B + b) * p.R + i] = m;
+    acc[0] += s_clfd - (static_cast<double>(m) + shift) * s_cl;
+    acc[1] += s_cl;
+    acc[2] += s_fd;
+    acc[3] += s_fd - static_cast<double>(S) * m;
+    acc[4] += s_cd;
+  }
+  __shared__ double red[5][CT_FINISH_THREADS];
+#pragma unroll
+  for (int k = 0; k < 5; ++k) red[k][threadIdx.x] = acc[k];
+  __syncthreads();
+  for (int w = CT_FINISH_THREADS / 2; w > 0; w >>= 1) {
+    if (threadIdx.x < w)
+#pragma unroll
+      for (int k = 0; k < 5; ++k) red[k][threadIdx.x] += red[k][threadIdx.x + w];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) {
+    const double n = static_cast<double>(p.B) * S * S;
+    const double old_mean = red[2][0] / n;
+    const double mean_c = red[3][0] / n;
+    const double offset = p.pointwise ? (old_mean - mean_c) : 0.0;
+    stats[call * 4 + 0] = static_cast<float>(-(red[0][0] + offset * red[1][0]) / n);
+    stats[call * 4 + 1] = static_cast<float>(red[4][0] / n);
+    stats[call * 4 + 2] = static_cast<float>(old_mean);
+    stats[call * 4 + 3] = static_cast<float>(mean_c);
+  }
+}
+
+// centres fd_out in place with the row means and writes the unreduced loss elements
+__global__ void corr_tiled_elems_kernel(const float* __restrict__ cd, float* __restrict__ fdc,
+                                        const float* __restrict__ rowmean, const float* __restrict__ stats,
+                                        float* __restrict__ loss, TiledParams p) {
+  const long long per_call = 1ll * p.B * p.S * p.S;
+  const long long idx = 1ll * blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= per_call * p.ncalls) return;
+  const int call = static_cast<int>(idx / per_call);
+  const long long row = idx / p.S;  // (call * B + b) * S + i
+  const int i = static_cast<int>(row % p.S);
+  const long long cb = row / p.S;   // call * B + b
+  const float v = fdc[idx] - rowmean[cb * p.R + i];
+  fdc[idx] = v;
+  if (loss) {
+    const float offset = p.pointwise ? (stats[call * 4 + 2] - stats[call * 4 + 3]) : 0.f;
+    const float cl = fminf(fmaxf(cd[idx], p.clamp_lo), p.clamp_hi);
+    loss[idx] = -cl * (v + offset - p.shift[call]);
+  }
+}
+
+// ---------------------------------------------------------------------------------------------
 // 5. normalisation + grid_sample backward, as a gather: one warp per destination pixel (of code or code_pos) visits
 //    every (slot, image, sample) whose bilinear taps reach that pixel, in a fixed order, and writes its channels once —
 //    no atomics, so the code gradient is bit-reproducible run to run.
 // ---------------------------------------------------------------------------------------------
 struct SampleBwdParams {
   SampleParams f;        // forward description of the code sampling (src = code, src_pos = code_pos)
-  const float* dtiles;   // [nslots][B][128][CL_DT_LD]
+  const float* dtiles;   // [nslots][B][rows][CL_DT_LD], rows = tile_rows(S)
   float* dsrc;           // gradient wrt src, same strides as src, fp32, zero-initialised / accumulated into
   float* dsrc_pos;
 };
 
 // d/dv of the normalised sample v/||v|| for (slot, b, s), lane-owned channels lane + 32 k
-template <int NV>
+template <int NV, bool kTiled>
 __device__ __forceinline__ void sample_dv(const SampleBwdParams& q, int slot, int b, int s, const Taps& t,
                                           const float* src, int img, int lane, float (&dv)[NV]) {
   const SampleParams& p = q.f;
   auto off = [&](int pix) { return static_cast<long long>(pix / p.W) * p.sy + static_cast<long long>(pix % p.W) * p.sx; };
   const long long o00 = off(t.i00), o01 = off(t.i01), o10 = off(t.i10), o11 = off(t.i11);
   const long long base = static_cast<long long>(img) * p.sb;
-  const float* g = q.dtiles + ((static_cast<size_t>(slot) * p.B + b) * CL_ROWS + s) * CL_DT_LD;
+  const float* g = q.dtiles + ((static_cast<size_t>(slot) * p.B + b) * tile_rows<kTiled>(p.S) + s) * CL_DT_LD;
   float v[NV], gr[NV];
   float ss = 0.f, dot = 0.f;
 #pragma unroll
@@ -641,7 +1023,7 @@ __device__ __forceinline__ void sample_dv(const SampleBwdParams& q, int slot, in
   }
 }
 
-template <int NV>
+template <int NV, bool kTiled = false>
 __global__ void __launch_bounds__(256)
 sample_norm_bwd_kernel(SampleBwdParams q) {
   const SampleParams& p = q.f;
@@ -687,7 +1069,7 @@ sample_norm_bwd_kernel(SampleBwdParams q) {
             const float wm = __shfl_sync(0xffffffffu, w, src_lane);
             const Taps tm = make_taps(coords, b, s0 + src_lane, p.fs, p.H, p.W);
             float dv[NV];
-            sample_dv<NV>(q, slot, b, s0 + src_lane, tm, reinterpret_cast<const float*>(src), img, lane, dv);
+            sample_dv<NV, kTiled>(q, slot, b, s0 + src_lane, tm, reinterpret_cast<const float*>(src), img, lane, dv);
 #pragma unroll
             for (int k = 0; k < NV; ++k) acc[k] += dv[k] * wm;
           }
@@ -726,10 +1108,14 @@ static int fill_sample_params(SampleParams& sp, const void* src, const void* src
                               long long sc, long long sy, long long sx, const float* chan_scale,
                               const float* chan_scale_pos, const float* coords1, const float* coords2,
                               const long long* perms, void* tiles, int B, int C, int Cpad, int H, int W, int fs,
-                              int nslots) {
+                              int nslots, bool tiled = false) {
   STEGO_CHECK_ARG(src && src_pos && coords1 && coords2, "sample_norm: null pointer");
   STEGO_CHECK_ARG(nslots >= 2 && (nslots == 2 || perms), "sample_norm: nslots=%d needs perms", nslots);
-  STEGO_CHECK_ARG(fs * fs <= CL_ROWS, "sample_norm: feature_samples^2 = %d exceeds the 128-row tile", fs * fs);
+  if (!tiled) {
+    STEGO_CHECK_ARG(fs * fs <= CL_ROWS, "sample_norm: feature_samples^2 = %d exceeds the 128-row tile", fs * fs);
+  } else {
+    STEGO_CHECK_ARG(fs >= 1 && fs <= CT_MAX_FS, "sample_norm_tiled: feature_samples=%d outside 1..%d", fs, CT_MAX_FS);
+  }
   STEGO_CHECK_ARG(C > 0 && C <= Cpad && Cpad % 64 == 0 && Cpad <= 768, "sample_norm: C=%d Cpad=%d", C, Cpad);
   STEGO_CHECK_ARG(B > 0 && H > 1 && W > 1, "sample_norm: B=%d H=%d W=%d", B, H, W);
   sp.src = src; sp.src_pos = src_pos; sp.src_bf16 = src_bf16;
@@ -746,45 +1132,67 @@ static int fill_sample_params(SampleParams& sp, const void* src, const void* src
 
 using namespace stego;
 
-extern "C" int stego_sample_norm_fwd(const void* src, const void* src_pos, int src_is_bf16, long long stride_b,
-                                     long long stride_c, long long stride_y, long long stride_x,
-                                     const float* chan_scale, const float* chan_scale_pos, const float* coords1,
-                                     const float* coords2, const long long* perms, void* tiles, int B, int C,
-                                     int Cpad, int H, int W, int feature_samples, int nslots, int perms_are_raw_randperm,
-                                     void* stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+template <bool kTiled>
+static int sample_norm_fwd(const void* src, const void* src_pos, int src_is_bf16, long long stride_b,
+                           long long stride_c, long long stride_y, long long stride_x, const float* chan_scale,
+                           const float* chan_scale_pos, const float* coords1, const float* coords2,
+                           const long long* perms, void* tiles, int B, int C, int Cpad, int H, int W,
+                           int feature_samples, int nslots, int perms_are_raw_randperm, cudaStream_t stream) {
   SampleParams sp;
   int rc = fill_sample_params(sp, src, src_pos, src_is_bf16, stride_b, stride_c, stride_y, stride_x, chan_scale,
-                              chan_scale_pos, coords1, coords2, perms, tiles, B, C, Cpad, H, W, feature_samples, nslots);
+                              chan_scale_pos, coords1, coords2, perms, tiles, B, C, Cpad, H, W, feature_samples, nslots,
+                              kTiled);
   if (rc != STEGO_OK) return rc;
   sp.perms_raw = perms_are_raw_randperm;
   STEGO_CHECK_ARG(tiles, "stego_sample_norm_fwd: null tiles");
-  const int warps = nslots * B * CL_ROWS;
+  const int warps = nslots * B * tile_rows<kTiled>(sp.S);
   const int blocks = (warps + 7) / 8;
   const bool aligned = ((reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(src_pos) |
                          reinterpret_cast<uintptr_t>(tiles)) & 15u) == 0 &&
                        stride_b % 8 == 0 && stride_y % 8 == 0 && stride_x % 8 == 0;
   if (src_is_bf16 && stride_c == 1 && C % 8 == 0 && Cpad == C && aligned && C <= 768) {
     const int ni = (C + 255) / 256;
-    if (ni == 1) sample_norm_vec8_kernel<1><<<blocks, 256, 0, stream>>>(sp);
-    else if (ni == 2) sample_norm_vec8_kernel<2><<<blocks, 256, 0, stream>>>(sp);
-    else sample_norm_vec8_kernel<3><<<blocks, 256, 0, stream>>>(sp);
+    if (ni == 1) sample_norm_vec8_kernel<1, kTiled><<<blocks, 256, 0, stream>>>(sp);
+    else if (ni == 2) sample_norm_vec8_kernel<2, kTiled><<<blocks, 256, 0, stream>>>(sp);
+    else sample_norm_vec8_kernel<3, kTiled><<<blocks, 256, 0, stream>>>(sp);
     STEGO_CHECK_LAUNCH("sample_norm_vec8_kernel");
     return STEGO_OK;
   }
   switch (Cpad / 32) {
-    case 2: sample_norm_kernel<2><<<blocks, 256, 0, stream>>>(sp); break;
-    case 4: sample_norm_kernel<4><<<blocks, 256, 0, stream>>>(sp); break;
-    case 6: sample_norm_kernel<6><<<blocks, 256, 0, stream>>>(sp); break;
-    case 8: sample_norm_kernel<8><<<blocks, 256, 0, stream>>>(sp); break;
-    case 12: sample_norm_kernel<12><<<blocks, 256, 0, stream>>>(sp); break;
-    case 24: sample_norm_kernel<24><<<blocks, 256, 0, stream>>>(sp); break;
+    case 2: sample_norm_kernel<2, kTiled><<<blocks, 256, 0, stream>>>(sp); break;
+    case 4: sample_norm_kernel<4, kTiled><<<blocks, 256, 0, stream>>>(sp); break;
+    case 6: sample_norm_kernel<6, kTiled><<<blocks, 256, 0, stream>>>(sp); break;
+    case 8: sample_norm_kernel<8, kTiled><<<blocks, 256, 0, stream>>>(sp); break;
+    case 12: sample_norm_kernel<12, kTiled><<<blocks, 256, 0, stream>>>(sp); break;
+    case 24: sample_norm_kernel<24, kTiled><<<blocks, 256, 0, stream>>>(sp); break;
     default:
       set_error("stego_sample_norm_fwd: Cpad=%d unsupported (64,128,192,256,384,768)", Cpad);
       return STEGO_ERR_UNSUPPORTED;
   }
   STEGO_CHECK_LAUNCH("sample_norm_kernel");
   return STEGO_OK;
+}
+
+extern "C" int stego_sample_norm_fwd(const void* src, const void* src_pos, int src_is_bf16, long long stride_b,
+                                     long long stride_c, long long stride_y, long long stride_x,
+                                     const float* chan_scale, const float* chan_scale_pos, const float* coords1,
+                                     const float* coords2, const long long* perms, void* tiles, int B, int C,
+                                     int Cpad, int H, int W, int feature_samples, int nslots, int perms_are_raw_randperm,
+                                     void* stream_) {
+  return sample_norm_fwd<false>(src, src_pos, src_is_bf16, stride_b, stride_c, stride_y, stride_x, chan_scale,
+                                chan_scale_pos, coords1, coords2, perms, tiles, B, C, Cpad, H, W, feature_samples,
+                                nslots, perms_are_raw_randperm, reinterpret_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int stego_sample_norm_tiled_fwd(const void* src, const void* src_pos, int src_is_bf16, long long stride_b,
+                                           long long stride_c, long long stride_y, long long stride_x,
+                                           const float* chan_scale, const float* chan_scale_pos, const float* coords1,
+                                           const float* coords2, const long long* perms, void* tiles, int B, int C,
+                                           int Cpad, int H, int W, int feature_samples, int nslots,
+                                           int perms_are_raw_randperm, void* stream_) {
+  return sample_norm_fwd<true>(src, src_pos, src_is_bf16, stride_b, stride_c, stride_y, stride_x, chan_scale,
+                               chan_scale_pos, coords1, coords2, perms, tiles, B, C, Cpad, H, W, feature_samples,
+                               nslots, perms_are_raw_randperm, reinterpret_cast<cudaStream_t>(stream_));
 }
 
 static int fill_corr_params(CorrParams& p, int B, int fs, int E, int D, int nslots, int ncalls, const int* slot_of_call,
@@ -870,22 +1278,156 @@ extern "C" int stego_corr_loss_bwd(const void* feat_tiles, const void* code_tile
   return launch_corr<true>(tmF, tmC, p, stream);
 }
 
+template <bool kTiled>
+static int sample_norm_bwd(const float* code, const float* code_pos, long long stride_b, long long stride_c,
+                           long long stride_y, long long stride_x, const float* coords1, const float* coords2,
+                           const long long* perms, const float* dtiles, float* dcode, float* dcode_pos, int B, int C,
+                           int H, int W, int feature_samples, int nslots, int perms_are_raw_randperm,
+                           cudaStream_t stream) {
+  STEGO_CHECK_ARG(dtiles && dcode && dcode_pos, "stego_sample_norm_bwd: null pointer");
+  STEGO_CHECK_ARG(C <= 96, "stego_sample_norm_bwd: C=%d unsupported (<= 96)", C);
+  SampleBwdParams q;
+  int rc = fill_sample_params(q.f, code, code_pos, 0, stride_b, stride_c, stride_y, stride_x, nullptr, nullptr,
+                              coords1, coords2, perms, nullptr, B, C, CL_CODE_PAD, H, W, feature_samples, nslots, kTiled);
+  if (rc != STEGO_OK) return rc;
+  q.f.perms_raw = perms_are_raw_randperm;
+  q.dtiles = dtiles; q.dsrc = dcode; q.dsrc_pos = dcode_pos;
+  const int warps = 2 * B * H * W;
+  sample_norm_bwd_kernel<3, kTiled><<<(warps + 7) / 8, 256, 0, stream>>>(q);
+  STEGO_CHECK_LAUNCH("sample_norm_bwd_kernel");
+  return STEGO_OK;
+}
+
 extern "C" int stego_sample_norm_bwd(const float* code, const float* code_pos, long long stride_b, long long stride_c,
                                      long long stride_y, long long stride_x, const float* coords1,
                                      const float* coords2, const long long* perms, const float* dtiles, float* dcode,
                                      float* dcode_pos, int B, int C, int H, int W, int feature_samples, int nslots,
                                      int perms_are_raw_randperm, void* stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  STEGO_CHECK_ARG(dtiles && dcode && dcode_pos, "stego_sample_norm_bwd: null pointer");
-  STEGO_CHECK_ARG(C <= 96, "stego_sample_norm_bwd: C=%d unsupported (<= 96)", C);
-  SampleBwdParams q;
-  int rc = fill_sample_params(q.f, code, code_pos, 0, stride_b, stride_c, stride_y, stride_x, nullptr, nullptr,
-                              coords1, coords2, perms, nullptr, B, C, CL_CODE_PAD, H, W, feature_samples, nslots);
-  if (rc != STEGO_OK) return rc;
-  q.f.perms_raw = perms_are_raw_randperm;
-  q.dtiles = dtiles; q.dsrc = dcode; q.dsrc_pos = dcode_pos;
-  const int warps = 2 * B * H * W;
-  sample_norm_bwd_kernel<3><<<(warps + 7) / 8, 256, 0, stream>>>(q);
-  STEGO_CHECK_LAUNCH("sample_norm_bwd_kernel");
+  return sample_norm_bwd<false>(code, code_pos, stride_b, stride_c, stride_y, stride_x, coords1, coords2, perms,
+                                dtiles, dcode, dcode_pos, B, C, H, W, feature_samples, nslots, perms_are_raw_randperm,
+                                reinterpret_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int stego_sample_norm_tiled_bwd(const float* code, const float* code_pos, long long stride_b,
+                                           long long stride_c, long long stride_y, long long stride_x,
+                                           const float* coords1, const float* coords2, const long long* perms,
+                                           const float* dtiles, float* dcode, float* dcode_pos, int B, int C, int H,
+                                           int W, int feature_samples, int nslots, int perms_are_raw_randperm,
+                                           void* stream_) {
+  return sample_norm_bwd<true>(code, code_pos, stride_b, stride_c, stride_y, stride_x, coords1, coords2, perms,
+                               dtiles, dcode, dcode_pos, B, C, H, W, feature_samples, nslots, perms_are_raw_randperm,
+                               reinterpret_cast<cudaStream_t>(stream_));
+}
+
+// ---------------------------------------------------------------------------------------------
+// multi-tile correlation loss (S > 128)
+// ---------------------------------------------------------------------------------------------
+static int fill_tiled_params(TiledParams& p, int B, int fs, int E, int D, int nslots, int ncalls,
+                             const int* slot_of_call, const float* shifts, int pointwise, int zero_clamp,
+                             int stabilize) {
+  STEGO_CHECK_ARG(B > 0 && fs >= 1 && E % 64 == 0 && E >= 64 && E <= 768, "corr_tiled: B=%d fs=%d E=%d", B, fs, E);
+  STEGO_CHECK_ARG(fs <= CT_MAX_FS, "corr_tiled: feature_samples=%d exceeds the supported maximum %d", fs, CT_MAX_FS);
+  STEGO_CHECK_ARG(D > 0 && D <= 96, "corr_tiled: code dim %d unsupported (<= 96)", D);
+  STEGO_CHECK_ARG(ncalls > 0 && ncalls <= CL_MAX_CALLS && nslots >= 2, "corr_tiled: ncalls=%d nslots=%d", ncalls,
+                  nslots);
+  p.B = B; p.S = fs * fs; p.R = tile_rows<true>(p.S); p.nT = p.R / CL_ROWS; p.E = E; p.D = D;
+  p.nslots = nslots; p.ncalls = ncalls;
+  for (int k = 0; k < ncalls; ++k) {
+    STEGO_CHECK_ARG(slot_of_call[k] >= 0 && slot_of_call[k] < nslots, "corr_tiled: slot_of_call[%d]=%d", k,
+                    slot_of_call[k]);
+    p.slot_of_call[k] = slot_of_call[k];
+    p.shift[k] = shifts[k];
+  }
+  p.pointwise = pointwise;
+  p.clamp_lo = zero_clamp ? 0.0f : -9999.0f;
+  p.clamp_hi = stabilize ? 0.8f : INFINITY;
+  p.rowpart = nullptr; p.cd_out = nullptr; p.fd_out = nullptr;
+  p.stats = nullptr; p.rowmean = nullptr; p.gscale = nullptr; p.gelem = nullptr; p.gcd = nullptr; p.dtiles = nullptr;
   return STEGO_OK;
+}
+
+static int encode_tiled_maps(const void* ftiles, const void* ctiles, const TiledParams& p, CUtensorMap* tmF,
+                             CUtensorMap* tmC) {
+  int rc;
+  const uint64_t rows = (uint64_t)2 * p.nslots * p.B * p.R;
+  {
+    uint64_t dims[2] = {(uint64_t)p.E, rows};
+    uint64_t str[1] = {(uint64_t)p.E * 2};
+    uint32_t box[2] = {64, 128};
+    if ((rc = make_tmap_bf16(tmF, ftiles, 2, dims, str, box)) != STEGO_OK) return rc;
+  }
+  {
+    uint64_t dims[2] = {(uint64_t)CL_CODE_PAD, rows};
+    uint64_t str[1] = {(uint64_t)CL_CODE_PAD * 2};
+    uint32_t box[2] = {64, 128};
+    if ((rc = make_tmap_bf16(tmC, ctiles, 2, dims, str, box)) != STEGO_OK) return rc;
+  }
+  return STEGO_OK;
+}
+
+template <int kMode>
+static int launch_corr_tiled(const CUtensorMap& tmF, const CUtensorMap& tmC, const TiledParams& p,
+                             cudaStream_t stream) {
+  constexpr int kRing = kMode != 0 ? 2 : 3;
+  constexpr size_t smem = size_t(kRing) * 2 * CL_TILE + 8 * CL_TILE + 512 + 1024;
+  static_assert(smem <= 232448, "exceeds the 227 KB of shared memory a CTA can opt into");
+  auto kern = corr_tiled_kernel<kMode>;
+  static bool configured = false;
+  if (!configured) {
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(corr_tiled)");
+    configured = true;
+  }
+  const dim3 grid = kMode == 0 ? dim3(p.B, p.ncalls, p.nT * p.nT) : dim3(p.B, p.nT);
+  kern<<<grid, CL_THREADS, smem, stream>>>(tmF, tmC, p);
+  STEGO_CHECK_LAUNCH("corr_tiled_kernel");
+  return STEGO_OK;
+}
+
+extern "C" int stego_corr_loss_tiled_fwd(const void* feat_tiles, const void* code_tiles, int B, int feature_samples,
+                                         int E, int D, int nslots, int ncalls, const int* slot_of_call_host,
+                                         const float* shifts_host, int pointwise, int zero_clamp, int stabilize,
+                                         float* row_partials, float* row_means, float* stats, float* cd_out,
+                                         float* fdc_out, float* loss_out, void* stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  STEGO_CHECK_ARG(feat_tiles && code_tiles && row_partials && row_means && stats && slot_of_call_host && shifts_host,
+                  "stego_corr_loss_tiled_fwd: null pointer");
+  STEGO_CHECK_ARG(!loss_out || (cd_out && fdc_out), "stego_corr_loss_tiled_fwd: loss_out needs cd_out and fdc_out");
+  TiledParams p;
+  int rc = fill_tiled_params(p, B, feature_samples, E, D, nslots, ncalls, slot_of_call_host, shifts_host, pointwise,
+                             zero_clamp, stabilize);
+  if (rc != STEGO_OK) return rc;
+  p.rowpart = row_partials; p.cd_out = cd_out; p.fd_out = fdc_out;
+  CUtensorMap tmF, tmC;
+  if ((rc = encode_tiled_maps(feat_tiles, code_tiles, p, &tmF, &tmC)) != STEGO_OK) return rc;
+  if ((rc = launch_corr_tiled<0>(tmF, tmC, p, stream)) != STEGO_OK) return rc;
+  corr_tiled_finish_kernel<<<ncalls, CT_FINISH_THREADS, 0, stream>>>(p, row_means, stats);
+  STEGO_CHECK_LAUNCH("corr_tiled_finish_kernel");
+  if (fdc_out) {
+    const long long n = 1ll * ncalls * B * p.S * p.S;
+    corr_tiled_elems_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(cd_out, fdc_out, row_means, stats,
+                                                                              loss_out, p);
+    STEGO_CHECK_LAUNCH("corr_tiled_elems_kernel");
+  }
+  return STEGO_OK;
+}
+
+extern "C" int stego_corr_loss_tiled_bwd(const void* feat_tiles, const void* code_tiles, int B, int feature_samples,
+                                         int E, int D, int nslots, int ncalls, const int* slot_of_call_host,
+                                         const float* shifts_host, int pointwise, int zero_clamp, int stabilize,
+                                         const float* stats, const float* row_means, const float* gscale,
+                                         const float* gelem, const float* gcd, float* dtiles, void* stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  STEGO_CHECK_ARG(feat_tiles && code_tiles && stats && row_means && gscale && dtiles && slot_of_call_host &&
+                  shifts_host, "stego_corr_loss_tiled_bwd: null pointer");
+  TiledParams p;
+  int rc = fill_tiled_params(p, B, feature_samples, E, D, nslots, ncalls, slot_of_call_host, shifts_host, pointwise,
+                             zero_clamp, stabilize);
+  if (rc != STEGO_OK) return rc;
+  p.stats = stats; p.rowmean = row_means; p.gscale = gscale; p.gelem = gelem; p.gcd = gcd; p.dtiles = dtiles;
+  CUtensorMap tmF, tmC;
+  if ((rc = encode_tiled_maps(feat_tiles, code_tiles, p, &tmF, &tmC)) != STEGO_OK) return rc;
+  // dB (every slot, slot 0 included for the intra call) then dA (slot 0): stream order fixes the summation order
+  if ((rc = launch_corr_tiled<2>(tmF, tmC, p, stream)) != STEGO_OK) return rc;
+  return launch_corr_tiled<1>(tmF, tmC, p, stream);
 }

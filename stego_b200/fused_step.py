@@ -91,9 +91,13 @@ class FusedStep:
         ws.dh = torch.empty(M, E, dtype=f32, device=dev) if nonlinear else None
         ws.dhb = torch.empty(M, E, dtype=bf, device=dev) if nonlinear else None
         # correspondence loss
-        ws.ftiles = torch.empty(2, spec.nslots, B, corr.TILE_ROWS, E, dtype=bf, device=dev)
-        ws.ctiles = torch.empty(2, spec.nslots, B, corr.TILE_ROWS, corr.CODE_PAD, dtype=bf, device=dev)
-        ws.partials = torch.empty(spec.ncalls, B, 8, dtype=f32, device=dev)
+        ws.ftiles = torch.empty(2, spec.nslots, B, spec.rows, E, dtype=bf, device=dev)
+        ws.ctiles = torch.empty(2, spec.nslots, B, spec.rows, corr.CODE_PAD, dtype=bf, device=dev)
+        if spec.tiled:
+            ws.partials = torch.empty(spec.ncalls, B, spec.n_tiles, spec.rows, 4, dtype=f32, device=dev)
+            ws.row_means = torch.empty(spec.ncalls, B, spec.rows, dtype=f32, device=dev)
+        else:
+            ws.partials = torch.empty(spec.ncalls, B, 8, dtype=f32, device=dev)
         ws.stats = torch.empty(spec.ncalls, 4, dtype=f32, device=dev)
         cw = float(cfg.correspondence_weight)
         wts = [cfg.pos_intra_weight * cw, cfg.pos_inter_weight * cw] + [cfg.neg_inter_weight * cw / spec.n_neg] * spec.n_neg
@@ -117,7 +121,7 @@ class FusedStep:
         ws.graph = None
         ws.eager_steps = 0
         # everything the kernels accumulate into: ONE buffer, ONE memset per step
-        sizes = dict(dlogits=B * hw * 32, dtiles=spec.nslots * B * corr.TILE_ROWS * corr.DT_LD, dall=M * P,
+        sizes = dict(dlogits=B * hw * 32, dtiles=spec.nslots * B * spec.rows * corr.DT_LD, dall=M * P,
                      dnc=n_clu * D, db_pad=P)
         total = sum(_round_up(v, 64) for v in sizes.values())
         ws.zbuf = torch.zeros(total, dtype=f32, device=dev)
@@ -179,19 +183,27 @@ class FusedStep:
         tok_pos = tok_all[B:]
         m3 = ws.M3[:B] if ws.M3 is not None else None
         p3 = ws.M3[B:] if ws.M3 is not None else None
-        _lib.check(lib.stego_sample_norm_fwd(
+        # feature_samples >= 12: the multi-tile kernels (same arguments for sampling, row means for the loss)
+        sample_fwd = lib.stego_sample_norm_tiled_fwd if spec.tiled else lib.stego_sample_norm_fwd
+        _lib.check(sample_fwd(
             _lib.ptr(tok_all), _lib.ptr(tok_pos), 1, hw * E, 1, fw * E, E, _lib.ptr(m3), _lib.ptr(p3),
             _lib.ptr(ws.c1), _lib.ptr(ws.c2), _lib.ptr(ws.perms), _lib.ptr(ws.ftiles), B, E, E, fh, fw, spec.fs,
             spec.nslots, 1, st), "stego_sample_norm_fwd")
         code_pos = ws.code[B * hw:]
-        _lib.check(lib.stego_sample_norm_fwd(
+        _lib.check(sample_fwd(
             _lib.ptr(ws.code), _lib.ptr(code_pos), 0, hw * P, 1, fw * P, P, 0, 0, _lib.ptr(ws.c1), _lib.ptr(ws.c2),
             _lib.ptr(ws.perms), _lib.ptr(ws.ctiles), B, D, corr.CODE_PAD, fh, fw, spec.fs, spec.nslots, 1, st),
             "stego_sample_norm_fwd")
-        _lib.check(lib.stego_corr_loss_fwd(
-            _lib.ptr(ws.ftiles), _lib.ptr(ws.ctiles), B, spec.fs, E, D, spec.nslots, spec.ncalls, ws.soc, ws.shf,
-            int(spec.pointwise), int(spec.zero_clamp), int(spec.stabilize), _lib.ptr(ws.partials), _lib.ptr(ws.stats),
-            0, 0, 0, st), "stego_corr_loss_fwd")
+        if spec.tiled:
+            _lib.check(lib.stego_corr_loss_tiled_fwd(
+                _lib.ptr(ws.ftiles), _lib.ptr(ws.ctiles), B, spec.fs, E, D, spec.nslots, spec.ncalls, ws.soc, ws.shf,
+                int(spec.pointwise), int(spec.zero_clamp), int(spec.stabilize), _lib.ptr(ws.partials),
+                _lib.ptr(ws.row_means), _lib.ptr(ws.stats), 0, 0, 0, st), "stego_corr_loss_tiled_fwd")
+        else:
+            _lib.check(lib.stego_corr_loss_fwd(
+                _lib.ptr(ws.ftiles), _lib.ptr(ws.ctiles), B, spec.fs, E, D, spec.nslots, spec.ncalls, ws.soc, ws.shf,
+                int(spec.pointwise), int(spec.zero_clamp), int(spec.stabilize), _lib.ptr(ws.partials),
+                _lib.ptr(ws.stats), 0, 0, 0, st), "stego_corr_loss_fwd")
         seg._mark("corr_loss_forward")
 
         # ---- probes on the detached code (train_segmentation.py:213-225): forward + backward in place
@@ -216,12 +228,19 @@ class FusedStep:
         _lib.check(lib.stego_cluster_lookup_bwd(
             _lib.ptr(ws.code), hw * P, 1, P, _lib.ptr(cl), B, D, ws.n_clu, hw, 0, 0.0, _lib.ptr(ws.one),
             _lib.ptr(ws.dnc), _lib.ptr(cl.grad), st), "stego_cluster_lookup_bwd")
-        _lib.check(lib.stego_corr_loss_bwd(
-            _lib.ptr(ws.ftiles), _lib.ptr(ws.ctiles), B, spec.fs, E, D, spec.nslots, spec.ncalls, ws.soc, ws.shf,
-            int(spec.pointwise), int(spec.zero_clamp), int(spec.stabilize), _lib.ptr(ws.stats), _lib.ptr(ws.gscale),
-            0, 0, _lib.ptr(ws.dtiles), st), "stego_corr_loss_bwd")
+        if spec.tiled:
+            _lib.check(lib.stego_corr_loss_tiled_bwd(
+                _lib.ptr(ws.ftiles), _lib.ptr(ws.ctiles), B, spec.fs, E, D, spec.nslots, spec.ncalls, ws.soc, ws.shf,
+                int(spec.pointwise), int(spec.zero_clamp), int(spec.stabilize), _lib.ptr(ws.stats),
+                _lib.ptr(ws.row_means), _lib.ptr(ws.gscale), 0, 0, _lib.ptr(ws.dtiles), st), "stego_corr_loss_tiled_bwd")
+        else:
+            _lib.check(lib.stego_corr_loss_bwd(
+                _lib.ptr(ws.ftiles), _lib.ptr(ws.ctiles), B, spec.fs, E, D, spec.nslots, spec.ncalls, ws.soc, ws.shf,
+                int(spec.pointwise), int(spec.zero_clamp), int(spec.stabilize), _lib.ptr(ws.stats),
+                _lib.ptr(ws.gscale), 0, 0, _lib.ptr(ws.dtiles), st), "stego_corr_loss_bwd")
         dall_pos = ws.dall[B * hw * P:]
-        _lib.check(lib.stego_sample_norm_bwd(
+        sample_bwd = lib.stego_sample_norm_tiled_bwd if spec.tiled else lib.stego_sample_norm_bwd
+        _lib.check(sample_bwd(
             _lib.ptr(ws.code), _lib.ptr(code_pos), hw * P, 1, fw * P, P, _lib.ptr(ws.c1), _lib.ptr(ws.c2),
             _lib.ptr(ws.perms), _lib.ptr(ws.dtiles), _lib.ptr(ws.dall), _lib.ptr(dall_pos), B, D, fh, fw, spec.fs,
             spec.nslots, 1, st), "stego_sample_norm_bwd")

@@ -366,7 +366,7 @@ class ContrastiveCorrelationLoss(nn.Module):
         coords1, coords2 = self.draw_coords(orig_feats, orig_salience, orig_salience_pos)
         B = orig_feats.shape[0]
         perms = [super_perm(B, orig_feats.device) for _ in range(cfg.neg_samples)]
-        spec = corr.LossSpec(cfg)
+        spec = corr.make_spec(cfg)
         losses, _cd_means, cd, elems = corr.corr_loss(orig_feats, orig_feats_pos, orig_code, orig_code_pos, coords1,
                                                       coords2, perms, spec, want_elems=True)
         fs = cfg.feature_samples

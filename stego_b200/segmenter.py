@@ -264,7 +264,7 @@ class LitUnsupervisedSegmenter(nn.Module):
         self.global_step = 0
         self.logged: Dict[str, torch.Tensor] = {}
         self._flat: Optional[FlatParams] = None
-        self._spec = corr.LossSpec(cfg)
+        self._spec = corr.make_spec(cfg)
         self._fused = None
         self.profile_marks = None  # optional list: bench.py --breakdown collects (name, cuda event) pairs here
 
