@@ -141,29 +141,45 @@ __device__ __forceinline__ void tma_prefetch_l2_2d(const CUtensorMap* m, int c0,
                : "memory");
 }
 
-// smem -> global tile store / fp32 reduce-add (bulk async group completion)
-__device__ __forceinline__ void tma_store_2d(const void* smem_src, const CUtensorMap* m, int c0, int c1) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];\n" ::"l"(
+// smem -> global tile store / fp32 reduce-add (bulk async group completion); the source is a shared-memory address
+// (smem_u32) or pointer
+__device__ __forceinline__ void tma_store_3d(uint32_t smem_src, const CUtensorMap* m, int c0, int c1, int c2) {
+  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];\n" ::"l"(
                    reinterpret_cast<uint64_t>(m)),
-               "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
+               "r"(smem_src), "r"(c0), "r"(c1), "r"(c2)
                : "memory");
 }
 __device__ __forceinline__ void tma_store_3d(const void* smem_src, const CUtensorMap* m, int c0, int c1, int c2) {
-  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];\n" ::"l"(
+  tma_store_3d(smem_u32(smem_src), m, c0, c1, c2);
+}
+__device__ __forceinline__ void tma_reduce_add_3d(uint32_t smem_src, const CUtensorMap* m, int c0, int c1, int c2) {
+  asm volatile("cp.reduce.async.bulk.tensor.3d.global.shared::cta.add.bulk_group [%0, {%2, %3, %4}], [%1];\n" ::"l"(
                    reinterpret_cast<uint64_t>(m)),
-               "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2)
+               "r"(smem_src), "r"(c0), "r"(c1), "r"(c2)
                : "memory");
 }
-__device__ __forceinline__ void tma_reduce_add_2d(const void* smem_src, const CUtensorMap* m, int c0, int c1) {
-  asm volatile("cp.reduce.async.bulk.tensor.2d.global.shared::cta.add.bulk_group [%0, {%2, %3}], [%1];\n" ::"l"(
-                   reinterpret_cast<uint64_t>(m)),
-               "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
-               : "memory");
+
+// shared-memory stores by 32-bit shared address
+__device__ __forceinline__ void st_shared_b32(uint32_t addr, uint32_t v) {
+  asm volatile("st.shared.b32 [%0], %1;\n" ::"r"(addr), "r"(v) : "memory");
+}
+__device__ __forceinline__ void st_shared_v2_f32(uint32_t addr, float a, float b) {
+  asm volatile("st.shared.v2.f32 [%0], {%1, %2};\n" ::"r"(addr), "f"(a), "f"(b) : "memory");
 }
 __device__ __forceinline__ void tma_commit_group() { asm volatile("cp.async.bulk.commit_group;\n" ::: "memory"); }
 template <int kPending>
 __device__ __forceinline__ void tma_wait_group_read() {
   asm volatile("cp.async.bulk.wait_group.read %0;\n" ::"n"(kPending) : "memory");
+}
+// full completion (the global writes done), not just the shared-memory read
+template <int kPending>
+__device__ __forceinline__ void tma_wait_group() {
+  asm volatile("cp.async.bulk.wait_group %0;\n" ::"n"(kPending) : "memory");
+}
+
+// named barrier over a subset of the CTA's warps (id 1..15; id 0 is __syncthreads)
+__device__ __forceinline__ void named_bar_sync(int id, int threads) {
+  asm volatile("bar.sync %0, %1;\n" ::"r"(id), "r"(threads) : "memory");
 }
 
 // ----------------------------------------------------------------------------------------------

@@ -8,13 +8,21 @@
 //   * segmentation head (reference: src/modules.py:73-81 cluster1/cluster2 1x1 convs) forward,
 //     dgrad (B operand MN-major) and wgrad (both operands MN-major, split-K + fp32 atomics).
 //
-// Structure: persistent CTAs (one per SM), 384 threads = three warpgroups:
-//   warpgroup 0     TMA producer (one thread: cp.async.bulk.tensor -> 128B-swizzled smem ring, mbarrier expect_tx)
-//   warpgroups 1,2  MMA + epilogue, rows 0..63 and 64..127 of the 128 x BN tile: wgmma with both operands in shared
-//                   memory, fp32 accumulators in registers (BN / 2 per thread), then bias / GELU / ReLU / residual and
-//                   the stores straight from the accumulator registers.
-// Operand tiles are 128 x 64 (A) and BN x 64 (B) bf16; accumulation fp32.
+// Structure: persistent CTAs (one per SM), 384 threads = three warpgroups, ping-pong schedule:
+//   warpgroup 0     TMA producer (one thread: cp.async.bulk.tensor -> 128B-swizzled smem ring, mbarrier expect_tx),
+//                   loading the CTA's tiles in order
+//   warpgroups 1,2  MMA + epilogue.  The CTA's i-th tile belongs to MMA warpgroup i % 2, which computes the whole
+//                   128 x 128 tile (two m64n128 wgmmas per k16 slice, 128 fp32 accumulators per thread).  The two take
+//                   turns on the tensor cores (an mbarrier hand-over after each mainloop), so one runs its mainloop
+//                   while the other runs its epilogue.
+// Epilogues: bias / GELU / ReLU in registers, then either
+//   * TMA: the tile is staged in 128B-swizzled shared memory in 16 KB column chunks and leaves by TMA bulk stores, or
+//     by TMA fp32 reduce-adds when the residual is the output itself (x += ...); no global loads; or
+//   * registers: paired stores straight from the accumulator fragments, for what TMA cannot express: split-K atomics,
+//     the patch-embed row remap, a residual other than the output, outputs (or rows of N outputs) not 16-byte aligned.
+// Operand tiles are 128 x 64 bf16 (A and B); accumulation fp32.
 #include <stdlib.h>
+#include <string.h>
 
 #include "common.cuh"
 #include "epilogue.cuh"
@@ -23,8 +31,11 @@
 namespace stego {
 
 constexpr int GEMM_BM = 128;
+constexpr int GEMM_BN = 128;
 constexpr int GEMM_BK = 64;
 constexpr int GEMM_THREADS = 384;
+constexpr uint32_t GEMM_STAGE_BYTES = (GEMM_BM + GEMM_BN) * GEMM_BK * 2;  // 32 KB
+constexpr uint32_t GEMM_CHUNK_BYTES = GEMM_BM * 128;                        // one [128 rows][128 B] staging chunk
 
 struct GemmParams {
   int M, N, K;        // logical GEMM sizes; K is the reduction length
@@ -40,19 +51,16 @@ struct GemmParams {
   int row_div;        // >0: patch-embed mode: out_row = r + r/row_div + 1, residual row = r % row_div + 1
   int atomic;         // 1: fp32 atomicAdd into out (split-K)
   int vec_ok;         // host-verified alignment for paired (8-byte fp32 / 4-byte bf16) accesses of out / residual / bias
+  int reduce_add;     // TMA epilogue: 1 = out += tile (residual is out), 0 = out = tile
   int batch;          // independent GEMMs of the same shape (third tensor-map dimension); 1 = plain GEMM
   long long out_bs;   // element stride between the outputs / residuals of consecutive batch entries
   long long res_bs;
 };
 
-// Epilogue of one warpgroup's 64 x BN accumulator, straight from the wgmma fragment: each thread holds rows
-// row_top and row_top + 8, and column pairs 8 c + 2 (lane % 4) + {0, 1}.
+// Bias and activation on one 64 x BN accumulator fragment: each thread holds column pairs 8 c + 2 (lane % 4) + {0, 1}
+// of rows row_top and row_top + 8.
 template <int BN>
-__device__ __forceinline__ void gemm_epilogue(float (&acc)[BN / 2], const GemmParams& p, int row_top, int col_base,
-                                              int tb) {
-  void* const outp = p.out_bf16 ? static_cast<void*>(reinterpret_cast<bf16*>(p.out) + tb * p.out_bs)
-                                : static_cast<void*>(reinterpret_cast<float*>(p.out) + tb * p.out_bs);
-  const float* const resp = p.residual ? p.residual + tb * p.res_bs : nullptr;
+__device__ __forceinline__ void gemm_bias_act(float (&acc)[BN / 2], const GemmParams& p, int col_base) {
   if (p.bias != nullptr) {
 #pragma unroll
     for (int c = 0; c < BN / 8; ++c) {
@@ -82,6 +90,16 @@ __device__ __forceinline__ void gemm_epilogue(float (&acc)[BN / 2], const GemmPa
 #pragma unroll
     for (int j = 0; j < BN / 2; ++j) acc[j] = fmaxf(acc[j], 0.0f);
   }
+}
+
+// Register epilogue of one 64 x BN accumulator fragment (after gemm_bias_act): residual, then paired stores or
+// atomics straight from the fragment, rows row_top and row_top + 8.
+template <int BN>
+__device__ __forceinline__ void gemm_store_regs(const float (&acc)[BN / 2], const GemmParams& p, int row_top,
+                                                int col_base, int tb) {
+  void* const outp = p.out_bf16 ? static_cast<void*>(reinterpret_cast<bf16*>(p.out) + tb * p.out_bs)
+                                : static_cast<void*>(reinterpret_cast<float*>(p.out) + tb * p.out_bs);
+  const float* const resp = p.residual ? p.residual + tb * p.res_bs : nullptr;
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     const int row = row_top + 8 * h;
@@ -136,27 +154,91 @@ __device__ __forceinline__ void gemm_epilogue(float (&acc)[BN / 2], const GemmPa
   }
 }
 
-template <int BN, int kStages, bool A_MN, bool B_MN>
+// TMA epilogue of one warpgroup's 128 x 128 tile (after gemm_bias_act).  The tile leaves in column chunks of 128 B per
+// row (64 bf16 or 32 fp32 columns), each staged as a [128 rows][128 B] SWIZZLE_128B box — the layout the output tensor
+// map describes — in one of the warpgroup's two 16 KB buffers, alternating, so writing chunk c overlaps the store of
+// chunk c - 1.  Every chunk is its own bulk group: before buffer reuse the issuing thread waits only until the store
+// two chunks back has READ its buffer.  Rows past M and columns past N are clipped by TMA.  The named barrier (one
+// per warpgroup, 128 threads) only orders the warpgroup's own staging writes against its issuing thread.
+template <bool kBf16>
+__device__ __forceinline__ void gemm_store_tma(const float (&acc)[2][GEMM_BN / 2], const GemmParams& p,
+                                               const CUtensorMap* tm_out, uint32_t stage, int bar_id, bool issuer,
+                                               int m0, int n0, int tb) {
+  constexpr int kCols = kBf16 ? 64 : 32;  // columns per chunk
+  const int lane = threadIdx.x & 31;
+  const int wq = (threadIdx.x >> 5) & 3;
+  const uint32_t q = lane & 3;
+  const uint32_t swz = (lane >> 2) & 7;  // row & 7 of every row this thread holds
+#pragma unroll
+  for (int ch = 0; ch < GEMM_BN / kCols; ++ch) {
+    const uint32_t buf = stage + (ch & 1) * GEMM_CHUNK_BYTES;
+    if (issuer) tma_wait_group_read<1>();
+    named_bar_sync(bar_id, 128);
+    // this thread's rows are 16 wq + lane / 4 + {0, 8, 64, 72}, all with the same row & 7
+    const uint32_t rbase = buf + (16 * wq + (lane >> 2)) * 128u;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+#pragma unroll
+      for (int e2 = 0; e2 < 2; ++e2) {
+        const uint32_t rp = rbase + (64 * h + 8 * e2) * 128u;
+        if constexpr (kBf16) {
+          // 64 columns: 8-column group j is 16-byte unit j of the row; this thread's pair sits at byte 4 q of it
+#pragma unroll
+          for (int j = 0; j < 8; ++j) {
+            const int c = 8 * ch + j;
+            st_shared_b32(rp + (((uint32_t)j ^ swz) << 4) + 4 * q,
+                          pack_bf16x2(acc[h][4 * c + 2 * e2], acc[h][4 * c + 2 * e2 + 1]));
+          }
+        } else {
+          // 32 columns: 8-column group j covers 16-byte units 2 j and 2 j + 1; the pair sits at byte 8 q of the two
+#pragma unroll
+          for (int j = 0; j < 4; ++j) {
+            const int c = 4 * ch + j;
+            const uint32_t unit = 2 * j + (q >> 1);
+            st_shared_v2_f32(rp + ((unit ^ swz) << 4) + 8 * (q & 1), acc[h][4 * c + 2 * e2],
+                             acc[h][4 * c + 2 * e2 + 1]);
+          }
+        }
+      }
+    }
+    fence_proxy_async_smem();  // generic-proxy smem writes -> visible to the TMA (async proxy) read
+    named_bar_sync(bar_id, 128);
+    if (issuer) {
+      const int col = n0 + ch * kCols;
+      if (p.reduce_add) tma_reduce_add_3d(buf, tm_out, col, m0, tb);
+      else tma_store_3d(buf, tm_out, col, m0, tb);
+      tma_commit_group();
+    }
+  }
+}
+
+// Advance a ring position by n stages.
+template <int kStages>
+__device__ __forceinline__ void ring_advance(uint32_t& stage, uint32_t& phase, int n) {
+  stage += n;
+  while (stage >= kStages) { stage -= kStages; phase ^= 1u; }
+}
+
+template <int kStages, bool A_MN, bool B_MN, bool kTmaEpi>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
-gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, GemmParams p) {
+gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                 const __grid_constant__ CUtensorMap tmOut, GemmParams p) {
   constexpr uint32_t A_BYTES = GEMM_BM * GEMM_BK * 2;  // 16 KB
-  constexpr uint32_t B_BYTES = BN * GEMM_BK * 2;
-  constexpr uint32_t STAGE_BYTES = A_BYTES + B_BYTES;
-  static_assert(BN == 128 || BN == 256, "BN must be 128 or 256");
-  static_assert(BN == 128 || (!A_MN && !B_MN), "256-wide tiles are K-major only");
-  constexpr int kBBox = 128;  // K-major B box rows
+  constexpr uint32_t STAGE_BYTES = GEMM_STAGE_BYTES;
 
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kStages * STAGE_BYTES);
+  uint8_t* staging = smem + kStages * STAGE_BYTES;  // kTmaEpi: two 16 KB chunk buffers per MMA warpgroup
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(staging + (kTmaEpi ? 4 * GEMM_CHUNK_BYTES : 0));
   uint64_t* empty_bar = full_bar + kStages;
+  uint64_t* turn_bar = empty_bar + kStages;  // turn_bar[w]: MMA warpgroup w may start its next mainloop
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int wg = warp >> 2;  // 0 producer, 1..2 MMA warpgroups
 
   const int tiles_m = (p.M + GEMM_BM - 1) / GEMM_BM;
-  const int tiles_n = (p.N + BN - 1) / BN;
+  const int tiles_n = (p.N + GEMM_BN - 1) / GEMM_BN;
   const int num_kb = (p.K + GEMM_BK - 1) / GEMM_BK;  // K tail: TMA zero-fills out-of-bounds
   const int tiles_per_batch = tiles_m * tiles_n * p.splits;
   const int total_tiles = tiles_per_batch * p.batch;
@@ -166,10 +248,13 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
+    if (kTmaEpi) tma_prefetch_desc(&tmOut);
     for (int s = 0; s < kStages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 2);  // one arrive per MMA warpgroup
+      mbar_init(&empty_bar[s], 1);  // every stage is consumed by exactly one MMA warpgroup
     }
+    mbar_init(&turn_bar[0], 1);
+    mbar_init(&turn_bar[1], 1);
     fence_barrier_init();
   }
   __syncthreads();
@@ -199,13 +284,11 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
               tma_load_3d(sa + blk * 8192, &tmA, &full_bar[stage], tm * GEMM_BM + blk * 64, kb * GEMM_BK, tb);
           }
           if (!B_MN) {
-#pragma unroll
-            for (int blk = 0; blk < BN / kBBox; ++blk)  // tensor-map box = kBBox rows
-              tma_load_3d(sb + blk * (kBBox * 128), &tmB, &full_bar[stage], kb * GEMM_BK, tn * BN + blk * kBBox, tb);
+            tma_load_3d(sb, &tmB, &full_bar[stage], kb * GEMM_BK, tn * GEMM_BN, tb);
           } else {
 #pragma unroll
-            for (int blk = 0; blk < BN / 64; ++blk)
-              tma_load_3d(sb + blk * 8192, &tmB, &full_bar[stage], tn * BN + blk * 64, kb * GEMM_BK, tb);
+            for (int blk = 0; blk < GEMM_BN / 64; ++blk)
+              tma_load_3d(sb + blk * 8192, &tmB, &full_bar[stage], tn * GEMM_BN + blk * 64, kb * GEMM_BK, tb);
           }
           if (++stage == kStages) { stage = 0; phase ^= 1u; }
         }
@@ -214,56 +297,87 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   } else {
     // ===================== MMA warpgroups =====================
     warpgroup_reg_alloc<232>();
-    const int mwg = wg - 1;  // rows 64 * mwg .. of every tile
-    // K-major A: rows 64.. start 64 x 128 B further; MN-major A: the second 64-wide M block, also 8 KB further
+    const int mwg = wg - 1;  // owns the CTA's tiles i with i % 2 == mwg
+    // rows 64.. of the A tile start 8 KB further in both layouts (K-major: 64 rows x 128 B; MN-major: the second
+    // 64-wide M block)
     constexpr uint32_t DESC_HI = smem_desc_hi_sw128(1024);
     constexpr uint32_t A_KSTEP = A_MN ? (2048u >> 4) : (32u >> 4);  // low-word step per k16 slice
     constexpr uint32_t B_KSTEP = B_MN ? (2048u >> 4) : (32u >> 4);
-    const uint32_t a_lo0 = smem_desc_lo(smem_u32(smem) + mwg * 8192u, 8192u);
+    constexpr uint32_t A_HALF = 8192u >> 4;
+    const uint32_t a_lo0 = smem_desc_lo(smem_u32(smem), 8192u);
     const uint32_t b_lo0 = smem_desc_lo(smem_u32(smem) + A_BYTES, 8192u);
     const bool leader = (threadIdx.x & 127) == 0;
+    const int wq = (threadIdx.x >> 5) & 3;
     uint32_t stage = 0, phase = 0;
-    float acc[BN / 2];
-    for (int t = sched_start; t < total_tiles; t += sched_step) {
+    float acc[2][GEMM_BN / 2];
+    int i = 0;
+    for (int t = sched_start; t < total_tiles; t += sched_step, ++i) {
       const int tb = t / tiles_per_batch, tl = t % tiles_per_batch;
       const int split = tl % p.splits;
       const int tn = (tl / p.splits) % tiles_n;
       const int tm = tl / (p.splits * tiles_n);
       const int kb0 = split * p.kb_per_split;
       const int kb1 = min(num_kb, kb0 + p.kb_per_split);
+      if ((i & 1) != mwg) {  // the partner's tile: its k-blocks pass through the ring in between
+        ring_advance<kStages>(stage, phase, kb1 - kb0);
+        continue;
+      }
+      // Wait for the turn: the partner has issued all MMAs of the tile before this one.  Tile i - 1 always exists,
+      // so a warpgroup never waits on a partner that has run out of tiles; the hand-over after the CTA's last tile
+      // completes a phase nobody waits for.
+      if (i > 0) mbar_wait(&turn_bar[mwg], ((i - 1) >> 1) & 1);
 #pragma unroll
-      for (int j = 0; j < BN / 2; ++j) acc[j] = 0.f;
+      for (int j = 0; j < GEMM_BN / 2; ++j) { acc[0][j] = 0.f; acc[1][j] = 0.f; }
       uint32_t prev_stage = 0;
       for (int kb = kb0; kb < kb1; ++kb) {
         mbar_wait(&full_bar[stage], phase);
         const uint32_t a_lo = a_lo0 + stage * (STAGE_BYTES >> 4);
         const uint32_t b_lo = b_lo0 + stage * (STAGE_BYTES >> 4);
-        fence_operands(acc);
+        fence_operands(acc[0]);
+        fence_operands(acc[1]);
         wgmma_fence();
 #pragma unroll
-        for (uint32_t k = 0; k < GEMM_BK / 16; ++k)
-          wgmma_ss<BN, A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, smem_desc_join(a_lo + k * A_KSTEP, DESC_HI),
-                                                  smem_desc_join(b_lo + k * B_KSTEP, DESC_HI), 1u);
+        for (uint32_t k = 0; k < GEMM_BK / 16; ++k) {
+          const uint64_t db = smem_desc_join(b_lo + k * B_KSTEP, DESC_HI);
+#pragma unroll
+          for (uint32_t h = 0; h < 2; ++h)
+            wgmma_ss<GEMM_BN, A_MN ? 1 : 0, B_MN ? 1 : 0>(
+                acc[h], smem_desc_join(a_lo + h * A_HALF + k * A_KSTEP, DESC_HI), db, 1u);
+        }
         wgmma_commit();
         wgmma_wait<1>();  // the previous k-block's MMAs have retired: its smem slot is reusable
         if (kb > kb0 && leader) mbar_arrive(&empty_bar[prev_stage]);
         prev_stage = stage;
         if (++stage == kStages) { stage = 0; phase ^= 1u; }
       }
+      if (leader) mbar_arrive(&turn_bar[mwg ^ 1]);  // hand the tensor cores to the partner
       wgmma_wait<0>();
-      fence_operands(acc);
+      fence_operands(acc[0]);
+      fence_operands(acc[1]);
       if (kb1 > kb0 && leader) mbar_arrive(&empty_bar[prev_stage]);
-      const int wq = (threadIdx.x >> 5) & 3;
-      gemm_epilogue<BN>(acc, p, tm * GEMM_BM + mwg * 64 + wq * 16 + (lane >> 2), tn * BN + 2 * (lane & 3), tb);
+      const int col_base = tn * GEMM_BN + 2 * (lane & 3);
+      gemm_bias_act<GEMM_BN>(acc[0], p, col_base);
+      gemm_bias_act<GEMM_BN>(acc[1], p, col_base);
+      if constexpr (kTmaEpi) {
+        const uint32_t st = smem_u32(staging) + mwg * 2 * GEMM_CHUNK_BYTES;
+        if (p.out_bf16) gemm_store_tma<true>(acc, p, &tmOut, st, 1 + mwg, leader, tm * GEMM_BM, tn * GEMM_BN, tb);
+        else gemm_store_tma<false>(acc, p, &tmOut, st, 1 + mwg, leader, tm * GEMM_BM, tn * GEMM_BN, tb);
+      } else {
+        const int row_top = tm * GEMM_BM + wq * 16 + (lane >> 2);
+        gemm_store_regs<GEMM_BN>(acc[0], p, row_top, col_base, tb);
+        gemm_store_regs<GEMM_BN>(acc[1], p, row_top + 64, col_base, tb);
+      }
     }
+    if (kTmaEpi && leader) tma_wait_group<0>();  // every store has completed before the CTA (and its smem) goes away
   }
 }
 
-template <int BN, int kStages, bool A_MN, bool B_MN>
-static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, cudaStream_t stream) {
-  constexpr size_t smem = size_t(kStages) * (GEMM_BM * GEMM_BK * 2 + BN * GEMM_BK * 2) + 1024 + 256;
+template <int kStages, bool A_MN, bool B_MN, bool kTmaEpi>
+static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmOut, const GemmParams& p,
+                       cudaStream_t stream) {
+  constexpr size_t smem = size_t(kStages) * GEMM_STAGE_BYTES + (kTmaEpi ? 4 * GEMM_CHUNK_BYTES : 0) + 1024 + 256;
   static_assert(smem <= 232448, "exceeds the 227 KB of shared memory a CTA can opt into");
-  auto kern = gemm_bf16_kernel<BN, kStages, A_MN, B_MN>;
+  auto kern = gemm_bf16_kernel<kStages, A_MN, B_MN, kTmaEpi>;
   static bool configured = false;
   if (!configured) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
@@ -271,12 +385,20 @@ static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const Gem
     configured = true;
   }
   const int tiles_m = (p.M + GEMM_BM - 1) / GEMM_BM;
-  const int tiles_n = (p.N + BN - 1) / BN;
+  const int tiles_n = (p.N + GEMM_BN - 1) / GEMM_BN;
   const int tiles = tiles_m * tiles_n * p.splits * p.batch;
   const int grid = tiles < num_sms() ? tiles : num_sms();
-  kern<<<grid, GEMM_THREADS, smem, stream>>>(tmA, tmB, p);
+  kern<<<grid, GEMM_THREADS, smem, stream>>>(tmA, tmB, tmOut, p);
   STEGO_CHECK_LAUNCH("gemm_bf16_kernel launch");
   return STEGO_OK;
+}
+
+// Ring depth: 6 x 32 KB stages, or 5 when the TMA epilogue's 64 KB of staging buffers share the CTA's shared memory.
+template <bool A_MN, bool B_MN>
+static int launch_gemm_epi(bool tma_epi, const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmOut,
+                           const GemmParams& p, cudaStream_t stream) {
+  if (tma_epi) return launch_gemm<5, A_MN, B_MN, true>(tmA, tmB, tmOut, p, stream);
+  return launch_gemm<6, A_MN, B_MN, false>(tmA, tmB, tmOut, p, stream);
 }
 
 }  // namespace stego
@@ -323,11 +445,17 @@ static int gemm_impl(const void* A, int lda, long long a_bs, int a_mn_major, con
   p.vec_ok = ((reinterpret_cast<uintptr_t>(out) % pair) == 0) && (ldo % 2 == 0) && (out_bs % 2 == 0) &&
              (residual == nullptr || ((reinterpret_cast<uintptr_t>(residual) % 8) == 0 && ldr % 2 == 0 && res_bs % 2 == 0)) &&
              (bias == nullptr || (reinterpret_cast<uintptr_t>(bias) % 8) == 0);
-  // Tile shape: 128 x 256 for wide-N K-major linears (qkv: N = 3E, fc1: N = 4E; halves the A re-reads from L2),
-  // 128 x 128 for everything else (incl. MN-major operands and split-K).
-  const bool wide = !a_mn_major && !b_mn_major && splits == 1 && N >= 1024;
+  // Epilogue: TMA stores (or fp32 TMA reduce-adds for out += ..., the residual being the output itself) whenever a
+  // tensor map can describe the output: no split-K atomics, no row remap, 16-byte aligned base and strides, and rows
+  // of whole 16-byte units — with N * size not a multiple of 16 B, the store's last 16-byte unit of a row wrote the
+  // padding columns after N (zeros) on the H100, and callers keep data there (the head's [M][72] code rows, N = 70).
+  const bool in_place = residual != nullptr && residual == out && ldr == ldo && !out_bf16;
+  const bool tma_epi = !atomic_out && row_div == 0 && (residual == nullptr || in_place) &&
+                       (reinterpret_cast<uintptr_t>(out) % 16) == 0 && (static_cast<size_t>(ldo) * esz) % 16 == 0 &&
+                       (static_cast<size_t>(out_bs) * esz) % 16 == 0 && (static_cast<size_t>(N) * esz) % 16 == 0;
+  p.reduce_add = tma_epi && in_place;
 
-  CUtensorMap tmA, tmB;
+  CUtensorMap tmA, tmB, tmOut;
   int rc;
   {
     // K-major: tensor is [batch][M][K] (inner = K). MN-major: tensor is [batch][K][M] (inner = M).
@@ -339,14 +467,23 @@ static int gemm_impl(const void* A, int lda, long long a_bs, int a_mn_major, con
   {
     uint64_t dims[3] = {b_mn_major ? (uint64_t)N : (uint64_t)K, b_mn_major ? (uint64_t)K : (uint64_t)N, (uint64_t)batch};
     uint64_t str[2] = {(uint64_t)ldb * 2, (uint64_t)b_bs * 2};
-    uint32_t box[3] = {64, b_mn_major ? 64u : 128u, 1};  // rows per B box: must match the kernel's kBBox
+    uint32_t box[3] = {64, b_mn_major ? 64u : (uint32_t)GEMM_BN, 1};
     if ((rc = make_tmap_bf16(&tmB, B, 3, dims, str, box)) != STEGO_OK) return rc;
   }
-  if (wide) return launch_gemm<256, 4, false, false>(tmA, tmB, p, stream);
-  if (!a_mn_major && !b_mn_major) return launch_gemm<128, 6, false, false>(tmA, tmB, p, stream);
-  if (!a_mn_major && b_mn_major) return launch_gemm<128, 6, false, true>(tmA, tmB, p, stream);
-  if (a_mn_major && b_mn_major) return launch_gemm<128, 6, true, true>(tmA, tmB, p, stream);
-  return launch_gemm<128, 6, true, false>(tmA, tmB, p, stream);
+  if (tma_epi) {
+    // exactly [batch][M][N]: TMA clips the stores of ragged tiles at M and N, never touching padding columns
+    uint64_t dims[3] = {(uint64_t)N, (uint64_t)M, (uint64_t)batch};
+    uint64_t str[2] = {(uint64_t)ldo * esz, (uint64_t)out_bs * esz};
+    uint32_t box[3] = {(uint32_t)(128 / esz), (uint32_t)GEMM_BM, 1};  // one staging chunk: [128 rows][128 B]
+    rc = out_bf16 ? make_tmap_bf16(&tmOut, out, 3, dims, str, box) : make_tmap_f32(&tmOut, out, 3, dims, str, box);
+    if (rc != STEGO_OK) return rc;
+  } else {
+    memset(&tmOut, 0, sizeof(tmOut));  // unused by the register epilogue
+  }
+  if (!a_mn_major && !b_mn_major) return launch_gemm_epi<false, false>(tma_epi, tmA, tmB, tmOut, p, stream);
+  if (!a_mn_major && b_mn_major) return launch_gemm_epi<false, true>(tma_epi, tmA, tmB, tmOut, p, stream);
+  if (a_mn_major && b_mn_major) return launch_gemm_epi<true, true>(tma_epi, tmA, tmB, tmOut, p, stream);
+  return launch_gemm_epi<true, false>(tma_epi, tmA, tmB, tmOut, p, stream);
 }
 
 // C-ABI: see include/stego_b200.h for the contract.

@@ -98,6 +98,11 @@ int make_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t*
   return make_tmap(CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, out, base, rank, dims, strides_bytes, box);
 }
 
+int make_tmap_f32(CUtensorMap* out, const void* base, int rank, const uint64_t* dims,
+                  const uint64_t* strides_bytes, const uint32_t* box) {
+  return make_tmap(CU_TENSOR_MAP_DATA_TYPE_FLOAT32, out, base, rank, dims, strides_bytes, box);
+}
+
 }  // namespace stego
 
 extern "C" const char* stego_last_error(void) { return stego::g_err; }
