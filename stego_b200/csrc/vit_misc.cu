@@ -81,7 +81,10 @@ layernorm_kernel(const float* __restrict__ x, const float* __restrict__ gamma, c
     v[i] = xr[lane + 32 * i];
     s += (v[i].x + v[i].y) + (v[i].z + v[i].w);
   }
-  const float mean = warp_sum(s) * (1.0f / E);
+  // __fmul_rn: the mean is rounded once and every `x - mean` subtracts that value.  A plain `sum * (1/E)` is contracted
+  // into each `x - mean` as fma(sum, -1/E, x), which keeps the error of the inexact 1/E (E = 384, 768) unrounded, so a
+  // constant row did not centre to exactly 0 and came out as beta - 1e-4 gamma instead of beta.
+  const float mean = __fmul_rn(warp_sum(s), 1.0f / E);
   float q = 0.f;
 #pragma unroll
   for (int i = 0; i < V4; ++i) {
@@ -137,7 +140,7 @@ layernorm_gap_kernel(const float* __restrict__ x, const float* __restrict__ gamm
       v[i] = xr[lane + 32 * i];
       s += (v[i].x + v[i].y) + (v[i].z + v[i].w);
     }
-    const float mean = warp_sum(s) * (1.0f / E);
+    const float mean = __fmul_rn(warp_sum(s), 1.0f / E);  // rounded once, as in layernorm_kernel
     float q = 0.f;
 #pragma unroll
     for (int i = 0; i < V4; ++i) {
