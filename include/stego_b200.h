@@ -228,7 +228,7 @@ STEGO_API int stego_linear_probe_ce(const float* code, long long ld_code, int C,
  *   lin_log_probs = log_softmax(linear_probe(code_up), 1);  clu_log_probs = cluster_probe(code_up, alpha, log_probs=True)
  * evaluated per output pixel from the LOW-RES code (the [B,C,H,W] upsampled tensor is never materialised).
  *   code: tokens-major low-res code [B*h*w][ld_code] fp32; lin_weight [n_lin][C], lin_bias [n_lin], clusters [n_clu][C];
- *   lr_scratch: [B*h*w][72] floats.  Outputs (each may be null): log-probabilities [B][n][H][W] fp32 and
+ *   lr_scratch: [B*h*w][80] floats, 8-byte aligned (low-res logits, centroid dots, fp64 Gram entries).  Outputs (each may be null): log-probabilities [B][n][H][W] fp32 and
  *   per-pixel argmax maps [B][H][W] uint8.  C <= 96, n_lin, n_clu <= 32, H >= h, W >= w.
  * Optional, fused (src/eval_segmentation.py:124-126,138-139; src/utils.py:219-229):
  *   code_flip  the code of the horizontally flipped images: the kernel evaluates (code + flip(code_flip)) / 2 (flip-TTA);

@@ -8,7 +8,10 @@
 //   * linear probe:  conv1x1(interp(code)) == interp(conv1x1(code))  -> interpolate the 27 low-res logits;
 //   * cluster probe: <interp(code), c_k> == interp(<code, c_k>)      -> interpolate the low-res dot products with the
 //     normalised centroids; ||interp(code)||^2 = sum_{t,t'} w_t w_t' <code_t, code_t'> needs only the Gram
-//     entries between neighbouring low-res pixels (self, right, down, down-right, down-left).
+//     entries between neighbouring low-res pixels (self, right, down, down-right, down-left).  Those entries and their
+//     combination are fp64: where neighbouring codes nearly cancel (a class edge where the code flips direction) the
+//     norm is a small difference of large terms, and in fp32 its error would grow with the square of
+//     sum_t w_t |code_t| / ||interp(code)|| instead of linearly, as it does when the code is upsampled first.
 // Two kernels: a per-low-res-pixel preparation (warp per pixel) and the per-output-pixel evaluation, which is
 // bound by writing the two [B,n,H,W] fp32 log-probability maps (HBM): 453 MB per 1024x2048 image.
 // Also fused here (src/eval_segmentation.py:124-126, 138-139; src/utils.py:219-229):
@@ -21,8 +24,19 @@
 
 namespace stego {
 
-constexpr int EV_LD = 72;  // floats per low-res pixel: [0,32) linear logits, [32,64) centroid dots, 64.. Gram entries
-constexpr int EV_SS = 64, EV_R = 65, EV_D = 66, EV_DR = 67, EV_DL = 68;
+constexpr int EV_LD = 80;  // floats per low-res pixel: [0,32) linear logits, [32,64) centroid dots, [64,74) Gram entries
+constexpr int EV_G = 64;   // the five fp64 Gram entries (self, right, down, down-right, down-left) start at this float
+constexpr int EV_SS = 0, EV_R = 1, EV_D = 2, EV_DR = 3, EV_DL = 4;  // their index among those doubles
+
+__device__ __forceinline__ double warp_sum_f64(double v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+
+__device__ __forceinline__ const double* ev_grams(const float* cell) {
+  return reinterpret_cast<const double*>(cell + EV_G);
+}
 
 struct EvalPrepParams {
   const float* code;   // [B*h*w][ld] tokens-major
@@ -85,16 +99,17 @@ eval_prep_kernel(EvalPrepParams p) {
         ndl[k] = 0.5f * (ndl[k] + ((ok && hd && hl) ? fp[(p.w + 1) * p.ld + c] : 0.f));
       }
     }
-    float g0 = 0.f, g1 = 0.f, g2 = 0.f, g3 = 0.f, g4 = 0.f;
+    double g0 = 0.0, g1 = 0.0, g2 = 0.0, g3 = 0.0, g4 = 0.0;  // products of fp32 values are exact in fp64
 #pragma unroll
     for (int k = 0; k < 3; ++k) {
-      g0 = fmaf(xr[k], xr[k], g0);
-      g1 = fmaf(xr[k], nr[k], g1);
-      g2 = fmaf(xr[k], nd[k], g2);
-      g3 = fmaf(xr[k], ndr[k], g3);
-      g4 = fmaf(xr[k], ndl[k], g4);
+      const double x = xr[k];
+      g0 = fma(x, x, g0);
+      g1 = fma(x, (double)nr[k], g1);
+      g2 = fma(x, (double)nd[k], g2);
+      g3 = fma(x, (double)ndr[k], g3);
+      g4 = fma(x, (double)ndl[k], g4);
     }
-    g0 = warp_sum(g0); g1 = warp_sum(g1); g2 = warp_sum(g2); g3 = warp_sum(g3); g4 = warp_sum(g4);
+    g0 = warp_sum_f64(g0); g1 = warp_sum_f64(g1); g2 = warp_sum_f64(g2); g3 = warp_sum_f64(g3); g4 = warp_sum_f64(g4);
     float dl = bk, dc = 0.f;
 #pragma unroll
     for (int k = 0; k < 3; ++k) {
@@ -111,7 +126,10 @@ eval_prep_kernel(EvalPrepParams p) {
     float* o = p.lr + r * EV_LD;
     o[lane] = dl;
     o[32 + lane] = dc;
-    if (lane == 0) { o[EV_SS] = g0; o[EV_R] = g1; o[EV_D] = g2; o[EV_DR] = g3; o[EV_DL] = g4; }
+    if (lane == 0) {
+      double* og = reinterpret_cast<double*>(o + EV_G);
+      og[EV_SS] = g0; og[EV_R] = g1; og[EV_D] = g2; og[EV_DR] = g3; og[EV_DL] = g4;
+    }
   }
 }
 
@@ -144,15 +162,15 @@ __device__ __forceinline__ void ev_src_index(int dst, float scale, int in_size, 
 // round 2: 64 x 16 tiles in four passes under a 120-register cap, two CTAs per SM: 1.35 ms instead of 1.00 ms per 4 frames.)
 constexpr int EVT_W = 64, EVT_ROWS = 4, EVT_PASSES = 1, EVT_H = EVT_ROWS * EVT_PASSES;
 
-// Gram entry <code_p, code_q> for box-relative low-res pixels p, q that are equal or 8-neighbours
-__device__ __forceinline__ float ev_gram(const float* slr, int bw, int py, int px, int qy, int qx) {
+// Gram entry <code_p, code_q> (fp64) for box-relative low-res pixels p, q that are equal or 8-neighbours
+__device__ __forceinline__ double ev_gram(const float* slr, int bw, int py, int px, int qy, int qx) {
   int dy = qy - py, dx = qx - px;
   if (dy < 0 || (dy == 0 && dx < 0)) {  // look the pair up from the upper / left pixel
     const int ty = py, tx = px;
     py = qy; px = qx; qy = ty; qx = tx;
     dy = -dy; dx = -dx;
   }
-  const float* e = slr + (py * bw + px) * EV_LD;
+  const double* e = ev_grams(slr + (py * bw + px) * EV_LD);
   if (dy == 0) return dx == 0 ? e[EV_SS] : e[EV_R];
   return dx == 0 ? e[EV_D] : (dx > 0 ? e[EV_DR] : e[EV_DL]);
 }
@@ -229,11 +247,14 @@ eval_probe_kernel(EvalProbeParams p) {
   }
   // ---- cluster probe: cosine similarity of the interpolated code with the centroids, log_softmax(alpha * .)
   if (p.clu_logp || p.clu_arg) {
-    float n2 = wa * wa * ea[EV_SS] + wb * wb * eb[EV_SS] + wc * wc * ec[EV_SS] + wd * wd * ed[EV_SS];
-    n2 += 2.f * (wa * wb * ev_gram(slr, bw, y0, x0, y0, x1) + wa * wc * ev_gram(slr, bw, y0, x0, y1, x0) +
-                 wa * wd * ev_gram(slr, bw, y0, x0, y1, x1) + wb * wc * ev_gram(slr, bw, y0, x1, y1, x0) +
-                 wb * wd * ev_gram(slr, bw, y0, x1, y1, x1) + wc * wd * ev_gram(slr, bw, y1, x0, y1, x1));
-    const float inv = 1.0f / fmaxf(sqrtf(fmaxf(n2, 0.f)), 1e-12f);
+    // the fp32 weights of the dots, combined in fp64 (their products are exact there)
+    const double da = wa, db = wb, dc = wc, dd = wd;
+    double n2 = da * da * ev_grams(ea)[EV_SS] + db * db * ev_grams(eb)[EV_SS] + dc * dc * ev_grams(ec)[EV_SS] +
+                dd * dd * ev_grams(ed)[EV_SS];
+    n2 += 2.0 * (da * db * ev_gram(slr, bw, y0, x0, y0, x1) + da * dc * ev_gram(slr, bw, y0, x0, y1, x0) +
+                 da * dd * ev_gram(slr, bw, y0, x0, y1, x1) + db * dc * ev_gram(slr, bw, y0, x1, y1, x0) +
+                 db * dd * ev_gram(slr, bw, y0, x1, y1, x1) + dc * dd * ev_gram(slr, bw, y1, x0, y1, x1));
+    const float inv = 1.0f / fmaxf(sqrtf(fmaxf(static_cast<float>(n2), 0.f)), 1e-12f);
     float z[32];
     float mx = -INFINITY;
     int arg = 0;
@@ -420,17 +441,22 @@ eval_probe_vec4_kernel(EvalProbeParams p) {
             make_uchar4((unsigned char)lin_pred[0], (unsigned char)lin_pred[1], (unsigned char)lin_pred[2], (unsigned char)lin_pred[3]);
     }
     if (p.clu_logp || p.clu_arg) {
-      const float gaa = ea[EV_SS], gbb = eb[EV_SS], gcc = ec[EV_SS], gdd = ed[EV_SS];
-      const float gab = ev_gram(slr, bw, y0, x0, y0, x1), gac = ev_gram(slr, bw, y0, x0, y1, x0);
-      const float gad = ev_gram(slr, bw, y0, x0, y1, x1), gbc = ev_gram(slr, bw, y0, x1, y1, x0);
-      const float gbd = ev_gram(slr, bw, y0, x1, y1, x1), gcd = ev_gram(slr, bw, y1, x0, y1, x1);
+      const double gaa = ev_grams(ea)[EV_SS], gbb = ev_grams(eb)[EV_SS], gcc = ev_grams(ec)[EV_SS], gdd = ev_grams(ed)[EV_SS];
+      const double gab = ev_gram(slr, bw, y0, x0, y0, x1), gac = ev_gram(slr, bw, y0, x0, y1, x0);
+      const double gad = ev_gram(slr, bw, y0, x0, y1, x1), gbc = ev_gram(slr, bw, y0, x1, y1, x0);
+      const double gbd = ev_gram(slr, bw, y0, x1, y1, x1), gcd = ev_gram(slr, bw, y1, x0, y1, x1);
+      // in fp64, once per thread: the vertically interpolated left / right codes l = (1-ly) a + ly c, r = (1-ly) b + ly d
+      // give |l|^2, <l, r>, |r|^2, and each pixel's |(1-lx) l + lx r|^2 is a quadratic in its lx
+      const double wy = ly, wy0 = 1.0 - wy;
+      const double ll = wy0 * (wy0 * gaa + 2.0 * wy * gac) + wy * wy * gcc;
+      const double rr = wy0 * (wy0 * gbb + 2.0 * wy * gbd) + wy * wy * gdd;
+      const double lr = wy0 * (wy0 * gab + wy * (gad + gbc)) + wy * wy * gcd;
       float scale[4];
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
-        const float wa = (1.f - ly) * (1.f - lx[j]), wb = (1.f - ly) * lx[j], wc = ly * (1.f - lx[j]), wd = ly * lx[j];
-        float n2 = wa * wa * gaa + wb * wb * gbb + wc * wc * gcc + wd * wd * gdd;
-        n2 += 2.f * (wa * wb * gab + wa * wc * gac + wa * wd * gad + wb * wc * gbc + wb * wd * gbd + wc * wd * gcd);
-        scale[j] = p.alpha / fmaxf(sqrtf(fmaxf(n2, 0.f)), 1e-12f);
+        const double wx = lx[j], wx0 = 1.0 - wx;
+        const double n2 = wx0 * (wx0 * ll + 2.0 * wx * lr) + wx * wx * rr;
+        scale[j] = p.alpha / fmaxf(sqrtf(fmaxf(static_cast<float>(n2), 0.f)), 1e-12f);
       }
       ev4_probe<NC, true>(ea + 32, eb + 32, ec + 32, ed + 32, ly, lx, scale,
                           p.clu_logp ? p.clu_logp + (1ll * b * NC) * plane + pix : nullptr, plane, clu_pred);
@@ -470,7 +496,7 @@ eval_probe_vec4_kernel(EvalProbeParams p) {
 using namespace stego;
 
 // code: tokens-major low-res code [B*h*w][ld_code] fp32 (what DinoFeaturizer produces); outputs at [H][W].
-// code_flip: the code of the horizontally flipped images (flip-TTA) or null.  lr_scratch: [B*h*w][72] floats.
+// code_flip: the code of the horizontally flipped images (flip-TTA) or null.  lr_scratch: [B*h*w][80] floats, 16-byte aligned.
 // label + confusion outputs (int64, accumulated): optional.  Any output pointer may be null.
 extern "C" int stego_eval_probes(const float* code, const float* code_flip, long long ld_code, int C, int B, int h, int w,
                                  int H, int W, const float* lin_weight, const float* lin_bias, int n_lin,
@@ -480,6 +506,7 @@ extern "C" int stego_eval_probes(const float* code, const float* code_flip, long
                                  long long* clu_confusion, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   STEGO_CHECK_ARG(code && lin_weight && lin_bias && clusters && lr_scratch, "stego_eval_probes: null pointer");
+  STEGO_CHECK_ARG((reinterpret_cast<uintptr_t>(lr_scratch) & 7u) == 0, "stego_eval_probes: lr_scratch not 8-byte aligned");
   STEGO_CHECK_ARG(C > 0 && C <= 96 && n_lin > 0 && n_lin <= 32 && n_clu > 0 && n_clu <= 32,
                   "stego_eval_probes: C=%d n_lin=%d n_clu=%d unsupported (C <= 96, classes <= 32)", C, n_lin, n_clu);
   STEGO_CHECK_ARG(B > 0 && h > 0 && w > 0 && H >= h && W >= w, "stego_eval_probes: bad sizes (upsampling only)");

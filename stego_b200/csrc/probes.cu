@@ -498,6 +498,7 @@ __global__ void linear_ce_finish_kernel(const double* __restrict__ acc, float* _
 }
 
 // dW[k][c] += (gscale/count) * sum_r dlogits[r][k] code[r][c];  db[k] += (gscale/count) * sum_r dlogits[r][k]
+// (count = 0 adds nothing: with every label ignored dlogits is all zero, and the reference's gradient is zero too)
 // One CTA per 128-row chunk: both operand tiles are staged in shared memory, every thread owns ~8 of the
 // n*C outputs and walks the 128 rows; one atomic per (CTA, output).
 constexpr int LW_ROWS = 128;
@@ -519,7 +520,9 @@ linear_wgrad_kernel(const float* __restrict__ dlogits, const float* __restrict__
     scode[i] = (r < nr) ? code[(r0 + r) * ld_code + c] : 0.f;
   }
   __syncthreads();
-  const float s = gscale / loss_out[1];
+  // no valid label pixel: the loss is NaN (0 / 0, as in the reference) but the gradient is zero, not 0 * inf
+  const float cnt = loss_out[1];
+  const float s = cnt > 0.f ? gscale / cnt : 0.f;
   for (int o = threadIdx.x; o < n * C; o += blockDim.x) {
     const int k = o / C, c = o % C;
     float acc = 0.f;
@@ -610,7 +613,13 @@ extern "C" int stego_cluster_lookup_bwd(const float* x, long long stride_b, long
     STEGO_CHECK_LAUNCH("cluster_lookup_cl_kernel<bwd>");
   } else {
     const int grid = cluster_grid(total);
-    const size_t smem = (size_t)(2 * n_classes * C + 8) * sizeof(float);
+    const size_t smem = (size_t)(2 * n_classes * C + 8) * sizeof(float);  // 48 KB and more from n * C > 6140
+    static size_t configured = 0;
+    if (smem > 48 * 1024 && smem > configured) {
+      cudaError_t e = cudaFuncSetAttribute(cluster_lookup_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+      if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(cluster_lookup_kernel<bwd>)");
+      configured = smem;
+    }
     cluster_lookup_kernel<true><<<grid, PR_THREADS, smem, stream>>>(p);
     STEGO_CHECK_LAUNCH("cluster_lookup_kernel<bwd>");
   }

@@ -19,9 +19,12 @@ from . import _lib
 
 
 def _tokens_major(code: torch.Tensor) -> torch.Tensor:
+    """fp32 view whose pixel (b, y, x) is row b*h*w + y*w + x at stride ld = stride(3), channels contiguous: the
+    addressing of the kernels.  Other views (NCHW, code[::2], crops) are copied."""
     x = code.detach()
-    w = x.shape[3]
-    if x.dtype != torch.float32 or x.stride(1) != 1 or x.stride(2) != w * x.stride(3):
+    B, _, h, w = x.shape
+    if (x.dtype != torch.float32 or x.stride(1) != 1 or x.stride(2) != w * x.stride(3)
+            or (B > 1 and x.stride(0) != h * w * x.stride(3))):
         x = x.float().permute(0, 2, 3, 1).contiguous().permute(0, 3, 1, 2)
     return x
 
@@ -52,20 +55,16 @@ def fused_probe_log_probs(code: torch.Tensor, linear_probe: torch.nn.Module, clu
     if code_flipped is not None:
         assert code_flipped.shape == code.shape
         xf = _tokens_major(code_flipped)
-        if xf.stride(3) != ld or xf.stride(0) != x.stride(0):
+        if xf.stride(3) != ld:  # one ld for both codes
             xf = xf.permute(0, 2, 3, 1).contiguous().permute(0, 3, 1, 2)
             x = x.permute(0, 2, 3, 1).contiguous().permute(0, 3, 1, 2)
-            ld = x.stride(3)
-        if x.stride(0) != h * w * ld or xf.stride(0) != h * w * ld:  # the kernel indexes rows as b*h*w + y*w + x
-            x = x.permute(0, 2, 3, 1).contiguous().permute(0, 3, 1, 2)
-            xf = xf.permute(0, 2, 3, 1).contiguous().permute(0, 3, 1, 2)
             ld = x.stride(3)
     wl = linear_probe.weight.detach().float().reshape(linear_probe.weight.shape[0], C).contiguous()
     bl = linear_probe.bias.detach().float().contiguous()
     cl = cluster_probe.clusters.detach().float().contiguous()
     n_lin, n_clu = wl.shape[0], cl.shape[0]
     dev = code.device
-    scratch = torch.empty(B * h * w, 72, dtype=torch.float32, device=dev)
+    scratch = torch.empty(B * h * w, 80, dtype=torch.float32, device=dev)  # eval_probes.cu EV_LD
     lin = torch.empty(B, n_lin, H, W, dtype=torch.float32, device=dev) if want_log_probs else None
     clu = torch.empty(B, n_clu, H, W, dtype=torch.float32, device=dev) if want_log_probs else None
     la = torch.empty(B, H, W, dtype=torch.uint8, device=dev) if want_argmax else None

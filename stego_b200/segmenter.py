@@ -189,7 +189,9 @@ class _LinearProbeCEFn(torch.autograd.Function):
         if n > 32 or C > 96:
             raise RuntimeError(f"stego_b200 linear probe: n_classes={n} (<=32) / dim={C} (<=96) unsupported")
         x = code_nchw.detach()
-        if x.dtype != torch.float32 or x.stride(1) != 1 or x.stride(2) != w * x.stride(3):
+        # the kernels address row b*h*w + y*w + x at stride ld: a batch stride other than h*w*ld (code[::2], a crop) is copied
+        if (x.dtype != torch.float32 or x.stride(1) != 1 or x.stride(2) != w * x.stride(3)
+                or (B > 1 and x.stride(0) != h * w * x.stride(3))):
             x = x.float().permute(0, 2, 3, 1).contiguous().permute(0, 3, 1, 2)
         ld = x.stride(3)
         rows = B * h * w
