@@ -87,6 +87,9 @@ STEGO_API int stego_layernorm_gap(const float* x, const float* gamma, const floa
 /* Attention.forward (:78-90) without the projections: softmax(q k^T / sqrt(64)) v, fused (flash-style) on
  * wgmma; qkv [B][N][3E] bf16 packed q|k|v with heads contiguous inside each third, out [B][N][E] bf16. */
 STEGO_API int stego_attention_fwd(const void* qkv, void* out, int B, int N, int E, int heads, void* stream);
+/* The attention matrix of the same Attention.forward (:83-84): probs [B][heads][N][N] fp32 row-major =
+ * softmax(q k^T / sqrt(64)) of the packed bf16 qkv above.  probs must be 4-byte aligned; B, heads <= 65535. */
+STEGO_API int stego_attention_probs(const void* qkv, float* probs, int B, int N, int E, int heads, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Correspondence loss (reference: src/modules.py:275-295, 325-398)

@@ -180,10 +180,11 @@ class VisionTransformer(nn.Module):
     # the kernel sequence
     # ------------------------------------------------------------------------------------------
     @torch.no_grad()
-    def forward_tokens(self, img: torch.Tensor, want_qkv: bool = False
+    def forward_tokens(self, img: torch.Tensor, want_qkv: bool = False, taps: Optional["BlockTaps"] = None
                        ) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
         """Returns (x, qkv_last): x = fp32 residual stream [B*N, E] after the last block (before the
-        final norm); qkv_last = packed bf16 [B*N, 3E] of the last block if requested."""
+        final norm); qkv_last = packed bf16 [B*N, 3E] of the last block if requested.  `taps` collects values of
+        the last taps.n blocks (see BlockTaps); the block outputs are computed the same way with or without it."""
         if not img.is_cuda:
             raise RuntimeError("stego_b200: the DINO ViT forward only exists as sm_90a kernels (no CPU fallback)")
         w = self._prepared()
@@ -206,14 +207,25 @@ class VisionTransformer(nn.Module):
         hid = torch.empty(B * N, w["blocks"][0]["fc1_w"].shape[0], dtype=torch.bfloat16, device=dev)
         Hd = hid.shape[1]
         blocks = w["blocks"]
-        for bw in blocks:
+        depth = len(blocks)
+        for i, bw in enumerate(blocks):
+            tap = taps is not None and depth - i <= taps.n
             ops.layernorm(x, bw["n1w"], bw["n1b"], y, eps=bw["eps1"])
             ops.gemm(y, bw["qkv_w"], qkv, M=B * N, N=3 * E, K=E, bias=bw["qkv_b"])
+            if tap:
+                taps.qkv.append(qkv.clone())
+                if taps.probs:
+                    taps.attn.append(ops.attention_probs(
+                        qkv, torch.empty(B, heads, N, N, dtype=torch.float32, device=dev), B, N, E, heads))
+                if taps.stop_at_last_probs and i == depth - 1:
+                    break
             ops.attention(qkv, ao, B, N, E, heads)
             ops.gemm(ao, bw["proj_w"], x, M=B * N, N=E, K=E, bias=bw["proj_b"], residual=x)
             ops.layernorm(x, bw["n2w"], bw["n2b"], y, eps=bw["eps2"])
             ops.gemm(y, bw["fc1_w"], hid, M=B * N, N=Hd, K=E, bias=bw["fc1_b"], act=ops.ACT_GELU)
             ops.gemm(hid, bw["fc2_w"], x, M=B * N, N=E, K=Hd, bias=bw["fc2_b"], residual=x)
+            if tap:
+                taps.x.append(x.clone())
         return x, (qkv if want_qkv else None)
 
     @torch.no_grad()
@@ -284,12 +296,8 @@ class VisionTransformer(nn.Module):
         return out
 
     def _all_tokens(self, img: torch.Tensor, want_qkv: bool = False):
-        B = img.shape[0]
         x, qkv = self.forward_tokens(img, want_qkv)
-        w = self._prepared()
-        out = torch.empty(x.shape[0], self.embed_dim, dtype=torch.bfloat16, device=x.device)
-        ops.layernorm(x, w["nw"], w["nb"], out, eps=self.norm.eps)
-        return out.view(B, -1, self.embed_dim), qkv
+        return self.final_norm(x, img.shape[0]), qkv
 
     # --- reference entry points ---------------------------------------------------------------
     def forward(self, x):
@@ -301,23 +309,60 @@ class VisionTransformer(nn.Module):
         tok, _ = self._all_tokens(x)
         return tok.float()
 
+    def block_taps(self, img: torch.Tensor, n: int, probs: bool = False, stop_at_last_probs: bool = False
+                   ) -> "BlockTaps":
+        """One forward pass that keeps the values of the last min(n, depth) blocks (n >= 1), oldest first."""
+        taps = BlockTaps(min(n, len(self.blocks)), probs, stop_at_last_probs)
+        self.forward_tokens(img, taps=taps)
+        return taps
+
+    def final_norm(self, x: torch.Tensor, B: int) -> torch.Tensor:
+        """The final LayerNorm of a residual stream [B*N, E] fp32 -> bf16 [B, N, E]."""
+        w = self._prepared()
+        out = torch.empty(x.shape[0], self.embed_dim, dtype=torch.bfloat16, device=x.device)
+        ops.layernorm(x, w["nw"], w["nb"], out, eps=self.norm.eps)
+        return out.view(B, -1, self.embed_dim)
+
+    def split_qkv(self, qkv: torch.Tensor, B: int) -> torch.Tensor:
+        """Packed bf16 [B*N, 3E] -> fp32 [3, B, heads, N, 64], the reference's qkv layout (:80)."""
+        E = self.embed_dim
+        return qkv.view(B, -1, 3, self.num_heads, E // self.num_heads).permute(2, 0, 3, 1, 4).float()
+
     def get_intermediate_feat(self, x, n=1):
-        """vision_transformer.py:225-237.  Only n=1 (what STEGO uses) is provided.  Returns
-        ([feat], [attn], [qkv]) like the reference: feat [B,N,E] fp32; qkv [3,B,heads,N,64];
-        attn is None — the fused attention kernel never materialises the [B,heads,N,N] matrix and STEGO
-        does not read it (src/modules.py:91-101)."""
-        if n != 1:
-            raise RuntimeError("stego_b200: get_intermediate_feat supports n=1 only")
-        tok, qkv = self._all_tokens(x, want_qkv=True)
-        B, N, E = tok.shape
-        qkv = qkv.view(B, N, 3, self.num_heads, E // self.num_heads).permute(2, 0, 3, 1, 4).float()
-        return [tok.float()], [None], [qkv]
+        """vision_transformer.py:225-237: (feat, attn, qkv) lists over the last n blocks (all of them for n >= depth,
+        none for n <= 0), oldest first.  feat = final norm of the block output, fp32 [B, N, E]; attn = softmax(q k^T / 8)
+        fp32 [B, heads, N, N] (stego_attention_probs); qkv fp32 [3, B, heads, N, 64]."""
+        if n <= 0:
+            return [], [], []
+        B = x.shape[0]
+        taps = self.block_taps(x, n, probs=True)
+        return ([self.final_norm(t, B).float() for t in taps.x], taps.attn,
+                [self.split_qkv(q, B) for q in taps.qkv])
+
+    def get_last_selfattention(self, x):
+        """vision_transformer.py:239-246: the attention matrix of the last block, fp32 [B, heads, N, N].  The last
+        block stops after its qkv GEMM, as the reference returns before the projection and the MLP."""
+        return self.block_taps(x, 1, probs=True, stop_at_last_probs=True).attn[0]
 
     def get_intermediate_layers(self, x, n=1):
-        if n != 1:
-            raise RuntimeError("stego_b200: get_intermediate_layers supports n=1 only")
-        tok, _ = self._all_tokens(x)
-        return [tok.float()]
+        """vision_transformer.py:248-256: final norm of the last n blocks' outputs, fp32 [B, N, E], oldest first."""
+        if n <= 0:
+            return []
+        B = x.shape[0]
+        return [self.final_norm(t, B).float() for t in self.block_taps(x, n).x]
+
+
+class BlockTaps:
+    """What forward_tokens keeps from each of the last n blocks: the packed bf16 qkv [B*N, 3E] (a copy: the qkv buffer
+    is reused by the next block), with probs=True the attention matrix fp32 [B, heads, N, N], and the fp32 residual
+    stream after the block [B*N, E] (a copy).  stop_at_last_probs ends the pass after the last block's attention
+    matrix (then the last block leaves no residual stream)."""
+
+    def __init__(self, n: int, probs: bool = False, stop_at_last_probs: bool = False):
+        self.n, self.probs, self.stop_at_last_probs = n, probs, stop_at_last_probs
+        self.qkv: List[torch.Tensor] = []
+        self.attn: List[torch.Tensor] = []
+        self.x: List[torch.Tensor] = []
 
 
 def vit_tiny(patch_size=16, **kwargs):

@@ -310,15 +310,24 @@ class DinoFeaturizer(nn.Module):
         assert (img.shape[3] % self.patch_size == 0)
         fh, fw = img.shape[2] // self.patch_size, img.shape[3] // self.patch_size
         B = img.shape[0]
+        if n < 1:
+            raise ValueError("DinoFeaturizer: n must be >= 1 (block depth - n is read)")
         with torch.no_grad():
+            # n = 1 reads the last block; n > 1 block depth - n (block 0 once n >= depth), as feat[0] / qkv[0] of
+            # get_intermediate_feat(img, n) do in the reference.  Attention matrices are never computed here.
             if return_class_feat:
-                return self.model(img).reshape(B, 1, 1, -1).permute(0, 3, 1, 2)
+                if n == 1:
+                    return self.model(img).reshape(B, 1, 1, -1).permute(0, 3, 1, 2)
+                x = self.model.block_taps(img, n).x[0]
+                return self.model.final_norm(x, B)[:, 0].float().reshape(B, 1, 1, -1).permute(0, 3, 1, 2)
             if self.feat_type == "feat":
-                tok = self.model.patch_features(img)  # [B, hw, E] bf16
+                if n == 1:
+                    tok = self.model.patch_features(img)  # [B, hw, E] bf16
+                else:
+                    tok = self.model.final_norm(self.model.block_taps(img, n).x[0], B)[:, 1:].contiguous()
             elif self.feat_type == "KK":
-                _, _, qkv = self.model.get_intermediate_feat(img, n=n)
-                k = qkv[0][1, :, :, 1:, :]  # [B, heads, hw, 64]
-                tok = k.permute(0, 2, 1, 3).reshape(B, fh * fw, -1).to(torch.bfloat16).contiguous()
+                qkv = self.model.block_taps(img, n).qkv[0]  # packed bf16 [B*N, 3E]: k is the middle third
+                tok = qkv.view(B, fh * fw + 1, 3, -1)[:, 1:, 1].contiguous()  # [B, hw, heads*64], head-major
             else:
                 raise ValueError("Unknown feat type:{}".format(self.feat_type))
         E = tok.shape[-1]

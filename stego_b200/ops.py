@@ -93,3 +93,13 @@ def attention(qkv: torch.Tensor, out: torch.Tensor, B: int, N: int, E: int, head
     _lib.check(_lib.load().stego_attention_fwd(_lib.ptr(qkv), _lib.ptr(out), B, N, E, heads, _lib.stream()),
                "stego_attention_fwd")
     return out
+
+
+def attention_probs(qkv: torch.Tensor, out: torch.Tensor, B: int, N: int, E: int, heads: int) -> torch.Tensor:
+    """softmax(q k^T / 8) as fp32 [B, heads, N, N] (stego_attention_probs). qkv [B*N, 3E] bf16."""
+    _lib.require_cuda(qkv, out)
+    assert qkv.dtype == torch.bfloat16 and qkv.is_contiguous() and qkv.shape == (B * N, 3 * E)
+    assert out.dtype == torch.float32 and out.is_contiguous() and out.numel() == B * heads * N * N
+    _lib.check(_lib.load().stego_attention_probs(_lib.ptr(qkv), _lib.ptr(out), B, N, E, heads, _lib.stream()),
+               "stego_attention_probs")
+    return out
