@@ -97,21 +97,25 @@ STEGO_API int stego_attention_probs(const void* qkv, float* probs, int B, int N,
  * "slot" = one distinct sampled operand: 0 = (src, coords1), 1 = (src_pos, coords2),
  * 2+i = (src[perm_i], coords2).  "call" = one ContrastiveCorrelationLoss.helper invocation; its A
  * operand is always slot 0 and its B operand is slot_of_call[call].
- * Operand tiles: bf16 [2 planes (hi, lo)][nslots][B][128][Cpad]; rows >= feature_samples^2 are zero.
+ * Operand tiles: bf16 [2 planes (hi, lo)][nslots][B][R][Cpad] with R = ceil(feature_samples^2 / 128) * 128 rows
+ * per (plane, slot, image), i.e. R = 128 for feature_samples <= 11; rows >= feature_samples^2 are zero.  Gradient
+ * tiles: fp32 [nslots][B][R][72].
  * ---------------------------------------------------------------------------------------------- */
 /* sample (:287-288) + norm (:275-276): bilinear border/align_corners=True gather at the coords, optional
  * per-(image,channel) scale (the Dropout2d noise of modules.py:116), L2 normalise (eps 1e-10), write
  * the hi/lo split tiles.  src strides are in elements; coords are [B][fs][fs][2] fp32;
  * perms [nslots-2][B] int64: super_perm results (:291-295), or — perms_are_raw_randperm = 1 — the raw randperm
- * draws, in which case the kernel applies super_perm's fix-up (p == b -> (p + 1) % B) itself. */
+ * draws, in which case the kernel applies super_perm's fix-up (p == b -> (p + 1) % B) itself.
+ * feature_samples 1..64.  This call and stego_sample_norm_bwd serve both loss kernel pairs below; they replace
+ * stego_sample_norm_tiled_fwd / _bwd, which had the same signatures. */
 STEGO_API int stego_sample_norm_fwd(const void* src, const void* src_pos, int src_is_bf16, long long stride_b,
                                     long long stride_c, long long stride_y, long long stride_x,
                                     const float* chan_scale, const float* chan_scale_pos, const float* coords1,
                                     const float* coords2, const long long* perms, void* tiles, int B, int C,
                                     int Cpad, int H, int W, int feature_samples, int nslots, int perms_are_raw_randperm,
                                     void* stream);
-/* helper (:325-347) for all calls at once: fd and cd einsums on wgmma (bf16 hi/lo split, fp32 accumulate),
- * pointwise centring, clamp, shift, product and reduction.  slot_of_call / shifts are HOST arrays.
+/* helper (:325-347) for all calls at once, feature_samples <= 11 (R = 128): fd and cd einsums on wgmma (bf16 hi/lo
+ * split, fp32 accumulate), pointwise centring, clamp, shift, product and reduction.  slot_of_call / shifts are HOST arrays.
  * partials: scratch [ncalls][B][8]; stats: out [ncalls][4] = {mean loss, mean cd, old_mean, mean of centred fd}.
  * Optional (may be null): cd_out / fdc_out / loss_out [ncalls][B][S][S] (loss_out needs the other two). */
 STEGO_API int stego_corr_loss_fwd(const void* feat_tiles, const void* code_tiles, int B, int feature_samples, int E,
@@ -135,17 +139,11 @@ STEGO_API int stego_sample_norm_bwd(const float* code, const float* code_pos, lo
                                     float* dcode_pos, int B, int C, int H, int W, int feature_samples, int nslots,
                                     int perms_are_raw_randperm, void* stream);
 
-/* Multi-tile counterparts of the four calls above for feature_samples 1..64 (S = fs^2 up to 4096 points; the
- * training path uses them for fs >= 12, where S exceeds one 128-row tile).  Tiles hold R = ceil(S / 128) * 128 rows
- * per (plane, slot, image): operand tiles bf16 [2][nslots][B][R][Cpad], gradient tiles fp32 [nslots][B][R][72].
- * The fd / cd einsums run per 128x128 (row tile, column tile) block on wgmma, with the same bf16 hi/lo split and fp32
- * accumulation; every reduction runs in a fixed order (no atomics), so results are bit-reproducible run to run. */
-STEGO_API int stego_sample_norm_tiled_fwd(const void* src, const void* src_pos, int src_is_bf16, long long stride_b,
-                                          long long stride_c, long long stride_y, long long stride_x,
-                                          const float* chan_scale, const float* chan_scale_pos, const float* coords1,
-                                          const float* coords2, const long long* perms, void* tiles, int B, int C,
-                                          int Cpad, int H, int W, int feature_samples, int nslots,
-                                          int perms_are_raw_randperm, void* stream);
+/* Multi-tile counterparts of the two loss calls above for feature_samples 1..64 (S = fs^2 up to 4096 points; the
+ * training path uses them for fs >= 12, where S exceeds one 128-row tile).  They take the tiles of
+ * stego_sample_norm_fwd and return gradient tiles for stego_sample_norm_bwd.  The fd / cd einsums run per 128x128
+ * (row tile, column tile) block on wgmma, with the same bf16 hi/lo split and fp32 accumulation; every reduction runs
+ * in a fixed order (no atomics), so results are bit-reproducible run to run. */
 /* row_partials: scratch [ncalls][B][R / 128][R][4] (per-row, per-column-tile sums of fd, clamp(cd) * fd, clamp(cd),
  * cd); row_means: out [ncalls][B][R], the pointwise row means of fd (0 when !pointwise), needed by the backward;
  * stats / cd_out / fdc_out / loss_out as for stego_corr_loss_fwd (fdc_out is centred with the row means). */
@@ -161,12 +159,6 @@ STEGO_API int stego_corr_loss_tiled_bwd(const void* feat_tiles, const void* code
                                         const float* shifts_host, int pointwise, int zero_clamp, int stabilize,
                                         const float* stats, const float* row_means, const float* gscale,
                                         const float* gelem, const float* gcd, float* dtiles, void* stream);
-STEGO_API int stego_sample_norm_tiled_bwd(const float* code, const float* code_pos, long long stride_b,
-                                          long long stride_c, long long stride_y, long long stride_x,
-                                          const float* coords1, const float* coords2, const long long* perms,
-                                          const float* dtiles, float* dcode, float* dcode_pos, int B, int C, int H,
-                                          int W, int feature_samples, int nslots, int perms_are_raw_randperm,
-                                          void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Segmentation head glue (reference: src/modules.py:73-81, 108-118) and optimiser

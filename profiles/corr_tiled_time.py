@@ -71,30 +71,13 @@ def kernel_case(cfg_name, fs, dev):
     gscale = torch.ones(K, device=dev)
     dtiles = torch.zeros(spec.nslots, B, R, corr.DT_LD, device=dev)
     dcode = torch.zeros(2 * B, h, h, 72, device=dev)[..., :D].permute(0, 3, 1, 2)
-    soc, shf = corr._i32(spec.slot_of_call), corr._f32(spec.shifts)
-    flags = (int(spec.pointwise), int(spec.zero_clamp), int(spec.stabilize))
+    partials, means = spec.scratch(B, dev)
+    fwd = lambda: spec.forward(ftiles, ctiles, B, E, D, partials, means, stats)
+    bwd = lambda: spec.backward(ftiles, ctiles, B, E, D, stats, means, gscale, None, None, dtiles)
+    sn_fwd, sn_bwd = lib.stego_sample_norm_fwd, lib.stego_sample_norm_bwd
     st = _lib.stream()
-    if spec.tiled:
-        partials = torch.empty(K, B, spec.n_tiles, R, 4, device=dev)
-        means = torch.empty(K, B, R, device=dev)
-        fwd = lambda: _lib.check(lib.stego_corr_loss_tiled_fwd(
-            _lib.ptr(ftiles), _lib.ptr(ctiles), B, fs, E, D, spec.nslots, K, soc, shf, *flags, _lib.ptr(partials),
-            _lib.ptr(means), _lib.ptr(stats), 0, 0, 0, st), "fwd")
-        bwd = lambda: _lib.check(lib.stego_corr_loss_tiled_bwd(
-            _lib.ptr(ftiles), _lib.ptr(ctiles), B, fs, E, D, spec.nslots, K, soc, shf, *flags, _lib.ptr(stats),
-            _lib.ptr(means), _lib.ptr(gscale), 0, 0, _lib.ptr(dtiles), st), "bwd")
-        sn_fwd, sn_bwd = lib.stego_sample_norm_tiled_fwd, lib.stego_sample_norm_tiled_bwd
-        scratch_bytes = 2 * partials.numel() * 4 + means.numel() * 4
-    else:
-        partials = torch.empty(K, B, 8, device=dev)
-        fwd = lambda: _lib.check(lib.stego_corr_loss_fwd(
-            _lib.ptr(ftiles), _lib.ptr(ctiles), B, fs, E, D, spec.nslots, K, soc, shf, *flags, _lib.ptr(partials),
-            _lib.ptr(stats), 0, 0, 0, st), "fwd")
-        bwd = lambda: _lib.check(lib.stego_corr_loss_bwd(
-            _lib.ptr(ftiles), _lib.ptr(ctiles), B, fs, E, D, spec.nslots, K, soc, shf, *flags, _lib.ptr(stats),
-            _lib.ptr(gscale), 0, 0, _lib.ptr(dtiles), st), "bwd")
-        sn_fwd, sn_bwd = lib.stego_sample_norm_fwd, lib.stego_sample_norm_bwd
-        scratch_bytes = partials.numel() * 4
+    # partials are written and read once; the multi-tile finish also writes the row means
+    scratch_bytes = (2 * partials.numel() + means.numel()) * 4 if spec.tiled else partials.numel() * 4
 
     def sample_fwd():
         sn_fwd(_lib.ptr(tok), _lib.ptr(tok[B:]), 1, h * h * E, 1, h * E, E, 0, 0, _lib.ptr(c1), _lib.ptr(c2),

@@ -53,11 +53,19 @@ def _describe(spec, cfg, n_neg: Optional[int]) -> None:
     # call 0: intra (A vs A), call 1: inter (A vs pos), calls 2..: negatives (A vs img[perm_i])
     spec.slot_of_call = [0, 1] + [2 + i for i in range(spec.n_neg)]
     spec.shifts = [float(cfg.pos_intra_shift), float(cfg.pos_inter_shift)] + [float(cfg.neg_inter_shift)] * spec.n_neg
+    spec._soc, spec._shf = _i32(spec.slot_of_call), _f32(spec.shifts)  # host arrays the loss entry points read
+
+
+def _loss_args(spec, ftiles, ctiles, B, E, D):
+    """the leading arguments every corr-loss entry point takes"""
+    return (_lib.ptr(ftiles), _lib.ptr(ctiles), B, spec.fs, E, D, spec.nslots, spec.ncalls, spec._soc, spec._shf,
+            int(spec.pointwise), int(spec.zero_clamp), int(spec.stabilize))
 
 
 class LossSpec:
     """Static description of one ContrastiveCorrelationLoss evaluation (which calls, which shifts) for the
-    single-tile kernels: all S = feature_samples^2 <= 128 points of an image in one 128-row tile."""
+    single-tile kernels: all S = feature_samples^2 <= 128 points of an image in one 128-row tile.  Each spec knows its
+    entry points: `scratch` allocates what `forward` needs, `forward` / `backward` launch the loss kernels."""
     tiled = False
     rows = TILE_ROWS  # operand / gradient tile rows per (slot, image)
 
@@ -65,6 +73,22 @@ class LossSpec:
         _describe(self, cfg, n_neg)
         if self.fs * self.fs > TILE_ROWS:
             raise RuntimeError(f"stego_b200: feature_samples={self.fs} exceeds the 128-row tile (max 11)")
+
+    def scratch(self, B, device):
+        """(partials, row_means) for `forward`; the single-tile kernels keep their row means in registers, so
+        row_means is empty."""
+        return (torch.empty(self.ncalls, B, 8, dtype=torch.float32, device=device),
+                torch.empty(0, dtype=torch.float32, device=device))
+
+    def forward(self, ftiles, ctiles, B, E, D, partials, row_means, stats, cd=None, fdc=None, elems=None):
+        _lib.check(_lib.load().stego_corr_loss_fwd(
+            *_loss_args(self, ftiles, ctiles, B, E, D), _lib.ptr(partials), _lib.ptr(stats), _lib.ptr(cd),
+            _lib.ptr(fdc), _lib.ptr(elems), _lib.stream()), "stego_corr_loss_fwd")
+
+    def backward(self, ftiles, ctiles, B, E, D, stats, row_means, gscale, gelem, gcd, dtiles):
+        _lib.check(_lib.load().stego_corr_loss_bwd(
+            *_loss_args(self, ftiles, ctiles, B, E, D), _lib.ptr(stats), _lib.ptr(gscale), _lib.ptr(gelem),
+            _lib.ptr(gcd), _lib.ptr(dtiles), _lib.stream()), "stego_corr_loss_bwd")
 
 
 class TiledLossSpec:
@@ -80,6 +104,21 @@ class TiledLossSpec:
         S = self.fs * self.fs
         self.rows = (S + TILE_ROWS - 1) // TILE_ROWS * TILE_ROWS
         self.n_tiles = self.rows // TILE_ROWS
+
+    def scratch(self, B, device):
+        """(per-row partials, row means) for `forward`; `backward` reads the row means."""
+        return (torch.empty(self.ncalls, B, self.n_tiles, self.rows, 4, dtype=torch.float32, device=device),
+                torch.empty(self.ncalls, B, self.rows, dtype=torch.float32, device=device))
+
+    def forward(self, ftiles, ctiles, B, E, D, partials, row_means, stats, cd=None, fdc=None, elems=None):
+        _lib.check(_lib.load().stego_corr_loss_tiled_fwd(
+            *_loss_args(self, ftiles, ctiles, B, E, D), _lib.ptr(partials), _lib.ptr(row_means), _lib.ptr(stats),
+            _lib.ptr(cd), _lib.ptr(fdc), _lib.ptr(elems), _lib.stream()), "stego_corr_loss_tiled_fwd")
+
+    def backward(self, ftiles, ctiles, B, E, D, stats, row_means, gscale, gelem, gcd, dtiles):
+        _lib.check(_lib.load().stego_corr_loss_tiled_bwd(
+            *_loss_args(self, ftiles, ctiles, B, E, D), _lib.ptr(stats), _lib.ptr(row_means), _lib.ptr(gscale),
+            _lib.ptr(gelem), _lib.ptr(gcd), _lib.ptr(dtiles), _lib.stream()), "stego_corr_loss_tiled_bwd")
 
 
 def make_spec(cfg, n_neg: Optional[int] = None):
@@ -100,13 +139,11 @@ def build_tiles(src: torch.Tensor, src_pos: torch.Tensor, coords1: torch.Tensor,
     src_pos = _same_layout(src, src_pos)
     tiles = torch.empty(2, spec.nslots, B, spec.rows, c_pad, dtype=torch.bfloat16, device=src.device)
     sb, sc, sy, sx = src.stride()
-    lib = _lib.load()
-    fn, name = ((lib.stego_sample_norm_tiled_fwd, "stego_sample_norm_tiled_fwd") if spec.tiled
-                else (lib.stego_sample_norm_fwd, "stego_sample_norm_fwd"))
-    rc = fn(_lib.ptr(src), _lib.ptr(src_pos), int(src.dtype == torch.bfloat16), sb, sc, sy, sx,
-            _lib.ptr(chan_scale), _lib.ptr(chan_scale_pos), _lib.ptr(coords1), _lib.ptr(coords2), _lib.ptr(perms),
-            _lib.ptr(tiles), B, C, c_pad, H, W, spec.fs, spec.nslots, int(raw_perms), _lib.stream())
-    _lib.check(rc, name)
+    rc = _lib.load().stego_sample_norm_fwd(
+        _lib.ptr(src), _lib.ptr(src_pos), int(src.dtype == torch.bfloat16), sb, sc, sy, sx,
+        _lib.ptr(chan_scale), _lib.ptr(chan_scale_pos), _lib.ptr(coords1), _lib.ptr(coords2), _lib.ptr(perms),
+        _lib.ptr(tiles), B, C, c_pad, H, W, spec.fs, spec.nslots, int(raw_perms), _lib.stream())
+    _lib.check(rc, "stego_sample_norm_fwd")
     return tiles
 
 
@@ -169,23 +206,8 @@ class _CorrLossFn(torch.autograd.Function):
             cd = torch.empty(spec.ncalls, B, S, S, dtype=torch.float32, device=dev)
             fdc = torch.empty_like(cd)
             elems = torch.empty_like(cd)
-        soc, shf = _i32(spec.slot_of_call), _f32(spec.shifts)
-        if spec.tiled:
-            partials = torch.empty(spec.ncalls, B, spec.n_tiles, spec.rows, 4, dtype=torch.float32, device=dev)
-            row_means = torch.empty(spec.ncalls, B, spec.rows, dtype=torch.float32, device=dev)
-            rc = _lib.load().stego_corr_loss_tiled_fwd(
-                _lib.ptr(ftiles), _lib.ptr(ctiles), B, spec.fs, E, D, spec.nslots, spec.ncalls, soc, shf,
-                int(spec.pointwise), int(spec.zero_clamp), int(spec.stabilize), _lib.ptr(partials),
-                _lib.ptr(row_means), _lib.ptr(stats), _lib.ptr(cd), _lib.ptr(fdc), _lib.ptr(elems), _lib.stream())
-            _lib.check(rc, "stego_corr_loss_tiled_fwd")
-        else:
-            partials = torch.empty(spec.ncalls, B, 8, dtype=torch.float32, device=dev)
-            row_means = torch.empty(0, device=dev)
-            rc = _lib.load().stego_corr_loss_fwd(
-                _lib.ptr(ftiles), _lib.ptr(ctiles), B, spec.fs, E, D, spec.nslots, spec.ncalls, soc, shf,
-                int(spec.pointwise), int(spec.zero_clamp), int(spec.stabilize), _lib.ptr(partials), _lib.ptr(stats),
-                _lib.ptr(cd), _lib.ptr(fdc), _lib.ptr(elems), _lib.stream())
-            _lib.check(rc, "stego_corr_loss_fwd")
+        partials, row_means = spec.scratch(B, dev)
+        spec.forward(ftiles, ctiles, B, E, D, partials, row_means, stats, cd, fdc, elems)
         ctx.spec = spec
         ctx.dims = (B, E, D, H, W)
         ctx.code_dtype = (code.dtype, code_pos.dtype if code_pos is not None else code.dtype)
@@ -209,20 +231,7 @@ class _CorrLossFn(torch.autograd.Function):
         gel = g_elems.to(torch.float32).contiguous() if g_elems is not None else None
         gcd = g_cd.to(torch.float32).contiguous() if g_cd is not None else None
         dtiles = torch.zeros(spec.nslots, B, spec.rows, DT_LD, dtype=torch.float32, device=dev)
-        soc, shf = _i32(spec.slot_of_call), _f32(spec.shifts)
-        lib = _lib.load()
-        if spec.tiled:
-            rc = lib.stego_corr_loss_tiled_bwd(
-                _lib.ptr(ftiles), _lib.ptr(ctiles), B, spec.fs, E, D, spec.nslots, spec.ncalls, soc, shf,
-                int(spec.pointwise), int(spec.zero_clamp), int(spec.stabilize), _lib.ptr(stats), _lib.ptr(row_means),
-                _lib.ptr(gscale), _lib.ptr(gel), _lib.ptr(gcd), _lib.ptr(dtiles), _lib.stream())
-            _lib.check(rc, "stego_corr_loss_tiled_bwd")
-        else:
-            rc = lib.stego_corr_loss_bwd(
-                _lib.ptr(ftiles), _lib.ptr(ctiles), B, spec.fs, E, D, spec.nslots, spec.ncalls, soc, shf,
-                int(spec.pointwise), int(spec.zero_clamp), int(spec.stabilize), _lib.ptr(stats), _lib.ptr(gscale),
-                _lib.ptr(gel), _lib.ptr(gcd), _lib.ptr(dtiles), _lib.stream())
-            _lib.check(rc, "stego_corr_loss_bwd")
+        spec.backward(ftiles, ctiles, B, E, D, stats, row_means, gscale, gel, gcd, dtiles)
         if ctx.pair:
             # code_f / code_pos_f are the two halves of one tensor: one zero-filled buffer with its layout
             full_size = (2 * B,) + tuple(code_f.shape[1:])
@@ -232,12 +241,11 @@ class _CorrLossFn(torch.autograd.Function):
             dcode = _zeros_strided_like(code_f)
             dcode_pos = _zeros_strided_like(code_f)
         sb, sc, sy, sx = code_f.stride()
-        fn, name = ((lib.stego_sample_norm_tiled_bwd, "stego_sample_norm_tiled_bwd") if spec.tiled
-                    else (lib.stego_sample_norm_bwd, "stego_sample_norm_bwd"))
-        rc = fn(_lib.ptr(code_f), _lib.ptr(code_pos_f), sb, sc, sy, sx, _lib.ptr(coords1), _lib.ptr(coords2),
-                _lib.ptr(perms_arg), _lib.ptr(dtiles), _lib.ptr(dcode), _lib.ptr(dcode_pos), B, D, H, W, spec.fs,
-                spec.nslots, int(ctx.raw_perms), _lib.stream())
-        _lib.check(rc, name)
+        rc = _lib.load().stego_sample_norm_bwd(
+            _lib.ptr(code_f), _lib.ptr(code_pos_f), sb, sc, sy, sx, _lib.ptr(coords1), _lib.ptr(coords2),
+            _lib.ptr(perms_arg), _lib.ptr(dtiles), _lib.ptr(dcode), _lib.ptr(dcode_pos), B, D, H, W, spec.fs,
+            spec.nslots, int(ctx.raw_perms), _lib.stream())
+        _lib.check(rc, "stego_sample_norm_bwd")
         d0, d1 = ctx.code_dtype
         if ctx.pair:
             return (dall.to(d0), None) + (None,) * 11

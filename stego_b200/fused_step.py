@@ -93,18 +93,12 @@ class FusedStep:
         # correspondence loss
         ws.ftiles = torch.empty(2, spec.nslots, B, spec.rows, E, dtype=bf, device=dev)
         ws.ctiles = torch.empty(2, spec.nslots, B, spec.rows, corr.CODE_PAD, dtype=bf, device=dev)
-        if spec.tiled:
-            ws.partials = torch.empty(spec.ncalls, B, spec.n_tiles, spec.rows, 4, dtype=f32, device=dev)
-            ws.row_means = torch.empty(spec.ncalls, B, spec.rows, dtype=f32, device=dev)
-        else:
-            ws.partials = torch.empty(spec.ncalls, B, 8, dtype=f32, device=dev)
+        ws.partials, ws.row_means = spec.scratch(B, dev)
         ws.stats = torch.empty(spec.ncalls, 4, dtype=f32, device=dev)
         cw = float(cfg.correspondence_weight)
         wts = [cfg.pos_intra_weight * cw, cfg.pos_inter_weight * cw] + [cfg.neg_inter_weight * cw / spec.n_neg] * spec.n_neg
         ws.call_w = (ctypes.c_float * len(wts))(*[float(v) for v in wts])
         ws.gscale = torch.tensor([float(v) for v in wts], dtype=f32, device=dev)
-        ws.soc = (ctypes.c_int * spec.ncalls)(*spec.slot_of_call)
-        ws.shf = (ctypes.c_float * spec.ncalls)(*spec.shifts)
         # probes
         n_lin = seg.linear_probe.weight.shape[0]
         n_clu = seg.cluster_probe.clusters.shape[0]
@@ -183,27 +177,16 @@ class FusedStep:
         tok_pos = tok_all[B:]
         m3 = ws.M3[:B] if ws.M3 is not None else None
         p3 = ws.M3[B:] if ws.M3 is not None else None
-        # feature_samples >= 12: the multi-tile kernels (same arguments for sampling, row means for the loss)
-        sample_fwd = lib.stego_sample_norm_tiled_fwd if spec.tiled else lib.stego_sample_norm_fwd
-        _lib.check(sample_fwd(
+        _lib.check(lib.stego_sample_norm_fwd(
             _lib.ptr(tok_all), _lib.ptr(tok_pos), 1, hw * E, 1, fw * E, E, _lib.ptr(m3), _lib.ptr(p3),
             _lib.ptr(ws.c1), _lib.ptr(ws.c2), _lib.ptr(ws.perms), _lib.ptr(ws.ftiles), B, E, E, fh, fw, spec.fs,
             spec.nslots, 1, st), "stego_sample_norm_fwd")
         code_pos = ws.code[B * hw:]
-        _lib.check(sample_fwd(
+        _lib.check(lib.stego_sample_norm_fwd(
             _lib.ptr(ws.code), _lib.ptr(code_pos), 0, hw * P, 1, fw * P, P, 0, 0, _lib.ptr(ws.c1), _lib.ptr(ws.c2),
             _lib.ptr(ws.perms), _lib.ptr(ws.ctiles), B, D, corr.CODE_PAD, fh, fw, spec.fs, spec.nslots, 1, st),
             "stego_sample_norm_fwd")
-        if spec.tiled:
-            _lib.check(lib.stego_corr_loss_tiled_fwd(
-                _lib.ptr(ws.ftiles), _lib.ptr(ws.ctiles), B, spec.fs, E, D, spec.nslots, spec.ncalls, ws.soc, ws.shf,
-                int(spec.pointwise), int(spec.zero_clamp), int(spec.stabilize), _lib.ptr(ws.partials),
-                _lib.ptr(ws.row_means), _lib.ptr(ws.stats), 0, 0, 0, st), "stego_corr_loss_tiled_fwd")
-        else:
-            _lib.check(lib.stego_corr_loss_fwd(
-                _lib.ptr(ws.ftiles), _lib.ptr(ws.ctiles), B, spec.fs, E, D, spec.nslots, spec.ncalls, ws.soc, ws.shf,
-                int(spec.pointwise), int(spec.zero_clamp), int(spec.stabilize), _lib.ptr(ws.partials),
-                _lib.ptr(ws.stats), 0, 0, 0, st), "stego_corr_loss_fwd")
+        spec.forward(ws.ftiles, ws.ctiles, B, E, D, ws.partials, ws.row_means, ws.stats)
         seg._mark("corr_loss_forward")
 
         # ---- probes on the detached code (train_segmentation.py:213-225): forward + backward in place
@@ -228,19 +211,9 @@ class FusedStep:
         _lib.check(lib.stego_cluster_lookup_bwd(
             _lib.ptr(ws.code), hw * P, 1, P, _lib.ptr(cl), B, D, ws.n_clu, hw, 0, 0.0, _lib.ptr(ws.one),
             _lib.ptr(ws.dnc), _lib.ptr(cl.grad), st), "stego_cluster_lookup_bwd")
-        if spec.tiled:
-            _lib.check(lib.stego_corr_loss_tiled_bwd(
-                _lib.ptr(ws.ftiles), _lib.ptr(ws.ctiles), B, spec.fs, E, D, spec.nslots, spec.ncalls, ws.soc, ws.shf,
-                int(spec.pointwise), int(spec.zero_clamp), int(spec.stabilize), _lib.ptr(ws.stats),
-                _lib.ptr(ws.row_means), _lib.ptr(ws.gscale), 0, 0, _lib.ptr(ws.dtiles), st), "stego_corr_loss_tiled_bwd")
-        else:
-            _lib.check(lib.stego_corr_loss_bwd(
-                _lib.ptr(ws.ftiles), _lib.ptr(ws.ctiles), B, spec.fs, E, D, spec.nslots, spec.ncalls, ws.soc, ws.shf,
-                int(spec.pointwise), int(spec.zero_clamp), int(spec.stabilize), _lib.ptr(ws.stats),
-                _lib.ptr(ws.gscale), 0, 0, _lib.ptr(ws.dtiles), st), "stego_corr_loss_bwd")
+        spec.backward(ws.ftiles, ws.ctiles, B, E, D, ws.stats, ws.row_means, ws.gscale, None, None, ws.dtiles)
         dall_pos = ws.dall[B * hw * P:]
-        sample_bwd = lib.stego_sample_norm_tiled_bwd if spec.tiled else lib.stego_sample_norm_bwd
-        _lib.check(sample_bwd(
+        _lib.check(lib.stego_sample_norm_bwd(
             _lib.ptr(ws.code), _lib.ptr(code_pos), hw * P, 1, fw * P, P, _lib.ptr(ws.c1), _lib.ptr(ws.c2),
             _lib.ptr(ws.perms), _lib.ptr(ws.dtiles), _lib.ptr(ws.dall), _lib.ptr(dall_pos), B, D, fh, fw, spec.fs,
             spec.nslots, 1, st), "stego_sample_norm_bwd")

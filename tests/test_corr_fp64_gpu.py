@@ -24,8 +24,9 @@ Bars (u = 2^-24; every |term| sum comes from the reference, see _corr_fp64.py):
                  |up (fdc + offset - shift)| is added to E_G and through it to the bar of every row it touches.
                  Elsewhere (including cd exactly at a bound with E_cd = 0, the exact-kink regime) the gradient
                  must meet the bar.
-The largest error / bar ratios are written to $STEGO_PARITY_DIR when it is set.  test_intended_kernels_ran checks
-with torch.profiler, in a child process, that each kind of case launches the kernels it means to test.
+The largest error / bar ratios are written to $STEGO_PARITY_DIR when it is set.  test_intended_kernel_phases_ran
+checks with torch.profiler, in a child process, that each kind of case launches the kernels (and corr_kernel
+phases) it means to test.
 """
 import json
 import os
@@ -261,32 +262,34 @@ def _kernel_cases(dev):
         gl = torch.ones(7, device=dev)
         return lambda: _run(x, cfg, False, code_layout == "pair72", True, gl, None, None)
 
-    single = ("corr_kernel<false>", "corr_kernel<true>", "corr_finish_kernel", "sample_norm_bwd_kernel<3, false>")
-    tiled = ("corr_tiled_kernel<0>", "corr_tiled_kernel<1>", "corr_tiled_kernel<2>", "corr_tiled_finish_kernel",
-             "sample_norm_bwd_kernel<3, true>")
+    # corr_kernel phases: 0 / 2 the single-tile forward / backward, 1 / 3 / 4 the multi-tile forward, dB and dA
+    single = ("corr_kernel<0>", "corr_kernel<2>", "corr_finish_kernel", "sample_norm_bwd_kernel<3>")
+    tiled = ("corr_kernel<1>", "corr_kernel<3>", "corr_kernel<4>", "corr_tiled_finish_kernel",
+             "sample_norm_bwd_kernel<3>")
+    not_single = ("corr_kernel<1>", "corr_kernel<3>", "corr_kernel<4>", "corr_tiled_finish_kernel")
+    not_tiled = ("corr_kernel<0>", "corr_kernel<2>", "corr_finish_kernel")
     return {
-        "vec8_single": (launch(384, "tok16", 11, "pair72"), ("sample_norm_vec8_kernel<2, false>",) + single,
-                        ("corr_tiled_kernel",)),
-        "vec8_tiled": (launch(768, "tok16", 16, "pair72"), ("sample_norm_vec8_kernel<3, true>",) + tiled,
-                       ("corr_kernel<",)),
-        "vec8_ni1": (launch(128, "tok16", 11, "pair72"), ("sample_norm_vec8_kernel<1, false>",), ()),
-        "generic_single": (launch(64, "nchw32", 11, "nchw"), ("sample_norm_kernel<2, false>",) + single,
-                           ("sample_norm_vec8_kernel<", "corr_tiled_kernel")),
-        "generic_tiled": (launch(768, "nchw32", 23, "nchw"), ("sample_norm_kernel<24, true>",) + tiled,
-                          ("sample_norm_vec8_kernel<", "corr_kernel<")),
+        "vec8_single": (launch(384, "tok16", 11, "pair72"), ("sample_norm_vec8_kernel<2>",) + single, not_single),
+        "vec8_tiled": (launch(768, "tok16", 16, "pair72"), ("sample_norm_vec8_kernel<3>",) + tiled, not_tiled),
+        "vec8_ni1": (launch(128, "tok16", 11, "pair72"), ("sample_norm_vec8_kernel<1>",), ()),
+        "generic_single": (launch(64, "nchw32", 11, "nchw"), ("sample_norm_kernel<2>",) + single,
+                           ("sample_norm_vec8_kernel<",) + not_single),
+        "generic_tiled": (launch(768, "nchw32", 23, "nchw"), ("sample_norm_kernel<24>",) + tiled,
+                          ("sample_norm_vec8_kernel<",) + not_tiled),
     }
 
 
-def test_intended_kernels_ran(cuda_dev):
-    """bf16 tokens-major features take the vec8 sampler, fp32 NCHW the generic one; fs <= 11 the single-tile kernels,
-    fs >= 12 the multi-tile ones."""
+def test_intended_kernel_phases_ran(cuda_dev):
+    """bf16 tokens-major features take the vec8 sampler, fp32 NCHW the generic one; fs <= 11 the single-tile phases
+    of corr_kernel (0, 2) and corr_finish_kernel, fs >= 12 the multi-tile phases (1, 3, 4) and corr_tiled_finish_kernel,
+    never the other schedule's."""
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     r = subprocess.run([sys.executable, os.path.abspath(__file__), "--kernel-names"], cwd=root, capture_output=True,
                        text=True, timeout=600)
     assert r.returncode == 0, r.stderr[-4000:]
     got = json.loads(r.stdout.strip().splitlines()[-1])
     for case, (want, not_want) in got["expect"].items():
-        names = [n.replace("(int)", "") for n in got["names"][case]]  # demangled as kernel<(int)2, false>
+        names = [n.replace("(int)", "") for n in got["names"][case]]  # demangled as kernel<(int)2>
         for k in want:
             assert any(k in n for n in names), (case, k, names)
         for k in not_want:
