@@ -378,13 +378,7 @@ extern "C" int stego_attention_fwd(const void* qkv, void* out, int B, int N, int
   uint64_t odims[3] = {(uint64_t)E, (uint64_t)N, (uint64_t)B};
   uint64_t ostr[2] = {(uint64_t)E * 2, (uint64_t)N * E * 2};
   if ((rc = make_tmap_bf16(&tmo, out, 3, odims, ostr, box)) != STEGO_OK) return rc;
-  static bool configured = false;
-  if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(attention_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         (int)ATT_SMEM_TOTAL);
-    if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(attention)");
-    configured = true;
-  }
+  if ((rc = opt_in_smem<attention_fwd_kernel>(ATT_SMEM_TOTAL, "attention_fwd_kernel")) != STEGO_OK) return rc;
   AttnParams p;
   p.N = N;
   p.E = E;
@@ -409,13 +403,7 @@ extern "C" int stego_attention_probs(const void* qkv, float* probs, int B, int N
   uint32_t box[3] = {64, 64, 1};
   int rc = make_tmap_bf16(&tm, qkv, 3, dims, str, box);
   if (rc != STEGO_OK) return rc;
-  static bool configured = false;
-  if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(attention_probs_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         (int)PRB_SMEM_TOTAL);
-    if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(attention_probs)");
-    configured = true;
-  }
+  if ((rc = opt_in_smem<attention_probs_kernel>(PRB_SMEM_TOTAL, "attention_probs_kernel")) != STEGO_OK) return rc;
   AttnParams p;
   p.N = N;
   p.E = E;

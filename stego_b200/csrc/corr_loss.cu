@@ -1014,13 +1014,8 @@ static int launch_corr(const CUtensorMap& tmF, const CUtensorMap& tmC, const Cor
   constexpr int kRing = kPhase >= CP_BWD ? 2 : 3;
   constexpr size_t smem = size_t(kRing) * 2 * CL_TILE + 8 * CL_TILE + 512 + 1024;
   static_assert(smem <= 232448, "exceeds the 227 KB of shared memory a CTA can opt into");
-  auto kern = corr_kernel<kPhase>;
-  static bool configured = false;
-  if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(corr)");
-    configured = true;
-  }
+  constexpr auto kern = corr_kernel<kPhase>;
+  if (const int rc = opt_in_smem<kern>(smem, "corr_kernel"); rc != STEGO_OK) return rc;
   const dim3 grid = kPhase == CP_FWD ? dim3(p.B, p.ncalls)
                   : kPhase == CP_FWD_ROWPART ? dim3(p.B, p.ncalls, p.nT * p.nT)
                   : kPhase == CP_BWD ? dim3(p.B) : dim3(p.B, p.nT);

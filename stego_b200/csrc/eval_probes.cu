@@ -19,8 +19,8 @@
 //     inside the preparation kernel (interpolation is linear, and the reference averages before it as well);
 //   * UnsupervisedMetrics.update for both probes: the [pred][actual] confusion counts are accumulated per CTA in shared
 //     memory from the argmax the kernel already has, one 64-bit atomic per non-zero cell per CTA.
-#include "common.cuh"
 #include "host_util.h"
+#include "probe_common.cuh"
 
 namespace stego {
 
@@ -64,13 +64,7 @@ eval_prep_kernel(EvalPrepParams p) {
     scT[i] = 0.f;
   }
   __syncthreads();
-  for (int k = warp; k < p.n_clu; k += 8) {
-    float ss = 0.f;
-    for (int c = lane; c < p.C; c += 32) { const float v = p.clusters[k * p.C + c]; ss += v * v; }
-    ss = warp_sum(ss);
-    const float inv = 1.0f / fmaxf(sqrtf(ss), 1e-12f);
-    for (int c = lane; c < p.C; c += 32) scT[c * 32 + k] = p.clusters[k * p.C + c] * inv;
-  }
+  normalize_centroids(p.clusters, p.n_clu, p.C, 8, scT, 1, 32);
   __syncthreads();
   const float bk = (lane < p.n_lin) ? p.bias[lane] : 0.f;
   const long long rows = 1ll * p.B * p.h * p.w;
@@ -111,18 +105,10 @@ eval_prep_kernel(EvalPrepParams p) {
     }
     g0 = warp_sum_f64(g0); g1 = warp_sum_f64(g1); g2 = warp_sum_f64(g2); g3 = warp_sum_f64(g3); g4 = warp_sum_f64(g4);
     float dl = bk, dc = 0.f;
-#pragma unroll
-    for (int k = 0; k < 3; ++k) {
-#pragma unroll 8
-      for (int j = 0; j < 32; ++j) {
-        const int c = 32 * k + j;
-        if (c < p.C) {
-          const float xc = __shfl_sync(0xffffffffu, xr[k], j);
-          dl = fmaf(xc, swT[c * 32 + lane], dl);
-          dc = fmaf(xc, scT[c * 32 + lane], dc);
-        }
-      }
-    }
+    for_each_channel(xr, p.C, [&](int c, float xc) {
+      dl = fmaf(xc, swT[c * 32 + lane], dl);
+      dc = fmaf(xc, scT[c * 32 + lane], dc);
+    });
     float* o = p.lr + r * EV_LD;
     o[lane] = dl;
     o[32 + lane] = dc;
@@ -149,18 +135,9 @@ struct EvalProbeParams {
   unsigned long long* clu_conf;  // [n_clu][n_cls]
 };
 
-__device__ __forceinline__ void ev_src_index(int dst, float scale, int in_size, int& i0, int& i1, float& l1) {
-  float s = scale * (dst + 0.5f) - 0.5f;  // ATen area_pixel_compute_source_index, align_corners=False
-  if (s < 0.f) s = 0.f;
-  i0 = static_cast<int>(s);
-  if (i0 > in_size - 1) i0 = in_size - 1;
-  i1 = i0 + ((i0 < in_size - 1) ? 1 : 0);
-  l1 = s - i0;
-}
-
 // Output tile of a CTA: 64 x 4 pixels, thread = pixel, x fastest (coalesced plane writes).  (Measured and rejected in
 // round 2: 64 x 16 tiles in four passes under a 120-register cap, two CTAs per SM: 1.35 ms instead of 1.00 ms per 4 frames.)
-constexpr int EVT_W = 64, EVT_ROWS = 4, EVT_PASSES = 1, EVT_H = EVT_ROWS * EVT_PASSES;
+constexpr int EVT_W = 64, EVT_H = 4;
 
 // Gram entry <code_p, code_q> (fp64) for box-relative low-res pixels p, q that are equal or 8-neighbours
 __device__ __forceinline__ double ev_gram(const float* slr, int bw, int py, int px, int qy, int qx) {
@@ -175,10 +152,10 @@ __device__ __forceinline__ double ev_gram(const float* slr, int bw, int py, int 
   return dx == 0 ? e[EV_D] : (dx > 0 ? e[EV_DR] : e[EV_DL]);
 }
 
-__global__ void __launch_bounds__(EVT_W* EVT_ROWS)
+__global__ void __launch_bounds__(EVT_W* EVT_H)
 eval_probe_kernel(EvalProbeParams p) {
   extern __shared__ float slr[];  // [box_h*box_w][EV_LD]
-  __shared__ unsigned int hist[2][32 * 32];  // [probe][pred * 32 + actual]
+  __shared__ ConfHist hist;
   const bool want_conf = p.label != nullptr;
   if (want_conf)
     for (int i = threadIdx.x; i < 2 * 32 * 32; i += blockDim.x) (&hist[0][0])[i] = 0u;
@@ -188,13 +165,9 @@ eval_probe_kernel(EvalProbeParams p) {
   const int X0 = tx * EVT_W, Y0 = ty * EVT_H;
   const int Xl = min(X0 + EVT_W - 1, p.W - 1), Yl = min(Y0 + EVT_H - 1, p.H - 1);
   const float sy = static_cast<float>(p.h) / p.H, sx = static_cast<float>(p.w) / p.W;
-  int by0, by1, bx0, bx1, tmp;
-  float ftmp;
-  ev_src_index(Y0, sy, p.h, by0, tmp, ftmp);
-  ev_src_index(Yl, sy, p.h, tmp, by1, ftmp);
-  ev_src_index(X0, sx, p.w, bx0, tmp, ftmp);
-  ev_src_index(Xl, sx, p.w, tmp, bx1, ftmp);
-  const int bh = by1 - by0 + 1, bw = bx1 - bx0 + 1;
+  int by0, bh, bx0, bw;
+  src_span(Y0, Yl, sy, p.h, by0, bh);
+  src_span(X0, Xl, sx, p.w, bx0, bw);
   const long long base = 1ll * b * p.h * p.w;
   for (int i = threadIdx.x; i < bh * bw * EV_LD; i += blockDim.x) {
     const int cell = i / EV_LD, k = i % EV_LD;
@@ -202,112 +175,92 @@ eval_probe_kernel(EvalProbeParams p) {
     slr[i] = p.lr[(base + 1ll * (by0 + r) * p.w + bx0 + c) * EV_LD + k];
   }
   __syncthreads();
-  for (int pass = 0; pass < EVT_PASSES; ++pass) {
-  const int X = X0 + (threadIdx.x % EVT_W), Y = Y0 + pass * EVT_ROWS + (threadIdx.x / EVT_W);
+  const int X = X0 + (threadIdx.x % EVT_W), Y = Y0 + (threadIdx.x / EVT_W);
   const bool active = X < p.W && Y < p.H;
   int lin_pred = -1, clu_pred = -1;
   if (active) {
-  int y0, y1, x0, x1;
-  float ly, lx;
-  ev_src_index(Y, sy, p.h, y0, y1, ly);
-  ev_src_index(X, sx, p.w, x0, x1, lx);
-  y0 -= by0; y1 -= by0; x0 -= bx0; x1 -= bx0;
-  const float wa = (1.f - ly) * (1.f - lx), wb = (1.f - ly) * lx, wc = ly * (1.f - lx), wd = ly * lx;
-  const float* ea = slr + (y0 * bw + x0) * EV_LD;
-  const float* eb = slr + (y0 * bw + x1) * EV_LD;
-  const float* ec = slr + (y1 * bw + x0) * EV_LD;
-  const float* ed = slr + (y1 * bw + x1) * EV_LD;
-  const long long plane = 1ll * p.H * p.W;
-  const long long pix = 1ll * Y * p.W + X;
-  // ---- linear probe: log_softmax of the interpolated logits
-  if (p.lin_logp || p.lin_arg) {
-    float z[32];
-    float mx = -INFINITY;
-    int arg = 0;
+    int y0, y1, x0, x1;
+    float ly, lx;
+    src_index(Y, sy, p.h, y0, y1, ly);
+    src_index(X, sx, p.w, x0, x1, lx);
+    y0 -= by0; y1 -= by0; x0 -= bx0; x1 -= bx0;
+    const float wa = (1.f - ly) * (1.f - lx), wb = (1.f - ly) * lx, wc = ly * (1.f - lx), wd = ly * lx;
+    const float* ea = slr + (y0 * bw + x0) * EV_LD;
+    const float* eb = slr + (y0 * bw + x1) * EV_LD;
+    const float* ec = slr + (y1 * bw + x0) * EV_LD;
+    const float* ed = slr + (y1 * bw + x1) * EV_LD;
+    const long long plane = 1ll * p.H * p.W;
+    const long long pix = 1ll * Y * p.W + X;
+    // ---- linear probe: log_softmax of the interpolated logits
+    if (p.lin_logp || p.lin_arg) {
+      float z[32];
+      float mx = -INFINITY;
+      int arg = 0;
 #pragma unroll
-    for (int k = 0; k < 32; ++k) {
-      if (k < p.n_lin) {
-        z[k] = wa * ea[k] + wb * eb[k] + wc * ec[k] + wd * ed[k];
-        if (z[k] > mx) { mx = z[k]; arg = k; }
+      for (int k = 0; k < 32; ++k) {
+        if (k < p.n_lin) {
+          z[k] = wa * ea[k] + wb * eb[k] + wc * ec[k] + wd * ed[k];
+          if (z[k] > mx) { mx = z[k]; arg = k; }
+        }
+      }
+      lin_pred = arg;
+      if (p.lin_arg) p.lin_arg[b * plane + pix] = static_cast<unsigned char>(arg);
+      if (p.lin_logp) {
+        float se = 0.f;
+#pragma unroll
+        for (int k = 0; k < 32; ++k)
+          if (k < p.n_lin) se += __expf(z[k] - mx);
+        const float lse = mx + __logf(se);
+        float* o = p.lin_logp + (1ll * b * p.n_lin) * plane + pix;
+#pragma unroll
+        for (int k = 0; k < 32; ++k)
+          if (k < p.n_lin) o[k * plane] = z[k] - lse;
       }
     }
-    lin_pred = arg;
-    if (p.lin_arg) p.lin_arg[b * plane + pix] = static_cast<unsigned char>(arg);
-    if (p.lin_logp) {
-      float se = 0.f;
+    // ---- cluster probe: cosine similarity of the interpolated code with the centroids, log_softmax(alpha * .)
+    if (p.clu_logp || p.clu_arg) {
+      // the fp32 weights of the dots, combined in fp64 (their products are exact there)
+      const double da = wa, db = wb, dc = wc, dd = wd;
+      double n2 = da * da * ev_grams(ea)[EV_SS] + db * db * ev_grams(eb)[EV_SS] + dc * dc * ev_grams(ec)[EV_SS] +
+                  dd * dd * ev_grams(ed)[EV_SS];
+      n2 += 2.0 * (da * db * ev_gram(slr, bw, y0, x0, y0, x1) + da * dc * ev_gram(slr, bw, y0, x0, y1, x0) +
+                   da * dd * ev_gram(slr, bw, y0, x0, y1, x1) + db * dc * ev_gram(slr, bw, y0, x1, y1, x0) +
+                   db * dd * ev_gram(slr, bw, y0, x1, y1, x1) + dc * dd * ev_gram(slr, bw, y1, x0, y1, x1));
+      const float inv = 1.0f / fmaxf(sqrtf(fmaxf(static_cast<float>(n2), 0.f)), 1e-12f);
+      float z[32];
+      float mx = -INFINITY;
+      int arg = 0;
 #pragma unroll
-      for (int k = 0; k < 32; ++k)
-        if (k < p.n_lin) se += __expf(z[k] - mx);
-      const float lse = mx + __logf(se);
-      float* o = p.lin_logp + (1ll * b * p.n_lin) * plane + pix;
+      for (int k = 0; k < 32; ++k) {
+        if (k < p.n_clu) {
+          z[k] = (wa * ea[32 + k] + wb * eb[32 + k] + wc * ec[32 + k] + wd * ed[32 + k]) * inv;
+          if (z[k] > mx) { mx = z[k]; arg = k; }
+        }
+      }
+      clu_pred = arg;
+      if (p.clu_arg) p.clu_arg[b * plane + pix] = static_cast<unsigned char>(arg);
+      if (p.clu_logp) {
+        float m2 = -INFINITY;
 #pragma unroll
-      for (int k = 0; k < 32; ++k)
-        if (k < p.n_lin) o[k * plane] = z[k] - lse;
-    }
-  }
-  // ---- cluster probe: cosine similarity of the interpolated code with the centroids, log_softmax(alpha * .)
-  if (p.clu_logp || p.clu_arg) {
-    // the fp32 weights of the dots, combined in fp64 (their products are exact there)
-    const double da = wa, db = wb, dc = wc, dd = wd;
-    double n2 = da * da * ev_grams(ea)[EV_SS] + db * db * ev_grams(eb)[EV_SS] + dc * dc * ev_grams(ec)[EV_SS] +
-                dd * dd * ev_grams(ed)[EV_SS];
-    n2 += 2.0 * (da * db * ev_gram(slr, bw, y0, x0, y0, x1) + da * dc * ev_gram(slr, bw, y0, x0, y1, x0) +
-                 da * dd * ev_gram(slr, bw, y0, x0, y1, x1) + db * dc * ev_gram(slr, bw, y0, x1, y1, x0) +
-                 db * dd * ev_gram(slr, bw, y0, x1, y1, x1) + dc * dd * ev_gram(slr, bw, y1, x0, y1, x1));
-    const float inv = 1.0f / fmaxf(sqrtf(fmaxf(static_cast<float>(n2), 0.f)), 1e-12f);
-    float z[32];
-    float mx = -INFINITY;
-    int arg = 0;
+        for (int k = 0; k < 32; ++k)
+          if (k < p.n_clu) m2 = fmaxf(m2, z[k] * p.alpha);
+        float se = 0.f;
 #pragma unroll
-    for (int k = 0; k < 32; ++k) {
-      if (k < p.n_clu) {
-        z[k] = (wa * ea[32 + k] + wb * eb[32 + k] + wc * ec[32 + k] + wd * ed[32 + k]) * inv;
-        if (z[k] > mx) { mx = z[k]; arg = k; }
+        for (int k = 0; k < 32; ++k)
+          if (k < p.n_clu) se += __expf(z[k] * p.alpha - m2);
+        const float lse = m2 + __logf(se);
+        float* o = p.clu_logp + (1ll * b * p.n_clu) * plane + pix;
+#pragma unroll
+        for (int k = 0; k < 32; ++k)
+          if (k < p.n_clu) o[k * plane] = z[k] * p.alpha - lse;
       }
     }
-    clu_pred = arg;
-    if (p.clu_arg) p.clu_arg[b * plane + pix] = static_cast<unsigned char>(arg);
-    if (p.clu_logp) {
-      float m2 = -INFINITY;
-#pragma unroll
-      for (int k = 0; k < 32; ++k)
-        if (k < p.n_clu) m2 = fmaxf(m2, z[k] * p.alpha);
-      float se = 0.f;
-#pragma unroll
-      for (int k = 0; k < 32; ++k)
-        if (k < p.n_clu) se += __expf(z[k] * p.alpha - m2);
-      const float lse = m2 + __logf(se);
-      float* o = p.clu_logp + (1ll * b * p.n_clu) * plane + pix;
-#pragma unroll
-      for (int k = 0; k < 32; ++k)
-        if (k < p.n_clu) o[k * plane] = z[k] * p.alpha - lse;
-    }
   }
-  }  // active
   if (want_conf) {
-    // UnsupervisedMetrics.update (src/utils.py:219-229): stats[pred][actual] += 1 over pixels with a valid label
-    if (active) {
-      const long long li = 1ll * b * p.H * p.W + 1ll * Y * p.W + X;
-      long long lab;
-      if (p.label_bytes == 8) lab = reinterpret_cast<const long long*>(p.label)[li];
-      else if (p.label_bytes == 4) lab = reinterpret_cast<const int*>(p.label)[li];
-      else lab = reinterpret_cast<const unsigned char*>(p.label)[li];
-      if (lab >= 0 && lab < p.n_cls) {
-        if (lin_pred >= 0 && lin_pred < p.n_cls) atomicAdd(&hist[0][lin_pred * 32 + static_cast<int>(lab)], 1u);
-        if (clu_pred >= 0 && clu_pred < p.n_cls) atomicAdd(&hist[1][clu_pred * 32 + static_cast<int>(lab)], 1u);
-      }
-    }
-  }
-  }  // pass
-  if (want_conf) {
-    __syncthreads();
-    for (int i = threadIdx.x; i < 2 * 32 * 32; i += blockDim.x) {
-      const unsigned int cnt = (&hist[0][0])[i];
-      if (cnt == 0u) continue;
-      const int probe = i >> 10, pred = (i >> 5) & 31, act = i & 31;
-      unsigned long long* dst = probe ? p.clu_conf : p.lin_conf;
-      if (dst && act < p.n_cls && pred < (probe ? p.n_clu : p.n_lin)) atomicAdd(dst + pred * p.n_cls + act, (unsigned long long)cnt);
-    }
+    if (active)
+      conf_hist_add(hist, read_label(p.label, p.label_bytes, 1ll * b * p.H * p.W + 1ll * Y * p.W + X), p.n_cls,
+                    lin_pred, clu_pred);
+    conf_hist_flush(hist, p.lin_conf, p.clu_conf, p.n_lin, p.n_clu, p.n_cls);
   }
 }
 
@@ -383,7 +336,7 @@ template <int NL, int NC>
 __global__ void __launch_bounds__(EV4_TW* EV4_ROWS, 2)
 eval_probe_vec4_kernel(EvalProbeParams p) {
   extern __shared__ __align__(16) float slr[];  // [box_h*box_w][EV_LD]
-  __shared__ unsigned int hist[2][32 * 32];     // [probe][pred * 32 + actual]
+  __shared__ ConfHist hist;
   const bool want_conf = p.label != nullptr;
   if (want_conf)
     for (int i = threadIdx.x; i < 2 * 32 * 32; i += blockDim.x) (&hist[0][0])[i] = 0u;
@@ -393,13 +346,9 @@ eval_probe_vec4_kernel(EvalProbeParams p) {
   const int X0 = tx * EV4_W, Y0 = ty * EV4_ROWS;
   const int Xl = min(X0 + EV4_W - 1, p.W - 1), Yl = min(Y0 + EV4_ROWS - 1, p.H - 1);
   const float sy = static_cast<float>(p.h) / p.H, sx = static_cast<float>(p.w) / p.W;
-  int by0, by1, bx0, bx1, tmp;
-  float ftmp;
-  ev_src_index(Y0, sy, p.h, by0, tmp, ftmp);
-  ev_src_index(Yl, sy, p.h, tmp, by1, ftmp);
-  ev_src_index(X0, sx, p.w, bx0, tmp, ftmp);
-  ev_src_index(Xl, sx, p.w, tmp, bx1, ftmp);
-  const int bh = by1 - by0 + 1, bw = bx1 - bx0 + 1;
+  int by0, bh, bx0, bw;
+  src_span(Y0, Yl, sy, p.h, by0, bh);
+  src_span(X0, Xl, sx, p.w, bx0, bw);
   const long long base = 1ll * b * p.h * p.w;
   {
     constexpr int LD4 = EV_LD / 4;
@@ -417,12 +366,12 @@ eval_probe_vec4_kernel(EvalProbeParams p) {
   if (active) {
     int y0, y1, x0, x1;
     float ly, lx[4];
-    ev_src_index(Y, sy, p.h, y0, y1, ly);
-    ev_src_index(X, sx, p.w, x0, x1, lx[0]);
+    src_index(Y, sy, p.h, y0, y1, ly);
+    src_index(X, sx, p.w, x0, x1, lx[0]);
 #pragma unroll
     for (int j = 1; j < 4; ++j) {  // same two columns for the whole group (host checks the upsampling factor)
       int t0, t1;
-      ev_src_index(X + j, sx, p.w, t0, t1, lx[j]);
+      src_index(X + j, sx, p.w, t0, t1, lx[j]);
     }
     y0 -= by0; y1 -= by0; x0 -= bx0; x1 -= bx0;
     const float* ea = slr + (y0 * bw + x0) * EV_LD;
@@ -464,31 +413,13 @@ eval_probe_vec4_kernel(EvalProbeParams p) {
         *reinterpret_cast<uchar4*>(p.clu_arg + b * plane + pix) =
             make_uchar4((unsigned char)clu_pred[0], (unsigned char)clu_pred[1], (unsigned char)clu_pred[2], (unsigned char)clu_pred[3]);
     }
-    if (want_conf) {  // UnsupervisedMetrics.update (src/utils.py:219-229)
-      const long long li = 1ll * b * plane + pix;
+    if (want_conf) {
 #pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        long long lab;
-        if (p.label_bytes == 8) lab = reinterpret_cast<const long long*>(p.label)[li + j];
-        else if (p.label_bytes == 4) lab = reinterpret_cast<const int*>(p.label)[li + j];
-        else lab = reinterpret_cast<const unsigned char*>(p.label)[li + j];
-        if (lab >= 0 && lab < p.n_cls) {
-          if (lin_pred[j] >= 0 && lin_pred[j] < p.n_cls) atomicAdd(&hist[0][lin_pred[j] * 32 + static_cast<int>(lab)], 1u);
-          if (clu_pred[j] >= 0 && clu_pred[j] < p.n_cls) atomicAdd(&hist[1][clu_pred[j] * 32 + static_cast<int>(lab)], 1u);
-        }
-      }
+      for (int j = 0; j < 4; ++j)
+        conf_hist_add(hist, read_label(p.label, p.label_bytes, b * plane + pix + j), p.n_cls, lin_pred[j], clu_pred[j]);
     }
   }
-  if (want_conf) {
-    __syncthreads();
-    for (int i = threadIdx.x; i < 2 * 32 * 32; i += blockDim.x) {
-      const unsigned int cnt = (&hist[0][0])[i];
-      if (cnt == 0u) continue;
-      const int probe = i >> 10, pred = (i >> 5) & 31, act = i & 31;
-      unsigned long long* dst = probe ? p.clu_conf : p.lin_conf;
-      if (dst && act < p.n_cls && pred < (probe ? NC : NL)) atomicAdd(dst + pred * p.n_cls + act, (unsigned long long)cnt);
-    }
-  }
+  if (want_conf) conf_hist_flush(hist, p.lin_conf, p.clu_conf, NL, NC, p.n_cls);
 }
 
 }  // namespace stego
@@ -536,32 +467,21 @@ extern "C" int stego_eval_probes(const float* code, const float* code_flip, long
                     (!clu_argmax || (reinterpret_cast<uintptr_t>(clu_argmax) & 3) == 0) &&
                     (reinterpret_cast<uintptr_t>(lr_scratch) & 15) == 0;
   const int tile_h = vec4 ? EV4_ROWS : EVT_H, tile_w = vec4 ? EV4_W : EVT_W;
-  p.box_h = (int)((double)tile_h * h / H) + 3;
-  p.box_w = (int)((double)tile_w * w / W) + 3;
-  if (p.box_h > h) p.box_h = h;
-  if (p.box_w > w) p.box_w = w;
+  p.box_h = src_span_max(tile_h, h, H);
+  p.box_w = src_span_max(tile_w, w, W);
   const size_t smem = (size_t)p.box_h * p.box_w * EV_LD * sizeof(float);
   STEGO_CHECK_ARG(smem <= 200 * 1024, "stego_eval_probes: upsample ratio needs %zu B of shared memory", smem);
   const long long tiles = 1ll * B * ((H + tile_h - 1) / tile_h) * ((W + tile_w - 1) / tile_w);
   STEGO_CHECK_ARG(tiles < (1ll << 31), "stego_eval_probes: too many tiles");
+  int rc;
   if (vec4) {
-    static size_t conf4 = 0;
-    if (smem > 48 * 1024 && smem > conf4) {
-      cudaError_t e = cudaFuncSetAttribute(eval_probe_vec4_kernel<27, 27>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-      if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(eval_probe_vec4)");
-      conf4 = smem;
-    }
+    if ((rc = opt_in_smem<eval_probe_vec4_kernel<27, 27>>(smem, "eval_probe_vec4_kernel")) != STEGO_OK) return rc;
     eval_probe_vec4_kernel<27, 27><<<(unsigned)tiles, EV4_TW * EV4_ROWS, smem, stream>>>(p);
     STEGO_CHECK_LAUNCH("eval_probe_vec4_kernel");
     return STEGO_OK;
   }
-  static size_t conf = 0;
-  if (smem > 48 * 1024 && smem > conf) {
-    cudaError_t e = cudaFuncSetAttribute(eval_probe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(eval_probe)");
-    conf = smem;
-  }
-  eval_probe_kernel<<<(unsigned)tiles, EVT_W * EVT_ROWS, smem, stream>>>(p);
+  if ((rc = opt_in_smem<eval_probe_kernel>(smem, "eval_probe_kernel")) != STEGO_OK) return rc;
+  eval_probe_kernel<<<(unsigned)tiles, EVT_W * EVT_H, smem, stream>>>(p);
   STEGO_CHECK_LAUNCH("eval_probe_kernel");
   return STEGO_OK;
 }

@@ -377,13 +377,8 @@ static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUt
                        cudaStream_t stream) {
   constexpr size_t smem = size_t(kStages) * GEMM_STAGE_BYTES + (kTmaEpi ? 4 * GEMM_CHUNK_BYTES : 0) + 1024 + 256;
   static_assert(smem <= 232448, "exceeds the 227 KB of shared memory a CTA can opt into");
-  auto kern = gemm_bf16_kernel<kStages, A_MN, B_MN, kTmaEpi>;
-  static bool configured = false;
-  if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(gemm)");
-    configured = true;
-  }
+  constexpr auto kern = gemm_bf16_kernel<kStages, A_MN, B_MN, kTmaEpi>;
+  if (const int rc = opt_in_smem<kern>(smem, "gemm_bf16_kernel"); rc != STEGO_OK) return rc;
   const int tiles_m = (p.M + GEMM_BM - 1) / GEMM_BM;
   const int tiles_n = (p.N + GEMM_BN - 1) / GEMM_BN;
   const int tiles = tiles_m * tiles_n * p.splits * p.batch;

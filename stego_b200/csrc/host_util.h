@@ -28,6 +28,19 @@ int make_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t*
 int make_tmap_f32(CUtensorMap* out, const void* base, int rank, const uint64_t* dims,
                   const uint64_t* strides_bytes, const uint32_t* box);
 
+// Lets Kernel launch with `bytes` of dynamic shared memory: above the 48 KB default that takes an opt-in, set
+// again only when a launch asks for more than before.  Returns STEGO_OK, or cuda_fail(e, what).
+template <auto Kernel>
+int opt_in_smem(size_t bytes, const char* what) {
+  static size_t configured = 0;
+  if (bytes > 48 * 1024 && bytes > configured) {
+    cudaError_t e = cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+    if (e != cudaSuccess) return cuda_fail(e, what);
+    configured = bytes;
+  }
+  return STEGO_OK;
+}
+
 #define STEGO_CHECK_ARG(cond, ...)       \
   do {                                   \
     if (!(cond)) {                       \

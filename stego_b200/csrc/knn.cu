@@ -229,12 +229,7 @@ extern "C" int stego_knn_topk(const float* feats, int n, int E, int k, void* pla
   uint32_t box[3] = {64, 128, 1};  // KNN_BM = KNN_BN = 128 rows
   int rc = make_tmap_bf16(&tm, planes_scratch, 3, dims, str, box);
   if (rc != STEGO_OK) return rc;
-  static bool configured = false;
-  if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(knn_topk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)KNN_SMEM);
-    if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(knn_topk)");
-    configured = true;
-  }
+  if ((rc = opt_in_smem<knn_topk_kernel>(KNN_SMEM, "knn_topk_kernel")) != STEGO_OK) return rc;
   KnnParams p;
   p.n = n; p.E = E; p.k = k; p.idx_out = idx_out; p.val_out = val_out;
   const int row_blocks = (n + KNN_BM - 1) / KNN_BM;

@@ -10,8 +10,8 @@
 // argmax is deterministic; centroids are normalised once per CTA into shared memory.
 #include <algorithm>
 
-#include "common.cuh"
 #include "host_util.h"
+#include "probe_common.cuh"
 
 namespace stego {
 
@@ -37,19 +37,6 @@ struct ClusterParams {
   float* dnc;                // [n][C] gradient wrt the NORMALISED centroids (atomically accumulated)
 };
 
-__device__ __forceinline__ void load_norm_clusters(const ClusterParams& p, float* snc) {
-  // normalise centroids (F.normalize, eps 1e-12) into smem: one warp per centroid round-robin
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
-  for (int k = warp; k < p.n; k += nw) {
-    float ss = 0.f;
-    for (int c = lane; c < p.C; c += 32) { const float v = p.clusters[k * p.C + c]; ss += v * v; }
-    ss = warp_sum(ss);
-    const float inv = 1.0f / fmaxf(sqrtf(ss), 1e-12f);
-    for (int c = lane; c < p.C; c += 32) snc[k * p.C + c] = p.clusters[k * p.C + c] * inv;
-  }
-  __syncthreads();
-}
-
 template <bool kBackward>
 __global__ void __launch_bounds__(PR_THREADS)
 cluster_lookup_kernel(ClusterParams p) {
@@ -57,7 +44,8 @@ cluster_lookup_kernel(ClusterParams p) {
   float* snc = sm;                         // [n][C]
   float* sacc = sm + p.n * p.C;            // backward: [n][C] block accumulator
   float* sred = sacc + (kBackward ? p.n * p.C : 0);  // [4]
-  load_norm_clusters(p, snc);
+  normalize_centroids(p.clusters, p.n, p.C, blockDim.x >> 5, snc, p.C, 1);
+  __syncthreads();
   if (kBackward) p.grad_scale *= p.grad_loss[0];
   if (kBackward) {
     for (int i = threadIdx.x; i < p.n * p.C; i += blockDim.x) sacc[i] = 0.f;
@@ -151,13 +139,7 @@ cluster_lookup_cl_kernel(ClusterParams p) {
   if (kBackward)
     for (int i = threadIdx.x; i < p.n * p.C; i += blockDim.x) sacc[i] = 0.f;
   __syncthreads();
-  for (int k = warp; k < p.n; k += 8) {
-    float ss = 0.f;
-    for (int c = lane; c < p.C; c += 32) { const float v = p.clusters[k * p.C + c]; ss += v * v; }
-    ss = warp_sum(ss);
-    const float inv = 1.0f / fmaxf(sqrtf(ss), 1e-12f);
-    for (int c = lane; c < p.C; c += 32) sncT[c * 32 + k] = p.clusters[k * p.C + c] * inv;
-  }
+  normalize_centroids(p.clusters, p.n, p.C, 8, sncT, 1, 32);
   __syncthreads();
   const float gs = kBackward ? p.grad_scale * p.grad_loss[0] : 0.f;
   const long long total = 1ll * p.B * p.npix;
@@ -167,27 +149,12 @@ cluster_lookup_cl_kernel(ClusterParams p) {
     const long long q = pix % p.npix;
     const float* xp = p.x + b * p.sb + q * p.sp;
     float xr[3];
-    float ss = 0.f;
-#pragma unroll
-    for (int k = 0; k < 3; ++k) {
-      const int c = lane + 32 * k;
-      xr[k] = (c < p.C) ? xp[c] : 0.f;
-    }
+    load_channels(xp, p.C, lane, xr);
     // same summation order as the per-thread kernel is not required for the norm (it only scales all classes)
-    ss = warp_sum(xr[0] * xr[0] + xr[1] * xr[1] + xr[2] * xr[2]);
+    const float ss = warp_sum(xr[0] * xr[0] + xr[1] * xr[1] + xr[2] * xr[2]);
     const float inv = 1.0f / fmaxf(sqrtf(ss), 1e-12f);
     float d = 0.f;
-#pragma unroll
-    for (int k = 0; k < 3; ++k) {
-#pragma unroll 8
-      for (int j = 0; j < 32; ++j) {
-        const int c = 32 * k + j;
-        if (c < p.C) {  // warp-uniform
-          const float xc = __shfl_sync(0xffffffffu, xr[k], j);
-          d = fmaf(xc * inv, sncT[c * 32 + lane], d);
-        }
-      }
-    }
+    for_each_channel(xr, p.C, [&](int c, float xc) { d = fmaf(xc * inv, sncT[c * 32 + lane], d); });
     const float ip = (lane < p.n) ? d : -INFINITY;
     const float best = warp_max(ip);
     const int arg = __ffs(__ballot_sync(0xffffffffu, ip == best)) - 1;  // first maximum, like torch.argmax
@@ -285,20 +252,9 @@ linear_logits_kernel(const float* __restrict__ code, long long ld_code, int C, c
   const float bk = (lane < n) ? bias[lane] : 0.f;
   for (long long r = 1ll * blockIdx.x * 8 + warp; r < rows; r += 1ll * gridDim.x * 8) {
     float xr[3];
-#pragma unroll
-    for (int k = 0; k < 3; ++k) {
-      const int c = lane + 32 * k;
-      xr[k] = (c < C) ? code[r * ld_code + c] : 0.f;
-    }
+    load_channels(code + r * ld_code, C, lane, xr);
     float d = bk;
-#pragma unroll
-    for (int k = 0; k < 3; ++k) {
-#pragma unroll 8
-      for (int j = 0; j < 32; ++j) {
-        const int c = 32 * k + j;
-        if (c < C) d = fmaf(__shfl_sync(0xffffffffu, xr[k], j), sw[c * 32 + lane], d);
-      }
-    }
+    for_each_channel(xr, C, [&](int c, float xc) { d = fmaf(xc, sw[c * 32 + lane], d); });
     logits[r * LP_LD + lane] = (lane < n) ? d : 0.f;
   }
 }
@@ -312,16 +268,6 @@ struct LinearCEParams {
   double* acc;           // [2]: loss sum, valid count (zeroed before the launch)
   int tiles_y, tiles_x, box_h, box_w;
 };
-
-__device__ __forceinline__ void src_index(int dst, float scale, int in_size, int& i0, int& i1, float& l1) {
-  // ATen area_pixel_compute_source_index (align_corners=False, non-cubic): clamp negative to 0
-  float s = scale * (dst + 0.5f) - 0.5f;
-  if (s < 0.f) s = 0.f;
-  i0 = static_cast<int>(s);
-  if (i0 > in_size - 1) i0 = in_size - 1;
-  i1 = i0 + ((i0 < in_size - 1) ? 1 : 0);
-  l1 = s - i0;
-}
 
 constexpr int LCE_TILE = 16;  // hi-res pixels per tile side (256 threads = one per pixel)
 
@@ -352,13 +298,9 @@ linear_ce_kernel(LinearCEParams p) {
   const int Y0 = ty * LCE_TILE, X0 = tx * LCE_TILE;
   const int Yl = min(Y0 + LCE_TILE - 1, p.H - 1), Xl = min(X0 + LCE_TILE - 1, p.W - 1);
   const float sy = static_cast<float>(p.h) / p.H, sx = static_cast<float>(p.w) / p.W;
-  int by0, by1, bx0, bx1, tmp;
-  float ftmp;
-  src_index(Y0, sy, p.h, by0, tmp, ftmp);
-  src_index(Yl, sy, p.h, tmp, by1, ftmp);
-  src_index(X0, sx, p.w, bx0, tmp, ftmp);
-  src_index(Xl, sx, p.w, tmp, bx1, ftmp);
-  const int bh = by1 - by0 + 1, bw = bx1 - bx0 + 1;  // <= box_h, box_w by construction on the host
+  int by0, bh, bx0, bw;  // bh <= box_h, bw <= box_w by construction on the host
+  src_span(Y0, Yl, sy, p.h, by0, bh);
+  src_span(X0, Xl, sx, p.w, bx0, bw);
   const long long base = 1ll * b * p.h * p.w;
   const int tid = threadIdx.x;
   const int warp = tid >> 5, lane = tid & 31;
@@ -400,13 +342,7 @@ linear_ce_kernel(LinearCEParams p) {
   const int py = tid / LCE_TILE, px = tid % LCE_TILE;
   const int Y = Y0 + py, X = X0 + px;
   const bool inb = (Y < p.H) && (X < p.W);
-  long long lab = -1;
-  if (inb) {
-    const long long li = (1ll * b * p.H + Y) * p.W + X;
-    if (p.label_bytes == 8) lab = reinterpret_cast<const long long*>(p.label)[li];
-    else if (p.label_bytes == 4) lab = reinterpret_cast<const int*>(p.label)[li];
-    else lab = reinterpret_cast<const unsigned char*>(p.label)[li];  // values >= n (e.g. 255) are ignored below
-  }
+  const long long lab = inb ? read_label(p.label, p.label_bytes, (1ll * b * p.H + Y) * p.W + X) : -1;
   const bool valid = inb && lab >= 0 && lab < n;
   float lsum = 0.f, cnt = 0.f;
   {
@@ -614,12 +550,7 @@ extern "C" int stego_cluster_lookup_bwd(const float* x, long long stride_b, long
   } else {
     const int grid = cluster_grid(total);
     const size_t smem = (size_t)(2 * n_classes * C + 8) * sizeof(float);  // 48 KB and more from n * C > 6140
-    static size_t configured = 0;
-    if (smem > 48 * 1024 && smem > configured) {
-      cudaError_t e = cudaFuncSetAttribute(cluster_lookup_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-      if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(cluster_lookup_kernel<bwd>)");
-      configured = smem;
-    }
+    if ((rc = opt_in_smem<cluster_lookup_kernel<true>>(smem, "cluster_lookup_kernel<bwd>")) != STEGO_OK) return rc;
     cluster_lookup_kernel<true><<<grid, PR_THREADS, smem, stream>>>(p);
     STEGO_CHECK_LAUNCH("cluster_lookup_kernel<bwd>");
   }
@@ -660,22 +591,14 @@ extern "C" int stego_linear_probe_ce(const float* code, long long ld_code, int C
   p.acc = reinterpret_cast<double*>(partials_scratch);
   p.tiles_y = (H + LCE_TILE - 1) / LCE_TILE;
   p.tiles_x = (Wimg + LCE_TILE - 1) / LCE_TILE;
-  p.box_h = (int)((double)LCE_TILE * h / H) + 3;
-  p.box_w = (int)((double)LCE_TILE * w / Wimg) + 3;
-  if (p.box_h > h) p.box_h = h;
-  if (p.box_w > w) p.box_w = w;
+  p.box_h = src_span_max(LCE_TILE, h, H);
+  p.box_w = src_span_max(LCE_TILE, w, Wimg);
   const size_t region = std::max((size_t)LCE_TILE * p.box_w * n_classes, (size_t)LCE_TILE * p.box_h * LCE_SLD);
   const size_t ce_smem = ((size_t)p.box_h * p.box_w * LCE_SLD + 256 * (size_t)n_classes + region +
                           (size_t)LCE_TILE * (p.box_w + p.box_h)) * sizeof(float);
   STEGO_CHECK_ARG(ce_smem <= 200 * 1024, "stego_linear_probe_ce: upsample ratio %dx%d -> %dx%d needs %zu B of smem", h, w, H, Wimg, ce_smem);
-  {
-    static size_t configured = 0;
-    if (ce_smem > 48 * 1024 && ce_smem > configured) {
-      cudaError_t e = cudaFuncSetAttribute(linear_ce_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ce_smem);
-      if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(linear_ce)");
-      configured = ce_smem;
-    }
-  }
+  int rc = opt_in_smem<linear_ce_kernel>(ce_smem, "linear_ce_kernel");
+  if (rc != STEGO_OK) return rc;
   {
     cudaError_t e = cudaMemsetAsync(partials_scratch, 0, 2 * sizeof(double), stream);
     if (e != cudaSuccess) return cuda_fail(e, "cudaMemsetAsync(linear_ce acc)");
@@ -688,12 +611,7 @@ extern "C" int stego_linear_probe_ce(const float* code, long long ld_code, int C
   if (dlogits_scratch) {
     const unsigned blocks = (unsigned)((rows + LW_ROWS - 1) / LW_ROWS);
     const size_t wsmem = (size_t)(LW_ROWS * 32 + LW_ROWS * C) * sizeof(float);
-    static size_t wconf = 0;
-    if (wsmem > 48 * 1024 && wsmem > wconf) {
-      cudaError_t e = cudaFuncSetAttribute(linear_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wsmem);
-      if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(linear_wgrad)");
-      wconf = wsmem;
-    }
+    if ((rc = opt_in_smem<linear_wgrad_kernel>(wsmem, "linear_wgrad_kernel")) != STEGO_OK) return rc;
     linear_wgrad_kernel<<<blocks, 256, wsmem, stream>>>(dlogits_scratch, code, ld_code, C, n_classes, rows, loss_out,
                                                         grad_loss, dW, db);
     STEGO_CHECK_LAUNCH("linear_wgrad_kernel");

@@ -15,21 +15,7 @@ from typing import Optional, Sequence, Tuple
 
 import torch
 
-from . import _lib
-
-
-def _tokens_major(code: torch.Tensor) -> torch.Tensor:
-    """fp32 view whose pixel (b, y, x) is row b*h*w + y*w + x at stride ld = stride(3), channels contiguous: the
-    addressing of the kernels.  Other views (NCHW, code[::2], crops) are copied."""
-    x = code.detach()
-    B, _, h, w = x.shape
-    if (x.dtype != torch.float32 or x.stride(1) != 1 or x.stride(2) != w * x.stride(3)
-            or (B > 1 and x.stride(0) != h * w * x.stride(3))):
-        x = x.float().permute(0, 2, 3, 1).contiguous().permute(0, 3, 1, 2)
-    return x
-
-
-_LABEL_BYTES = {torch.int64: 8, torch.int32: 4, torch.uint8: 1}
+from . import _lib, ops
 
 
 def fused_probe_log_probs(code: torch.Tensor, linear_probe: torch.nn.Module, cluster_probe: torch.nn.Module,
@@ -49,12 +35,12 @@ def fused_probe_log_probs(code: torch.Tensor, linear_probe: torch.nn.Module, clu
         raise RuntimeError("stego_b200.eval: CUDA tensors required (no CPU fallback)")
     B, C, h, w = code.shape
     H, W = int(size[0]), int(size[1])
-    x = _tokens_major(code)
+    x = ops.tokens_major(code)
     ld = x.stride(3)
     xf = None
     if code_flipped is not None:
         assert code_flipped.shape == code.shape
-        xf = _tokens_major(code_flipped)
+        xf = ops.tokens_major(code_flipped)
         if xf.stride(3) != ld:  # one ld for both codes
             xf = xf.permute(0, 2, 3, 1).contiguous().permute(0, 3, 1, 2)
             x = x.permute(0, 2, 3, 1).contiguous().permute(0, 3, 1, 2)
@@ -72,11 +58,7 @@ def fused_probe_log_probs(code: torch.Tensor, linear_probe: torch.nn.Module, clu
     lab, lab_bytes, n_cls = None, 0, 0
     if label is not None:
         _lib.require_cuda(label, linear_confusion, cluster_confusion)
-        lab = label.reshape(B, H, W)
-        if lab.dtype not in _LABEL_BYTES:
-            lab = lab.to(torch.long)
-        lab = lab.contiguous()
-        lab_bytes = _LABEL_BYTES[lab.dtype]
+        lab, lab_bytes = ops.probe_label(label, B, H, W)
         n_cls = n_lin
         for t, n in ((linear_confusion, n_lin), (cluster_confusion, n_clu)):
             if t is not None:

@@ -25,10 +25,6 @@ import torch
 from . import _lib, corr, ops
 
 
-# label dtypes the linear-probe CE kernel reads directly (int64 is the reference's; uint8 uses 255 = ignore)
-_LABEL_BYTES = {torch.int64: 8, torch.int32: 4, torch.uint8: 1}
-
-
 def _round_up(a: int, b: int) -> int:
     return (a + b - 1) // b * b
 
@@ -56,7 +52,7 @@ class FusedStep:
                 and cfg.rec_weight == 0 and cfg.aug_alignment_weight == 0 and cfg.crf_weight == 0
                 and cfg.neg_samples >= 1 and cfg.dino_feat_type == "feat"
                 and seg.linear_probe.weight.shape[0] <= 32 and seg.net.dim <= 96
-                and batch["label"].dtype in _LABEL_BYTES)
+                and batch["label"].dtype in ops.LABEL_BYTES)
 
     # ------------------------------------------------------------------------------------------
     def _alloc(self, B, H, W, LH, LW, dev, label_dtype):
@@ -104,14 +100,14 @@ class FusedStep:
         n_clu = seg.cluster_probe.clusters.shape[0]
         ws.n_lin, ws.n_clu = n_lin, n_clu
         ws.logits = torch.empty(B * hw, 32, dtype=f32, device=dev)
-        ws.ce_partials = torch.empty(16 * ws.num_sms * 2, dtype=f32, device=dev)
+        ws.ce_partials = ops.probe_scratch(dev)
         ws.lin_loss = torch.empty(2, dtype=f32, device=dev)
         ws.clu_loss = torch.empty(2, dtype=f32, device=dev)
-        ws.clu_scratch = torch.empty(16 * ws.num_sms, dtype=f32, device=dev)
+        ws.clu_scratch = ops.probe_scratch(dev)
         ws.one = torch.ones(1, dtype=f32, device=dev)
         ws.out4 = torch.empty(4, dtype=f32, device=dev)
         ws.label = torch.empty(B, LH, LW, dtype=label_dtype, device=dev)  # static copy: the tail graph bakes pointers
-        ws.label_bytes = _LABEL_BYTES[label_dtype]
+        ws.label_bytes = ops.LABEL_BYTES[label_dtype]
         ws.graph = None
         ws.eager_steps = 0
         # everything the kernels accumulate into: ONE buffer, ONE memset per step

@@ -407,8 +407,7 @@ class _ClusterLookupFn(torch.autograd.Function):
             xf = xf.contiguous()
         cl = clusters.detach().float().contiguous()
         loss = torch.empty(2, dtype=torch.float32, device=dev)
-        scratch = torch.empty(16 * torch.cuda.get_device_properties(dev).multi_processor_count, dtype=torch.float32,
-                              device=dev)
+        scratch = ops.probe_scratch(dev)
         probs = torch.empty(B, n, H, W, dtype=torch.float32, device=dev) if want_probs else None
         logp = torch.empty(B, n, H, W, dtype=torch.float32, device=dev) if want_logp else None
         rc = _lib.load().stego_cluster_lookup_fwd(

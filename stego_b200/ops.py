@@ -2,7 +2,8 @@
 
 These take torch CUDA tensors, pass raw device pointers + sizes + the current stream through
 ctypes and return torch tensors.  They allocate outputs with torch (PyTorch owns all memory) and
-never fall back to torch math.
+never fall back to torch math.  The probe entry points also share their input formats from here: the label
+dtypes, the tokens-major code view and the partials scratch.
 """
 from __future__ import annotations
 
@@ -103,3 +104,34 @@ def attention_probs(qkv: torch.Tensor, out: torch.Tensor, B: int, N: int, E: int
     _lib.check(_lib.load().stego_attention_probs(_lib.ptr(qkv), _lib.ptr(out), B, N, E, heads, _lib.stream()),
                "stego_attention_probs")
     return out
+
+
+# label dtypes the probe kernels read directly, by element size (int64 is the reference's; uint8 uses 255 = ignore)
+LABEL_BYTES = {torch.int64: 8, torch.int32: 4, torch.uint8: 1}
+
+
+def probe_label(label: torch.Tensor, B: int, H: int, W: int):
+    """(label, label_bytes) as the probe kernels read it: [B, H, W] contiguous int64 / int32 / uint8; any other dtype
+    becomes int64."""
+    lab = label.reshape(B, H, W)
+    if lab.dtype not in LABEL_BYTES:
+        lab = lab.to(torch.long)
+    lab = lab.contiguous()
+    return lab, LABEL_BYTES[lab.dtype]
+
+
+def tokens_major(code: torch.Tensor) -> torch.Tensor:
+    """Detached fp32 view of code [B, C, h, w] whose pixel (b, y, x) is row b*h*w + y*w + x at stride ld = stride(3),
+    channels contiguous: the addressing of the probe kernels.  Other views (NCHW, code[::2], crops) are copied."""
+    x = code.detach()
+    B, _, h, w = x.shape
+    if (x.dtype != torch.float32 or x.stride(1) != 1 or x.stride(2) != w * x.stride(3)
+            or (B > 1 and x.stride(0) != h * w * x.stride(3))):
+        x = x.float().permute(0, 2, 3, 1).contiguous().permute(0, 3, 1, 2)
+    return x
+
+
+def probe_scratch(device) -> torch.Tensor:
+    """The partials scratch of stego_cluster_lookup_fwd and stego_linear_probe_ce: 16 floats per SM."""
+    sms = torch.cuda.get_device_properties(device).multi_processor_count
+    return torch.empty(16 * sms, dtype=torch.float32, device=device)

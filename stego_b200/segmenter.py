@@ -25,7 +25,7 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
-from . import _lib, corr
+from . import _lib, corr, ops
 from .modules import ClusterLookup, ContrastiveCorrelationLoss, ContrastiveCRFLoss, DinoFeaturizer, \
     FeaturePyramidNet, _ClusterLookupFn, norm, pixel_cosine, sample
 
@@ -188,23 +188,14 @@ class _LinearProbeCEFn(torch.autograd.Function):
         dev = code_nchw.device
         if n > 32 or C > 96:
             raise RuntimeError(f"stego_b200 linear probe: n_classes={n} (<=32) / dim={C} (<=96) unsupported")
-        x = code_nchw.detach()
-        # the kernels address row b*h*w + y*w + x at stride ld: a batch stride other than h*w*ld (code[::2], a crop) is copied
-        if (x.dtype != torch.float32 or x.stride(1) != 1 or x.stride(2) != w * x.stride(3)
-                or (B > 1 and x.stride(0) != h * w * x.stride(3))):
-            x = x.float().permute(0, 2, 3, 1).contiguous().permute(0, 3, 1, 2)
+        x = ops.tokens_major(code_nchw)
         ld = x.stride(3)
         rows = B * h * w
         H, W = label.shape[-2], label.shape[-1]
-        lab = label.reshape(B, H, W)
-        if lab.dtype not in (torch.int64, torch.int32, torch.uint8):
-            lab = lab.to(torch.long)
-        lab = lab.contiguous()
-        label_bytes = {torch.int64: 8, torch.int32: 4, torch.uint8: 1}[lab.dtype]
+        lab, label_bytes = ops.probe_label(label, B, H, W)
         logits = torch.empty(rows, 32, dtype=torch.float32, device=dev)
         dlogits = torch.zeros(rows, 32, dtype=torch.float32, device=dev)
-        partials = torch.empty(16 * torch.cuda.get_device_properties(dev).multi_processor_count * 2,
-                               dtype=torch.float32, device=dev)
+        partials = ops.probe_scratch(dev)
         loss = torch.empty(2, dtype=torch.float32, device=dev)
         dW = torch.zeros(n, C, dtype=torch.float32, device=dev)
         db = torch.zeros(n, dtype=torch.float32, device=dev)
