@@ -18,6 +18,7 @@ TRAIN_DEFAULTS = dict(
     rec_weight=0.0, repulsion_weight=0.0, crf_weight=0.0,
     alpha=.5, beta=.15, gamma=.05, w1=10.0, w2=3.0, shift=0.00, crf_samples=1000,
     reset_probe_steps=None, hist_freq=100, batch_size=16, res=224, dataset_name="cocostuff27", output_root="../",
+    n_images=5,  # images per validation_step preview
     # stego_b200 execution switches (not in the reference config; read with getattr(..., default) by the modules)
     cuda_graph=True,   # replay the frozen ViT as one CUDA graph per input shape
     fused_step=True,   # hand-scheduled training step (fused_step.py) instead of the autograd-stitched one

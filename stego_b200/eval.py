@@ -97,6 +97,21 @@ class UnsupervisedMetrics:
     def reset(self):
         self.stats.zero_()
 
+    def map_clusters(self, clusters: torch.Tensor) -> torch.Tensor:
+        """utils.py:231-243: cluster ids -> the class ids the Hungarian matching of the last `compute()` assigned them.
+        With extra clusters, the unmatched ones map to -1 by the reference's own insertion rule (each missing index m
+        inserts -1 at position m + 1 of the assignment vector, or appends it at the end)."""
+        import numpy as np
+        cluster_to_class = self.assignments[1]
+        if self.extra_clusters > 0:
+            missing = sorted(set(range(self.n_classes + self.extra_clusters)) - set(self.assignments[0]))
+            for m in missing:
+                if m == cluster_to_class.shape[0]:
+                    cluster_to_class = np.append(cluster_to_class, -1)
+                else:
+                    cluster_to_class = np.insert(cluster_to_class, m + 1, -1)
+        return torch.as_tensor(cluster_to_class, device=clusters.device)[clusters]
+
     def compute(self):
         import numpy as np
         from scipy.optimize import linear_sum_assignment

@@ -474,3 +474,54 @@ class LitUnsupervisedSegmenter(nn.Module):
             self.reset_probes()
         self.global_step += 1
         return loss
+
+    # ---- validation -------------------------------------------------------------------------------
+    def validation_step(self, batch, batch_idx):
+        """train_segmentation.py:254-275: the eval-mode net, then upsampling to the label size, both probes, both
+        argmaxes and both `UnsupervisedMetrics.update` calls as ONE fused_probe_log_probs pass (the upsampled code is
+        never materialised).  `cluster_probe(code, None)[1].argmax(1)` is the argmax of the inner products, which is
+        the argmax of the kernel's alpha = 2 logits.
+
+        Waits for the previous step's parameter update, draws no random numbers and leaves the training step's CUDA
+        graphs and workspace alone.  The net's train / eval modes are restored on exit: there is no Trainer to call
+        `.train()` afterwards, and the hand-scheduled step only runs on a net in training mode.  Returns the
+        reference's preview dict on the CPU (first cfg.n_images entries, int64 predictions)."""
+        from .eval import fused_probe_log_probs
+        self.flush()
+        img, label = batch["img"], batch["label"]
+        n_images = getattr(self.cfg, "n_images", 5)
+        modes = [(m, m.training) for m in self.net.modules()]
+        self.net.eval()
+        try:
+            with torch.no_grad():
+                _, code = self.net(img)
+                out = fused_probe_log_probs(code, self.linear_probe, self.cluster_probe, label.shape[-2:], 2.0,
+                                            want_log_probs=False, want_argmax=n_images > 0, label=label,
+                                            linear_confusion=self.linear_metrics.stats,
+                                            cluster_confusion=self.cluster_metrics.stats)
+        finally:
+            for m, mode in modes:
+                m.training = mode
+        none = torch.empty(0, *label.shape[-2:], dtype=torch.long)
+        return {"img": img[:n_images].detach().cpu(),
+                "linear_preds": out[2][:n_images].long().cpu() if n_images > 0 else none,
+                "cluster_preds": out[3][:n_images].long().cpu() if n_images > 0 else none,
+                "label": label[:n_images].detach().cpu()}
+
+    def validation_epoch_end(self, outputs=None) -> Dict[str, float]:
+        """train_segmentation.py:277-283, 361-371 without the figures: sum both confusion matrices over the ranks (what
+        torchmetrics' dist_reduce_fx="sum" does; once per epoch gives the same sums as once per step), compute mIoU /
+        accuracy, log them once global_step > 2, reset both metrics.  Returns the metric dict (keys `test/linear/mIoU`,
+        `test/linear/Accuracy`, `test/cluster/mIoU`, `test/cluster/Accuracy`) for callers that pick checkpoints
+        themselves.  The Hungarian assignment stays on `cluster_metrics` for `map_clusters`."""
+        import torch.distributed as dist
+        if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
+            for m in (self.linear_metrics, self.cluster_metrics):
+                dist.all_reduce(m.stats, op=dist.ReduceOp.SUM)
+        tb_metrics = {**self.linear_metrics.compute(), **self.cluster_metrics.compute()}
+        if self.global_step > 2:
+            for k, v in tb_metrics.items():
+                self.log(k, v)
+        self.linear_metrics.reset()
+        self.cluster_metrics.reset()
+        return tb_metrics
