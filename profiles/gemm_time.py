@@ -76,9 +76,6 @@ def cases(cfg, dev):
     dyb[:, :D] = bf(Mh, D)
     dh, dw, dwa = torch.empty(Mh, E, device=dev), torch.zeros(D, E, device=dev), torch.zeros(E, E, device=dev)
 
-    def splits_for(r, c):
-        return max(1, min(Mh // 512, sms // (((r + 127) // 128) * ((c + 127) // 128))))
-
     def lin(M, N, K, out_b, res_b=0, extra_b=0):  # flops, bytes
         return 2.0 * M * N * K, 2.0 * (M * K + N * K) + M * N * (out_b + res_b) + extra_b
 
@@ -102,9 +99,11 @@ def cases(cfg, dev):
         ("head_dgrad", lin(Mh, E, 128, 4),
          lambda: ops.gemm(dyb, wbp, dh, M=Mh, N=E, K=128, b_mn=True)),
         ("head_wgrad_cluster", lin(D, E, Mh, 4),
-         lambda: ops.gemm(dyb, x1, dw, M=D, N=E, K=Mh, a_mn=True, b_mn=True, splits=splits_for(D, E), atomic=True)),
+         lambda: ops.gemm(dyb, x1, dw, M=D, N=E, K=Mh, a_mn=True, b_mn=True, splits=ops.wgrad_splits(Mh, D, E, sms),
+                          atomic=True)),
         ("head_wgrad_a", lin(E, E, Mh, 4),
-         lambda: ops.gemm(hh, x1, dwa, M=E, N=E, K=Mh, a_mn=True, b_mn=True, splits=splits_for(E, E), atomic=True)),
+         lambda: ops.gemm(hh, x1, dwa, M=E, N=E, K=Mh, a_mn=True, b_mn=True, splits=ops.wgrad_splits(Mh, E, E, sms),
+                          atomic=True)),
     ]
 
 

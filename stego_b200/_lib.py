@@ -81,6 +81,24 @@ def launch_count() -> int:
     return int(load().stego_launch_count()) + replayed_launches
 
 
+class Graph:
+    """`fn()` captured as one CUDA graph on the current stream, with its result; `replay` counts the graph's launches
+    of this library in replayed_launches (stego_launch_count does not see them)."""
+
+    def __init__(self, fn):
+        torch.cuda.synchronize()
+        self.graph = torch.cuda.CUDAGraph()
+        n0 = load().stego_launch_count()
+        with torch.cuda.graph(self.graph):
+            self.result = fn()
+        self.launches = load().stego_launch_count() - n0
+
+    def replay(self) -> None:
+        global replayed_launches
+        self.graph.replay()
+        replayed_launches += self.launches
+
+
 def last_error() -> str:
     return load().stego_last_error().decode("utf-8", "replace")
 

@@ -133,18 +133,30 @@ def make_spec(cfg, n_neg: Optional[int] = None):
 def build_tiles(src: torch.Tensor, src_pos: torch.Tensor, coords1: torch.Tensor, coords2: torch.Tensor,
                 perms: Optional[torch.Tensor], spec: LossSpec, c_pad: int,
                 chan_scale: Optional[torch.Tensor] = None, chan_scale_pos: Optional[torch.Tensor] = None,
-                raw_perms: bool = False) -> torch.Tensor:
-    """sample + norm for every slot -> bf16 hi/lo tiles [2][nslots][B][spec.rows][c_pad]."""
+                raw_perms: bool = False, *, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """sample + norm for every slot -> bf16 hi/lo tiles [2][nslots][B][spec.rows][c_pad], written into `out` when it
+    is given.  src_pos is copied into src's strides unless it has them already."""
     B, C, H, W = src.shape
     src_pos = _same_layout(src, src_pos)
-    tiles = torch.empty(2, spec.nslots, B, spec.rows, c_pad, dtype=torch.bfloat16, device=src.device)
+    if out is None:
+        out = torch.empty(2, spec.nslots, B, spec.rows, c_pad, dtype=torch.bfloat16, device=src.device)
     sb, sc, sy, sx = src.stride()
     rc = _lib.load().stego_sample_norm_fwd(
         _lib.ptr(src), _lib.ptr(src_pos), int(src.dtype == torch.bfloat16), sb, sc, sy, sx,
         _lib.ptr(chan_scale), _lib.ptr(chan_scale_pos), _lib.ptr(coords1), _lib.ptr(coords2), _lib.ptr(perms),
-        _lib.ptr(tiles), B, C, c_pad, H, W, spec.fs, spec.nslots, int(raw_perms), _lib.stream())
+        _lib.ptr(out), B, C, c_pad, H, W, spec.fs, spec.nslots, int(raw_perms), _lib.stream())
     _lib.check(rc, "stego_sample_norm_fwd")
-    return tiles
+    return out
+
+
+def sample_norm_backward(code, code_pos, coords1, coords2, perms, spec, dtiles, dcode, dcode_pos, raw_perms=False):
+    """dcode / dcode_pos += dtiles taken back through build_tiles of fp32 code / code_pos [B, D, H, W] (all four in
+    code's strides): they must arrive zeroed."""
+    B, D, H, W = code.shape
+    _lib.check(_lib.load().stego_sample_norm_bwd(
+        _lib.ptr(code), _lib.ptr(code_pos), *code.stride(), _lib.ptr(coords1), _lib.ptr(coords2), _lib.ptr(perms),
+        _lib.ptr(dtiles), _lib.ptr(dcode), _lib.ptr(dcode_pos), B, D, H, W, spec.fs, spec.nslots, int(raw_perms),
+        _lib.stream()), "stego_sample_norm_bwd")
 
 
 def _prep_common(feats, feats_pos, code, code_pos, coords1, coords2, perms, spec: LossSpec):
@@ -240,12 +252,8 @@ class _CorrLossFn(torch.autograd.Function):
         else:
             dcode = _zeros_strided_like(code_f)
             dcode_pos = _zeros_strided_like(code_f)
-        sb, sc, sy, sx = code_f.stride()
-        rc = _lib.load().stego_sample_norm_bwd(
-            _lib.ptr(code_f), _lib.ptr(code_pos_f), sb, sc, sy, sx, _lib.ptr(coords1), _lib.ptr(coords2),
-            _lib.ptr(perms_arg), _lib.ptr(dtiles), _lib.ptr(dcode), _lib.ptr(dcode_pos), B, D, H, W, spec.fs,
-            spec.nslots, int(ctx.raw_perms), _lib.stream())
-        _lib.check(rc, "stego_sample_norm_bwd")
+        sample_norm_backward(code_f, code_pos_f, coords1, coords2, perms_arg, spec, dtiles, dcode, dcode_pos,
+                             ctx.raw_perms)
         d0, d1 = ctx.code_dtype
         if ctx.pair:
             return (dall.to(d0), None) + (None,) * 11

@@ -255,21 +255,15 @@ class VisionTransformer(nn.Module):
         if key not in graphs:
             img = torch.cat([p.to(dt) for p in parts], 0) if len(parts) > 1 else parts[0].to(dt)
             self._patch_features_eager(img)  # warm-up: kernel attributes, pos-embed cache, allocator
-            torch.cuda.synchronize()
             static_in = img.detach().contiguous().clone()
-            g = torch.cuda.CUDAGraph()
-            n0 = _lib.load().stego_launch_count()
-            with torch.cuda.graph(g):
-                static_out = self._patch_features_eager(static_in)
-            graphs[key] = (g, static_in, static_out, _lib.load().stego_launch_count() - n0)
-        g, static_in, static_out, nlaunch = graphs[key]
+            graphs[key] = (_lib.Graph(lambda: self._patch_features_eager(static_in)), static_in)
+        g, static_in = graphs[key]
         off = 0
         for part in parts:
             static_in[off:off + part.shape[0]].copy_(part)
             off += part.shape[0]
         g.replay()
-        _lib.replayed_launches += nlaunch
-        return static_out
+        return g.result
 
     def _patch_features_eager(self, img: torch.Tensor) -> torch.Tensor:
         B = img.shape[0]

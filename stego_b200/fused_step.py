@@ -1,5 +1,5 @@
 """Hand-scheduled training step: the kernel sequence of `LitUnsupervisedSegmenter.training_step`
-(src/train_segmentation.py:112-245) issued directly through the C-ABI, without autograd.
+(src/train_segmentation.py:112-245) without autograd.
 
 The autograd path (segmenter._training_step_autograd) stitches ~10 custom nodes together and leaves ~110 tiny
 torch kernels (zero fills, RNG post-processing, gradient accumulation, scalar loss arithmetic) on the critical
@@ -10,11 +10,13 @@ path, each costing ~4 us of launch latency behind the frozen ViT.  Here
     draws (same torch RNG calls in the same order as the reference: net(img) x3 noises, net(img_pos) x3,
     rand x2, randperm x neg_samples), the bf16 operand copies of the trainable head weights, and ONE memset of
     all accumulate-into buffers (+ the flat gradient buffer) — runs on a side stream concurrently with the ViT graph;
-  * forward and backward kernels are called in order, weight gradients are accumulated straight into the flat
+  * forward and backward stages are called in order, weight gradients are accumulated straight into the flat
     gradient buffer (no per-parameter AccumulateGrad kernels), and the scalar loss arithmetic is one launch.
 
-Numerically this is the same kernel sequence as the autograd path (tests/test_modules_gpu.py checks both against the
-oracle and against each other).
+The stages are the functions the autograd nodes call (modules.pack_head_weights / head_forward / head_backward /
+cluster_lookup_forward / cluster_lookup_backward, corr.build_tiles / sample_norm_backward / LossSpec,
+segmenter.linear_probe_ce_step), given the workspace instead of per-call buffers: both paths launch the same kernels
+with the same arguments.  Only stego_step_losses is called from here alone.
 """
 from __future__ import annotations
 
@@ -22,7 +24,7 @@ import ctypes
 
 import torch
 
-from . import _lib, corr, ops
+from . import _lib, corr, modules, ops, segmenter
 
 
 def _round_up(a: int, b: int) -> int:
@@ -67,7 +69,6 @@ class FusedStep:
         f32, bf = torch.float32, torch.bfloat16
         nonlinear = net.proj_type == "nonlinear"
         ws.dims = (B, E, D, P, fh, fw, hw, M, nonlinear)
-        ws.num_sms = torch.cuda.get_device_properties(dev).multi_processor_count
         # RNG outputs
         ws.M1 = torch.empty(2 * B, E, 1, 1, dtype=f32, device=dev)
         ws.M2 = torch.empty(2 * B, E, 1, 1, dtype=f32, device=dev) if nonlinear else None
@@ -96,9 +97,7 @@ class FusedStep:
         ws.call_w = (ctypes.c_float * len(wts))(*[float(v) for v in wts])
         ws.gscale = torch.tensor([float(v) for v in wts], dtype=f32, device=dev)
         # probes
-        n_lin = seg.linear_probe.weight.shape[0]
         n_clu = seg.cluster_probe.clusters.shape[0]
-        ws.n_lin, ws.n_clu = n_lin, n_clu
         ws.logits = torch.empty(B * hw, 32, dtype=f32, device=dev)
         ws.ce_partials = ops.probe_scratch(dev)
         ws.lin_loss = torch.empty(2, dtype=f32, device=dev)
@@ -107,7 +106,6 @@ class FusedStep:
         ws.one = torch.ones(1, dtype=f32, device=dev)
         ws.out4 = torch.empty(4, dtype=f32, device=dev)
         ws.label = torch.empty(B, LH, LW, dtype=label_dtype, device=dev)  # static copy: the tail graph bakes pointers
-        ws.label_bytes = ops.LABEL_BYTES[label_dtype]
         ws.graph = None
         ws.eager_steps = 0
         # everything the kernels accumulate into: ONE buffer, ONE memset per step
@@ -119,7 +117,6 @@ class FusedStep:
         for name, n in sizes.items():
             setattr(ws, name, ws.zbuf[off:off + n])
             off += _round_up(n, 64)
-        ws.label_shape = (LH, LW)
         return ws
 
     # ------------------------------------------------------------------------------------------
@@ -139,11 +136,8 @@ class FusedStep:
         torch.rand(ws.c2.shape, out=ws.c2).mul_(2).sub_(1)
         for i in range(ws.perms.shape[0]):                  # super_perm's randperm (modules.py:291-295)
             torch.randperm(B, device=ws.perms.device, dtype=torch.long, out=ws.perms[i])
-        c1 = net.cluster1[0]
-        ws.w1p[:D].copy_(c1.weight.detach().view(D, E))
-        if nonlinear:
-            ws.wab.copy_(net.cluster2[0].weight.detach().view(E, E))
-            ws.wbp[:D].copy_(net.cluster2[2].weight.detach().view(D, E))
+        w1, _, wa, _, wb, _ = net.head_params()
+        modules.pack_head_weights(w1, wa, wb, ws.w1p, ws.wab, ws.wbp)
         ws.zbuf.zero_()
         seg._flat.grad.zero_()
 
@@ -151,95 +145,51 @@ class FusedStep:
     def _tail(self, ws, tok_all):
         """Head forward .. head backward on the current stream: static workspace, no allocation, no RNG, no host
         synchronisation — captured as one CUDA graph after the first (eager) step."""
-        seg, cfg, net = self.seg, self.seg.cfg, self.seg.net
-        lib = _lib.load()
+        seg, net = self.seg, self.seg.net
         B, E, D, P, fh, fw, hw, M, nonlinear = ws.dims
         spec = seg._spec
-        st = _lib.stream()
-        feat_tok = tok_all.reshape(M, E)
+        params = net.head_params()
+        _, b1, _, ba, _, bb = params
+        # [2B, C, h, w] views of the tokens-major features and of the padded code storage: img rows, then img_pos rows
+        feats = tok_all.view(2 * B, fh, fw, E).permute(0, 3, 1, 2)
+        code = ws.code.view(2 * B, fh, fw, P)[..., :D].permute(0, 3, 1, 2)
 
         # ---- head forward (modules.py:108-111)
-        _lib.check(lib.stego_head_dropout3(_lib.ptr(feat_tok), _lib.ptr(ws.M1), _lib.ptr(ws.M2), 0, _lib.ptr(ws.x1),
-                                           _lib.ptr(ws.x2), 0, 2 * B, hw, E, st), "stego_head_dropout3")
-        c1 = net.cluster1[0]
-        ops.gemm(ws.x1, ws.w1p, ws.code, M=M, N=D, K=E, bias=c1.bias.detach())
-        if nonlinear:
-            ca, cb = net.cluster2[0], net.cluster2[2]
-            ops.gemm(ws.x2, ws.wab, ws.hid, M=M, N=E, K=E, bias=ca.bias.detach(), act=ops.ACT_RELU)
-            ops.gemm(ws.hid, ws.wbp, ws.code, M=M, N=D, K=E, bias=cb.bias.detach(), residual=ws.code)
+        modules.head_forward(tok_all.reshape(M, E), ws.M1, ws.M2, 2 * B, hw, ws.x1, ws.x2, ws.hid, ws.code, ws.w1p, b1,
+                             ws.wab, ba, ws.wbp, bb)
         seg._mark("head_forward")
 
         # ---- correspondence loss forward (modules.py:349-398)
-        tok_pos = tok_all[B:]
-        m3 = ws.M3[:B] if ws.M3 is not None else None
-        p3 = ws.M3[B:] if ws.M3 is not None else None
-        _lib.check(lib.stego_sample_norm_fwd(
-            _lib.ptr(tok_all), _lib.ptr(tok_pos), 1, hw * E, 1, fw * E, E, _lib.ptr(m3), _lib.ptr(p3),
-            _lib.ptr(ws.c1), _lib.ptr(ws.c2), _lib.ptr(ws.perms), _lib.ptr(ws.ftiles), B, E, E, fh, fw, spec.fs,
-            spec.nslots, 1, st), "stego_sample_norm_fwd")
-        code_pos = ws.code[B * hw:]
-        _lib.check(lib.stego_sample_norm_fwd(
-            _lib.ptr(ws.code), _lib.ptr(code_pos), 0, hw * P, 1, fw * P, P, 0, 0, _lib.ptr(ws.c1), _lib.ptr(ws.c2),
-            _lib.ptr(ws.perms), _lib.ptr(ws.ctiles), B, D, corr.CODE_PAD, fh, fw, spec.fs, spec.nslots, 1, st),
-            "stego_sample_norm_fwd")
+        m3, p3 = (ws.M3[:B], ws.M3[B:]) if ws.M3 is not None else (None, None)
+        corr.build_tiles(feats[:B], feats[B:], ws.c1, ws.c2, ws.perms, spec, E, m3, p3, raw_perms=True, out=ws.ftiles)
+        corr.build_tiles(code[:B], code[B:], ws.c1, ws.c2, ws.perms, spec, corr.CODE_PAD, raw_perms=True,
+                         out=ws.ctiles)
         spec.forward(ws.ftiles, ws.ctiles, B, E, D, ws.partials, ws.row_means, ws.stats)
         seg._mark("corr_loss_forward")
 
         # ---- probes on the detached code (train_segmentation.py:213-225): forward + backward in place
-        lp = seg.linear_probe
-        lab = ws.label
-        LH, LW = ws.label_shape
-        _lib.check(lib.stego_linear_probe_ce(
-            _lib.ptr(ws.code), P, D, _lib.ptr(lp.weight), _lib.ptr(lp.bias), ws.n_lin, _lib.ptr(lab), ws.label_bytes, B, fh, fw,
-            LH, LW,
-            _lib.ptr(ws.logits), _lib.ptr(ws.dlogits), _lib.ptr(ws.ce_partials), _lib.ptr(ws.lin_loss), 1.0,
-            _lib.ptr(lp.weight.grad), _lib.ptr(lp.bias.grad), st), "stego_linear_probe_ce")
-        cl = seg.cluster_probe.clusters
-        _lib.check(lib.stego_cluster_lookup_fwd(
-            _lib.ptr(ws.code), hw * P, 1, P, _lib.ptr(cl), B, D, ws.n_clu, hw, 0, 0.0, 0, 0, 0, _lib.ptr(ws.clu_loss),
-            _lib.ptr(ws.clu_scratch), st), "stego_cluster_lookup_fwd")
-        out4 = ws.out4
-        _lib.check(lib.stego_step_losses(_lib.ptr(ws.stats), spec.ncalls, ws.call_w, _lib.ptr(ws.lin_loss),
-                                         _lib.ptr(ws.clu_loss), _lib.ptr(out4), st), "stego_step_losses")
+        lp, cl = seg.linear_probe, seg.cluster_probe.clusters
+        segmenter.linear_probe_ce_step(code[:B], lp.weight, lp.bias, ws.label, ws.logits, ws.dlogits, ws.ce_partials,
+                                       ws.lin_loss, lp.weight.grad, lp.bias.grad, 1.0)
+        modules.cluster_lookup_forward(code[:B], cl, None, ws.clu_loss, ws.clu_scratch)
+        _lib.check(_lib.load().stego_step_losses(_lib.ptr(ws.stats), spec.ncalls, ws.call_w, _lib.ptr(ws.lin_loss),
+                                                 _lib.ptr(ws.clu_loss), _lib.ptr(ws.out4), _lib.stream()),
+                   "stego_step_losses")
         seg._mark("probes_forward")
 
         # ---- backward (manual_backward, :227)
-        _lib.check(lib.stego_cluster_lookup_bwd(
-            _lib.ptr(ws.code), hw * P, 1, P, _lib.ptr(cl), B, D, ws.n_clu, hw, 0, 0.0, _lib.ptr(ws.one),
-            _lib.ptr(ws.dnc), _lib.ptr(cl.grad), st), "stego_cluster_lookup_bwd")
+        modules.cluster_lookup_backward(code[:B], cl, None, ws.one, ws.dnc, cl.grad)
         spec.backward(ws.ftiles, ws.ctiles, B, E, D, ws.stats, ws.row_means, ws.gscale, None, None, ws.dtiles)
-        dall_pos = ws.dall[B * hw * P:]
-        _lib.check(lib.stego_sample_norm_bwd(
-            _lib.ptr(ws.code), _lib.ptr(code_pos), hw * P, 1, fw * P, P, _lib.ptr(ws.c1), _lib.ptr(ws.c2),
-            _lib.ptr(ws.perms), _lib.ptr(ws.dtiles), _lib.ptr(ws.dall), _lib.ptr(dall_pos), B, D, fh, fw, spec.fs,
-            spec.nslots, 1, st), "stego_sample_norm_bwd")
+        dall = ws.dall.view(M, P)
+        corr.sample_norm_backward(code[:B], code[B:], ws.c1, ws.c2, ws.perms, spec, ws.dtiles, dall[:B * hw],
+                                  dall[B * hw:], raw_perms=True)
         # head backward: d(code) [M, P] -> bias / weight gradients straight into the flat gradient buffer
-        _lib.check(lib.stego_cast_pad_bf16(_lib.ptr(ws.dall), P, D, _lib.ptr(ws.dyb), 128, M, st), "stego_cast_pad_bf16")
-        _lib.check(lib.stego_colsum(_lib.ptr(ws.dall), 0, P, P, M, _lib.ptr(ws.db_pad), st), "stego_colsum")
-        c1.bias.grad.copy_(ws.db_pad[:D])
-
-        def splits_for(out_rows, out_cols):
-            # split-K so that tiles x splits fills ONE wave of the persistent GEMM (one CTA per SM): at most num_sms
-            # CTAs (more splits would make a second round of the grid)
-            tiles = ((out_rows + 127) // 128) * ((out_cols + 127) // 128)
-            return max(1, min(M // 512, ws.num_sms // tiles))
-        ops.gemm(ws.dyb, ws.x1, c1.weight.grad.view(D, E), M=D, N=E, K=M, a_mn=True, b_mn=True,
-                 splits=splits_for(D, E), atomic=True)
-        if nonlinear:
-            cb.bias.grad.copy_(ws.db_pad[:D])
-            ops.gemm(ws.dyb, ws.hid, cb.weight.grad.view(D, E), M=D, N=E, K=M, a_mn=True, b_mn=True,
-                     splits=splits_for(D, E), atomic=True)
-            ops.gemm(ws.dyb, ws.wbp, ws.dh, M=M, N=E, K=128, b_mn=True)
-            _lib.check(lib.stego_relu_bwd_bf16(_lib.ptr(ws.dh), _lib.ptr(ws.hid), _lib.ptr(ws.dhb), M * E, st),
-                       "stego_relu_bwd_bf16")
-            _lib.check(lib.stego_colsum(_lib.ptr(ws.dhb), 1, E, E, M, _lib.ptr(ca.bias.grad), st), "stego_colsum")
-            ops.gemm(ws.dhb, ws.x2, ca.weight.grad.view(E, E), M=E, N=E, K=M, a_mn=True, b_mn=True,
-                     splits=splits_for(E, E), atomic=True)
+        modules.head_backward(dall, ws.x1, ws.x2, ws.hid, ws.wbp, ws.dyb, ws.db_pad, ws.dh, ws.dhb,
+                              *[p.grad if p is not None else None for p in params])
 
     # ------------------------------------------------------------------------------------------
     def run(self, batch):
         seg, cfg, net = self.seg, self.seg.cfg, self.seg.net
-        lib = _lib.load()
         img, img_pos, label = batch["img"], batch["img_pos"], batch["label"]
         dev = img.device
         B, _, H, W = img.shape
@@ -278,18 +228,11 @@ class FusedStep:
             seg._mark("vit_forward")
             if use_graph and ws.graph is not None and ws.graph[1] == tok_all.data_ptr():
                 ws.graph[0].replay()
-                _lib.replayed_launches += ws.graph[2]
             elif use_graph and ws.eager_steps >= 1:
                 # second step on this shape: capture head fwd .. head bwd (static workspace, no allocation, no RNG) as ONE
                 # CUDA graph; the eager first step has already set kernel attributes and warmed the allocator
-                torch.cuda.synchronize()
-                g = torch.cuda.CUDAGraph()
-                n0 = lib.stego_launch_count()
-                with torch.cuda.graph(g):
-                    self._tail(ws, tok_all)
-                ws.graph = (g, tok_all.data_ptr(), lib.stego_launch_count() - n0)
-                g.replay()
-                _lib.replayed_launches += ws.graph[2]
+                ws.graph = (_lib.Graph(lambda: self._tail(ws, tok_all)), tok_all.data_ptr())
+                ws.graph[0].replay()
             else:
                 self._tail(ws, tok_all)
                 ws.eager_steps += 1

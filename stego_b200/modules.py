@@ -125,87 +125,99 @@ class LambdaLayer(nn.Module):
 
 
 # ==================================================================================================
-# segmentation head (cluster1 + cluster2) as one autograd node over wgmma GEMMs
+# segmentation head (cluster1 + cluster2): stage functions over caller-owned buffers (they allocate nothing, so the
+# fused step captures them in its CUDA graph) and the autograd node.  Linear head: every cluster2 argument is None.
 # ==================================================================================================
-class _HeadFn(torch.autograd.Function):
+def pack_head_weights(w1, wa, wb, w1p, wab, wbp) -> None:
+    """bf16 operand copies of the trainable head weights: w1 / wb into the first D rows of w1p / wbp [128, E] (rows
+    >= D must be zero: the dgrad GEMM reads all 128), wa into wab [E, E]."""
+    D = w1.shape[0]
+    w1p[:D].copy_(w1.detach().reshape(D, -1))
+    if wab is not None:
+        wab.copy_(wa.detach().reshape(wab.shape))
+        wbp[:D].copy_(wb.detach().reshape(D, -1))
+
+
+def head_forward(feat_tok, m1, m2, B, hw, x1, x2, hid, code, w1p, b1, wab=None, ba=None, wbp=None, bb=None) -> None:
     """code = conv1x1(E->D)(f*m1) + conv1x1(E->D)(relu(conv1x1(E->E)(f*m2)))   (modules.py:108-111)
 
-    feat_tok: [M, E] bf16 tokens-major (frozen backbone output, no grad); masks: [B, E] fp32 or None.
-    Output: code storage [M, P] fp32 (P = D rounded up to 8; columns >= D are padding)."""
+    feat_tok: [M = B*hw, E] bf16 tokens-major; m1 / m2: [B, E] fp32 Dropout2d noises (x1 / x2 receive f*m1 / f*m2), or
+    None with x1 = x2 = feat_tok.  code: [M, P] fp32 with zero padding columns (P = D rounded up to 8)."""
+    M, E = feat_tok.shape
+    D = b1.shape[0]
+    if m1 is not None:
+        _lib.check(_lib.load().stego_head_dropout3(_lib.ptr(feat_tok), _lib.ptr(m1), _lib.ptr(m2), 0, _lib.ptr(x1),
+                                                   _lib.ptr(x2), 0, B, hw, E, _lib.stream()), "stego_head_dropout3")
+    ops.gemm(x1, w1p, code, M=M, N=D, K=E, bias=b1)
+    if wab is not None:
+        ops.gemm(x2, wab, hid, M=M, N=E, K=E, bias=ba, act=ops.ACT_RELU)
+        ops.gemm(hid, wbp, code, M=M, N=D, K=E, bias=bb, residual=code)
+
+
+def head_backward(dcode, x1, x2, hid, wbp, dyb, db_pad, dh, dhb, dw1, db1, dwa, dba, dwb, dbb) -> None:
+    """The six parameter gradients (in the parameters' shapes) from d(code) [M, >= D] (columns contiguous).  Scratch:
+    dyb [M, 128] bf16, d(code) padded for the GEMMs; db_pad [P], the column sum of d(code) (over its zero padding
+    columns too when it has them: vector loads), copied into both D-wide bias gradients db1 and dbb; dh / dhb [M, E],
+    d(hidden) before / after the ReLU.  db_pad, dw1, dwa, dba and dwb are accumulated into and must arrive zeroed."""
+    M, E = x1.shape
+    D, P, ld = db1.shape[0], db_pad.shape[0], dcode.stride(0)
+    lib, st = _lib.load(), _lib.stream()
+    sms = torch.cuda.get_device_properties(dcode.device).multi_processor_count
+    wgrad = lambda a, b, out, rows: ops.gemm(a, b, out.view(rows, E), M=rows, N=E, K=M, a_mn=True, b_mn=True,
+                                             splits=ops.wgrad_splits(M, rows, E, sms), atomic=True)
+    _lib.check(lib.stego_cast_pad_bf16(_lib.ptr(dcode), ld, D, _lib.ptr(dyb), 128, M, st), "stego_cast_pad_bf16")
+    _lib.check(lib.stego_colsum(_lib.ptr(dcode), 0, ld, P if dcode.shape[1] >= P else D, M, _lib.ptr(db_pad), st),
+               "stego_colsum")
+    db1.copy_(db_pad[:D])
+    wgrad(dyb, x1, dw1, D)
+    if hid is not None:
+        dbb.copy_(db_pad[:D])
+        wgrad(dyb, hid, dwb, D)
+        # dH = dY . Wb  (B operand [K=c][N=E] is MN-major), then ReLU backward -> bf16 operand
+        ops.gemm(dyb, wbp, dh, M=M, N=E, K=128, b_mn=True)
+        _lib.check(lib.stego_relu_bwd_bf16(_lib.ptr(dh), _lib.ptr(hid), _lib.ptr(dhb), M * E, st), "stego_relu_bwd_bf16")
+        _lib.check(lib.stego_colsum(_lib.ptr(dhb), 1, E, E, M, _lib.ptr(dba), st), "stego_colsum")
+        wgrad(dhb, x2, dwa, E)
+
+
+class _HeadFn(torch.autograd.Function):
+    """head_forward / head_backward over per-call buffers.  feat_tok: [M, E] bf16 (no grad); masks: [B, E] fp32 or
+    None.  Output: code storage [M, P] fp32 (columns >= D are padding)."""
 
     @staticmethod
     def forward(ctx, feat_tok, m1, m2, B, hw, w1, b1, wa, ba, wb, bb):
         M, E = feat_tok.shape
-        D = w1.shape[0]
-        dev = feat_tok.device
-        P = _round_up(D, 8)
         nonlinear = wa is not None
+        bf16 = dict(dtype=torch.bfloat16, device=feat_tok.device)
+        w1p = torch.zeros(128, E, **bf16)
+        wab, wbp, hid = (torch.empty(E, E, **bf16), torch.zeros(128, E, **bf16), torch.empty(M, E, **bf16)) \
+            if nonlinear else (None, None, None)
+        pack_head_weights(w1, wa, wb, w1p, wab, wbp)
+        x1 = x2 = feat_tok
         if m1 is not None:
-            x1 = torch.empty_like(feat_tok)
-            x2 = torch.empty_like(feat_tok) if nonlinear else None
-            rc = _lib.load().stego_head_dropout3(_lib.ptr(feat_tok), _lib.ptr(m1), _lib.ptr(m2) if nonlinear else 0, 0,
-                                                 _lib.ptr(x1), _lib.ptr(x2), 0, B, hw, E, _lib.stream())
-            _lib.check(rc, "stego_head_dropout3")
-        else:
-            x1 = x2 = feat_tok
-        # bf16 operand copies of the (small) trainable weights, zero-padded to 128 output rows
-        w1p = torch.zeros(128, E, dtype=torch.bfloat16, device=dev)
-        w1p[:D] = w1.detach().reshape(D, E)
-        code = torch.zeros(M, P, dtype=torch.float32, device=dev)
-        ops.gemm(x1, w1p, code, M=M, N=D, K=E, bias=b1.detach().float().contiguous())
-        hid = wbp = wab = None
-        if nonlinear:
-            wab = wa.detach().reshape(E, E).to(torch.bfloat16).contiguous()
-            wbp = torch.zeros(128, E, dtype=torch.bfloat16, device=dev)
-            wbp[:D] = wb.detach().reshape(D, E)
-            hid = torch.empty(M, E, dtype=torch.bfloat16, device=dev)
-            ops.gemm(x2, wab, hid, M=M, N=E, K=E, bias=ba.detach().float().contiguous(), act=ops.ACT_RELU)
-            ops.gemm(hid, wbp, code, M=M, N=D, K=E, bias=bb.detach().float().contiguous(), residual=code)
-        ctx.save_for_backward(x1, x2 if nonlinear else None, hid, wab, wbp)
-        ctx.dims = (M, E, D, P, nonlinear)
-        ctx.shapes = (w1.shape, wa.shape if nonlinear else None, wb.shape if nonlinear else None)
+            x1, x2 = torch.empty_like(feat_tok), torch.empty_like(feat_tok) if nonlinear else None
+        code = torch.zeros(M, _round_up(w1.shape[0], 8), dtype=torch.float32, device=feat_tok.device)
+        f32 = lambda t: t.detach().float().contiguous() if t is not None else None
+        head_forward(feat_tok, m1, m2, B, hw, x1, x2, hid, code, w1p, f32(b1), wab, f32(ba), wbp, f32(bb))
+        ctx.save_for_backward(x1, x2 if nonlinear else None, hid, wbp)
+        ctx.shapes = [p.shape if p is not None else None for p in (w1, b1, wa, ba, wb, bb)]
         return code
 
     @staticmethod
     def backward(ctx, dcode):
-        x1, x2, hid, wab, wbp = ctx.saved_tensors
-        M, E, D, P, nonlinear = ctx.dims
-        dev = dcode.device
-        lib = _lib.load()
+        x1, x2, hid, wbp = ctx.saved_tensors
+        s1, sb1, sa, sba, sb, sbb = ctx.shapes
+        f32 = dict(dtype=torch.float32, device=dcode.device)
         dcode = dcode.contiguous() if dcode.stride(1) != 1 else dcode
-        dyb = torch.empty(M, 128, dtype=torch.bfloat16, device=dev)
-        _lib.check(lib.stego_cast_pad_bf16(_lib.ptr(dcode), dcode.stride(0), D, _lib.ptr(dyb), 128, M, _lib.stream()),
-                   "stego_cast_pad_bf16")
-        sms = torch.cuda.get_device_properties(dev).multi_processor_count
-
-        def splits_for(out_rows, out_cols):
-            tiles = ((out_rows + 127) // 128) * ((out_cols + 127) // 128)
-            return max(1, min(M // 512, sms // tiles))  # tiles x splits = one wave of the persistent GEMM grid
-        # bias gradient: column sums over the padded row (padding columns of d(code) are zero) -> vector loads
-        db_pad = torch.zeros(P, dtype=torch.float32, device=dev)
-        _lib.check(lib.stego_colsum(_lib.ptr(dcode), 0, dcode.stride(0), P if dcode.shape[1] >= P else D, M,
-                                    _lib.ptr(db_pad), _lib.stream()), "stego_colsum")
-        db = db_pad[:D].contiguous()
-        dw1 = torch.zeros(D, E, dtype=torch.float32, device=dev)
-        ops.gemm(dyb, x1, dw1, M=D, N=E, K=M, a_mn=True, b_mn=True, splits=splits_for(D, E), atomic=True)
-        dwa = dba = dwb = dbb = None
-        if nonlinear:
-            dwb = torch.zeros(D, E, dtype=torch.float32, device=dev)
-            ops.gemm(dyb, hid, dwb, M=D, N=E, K=M, a_mn=True, b_mn=True, splits=splits_for(D, E), atomic=True)
-            dbb = db.clone()
-            # dH = dY . Wb  (B operand [K=c][N=E] is MN-major), then ReLU backward -> bf16 operand
-            dh = torch.empty(M, E, dtype=torch.float32, device=dev)
-            ops.gemm(dyb, wbp, dh, M=M, N=E, K=128, b_mn=True)
-            dhb = torch.empty(M, E, dtype=torch.bfloat16, device=dev)
-            _lib.check(lib.stego_relu_bwd_bf16(_lib.ptr(dh), _lib.ptr(hid), _lib.ptr(dhb), M * E, _lib.stream()),
-                       "stego_relu_bwd_bf16")
-            dba = torch.zeros(E, dtype=torch.float32, device=dev)
-            _lib.check(lib.stego_colsum(_lib.ptr(dhb), 1, E, E, M, _lib.ptr(dba), _lib.stream()), "stego_colsum")
-            dwa = torch.zeros(E, E, dtype=torch.float32, device=dev)
-            ops.gemm(dhb, x2, dwa, M=E, N=E, K=M, a_mn=True, b_mn=True, splits=splits_for(E, E), atomic=True)
-        s1, sa, sb_ = ctx.shapes
-        return (None, None, None, None, None, dw1.reshape(s1), db,
-                dwa.reshape(sa) if nonlinear else None, dba, dwb.reshape(sb_) if nonlinear else None, dbb)
+        dyb = torch.empty(x1.shape[0], 128, dtype=torch.bfloat16, device=dcode.device)
+        db_pad = torch.zeros(_round_up(s1[0], 8), **f32)
+        dw1, db1 = torch.zeros(s1, **f32), torch.empty(sb1, **f32)
+        dwa = dba = dwb = dbb = dh = dhb = None
+        if hid is not None:
+            dwa, dba, dwb, dbb = torch.zeros(sa, **f32), torch.zeros(sba, **f32), torch.zeros(sb, **f32), torch.empty(sbb, **f32)
+            dh, dhb = torch.empty(x1.shape, **f32), torch.empty_like(x1)
+        head_backward(dcode, x1, x2, hid, wbp, dyb, db_pad, dh, dhb, dw1, db1, dwa, dba, dwb, dbb)
+        return (None,) * 5 + (dw1, db1, dwa, dba, dwb, dbb)
 
 
 def _draw_dropout2d_noise(batch: int, channels: int, p: float, device) -> torch.Tensor:
@@ -290,17 +302,19 @@ class DinoFeaturizer(nn.Module):
             m3 = _draw_dropout2d_noise(batch, E, 0.1, device).view(batch, E)
         return m1, m2, m3
 
+    def head_params(self):
+        """(w1, b1, wa, ba, wb, bb): cluster1 and the two convs of cluster2, whose entries are None for the linear head."""
+        c1 = self.cluster1[0]
+        if self.proj_type != "nonlinear":
+            return c1.weight, c1.bias, None, None, None, None
+        ca, cb = self.cluster2[0], self.cluster2[2]
+        return c1.weight, c1.bias, ca.weight, ca.bias, cb.weight, cb.bias
+
     def head_code(self, feat_tok: torch.Tensor, m1, m2, fh: int, fw: int) -> torch.Tensor:
         """cluster1 (+ cluster2) on tokens-major features -> code [B, dim, h, w] (view of padded storage)."""
         B, hw, E = feat_tok.shape
-        c1 = self.cluster1[0]
-        if self.proj_type == "nonlinear":
-            ca, cb = self.cluster2[0], self.cluster2[2]
-            store = _HeadFn.apply(feat_tok.reshape(B * hw, E), m1, m2, B, hw, c1.weight, c1.bias, ca.weight, ca.bias,
-                                  cb.weight, cb.bias)
-        else:
-            store = _HeadFn.apply(feat_tok.reshape(B * hw, E), m1, None, B, hw, c1.weight, c1.bias, None, None, None,
-                                  None)
+        m2 = m2 if self.proj_type == "nonlinear" else None
+        store = _HeadFn.apply(feat_tok.reshape(B * hw, E), m1, m2, B, hw, *self.head_params())
         return store.view(B, fh, fw, -1)[..., :self.dim].permute(0, 3, 1, 2)
 
     # ---- reference entry point -------------------------------------------------------------------
@@ -392,6 +406,25 @@ class ContrastiveCorrelationLoss(nn.Module):
 # ==================================================================================================
 # ClusterLookup (modules.py:134-161)
 # ==================================================================================================
+def cluster_lookup_forward(x, clusters, alpha, loss, scratch, probs=None, log_probs=None) -> None:
+    """ClusterLookup.forward (modules.py:146-161) of x, an fp32 [B, C, H, W] view whose pixel y*W + x is ONE stride,
+    into loss[0] (and the optional probs / log_probs [B, n, H, W]); alpha None is the one-hot argmax."""
+    B, C, H, W = x.shape
+    _lib.check(_lib.load().stego_cluster_lookup_fwd(
+        _lib.ptr(x), x.stride(0), x.stride(1), x.stride(3), _lib.ptr(clusters), B, C, clusters.shape[0], H * W,
+        int(alpha is not None), float(alpha) if alpha is not None else 0.0, 0, _lib.ptr(probs), _lib.ptr(log_probs),
+        _lib.ptr(loss), _lib.ptr(scratch), _lib.stream()), "stego_cluster_lookup_fwd")
+
+
+def cluster_lookup_backward(x, clusters, alpha, grad_loss, dnc, dclusters) -> None:
+    """dclusters += grad_loss[0] * d(loss)/d(clusters); dclusters and the scratch dnc must arrive zeroed."""
+    B, C, H, W = x.shape
+    _lib.check(_lib.load().stego_cluster_lookup_bwd(
+        _lib.ptr(x), x.stride(0), x.stride(1), x.stride(3), _lib.ptr(clusters), B, C, clusters.shape[0], H * W,
+        int(alpha is not None), float(alpha) if alpha is not None else 0.0, _lib.ptr(grad_loss), _lib.ptr(dnc),
+        _lib.ptr(dclusters), _lib.stream()), "stego_cluster_lookup_bwd")
+
+
 class _ClusterLookupFn(torch.autograd.Function):
 
     @staticmethod
@@ -407,14 +440,9 @@ class _ClusterLookupFn(torch.autograd.Function):
             xf = xf.contiguous()
         cl = clusters.detach().float().contiguous()
         loss = torch.empty(2, dtype=torch.float32, device=dev)
-        scratch = ops.probe_scratch(dev)
         probs = torch.empty(B, n, H, W, dtype=torch.float32, device=dev) if want_probs else None
         logp = torch.empty(B, n, H, W, dtype=torch.float32, device=dev) if want_logp else None
-        rc = _lib.load().stego_cluster_lookup_fwd(
-            _lib.ptr(xf), xf.stride(0), xf.stride(1), xf.stride(3), _lib.ptr(cl), B, C, n, H * W,
-            int(alpha is not None), float(alpha) if alpha is not None else 0.0, 0, _lib.ptr(probs), _lib.ptr(logp),
-            _lib.ptr(loss), _lib.ptr(scratch), _lib.stream())
-        _lib.check(rc, "stego_cluster_lookup_fwd")
+        cluster_lookup_forward(xf, cl, alpha, loss, ops.probe_scratch(dev), probs, logp)
         ctx.save_for_backward(xf, cl)
         ctx.alpha = alpha
         ctx.shape = clusters.shape
@@ -427,17 +455,10 @@ class _ClusterLookupFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g_loss, _gp, _gl):
         xf, cl = ctx.saved_tensors
-        B, C, H, W = xf.shape
-        n = cl.shape[0]
-        dnc = torch.zeros(n, C, dtype=torch.float32, device=xf.device)
-        dcl = torch.zeros(n, C, dtype=torch.float32, device=xf.device)
-        alpha = ctx.alpha
+        dnc = torch.zeros(cl.shape, dtype=torch.float32, device=xf.device)
+        dcl = torch.zeros(cl.shape, dtype=torch.float32, device=xf.device)
         g = (g_loss if g_loss is not None else torch.zeros((), device=xf.device)).to(torch.float32).reshape(1).contiguous()
-        rc = _lib.load().stego_cluster_lookup_bwd(
-            _lib.ptr(xf), xf.stride(0), xf.stride(1), xf.stride(3), _lib.ptr(cl), B, C, n, H * W,
-            int(alpha is not None), float(alpha) if alpha is not None else 0.0, _lib.ptr(g), _lib.ptr(dnc), _lib.ptr(dcl),
-            _lib.stream())
-        _lib.check(rc, "stego_cluster_lookup_bwd")
+        cluster_lookup_backward(xf, cl, ctx.alpha, g, dnc, dcl)
         return None, dcl.reshape(ctx.shape), None, None, None
 
 

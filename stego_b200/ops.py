@@ -1,9 +1,10 @@
-"""Thin Python wrappers over the C-ABI (one function per extern "C" entry point).
+"""Thin Python wrappers over the C-ABI entry points of the GEMMs, the attention and the ViT glue.
 
 These take torch CUDA tensors, pass raw device pointers + sizes + the current stream through
 ctypes and return torch tensors.  They allocate outputs with torch (PyTorch owns all memory) and
-never fall back to torch math.  The probe entry points also share their input formats from here: the label
-dtypes, the tokens-major code view and the partials scratch.
+never fall back to torch math.  The training step's other entry points are called from the stage functions in
+modules.py, corr.py and segmenter.py, which share from here the probes' input formats (label dtypes, tokens-major
+code view, partials scratch) and the split-K rule of the head's weight-gradient GEMMs.
 """
 from __future__ import annotations
 
@@ -37,6 +38,13 @@ def gemm(a: torch.Tensor, b: torch.Tensor, out: torch.Tensor, *, M: int, N: int,
         _lib.stream())
     _lib.check(rc, "stego_gemm_bf16")
     return out
+
+
+def wgrad_splits(K: int, out_rows: int, out_cols: int, num_sms: int) -> int:
+    """Split-K count of a weight-gradient GEMM (K = activation rows): tiles x splits fills ONE wave of the persistent
+    GEMM grid (one CTA per SM; more splits would make a second round of the grid), each split at least 512 rows deep."""
+    tiles = ((out_rows + 127) // 128) * ((out_cols + 127) // 128)
+    return max(1, min(K // 512, num_sms // tiles))
 
 
 def gemm_batched(a: torch.Tensor, b: torch.Tensor, out: torch.Tensor, *, a_mn: bool = False, b_mn: bool = False,

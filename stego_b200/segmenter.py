@@ -178,6 +178,18 @@ def allreduce_gradients(flat: FlatParams) -> None:
 # --------------------------------------------------------------------------------------------------
 # linear probe: 1x1 conv -> bilinear upsample -> masked CE, forward + backward in one fused call
 # --------------------------------------------------------------------------------------------------
+def linear_probe_ce_step(x, weight, bias, label, logits, dlogits, partials, loss, dW, db, grad_scale: float) -> None:
+    """Linear probe forward + backward (train_segmentation.py:213-218) of x, a tokens-major [B, C, h, w] view
+    (ops.tokens_major), against label [B, H, W] (an ops.LABEL_BYTES dtype): loss [2] = (mean CE, valid pixels), dW / db
+    += grad_scale * gradient.  dlogits, dW and db are accumulated into and must arrive zeroed."""
+    B, C, h, w = x.shape
+    H, W = label.shape[-2], label.shape[-1]
+    _lib.check(_lib.load().stego_linear_probe_ce(
+        _lib.ptr(x), x.stride(3), C, _lib.ptr(weight), _lib.ptr(bias), weight.shape[0], _lib.ptr(label),
+        ops.LABEL_BYTES[label.dtype], B, h, w, H, W, _lib.ptr(logits), _lib.ptr(dlogits), _lib.ptr(partials),
+        _lib.ptr(loss), grad_scale, _lib.ptr(dW), _lib.ptr(db), _lib.stream()), "stego_linear_probe_ce")
+
+
 class _LinearProbeCEFn(torch.autograd.Function):
 
     @staticmethod
@@ -188,24 +200,17 @@ class _LinearProbeCEFn(torch.autograd.Function):
         dev = code_nchw.device
         if n > 32 or C > 96:
             raise RuntimeError(f"stego_b200 linear probe: n_classes={n} (<=32) / dim={C} (<=96) unsupported")
-        x = ops.tokens_major(code_nchw)
-        ld = x.stride(3)
         rows = B * h * w
-        H, W = label.shape[-2], label.shape[-1]
-        lab, label_bytes = ops.probe_label(label, B, H, W)
+        lab, _ = ops.probe_label(label, B, label.shape[-2], label.shape[-1])
         logits = torch.empty(rows, 32, dtype=torch.float32, device=dev)
         dlogits = torch.zeros(rows, 32, dtype=torch.float32, device=dev)
-        partials = ops.probe_scratch(dev)
         loss = torch.empty(2, dtype=torch.float32, device=dev)
         dW = torch.zeros(n, C, dtype=torch.float32, device=dev)
         db = torch.zeros(n, dtype=torch.float32, device=dev)
         wf = weight.detach().float().reshape(n, C).contiguous()
         bf = bias.detach().float().contiguous()
-        rc = _lib.load().stego_linear_probe_ce(_lib.ptr(x), ld, C, _lib.ptr(wf), _lib.ptr(bf), n, _lib.ptr(lab), label_bytes, B,
-                                               h, w,
-                                               H, W, _lib.ptr(logits), _lib.ptr(dlogits), _lib.ptr(partials),
-                                               _lib.ptr(loss), 1.0, _lib.ptr(dW), _lib.ptr(db), _lib.stream())
-        _lib.check(rc, "stego_linear_probe_ce")
+        linear_probe_ce_step(ops.tokens_major(code_nchw), wf, bf, lab, logits, dlogits, ops.probe_scratch(dev), loss,
+                             dW, db, 1.0)
         ctx.save_for_backward(dW, db)
         ctx.wshape = weight.shape
         return loss[0]
