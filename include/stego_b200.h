@@ -114,6 +114,16 @@ STEGO_API int stego_sample_norm_fwd(const void* src, const void* src_pos, int sr
                                     const float* coords2, const long long* perms, void* tiles, int B, int C,
                                     int Cpad, int H, int W, int feature_samples, int nslots, int perms_are_raw_randperm,
                                     void* stream);
+/* The same tiles for the ground-truth teacher signal of cfg.use_true_labels (train_segmentation.py:135-137):
+ * one_hot_feats(label + 1, n_classes + 1) (utils.py:65-66) sampled and normalised without materialising it.  label /
+ * label_pos: contiguous [B][H][W] of label_bytes = 8 (int64), 4 (int32) or 1 (uint8) per element.  Class 0 is
+ * "unlabelled": a label outside 0 .. n_classes - 1 (-1, uint8 255 or any other value) maps to it, where F.one_hot
+ * would raise.  n_classes + 1 <= Cpad <= 256, Cpad a multiple of 64, H and W >= 2; coords, perms, slots and rows as
+ * above.  On the same coordinates the tiles are bit-identical to stego_sample_norm_fwd's on the fp32 one-hot map. */
+STEGO_API int stego_sample_labels_fwd(const void* label, const void* label_pos, int label_bytes, const float* coords1,
+                                      const float* coords2, const long long* perms, void* tiles, int B, int n_classes,
+                                      int Cpad, int H, int W, int feature_samples, int nslots,
+                                      int perms_are_raw_randperm, void* stream);
 /* helper (:325-347) for all calls at once, feature_samples <= 11 (R = 128): fd and cd einsums on wgmma (bf16 hi/lo
  * split, fp32 accumulate), pointwise centring, clamp, shift, product and reduction.  slot_of_call / shifts are HOST arrays.
  * partials: scratch [ncalls][B][8]; stats: out [ncalls][4] = {mean loss, mean cd, old_mean, mean of centred fd}.

@@ -11,12 +11,25 @@ from typing import List, Optional, Sequence, Tuple
 
 import torch
 
-from . import _lib
+from . import _lib, ops
 
 CODE_PAD = 128   # code channels are zero-padded to two 64-wide k-blocks in the operand tiles
 TILE_ROWS = 128  # feature_samples^2 <= 128
 DT_LD = 72       # row stride of the gradient tiles
 MAX_TILED_FS = 64  # the multi-tile kernels take feature_samples up to 64 (S = 4096 points per image)
+TEACHER_WIDTHS = (64, 128, 192, 256, 384, 768)  # operand-tile widths of the teacher signal the sampler takes
+
+
+def teacher_width(C: int) -> int:
+    """Operand-tile width of a C-channel teacher signal (features, or the one-hot label map of use_true_labels): C
+    itself when it is a multiple of 64, else C zero-padded to the narrowest of TEACHER_WIDTHS (all multiples of 64).
+    Padding channels are zero and change no normalised value and no correlation."""
+    if C % 64 == 0:
+        return C
+    for w in TEACHER_WIDTHS:
+        if C <= w:
+            return w
+    raise RuntimeError(f"stego_b200: teacher signal of {C} channels unsupported (1..{TEACHER_WIDTHS[-1]})")
 
 
 def _i32(vals: Sequence[int]):
@@ -149,6 +162,34 @@ def build_tiles(src: torch.Tensor, src_pos: torch.Tensor, coords1: torch.Tensor,
     return out
 
 
+def build_label_tiles(label: torch.Tensor, label_pos: torch.Tensor, coords1: torch.Tensor, coords2: torch.Tensor,
+                      perms: Optional[torch.Tensor], spec: LossSpec, n_classes: int, *, raw_perms: bool = False,
+                      out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """The teacher operand of cfg.use_true_labels (train_segmentation.py:135-137): the tiles build_tiles makes of the
+    fp32 map one_hot_feats(label + 1, n_classes + 1) (utils.py:65-66), bit for bit, read from the label maps directly —
+    the one-hot maps and their gathered copies are never materialised.  Tiles [2][nslots][B][spec.rows][Cpad] with
+    Cpad = teacher_width(n_classes + 1) <= 256, written into `out` when it is given.
+
+    label / label_pos: [B, H, W] (or [B, 1, H, W]) int64, int32 or uint8, at any resolution (the sampling coordinates
+    are normalised).  A label outside 0 .. n_classes - 1 — the reference's -1, uint8 255, or any other value — is class
+    0, "unlabelled"; the reference's F.one_hot raises on values >= n_classes or < -1 instead."""
+    B = label.shape[0]
+    H, W = label.shape[-2], label.shape[-1]
+    if label_pos.shape[0] != B or tuple(label_pos.shape[-2:]) != (H, W):
+        raise RuntimeError(f"stego_b200: label_pos {tuple(label_pos.shape)} does not match label {tuple(label.shape)}")
+    if not 1 <= n_classes <= 255:
+        raise RuntimeError(f"stego_b200: use_true_labels takes n_classes 1..255, got {n_classes}")
+    lab, nbytes = ops.probe_label(label, B, H, W)
+    lab_pos, _ = ops.probe_label(label_pos.to(lab.dtype), B, H, W)
+    c_pad = teacher_width(n_classes + 1)
+    if out is None:
+        out = torch.empty(2, spec.nslots, B, spec.rows, c_pad, dtype=torch.bfloat16, device=label.device)
+    _lib.check(_lib.load().stego_sample_labels_fwd(
+        _lib.ptr(lab), _lib.ptr(lab_pos), nbytes, _lib.ptr(coords1), _lib.ptr(coords2), _lib.ptr(perms), _lib.ptr(out),
+        B, int(n_classes), c_pad, H, W, spec.fs, spec.nslots, int(raw_perms), _lib.stream()), "stego_sample_labels_fwd")
+    return out
+
+
 def sample_norm_backward(code, code_pos, coords1, coords2, perms, spec, dtiles, dcode, dcode_pos, raw_perms=False):
     """dcode / dcode_pos += dtiles taken back through build_tiles of fp32 code / code_pos [B, D, H, W] (all four in
     code's strides): they must arrive zeroed."""
@@ -159,23 +200,44 @@ def sample_norm_backward(code, code_pos, coords1, coords2, perms, spec, dtiles, 
         _lib.stream()), "stego_sample_norm_bwd")
 
 
-def _prep_common(feats, feats_pos, code, code_pos, coords1, coords2, perms, spec: LossSpec):
-    _lib.require_cuda(feats, feats_pos, code, code_pos, coords1, coords2)
-    B, E, H, W = feats.shape
-    D = code.shape[1]
-    if feats.dtype not in (torch.float32, torch.bfloat16):
-        raise RuntimeError("stego_b200: feats must be fp32 or bf16")
-    if E % 64 != 0 or E > 768:
-        raise RuntimeError(f"stego_b200: feature channels {E} unsupported (multiple of 64, <= 768)")
+def _prep_common(feats, feats_pos, code, code_pos, coords1, coords2, perms, spec: LossSpec, ftiles=None,
+                 any_teacher=False):
+    """Checks the inputs; returns B, the teacher tile width E, D, code's H, W, and the coords / perms as the kernels
+    read them.  The teacher signal feats / feats_pos is sampled at width E: its channel count, a multiple of 64 up to
+    768, on code's spatial grid — or, with any_teacher, what the reference's module takes: any channel count up to 768
+    (E = teacher_width(C)) at any spatial size (the sampling coordinates are normalised).  ftiles, when given, are the
+    prebuilt teacher tiles (build_label_tiles) and feats / feats_pos are not read."""
+    _lib.require_cuda(code, code_pos, coords1, coords2)
+    B, D, H, W = code.shape
+    if ftiles is not None:
+        E = ftiles.shape[-1]
+        if (ftiles.dtype != torch.bfloat16 or E % 64 != 0 or E > 768
+                or tuple(ftiles.shape[:4]) != (2, spec.nslots, B, spec.rows)):
+            raise RuntimeError(f"stego_b200: teacher tiles {tuple(ftiles.shape)} {ftiles.dtype} do not match "
+                               f"(2, {spec.nslots}, {B}, {spec.rows}, E % 64 == 0) bf16")
+    else:
+        _lib.require_cuda(feats, feats_pos)
+        if feats.dtype not in (torch.float32, torch.bfloat16):
+            raise RuntimeError("stego_b200: feats must be fp32 or bf16")
+        E = feats.shape[1]
+        if any_teacher:
+            if not 1 <= E <= 768:
+                raise RuntimeError(f"stego_b200: teacher channels {E} unsupported (1..768)")
+            E = teacher_width(E)
+            if feats.shape[0] != B or feats_pos.shape != feats.shape:
+                raise RuntimeError("stego_b200: feats/code shape mismatch")
+        else:
+            if E % 64 != 0 or E > 768:
+                raise RuntimeError(f"stego_b200: feature channels {E} unsupported (multiple of 64, <= 768)")
+            if code.shape[2:] != feats.shape[2:] or feats.shape[0] != B:
+                raise RuntimeError("stego_b200: feats/code shape mismatch")
     if D > 96:
         raise RuntimeError(f"stego_b200: code dim {D} unsupported (<= 96)")
-    if code.shape[2:] != feats.shape[2:] or code.shape[0] != B:
-        raise RuntimeError("stego_b200: feats/code shape mismatch")
     coords1 = coords1.to(torch.float32).contiguous()
     coords2 = coords2.to(torch.float32).contiguous()
     if spec.n_neg > 0:
-        perms_t = torch.stack([p.to(device=feats.device, dtype=torch.long) for p in perms]).contiguous() \
-            if not torch.is_tensor(perms) else perms.to(device=feats.device, dtype=torch.long).contiguous()
+        perms_t = torch.stack([p.to(device=code.device, dtype=torch.long) for p in perms]).contiguous() \
+            if not torch.is_tensor(perms) else perms.to(device=code.device, dtype=torch.long).contiguous()
         assert perms_t.shape == (spec.n_neg, B)
     else:
         perms_t = None
@@ -187,7 +249,7 @@ class _CorrLossFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, code, code_pos, feats, feats_pos, coords1, coords2, perms, spec: LossSpec, want_elems: bool,
-                chan_scale, chan_scale_pos, raw_perms=False, pair=False):
+                chan_scale, chan_scale_pos, raw_perms=False, pair=False, ftiles=None, any_teacher=False):
         # pair=True: `code` is the [2B, D, h, w] output of ONE head pass over img ++ img_pos (code_pos is None); its
         # gradient is then produced in one buffer instead of two tensors that autograd has to re-assemble.
         if pair:
@@ -197,18 +259,19 @@ class _CorrLossFn(torch.autograd.Function):
                 code_all = code_all.float()
             code_f, code_pos_f = code_all[:half], code_all[half:]
             B, E, D, H, W, coords1, coords2, perms_t = _prep_common(feats, feats_pos, code_f, code_pos_f, coords1,
-                                                                     coords2, perms, spec)
+                                                                     coords2, perms, spec, ftiles, any_teacher)
         else:
             B, E, D, H, W, coords1, coords2, perms_t = _prep_common(feats, feats_pos, code, code_pos, coords1, coords2,
-                                                                     perms, spec)
+                                                                     perms, spec, ftiles, any_teacher)
             code_f = code.detach()
             if code_f.dtype != torch.float32:
                 code_f = code_f.float()
             code_pos_f = _same_layout(code_f, code_pos.detach().to(torch.float32))
         ctx.pair = bool(pair)
         dev = code.device
-        ftiles = build_tiles(feats.detach(), feats_pos.detach(), coords1, coords2, perms_t, spec, E, chan_scale,
-                             chan_scale_pos, raw_perms)
+        if ftiles is None:
+            ftiles = build_tiles(feats.detach(), feats_pos.detach(), coords1, coords2, perms_t, spec, E, chan_scale,
+                                 chan_scale_pos, raw_perms)
         ctiles = build_tiles(code_f, code_pos_f, coords1, coords2, perms_t, spec, CODE_PAD, raw_perms=raw_perms)
         ctx.raw_perms = bool(raw_perms)
         S = spec.fs * spec.fs
@@ -256,17 +319,22 @@ class _CorrLossFn(torch.autograd.Function):
                              ctx.raw_perms)
         d0, d1 = ctx.code_dtype
         if ctx.pair:
-            return (dall.to(d0), None) + (None,) * 11
-        return (dcode.to(d0), dcode_pos.to(d1)) + (None,) * 11
+            return (dall.to(d0), None) + (None,) * 13
+        return (dcode.to(d0), dcode_pos.to(d1)) + (None,) * 13
 
 
 def corr_loss(feats, feats_pos, code, code_pos, coords1, coords2, perms, spec: LossSpec, want_elems: bool = False,
-              chan_scale=None, chan_scale_pos=None, raw_perms: bool = False, pair: bool = False):
+              chan_scale=None, chan_scale_pos=None, raw_perms: bool = False, pair: bool = False, *,
+              ftiles: Optional[torch.Tensor] = None, any_teacher: bool = False):
     """raw_perms=True: `perms` holds the raw torch.randperm draws and the sampling kernel applies super_perm's
     fix-up itself (saves the eq/add/remainder launches of modules.super_perm).
     pair=True: `code` holds code ++ code_pos ([2B, D, h, w], one head pass) and `code_pos` is None.
+    ftiles: the teacher operand already sampled (build_label_tiles for use_true_labels, drawn on the same coords1 /
+    coords2 / perms); feats / feats_pos are then not read and may be None.
+    any_teacher=True: feats / feats_pos may have any channel count up to 768 and any spatial size, as the reference's
+    ContrastiveCorrelationLoss accepts (see _prep_common); without it they are code-sized with channels % 64 == 0.
     spec: a LossSpec (single-tile kernels) or a TiledLossSpec (multi-tile kernels); make_spec picks by feature_samples.
     Returns (losses[ncalls], cd_means[ncalls], cd[ncalls,B,S,S]|None, loss_elems|None).
     losses[k] is the mean of helper call k (0 intra, 1 inter, 2.. negatives); differentiable wrt code/code_pos."""
     return _CorrLossFn.apply(code, code_pos, feats, feats_pos, coords1, coords2, perms, spec, want_elems,
-                             chan_scale, chan_scale_pos, raw_perms, pair)
+                             chan_scale, chan_scale_pos, raw_perms, pair, ftiles, any_teacher)

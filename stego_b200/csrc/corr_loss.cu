@@ -23,6 +23,7 @@
 //                       into d_code, fixed order, no atomics).
 #include "common.cuh"
 #include "host_util.h"
+#include "probe_common.cuh"
 
 namespace stego {
 
@@ -39,6 +40,7 @@ struct SampleParams {
   const void* src;      // slot 0 and slots >= 2 (through perm)
   const void* src_pos;  // slot 1
   int src_bf16;         // element type of both sources
+  int label_bytes;      // label source (sample_labels_kernel): width of one label, 8 / 4 / 1
   long long sb, sc, sy, sx;  // element strides (batch, channel, y, x) — shared by src and src_pos
   const float* chan_scale;      // optional [B][C] per-(image,channel) multiplier (Dropout2d noise), slot 0/2+
   const float* chan_scale_pos;  // same for src_pos
@@ -97,9 +99,14 @@ __device__ __forceinline__ void slot_source(const SampleParams& p, int slot, int
 
 // One warp per tile row: row s of (slot, image b) in block (s / 8, slot * B + b).  Generic strides / dtypes; each
 // lane owns channels lane, lane+32, ...
-template <int NV>  // NV = Cpad / 32
-__global__ void __launch_bounds__(256)
-sample_norm_kernel(SampleParams p) {
+// kLabels: the source is a label map [B][H][W] (strides sb, sy, sx; sc unused) read as the C = n_classes + 1 channel
+// map one_hot_feats(label + 1, C) of train_segmentation.py:135-137 (utils.py:65-66) without materialising it: channel c
+// of a tap is 1 when the tap's class is c, else 0.  A label outside 0 .. n_classes - 1 (-1, uint8 255, any other value)
+// is class 0, where F.one_hot would raise on values >= n_classes or < -1.  The products and sums below are then the
+// ones the feature path computes on the materialised fp32 one-hot map (times 0 or 1 and adding 0 are exact): the tiles
+// are bit-identical.  One body, two kernels: sample_norm_kernel (features) and sample_labels_kernel (labels).
+template <int NV, bool kLabels>  // NV = Cpad / 32
+__device__ __forceinline__ void sample_norm_row(const SampleParams& p) {
   const int R = p.R;
   const int s = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);  // grid (R / 8, nslots * B)
   const int lane = threadIdx.x & 31;
@@ -121,6 +128,14 @@ sample_norm_kernel(SampleParams p) {
   auto off = [&](int pix) { return static_cast<long long>(pix / p.W) * p.sy + static_cast<long long>(pix % p.W) * p.sx; };
   const long long o00 = off(t.i00), o01 = off(t.i01), o10 = off(t.i10), o11 = off(t.i11);
   const long long base = static_cast<long long>(img) * p.sb;
+  int k00 = 0, k01 = 0, k10 = 0, k11 = 0;  // classes of the four taps (label source)
+  if constexpr (kLabels) {
+    auto cls = [&](long long o) {
+      const long long l = read_label(src, p.label_bytes, base + o);
+      return (l >= 0 && l < p.C - 1) ? static_cast<int>(l) + 1 : 0;
+    };
+    k00 = cls(o00); k01 = cls(o01); k10 = cls(o10); k11 = cls(o11);
+  }
   float ss = 0.f;
 #pragma unroll
   for (int k = 0; k < NV; ++k) {
@@ -129,7 +144,10 @@ sample_norm_kernel(SampleParams p) {
     if (c < p.C) {
       const long long cb = base + static_cast<long long>(c) * p.sc;
       float a00, a01, a10, a11;
-      if (p.src_bf16) {
+      if constexpr (kLabels) {
+        a00 = k00 == c ? 1.f : 0.f; a01 = k01 == c ? 1.f : 0.f;
+        a10 = k10 == c ? 1.f : 0.f; a11 = k11 == c ? 1.f : 0.f;
+      } else if (p.src_bf16) {
         const bf16* q = reinterpret_cast<const bf16*>(src) + cb;
         a00 = __bfloat162float(q[o00]); a01 = __bfloat162float(q[o01]);
         a10 = __bfloat162float(q[o10]); a11 = __bfloat162float(q[o11]);
@@ -157,6 +175,12 @@ sample_norm_kernel(SampleParams p) {
     lo[lane + 32 * k] = __float2bfloat16_rn(n - __bfloat162float(h));
   }
 }
+
+template <int NV>
+__global__ void __launch_bounds__(256) sample_norm_kernel(SampleParams p) { sample_norm_row<NV, false>(p); }
+
+template <int NV>
+__global__ void __launch_bounds__(256) sample_labels_kernel(SampleParams p) { sample_norm_row<NV, true>(p); }
 
 // Vectorised variant for the layout the training step uses: bf16 source, channel stride 1 (tokens-major),
 // C % 8 == 0, Cpad == C.  Each lane owns 8 consecutive channels per step: four 16-byte tap loads, two 16-byte tile
@@ -903,7 +927,7 @@ static int fill_sample_params(SampleParams& sp, const void* src, const void* src
   STEGO_CHECK_ARG(fs >= 1 && fs <= CT_MAX_FS, "sample_norm: feature_samples=%d outside 1..%d", fs, CT_MAX_FS);
   STEGO_CHECK_ARG(C > 0 && C <= Cpad && Cpad % 64 == 0 && Cpad <= 768, "sample_norm: C=%d Cpad=%d", C, Cpad);
   STEGO_CHECK_ARG(B > 0 && H > 1 && W > 1, "sample_norm: B=%d H=%d W=%d", B, H, W);
-  sp.src = src; sp.src_pos = src_pos; sp.src_bf16 = src_bf16;
+  sp.src = src; sp.src_pos = src_pos; sp.src_bf16 = src_bf16; sp.label_bytes = 0;
   sp.sb = sb; sp.sc = sc; sp.sy = sy; sp.sx = sx;
   sp.chan_scale = chan_scale; sp.chan_scale_pos = chan_scale_pos;
   sp.coords1 = coords1; sp.coords2 = coords2; sp.perms = perms; sp.perms_raw = 0;
@@ -911,6 +935,33 @@ static int fill_sample_params(SampleParams& sp, const void* src, const void* src
   sp.B = B; sp.C = C; sp.Cpad = Cpad; sp.H = H; sp.W = W; sp.fs = fs; sp.S = fs * fs; sp.nslots = nslots;
   sp.R = (sp.S + CL_ROWS - 1) / CL_ROWS * CL_ROWS;
   sp.eps = 1e-10f;
+  return STEGO_OK;
+}
+
+// The generic sampler for sp.Cpad: 64 .. 256 channels for both sources, 384 and 768 for features only.
+template <int NV, bool kLabels>
+static void launch_sampler(const SampleParams& sp, dim3 blocks, cudaStream_t stream) {
+  if constexpr (kLabels) sample_labels_kernel<NV><<<blocks, 256, 0, stream>>>(sp);
+  else sample_norm_kernel<NV><<<blocks, 256, 0, stream>>>(sp);
+}
+
+template <bool kLabels>
+static int launch_sample_norm(const SampleParams& sp, cudaStream_t stream, const char* who) {
+  const dim3 blocks(sp.R / 8, sp.nslots * sp.B);  // 8 warps per block, one per tile row
+  switch (sp.Cpad / 32) {
+    case 2: launch_sampler<2, kLabels>(sp, blocks, stream); break;
+    case 4: launch_sampler<4, kLabels>(sp, blocks, stream); break;
+    case 6: launch_sampler<6, kLabels>(sp, blocks, stream); break;
+    case 8: launch_sampler<8, kLabels>(sp, blocks, stream); break;
+    default:
+      if constexpr (!kLabels) {
+        if (sp.Cpad == 384) { launch_sampler<12, false>(sp, blocks, stream); break; }
+        if (sp.Cpad == 768) { launch_sampler<24, false>(sp, blocks, stream); break; }
+      }
+      set_error("%s: Cpad=%d unsupported (%s)", who, sp.Cpad, kLabels ? "64,128,192,256" : "64,128,192,256,384,768");
+      return STEGO_ERR_UNSUPPORTED;
+  }
+  STEGO_CHECK_LAUNCH(kLabels ? "sample_labels_kernel" : "sample_norm_kernel");
   return STEGO_OK;
 }
 
@@ -944,19 +995,28 @@ extern "C" int stego_sample_norm_fwd(const void* src, const void* src_pos, int s
     STEGO_CHECK_LAUNCH("sample_norm_vec8_kernel");
     return STEGO_OK;
   }
-  switch (Cpad / 32) {
-    case 2: sample_norm_kernel<2><<<blocks, 256, 0, stream>>>(sp); break;
-    case 4: sample_norm_kernel<4><<<blocks, 256, 0, stream>>>(sp); break;
-    case 6: sample_norm_kernel<6><<<blocks, 256, 0, stream>>>(sp); break;
-    case 8: sample_norm_kernel<8><<<blocks, 256, 0, stream>>>(sp); break;
-    case 12: sample_norm_kernel<12><<<blocks, 256, 0, stream>>>(sp); break;
-    case 24: sample_norm_kernel<24><<<blocks, 256, 0, stream>>>(sp); break;
-    default:
-      set_error("stego_sample_norm_fwd: Cpad=%d unsupported (64,128,192,256,384,768)", Cpad);
-      return STEGO_ERR_UNSUPPORTED;
-  }
-  STEGO_CHECK_LAUNCH("sample_norm_kernel");
-  return STEGO_OK;
+  return launch_sample_norm<false>(sp, stream, "stego_sample_norm_fwd");
+}
+
+extern "C" int stego_sample_labels_fwd(const void* label, const void* label_pos, int label_bytes,
+                                       const float* coords1, const float* coords2, const long long* perms, void* tiles,
+                                       int B, int n_classes, int Cpad, int H, int W, int feature_samples, int nslots,
+                                       int perms_are_raw_randperm, void* stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  STEGO_CHECK_ARG(label_bytes == 8 || label_bytes == 4 || label_bytes == 1,
+                  "stego_sample_labels_fwd: label_bytes=%d (8, 4 or 1)", label_bytes);
+  STEGO_CHECK_ARG(n_classes >= 1 && n_classes + 1 <= 256, "stego_sample_labels_fwd: n_classes=%d outside 1..255",
+                  n_classes);
+  STEGO_CHECK_ARG(Cpad <= 256, "stego_sample_labels_fwd: Cpad=%d exceeds 256", Cpad);
+  SampleParams sp;
+  int rc = fill_sample_params(sp, label, label_pos, 0, static_cast<long long>(H) * W, 0, W, 1, nullptr, nullptr,
+                              coords1, coords2, perms, tiles, B, n_classes + 1, Cpad, H, W, feature_samples, nslots);
+  if (rc != STEGO_OK) return rc;
+  sp.label_bytes = label_bytes;
+  sp.perms_raw = perms_are_raw_randperm;
+  STEGO_CHECK_ARG(tiles, "stego_sample_labels_fwd: null tiles");
+  STEGO_CHECK_ARG(nslots * B <= 65535, "stego_sample_labels_fwd: nslots * B = %d exceeds 65535", nslots * B);
+  return launch_sample_norm<true>(sp, stream, "stego_sample_labels_fwd");
 }
 
 extern "C" int stego_sample_norm_bwd(const float* code, const float* code_pos, long long stride_b, long long stride_c,

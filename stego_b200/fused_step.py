@@ -14,7 +14,7 @@ path, each costing ~4 us of launch latency behind the frozen ViT.  Here
     gradient buffer (no per-parameter AccumulateGrad kernels), and the scalar loss arithmetic is one launch.
 
 The stages are the functions the autograd nodes call (modules.pack_head_weights / head_forward / head_backward /
-cluster_lookup_forward / cluster_lookup_backward, corr.build_tiles / sample_norm_backward / LossSpec,
+cluster_lookup_forward / cluster_lookup_backward, corr.build_tiles / build_label_tiles / sample_norm_backward / LossSpec,
 segmenter.linear_probe_ce_step), given the workspace instead of per-call buffers: both paths launch the same kernels
 with the same arguments.  Only stego_step_losses is called from here alone.
 """
@@ -50,14 +50,16 @@ class FusedStep:
         seg, cfg = self.seg, self.seg.cfg
         img = batch["img"]
         return (img.is_cuda and seg.training and seg.net.training and cfg.correspondence_weight > 0
-                and not cfg.use_salience and not cfg.use_true_labels and seg.net.proj_type is not None
+                and not cfg.use_salience and seg.net.proj_type is not None
                 and cfg.rec_weight == 0 and cfg.aug_alignment_weight == 0 and cfg.crf_weight == 0
                 and cfg.neg_samples >= 1 and cfg.dino_feat_type == "feat"
                 and seg.linear_probe.weight.shape[0] <= 32 and seg.net.dim <= 96
-                and batch["label"].dtype in ops.LABEL_BYTES)
+                and batch["label"].dtype in ops.LABEL_BYTES
+                and (not cfg.use_true_labels or (batch.get("label_pos") is not None and seg.n_classes <= 255
+                                                 and batch["label_pos"].dtype in ops.LABEL_BYTES)))
 
     # ------------------------------------------------------------------------------------------
-    def _alloc(self, B, H, W, LH, LW, dev, label_dtype):
+    def _alloc(self, B, H, W, LH, LW, dev, label_dtype, label_pos_dtype):
         seg, cfg, net = self.seg, self.seg.cfg, self.seg.net
         ws = _Workspace()
         E, D = net.n_feats, net.dim
@@ -87,8 +89,9 @@ class FusedStep:
         ws.dyb = torch.empty(M, 128, dtype=bf, device=dev)
         ws.dh = torch.empty(M, E, dtype=f32, device=dev) if nonlinear else None
         ws.dhb = torch.empty(M, E, dtype=bf, device=dev) if nonlinear else None
-        # correspondence loss
-        ws.ftiles = torch.empty(2, spec.nslots, B, spec.rows, E, dtype=bf, device=dev)
+        # correspondence loss; the teacher operand is the features, or with use_true_labels the one-hot labels
+        ws.ET = corr.teacher_width(seg.n_classes + 1) if cfg.use_true_labels else E
+        ws.ftiles = torch.empty(2, spec.nslots, B, spec.rows, ws.ET, dtype=bf, device=dev)
         ws.ctiles = torch.empty(2, spec.nslots, B, spec.rows, corr.CODE_PAD, dtype=bf, device=dev)
         ws.partials, ws.row_means = spec.scratch(B, dev)
         ws.stats = torch.empty(spec.ncalls, 4, dtype=f32, device=dev)
@@ -106,6 +109,7 @@ class FusedStep:
         ws.one = torch.ones(1, dtype=f32, device=dev)
         ws.out4 = torch.empty(4, dtype=f32, device=dev)
         ws.label = torch.empty(B, LH, LW, dtype=label_dtype, device=dev)  # static copy: the tail graph bakes pointers
+        ws.label_pos = torch.empty(B, LH, LW, dtype=label_pos_dtype, device=dev) if cfg.use_true_labels else None
         ws.graph = None
         ws.eager_steps = 0
         # everything the kernels accumulate into: ONE buffer, ONE memset per step
@@ -160,11 +164,16 @@ class FusedStep:
         seg._mark("head_forward")
 
         # ---- correspondence loss forward (modules.py:349-398)
-        m3, p3 = (ws.M3[:B], ws.M3[B:]) if ws.M3 is not None else (None, None)
-        corr.build_tiles(feats[:B], feats[B:], ws.c1, ws.c2, ws.perms, spec, E, m3, p3, raw_perms=True, out=ws.ftiles)
+        if ws.label_pos is not None:  # use_true_labels (train_segmentation.py:135-137)
+            corr.build_label_tiles(ws.label, ws.label_pos, ws.c1, ws.c2, ws.perms, spec, seg.n_classes, raw_perms=True,
+                                   out=ws.ftiles)
+        else:
+            m3, p3 = (ws.M3[:B], ws.M3[B:]) if ws.M3 is not None else (None, None)
+            corr.build_tiles(feats[:B], feats[B:], ws.c1, ws.c2, ws.perms, spec, E, m3, p3, raw_perms=True,
+                             out=ws.ftiles)
         corr.build_tiles(code[:B], code[B:], ws.c1, ws.c2, ws.perms, spec, corr.CODE_PAD, raw_perms=True,
                          out=ws.ctiles)
-        spec.forward(ws.ftiles, ws.ctiles, B, E, D, ws.partials, ws.row_means, ws.stats)
+        spec.forward(ws.ftiles, ws.ctiles, B, ws.ET, D, ws.partials, ws.row_means, ws.stats)
         seg._mark("corr_loss_forward")
 
         # ---- probes on the detached code (train_segmentation.py:213-225): forward + backward in place
@@ -179,7 +188,7 @@ class FusedStep:
 
         # ---- backward (manual_backward, :227)
         modules.cluster_lookup_backward(code[:B], cl, None, ws.one, ws.dnc, cl.grad)
-        spec.backward(ws.ftiles, ws.ctiles, B, E, D, ws.stats, ws.row_means, ws.gscale, None, None, ws.dtiles)
+        spec.backward(ws.ftiles, ws.ctiles, B, ws.ET, D, ws.stats, ws.row_means, ws.gscale, None, None, ws.dtiles)
         dall = ws.dall.view(M, P)
         corr.sample_norm_backward(code[:B], code[B:], ws.c1, ws.c2, ws.perms, spec, ws.dtiles, dall[:B * hw],
                                   dall[B * hw:], raw_perms=True)
@@ -198,11 +207,13 @@ class FusedStep:
             seg.configure_optimizers()
         seg._flat.ensure_bound()  # parameters / .grad still are the views into the flat buffers the kernels write
         net_optim, linear_probe_optim, cluster_probe_optim = seg.optimizers()
+        label_pos = batch["label_pos"] if cfg.use_true_labels else None
         # a new flat parameter buffer (or another label dtype) invalidates the captured graph
-        key = (B, H, W, LH, LW, dev.index, id(seg._flat), label.dtype)
+        key = (B, H, W, LH, LW, dev.index, id(seg._flat), label.dtype,
+               label_pos.dtype if label_pos is not None else None)
         if self.key != key:
             self.flush()
-            self.ws = self._alloc(B, H, W, LH, LW, dev, label.dtype)
+            self.ws = self._alloc(B, H, W, LH, LW, dev, label.dtype, key[-1])
             self.key = key
             self.side = torch.cuda.Stream(device=dev)
         ws = self.ws
@@ -224,6 +235,8 @@ class FusedStep:
         with torch.no_grad():
             tok_all = net.backbone_tokens([img, img_pos], use_graph=getattr(cfg, "cuda_graph", True))  # [2B,hw,E] bf16
             ws.label.copy_(label.reshape(B, LH, LW))
+            if label_pos is not None:
+                ws.label_pos.copy_(label_pos.reshape(B, LH, LW))
             main.wait_event(ready)
             seg._mark("vit_forward")
             if use_graph and ws.graph is not None and ws.graph[1] == tok_all.data_ptr():

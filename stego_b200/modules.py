@@ -390,8 +390,10 @@ class ContrastiveCorrelationLoss(nn.Module):
         B = orig_feats.shape[0]
         perms = [super_perm(B, orig_feats.device) for _ in range(cfg.neg_samples)]
         spec = corr.make_spec(cfg)
+        # any_teacher: like the reference, the teacher signal may be of any width and resolution, e.g. the one-hot label
+        # maps of use_true_labels ([B, n_classes + 1, H, W] at label resolution, train_segmentation.py:135-137)
         losses, _cd_means, cd, elems = corr.corr_loss(orig_feats, orig_feats_pos, orig_code, orig_code_pos, coords1,
-                                                      coords2, perms, spec, want_elems=True)
+                                                      coords2, perms, spec, want_elems=True, any_teacher=True)
         fs = cfg.feature_samples
         five = (fs, fs, fs, fs)
         neg = cfg.neg_samples

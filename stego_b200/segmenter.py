@@ -175,6 +175,15 @@ def allreduce_gradients(flat: FlatParams) -> None:
         flat.grad_scale = 1.0
 
 
+def true_label_pos(batch) -> torch.Tensor:
+    """batch["label_pos"], the labels of img_pos that cfg.use_true_labels takes as the positive teacher signal
+    (train_segmentation.py:128, 136-137)."""
+    if batch.get("label_pos") is None:
+        raise RuntimeError("stego_b200: cfg.use_true_labels needs batch['label_pos'] (the labels of img_pos) next to "
+                           "batch['label']")
+    return batch["label_pos"]
+
+
 # --------------------------------------------------------------------------------------------------
 # linear probe: 1x1 conv -> bilinear upsample -> masked CE, forward + backward in one fused call
 # --------------------------------------------------------------------------------------------------
@@ -411,8 +420,7 @@ class LitUnsupervisedSegmenter(nn.Module):
         if use_pos:
             code_pos = code_all[B:]
             feats_pos = tok_all[B:].view(B, fh, fw, E).permute(0, 3, 1, 2)
-            if cfg.use_true_labels:
-                raise RuntimeError("stego_b200: use_true_labels is not part of the fused path")
+            label_pos = true_label_pos(batch) if cfg.use_true_labels else None
             salience = batch["mask"].to(torch.float32).squeeze(1) if cfg.use_salience else None
             salience_pos = batch["mask_pos"].to(torch.float32).squeeze(1) if cfg.use_salience else None
             lossfn = self.contrastive_corr_loss_fn
@@ -421,11 +429,20 @@ class LitUnsupervisedSegmenter(nn.Module):
             perms = torch.empty(cfg.neg_samples, B, dtype=torch.long, device=img.device)
             for i in range(cfg.neg_samples):
                 torch.randperm(B, device=img.device, dtype=torch.long, out=perms[i])
-            # the returned-feature dropout (modules.py:116) is folded into the sampling kernel (chan_scale)
-            losses, cd_means, _, _ = corr.corr_loss(feats, feats_pos, code_all, None, coords1, coords2, perms, self._spec,
-                                                    want_elems=False, chan_scale=m3 if cfg.dropout else None,
-                                                    chan_scale_pos=p3 if cfg.dropout else None, raw_perms=True,
-                                                    pair=True)
+            if cfg.use_true_labels:
+                # train_segmentation.py:135-137: the teacher signal is the one-hot ground truth, sampled straight from
+                # the label maps (m3 / p3 were drawn, as the reference's net() calls draw them, and scale nothing)
+                ftiles = corr.build_label_tiles(label, label_pos, coords1, coords2, perms, self._spec, self.n_classes,
+                                                raw_perms=True)
+                losses, cd_means, _, _ = corr.corr_loss(None, None, code_all, None, coords1, coords2, perms, self._spec,
+                                                        want_elems=False, raw_perms=True, pair=True, ftiles=ftiles)
+            else:
+                # the returned-feature dropout (modules.py:116) is folded into the sampling kernel (chan_scale)
+                losses, cd_means, _, _ = corr.corr_loss(feats, feats_pos, code_all, None, coords1, coords2, perms,
+                                                        self._spec, want_elems=False,
+                                                        chan_scale=m3 if cfg.dropout else None,
+                                                        chan_scale_pos=p3 if cfg.dropout else None, raw_perms=True,
+                                                        pair=True)
             pos_intra_loss, pos_inter_loss = losses[0], losses[1]
             neg_inter_loss = losses[2:].mean()
             self.log('loss/pos_intra', pos_intra_loss)
