@@ -171,6 +171,37 @@ STEGO_API int stego_corr_loss_tiled_bwd(const void* feat_tiles, const void* code
                                         const float* gelem, const float* gcd, float* dtiles, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * TensorBoard histograms (SummaryWriter.add_histogram with its default bins="tensorflow")
+ * ---------------------------------------------------------------------------------------------- */
+/* The 1549 float64 bucket edges of torch's SummaryWriter.default_bins (edges, may be null) and the 1550 fp32
+ * thresholds the kernels compare against (thresholds, may be null): the smallest float >= each edge, then the largest
+ * float <= the last edge.  Host arrays; no CUDA call. */
+STEGO_API int stego_tb_tables(double* edges, float* thresholds);
+/* np.histogram(values.astype(float64), default_bins) of n fp32 device values: counts [1548] int64 (overwritten; bucket
+ * k is [e_k, e_k+1), the last one closed, values outside [e_0, e_1548] not counted) and stats [4] float64 = min, max,
+ * sum, sum of squares.  thresholds: device copy of stego_tb_tables' table; cta_partials: scratch [264][4] float64.
+ * Counts are exact; the sums are reduced in a fixed order (bit-reproducible). */
+STEGO_API int stego_tb_histogram(const float* values, long long n, const float* thresholds, long long* counts,
+                                 double* cta_partials, double* stats, void* stream);
+/* stego_corr_loss_fwd / stego_corr_loss_tiled_fwd that also bin cd (the values cd_out would hold, padding excluded)
+ * into three histograms: group 0 = call 0, 1 = call 1, 2 = calls 2.. (the negatives).  Every other output is
+ * bit-identical to the plain call.  hist_counts [3][1548] int64 (overwritten); hist_stats [3][4] float64 as for
+ * stego_tb_histogram; hist_cta_partials: scratch [ncalls][B][4] float64 (tiled: [ncalls][B][(R/128)^2][4]). */
+STEGO_API int stego_corr_loss_fwd_hist(const void* feat_tiles, const void* code_tiles, int B, int feature_samples,
+                                       int E, int D, int nslots, int ncalls, const int* slot_of_call_host,
+                                       const float* shifts_host, int pointwise, int zero_clamp, int stabilize,
+                                       float* partials, float* stats, float* cd_out, float* fdc_out, float* loss_out,
+                                       const float* thresholds, long long* hist_counts, double* hist_cta_partials,
+                                       double* hist_stats, void* stream);
+STEGO_API int stego_corr_loss_tiled_fwd_hist(const void* feat_tiles, const void* code_tiles, int B,
+                                             int feature_samples, int E, int D, int nslots, int ncalls,
+                                             const int* slot_of_call_host, const float* shifts_host, int pointwise,
+                                             int zero_clamp, int stabilize, float* row_partials, float* row_means,
+                                             float* stats, float* cd_out, float* fdc_out, float* loss_out,
+                                             const float* thresholds, long long* hist_counts,
+                                             double* hist_cta_partials, double* hist_stats, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Segmentation head glue (reference: src/modules.py:73-81, 108-118) and optimiser
  * ---------------------------------------------------------------------------------------------- */
 /* Apply the three Dropout2d noises of DinoFeaturizer.forward (:109,:111,:116) in one pass:

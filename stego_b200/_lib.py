@@ -35,6 +35,7 @@ _CTYPES = {
     "unsigned char*": ctypes.c_void_p,
     "const unsigned char*": ctypes.c_void_p,
     "const double*": ctypes.c_void_p,
+    "double*": ctypes.c_void_p,
 }
 
 

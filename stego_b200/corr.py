@@ -81,6 +81,7 @@ class LossSpec:
     entry points: `scratch` allocates what `forward` needs, `forward` / `backward` launch the loss kernels."""
     tiled = False
     rows = TILE_ROWS  # operand / gradient tile rows per (slot, image)
+    hist_ctas = 1     # forward CTAs per (image, call)
 
     def __init__(self, cfg, n_neg: Optional[int] = None):
         _describe(self, cfg, n_neg)
@@ -93,10 +94,15 @@ class LossSpec:
         return (torch.empty(self.ncalls, B, 8, dtype=torch.float32, device=device),
                 torch.empty(0, dtype=torch.float32, device=device))
 
-    def forward(self, ftiles, ctiles, B, E, D, partials, row_means, stats, cd=None, fdc=None, elems=None):
-        _lib.check(_lib.load().stego_corr_loss_fwd(
-            *_loss_args(self, ftiles, ctiles, B, E, D), _lib.ptr(partials), _lib.ptr(stats), _lib.ptr(cd),
-            _lib.ptr(fdc), _lib.ptr(elems), _lib.stream()), "stego_corr_loss_fwd")
+    def forward(self, ftiles, ctiles, B, E, D, partials, row_means, stats, cd=None, fdc=None, elems=None, hist=None):
+        """hist: a hist.CdHistogram; the forward then also bins cd into its three histograms (same other outputs)."""
+        lib = _lib.load()
+        args = (*_loss_args(self, ftiles, ctiles, B, E, D), _lib.ptr(partials), _lib.ptr(stats), _lib.ptr(cd),
+                _lib.ptr(fdc), _lib.ptr(elems))
+        if hist is None:
+            _lib.check(lib.stego_corr_loss_fwd(*args, _lib.stream()), "stego_corr_loss_fwd")
+        else:
+            _lib.check(lib.stego_corr_loss_fwd_hist(*args, *hist.args(), _lib.stream()), "stego_corr_loss_fwd_hist")
 
     def backward(self, ftiles, ctiles, B, E, D, stats, row_means, gscale, gelem, gcd, dtiles):
         _lib.check(_lib.load().stego_corr_loss_bwd(
@@ -117,16 +123,22 @@ class TiledLossSpec:
         S = self.fs * self.fs
         self.rows = (S + TILE_ROWS - 1) // TILE_ROWS * TILE_ROWS
         self.n_tiles = self.rows // TILE_ROWS
+        self.hist_ctas = self.n_tiles * self.n_tiles
 
     def scratch(self, B, device):
         """(per-row partials, row means) for `forward`; `backward` reads the row means."""
         return (torch.empty(self.ncalls, B, self.n_tiles, self.rows, 4, dtype=torch.float32, device=device),
                 torch.empty(self.ncalls, B, self.rows, dtype=torch.float32, device=device))
 
-    def forward(self, ftiles, ctiles, B, E, D, partials, row_means, stats, cd=None, fdc=None, elems=None):
-        _lib.check(_lib.load().stego_corr_loss_tiled_fwd(
-            *_loss_args(self, ftiles, ctiles, B, E, D), _lib.ptr(partials), _lib.ptr(row_means), _lib.ptr(stats),
-            _lib.ptr(cd), _lib.ptr(fdc), _lib.ptr(elems), _lib.stream()), "stego_corr_loss_tiled_fwd")
+    def forward(self, ftiles, ctiles, B, E, D, partials, row_means, stats, cd=None, fdc=None, elems=None, hist=None):
+        lib = _lib.load()
+        args = (*_loss_args(self, ftiles, ctiles, B, E, D), _lib.ptr(partials), _lib.ptr(row_means), _lib.ptr(stats),
+                _lib.ptr(cd), _lib.ptr(fdc), _lib.ptr(elems))
+        if hist is None:
+            _lib.check(lib.stego_corr_loss_tiled_fwd(*args, _lib.stream()), "stego_corr_loss_tiled_fwd")
+        else:
+            _lib.check(lib.stego_corr_loss_tiled_fwd_hist(*args, *hist.args(), _lib.stream()),
+                       "stego_corr_loss_tiled_fwd_hist")
 
     def backward(self, ftiles, ctiles, B, E, D, stats, row_means, gscale, gelem, gcd, dtiles):
         _lib.check(_lib.load().stego_corr_loss_tiled_bwd(
@@ -249,7 +261,7 @@ class _CorrLossFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, code, code_pos, feats, feats_pos, coords1, coords2, perms, spec: LossSpec, want_elems: bool,
-                chan_scale, chan_scale_pos, raw_perms=False, pair=False, ftiles=None, any_teacher=False):
+                chan_scale, chan_scale_pos, raw_perms=False, pair=False, ftiles=None, any_teacher=False, hist=None):
         # pair=True: `code` is the [2B, D, h, w] output of ONE head pass over img ++ img_pos (code_pos is None); its
         # gradient is then produced in one buffer instead of two tensors that autograd has to re-assemble.
         if pair:
@@ -282,7 +294,7 @@ class _CorrLossFn(torch.autograd.Function):
             fdc = torch.empty_like(cd)
             elems = torch.empty_like(cd)
         partials, row_means = spec.scratch(B, dev)
-        spec.forward(ftiles, ctiles, B, E, D, partials, row_means, stats, cd, fdc, elems)
+        spec.forward(ftiles, ctiles, B, E, D, partials, row_means, stats, cd, fdc, elems, hist)
         ctx.spec = spec
         ctx.dims = (B, E, D, H, W)
         ctx.code_dtype = (code.dtype, code_pos.dtype if code_pos is not None else code.dtype)
@@ -319,13 +331,13 @@ class _CorrLossFn(torch.autograd.Function):
                              ctx.raw_perms)
         d0, d1 = ctx.code_dtype
         if ctx.pair:
-            return (dall.to(d0), None) + (None,) * 13
-        return (dcode.to(d0), dcode_pos.to(d1)) + (None,) * 13
+            return (dall.to(d0), None) + (None,) * 14
+        return (dcode.to(d0), dcode_pos.to(d1)) + (None,) * 14
 
 
 def corr_loss(feats, feats_pos, code, code_pos, coords1, coords2, perms, spec: LossSpec, want_elems: bool = False,
               chan_scale=None, chan_scale_pos=None, raw_perms: bool = False, pair: bool = False, *,
-              ftiles: Optional[torch.Tensor] = None, any_teacher: bool = False):
+              ftiles: Optional[torch.Tensor] = None, any_teacher: bool = False, hist=None):
     """raw_perms=True: `perms` holds the raw torch.randperm draws and the sampling kernel applies super_perm's
     fix-up itself (saves the eq/add/remainder launches of modules.super_perm).
     pair=True: `code` holds code ++ code_pos ([2B, D, h, w], one head pass) and `code_pos` is None.
@@ -334,7 +346,8 @@ def corr_loss(feats, feats_pos, code, code_pos, coords1, coords2, perms, spec: L
     any_teacher=True: feats / feats_pos may have any channel count up to 768 and any spatial size, as the reference's
     ContrastiveCorrelationLoss accepts (see _prep_common); without it they are code-sized with channels % 64 == 0.
     spec: a LossSpec (single-tile kernels) or a TiledLossSpec (multi-tile kernels); make_spec picks by feature_samples.
+    hist: a hist.CdHistogram for (spec, B): the forward also bins the cd of the three loss groups into it.
     Returns (losses[ncalls], cd_means[ncalls], cd[ncalls,B,S,S]|None, loss_elems|None).
     losses[k] is the mean of helper call k (0 intra, 1 inter, 2.. negatives); differentiable wrt code/code_pos."""
     return _CorrLossFn.apply(code, code_pos, feats, feats_pos, coords1, coords2, perms, spec, want_elems,
-                             chan_scale, chan_scale_pos, raw_perms, pair, ftiles, any_teacher)
+                             chan_scale, chan_scale_pos, raw_perms, pair, ftiles, any_teacher, hist)

@@ -24,6 +24,7 @@
 #include "common.cuh"
 #include "host_util.h"
 #include "probe_common.cuh"
+#include "tb_hist.cuh"
 
 namespace stego {
 
@@ -309,6 +310,10 @@ struct CorrParams {
   const float* gelem;    // optional [ncalls][B][S][S] upstream grad of unreduced loss elements
   const float* gcd;      // optional [ncalls][B][S][S] upstream grad of cd elements
   float* dtiles;         // [nslots][B][R][CL_DT_LD] fp32, zero-initialised by the caller
+  // histogram variants (kVariant | CP_HIST) only: TensorBoard histograms of cd per group (call 0, call 1, calls 2..)
+  const float* hist_thr;             // [TB_THR] fp32 bucket thresholds (tb_hist.cuh)
+  unsigned long long* hist_counts;   // [3][TB_BINS], zeroed by the caller, added to with integer atomics
+  double* hist_part;                 // [ncalls][B][CTAs per (image, call)][4]: min, max, sum, sum of squares
 };
 
 constexpr int CL_THREADS = 384;  // two MMA warpgroups (rows 0..63 / 64..127 of the tile) + the TMA producer warpgroup
@@ -320,6 +325,7 @@ constexpr int CP_FWD_ROWPART = 1;  // multi-tile, grid (B, ncalls, nT^2): per-ro
 constexpr int CP_BWD = 2;          // whole row, grid (B): the calls in order, dA -> slot 0 and dB -> the call's slot
 constexpr int CP_BWD_DB = 3;       // multi-tile, grid (B, nT): CTA per (image, ct) walking (call, rt) -> dB rows ct
 constexpr int CP_BWD_DA = 4;       // multi-tile, grid (B, nT): CTA per (image, rt) walking (call, ct) -> dA rows rt
+constexpr int CP_HIST = 8;         // flag on CP_FWD / CP_FWD_ROWPART: also bin cd into TensorBoard histograms
 
 // unit u of this CTA -> (call, row tile, column tile)
 template <int kPhase>
@@ -348,9 +354,60 @@ __device__ __forceinline__ void split_pass(int pass, int& pa, int& pb) {
   pb = (pass == 2) ? 1 : 0;
 }
 
-template <int kPhase>
+// Histogram epilogue of the forward variants: bins this CTA's cd block into the TensorBoard histogram of the call's
+// group (0: call 0, 1: call 1, 2: the negatives, which the reference concatenates) and writes the CTA's min / max / sum
+// / sum-of-squares partial.  Only elements with row and column < S are values of the reference's cd tensors: the
+// padding rows / columns of the 128-row tiles hold cd = 0 and are skipped.  Run by the 256 MMA threads after a
+// bar.sync that both warpgroups reach past their wgmma_wait<0>.  The bins live in the operand ring, which is free then:
+// a forward CTA runs one unit, its producer issues no load after the unit's last stage, every stage's full barrier has
+// been waited on (so each TMA write into the ring has landed), and no wgmma reads the ring any more.
+__device__ __forceinline__ void corr_hist_epilogue(const CorrParams& p, const float (&cd)[64], int i0, int j0, int call,
+                                                   int b, uint8_t* smem, int warp, int lane) {
+  float* thr = reinterpret_cast<float*>(smem);
+  uint32_t* bins = reinterpret_cast<uint32_t*>(smem + 6208);             // after TB_THR floats, 16-byte aligned
+  TbStats* wred = reinterpret_cast<TbStats*>(smem + 6208 + 4 * TB_BINS);  // [8 warps]
+  const int tid = threadIdx.x;  // 0 .. 255: the MMA warpgroups
+  for (int k = tid; k < TB_THR; k += 256) thr[k] = p.hist_thr[k];
+  for (int k = tid; k < TB_BINS; k += 256) bins[k] = 0;
+  asm volatile("bar.sync 1, 256;\n" ::: "memory");
+  const int S = p.S;
+  TbStats st;
+  st.init();
+#pragma unroll
+  for (int t = 0; t < 64; ++t) {
+    const int i = i0 + 8 * ((t >> 1) & 1);
+    const int j = j0 + 8 * (t >> 2) + (t & 1);
+    if (i < S && j < S) {
+      const int k = tb_bucket(cd[t], thr);
+      if (k >= 0) atomicAdd(&bins[k], 1u);
+      st.add(cd[t]);
+    }
+  }
+  st.warp_reduce();
+  if (lane == 0) wred[warp] = st;
+  asm volatile("bar.sync 1, 256;\n" ::: "memory");
+  unsigned long long* counts = p.hist_counts + static_cast<size_t>(min(call, 2)) * TB_BINS;
+  for (int k = tid; k < TB_BINS; k += 256)
+    if (bins[k]) atomicAdd(&counts[k], static_cast<unsigned long long>(bins[k]));
+  if (tid == 0) {
+    TbStats c = wred[0];
+    for (int w = 1; w < 8; ++w) {
+      c.mn = fminf(c.mn, wred[w].mn);
+      c.mx = fmaxf(c.mx, wred[w].mx);
+      c.s += wred[w].s;
+      c.s2 += wred[w].s2;
+    }
+    double* o = p.hist_part + ((static_cast<size_t>(call) * p.B + b) * gridDim.z + blockIdx.z) * 4;
+    o[0] = c.mn; o[1] = c.mx; o[2] = c.s; o[3] = c.s2;
+  }
+}
+
+template <int kVariant>
 __global__ void __launch_bounds__(CL_THREADS, 1)
 corr_kernel(const __grid_constant__ CUtensorMap tmF, const __grid_constant__ CUtensorMap tmC, CorrParams p) {
+  constexpr int kPhase = kVariant & ~CP_HIST;
+  constexpr bool kHist = (kVariant & CP_HIST) != 0;
+  static_assert(!kHist || kPhase <= CP_FWD_ROWPART, "histograms are a forward epilogue");
   constexpr bool kBackward = kPhase >= CP_BWD;
   constexpr bool kDA = kPhase == CP_BWD || kPhase == CP_BWD_DA;
   constexpr bool kDB = kPhase == CP_BWD || kPhase == CP_BWD_DB;
@@ -521,6 +578,10 @@ corr_kernel(const __grid_constant__ CUtensorMap tmF, const __grid_constant__ CUt
           *reinterpret_cast<float4*>(p.rowpart + (((static_cast<size_t>(call) * p.B + b) * p.nT + ct) * p.R + i) * 4) =
               make_float4(r_fd[h], r_clfd[h], r_cl[h], r_cd[h]);
       }
+      if constexpr (kHist) {
+        asm volatile("bar.sync 1, 256;\n" ::: "memory");
+        corr_hist_epilogue(p, cd, i0, j0, call, b, smem, warp, lane);
+      }
       return;
     }
     // the row means of fd for fragment halves 0 / 1: from the row sums over the valid columns of the whole-row unit
@@ -580,6 +641,7 @@ corr_kernel(const __grid_constant__ CUtensorMap tmF, const __grid_constant__ CUt
         for (int w = 0; w < 8; ++w) tot += red[w * 8 + lane];
         p.partials[(static_cast<size_t>(call) * p.B + b) * 8 + lane] = tot;
       }
+      if constexpr (kHist) corr_hist_epilogue(p, cd, i0, j0, call, b, smem, warp, lane);
       return;
     }
     {
@@ -1066,15 +1128,17 @@ static int fill_corr_params(CorrParams& p, bool tiled, int B, int fs, int E, int
   p.clamp_hi = stabilize ? 0.8f : INFINITY;
   p.partials = nullptr; p.rowpart = nullptr; p.cd_out = nullptr; p.fd_out = nullptr;
   p.stats = nullptr; p.rowmean = nullptr; p.gscale = nullptr; p.gelem = nullptr; p.gcd = nullptr; p.dtiles = nullptr;
+  p.hist_thr = nullptr; p.hist_counts = nullptr; p.hist_part = nullptr;
   return STEGO_OK;
 }
 
-template <int kPhase>
+template <int kVariant>
 static int launch_corr(const CUtensorMap& tmF, const CUtensorMap& tmC, const CorrParams& p, cudaStream_t stream) {
+  constexpr int kPhase = kVariant & ~CP_HIST;
   constexpr int kRing = kPhase >= CP_BWD ? 2 : 3;
   constexpr size_t smem = size_t(kRing) * 2 * CL_TILE + 8 * CL_TILE + 512 + 1024;
   static_assert(smem <= 232448, "exceeds the 227 KB of shared memory a CTA can opt into");
-  constexpr auto kern = corr_kernel<kPhase>;
+  constexpr auto kern = corr_kernel<kVariant>;
   if (const int rc = opt_in_smem<kern>(smem, "corr_kernel"); rc != STEGO_OK) return rc;
   const dim3 grid = kPhase == CP_FWD ? dim3(p.B, p.ncalls)
                   : kPhase == CP_FWD_ROWPART ? dim3(p.B, p.ncalls, p.nT * p.nT)
@@ -1084,13 +1148,38 @@ static int launch_corr(const CUtensorMap& tmF, const CUtensorMap& tmC, const Cor
   return STEGO_OK;
 }
 
-// host arrays (slot_of_call, shifts) are plain host pointers: they are copied into kernel parameters.
-extern "C" int stego_corr_loss_fwd(const void* feat_tiles, const void* code_tiles, int B, int feature_samples, int E,
-                                   int D, int nslots, int ncalls, const int* slot_of_call_host,
-                                   const float* shifts_host, int pointwise, int zero_clamp, int stabilize,
-                                   float* partials, float* stats, float* cd_out, float* fdc_out, float* loss_out,
-                                   void* stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+// Histogram outputs of the *_fwd_hist entry points (null: the plain forward).
+struct HistOut {
+  const float* thresholds;  // [TB_THR]
+  long long* counts;        // [3][TB_BINS], overwritten
+  double* cta_partials;     // scratch [ncalls][B][CTAs per (image, call)][4]
+  double* stats;            // [3][4]: min, max, sum, sum of squares per group
+};
+
+// Zeroes the counts and points the kernel at the histogram outputs.
+static int hist_prepare(CorrParams& p, const HistOut& h, cudaStream_t stream, const char* who) {
+  STEGO_CHECK_ARG(h.thresholds && h.counts && h.cta_partials && h.stats, "%s: null histogram pointer", who);
+  cudaError_t e = cudaMemsetAsync(h.counts, 0, sizeof(long long) * TB_GROUPS_MAX * TB_BINS, stream);
+  if (e != cudaSuccess) return cuda_fail(e, who);
+  p.hist_thr = h.thresholds;
+  p.hist_counts = reinterpret_cast<unsigned long long*>(h.counts);
+  p.hist_part = h.cta_partials;
+  return STEGO_OK;
+}
+
+// min / max / sums per group from the per-CTA partials: group 0 = call 0, 1 = call 1, 2 = calls 2..
+static int hist_finish(const CorrParams& p, const HistOut& h, int ctas_per_call, cudaStream_t stream) {
+  const int per_call = p.B * ctas_per_call;
+  int first[TB_GROUPS_MAX + 1] = {0, per_call, 2 * per_call, p.ncalls * per_call};
+  const int ngroups = p.ncalls < TB_GROUPS_MAX ? p.ncalls : TB_GROUPS_MAX;
+  first[ngroups] = p.ncalls * per_call;
+  return tb_launch_finish(h.cta_partials, first, ngroups, h.stats, stream);
+}
+
+static int corr_fwd(const void* feat_tiles, const void* code_tiles, int B, int feature_samples, int E, int D,
+                    int nslots, int ncalls, const int* slot_of_call_host, const float* shifts_host, int pointwise,
+                    int zero_clamp, int stabilize, float* partials, float* stats, float* cd_out, float* fdc_out,
+                    float* loss_out, const HistOut* hist, cudaStream_t stream) {
   STEGO_CHECK_ARG(feat_tiles && code_tiles && partials && stats && slot_of_call_host && shifts_host,
                   "stego_corr_loss_fwd: null pointer");
   STEGO_CHECK_ARG(!loss_out || (cd_out && fdc_out), "stego_corr_loss_fwd: loss_out needs cd_out and fdc_out");
@@ -1101,7 +1190,13 @@ extern "C" int stego_corr_loss_fwd(const void* feat_tiles, const void* code_tile
   p.partials = partials; p.cd_out = cd_out; p.fd_out = fdc_out;
   CUtensorMap tmF, tmC;
   if ((rc = encode_tile_maps(feat_tiles, code_tiles, p, &tmF, &tmC)) != STEGO_OK) return rc;
-  if ((rc = launch_corr<CP_FWD>(tmF, tmC, p, stream)) != STEGO_OK) return rc;
+  if (hist) {
+    if ((rc = hist_prepare(p, *hist, stream, "stego_corr_loss_fwd_hist")) != STEGO_OK) return rc;
+    if ((rc = launch_corr<CP_FWD | CP_HIST>(tmF, tmC, p, stream)) != STEGO_OK) return rc;
+    if ((rc = hist_finish(p, *hist, 1, stream)) != STEGO_OK) return rc;
+  } else if ((rc = launch_corr<CP_FWD>(tmF, tmC, p, stream)) != STEGO_OK) {
+    return rc;
+  }
   corr_finish_kernel<<<ncalls, 32, 0, stream>>>(partials, stats, ncalls, B, p.S, pointwise);
   STEGO_CHECK_LAUNCH("corr_finish_kernel");
   if (loss_out) {
@@ -1111,6 +1206,29 @@ extern "C" int stego_corr_loss_fwd(const void* feat_tiles, const void* code_tile
     STEGO_CHECK_LAUNCH("corr_loss_elems_kernel");
   }
   return STEGO_OK;
+}
+
+// host arrays (slot_of_call, shifts) are plain host pointers: they are copied into kernel parameters.
+extern "C" int stego_corr_loss_fwd(const void* feat_tiles, const void* code_tiles, int B, int feature_samples, int E,
+                                   int D, int nslots, int ncalls, const int* slot_of_call_host,
+                                   const float* shifts_host, int pointwise, int zero_clamp, int stabilize,
+                                   float* partials, float* stats, float* cd_out, float* fdc_out, float* loss_out,
+                                   void* stream_) {
+  return corr_fwd(feat_tiles, code_tiles, B, feature_samples, E, D, nslots, ncalls, slot_of_call_host, shifts_host,
+                  pointwise, zero_clamp, stabilize, partials, stats, cd_out, fdc_out, loss_out, nullptr,
+                  reinterpret_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int stego_corr_loss_fwd_hist(const void* feat_tiles, const void* code_tiles, int B, int feature_samples,
+                                        int E, int D, int nslots, int ncalls, const int* slot_of_call_host,
+                                        const float* shifts_host, int pointwise, int zero_clamp, int stabilize,
+                                        float* partials, float* stats, float* cd_out, float* fdc_out, float* loss_out,
+                                        const float* thresholds, long long* hist_counts, double* hist_cta_partials,
+                                        double* hist_stats, void* stream_) {
+  const HistOut h{thresholds, hist_counts, hist_cta_partials, hist_stats};
+  return corr_fwd(feat_tiles, code_tiles, B, feature_samples, E, D, nslots, ncalls, slot_of_call_host, shifts_host,
+                  pointwise, zero_clamp, stabilize, partials, stats, cd_out, fdc_out, loss_out, &h,
+                  reinterpret_cast<cudaStream_t>(stream_));
 }
 
 extern "C" int stego_corr_loss_bwd(const void* feat_tiles, const void* code_tiles, int B, int feature_samples, int E,
@@ -1131,12 +1249,10 @@ extern "C" int stego_corr_loss_bwd(const void* feat_tiles, const void* code_tile
   return launch_corr<CP_BWD>(tmF, tmC, p, stream);
 }
 
-extern "C" int stego_corr_loss_tiled_fwd(const void* feat_tiles, const void* code_tiles, int B, int feature_samples,
-                                         int E, int D, int nslots, int ncalls, const int* slot_of_call_host,
-                                         const float* shifts_host, int pointwise, int zero_clamp, int stabilize,
-                                         float* row_partials, float* row_means, float* stats, float* cd_out,
-                                         float* fdc_out, float* loss_out, void* stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+static int corr_tiled_fwd(const void* feat_tiles, const void* code_tiles, int B, int feature_samples, int E, int D,
+                          int nslots, int ncalls, const int* slot_of_call_host, const float* shifts_host, int pointwise,
+                          int zero_clamp, int stabilize, float* row_partials, float* row_means, float* stats,
+                          float* cd_out, float* fdc_out, float* loss_out, const HistOut* hist, cudaStream_t stream) {
   STEGO_CHECK_ARG(feat_tiles && code_tiles && row_partials && row_means && stats && slot_of_call_host && shifts_host,
                   "stego_corr_loss_tiled_fwd: null pointer");
   STEGO_CHECK_ARG(!loss_out || (cd_out && fdc_out), "stego_corr_loss_tiled_fwd: loss_out needs cd_out and fdc_out");
@@ -1147,7 +1263,13 @@ extern "C" int stego_corr_loss_tiled_fwd(const void* feat_tiles, const void* cod
   p.rowpart = row_partials; p.cd_out = cd_out; p.fd_out = fdc_out;
   CUtensorMap tmF, tmC;
   if ((rc = encode_tile_maps(feat_tiles, code_tiles, p, &tmF, &tmC)) != STEGO_OK) return rc;
-  if ((rc = launch_corr<CP_FWD_ROWPART>(tmF, tmC, p, stream)) != STEGO_OK) return rc;
+  if (hist) {
+    if ((rc = hist_prepare(p, *hist, stream, "stego_corr_loss_tiled_fwd_hist")) != STEGO_OK) return rc;
+    if ((rc = launch_corr<CP_FWD_ROWPART | CP_HIST>(tmF, tmC, p, stream)) != STEGO_OK) return rc;
+    if ((rc = hist_finish(p, *hist, p.nT * p.nT, stream)) != STEGO_OK) return rc;
+  } else if ((rc = launch_corr<CP_FWD_ROWPART>(tmF, tmC, p, stream)) != STEGO_OK) {
+    return rc;
+  }
   corr_tiled_finish_kernel<<<ncalls, CT_FINISH_THREADS, 0, stream>>>(p, row_means, stats);
   STEGO_CHECK_LAUNCH("corr_tiled_finish_kernel");
   if (fdc_out) {
@@ -1157,6 +1279,29 @@ extern "C" int stego_corr_loss_tiled_fwd(const void* feat_tiles, const void* cod
     STEGO_CHECK_LAUNCH("corr_tiled_elems_kernel");
   }
   return STEGO_OK;
+}
+
+extern "C" int stego_corr_loss_tiled_fwd(const void* feat_tiles, const void* code_tiles, int B, int feature_samples,
+                                         int E, int D, int nslots, int ncalls, const int* slot_of_call_host,
+                                         const float* shifts_host, int pointwise, int zero_clamp, int stabilize,
+                                         float* row_partials, float* row_means, float* stats, float* cd_out,
+                                         float* fdc_out, float* loss_out, void* stream_) {
+  return corr_tiled_fwd(feat_tiles, code_tiles, B, feature_samples, E, D, nslots, ncalls, slot_of_call_host,
+                        shifts_host, pointwise, zero_clamp, stabilize, row_partials, row_means, stats, cd_out, fdc_out,
+                        loss_out, nullptr, reinterpret_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int stego_corr_loss_tiled_fwd_hist(const void* feat_tiles, const void* code_tiles, int B,
+                                              int feature_samples, int E, int D, int nslots, int ncalls,
+                                              const int* slot_of_call_host, const float* shifts_host, int pointwise,
+                                              int zero_clamp, int stabilize, float* row_partials, float* row_means,
+                                              float* stats, float* cd_out, float* fdc_out, float* loss_out,
+                                              const float* thresholds, long long* hist_counts,
+                                              double* hist_cta_partials, double* hist_stats, void* stream_) {
+  const HistOut h{thresholds, hist_counts, hist_cta_partials, hist_stats};
+  return corr_tiled_fwd(feat_tiles, code_tiles, B, feature_samples, E, D, nslots, ncalls, slot_of_call_host,
+                        shifts_host, pointwise, zero_clamp, stabilize, row_partials, row_means, stats, cd_out, fdc_out,
+                        loss_out, &h, reinterpret_cast<cudaStream_t>(stream_));
 }
 
 extern "C" int stego_corr_loss_tiled_bwd(const void* feat_tiles, const void* code_tiles, int B, int feature_samples,

@@ -112,6 +112,8 @@ class FusedStep:
         ws.label_pos = torch.empty(B, LH, LW, dtype=label_pos_dtype, device=dev) if cfg.use_true_labels else None
         ws.graph = None
         ws.eager_steps = 0
+        ws.hist = None        # hist.CdHistogram and the tail graph that fills it, made on the first histogram step
+        ws.hist_graph = None
         # everything the kernels accumulate into: ONE buffer, ONE memset per step
         sizes = dict(dlogits=B * hw * 32, dtiles=spec.nslots * B * spec.rows * corr.DT_LD, dall=M * P,
                      dnc=n_clu * D, db_pad=P)
@@ -146,9 +148,10 @@ class FusedStep:
         seg._flat.grad.zero_()
 
     # ------------------------------------------------------------------------------------------
-    def _tail(self, ws, tok_all):
+    def _tail(self, ws, tok_all, hist=None):
         """Head forward .. head backward on the current stream: static workspace, no allocation, no RNG, no host
-        synchronisation — captured as one CUDA graph after the first (eager) step."""
+        synchronisation — captured as one CUDA graph after the first (eager) step.  hist: the correlation forward also
+        bins the cd histograms into it (a second graph, for the steps that log them)."""
         seg, net = self.seg, self.seg.net
         B, E, D, P, fh, fw, hw, M, nonlinear = ws.dims
         spec = seg._spec
@@ -173,7 +176,7 @@ class FusedStep:
                              out=ws.ftiles)
         corr.build_tiles(code[:B], code[B:], ws.c1, ws.c2, ws.perms, spec, corr.CODE_PAD, raw_perms=True,
                          out=ws.ctiles)
-        spec.forward(ws.ftiles, ws.ctiles, B, ws.ET, D, ws.partials, ws.row_means, ws.stats)
+        spec.forward(ws.ftiles, ws.ctiles, B, ws.ET, D, ws.partials, ws.row_means, ws.stats, hist=hist)
         seg._mark("corr_loss_forward")
 
         # ---- probes on the detached code (train_segmentation.py:213-225): forward + backward in place
@@ -218,6 +221,7 @@ class FusedStep:
             self.side = torch.cuda.Stream(device=dev)
         ws = self.ws
         B, E, D, P, fh, fw, hw, M, nonlinear = ws.dims
+        spec = seg._spec
         main = torch.cuda.current_stream()
         seg._mark("start")
 
@@ -239,7 +243,21 @@ class FusedStep:
                 ws.label_pos.copy_(label_pos.reshape(B, LH, LW))
             main.wait_event(ready)
             seg._mark("vit_forward")
-            if use_graph and ws.graph is not None and ws.graph[1] == tok_all.data_ptr():
+            if seg.should_log_hist():
+                # histogram steps replay a tail graph of their own (captured the first time one is needed), so the
+                # graph of every other step stays what it is
+                if ws.hist is None:
+                    from .hist import CdHistogram
+                    ws.hist = CdHistogram(spec, B, dev)
+                if use_graph and ws.hist_graph is not None and ws.hist_graph[1] == tok_all.data_ptr():
+                    ws.hist_graph[0].replay()
+                elif use_graph and ws.eager_steps >= 1:
+                    ws.hist_graph = (_lib.Graph(lambda: self._tail(ws, tok_all, ws.hist)), tok_all.data_ptr())
+                    ws.hist_graph[0].replay()
+                else:
+                    self._tail(ws, tok_all, ws.hist)
+                seg._stage_histograms(ws.hist)
+            elif use_graph and ws.graph is not None and ws.graph[1] == tok_all.data_ptr():
                 ws.graph[0].replay()
             elif use_graph and ws.eager_steps >= 1:
                 # second step on this shape: capture head fwd .. head bwd (static workspace, no allocation, no RNG) as ONE

@@ -274,6 +274,14 @@ class LitUnsupervisedSegmenter(nn.Module):
         self._spec = corr.make_spec(cfg)
         self._fused = None
         self.profile_marks = None  # optional list: bench.py --breakdown collects (name, cuda event) pairs here
+        # cd histograms every cfg.hist_freq steps (train_segmentation.py:144-146, 165-168) go to
+        # logger.experiment.add_histogram_raw: anything with that, e.g. a Lightning TensorBoardLogger or
+        # SimpleNamespace(experiment=SummaryWriter(...)).  None: no histograms, and the step launches nothing extra.
+        # Under torch.distributed each rank bins its own shard; set the logger on rank 0 only, as the reference writes
+        # from rank 0's experiment.
+        self.logger = None
+        self.logged_histograms: Dict[str, dict] = {}  # tag -> the add_histogram_raw fields last passed to the logger
+        self._hist_pending = None  # (hist.CdHistogram, global_step) staged by a step, delivered by the next one
 
     # ---- Lightning-shaped surface ----------------------------------------------------------------
     def forward(self, x):
@@ -296,6 +304,28 @@ class LitUnsupervisedSegmenter(nn.Module):
         parameters / gradients / optimiser state outside training_step (forward and state_dict do)."""
         if self._fused is not None:
             self._fused.flush()
+        self._deliver_histograms()
+
+    def should_log_hist(self) -> bool:
+        """train_segmentation.py:142-144 (should_log_hist), for a step that has a logger and a correspondence loss."""
+        f = getattr(self.cfg, "hist_freq", None)
+        return (self.logger is not None and f is not None and self.global_step % f == 0 and self.global_step > 0
+                and self.cfg.correspondence_weight > 0)
+
+    def _stage_histograms(self, h) -> None:
+        """Queue the copies of a step's histograms to the host; the next training_step or flush() logs them."""
+        h.stage()
+        self._hist_pending = (h, self.global_step)
+
+    def _deliver_histograms(self) -> None:
+        if self._hist_pending is None:
+            return
+        h, step = self._hist_pending
+        self._hist_pending = None
+        for tag, f in h.results().items():
+            self.logged_histograms[tag] = f
+            if self.logger is not None:
+                self.logger.experiment.add_histogram_raw(tag, global_step=step, **f)
 
     def state_dict(self, *args, **kwargs):
         self.check_update_health()
@@ -374,6 +404,7 @@ class LitUnsupervisedSegmenter(nn.Module):
         """train_segmentation.py:112-245.  The shipped configuration (dino arch, correspondence loss, no salience /
         rec / aug / crf terms) runs as the hand-scheduled kernel sequence of fused_step.FusedStep; anything else
         (or cfg.fused_step = False) takes the autograd-stitched path below.  Both compute the same step."""
+        self._deliver_histograms()
         if getattr(self.cfg, "fused_step", True):
             if self._fused is None:
                 from .fused_step import FusedStep
@@ -417,6 +448,7 @@ class LitUnsupervisedSegmenter(nn.Module):
 
         self._mark("head_forward")
         loss = 0
+        hist = None
         if use_pos:
             code_pos = code_all[B:]
             feats_pos = tok_all[B:].view(B, fh, fw, E).permute(0, 3, 1, 2)
@@ -424,6 +456,9 @@ class LitUnsupervisedSegmenter(nn.Module):
             salience = batch["mask"].to(torch.float32).squeeze(1) if cfg.use_salience else None
             salience_pos = batch["mask_pos"].to(torch.float32).squeeze(1) if cfg.use_salience else None
             lossfn = self.contrastive_corr_loss_fn
+            if self.should_log_hist():
+                from .hist import CdHistogram
+                hist = CdHistogram(self._spec, B, img.device)
             coords1, coords2 = lossfn.draw_coords(feats, salience, salience_pos)
             # same RNG calls as modules.super_perm (randperm per negative); its fix-up runs inside the sampling kernel
             perms = torch.empty(cfg.neg_samples, B, dtype=torch.long, device=img.device)
@@ -435,14 +470,17 @@ class LitUnsupervisedSegmenter(nn.Module):
                 ftiles = corr.build_label_tiles(label, label_pos, coords1, coords2, perms, self._spec, self.n_classes,
                                                 raw_perms=True)
                 losses, cd_means, _, _ = corr.corr_loss(None, None, code_all, None, coords1, coords2, perms, self._spec,
-                                                        want_elems=False, raw_perms=True, pair=True, ftiles=ftiles)
+                                                        want_elems=False, raw_perms=True, pair=True, ftiles=ftiles,
+                                                        hist=hist)
             else:
                 # the returned-feature dropout (modules.py:116) is folded into the sampling kernel (chan_scale)
                 losses, cd_means, _, _ = corr.corr_loss(feats, feats_pos, code_all, None, coords1, coords2, perms,
                                                         self._spec, want_elems=False,
                                                         chan_scale=m3 if cfg.dropout else None,
                                                         chan_scale_pos=p3 if cfg.dropout else None, raw_perms=True,
-                                                        pair=True)
+                                                        pair=True, hist=hist)
+            if hist is not None:
+                self._stage_histograms(hist)
             pos_intra_loss, pos_inter_loss = losses[0], losses[1]
             neg_inter_loss = losses[2:].mean()
             self.log('loss/pos_intra', pos_intra_loss)
