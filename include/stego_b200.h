@@ -318,6 +318,37 @@ STEGO_API int stego_crf_update(const float* unary, const int* off_g, const float
                                const int* off_b, const float* bary_b, const float* val_b, const float* norm_b, float w_g,
                                float w_b, float* Q, float* q_out, unsigned char* argmax_out, long long N, int C, void* stream);
 
+/* ---- CRF-refined evaluation (src/eval_segmentation.py:124-141 with run_crf=True): both probes' dense CRFs for a batch
+ * of frames, deterministic (gather splats, no float atomics).  Rows of 64 floats per pixel and lattice point: linear
+ * probe in [0, 32), cluster probe in [32, 64).
+ * stego_eval_crf_unary: the inputs of stego_eval_probes (lr_scratch [B*h*w][80] floats) -> unary energies
+ *   -log(clip(softmax(probe), 1e-5, 1)) and the initial Q = softmax(-U), both [B*H*W][64] fp32, 16-byte aligned.
+ * stego_eval_crf_norm: NORMALIZE_SYMMETRIC factor norm [N] of a lattice (offset, bary [N][d+1]; CSR rowptr [M+1] and
+ *   slots [N*(d+1)] = pixel*(d+1)+vertex sorted by point; n1 / n2 [d+1][M], -1 = missing); values, values_tmp [M] scratch.
+ * stego_eval_crf_mean_field: n_iter mean-field iterations of B frames of N pixels.  Position lattice (*_g, Mg points):
+ *   one frame's, shared by the B frames.  Bilateral lattice (*_b, Mb points): the frames' lattices concatenated over
+ *   B*N pixels.  Scratch val_g, tmp_g [B*Mg][64], val_b, tmp_b [Mb][64].  Last-iteration outputs, each optional:
+ *   marginals lin_q [B][n_lin][N], clu_q [B][n_clu][N]; argmax maps lin_pred, clu_pred [B][N] uint8 (lowest index on
+ *   ties); with label [B][N] (label_bytes 8 / 4 / 1) the int64 confusion counts lin_conf [n_lin][n_label_classes],
+ *   clu_conf [n_clu][n_label_classes] are incremented at [pred][actual] for every pixel with
+ *   0 <= label < n_label_classes and pred < n_label_classes. */
+STEGO_API int stego_eval_crf_unary(const float* code, const float* code_flip, long long ld_code, int C, int B, int h, int w,
+                                   int H, int W, const float* lin_weight, const float* lin_bias, int n_lin,
+                                   const float* clusters, int n_clu, float alpha, float* lr_scratch, float* unary, float* Q,
+                                   void* stream);
+STEGO_API int stego_eval_crf_norm(int d, long long N, int M, const int* offset, const float* bary, const int* rowptr,
+                                  const int* slots, const int* n1, const int* n2, float* values, float* values_tmp,
+                                  float* norm_out, void* stream);
+STEGO_API int stego_eval_crf_mean_field(int B, long long N, int n_lin, int n_clu, int n_iter, const float* unary, float* Q,
+                                        const int* off_g, const float* bary_g, const int* rowptr_g, const int* slots_g,
+                                        const int* n1_g, const int* n2_g, const float* norm_g, int Mg,
+                                        const int* off_b, const float* bary_b, const int* rowptr_b, const int* slots_b,
+                                        const int* n1_b, const int* n2_b, const float* norm_b, int Mb, float w_g,
+                                        float w_b, float* val_g, float* tmp_g, float* val_b, float* tmp_b, float* lin_q,
+                                        float* clu_q, unsigned char* lin_pred, unsigned char* clu_pred,
+                                        const void* label, int label_bytes, int n_label_classes, long long* lin_conf,
+                                        long long* clu_conf, void* stream);
+
 /* ---- contrastive CRF loss (optional training term; replaces ContrastiveCRFLoss.forward, src/modules.py:449-469, and its
  * autograd backward).  guidance [B, Cg <= 3, H, W] and clusters [B, C <= 80, H, W] are fp32 with arbitrary element strides;
  * coords is the reference's int64 [2][n] tensor (row 0 indexes H, row 1 indexes W; shared by the batch).

@@ -28,7 +28,7 @@ _LD = 32  # floats per pixel / lattice-point row (classes padded to a warp)
 
 class _Lattice:
     """One permutohedral lattice: per-pixel vertex ids + barycentric weights, neighbour tables, symmetric norm."""
-    __slots__ = ("d", "N", "M", "offset", "bary", "n1", "n2", "norm")
+    __slots__ = ("d", "N", "M", "offset", "bary", "n1", "n2", "norm", "rowptr", "slots")
 
 
 def _unpack(keys: torch.Tensor, d: int, bits: int) -> torch.Tensor:
@@ -46,10 +46,10 @@ def _pack(coords: torch.Tensor, d: int, bits: int) -> torch.Tensor:
     return key
 
 
-def _build_lattice(H: int, W: int, d: int, sxy: float, srgb: float, image_u8: Optional[torch.Tensor], dev) -> _Lattice:
-    """Lattice construction, once per image (the position-only lattice is cached per frame size by the caller):
-    the embedding of every pixel is a kernel; de-duplicating the vertex keys and finding the blur neighbours are a sort
-    and binary searches (torch.unique / searchsorted)."""
+def _lattice_points(H: int, W: int, d: int, sxy: float, srgb: float, image_u8: Optional[torch.Tensor], dev) -> _Lattice:
+    """Lattice construction without the normalisation: the embedding of every pixel is a kernel; de-duplicating the
+    vertex keys and finding the blur neighbours are a sort and binary searches (torch.unique / searchsorted).  One host
+    sync, for the number of lattice points."""
     lib = _lib.load()
     N = H * W
     keys = torch.empty(N, d + 1, dtype=torch.long, device=dev)
@@ -76,6 +76,15 @@ def _build_lattice(H: int, W: int, d: int, sxy: float, srgb: float, image_u8: Op
     lat.offset = inv.reshape(N, d + 1).to(torch.int32).contiguous()
     lat.bary = bary
     lat.n1, lat.n2 = n1.contiguous(), n2.contiguous()
+    return lat
+
+
+def _build_lattice(H: int, W: int, d: int, sxy: float, srgb: float, image_u8: Optional[torch.Tensor], dev) -> _Lattice:
+    """Lattice construction, once per image (the position-only lattice is cached per frame size by the caller):
+    `_lattice_points` and the symmetric normalisation."""
+    lib = _lib.load()
+    lat = _lattice_points(H, W, d, sxy, srgb, image_u8, dev)
+    N, M = lat.N, lat.M
     # NORMALIZE_SYMMETRIC: norm = 1 / sqrt(K 1 + 1e-20), K 1 = slice(blur(splat(ones)))
     values = torch.zeros(M + 1, _LD, dtype=torch.float32, device=dev)
     tmp = torch.zeros(M + 1, _LD, dtype=torch.float32, device=dev)
@@ -91,13 +100,18 @@ def _build_lattice(H: int, W: int, d: int, sxy: float, srgb: float, image_u8: Op
 _POSITION_LATTICES: Dict[Tuple[int, int, float, int], _Lattice] = {}
 
 
+_IMAGENET_STATS: Dict[torch.device, Tuple[torch.Tensor, torch.Tensor]] = {}
+
+
 def prepare_image(image_tensor: torch.Tensor) -> torch.Tensor:
     """src/crf.py:23: `np.array(VF.to_pil_image(unnorm(image_tensor)))[:, :, ::-1]` on the device: un-normalise with the
     ImageNet statistics (src/utils.py:140-141), x 255, truncate to uint8, reverse the channel order -> [H, W, 3] uint8.
     (Values outside [0, 255] are clamped; the reference's float->uint8 cast of such values is undefined.)"""
     dev = image_tensor.device
-    mean = torch.tensor([0.485, 0.456, 0.406], device=dev).view(3, 1, 1)
-    std = torch.tensor([0.229, 0.224, 0.225], device=dev).view(3, 1, 1)
+    if dev not in _IMAGENET_STATS:  # built once per device: a tensor from a host list is a synchronising copy
+        _IMAGENET_STATS[dev] = (torch.tensor([0.485, 0.456, 0.406], device=dev).view(3, 1, 1),
+                                torch.tensor([0.229, 0.224, 0.225], device=dev).view(3, 1, 1))
+    mean, std = _IMAGENET_STATS[dev]
     img = (image_tensor.detach().float() * std + mean).mul(255).clamp_(0, 255).to(torch.uint8)
     return img.flip(0).permute(1, 2, 0).contiguous()
 

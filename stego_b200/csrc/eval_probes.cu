@@ -152,6 +152,94 @@ __device__ __forceinline__ double ev_gram(const float* slr, int bw, int py, int 
   return dx == 0 ? e[EV_D] : (dx > 0 ? e[EV_DR] : e[EV_DL]);
 }
 
+// The output tile of CTA blockIdx.x (tile_w x tile_h pixels of image b, tiles row-major per image) and the low-res
+// box [by0, by0 + bh) x [bx0, bx0 + bw) its pixels interpolate from, copied from the preparation table lr into
+// shared memory slr [bh*bw][EV_LD].  Shared by eval_probe_kernel and eval_crf_unary_kernel; the caller synchronises.
+struct EvTile {
+  int b, X0, Y0, by0, bh, bx0, bw;
+  float sy, sx;
+};
+
+__device__ __forceinline__ EvTile ev_tile_load(const float* lr, float* slr, int h, int w, int H, int W, int tile_w,
+                                               int tile_h) {
+  EvTile t;
+  const int tiles_x = (W + tile_w - 1) / tile_w, tiles_y = (H + tile_h - 1) / tile_h;
+  const int tile = blockIdx.x;
+  const int tx = tile % tiles_x, ty = (tile / tiles_x) % tiles_y;
+  t.b = tile / (tiles_x * tiles_y);
+  t.X0 = tx * tile_w;
+  t.Y0 = ty * tile_h;
+  const int Xl = min(t.X0 + tile_w - 1, W - 1), Yl = min(t.Y0 + tile_h - 1, H - 1);
+  t.sy = static_cast<float>(h) / H;
+  t.sx = static_cast<float>(w) / W;
+  src_span(t.Y0, Yl, t.sy, h, t.by0, t.bh);
+  src_span(t.X0, Xl, t.sx, w, t.bx0, t.bw);
+  const long long base = 1ll * t.b * h * w;
+  for (int i = threadIdx.x; i < t.bh * t.bw * EV_LD; i += blockDim.x) {
+    const int cell = i / EV_LD, k = i % EV_LD;
+    const int r = cell / t.bw, c = cell % t.bw;
+    slr[i] = lr[(base + 1ll * (t.by0 + r) * w + t.bx0 + c) * EV_LD + k];
+  }
+  return t;
+}
+
+// The four box-relative corners of output pixel (Y, X) and their bilinear weights
+struct EvCorners {
+  const float *ea, *eb, *ec, *ed;
+  float wa, wb, wc, wd;
+  int y0, y1, x0, x1;
+};
+
+__device__ __forceinline__ EvCorners ev_corners(const float* slr, const EvTile& t, int h, int w, int Y, int X) {
+  EvCorners e;
+  float ly, lx;
+  src_index(Y, t.sy, h, e.y0, e.y1, ly);
+  src_index(X, t.sx, w, e.x0, e.x1, lx);
+  e.y0 -= t.by0; e.y1 -= t.by0; e.x0 -= t.bx0; e.x1 -= t.bx0;
+  e.wa = (1.f - ly) * (1.f - lx); e.wb = (1.f - ly) * lx; e.wc = ly * (1.f - lx); e.wd = ly * lx;
+  e.ea = slr + (e.y0 * t.bw + e.x0) * EV_LD;
+  e.eb = slr + (e.y0 * t.bw + e.x1) * EV_LD;
+  e.ec = slr + (e.y1 * t.bw + e.x0) * EV_LD;
+  e.ed = slr + (e.y1 * t.bw + e.x1) * EV_LD;
+  return e;
+}
+
+// Linear probe: the interpolated logits z[k < n], their maximum and first argmax
+__device__ __forceinline__ void ev_linear(const EvCorners& e, int n, float (&z)[32], float& mx, int& arg) {
+  mx = -INFINITY;
+  arg = 0;
+#pragma unroll
+  for (int k = 0; k < 32; ++k) {
+    if (k < n) {
+      z[k] = e.wa * e.ea[k] + e.wb * e.eb[k] + e.wc * e.ec[k] + e.wd * e.ed[k];
+      if (z[k] > mx) { mx = z[k]; arg = k; }
+    }
+  }
+}
+
+// Cluster probe: cosine similarities z[k < n] of the interpolated code with the normalised centroids, their maximum and
+// first argmax.  The squared norm of the interpolated code comes from the fp32 weights and the fp64 Gram entries,
+// combined in fp64 (their products are exact there).
+__device__ __forceinline__ void ev_cluster(const float* slr, int bw, const EvCorners& e, int n, float (&z)[32],
+                                           float& mx, int& arg) {
+  const double da = e.wa, db = e.wb, dc = e.wc, dd = e.wd;
+  double n2 = da * da * ev_grams(e.ea)[EV_SS] + db * db * ev_grams(e.eb)[EV_SS] + dc * dc * ev_grams(e.ec)[EV_SS] +
+              dd * dd * ev_grams(e.ed)[EV_SS];
+  n2 += 2.0 * (da * db * ev_gram(slr, bw, e.y0, e.x0, e.y0, e.x1) + da * dc * ev_gram(slr, bw, e.y0, e.x0, e.y1, e.x0) +
+               da * dd * ev_gram(slr, bw, e.y0, e.x0, e.y1, e.x1) + db * dc * ev_gram(slr, bw, e.y0, e.x1, e.y1, e.x0) +
+               db * dd * ev_gram(slr, bw, e.y0, e.x1, e.y1, e.x1) + dc * dd * ev_gram(slr, bw, e.y1, e.x0, e.y1, e.x1));
+  const float inv = 1.0f / fmaxf(sqrtf(fmaxf(static_cast<float>(n2), 0.f)), 1e-12f);
+  mx = -INFINITY;
+  arg = 0;
+#pragma unroll
+  for (int k = 0; k < 32; ++k) {
+    if (k < n) {
+      z[k] = (e.wa * e.ea[32 + k] + e.wb * e.eb[32 + k] + e.wc * e.ec[32 + k] + e.wd * e.ed[32 + k]) * inv;
+      if (z[k] > mx) { mx = z[k]; arg = k; }
+    }
+  }
+}
+
 __global__ void __launch_bounds__(EVT_W* EVT_H)
 eval_probe_kernel(EvalProbeParams p) {
   extern __shared__ float slr[];  // [box_h*box_w][EV_LD]
@@ -159,50 +247,22 @@ eval_probe_kernel(EvalProbeParams p) {
   const bool want_conf = p.label != nullptr;
   if (want_conf)
     for (int i = threadIdx.x; i < 2 * 32 * 32; i += blockDim.x) (&hist[0][0])[i] = 0u;
-  const int tiles_x = (p.W + EVT_W - 1) / EVT_W, tiles_y = (p.H + EVT_H - 1) / EVT_H;
-  const int tile = blockIdx.x;
-  const int tx = tile % tiles_x, ty = (tile / tiles_x) % tiles_y, b = tile / (tiles_x * tiles_y);
-  const int X0 = tx * EVT_W, Y0 = ty * EVT_H;
-  const int Xl = min(X0 + EVT_W - 1, p.W - 1), Yl = min(Y0 + EVT_H - 1, p.H - 1);
-  const float sy = static_cast<float>(p.h) / p.H, sx = static_cast<float>(p.w) / p.W;
-  int by0, bh, bx0, bw;
-  src_span(Y0, Yl, sy, p.h, by0, bh);
-  src_span(X0, Xl, sx, p.w, bx0, bw);
-  const long long base = 1ll * b * p.h * p.w;
-  for (int i = threadIdx.x; i < bh * bw * EV_LD; i += blockDim.x) {
-    const int cell = i / EV_LD, k = i % EV_LD;
-    const int r = cell / bw, c = cell % bw;
-    slr[i] = p.lr[(base + 1ll * (by0 + r) * p.w + bx0 + c) * EV_LD + k];
-  }
+  const EvTile t = ev_tile_load(p.lr, slr, p.h, p.w, p.H, p.W, EVT_W, EVT_H);
+  const int b = t.b;
   __syncthreads();
-  const int X = X0 + (threadIdx.x % EVT_W), Y = Y0 + (threadIdx.x / EVT_W);
+  const int X = t.X0 + (threadIdx.x % EVT_W), Y = t.Y0 + (threadIdx.x / EVT_W);
   const bool active = X < p.W && Y < p.H;
   int lin_pred = -1, clu_pred = -1;
   if (active) {
-    int y0, y1, x0, x1;
-    float ly, lx;
-    src_index(Y, sy, p.h, y0, y1, ly);
-    src_index(X, sx, p.w, x0, x1, lx);
-    y0 -= by0; y1 -= by0; x0 -= bx0; x1 -= bx0;
-    const float wa = (1.f - ly) * (1.f - lx), wb = (1.f - ly) * lx, wc = ly * (1.f - lx), wd = ly * lx;
-    const float* ea = slr + (y0 * bw + x0) * EV_LD;
-    const float* eb = slr + (y0 * bw + x1) * EV_LD;
-    const float* ec = slr + (y1 * bw + x0) * EV_LD;
-    const float* ed = slr + (y1 * bw + x1) * EV_LD;
+    const EvCorners e = ev_corners(slr, t, p.h, p.w, Y, X);
     const long long plane = 1ll * p.H * p.W;
     const long long pix = 1ll * Y * p.W + X;
     // ---- linear probe: log_softmax of the interpolated logits
     if (p.lin_logp || p.lin_arg) {
       float z[32];
-      float mx = -INFINITY;
-      int arg = 0;
-#pragma unroll
-      for (int k = 0; k < 32; ++k) {
-        if (k < p.n_lin) {
-          z[k] = wa * ea[k] + wb * eb[k] + wc * ec[k] + wd * ed[k];
-          if (z[k] > mx) { mx = z[k]; arg = k; }
-        }
-      }
+      float mx;
+      int arg;
+      ev_linear(e, p.n_lin, z, mx, arg);
       lin_pred = arg;
       if (p.lin_arg) p.lin_arg[b * plane + pix] = static_cast<unsigned char>(arg);
       if (p.lin_logp) {
@@ -219,24 +279,10 @@ eval_probe_kernel(EvalProbeParams p) {
     }
     // ---- cluster probe: cosine similarity of the interpolated code with the centroids, log_softmax(alpha * .)
     if (p.clu_logp || p.clu_arg) {
-      // the fp32 weights of the dots, combined in fp64 (their products are exact there)
-      const double da = wa, db = wb, dc = wc, dd = wd;
-      double n2 = da * da * ev_grams(ea)[EV_SS] + db * db * ev_grams(eb)[EV_SS] + dc * dc * ev_grams(ec)[EV_SS] +
-                  dd * dd * ev_grams(ed)[EV_SS];
-      n2 += 2.0 * (da * db * ev_gram(slr, bw, y0, x0, y0, x1) + da * dc * ev_gram(slr, bw, y0, x0, y1, x0) +
-                   da * dd * ev_gram(slr, bw, y0, x0, y1, x1) + db * dc * ev_gram(slr, bw, y0, x1, y1, x0) +
-                   db * dd * ev_gram(slr, bw, y0, x1, y1, x1) + dc * dd * ev_gram(slr, bw, y1, x0, y1, x1));
-      const float inv = 1.0f / fmaxf(sqrtf(fmaxf(static_cast<float>(n2), 0.f)), 1e-12f);
       float z[32];
-      float mx = -INFINITY;
-      int arg = 0;
-#pragma unroll
-      for (int k = 0; k < 32; ++k) {
-        if (k < p.n_clu) {
-          z[k] = (wa * ea[32 + k] + wb * eb[32 + k] + wc * ec[32 + k] + wd * ed[32 + k]) * inv;
-          if (z[k] > mx) { mx = z[k]; arg = k; }
-        }
-      }
+      float mx;
+      int arg;
+      ev_cluster(slr, t.bw, e, p.n_clu, z, mx, arg);
       clu_pred = arg;
       if (p.clu_arg) p.clu_arg[b * plane + pix] = static_cast<unsigned char>(arg);
       if (p.clu_logp) {
@@ -262,6 +308,81 @@ eval_probe_kernel(EvalProbeParams p) {
                     lin_pred, clu_pred);
     conf_hist_flush(hist, p.lin_conf, p.clu_conf, p.n_lin, p.n_clu, p.n_cls);
   }
+}
+
+// ---- dense-CRF unaries straight from the preparation table (stego_eval_crf_unary) -------------------------------------
+// The CRF-refined evaluation (src/eval_segmentation.py:133-135 -> src/crf.py:22-45) runs the dense CRF on each probe's
+// log-probabilities.  This kernel evaluates both probes per output pixel exactly as eval_probe_kernel does and writes,
+// instead of the [B,n,H,W] log-probability planes, one 64-float row per pixel of the CRF's unary table
+// U = -log(clip(softmax, 1e-5, 1)) (pydensecrf.utils.unary_from_softmax) and one of the initial Q = softmax(-U)
+// (densecrf.cpp inference): linear probe in [0, 32), cluster probe in [32, 64), zeros beyond each probe's class count.
+constexpr int EVC_LD = 64;
+
+// One probe's unary and initial-Q half rows from its scores s[k < n] (softmax(s) = the probe's probabilities)
+__device__ __forceinline__ void ev_crf_half_rows(const float (&s)[32], int n, float* u_row, float* q_row) {
+  float mx = -INFINITY;
+#pragma unroll
+  for (int k = 0; k < 32; ++k)
+    if (k < n) mx = fmaxf(mx, s[k]);
+  float se = 0.f;
+#pragma unroll
+  for (int k = 0; k < 32; ++k)
+    if (k < n) se += __expf(s[k] - mx);
+  float u[32];
+  float m2 = -INFINITY;
+#pragma unroll
+  for (int k = 0; k < 32; ++k) {
+    u[k] = 0.f;
+    if (k < n) {
+      u[k] = -__logf(fminf(fmaxf(__expf(s[k] - mx) / se, 1e-5f), 1.0f));
+      m2 = fmaxf(m2, -u[k]);
+    }
+  }
+  float s2 = 0.f;
+#pragma unroll
+  for (int k = 0; k < 32; ++k)
+    if (k < n) s2 += __expf(-u[k] - m2);
+#pragma unroll
+  for (int k = 0; k < 32; k += 4) {
+    float4 uv, qv;
+    uv.x = u[k]; uv.y = u[k + 1]; uv.z = u[k + 2]; uv.w = u[k + 3];
+    qv.x = (k < n) ? __expf(-u[k] - m2) / s2 : 0.f;
+    qv.y = (k + 1 < n) ? __expf(-u[k + 1] - m2) / s2 : 0.f;
+    qv.z = (k + 2 < n) ? __expf(-u[k + 2] - m2) / s2 : 0.f;
+    qv.w = (k + 3 < n) ? __expf(-u[k + 3] - m2) / s2 : 0.f;
+    *reinterpret_cast<float4*>(u_row + k) = uv;
+    *reinterpret_cast<float4*>(q_row + k) = qv;
+  }
+}
+
+struct EvalCrfUnaryParams {
+  const float* lr;  // [B*h*w][EV_LD]
+  int B, h, w, H, W, n_lin, n_clu;
+  float alpha;
+  float* unary;     // [B*H*W][EVC_LD]
+  float* Q;         // [B*H*W][EVC_LD]
+};
+
+__global__ void __launch_bounds__(EVT_W* EVT_H)
+eval_crf_unary_kernel(EvalCrfUnaryParams p) {
+  extern __shared__ float slr[];  // [box_h*box_w][EV_LD]
+  const EvTile t = ev_tile_load(p.lr, slr, p.h, p.w, p.H, p.W, EVT_W, EVT_H);
+  __syncthreads();
+  const int X = t.X0 + (threadIdx.x % EVT_W), Y = t.Y0 + (threadIdx.x / EVT_W);
+  if (X >= p.W || Y >= p.H) return;
+  const EvCorners e = ev_corners(slr, t, p.h, p.w, Y, X);
+  const long long row = (1ll * t.b * p.H + Y) * p.W + X;
+  float* u_row = p.unary + row * EVC_LD;
+  float* q_row = p.Q + row * EVC_LD;
+  float z[32];
+  float mx;
+  int arg;
+  ev_linear(e, p.n_lin, z, mx, arg);
+  ev_crf_half_rows(z, p.n_lin, u_row, q_row);
+  ev_cluster(slr, t.bw, e, p.n_clu, z, mx, arg);
+#pragma unroll
+  for (int k = 0; k < 32; ++k) z[k] *= p.alpha;
+  ev_crf_half_rows(z, p.n_clu, u_row + 32, q_row + 32);
 }
 
 
@@ -426,6 +547,21 @@ eval_probe_vec4_kernel(EvalProbeParams p) {
 
 using namespace stego;
 
+// eval_prep_kernel over the B*h*w low-res pixels (arguments checked by the caller)
+static int launch_eval_prep(const float* code, const float* code_flip, long long ld_code, int C, int B, int h, int w,
+                            const float* lin_weight, const float* lin_bias, int n_lin, const float* clusters, int n_clu,
+                            float* lr_scratch, cudaStream_t stream) {
+  EvalPrepParams q;
+  q.code = code; q.code_flip = code_flip; q.ld = ld_code; q.B = B; q.h = h; q.w = w; q.C = C; q.W = lin_weight; q.bias = lin_bias;
+  q.n_lin = n_lin; q.clusters = clusters; q.n_clu = n_clu; q.lr = lr_scratch;
+  const long long rows = 1ll * B * h * w;
+  long long g = (rows + 7) / 8;
+  const long long cap = 16ll * num_sms();
+  eval_prep_kernel<<<(unsigned)(g < cap ? g : cap), 256, (size_t)C * 64 * sizeof(float), stream>>>(q);
+  STEGO_CHECK_LAUNCH("eval_prep_kernel");
+  return STEGO_OK;
+}
+
 // code: tokens-major low-res code [B*h*w][ld_code] fp32 (what DinoFeaturizer produces); outputs at [H][W].
 // code_flip: the code of the horizontally flipped images (flip-TTA) or null.  lr_scratch: [B*h*w][80] floats, 16-byte aligned.
 // label + confusion outputs (int64, accumulated): optional.  Any output pointer may be null.
@@ -444,14 +580,10 @@ extern "C" int stego_eval_probes(const float* code, const float* code_flip, long
   STEGO_CHECK_ARG(!label || ((label_bytes == 8 || label_bytes == 4 || label_bytes == 1) && n_label_classes > 0 &&
                              n_label_classes <= 32 && (lin_confusion || clu_confusion)),
                   "stego_eval_probes: confusion counts need label_bytes in {8,4,1}, n_label_classes <= 32 and an output");
-  EvalPrepParams q;
-  q.code = code; q.code_flip = code_flip; q.ld = ld_code; q.B = B; q.h = h; q.w = w; q.C = C; q.W = lin_weight; q.bias = lin_bias;
-  q.n_lin = n_lin; q.clusters = clusters; q.n_clu = n_clu; q.lr = lr_scratch;
-  const long long rows = 1ll * B * h * w;
-  long long g = (rows + 7) / 8;
-  const long long cap = 16ll * num_sms();
-  eval_prep_kernel<<<(unsigned)(g < cap ? g : cap), 256, (size_t)C * 64 * sizeof(float), stream>>>(q);
-  STEGO_CHECK_LAUNCH("eval_prep_kernel");
+  int rc;
+  if ((rc = launch_eval_prep(code, code_flip, ld_code, C, B, h, w, lin_weight, lin_bias, n_lin, clusters, n_clu,
+                             lr_scratch, stream)) != STEGO_OK)
+    return rc;
   EvalProbeParams p;
   p.lr = lr_scratch; p.B = B; p.h = h; p.w = w; p.H = H; p.W = W; p.n_lin = n_lin; p.n_clu = n_clu; p.alpha = alpha;
   p.lin_logp = lin_log_probs; p.clu_logp = clu_log_probs; p.lin_arg = lin_argmax; p.clu_arg = clu_argmax;
@@ -473,7 +605,6 @@ extern "C" int stego_eval_probes(const float* code, const float* code_flip, long
   STEGO_CHECK_ARG(smem <= 200 * 1024, "stego_eval_probes: upsample ratio needs %zu B of shared memory", smem);
   const long long tiles = 1ll * B * ((H + tile_h - 1) / tile_h) * ((W + tile_w - 1) / tile_w);
   STEGO_CHECK_ARG(tiles < (1ll << 31), "stego_eval_probes: too many tiles");
-  int rc;
   if (vec4) {
     if ((rc = opt_in_smem<eval_probe_vec4_kernel<27, 27>>(smem, "eval_probe_vec4_kernel")) != STEGO_OK) return rc;
     eval_probe_vec4_kernel<27, 27><<<(unsigned)tiles, EV4_TW * EV4_ROWS, smem, stream>>>(p);
@@ -483,5 +614,37 @@ extern "C" int stego_eval_probes(const float* code, const float* code_flip, long
   if ((rc = opt_in_smem<eval_probe_kernel>(smem, "eval_probe_kernel")) != STEGO_OK) return rc;
   eval_probe_kernel<<<(unsigned)tiles, EVT_W * EVT_H, smem, stream>>>(p);
   STEGO_CHECK_LAUNCH("eval_probe_kernel");
+  return STEGO_OK;
+}
+
+// The dense-CRF unaries of both probes at [H][W] (see eval_crf_unary_kernel): the same inputs as stego_eval_probes;
+// unary and Q: [B*H*W][64] fp32, 16-byte aligned (linear probe in floats [0, 32), cluster probe in [32, 64)).
+extern "C" int stego_eval_crf_unary(const float* code, const float* code_flip, long long ld_code, int C, int B, int h, int w,
+                                    int H, int W, const float* lin_weight, const float* lin_bias, int n_lin,
+                                    const float* clusters, int n_clu, float alpha, float* lr_scratch, float* unary, float* Q,
+                                    void* stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  STEGO_CHECK_ARG(code && lin_weight && lin_bias && clusters && lr_scratch && unary && Q, "stego_eval_crf_unary: null pointer");
+  STEGO_CHECK_ARG((reinterpret_cast<uintptr_t>(lr_scratch) & 7u) == 0 && (reinterpret_cast<uintptr_t>(unary) & 15u) == 0 &&
+                  (reinterpret_cast<uintptr_t>(Q) & 15u) == 0,
+                  "stego_eval_crf_unary: lr_scratch must be 8-byte aligned, unary and Q 16-byte aligned");
+  STEGO_CHECK_ARG(C > 0 && C <= 96 && n_lin > 0 && n_lin <= 32 && n_clu > 0 && n_clu <= 32,
+                  "stego_eval_crf_unary: C=%d n_lin=%d n_clu=%d unsupported (C <= 96, classes <= 32)", C, n_lin, n_clu);
+  STEGO_CHECK_ARG(B > 0 && h > 0 && w > 0 && H >= h && W >= w, "stego_eval_crf_unary: bad sizes (upsampling only)");
+  const int box_h = src_span_max(EVT_H, h, H), box_w = src_span_max(EVT_W, w, W);
+  const size_t smem = (size_t)box_h * box_w * EV_LD * sizeof(float);
+  STEGO_CHECK_ARG(smem <= 200 * 1024, "stego_eval_crf_unary: upsample ratio needs %zu B of shared memory", smem);
+  const long long tiles = 1ll * B * ((H + EVT_H - 1) / EVT_H) * ((W + EVT_W - 1) / EVT_W);
+  STEGO_CHECK_ARG(tiles < (1ll << 31), "stego_eval_crf_unary: too many tiles");
+  int rc;
+  if ((rc = launch_eval_prep(code, code_flip, ld_code, C, B, h, w, lin_weight, lin_bias, n_lin, clusters, n_clu,
+                             lr_scratch, stream)) != STEGO_OK)
+    return rc;
+  if ((rc = opt_in_smem<eval_crf_unary_kernel>(smem, "eval_crf_unary_kernel")) != STEGO_OK) return rc;
+  EvalCrfUnaryParams p;
+  p.lr = lr_scratch; p.B = B; p.h = h; p.w = w; p.H = H; p.W = W; p.n_lin = n_lin; p.n_clu = n_clu; p.alpha = alpha;
+  p.unary = unary; p.Q = Q;
+  eval_crf_unary_kernel<<<(unsigned)tiles, EVT_W * EVT_H, smem, stream>>>(p);
+  STEGO_CHECK_LAUNCH("eval_crf_unary_kernel");
   return STEGO_OK;
 }

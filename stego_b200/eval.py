@@ -8,14 +8,17 @@ materialising the upsampled code.
 becomes `fused_probe_log_probs(code_lowres, model.linear_probe, model.cluster_probe, label.shape[-2:], 2)`.
 At 1024x2048 the reference moves 587 MB (fp32 upsampled code) per image per probe before it even starts;
 the fused kernel reads the 9 MB low-res code and writes only the outputs (stego_eval_probes, eval_probes.cu).
+
+With `run_crf=True` the reference then runs the dense CRF on each probe's log-probabilities of every frame
+(eval_segmentation.py:133-141); `fused_eval_crf` is that whole loop body as one batched call (eval_crf.cu).
 """
 from __future__ import annotations
 
-from typing import Optional, Sequence, Tuple
+from typing import Dict, Optional, Sequence, Tuple
 
 import torch
 
-from . import _lib, ops
+from . import _lib, crf, ops
 
 
 def fused_probe_log_probs(code: torch.Tensor, linear_probe: torch.nn.Module, cluster_probe: torch.nn.Module,
@@ -35,19 +38,10 @@ def fused_probe_log_probs(code: torch.Tensor, linear_probe: torch.nn.Module, clu
         raise RuntimeError("stego_b200.eval: CUDA tensors required (no CPU fallback)")
     B, C, h, w = code.shape
     H, W = int(size[0]), int(size[1])
-    x = ops.tokens_major(code)
-    ld = x.stride(3)
-    xf = None
     if code_flipped is not None:
         assert code_flipped.shape == code.shape
-        xf = ops.tokens_major(code_flipped)
-        if xf.stride(3) != ld:  # one ld for both codes
-            xf = xf.permute(0, 2, 3, 1).contiguous().permute(0, 3, 1, 2)
-            x = x.permute(0, 2, 3, 1).contiguous().permute(0, 3, 1, 2)
-            ld = x.stride(3)
-    wl = linear_probe.weight.detach().float().reshape(linear_probe.weight.shape[0], C).contiguous()
-    bl = linear_probe.bias.detach().float().contiguous()
-    cl = cluster_probe.clusters.detach().float().contiguous()
+    x, xf, ld = _probe_codes(code, code_flipped)
+    wl, bl, cl = _probe_tables(linear_probe, cluster_probe, C)
     n_lin, n_clu = wl.shape[0], cl.shape[0]
     dev = code.device
     scratch = torch.empty(B * h * w, 80, dtype=torch.float32, device=dev)  # eval_probes.cu EV_LD
@@ -73,6 +67,204 @@ def fused_probe_log_probs(code: torch.Tensor, linear_probe: torch.nn.Module, clu
     if want_argmax:
         return lin, clu, la, ca
     return lin, clu
+
+
+def _probe_codes(code: torch.Tensor, code_flipped: Optional[torch.Tensor]):
+    """(x, xf, ld): the code and the flipped image's code (or None) as tokens-major fp32 views with one row stride ld."""
+    x = ops.tokens_major(code)
+    ld = x.stride(3)
+    xf = None
+    if code_flipped is not None:
+        xf = ops.tokens_major(code_flipped)
+        if xf.stride(3) != ld:  # one ld for both codes
+            xf = xf.permute(0, 2, 3, 1).contiguous().permute(0, 3, 1, 2)
+            x = x.permute(0, 2, 3, 1).contiguous().permute(0, 3, 1, 2)
+            ld = x.stride(3)
+    return x, xf, ld
+
+
+def _probe_tables(linear_probe: torch.nn.Module, cluster_probe: torch.nn.Module, C: int):
+    """(weight [n_lin, C], bias [n_lin], clusters [n_clu, C]) as contiguous fp32."""
+    wl = linear_probe.weight.detach().float().reshape(linear_probe.weight.shape[0], C).contiguous()
+    bl = linear_probe.bias.detach().float().contiguous()
+    cl = cluster_probe.clusters.detach().float().contiguous()
+    return wl, bl, cl
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# CRF-refined evaluation
+# ----------------------------------------------------------------------------------------------------------------------
+_CRF_LD = 64  # eval_crf.cu: floats per pixel / lattice-point row (linear probe in [0, 32), cluster probe in [32, 64))
+_GATHER_POSITION_LATTICES: Dict[Tuple[int, int, int], "crf._Lattice"] = {}
+
+
+def _csr(lat) -> None:
+    """The (pixel, vertex) slots of every lattice point as a CSR list: `slots` sorted by point, ascending slot index
+    within a point (a stable sort of the point ids), and `rowptr` [M + 1]."""
+    ids = lat.offset.reshape(-1)
+    order = torch.argsort(ids, stable=True)
+    lat.slots = order.to(torch.int32)
+    lat.rowptr = torch.searchsorted(ids[order], torch.arange(lat.M + 1, dtype=torch.int32, device=ids.device)) \
+        .to(torch.int32)
+
+
+def _gather_norm(lat) -> None:
+    """lat.norm by stego_eval_crf_norm: the symmetric normalisation with gather splats (no float atomics)."""
+    dev = lat.offset.device
+    values = torch.empty(lat.M, dtype=torch.float32, device=dev)
+    tmp = torch.empty(lat.M, dtype=torch.float32, device=dev)
+    lat.norm = torch.empty(lat.N, dtype=torch.float32, device=dev)
+    _lib.check(_lib.load().stego_eval_crf_norm(lat.d, lat.N, lat.M, _lib.ptr(lat.offset), _lib.ptr(lat.bary),
+                                               _lib.ptr(lat.rowptr), _lib.ptr(lat.slots), _lib.ptr(lat.n1),
+                                               _lib.ptr(lat.n2), _lib.ptr(values), _lib.ptr(tmp), _lib.ptr(lat.norm),
+                                               _lib.stream()), "stego_eval_crf_norm")
+
+
+def _position_lattice(H: int, W: int, dev):
+    """The Gaussian kernel's lattice of an H x W frame with its CSR list and gather normalisation, cached per frame
+    size: it depends on pixel positions only, so every frame of every batch of that size shares it."""
+    key = (H, W, dev.index)
+    if key not in _GATHER_POSITION_LATTICES:
+        lat = crf._lattice_points(H, W, 2, crf.POS_XY_STD, 0.0, None, dev)
+        _csr(lat)
+        _gather_norm(lat)
+        _GATHER_POSITION_LATTICES[key] = lat
+    return _GATHER_POSITION_LATTICES[key]
+
+
+def _bilateral_lattice(img: torch.Tensor):
+    """The bilateral lattices of the B frames of img [B, 3, H, W], concatenated into one lattice over the B*H*W pixels
+    (point ids, neighbour tables and slots offset by each frame's base), with its gather normalisation.  One host sync
+    per frame (the number of lattice points)."""
+    B, _, H, W = img.shape
+    dev = img.device
+    N = H * W
+    frames = []
+    for b in range(B):
+        lat = crf._lattice_points(H, W, 5, crf.Bi_XY_STD, crf.Bi_RGB_STD, crf.prepare_image(img[b]), dev)
+        _csr(lat)
+        frames.append(lat)
+    if B == 1:
+        out = frames[0]
+    else:
+        bases, m = [], 0
+        for lat in frames:
+            bases.append(m)
+            m += lat.M
+        out = crf._Lattice()
+        out.d, out.N, out.M = 5, B * N, m
+        out.offset = torch.cat([lat.offset + base for lat, base in zip(frames, bases)])
+        out.bary = torch.cat([lat.bary for lat in frames])
+        out.n1, out.n2 = (torch.cat([torch.where(t >= 0, t + base, t) for t, base in zip(ts, bases)], 1).contiguous()
+                          for ts in ([lat.n1 for lat in frames], [lat.n2 for lat in frames]))
+        slots_per_frame = N * 6
+        out.slots = torch.cat([lat.slots + b * slots_per_frame for b, lat in enumerate(frames)])
+        out.rowptr = torch.cat([lat.rowptr[:-1] + b * slots_per_frame for b, lat in enumerate(frames)] +
+                               [torch.full((1,), B * slots_per_frame, dtype=torch.int32, device=dev)])
+    _gather_norm(out)
+    return out
+
+
+_LABEL_DTYPES = (torch.uint8, torch.int32, torch.int64)
+
+
+def _check_crf_args(code, linear_probe, cluster_probe, img, code_flipped, label, linear_confusion, cluster_confusion):
+    """Every argument of fused_eval_crf checked before anything is launched: shapes, dtypes and limits first (ValueError),
+    then the device (RuntimeError: CUDA tensors only).  Returns (B, C, h, w, H, W, n_lin, n_clu)."""
+    if code.dim() != 4 or img.dim() != 4 or img.shape[1] != 3 or img.shape[0] != code.shape[0]:
+        raise ValueError(f"fused_eval_crf: code [B, C, h, w] and img [B, 3, H, W] expected, got {tuple(code.shape)} and "
+                         f"{tuple(img.shape)}")
+    B, C, h, w = code.shape
+    H, W = int(img.shape[2]), int(img.shape[3])
+    n_lin, n_clu = int(linear_probe.weight.shape[0]), int(cluster_probe.clusters.shape[0])
+    if not (0 < C <= 96 and 0 < n_lin <= 32 and 0 < n_clu <= 32):
+        raise ValueError(f"fused_eval_crf: C={C}, n_lin={n_lin}, n_clu={n_clu} unsupported (C <= 96, classes <= 32)")
+    if linear_probe.weight[0].numel() != C or cluster_probe.clusters.shape[1] != C:
+        raise ValueError(f"fused_eval_crf: probes of {linear_probe.weight[0].numel()} / {cluster_probe.clusters.shape[1]} "
+                         f"channels for a code of {C}")
+    if H < h or W < w:
+        raise ValueError(f"fused_eval_crf: img {H}x{W} is smaller than the code {h}x{w} (upsampling only)")
+    if code_flipped is not None and code_flipped.shape != code.shape:
+        raise ValueError(f"fused_eval_crf: code_flipped {tuple(code_flipped.shape)} != code {tuple(code.shape)}")
+    if label is not None:
+        if tuple(label.shape[-2:]) != (H, W) or label.numel() != B * H * W:
+            raise ValueError(f"fused_eval_crf: label {tuple(label.shape)} does not match img {B}x{H}x{W}")
+        if label.dtype not in _LABEL_DTYPES:
+            raise ValueError(f"fused_eval_crf: label dtype {label.dtype} unsupported (uint8, int32 or int64)")
+        if linear_confusion is None and cluster_confusion is None:
+            raise ValueError("fused_eval_crf: label given without a confusion matrix to accumulate into")
+    elif linear_confusion is not None or cluster_confusion is not None:
+        raise ValueError("fused_eval_crf: confusion matrices given without a label")
+    for t, n, name in ((linear_confusion, n_lin, "linear_confusion"), (cluster_confusion, n_clu, "cluster_confusion")):
+        if t is not None and (t.dtype != torch.int64 or not t.is_contiguous() or tuple(t.shape) != (n, n_lin)):
+            raise ValueError(f"fused_eval_crf: {name} must be a contiguous int64 [{n}, {n_lin}] tensor, got "
+                             f"{t.dtype} {tuple(t.shape)}")
+    _lib.require_cuda(code, img, code_flipped, label, linear_confusion, cluster_confusion, linear_probe.weight,
+                      linear_probe.bias, cluster_probe.clusters)
+    return B, C, h, w, H, W, n_lin, n_clu
+
+
+def fused_eval_crf(code: torch.Tensor, linear_probe: torch.nn.Module, cluster_probe: torch.nn.Module, img: torch.Tensor,
+                   alpha: float = 2.0, code_flipped: Optional[torch.Tensor] = None, label: Optional[torch.Tensor] = None,
+                   linear_confusion: Optional[torch.Tensor] = None, cluster_confusion: Optional[torch.Tensor] = None,
+                   want_marginals: bool = False):
+    """The reference's CRF-refined eval step (eval_segmentation.py:124-141 with run_crf=True) as one batched call:
+
+        code = (code + code_flipped.flip(3)) / 2                  # when code_flipped is given (flip-TTA)
+        code = F.interpolate(code, img.shape[-2:], mode='bilinear', align_corners=False)
+        linear_probs  = torch.log_softmax(linear_probe(code), dim=1)
+        cluster_probs = cluster_probe(code, alpha, log_probs=True)
+        lin_pred = stack([dense_crf(img[b], linear_probs[b])  for b]).argmax(1)      # src/crf.py:22-45
+        clu_pred = stack([dense_crf(img[b], cluster_probs[b]) for b]).argmax(1)
+        linear_metrics.update(lin_pred, label); cluster_metrics.update(clu_pred, label)
+
+    code: low-res [B, C, h, w] (C <= 96, any strides); img: the normalised frames [B, 3, H, W]; both CUDA.  Returns
+    (lin_pred, clu_pred) uint8 [B, H, W], the argmax of each probe's CRF marginals (lowest index on ties), and with
+    want_marginals also (lin_Q [B, n_lin, H, W], clu_Q [B, n_clu, H, W]) fp32.  label [B, H, W] (uint8 with 255 =
+    ignore, int32 or int64; the spatial size of img) with int64 `linear_confusion [n_lin, n_lin]` /
+    `cluster_confusion [n_clu, n_lin]` (e.g. UnsupervisedMetrics.stats), accumulated in place: a pixel counts when
+    0 <= label < n_lin and pred < n_lin (utils.py:219-229).  n_lin, n_clu <= 32 (extra clusters included).
+
+    The log-probability maps are never written: the CRF unaries come straight from the low-res probe table.  Both probes
+    share one bilateral lattice per frame, all frames run through each stage in one launch, and the splats are gathers
+    in a fixed order, so two calls are bit-identical and a frame's results do not depend on the rest of the batch.
+    The dense CRF itself is the one of stego_b200.crf (parameters of src/crf.py:13-19, 10 mean-field iterations).
+    Host syncs: one per frame (the bilateral lattice's size from torch.unique), plus one the first time a frame size is
+    seen (its cached position lattice).  Everything is checked before the first launch."""
+    B, C, h, w, H, W, n_lin, n_clu = _check_crf_args(code, linear_probe, cluster_probe, img, code_flipped, label,
+                                                      linear_confusion, cluster_confusion)
+    lib = _lib.load()
+    dev = code.device
+    N = H * W
+    x, xf, ld = _probe_codes(code, code_flipped)
+    wl, bl, cl = _probe_tables(linear_probe, cluster_probe, C)
+    scratch = torch.empty(B * h * w, 80, dtype=torch.float32, device=dev)  # eval_probes.cu EV_LD
+    unary = torch.empty(B * N, _CRF_LD, dtype=torch.float32, device=dev)
+    Q = torch.empty(B * N, _CRF_LD, dtype=torch.float32, device=dev)
+    _lib.check(lib.stego_eval_crf_unary(_lib.ptr(x), _lib.ptr(xf), ld, C, B, h, w, H, W, _lib.ptr(wl), _lib.ptr(bl), n_lin,
+                                        _lib.ptr(cl), n_clu, float(alpha), _lib.ptr(scratch), _lib.ptr(unary), _lib.ptr(Q),
+                                        _lib.stream()), "stego_eval_crf_unary")
+    lg = _position_lattice(H, W, dev)
+    lb = _bilateral_lattice(img.detach())
+    val_g = torch.empty(2, B * lg.M, _CRF_LD, dtype=torch.float32, device=dev)
+    val_b = torch.empty(2, lb.M, _CRF_LD, dtype=torch.float32, device=dev)
+    lin_pred = torch.empty(B, H, W, dtype=torch.uint8, device=dev)
+    clu_pred = torch.empty(B, H, W, dtype=torch.uint8, device=dev)
+    lin_q = torch.empty(B, n_lin, H, W, dtype=torch.float32, device=dev) if want_marginals else None
+    clu_q = torch.empty(B, n_clu, H, W, dtype=torch.float32, device=dev) if want_marginals else None
+    lab, lab_bytes = (None, 0) if label is None else ops.probe_label(label, B, H, W)
+    _lib.check(lib.stego_eval_crf_mean_field(
+        B, N, n_lin, n_clu, crf.MAX_ITER, _lib.ptr(unary), _lib.ptr(Q),
+        _lib.ptr(lg.offset), _lib.ptr(lg.bary), _lib.ptr(lg.rowptr), _lib.ptr(lg.slots), _lib.ptr(lg.n1), _lib.ptr(lg.n2),
+        _lib.ptr(lg.norm), lg.M,
+        _lib.ptr(lb.offset), _lib.ptr(lb.bary), _lib.ptr(lb.rowptr), _lib.ptr(lb.slots), _lib.ptr(lb.n1), _lib.ptr(lb.n2),
+        _lib.ptr(lb.norm), lb.M, float(crf.POS_W), float(crf.Bi_W),
+        _lib.ptr(val_g[0]), _lib.ptr(val_g[1]), _lib.ptr(val_b[0]), _lib.ptr(val_b[1]), _lib.ptr(lin_q), _lib.ptr(clu_q),
+        _lib.ptr(lin_pred), _lib.ptr(clu_pred), _lib.ptr(lab), lab_bytes, n_lin if label is not None else 0,
+        _lib.ptr(linear_confusion), _lib.ptr(cluster_confusion), _lib.stream()), "stego_eval_crf_mean_field")
+    if want_marginals:
+        return lin_pred, clu_pred, lin_q, clu_q
+    return lin_pred, clu_pred
 
 
 class UnsupervisedMetrics:
