@@ -217,9 +217,11 @@ STEGO_API int stego_relu_bwd_bf16(const float* dh, const void* h_bf16, void* out
 /* Bias gradients: out[C] += column sums of in [rows][ld] (fp32 or bf16). */
 STEGO_API int stego_colsum(const void* in, int in_is_bf16, int ld, int C, long long rows, float* out, void* stream);
 /* torch.optim.Adam step (src/train_segmentation.py:379-381; amsgrad off, weight_decay 0) on a flat fp32 buffer;
- * `step` is 1-based; grad is multiplied by grad_scale first (1/world_size after a sum-allreduce). */
+ * `step` is 1-based; grad is multiplied by grad_scale first (1/world_size after a sum-allreduce).  The coefficients
+ * 1 - beta1, 1 - beta2, lr / (1 - beta1^step) and sqrt(1 - beta2^step) are formed in double from the double
+ * hyper-parameters and rounded to fp32 once each. */
 STEGO_API int stego_adam_step(float* param, const float* grad, float* exp_avg, float* exp_avg_sq, long long n,
-                              float lr, float beta1, float beta2, float eps, int step, float grad_scale,
+                              double lr, double beta1, double beta2, double eps, int step, float grad_scale,
                               void* stream);
 
 /* The scalar arithmetic at the end of training_step (src/train_segmentation.py:196-201, 219-225) in one launch:

@@ -22,6 +22,7 @@ replayed_launches = 0  # kernels launched through CUDA-graph replays (not seen b
 _CTYPES = {
     "int": ctypes.c_int,
     "float": ctypes.c_float,
+    "double": ctypes.c_double,
     "long long": ctypes.c_longlong,
     "void*": ctypes.c_void_p,
     "const void*": ctypes.c_void_p,

@@ -328,4 +328,36 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
   return *reinterpret_cast<uint32_t*>(&v);
 }
 
+// ----------------------------------------------------------------------------------------------
+// torch.optim.Adam (amsgrad=False, weight_decay=0, maximize=False), shared by adam_kernel (head.cu) and
+// p2p_adam_kernel (p2p_update.cu) so that the two updates are bit-identical.
+// ----------------------------------------------------------------------------------------------
+// The step's coefficients, formed in double from the optimiser's (double) hyper-parameters and rounded to fp32 once
+// each: 1 - beta taken from the rounded beta would be 216 u too small for beta2 = 0.999 (fp32(0.999) = 0.99900001).
+struct AdamCoef {
+  float b1, c1, b2, c2;  // beta1, 1 - beta1, beta2, 1 - beta2
+  float step_size;       // lr / (1 - beta1^step)
+  float sqrt_bc2;        // sqrt(1 - beta2^step)
+  float eps;
+};
+inline AdamCoef adam_coef(double lr, double beta1, double beta2, double eps, double step) {
+  AdamCoef c;
+  c.b1 = static_cast<float>(beta1);
+  c.c1 = static_cast<float>(1.0 - beta1);
+  c.b2 = static_cast<float>(beta2);
+  c.c2 = static_cast<float>(1.0 - beta2);
+  c.step_size = static_cast<float>(lr / (1.0 - pow(beta1, step)));
+  c.sqrt_bc2 = static_cast<float>(sqrt(1.0 - pow(beta2, step)));
+  c.eps = static_cast<float>(eps);
+  return c;
+}
+// One element, every rounding spelled out (no contraction left to the compiler):
+//   m = fma(1-b1, g, m b1);  v = fma((1-b2) g, g, v b2);  p = fma(-step_size, m / (sqrt(v) / sqrt_bc2 + eps), p)
+__device__ __forceinline__ void adam_elem(float& p, float& m, float& v, float g, const AdamCoef& c) {
+  m = __fmaf_rn(c.c1, g, __fmul_rn(m, c.b1));
+  v = __fmaf_rn(__fmul_rn(c.c2, g), g, __fmul_rn(v, c.b2));
+  const float denom = __fadd_rn(__fdiv_rn(__fsqrt_rn(v), c.sqrt_bc2), c.eps);
+  p = __fmaf_rn(-c.step_size, __fdiv_rn(m, denom), p);
+}
+
 }  // namespace stego

@@ -143,19 +143,17 @@ colsum_scalar_kernel(const T* __restrict__ in, int ld, int C, long long rows, in
   atomicAdd(out + c, acc);
 }
 
-// torch.optim.Adam (amsgrad=False, weight_decay=0, maximize=False): step is 1-based.
+// torch.optim.Adam (amsgrad=False, weight_decay=0, maximize=False) with the host-formed coefficients of one step.
 __global__ void __launch_bounds__(256)
 adam_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
-            long long n, float lr, float b1, float b2, float eps, float bc1, float sqrt_bc2, float grad_scale) {
+            long long n, AdamCoef c, float grad_scale) {
   const long long i = 1ll * blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  const float gi = g[i] * grad_scale;
-  const float mi = m[i] * b1 + (1.f - b1) * gi;
-  const float vi = v[i] * b2 + (1.f - b2) * gi * gi;
+  float pi = p[i], mi = m[i], vi = v[i];
+  adam_elem(pi, mi, vi, __fmul_rn(g[i], grad_scale), c);
   m[i] = mi;
   v[i] = vi;
-  const float denom = sqrtf(vi) / sqrt_bc2 + eps;
-  p[i] -= (lr / bc1) * (mi / denom);
+  p[i] = pi;
 }
 
 }  // namespace stego
@@ -269,14 +267,12 @@ extern "C" int stego_step_losses(const float* corr_stats, int ncalls, const floa
 }
 
 extern "C" int stego_adam_step(float* param, const float* grad, float* exp_avg, float* exp_avg_sq, long long n,
-                               float lr, float beta1, float beta2, float eps, int step, float grad_scale,
+                               double lr, double beta1, double beta2, double eps, int step, float grad_scale,
                                void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   STEGO_CHECK_ARG(param && grad && exp_avg && exp_avg_sq && n > 0 && step >= 1, "stego_adam_step: bad args");
-  const double bc1 = 1.0 - pow((double)beta1, (double)step);
-  const double bc2 = 1.0 - pow((double)beta2, (double)step);
-  adam_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(param, grad, exp_avg, exp_avg_sq, n, lr, beta1, beta2,
-                                                               eps, (float)bc1, (float)sqrt(bc2), grad_scale);
+  adam_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(param, grad, exp_avg, exp_avg_sq, n,
+                                                               adam_coef(lr, beta1, beta2, eps, step), grad_scale);
   STEGO_CHECK_LAUNCH("adam_kernel");
   return STEGO_OK;
 }

@@ -67,7 +67,7 @@ __global__ void __launch_bounds__(32) p2p_signal_wait_kernel(P2pSignalParams p) 
 
 struct P2pAdamGroup {
   long long start, numel;
-  float lr, b1, b2, eps, bc1, sqrt_bc2;
+  AdamCoef c;
 };
 struct P2pAdamParams {
   const float* exports[P2P_MAX_WORLD];  // export[e & 1] of every rank
@@ -88,14 +88,11 @@ __global__ void __launch_bounds__(256) p2p_adam_kernel(P2pAdamParams p) {
 #pragma unroll
   for (int k = 0; k < P2P_MAX_GROUPS; ++k) {
     if (k < p.ngroups && i >= p.groups[k].start && i < p.groups[k].start + p.groups[k].numel) {
-      const P2pAdamGroup& q = p.groups[k];
-      const float gi = g * p.grad_scale;
-      const float mi = p.m[i] * q.b1 + (1.f - q.b1) * gi;
-      const float vi = p.v[i] * q.b2 + (1.f - q.b2) * gi * gi;
+      float pi = p.param[i], mi = p.m[i], vi = p.v[i];
+      adam_elem(pi, mi, vi, __fmul_rn(g, p.grad_scale), p.groups[k].c);
       p.m[i] = mi;
       p.v[i] = vi;
-      const float denom = sqrtf(vi) / q.sqrt_bc2 + q.eps;
-      p.param[i] -= (q.lr / q.bc1) * (mi / denom);
+      p.param[i] = pi;
     }
   }
 }
@@ -188,12 +185,7 @@ extern "C" int stego_p2p_adam(const long long* peer_exports, int world, float* p
     STEGO_CHECK_ARG(d[0] >= 0 && d[1] > 0 && d[0] + d[1] <= (double)n && d[6] >= 1, "stego_p2p_adam: bad group %d", k);
     p.groups[k].start = static_cast<long long>(d[0]);
     p.groups[k].numel = static_cast<long long>(d[1]);
-    p.groups[k].lr = static_cast<float>(d[2]);
-    p.groups[k].b1 = static_cast<float>(d[3]);
-    p.groups[k].b2 = static_cast<float>(d[4]);
-    p.groups[k].eps = static_cast<float>(d[5]);
-    p.groups[k].bc1 = static_cast<float>(1.0 - pow(d[3], d[6]));
-    p.groups[k].sqrt_bc2 = static_cast<float>(sqrt(1.0 - pow(d[4], d[6])));
+    p.groups[k].c = adam_coef(d[2], d[3], d[4], d[5], d[6]);
   }
   p.param = param; p.grad = grad; p.m = exp_avg; p.v = exp_avg_sq; p.n = n; p.grad_scale = grad_scale;
   p2p_adam_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(p);

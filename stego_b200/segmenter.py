@@ -103,9 +103,10 @@ class FusedAdam:
         self.steps += 1
         pg = self.param_groups[0]
         sl = slice(g.start, g.start + g.numel)
+        # the hyper-parameters go over as doubles: the kernel's coefficients (1 - beta2 above all) are formed from them
         rc = _lib.load().stego_adam_step(_lib.ptr(o.param[sl]), _lib.ptr(o.grad[sl]), _lib.ptr(o.exp_avg[sl]),
-                                         _lib.ptr(o.exp_avg_sq[sl]), g.numel, float(pg["lr"]), pg["betas"][0],
-                                         pg["betas"][1], pg["eps"], self.steps, o.grad_scale, _lib.stream())
+                                         _lib.ptr(o.exp_avg_sq[sl]), g.numel, float(pg["lr"]), float(pg["betas"][0]),
+                                         float(pg["betas"][1]), float(pg["eps"]), self.steps, o.grad_scale, _lib.stream())
         _lib.check(rc, "stego_adam_step")
 
 
