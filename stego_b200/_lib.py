@@ -6,6 +6,7 @@ RuntimeError is raised.  Nothing here imports the oracle.
 from __future__ import annotations
 
 import ctypes
+import gc
 import os
 import re
 from typing import Dict, List, Tuple
@@ -89,11 +90,21 @@ class Graph:
 
     def __init__(self, fn):
         torch.cuda.synchronize()
-        self.graph = torch.cuda.CUDAGraph()
-        n0 = load().stego_launch_count()
-        with torch.cuda.graph(self.graph):
-            self.result = fn()
-        self.launches = load().stego_launch_count() - n0
+        # A dead graph in a reference cycle (a model's graphs hold closures over the model) is destroyed by whichever
+        # garbage-collector pass finds it.  Destroying a graph is not permitted while a stream is capturing and
+        # invalidates the capture, so collect first and let no automatic pass run inside the capture.
+        gc.collect()
+        enabled = gc.isenabled()
+        gc.disable()
+        try:
+            self.graph = torch.cuda.CUDAGraph()
+            n0 = load().stego_launch_count()
+            with torch.cuda.graph(self.graph):
+                self.result = fn()
+            self.launches = load().stego_launch_count() - n0
+        finally:
+            if enabled:
+                gc.enable()
 
     def replay(self) -> None:
         global replayed_launches

@@ -189,6 +189,35 @@ def test_training_step_logs_histograms_without_changing_the_step(cuda_dev, fused
     assert set(model.logged_histograms) == set(hist.TAGS)
 
 
+def test_graph_capture_outlives_dead_graph_cycles(cuda_dev):
+    """The test above builds two models per parameter: the previous models' graphs die in reference cycles (their
+    captured closures hold the model).  If the garbage collector destroyed one while the next model captured, the
+    capture would be invalidated.  _lib.Graph collects before capturing and holds automatic collection off until the
+    capture ends, even when every allocation would otherwise trigger a pass."""
+    import gc
+    from stego_b200 import _lib
+    x = torch.zeros(1024, device=cuda_dev)
+
+    class Holder:
+        pass
+
+    for _ in range(3):
+        h = Holder()
+        h.self = h
+        h.graph = _lib.Graph(lambda: x.add_(1.0))
+        del h
+    old = gc.get_threshold()
+    gc.set_threshold(1, 1, 1)
+    try:
+        g = _lib.Graph(lambda: [x.add_(1.0) for _ in range(100)][-1])
+    finally:
+        gc.set_threshold(*old)
+    assert gc.isenabled()
+    g.replay()
+    torch.cuda.synchronize()
+    assert (x == 100).all()
+
+
 def test_histograms_equal_the_steps_cd(cuda_dev):
     """The counts a hist step logs are np.histogram of that step's cd: recomputed by the autograd path's loss with
     want_elems on the same draws."""
