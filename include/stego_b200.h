@@ -202,6 +202,25 @@ STEGO_API int stego_corr_loss_tiled_fwd_hist(const void* feat_tiles, const void*
                                              double* hist_cta_partials, double* hist_stats, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Correspondence precision-recall (plot_pr_curves.py:108-167): do feature / code correlations predict label agreement?
+ * ---------------------------------------------------------------------------------------------- */
+#define STEGO_PR_BINS 4096
+/* ids: out int32 [2][B][R] (R = ceil(fs^2 / 128) * 128; rows fs^2 .. R - 1 are not written): for slot 0 (coords1) and
+ * slot 1 (coords2) of image b, the class of sample s when every bilinear tap with a non-zero weight has that class,
+ * else -1.  A tap's class is label + 1 for 0 <= label < n_classes, else 0 ("unlabelled").  label: contiguous
+ * [B][H][W] of label_bytes = 8 / 4 / 1; coords as for stego_sample_norm_fwd.  n_classes 1..255, fs 1..64. */
+STEGO_API int stego_sample_label_ids(const void* label, int label_bytes, const float* coords1, const float* coords2,
+                                     int* ids, int B, int n_classes, int H, int W, int feature_samples, void* stream);
+/* Adds the precision-recall counts of one batch to counts, int64 [2][2][STEGO_PR_BINS]: [0 = fd (features), 1 = cd
+ * (code)][0 = negative, 1 = positive pair][bin].  Tiles: stego_sample_norm_fwd's with nslots = 2 of the same image
+ * (slot 0 at coords1, slot 1 at coords2), features E wide (a multiple of 64, <= 768), code padded to 128 (D <= 96).
+ * Every pair (i, j) of samples of one image is scored by its raw cosine, binned at
+ * clamp(floor((score + 1) * STEGO_PR_BINS / 2), 0, STEGO_PR_BINS - 1) in fp32, and is positive when ids of both
+ * samples are the same class (>= 0).  Integer atomics: the counts are exact and reproducible. */
+STEGO_API int stego_corr_pr(const void* feat_tiles, const void* code_tiles, const int* ids, long long* counts, int B,
+                            int feature_samples, int E, int D, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Segmentation head glue (reference: src/modules.py:73-81, 108-118) and optimiser
  * ---------------------------------------------------------------------------------------------- */
 /* Apply the three Dropout2d noises of DinoFeaturizer.forward (:109,:111,:116) in one pass:

@@ -33,6 +33,7 @@ constexpr int CL_CODE_PAD = 128; // code channels padded to 2 k-blocks
 constexpr int CL_MAX_CALLS = 16;
 constexpr int CL_DT_LD = 72;     // row stride (floats) of the per-slot gradient tiles
 constexpr int CT_MAX_FS = 64;    // largest feature_samples (S = 4096 points per image)
+constexpr int CL_PR_BINS = 4096; // score bins of the precision-recall counts (STEGO_PR_BINS)
 
 // ---------------------------------------------------------------------------------------------
 // 1. sampling + normalisation
@@ -183,6 +184,38 @@ __global__ void __launch_bounds__(256) sample_norm_kernel(SampleParams p) { samp
 template <int NV>
 __global__ void __launch_bounds__(256) sample_labels_kernel(SampleParams p) { sample_norm_row<NV, true>(p); }
 
+// Pure class id of each sample point, for the precision-recall counts (CP_PR): ids[slot][b][s] = c when every tap of
+// make_taps with a non-zero weight has class c, else -1 ("mixed").  A tap's class is sample_labels_kernel's: label + 1
+// for 0 <= label < n_classes, else 0.  Slot 0 samples image b at coords1, slot 1 the same image at coords2.  In fp32 a
+// tap weight is zero exactly when its exact value is, so "pure" is exactly "the sampled one-hot vector is e_c".  One
+// thread per sample; rows S .. R - 1 of ids are not written (CP_PR never reads them).
+__global__ void __launch_bounds__(256)
+sample_label_ids_kernel(const void* label, int label_bytes, const float* coords1, const float* coords2, int* ids, int B,
+                        int n_classes, int H, int W, int fs, int R) {
+  const int S = fs * fs;
+  const long long idx = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (idx >= 2ll * B * S) return;
+  const int s = static_cast<int>(idx % S);
+  const int sb = static_cast<int>(idx / S);  // slot * B + b
+  const int b = sb % B;
+  const Taps t = make_taps(sb >= B ? coords2 : coords1, b, s, fs, H, W);
+  const long long base = static_cast<long long>(b) * H * W;
+  int c = -1;
+  bool mixed = false;
+  auto visit = [&](float w, int pix) {
+    if (w == 0.f) return;
+    const long long l = read_label(label, label_bytes, base + pix);
+    const int k = (l >= 0 && l < n_classes) ? static_cast<int>(l) + 1 : 0;
+    if (c < 0) c = k;
+    else if (k != c) mixed = true;
+  };
+  visit(t.w00, t.i00);
+  visit(t.w01, t.i01);
+  visit(t.w10, t.i10);
+  visit(t.w11, t.i11);
+  ids[static_cast<size_t>(sb) * R + s] = mixed ? -1 : c;
+}
+
 // Vectorised variant for the layout the training step uses: bf16 source, channel stride 1 (tokens-major),
 // C % 8 == 0, Cpad == C.  Each lane owns 8 consecutive channels per step: four 16-byte tap loads, two 16-byte tile
 // stores (hi, lo) — 8x fewer memory instructions than the generic kernel.
@@ -314,6 +347,9 @@ struct CorrParams {
   const float* hist_thr;             // [TB_THR] fp32 bucket thresholds (tb_hist.cuh)
   unsigned long long* hist_counts;   // [3][TB_BINS], zeroed by the caller, added to with integer atomics
   double* hist_part;                 // [ncalls][B][CTAs per (image, call)][4]: min, max, sum, sum of squares
+  // precision-recall phase (CP_PR) only
+  const int* pr_ids;                 // [2][B][R]: pure class id of each sample of slot 0 / slot 1, -1 if mixed
+  unsigned long long* pr_counts;     // [2 (fd, cd)][2 (negative, positive)][CL_PR_BINS], added to
 };
 
 constexpr int CL_THREADS = 384;  // two MMA warpgroups (rows 0..63 / 64..127 of the tile) + the TMA producer warpgroup
@@ -326,13 +362,15 @@ constexpr int CP_BWD = 2;          // whole row, grid (B): the calls in order, d
 constexpr int CP_BWD_DB = 3;       // multi-tile, grid (B, nT): CTA per (image, ct) walking (call, rt) -> dB rows ct
 constexpr int CP_BWD_DA = 4;       // multi-tile, grid (B, nT): CTA per (image, rt) walking (call, ct) -> dA rows rt
 constexpr int CP_HIST = 8;         // flag on CP_FWD / CP_FWD_ROWPART: also bin cd into TensorBoard histograms
+constexpr int CP_PR = 16;          // grid (B, 1, nT^2) like CP_FWD_ROWPART, one call (slot 0 vs slot 1): bin raw fd and
+                                   // cd by label agreement into precision-recall counts; no loss, fd or cd output
 
 // unit u of this CTA -> (call, row tile, column tile)
 template <int kPhase>
 __device__ __forceinline__ void corr_unit(const CorrParams& p, int u, int& call, int& rt, int& ct) {
   if constexpr (kPhase == CP_FWD) {
     call = blockIdx.y; rt = 0; ct = 0;
-  } else if constexpr (kPhase == CP_FWD_ROWPART) {
+  } else if constexpr (kPhase == CP_FWD_ROWPART || kPhase == CP_PR) {
     call = blockIdx.y; rt = blockIdx.z / p.nT; ct = blockIdx.z % p.nT;
   } else if constexpr (kPhase == CP_BWD) {
     call = u; rt = 0; ct = 0;
@@ -402,13 +440,60 @@ __device__ __forceinline__ void corr_hist_epilogue(const CorrParams& p, const fl
   }
 }
 
+// Score bin of the precision-recall counts: clamp(floor((score + 1) * CL_PR_BINS / 2), 0, CL_PR_BINS - 1) in fp32.  The
+// scale is a power of two, so the only rounding is score + 1, and the bin is non-decreasing in the score.
+__device__ __forceinline__ int pr_bin(float score) {
+  const int k = static_cast<int>(floorf((score + 1.f) * static_cast<float>(CL_PR_BINS / 2)));
+  return min(max(k, 0), CL_PR_BINS - 1);
+}
+
+// Precision-recall epilogue (CP_PR): bins the raw fd and cd of every element with row and column < S by score
+// (pr_bin) and by label agreement — positive when row sample i (slot 0) and column sample j (slot 1) are both pure with
+// the same class (sample_label_ids_kernel).  The per-CTA uint32 bins [2 (fd, cd)][2 (negative, positive)][CL_PR_BINS]
+// (64 KB) and the unit's 128 row and 128 column ids live in the operand ring, free here for the reasons
+// corr_hist_epilogue gives; the caller's bar.sync has put both warpgroups past their wgmma_wait<0>.  The non-empty bins
+// are then added to the global counts with one integer atomic each, so the counts are exact and run-to-run identical.
+__device__ __forceinline__ void corr_pr_epilogue(const CorrParams& p, const float (&fd)[64], const float (&cd)[64],
+                                                 int i_loc, int j_base, int rt, int ct, int b, uint8_t* smem) {
+  uint32_t* bins = reinterpret_cast<uint32_t*>(smem);
+  int* rid = reinterpret_cast<int*>(smem + 4 * 4 * CL_PR_BINS);  // [128] ids of the unit's rows
+  int* cid = rid + CL_ROWS;                                      // [128] ids of the unit's columns
+  const int tid = threadIdx.x;  // 0 .. 255: the MMA warpgroups
+  const int S = p.S;
+  for (int k = tid; k < CL_PR_BINS; k += 256) reinterpret_cast<uint4*>(bins)[k] = make_uint4(0, 0, 0, 0);
+  if (tid < CL_ROWS) {
+    const int i = rt * CL_ROWS + tid;
+    rid[tid] = i < S ? p.pr_ids[static_cast<size_t>(b) * p.R + i] : -1;
+  } else {
+    const int j = ct * CL_ROWS + tid - CL_ROWS;
+    cid[tid - CL_ROWS] = j < S ? p.pr_ids[(static_cast<size_t>(p.B) + b) * p.R + j] : -1;
+  }
+  asm volatile("bar.sync 1, 256;\n" ::: "memory");
+  const int r0 = rid[i_loc], r1 = rid[i_loc + 8];
+#pragma unroll
+  for (int t = 0; t < 64; ++t) {
+    const int h = (t >> 1) & 1;
+    const int jl = 8 * (t >> 2) + j_base + (t & 1);
+    if (rt * CL_ROWS + i_loc + 8 * h < S && ct * CL_ROWS + jl < S) {
+      const int ri = h ? r1 : r0;
+      const int pos = (ri >= 0 && ri == cid[jl]) ? CL_PR_BINS : 0;
+      atomicAdd(&bins[pos + pr_bin(fd[t])], 1u);
+      atomicAdd(&bins[2 * CL_PR_BINS + pos + pr_bin(cd[t])], 1u);
+    }
+  }
+  asm volatile("bar.sync 1, 256;\n" ::: "memory");
+  for (int k = tid; k < 4 * CL_PR_BINS; k += 256)
+    if (bins[k]) atomicAdd(&p.pr_counts[k], static_cast<unsigned long long>(bins[k]));
+}
+
 template <int kVariant>
 __global__ void __launch_bounds__(CL_THREADS, 1)
 corr_kernel(const __grid_constant__ CUtensorMap tmF, const __grid_constant__ CUtensorMap tmC, CorrParams p) {
   constexpr int kPhase = kVariant & ~CP_HIST;
   constexpr bool kHist = (kVariant & CP_HIST) != 0;
   static_assert(!kHist || kPhase <= CP_FWD_ROWPART, "histograms are a forward epilogue");
-  constexpr bool kBackward = kPhase >= CP_BWD;
+  constexpr bool kPR = kPhase == CP_PR;
+  constexpr bool kBackward = kPhase >= CP_BWD && !kPR;
   constexpr bool kDA = kPhase == CP_BWD || kPhase == CP_BWD_DA;
   constexpr bool kDB = kPhase == CP_BWD || kPhase == CP_BWD_DB;
   // smem: ring of kRing stages x (A 16K + B 16K) for the feature GEMM, then the resident code tiles.
@@ -417,6 +502,7 @@ corr_kernel(const __grid_constant__ CUtensorMap tmF, const __grid_constant__ CUt
   constexpr uint32_t CODE_BYTES = 8 * CL_TILE;  // Ac: [plane][kb] 4 tiles, Bc: 4 tiles
   constexpr uint32_t OFF_CODE = RING_BYTES;
   constexpr uint32_t OFF_BAR = OFF_CODE + CODE_BYTES;
+  static_assert(!kPR || RING_BYTES >= 4 * 4 * CL_PR_BINS + 2 * 4 * CL_ROWS, "the PR bins live in the operand ring");
 
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -541,6 +627,11 @@ corr_kernel(const __grid_constant__ CUtensorMap tmF, const __grid_constant__ CUt
       if (leader) mbar_arrive(&empty_bar[prev]);
     }
 
+    if constexpr (kPR) {
+      asm volatile("bar.sync 1, 256;\n" ::: "memory");
+      corr_pr_epilogue(p, fd, cd, i_loc, j_base, rt, ct, b, smem);
+      return;
+    }
     // ===================== epilogue on the accumulator fragments =====================
     const int i0 = rt * CL_ROWS + i_loc;  // rows of fragment halves 0 / 1: i0, i0 + 8
     const int j0 = ct * CL_ROWS + j_base;
@@ -1129,19 +1220,20 @@ static int fill_corr_params(CorrParams& p, bool tiled, int B, int fs, int E, int
   p.partials = nullptr; p.rowpart = nullptr; p.cd_out = nullptr; p.fd_out = nullptr;
   p.stats = nullptr; p.rowmean = nullptr; p.gscale = nullptr; p.gelem = nullptr; p.gcd = nullptr; p.dtiles = nullptr;
   p.hist_thr = nullptr; p.hist_counts = nullptr; p.hist_part = nullptr;
+  p.pr_ids = nullptr; p.pr_counts = nullptr;
   return STEGO_OK;
 }
 
 template <int kVariant>
 static int launch_corr(const CUtensorMap& tmF, const CUtensorMap& tmC, const CorrParams& p, cudaStream_t stream) {
   constexpr int kPhase = kVariant & ~CP_HIST;
-  constexpr int kRing = kPhase >= CP_BWD ? 2 : 3;
+  constexpr int kRing = (kPhase >= CP_BWD && kPhase <= CP_BWD_DA) ? 2 : 3;
   constexpr size_t smem = size_t(kRing) * 2 * CL_TILE + 8 * CL_TILE + 512 + 1024;
   static_assert(smem <= 232448, "exceeds the 227 KB of shared memory a CTA can opt into");
   constexpr auto kern = corr_kernel<kVariant>;
   if (const int rc = opt_in_smem<kern>(smem, "corr_kernel"); rc != STEGO_OK) return rc;
   const dim3 grid = kPhase == CP_FWD ? dim3(p.B, p.ncalls)
-                  : kPhase == CP_FWD_ROWPART ? dim3(p.B, p.ncalls, p.nT * p.nT)
+                  : (kPhase == CP_FWD_ROWPART || kPhase == CP_PR) ? dim3(p.B, p.ncalls, p.nT * p.nT)
                   : kPhase == CP_BWD ? dim3(p.B) : dim3(p.B, p.nT);
   kern<<<grid, CL_THREADS, smem, stream>>>(tmF, tmC, p);
   STEGO_CHECK_LAUNCH("corr_kernel");
@@ -1322,4 +1414,41 @@ extern "C" int stego_corr_loss_tiled_bwd(const void* feat_tiles, const void* cod
   // dB (every slot, slot 0 included for the intra call) then dA (slot 0): stream order fixes the summation order
   if ((rc = launch_corr<CP_BWD_DB>(tmF, tmC, p, stream)) != STEGO_OK) return rc;
   return launch_corr<CP_BWD_DA>(tmF, tmC, p, stream);
+}
+
+extern "C" int stego_sample_label_ids(const void* label, int label_bytes, const float* coords1, const float* coords2,
+                                      int* ids, int B, int n_classes, int H, int W, int feature_samples, void* stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  STEGO_CHECK_ARG(label && coords1 && coords2 && ids, "stego_sample_label_ids: null pointer");
+  STEGO_CHECK_ARG(label_bytes == 8 || label_bytes == 4 || label_bytes == 1,
+                  "stego_sample_label_ids: label_bytes=%d (8, 4 or 1)", label_bytes);
+  STEGO_CHECK_ARG(n_classes >= 1 && n_classes <= 255, "stego_sample_label_ids: n_classes=%d outside 1..255", n_classes);
+  STEGO_CHECK_ARG(feature_samples >= 1 && feature_samples <= CT_MAX_FS,
+                  "stego_sample_label_ids: feature_samples=%d outside 1..%d", feature_samples, CT_MAX_FS);
+  STEGO_CHECK_ARG(B > 0 && H > 1 && W > 1, "stego_sample_label_ids: B=%d H=%d W=%d", B, H, W);
+  const int S = feature_samples * feature_samples;
+  const int R = (S + CL_ROWS - 1) / CL_ROWS * CL_ROWS;
+  const long long n = 2ll * B * S;
+  sample_label_ids_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, stream>>>(
+      label, label_bytes, coords1, coords2, ids, B, n_classes, H, W, feature_samples, R);
+  STEGO_CHECK_LAUNCH("sample_label_ids_kernel");
+  return STEGO_OK;
+}
+
+extern "C" int stego_corr_pr(const void* feat_tiles, const void* code_tiles, const int* ids, long long* counts, int B,
+                             int feature_samples, int E, int D, void* stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  STEGO_CHECK_ARG(feat_tiles && code_tiles && ids && counts, "stego_corr_pr: null pointer");
+  STEGO_CHECK_ARG(feature_samples >= 1 && feature_samples <= CT_MAX_FS,
+                  "stego_corr_pr: feature_samples=%d outside 1..%d", feature_samples, CT_MAX_FS);
+  const int slot_of_call[1] = {1};
+  const float shifts[1] = {0.f};
+  CorrParams p;
+  int rc = fill_corr_params(p, true, B, feature_samples, E, D, 2, 1, slot_of_call, shifts, 0, 0, 0);
+  if (rc != STEGO_OK) return rc;
+  p.pr_ids = ids;
+  p.pr_counts = reinterpret_cast<unsigned long long*>(counts);
+  CUtensorMap tmF, tmC;
+  if ((rc = encode_tile_maps(feat_tiles, code_tiles, p, &tmF, &tmC)) != STEGO_OK) return rc;
+  return launch_corr<CP_PR>(tmF, tmC, p, stream);
 }

@@ -569,6 +569,30 @@ class LitUnsupervisedSegmenter(nn.Module):
                 "cluster_preds": out[3][:n_images].long().cpu() if n_images > 0 else none,
                 "label": label[:n_images].detach().cpu()}
 
+    def correspondence_pr_step(self, batch, metric) -> None:
+        """plot_pr_curves.py:126-142 (LitRecalibrator.validation_step) for the two methods this package has: the head's
+        code ("STEGO (Ours)", :140) and the backbone features ("DINO", :141) of the eval-mode net, scored against
+        the labels by `metric`, a correspondence.CorrespondencePR.  Draws coords1 then coords2 with the reference's two
+        `torch.rand([B, fs, fs, 2]) * 2 - 1` calls (:134-136) at cfg.feature_samples, on the image's device.
+
+        Like validation_step it waits for the previous step's parameter update, leaves the training step's CUDA graphs
+        and workspace alone and restores the net's train / eval modes on exit.  Nothing is copied to the host."""
+        self.flush()
+        img, label = batch["img"], batch["label"]
+        modes = [(m, m.training) for m in self.net.modules()]
+        self.net.eval()
+        try:
+            with torch.no_grad():
+                feats, code = self.net(img)
+                fs = int(self.cfg.feature_samples)
+                coord_shape = [img.shape[0], fs, fs, 2]
+                coords1 = torch.rand(coord_shape, device=img.device) * 2 - 1
+                coords2 = torch.rand(coord_shape, device=img.device) * 2 - 1
+                metric.update(feats, code, label, coords1, coords2)
+        finally:
+            for m, mode in modes:
+                m.training = mode
+
     def validation_epoch_end(self, outputs=None) -> Dict[str, float]:
         """train_segmentation.py:277-283, 361-371 without the figures: sum both confusion matrices over the ranks (what
         torchmetrics' dist_reduce_fx="sum" does; once per epoch gives the same sums as once per step), compute mIoU /
