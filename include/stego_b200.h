@@ -221,6 +221,31 @@ STEGO_API int stego_corr_pr(const void* feat_tiles, const void* code_tiles, cons
                             int feature_samples, int E, int D, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Dense correspondence heatmaps (plot_dino_correspondence.py:39-58, get_heatmaps), in four steps around one
+ * stego_gemm_bf16_batched call raw[b] = q_ops[b] . t_ops[b]^T (M = P, N = h w, K = nseg * Epad, fp32 [B][P][h w]).
+ * Feature maps have element strides (batch, channel, y, x), fp32 or bf16 (is_bf16); 1 <= E <= 768, Epad a multiple of 8
+ * >= E (<= 768); nseg = 2 for a bf16 target, 3 for an fp32 one.
+ * ---------------------------------------------------------------------------------------------- */
+/* Target map [B][E][h][w] -> ops bf16 [B][h w][nseg * Epad] (K-major; bf16: [t | t], fp32: [hi | hi | lo] with
+ * t = hi + lo; zeros past E in each segment) and inv_norm fp32 [B][h w] = 1 / max(||t||, 1e-12). */
+STEGO_API int stego_heatmap_prep_target(const void* target, int target_is_bf16, long long stride_b, long long stride_c,
+                                        long long stride_y, long long stride_x, int B, int E, int h, int w, int Epad,
+                                        void* ops, float* inv_norm, void* stream);
+/* grid_sample (bilinear, border, align_corners=True) of feats [B][E][h][w] at points fp32 [B][P][2] = (x, y), L2
+ * normalised in fp32 (eps 1e-12) and split n = hi + lo -> ops bf16 [B][P][nseg * Epad]: [hi | lo] (nseg 2) or
+ * [hi | lo | hi] (nseg 3), the counterpart of the target's operand. */
+STEGO_API int stego_heatmap_sample_queries(const void* feats, int feats_is_bf16, long long stride_b, long long stride_c,
+                                           long long stride_y, long long stride_x, const float* points, int B, int P,
+                                           int E, int h, int w, int Epad, int nseg, void* ops, void* stream);
+/* In place on corr fp32 [B][P][hw] (the GEMM's raw dots): c = raw * inv_norm[b], then max(c - mean_j c, 0) per row;
+ * the row mean is reduced in a fixed order (bit-reproducible). */
+STEGO_API int stego_heatmap_finish(float* corr, const float* inv_norm, int B, int P, int hw, void* stream);
+/* F.interpolate(in, (H, W), mode="bilinear", align_corners=True): in fp32 [n][h][w] -> out fp32 [n][H][W] (64-bit
+ * offsets, H <= 65535), with the arithmetic of ATen's CUDA upsample_bilinear2d; 16-byte streaming stores when W % 4 == 0
+ * and out is 16-byte aligned. */
+STEGO_API int stego_heatmap_upsample(const float* in, float* out, long long n, int h, int w, int H, int W, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Segmentation head glue (reference: src/modules.py:73-81, 108-118) and optimiser
  * ---------------------------------------------------------------------------------------------- */
 /* Apply the three Dropout2d noises of DinoFeaturizer.forward (:109,:111,:116) in one pass:

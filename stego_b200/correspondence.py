@@ -175,3 +175,90 @@ class CorrespondencePR:
         """One device-to-host copy of the counts, then `pr_from_counts` per method (float64, host)."""
         c = self.counts.cpu().numpy()
         return {m: pr_from_counts(c[k, 0], c[k, 1]) for k, m in enumerate(METHODS)}
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Dense correspondence heatmaps (src/plot_dino_correspondence.py:39-58)
+# ---------------------------------------------------------------------------------------------------------------------
+def _strides(t: torch.Tensor):
+    return (int(s) for s in t.stride())
+
+
+def correspondence_heatmaps(feats: torch.Tensor, target: torch.Tensor, query_points: torch.Tensor,
+                            size) -> torch.Tensor:
+    """The heatmaps of `get_heatmaps` for a batch: out[b, p] = F.interpolate(clamp(c - c.mean(), 0), size, bilinear,
+    align_corners=True) with c[j] = <normalize(sample(feats, query_points)[b, :, p]), normalize(target[b, :, j])>
+    (F.normalize's eps 1e-12) over every position j of target[b].  `target = feats` gives the "Self Correspondence"
+    maps, the features of the KNN image the "KNN Correspondence" maps.
+
+    feats [B, E, h, w] and target [B, E, h', w']: fp32 or bf16, any memory layout, 1 <= E <= 768; query_points
+    [B, P, 1, 2] (x, y) in [-1, 1] (values beyond are clamped to the border, as grid_sample does); size = (H, W).
+    Returns fp32 [B, P, H, W] on the device, without synchronising with the host."""
+    _lib.require_cuda(feats, target, query_points)
+    for t in (target, query_points):
+        if t.device != feats.device:
+            raise RuntimeError(f"stego_b200: correspondence_heatmaps input on {t.device}, feats on {feats.device}")
+    if feats.dim() != 4 or target.dim() != 4:
+        raise RuntimeError("stego_b200: feats and target must be [B, C, h, w]")
+    B, E, h, w = feats.shape
+    if target.shape[0] != B or target.shape[1] != E:
+        raise RuntimeError(f"stego_b200: target {tuple(target.shape)} does not match feats {tuple(feats.shape)} in "
+                           "batch and channels")
+    if query_points.dim() != 4 or query_points.shape[0] != B or query_points.shape[2] != 1 \
+            or query_points.shape[3] != 2:
+        raise RuntimeError(f"stego_b200: query_points must be [B, P, 1, 2], got {tuple(query_points.shape)}")
+    if not query_points.is_floating_point():
+        raise RuntimeError(f"stego_b200: query_points must be floating point, got {query_points.dtype}")
+    for name, t in (("feats", feats), ("target", target)):
+        if t.dtype not in (torch.float32, torch.bfloat16):
+            raise RuntimeError(f"stego_b200: {name} must be fp32 or bf16, got {t.dtype}")
+    if not 1 <= E <= 768:
+        raise RuntimeError(f"stego_b200: feature channels {E} unsupported (1..768)")
+    if len(tuple(size)) != 2:
+        raise RuntimeError(f"stego_b200: size must be (H, W), got {size}")
+    H, W = (int(s) for s in size)
+    P = query_points.shape[1]
+    ht, wt = target.shape[2], target.shape[3]
+    if min(B, P, h, w, ht, wt) < 1 or not 1 <= H <= 65535 or W < 1:
+        raise RuntimeError(f"stego_b200: empty or oversized heatmap request: B={B} P={P} feats {h}x{w} "
+                           f"target {ht}x{wt} size {H}x{W}")
+    dev = feats.device
+    e_pad = -(-E // 8) * 8
+    t_bf16 = target.dtype == torch.bfloat16
+    nseg = 2 if t_bf16 else 3
+    lib = _lib.load()
+    f, t = feats.detach(), target.detach()
+    t_ops = torch.empty(B, ht * wt, nseg * e_pad, dtype=torch.bfloat16, device=dev)
+    inv = torch.empty(B, ht * wt, dtype=torch.float32, device=dev)
+    _lib.check(lib.stego_heatmap_prep_target(_lib.ptr(t), int(t_bf16), *_strides(t), B, E, ht, wt, e_pad,
+                                             _lib.ptr(t_ops), _lib.ptr(inv), _lib.stream()),
+               "stego_heatmap_prep_target")
+    pts = query_points.detach().to(torch.float32).contiguous()
+    q_ops = torch.empty(B, P, nseg * e_pad, dtype=torch.bfloat16, device=dev)
+    _lib.check(lib.stego_heatmap_sample_queries(_lib.ptr(f), int(f.dtype == torch.bfloat16), *_strides(f),
+                                                _lib.ptr(pts), B, P, E, h, w, e_pad, nseg, _lib.ptr(q_ops),
+                                                _lib.stream()), "stego_heatmap_sample_queries")
+    corr = ops.gemm_batched(q_ops, t_ops, torch.empty(B, P, ht * wt, dtype=torch.float32, device=dev))
+    _lib.check(lib.stego_heatmap_finish(_lib.ptr(corr), _lib.ptr(inv), B, P, ht * wt, _lib.stream()),
+               "stego_heatmap_finish")
+    out = torch.empty(B, P, H, W, dtype=torch.float32, device=dev)
+    _lib.check(lib.stego_heatmap_upsample(_lib.ptr(corr), _lib.ptr(out), B * P, ht, wt, H, W, _lib.stream()),
+               "stego_heatmap_upsample")
+    return out
+
+
+def get_heatmaps(net, img: torch.Tensor, img_pos: torch.Tensor, query_points: torch.Tensor):
+    """Drop-in for the reference's `get_heatmaps(net, img, img_pos, query_points)` (plot_dino_correspondence.py:39-58):
+    `net(x)[0]` are the features of one image; returns the ("Self", "KNN") correspondence heatmaps as CPU fp32 tensors
+    [P, H, W] and [P, H', W'] at the sizes of img and img_pos.  `net` runs in whatever mode the caller left it.  Like the
+    reference it takes one image (B = 1); for a batch call `correspondence_heatmaps` directly."""
+    if img.shape[0] != 1 or img_pos.shape[0] != 1 or query_points.dim() != 4 or query_points.shape[0] != 1:
+        raise RuntimeError(f"stego_b200: get_heatmaps takes one image, as the reference does (img "
+                           f"{tuple(img.shape)}, img_pos {tuple(img_pos.shape)}, query_points "
+                           f"{tuple(query_points.shape)}); use correspondence_heatmaps for a batch")
+    feats1, _ = net(img.cuda())
+    feats2, _ = net(img_pos.cuda())
+    qp = query_points.to(feats1.device)
+    heatmap_intra = correspondence_heatmaps(feats1, feats1, qp, img.shape[2:])[0].cpu()
+    heatmap_inter = correspondence_heatmaps(feats1, feats2, qp, img_pos.shape[2:])[0].cpu()
+    return heatmap_intra, heatmap_inter

@@ -24,6 +24,7 @@
 #include "common.cuh"
 #include "host_util.h"
 #include "probe_common.cuh"
+#include "taps.cuh"
 #include "tb_hist.cuh"
 
 namespace stego {
@@ -56,36 +57,12 @@ struct SampleParams {
   float eps;
 };
 
-struct Taps {
-  int i00, i01, i10, i11;      // pixel offsets (y*W + x), clamped in-bounds
-  float w00, w01, w10, w11;    // nw, ne, sw, se weights (0 for out-of-bounds taps)
-};
-
-// grid_sample(bilinear, padding_mode='border', align_corners=True) source taps for sample index s = i*fs + j,
-// which reads coords[b][j][i] because `sample` permutes the grid (modules.py:288).
+// grid_sample(bilinear, padding_mode='border', align_corners=True) source taps (taps.cuh) for sample index
+// s = i*fs + j, which reads coords[b][j][i] because `sample` permutes the grid (modules.py:288).
 __device__ __forceinline__ Taps make_taps(const float* coords, int b, int s, int fs, int H, int W) {
   const int i = s / fs, j = s % fs;
   const float* cp = coords + ((static_cast<long long>(b) * fs + j) * fs + i) * 2;
-  float x = ((cp[0] + 1.f) / 2.f) * (W - 1);
-  float y = ((cp[1] + 1.f) / 2.f) * (H - 1);
-  x = fminf(fmaxf(x, 0.f), static_cast<float>(W - 1));
-  y = fminf(fmaxf(y, 0.f), static_cast<float>(H - 1));
-  const float x0 = floorf(x), y0 = floorf(y);
-  const float x1 = x0 + 1.f, y1 = y0 + 1.f;
-  Taps t;
-  t.w00 = (x1 - x) * (y1 - y);
-  t.w01 = (x - x0) * (y1 - y);
-  t.w10 = (x1 - x) * (y - y0);
-  t.w11 = (x - x0) * (y - y0);
-  const int ix0 = static_cast<int>(x0), iy0 = static_cast<int>(y0);
-  int ix1 = ix0 + 1, iy1 = iy0 + 1;
-  if (ix1 > W - 1) { ix1 = W - 1; t.w01 = 0.f; t.w11 = 0.f; }
-  if (iy1 > H - 1) { iy1 = H - 1; t.w10 = 0.f; t.w11 = 0.f; }
-  t.i00 = iy0 * W + ix0;
-  t.i01 = iy0 * W + ix1;
-  t.i10 = iy1 * W + ix0;
-  t.i11 = iy1 * W + ix1;
-  return t;
+  return grid_taps(cp[0], cp[1], H, W);
 }
 
 __device__ __forceinline__ void slot_source(const SampleParams& p, int slot, int b, const void*& src,
