@@ -340,60 +340,49 @@ STEGO_API int stego_knn_topk(const float* feats, int n, int E, int k, void* plan
 /* ------------------------------------------------------------------------------------------------
  * Dense CRF post-processing (BASELINE.json configs[4]; src/crf.py:22-45 -> pydensecrf, third-party, parity UNPINNED:
  * the kernels follow the published densecrf / permutohedral-lattice algorithm as restated by oracle/crf_oracle.py).
- * Rows of Q / unary / lattice values are 32 floats (classes padded to a warp); C <= 32.
+ * Rows of Q / unary / lattice values are 32 floats per probe (classes padded to a warp); C <= 32.
  * ---------------------------------------------------------------------------------------------- */
 /* Permutohedral embedding of every pixel of an [H][W] frame: features (x/sxy, y/sxy) for d = 2, plus the three
  * image channels / srgb for d = 5 (image [H][W][3] uint8).  keys [N][d+1] int64 (packed lattice vertex coordinates),
  * bary [N][d+1] fp32 barycentric weights. */
 STEGO_API int stego_crf_lattice(int H, int W, int d, float sxy, float srgb, const unsigned char* image, long long* keys,
                                 float* bary, void* stream);
-/* Splat scale[pixel] * in[pixel][:C] (in null: ones; scale null: 1) onto the lattice (values: [(M+1)][32], zeroed by the
- * caller; row 0 = missing neighbour) and blur along the d+1 axes (n1 / n2: [d+1][M] neighbour ids, -1 = missing).
- * Result in values_tmp for d = 2, in values for d = 5. */
-STEGO_API int stego_crf_splat_blur(int d, long long N, int M, int C, const int* offset, const float* bary, const float* scale,
-                                   const float* in, const int* n1, const int* n2, float* values, float* values_tmp,
-                                   void* stream);
-/* NORMALIZE_SYMMETRIC factor of a kernel from the blurred ones-splat: norm[pixel] = 1 / sqrt(K 1 + 1e-20). */
-STEGO_API int stego_crf_norm(int d, long long N, const int* offset, const float* bary, const float* values, float* norm_out,
-                             void* stream);
 /* Class scores [C][N] at full resolution -> unary energies -log(clip(softmax, 1e-5, 1)) [N][32] and Q_0 = softmax(-U). */
 STEGO_API int stego_crf_unary(const float* logits, float* unary, float* Q, long long N, int C, void* stream);
-/* One mean-field update Q <- softmax(-U + w_g n_g K_g(n_g Q) + w_b n_b K_b(n_b Q)) from the blurred lattice values of the
- * Gaussian (d = 2) and bilateral (d = 5) kernels; q_out [C][N] and argmax_out [N] are optional (last iteration). */
-STEGO_API int stego_crf_update(const float* unary, const int* off_g, const float* bary_g, const float* val_g, const float* norm_g,
-                               const int* off_b, const float* bary_b, const float* val_b, const float* norm_b, float w_g,
-                               float w_b, float* Q, float* q_out, unsigned char* argmax_out, long long N, int C, void* stream);
+/* NORMALIZE_SYMMETRIC factor norm [N] = 1 / sqrt(K 1 + 1e-20) of a lattice (offset, bary [N][d+1]; CSR rowptr [M+1]
+ * and slots [N*(d+1)] = pixel*(d+1)+vertex sorted by point; n1 / n2 [d+1][M], -1 = missing); values, values_tmp [M]
+ * scratch. */
+STEGO_API int stego_crf_norm(int d, long long N, int M, const int* offset, const float* bary, const int* rowptr,
+                             const int* slots, const int* n1, const int* n2, float* values, float* values_tmp,
+                             float* norm_out, void* stream);
+/* n_iter >= 1 mean-field iterations Q <- softmax(-U + w_g n_g K_g(n_g Q) + w_b n_b K_b(n_b Q)) of B frames of N pixels,
+ * deterministic (gather splats, no float atomics).  One probe (n_clu = 0): rows of 32 floats per pixel and lattice
+ * point, classes n_lin (unary and Q from stego_crf_unary).  Two probes: rows of 64 floats, the linear probe in
+ * [0, 32) and the cluster probe in [32, 64) (stego_eval_crf_unary).  Position lattice (*_g, Mg points): one frame's,
+ * shared by the B frames.  Bilateral lattice (*_b, Mb points): the frames' lattices concatenated over B*N pixels.
+ * Scratch val_g, tmp_g [B*Mg][row], val_b, tmp_b [Mb][row].  Last-iteration outputs, each optional: marginals
+ * lin_q [B][n_lin][N], clu_q [B][n_clu][N]; argmax maps lin_pred, clu_pred [B][N] uint8 (lowest index on ties); with
+ * label [B][N] (label_bytes 8 / 4 / 1) the int64 confusion counts lin_conf [n_lin][n_label_classes],
+ * clu_conf [n_clu][n_label_classes] are incremented at [pred][actual] for every pixel with
+ * 0 <= label < n_label_classes and pred < n_label_classes. */
+STEGO_API int stego_crf_mean_field(int B, long long N, int n_lin, int n_clu, int n_iter, const float* unary, float* Q,
+                                   const int* off_g, const float* bary_g, const int* rowptr_g, const int* slots_g,
+                                   const int* n1_g, const int* n2_g, const float* norm_g, int Mg,
+                                   const int* off_b, const float* bary_b, const int* rowptr_b, const int* slots_b,
+                                   const int* n1_b, const int* n2_b, const float* norm_b, int Mb, float w_g,
+                                   float w_b, float* val_g, float* tmp_g, float* val_b, float* tmp_b, float* lin_q,
+                                   float* clu_q, unsigned char* lin_pred, unsigned char* clu_pred,
+                                   const void* label, int label_bytes, int n_label_classes, long long* lin_conf,
+                                   long long* clu_conf, void* stream);
 
 /* ---- CRF-refined evaluation (src/eval_segmentation.py:124-141 with run_crf=True): both probes' dense CRFs for a batch
- * of frames, deterministic (gather splats, no float atomics).  Rows of 64 floats per pixel and lattice point: linear
- * probe in [0, 32), cluster probe in [32, 64).
+ * of frames through stego_crf_mean_field with two probes per row.
  * stego_eval_crf_unary: the inputs of stego_eval_probes (lr_scratch [B*h*w][80] floats) -> unary energies
- *   -log(clip(softmax(probe), 1e-5, 1)) and the initial Q = softmax(-U), both [B*H*W][64] fp32, 16-byte aligned.
- * stego_eval_crf_norm: NORMALIZE_SYMMETRIC factor norm [N] of a lattice (offset, bary [N][d+1]; CSR rowptr [M+1] and
- *   slots [N*(d+1)] = pixel*(d+1)+vertex sorted by point; n1 / n2 [d+1][M], -1 = missing); values, values_tmp [M] scratch.
- * stego_eval_crf_mean_field: n_iter mean-field iterations of B frames of N pixels.  Position lattice (*_g, Mg points):
- *   one frame's, shared by the B frames.  Bilateral lattice (*_b, Mb points): the frames' lattices concatenated over
- *   B*N pixels.  Scratch val_g, tmp_g [B*Mg][64], val_b, tmp_b [Mb][64].  Last-iteration outputs, each optional:
- *   marginals lin_q [B][n_lin][N], clu_q [B][n_clu][N]; argmax maps lin_pred, clu_pred [B][N] uint8 (lowest index on
- *   ties); with label [B][N] (label_bytes 8 / 4 / 1) the int64 confusion counts lin_conf [n_lin][n_label_classes],
- *   clu_conf [n_clu][n_label_classes] are incremented at [pred][actual] for every pixel with
- *   0 <= label < n_label_classes and pred < n_label_classes. */
+ *   -log(clip(softmax(probe), 1e-5, 1)) and the initial Q = softmax(-U), both [B*H*W][64] fp32, 16-byte aligned. */
 STEGO_API int stego_eval_crf_unary(const float* code, const float* code_flip, long long ld_code, int C, int B, int h, int w,
                                    int H, int W, const float* lin_weight, const float* lin_bias, int n_lin,
                                    const float* clusters, int n_clu, float alpha, float* lr_scratch, float* unary, float* Q,
                                    void* stream);
-STEGO_API int stego_eval_crf_norm(int d, long long N, int M, const int* offset, const float* bary, const int* rowptr,
-                                  const int* slots, const int* n1, const int* n2, float* values, float* values_tmp,
-                                  float* norm_out, void* stream);
-STEGO_API int stego_eval_crf_mean_field(int B, long long N, int n_lin, int n_clu, int n_iter, const float* unary, float* Q,
-                                        const int* off_g, const float* bary_g, const int* rowptr_g, const int* slots_g,
-                                        const int* n1_g, const int* n2_g, const float* norm_g, int Mg,
-                                        const int* off_b, const float* bary_b, const int* rowptr_b, const int* slots_b,
-                                        const int* n1_b, const int* n2_b, const float* norm_b, int Mb, float w_g,
-                                        float w_b, float* val_g, float* tmp_g, float* val_b, float* tmp_b, float* lin_q,
-                                        float* clu_q, unsigned char* lin_pred, unsigned char* clu_pred,
-                                        const void* label, int label_bytes, int n_label_classes, long long* lin_conf,
-                                        long long* clu_conf, void* stream);
 
 /* ---- contrastive CRF loss (optional training term; replaces ContrastiveCRFLoss.forward, src/modules.py:449-469, and its
  * autograd backward).  guidance [B, Cg <= 3, H, W] and clusters [B, C <= 80, H, W] are fp32 with arbitrary element strides;

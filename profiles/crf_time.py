@@ -22,10 +22,15 @@ def timed(fn, n=3):
     return (time.perf_counter() - t0) / n * 1e3
 
 
-lat_g = timed(lambda: crf._build_lattice(H, W, 2, 1, 0, None, dev))
-lat_b = timed(lambda: crf._build_lattice(H, W, 5, 67, 3, image, dev))
-lb = crf._build_lattice(H, W, 5, 67, 3, image, dev)
-lg = crf._build_lattice(H, W, 2, 1, 0, None, dev)
+def build(d):
+    lat = crf._lattice_points(H, W, d, 1 if d == 2 else 67, 0 if d == 2 else 3, None if d == 2 else image, dev)
+    crf._norm(lat)
+    return lat
+
+
+lat_g = timed(lambda: build(2))
+lat_b = timed(lambda: build(5))
+lg, lb = build(2), build(5)
 print(f"lattice build: position {lat_g:.1f} ms (M = {lg.M}), bilateral {lat_b:.1f} ms (M = {lb.M}); pixels {H * W}")
 for it in (0, 1, 10):
     ms = timed(lambda: crf.mean_field(logp, image, it))

@@ -9,7 +9,7 @@ No CPU fallback: CUDA tensors only.
 """
 from __future__ import annotations
 
-from typing import Dict, Optional, Tuple
+from typing import Dict, Iterable, Optional, Tuple
 
 import torch
 import torch.nn.functional as F
@@ -23,11 +23,12 @@ Bi_W = 4
 Bi_XY_STD = 67
 Bi_RGB_STD = 3
 
-_LD = 32  # floats per pixel / lattice-point row (classes padded to a warp)
+_LD = 32  # floats per pixel / lattice-point row of one probe (classes padded to a warp)
 
 
 class _Lattice:
-    """One permutohedral lattice: per-pixel vertex ids + barycentric weights, neighbour tables, symmetric norm."""
+    """One permutohedral lattice: per-pixel vertex ids + barycentric weights, neighbour tables, CSR slot list,
+    symmetric norm."""
     __slots__ = ("d", "N", "M", "offset", "bary", "n1", "n2", "norm", "rowptr", "slots")
 
 
@@ -48,8 +49,10 @@ def _pack(coords: torch.Tensor, d: int, bits: int) -> torch.Tensor:
 
 def _lattice_points(H: int, W: int, d: int, sxy: float, srgb: float, image_u8: Optional[torch.Tensor], dev) -> _Lattice:
     """Lattice construction without the normalisation: the embedding of every pixel is a kernel; de-duplicating the
-    vertex keys and finding the blur neighbours are a sort and binary searches (torch.unique / searchsorted).  One host
-    sync, for the number of lattice points."""
+    vertex keys and finding the blur neighbours are a sort and binary searches (torch.unique / searchsorted).  The
+    (pixel, vertex) slots of every point form a CSR list: `slots` sorted by point, ascending slot index within a point
+    (a stable sort of the point ids), and `rowptr` [M + 1]; the gather splat sums them in that order.  One host sync,
+    for the number of lattice points."""
     lib = _lib.load()
     N = H * W
     keys = torch.empty(N, d + 1, dtype=torch.long, device=dev)
@@ -76,28 +79,67 @@ def _lattice_points(H: int, W: int, d: int, sxy: float, srgb: float, image_u8: O
     lat.offset = inv.reshape(N, d + 1).to(torch.int32).contiguous()
     lat.bary = bary
     lat.n1, lat.n2 = n1.contiguous(), n2.contiguous()
+    ids = lat.offset.reshape(-1)
+    order = torch.argsort(ids, stable=True)
+    lat.slots = order.to(torch.int32)
+    lat.rowptr = torch.searchsorted(ids[order], torch.arange(M + 1, dtype=torch.int32, device=dev)).to(torch.int32)
     return lat
 
 
-def _build_lattice(H: int, W: int, d: int, sxy: float, srgb: float, image_u8: Optional[torch.Tensor], dev) -> _Lattice:
-    """Lattice construction, once per image (the position-only lattice is cached per frame size by the caller):
-    `_lattice_points` and the symmetric normalisation."""
-    lib = _lib.load()
-    lat = _lattice_points(H, W, d, sxy, srgb, image_u8, dev)
-    N, M = lat.N, lat.M
-    # NORMALIZE_SYMMETRIC: norm = 1 / sqrt(K 1 + 1e-20), K 1 = slice(blur(splat(ones)))
-    values = torch.zeros(M + 1, _LD, dtype=torch.float32, device=dev)
-    tmp = torch.zeros(M + 1, _LD, dtype=torch.float32, device=dev)
-    _lib.check(lib.stego_crf_splat_blur(d, N, M, 1, _lib.ptr(lat.offset), _lib.ptr(lat.bary), 0, 0, _lib.ptr(lat.n1),
-                                        _lib.ptr(lat.n2), _lib.ptr(values), _lib.ptr(tmp), _lib.stream()), "stego_crf_splat_blur")
-    blurred = tmp if (d + 1) % 2 else values
-    lat.norm = torch.empty(N, dtype=torch.float32, device=dev)
-    _lib.check(lib.stego_crf_norm(d, N, _lib.ptr(lat.offset), _lib.ptr(lat.bary), _lib.ptr(blurred), _lib.ptr(lat.norm),
-                                  _lib.stream()), "stego_crf_norm")
-    return lat
+def _norm(lat: _Lattice) -> None:
+    """lat.norm, densecrf's NORMALIZE_SYMMETRIC factor 1 / sqrt(K 1 + 1e-20), by stego_crf_norm (a gather ones-splat)."""
+    dev = lat.offset.device
+    values = torch.empty(lat.M, dtype=torch.float32, device=dev)
+    tmp = torch.empty(lat.M, dtype=torch.float32, device=dev)
+    lat.norm = torch.empty(lat.N, dtype=torch.float32, device=dev)
+    _lib.check(_lib.load().stego_crf_norm(lat.d, lat.N, lat.M, _lib.ptr(lat.offset), _lib.ptr(lat.bary),
+                                          _lib.ptr(lat.rowptr), _lib.ptr(lat.slots), _lib.ptr(lat.n1), _lib.ptr(lat.n2),
+                                          _lib.ptr(values), _lib.ptr(tmp), _lib.ptr(lat.norm), _lib.stream()),
+               "stego_crf_norm")
 
 
-_POSITION_LATTICES: Dict[Tuple[int, int, float, int], _Lattice] = {}
+_POSITION_LATTICES: Dict[Tuple[int, int, int], _Lattice] = {}
+
+
+def _position_lattice(H: int, W: int, dev) -> _Lattice:
+    """The Gaussian kernel's lattice of an H x W frame with its normalisation, cached per frame size: it depends on
+    pixel positions only, so every frame of that size shares it."""
+    key = (H, W, dev.index)
+    if key not in _POSITION_LATTICES:
+        lat = _lattice_points(H, W, 2, POS_XY_STD, 0.0, None, dev)
+        _norm(lat)
+        _POSITION_LATTICES[key] = lat
+    return _POSITION_LATTICES[key]
+
+
+def _bilateral_lattice(images_u8: Iterable[torch.Tensor]) -> _Lattice:
+    """The bilateral lattices of B frames ([H, W, 3] uint8 each, prepare_image's layout), concatenated into one lattice
+    over the B*H*W pixels (point ids, neighbour tables and slots offset by each frame's base), with its normalisation.
+    One host sync per frame (the number of lattice points)."""
+    frames = []
+    for image in images_u8:
+        H, W = image.shape[:2]
+        frames.append(_lattice_points(H, W, 5, Bi_XY_STD, Bi_RGB_STD, image, image.device))
+    if len(frames) == 1:
+        out = frames[0]
+    else:
+        B, N, dev = len(frames), frames[0].N, frames[0].offset.device
+        bases, m = [], 0
+        for lat in frames:
+            bases.append(m)
+            m += lat.M
+        out = _Lattice()
+        out.d, out.N, out.M = 5, B * N, m
+        out.offset = torch.cat([lat.offset + base for lat, base in zip(frames, bases)])
+        out.bary = torch.cat([lat.bary for lat in frames])
+        out.n1, out.n2 = (torch.cat([torch.where(t >= 0, t + base, t) for t, base in zip(ts, bases)], 1).contiguous()
+                          for ts in ([lat.n1 for lat in frames], [lat.n2 for lat in frames]))
+        slots_per_frame = N * 6
+        out.slots = torch.cat([lat.slots + b * slots_per_frame for b, lat in enumerate(frames)])
+        out.rowptr = torch.cat([lat.rowptr[:-1] + b * slots_per_frame for b, lat in enumerate(frames)] +
+                               [torch.full((1,), B * slots_per_frame, dtype=torch.int32, device=dev)])
+    _norm(out)
+    return out
 
 
 _IMAGENET_STATS: Dict[torch.device, Tuple[torch.Tensor, torch.Tensor]] = {}
@@ -126,34 +168,26 @@ def mean_field(logits_full: torch.Tensor, image_u8: torch.Tensor, n_iter: int = 
         raise RuntimeError(f"stego_b200.crf: {C} classes unsupported (<= {_LD})")
     dev = logits_full.device
     N = H * W
-    key = (H, W, float(POS_XY_STD), dev.index)
-    if key not in _POSITION_LATTICES:
-        _POSITION_LATTICES[key] = _build_lattice(H, W, 2, POS_XY_STD, 0.0, None, dev)
-    lg = _POSITION_LATTICES[key]
-    lb = _build_lattice(H, W, 5, Bi_XY_STD, Bi_RGB_STD, image_u8, dev)
+    lg = _position_lattice(H, W, dev)
+    lb = _bilateral_lattice([image_u8])
     logits = logits_full.detach().float().contiguous()
     unary = torch.empty(N, _LD, dtype=torch.float32, device=dev)
     Q = torch.empty(N, _LD, dtype=torch.float32, device=dev)
     _lib.check(lib.stego_crf_unary(_lib.ptr(logits), _lib.ptr(unary), _lib.ptr(Q), N, C, _lib.stream()), "stego_crf_unary")
-    vg = torch.empty(2, lg.M + 1, _LD, dtype=torch.float32, device=dev)
-    vb = torch.empty(2, lb.M + 1, _LD, dtype=torch.float32, device=dev)
     q_out = torch.empty(C, H, W, dtype=torch.float32, device=dev)
     arg = torch.empty(H, W, dtype=torch.uint8, device=dev) if want_argmax else None
-    for it in range(n_iter):
-        vg.zero_()
-        vb.zero_()
-        _lib.check(lib.stego_crf_splat_blur(2, N, lg.M, C, _lib.ptr(lg.offset), _lib.ptr(lg.bary), _lib.ptr(lg.norm), _lib.ptr(Q),
-                                            _lib.ptr(lg.n1), _lib.ptr(lg.n2), _lib.ptr(vg[0]), _lib.ptr(vg[1]), _lib.stream()),
-                   "stego_crf_splat_blur")
-        _lib.check(lib.stego_crf_splat_blur(5, N, lb.M, C, _lib.ptr(lb.offset), _lib.ptr(lb.bary), _lib.ptr(lb.norm), _lib.ptr(Q),
-                                            _lib.ptr(lb.n1), _lib.ptr(lb.n2), _lib.ptr(vb[0]), _lib.ptr(vb[1]), _lib.stream()),
-                   "stego_crf_splat_blur")
-        last = it == n_iter - 1
-        _lib.check(lib.stego_crf_update(_lib.ptr(unary), _lib.ptr(lg.offset), _lib.ptr(lg.bary), _lib.ptr(vg[1]), _lib.ptr(lg.norm),
-                                        _lib.ptr(lb.offset), _lib.ptr(lb.bary), _lib.ptr(vb[0]), _lib.ptr(lb.norm), float(POS_W),
-                                        float(Bi_W), _lib.ptr(Q), _lib.ptr(q_out) if last else 0,
-                                        _lib.ptr(arg) if (last and want_argmax) else 0, N, C, _lib.stream()), "stego_crf_update")
-    if n_iter == 0:
+    if n_iter > 0:
+        vg = torch.empty(2, lg.M, _LD, dtype=torch.float32, device=dev)
+        vb = torch.empty(2, lb.M, _LD, dtype=torch.float32, device=dev)
+        _lib.check(lib.stego_crf_mean_field(
+            1, N, C, 0, n_iter, _lib.ptr(unary), _lib.ptr(Q),
+            _lib.ptr(lg.offset), _lib.ptr(lg.bary), _lib.ptr(lg.rowptr), _lib.ptr(lg.slots), _lib.ptr(lg.n1),
+            _lib.ptr(lg.n2), _lib.ptr(lg.norm), lg.M,
+            _lib.ptr(lb.offset), _lib.ptr(lb.bary), _lib.ptr(lb.rowptr), _lib.ptr(lb.slots), _lib.ptr(lb.n1),
+            _lib.ptr(lb.n2), _lib.ptr(lb.norm), lb.M, float(POS_W), float(Bi_W),
+            _lib.ptr(vg[0]), _lib.ptr(vg[1]), _lib.ptr(vb[0]), _lib.ptr(vb[1]), _lib.ptr(q_out), 0, _lib.ptr(arg), 0,
+            0, 0, 0, 0, 0, _lib.stream()), "stego_crf_mean_field")
+    else:
         q_out.copy_(Q[:, :C].t().reshape(C, H, W))
         if want_argmax:
             arg.copy_(q_out.argmax(0).to(torch.uint8))

@@ -10,11 +10,12 @@ At 1024x2048 the reference moves 587 MB (fp32 upsampled code) per image per prob
 the fused kernel reads the 9 MB low-res code and writes only the outputs (stego_eval_probes, eval_probes.cu).
 
 With `run_crf=True` the reference then runs the dense CRF on each probe's log-probabilities of every frame
-(eval_segmentation.py:133-141); `fused_eval_crf` is that whole loop body as one batched call (eval_crf.cu).
+(eval_segmentation.py:133-141); `fused_eval_crf` is that whole loop body as one batched call (crf.cu's mean field
+with both probes in one row).
 """
 from __future__ import annotations
 
-from typing import Dict, Optional, Sequence, Tuple
+from typing import Optional, Sequence
 
 import torch
 
@@ -94,75 +95,7 @@ def _probe_tables(linear_probe: torch.nn.Module, cluster_probe: torch.nn.Module,
 # ----------------------------------------------------------------------------------------------------------------------
 # CRF-refined evaluation
 # ----------------------------------------------------------------------------------------------------------------------
-_CRF_LD = 64  # eval_crf.cu: floats per pixel / lattice-point row (linear probe in [0, 32), cluster probe in [32, 64))
-_GATHER_POSITION_LATTICES: Dict[Tuple[int, int, int], "crf._Lattice"] = {}
-
-
-def _csr(lat) -> None:
-    """The (pixel, vertex) slots of every lattice point as a CSR list: `slots` sorted by point, ascending slot index
-    within a point (a stable sort of the point ids), and `rowptr` [M + 1]."""
-    ids = lat.offset.reshape(-1)
-    order = torch.argsort(ids, stable=True)
-    lat.slots = order.to(torch.int32)
-    lat.rowptr = torch.searchsorted(ids[order], torch.arange(lat.M + 1, dtype=torch.int32, device=ids.device)) \
-        .to(torch.int32)
-
-
-def _gather_norm(lat) -> None:
-    """lat.norm by stego_eval_crf_norm: the symmetric normalisation with gather splats (no float atomics)."""
-    dev = lat.offset.device
-    values = torch.empty(lat.M, dtype=torch.float32, device=dev)
-    tmp = torch.empty(lat.M, dtype=torch.float32, device=dev)
-    lat.norm = torch.empty(lat.N, dtype=torch.float32, device=dev)
-    _lib.check(_lib.load().stego_eval_crf_norm(lat.d, lat.N, lat.M, _lib.ptr(lat.offset), _lib.ptr(lat.bary),
-                                               _lib.ptr(lat.rowptr), _lib.ptr(lat.slots), _lib.ptr(lat.n1),
-                                               _lib.ptr(lat.n2), _lib.ptr(values), _lib.ptr(tmp), _lib.ptr(lat.norm),
-                                               _lib.stream()), "stego_eval_crf_norm")
-
-
-def _position_lattice(H: int, W: int, dev):
-    """The Gaussian kernel's lattice of an H x W frame with its CSR list and gather normalisation, cached per frame
-    size: it depends on pixel positions only, so every frame of every batch of that size shares it."""
-    key = (H, W, dev.index)
-    if key not in _GATHER_POSITION_LATTICES:
-        lat = crf._lattice_points(H, W, 2, crf.POS_XY_STD, 0.0, None, dev)
-        _csr(lat)
-        _gather_norm(lat)
-        _GATHER_POSITION_LATTICES[key] = lat
-    return _GATHER_POSITION_LATTICES[key]
-
-
-def _bilateral_lattice(img: torch.Tensor):
-    """The bilateral lattices of the B frames of img [B, 3, H, W], concatenated into one lattice over the B*H*W pixels
-    (point ids, neighbour tables and slots offset by each frame's base), with its gather normalisation.  One host sync
-    per frame (the number of lattice points)."""
-    B, _, H, W = img.shape
-    dev = img.device
-    N = H * W
-    frames = []
-    for b in range(B):
-        lat = crf._lattice_points(H, W, 5, crf.Bi_XY_STD, crf.Bi_RGB_STD, crf.prepare_image(img[b]), dev)
-        _csr(lat)
-        frames.append(lat)
-    if B == 1:
-        out = frames[0]
-    else:
-        bases, m = [], 0
-        for lat in frames:
-            bases.append(m)
-            m += lat.M
-        out = crf._Lattice()
-        out.d, out.N, out.M = 5, B * N, m
-        out.offset = torch.cat([lat.offset + base for lat, base in zip(frames, bases)])
-        out.bary = torch.cat([lat.bary for lat in frames])
-        out.n1, out.n2 = (torch.cat([torch.where(t >= 0, t + base, t) for t, base in zip(ts, bases)], 1).contiguous()
-                          for ts in ([lat.n1 for lat in frames], [lat.n2 for lat in frames]))
-        slots_per_frame = N * 6
-        out.slots = torch.cat([lat.slots + b * slots_per_frame for b, lat in enumerate(frames)])
-        out.rowptr = torch.cat([lat.rowptr[:-1] + b * slots_per_frame for b, lat in enumerate(frames)] +
-                               [torch.full((1,), B * slots_per_frame, dtype=torch.int32, device=dev)])
-    _gather_norm(out)
-    return out
+_CRF_LD = 64  # crf.cu rows of two probes: linear probe in [0, 32), cluster probe in [32, 64)
 
 
 _LABEL_DTYPES = (torch.uint8, torch.int32, torch.int64)
@@ -244,8 +177,8 @@ def fused_eval_crf(code: torch.Tensor, linear_probe: torch.nn.Module, cluster_pr
     _lib.check(lib.stego_eval_crf_unary(_lib.ptr(x), _lib.ptr(xf), ld, C, B, h, w, H, W, _lib.ptr(wl), _lib.ptr(bl), n_lin,
                                         _lib.ptr(cl), n_clu, float(alpha), _lib.ptr(scratch), _lib.ptr(unary), _lib.ptr(Q),
                                         _lib.stream()), "stego_eval_crf_unary")
-    lg = _position_lattice(H, W, dev)
-    lb = _bilateral_lattice(img.detach())
+    lg = crf._position_lattice(H, W, dev)
+    lb = crf._bilateral_lattice(crf.prepare_image(frame) for frame in img.detach())
     val_g = torch.empty(2, B * lg.M, _CRF_LD, dtype=torch.float32, device=dev)
     val_b = torch.empty(2, lb.M, _CRF_LD, dtype=torch.float32, device=dev)
     lin_pred = torch.empty(B, H, W, dtype=torch.uint8, device=dev)
@@ -253,7 +186,7 @@ def fused_eval_crf(code: torch.Tensor, linear_probe: torch.nn.Module, cluster_pr
     lin_q = torch.empty(B, n_lin, H, W, dtype=torch.float32, device=dev) if want_marginals else None
     clu_q = torch.empty(B, n_clu, H, W, dtype=torch.float32, device=dev) if want_marginals else None
     lab, lab_bytes = (None, 0) if label is None else ops.probe_label(label, B, H, W)
-    _lib.check(lib.stego_eval_crf_mean_field(
+    _lib.check(lib.stego_crf_mean_field(
         B, N, n_lin, n_clu, crf.MAX_ITER, _lib.ptr(unary), _lib.ptr(Q),
         _lib.ptr(lg.offset), _lib.ptr(lg.bary), _lib.ptr(lg.rowptr), _lib.ptr(lg.slots), _lib.ptr(lg.n1), _lib.ptr(lg.n2),
         _lib.ptr(lg.norm), lg.M,
@@ -261,7 +194,7 @@ def fused_eval_crf(code: torch.Tensor, linear_probe: torch.nn.Module, cluster_pr
         _lib.ptr(lb.norm), lb.M, float(crf.POS_W), float(crf.Bi_W),
         _lib.ptr(val_g[0]), _lib.ptr(val_g[1]), _lib.ptr(val_b[0]), _lib.ptr(val_b[1]), _lib.ptr(lin_q), _lib.ptr(clu_q),
         _lib.ptr(lin_pred), _lib.ptr(clu_pred), _lib.ptr(lab), lab_bytes, n_lin if label is not None else 0,
-        _lib.ptr(linear_confusion), _lib.ptr(cluster_confusion), _lib.stream()), "stego_eval_crf_mean_field")
+        _lib.ptr(linear_confusion), _lib.ptr(cluster_confusion), _lib.stream()), "stego_crf_mean_field")
     if want_marginals:
         return lin_pred, clu_pred, lin_q, clu_q
     return lin_pred, clu_pred

@@ -1,5 +1,5 @@
-"""fp64 references of the dense CRF (csrc/crf.cu through stego_b200/crf.py, csrc/eval_crf.cu through
-stego_b200/eval.py::fused_eval_crf), shared by the CRF tests.
+"""fp64 references of the dense CRF (csrc/crf.cu through stego_b200/crf.py and stego_b200/eval.py::fused_eval_crf),
+shared by the CRF tests.
 
 Plain, vectorised torch (no Python loop over pixels or lattice points), device-agnostic: the GPU tests run these in
 float64 on the device at the c4 frame, the CPU test pins them to the fp32 restatement oracle/crf_oracle.py.  The
@@ -12,7 +12,7 @@ blur stencil, slice scale and NORMALIZE_SYMMETRIC kernels, Potts mean field):
                   bary >= 0 and sum_r bary_r = 1.
   lattice_tables  unique points, offsets, the 2(d+1) neighbour tables and the stable-sorted CSR list, from full vertex
                   tuples packed in a mixed radix over the observed coordinate range (not crf._pack's fixed-width fields);
-                  `concat` is the B-frame concatenation of eval._bilateral_lattice.
+                  `concat` is the B-frame concatenation of crf._bilateral_lattice.
   filter          splat, d+1 blur passes and slice on a given lattice, with the magnitude and error-propagation
                   vectors of the fp32 bars (derived in tests/test_crf_fp64_gpu.py).
   norm, unary_from_logits, update, mean_field.
@@ -171,7 +171,7 @@ def lattice_tables(verts):
 
 
 def concat(tables):
-    """eval._bilateral_lattice's concatenation of B frames' tables: point ids, neighbours (-1 kept) and slots offset
+    """crf._bilateral_lattice's concatenation of B frames' tables: point ids, neighbours (-1 kept) and slots offset
     by each frame's base.  Returns the concatenated dict and the bases [B]."""
     Ms = torch.tensor([t["M"] for t in tables])
     bases = torch.cat([torch.zeros(1, dtype=torch.long), Ms.cumsum(0)[:-1]])

@@ -1,6 +1,6 @@
 """The dense CRF against the float64 references of tests/_crf_fp64.py, stage by stage and elementwise: csrc/crf.cu
-(stego_b200.crf: dense_crf / batched_crf) and csrc/eval_crf.cu (stego_b200.eval.fused_eval_crf), at the c4 frame
-(1024 x 2048, 27 classes), the reference eval batch (16 x 320^2, n_lin != n_clu) and small edge frames.
+with one probe per row (stego_b200.crf: dense_crf / batched_crf) and with two (stego_b200.eval.fused_eval_crf), at
+the c4 frame (1024 x 2048, 27 classes), the reference eval batch (16 x 320^2, n_lin != n_clu) and small edge frames.
 
 Bars (u = 2^-24, gamma_k = k u / (1 - k u)):
   embedding    elevated: the features x * fp32(1 / sxy) (two roundings), the scale factors (five) and their product
@@ -15,7 +15,7 @@ Bars (u = 2^-24, gamma_k = k u / (1 - k u)):
                weight is the difference of two residuals / (d+1)): it cannot be relative, the residuals cancel
                |elevated|.
   tables       exact: M, offsets, both neighbour tables, the CSR list and the per-frame bases of the concatenation.
-  splat        gamma_{m_i + 1} sum |b v| over the m_i slots of point i (atomics: any order).
+  splat        gamma_{m_i + 1} sum |b v| over the m_i slots of point i (summed in CSR order; the bar holds for any).
   blur pass    err' = blur(err) (1 + gamma_2) + gamma_2 blur(magnitudes)   (two roundings of old + 0.5 (a + b)).
   norm         half the relative error of the slice (propagated blur error + gamma_{d+4} of its |terms|) plus the
                correctly rounded sqrt and divide.
@@ -152,8 +152,7 @@ def _tables_equal(lat, t):
     assert lat.M == t["M"]
     assert torch.equal(lat.offset.long(), t["offset"])
     assert torch.equal(lat.n1.long(), t["n1"]) and torch.equal(lat.n2.long(), t["n2"])
-    if getattr(lat, "slots", None) is not None:
-        assert torch.equal(lat.slots.long(), t["slots"]) and torch.equal(lat.rowptr.long(), t["rowptr"])
+    assert torch.equal(lat.slots.long(), t["slots"]) and torch.equal(lat.rowptr.long(), t["rowptr"])
     for j in range(t["d"] + 1):
         has = lat.n1[j] >= 0
         i = torch.arange(lat.M, device=lat.n1.device)[has]
@@ -168,15 +167,14 @@ TABLES = [("pos_c4", 1, 1024, 2048, 2, None), ("bil_c4_noise", 1, 1024, 2048, 5,
 
 
 @pytest.mark.parametrize("name,B,H,W,d,kind", TABLES, ids=[t[0] for t in TABLES])
-def test_lattice_tables(cuda_dev, name, B, H, W, d, kind):
-    """crf._lattice_points, eval._csr and eval._bilateral_lattice's concatenation equal the tables rebuilt from the
-    kernel's keys with an independent packing."""
-    from stego_b200 import crf, eval as ev
+def test_crf_lattice_tables(cuda_dev, name, B, H, W, d, kind):
+    """crf._lattice_points (with its CSR list) and crf._bilateral_lattice's concatenation equal the tables rebuilt from
+    the kernel's keys with an independent packing."""
+    from stego_b200 import crf
     if d == 2:
         keys, _ = _kernel_keys(H, W, 2, None, cuda_dev)
         t = R.lattice_tables(R.unpack(keys, 2, 30))
         lat = crf._lattice_points(H, W, 2, R.POS_XY_STD, 0.0, None, cuda_dev)
-        ev._csr(lat)
         _tables_equal(lat, t)
         return
     kinds = [kind] * B if kind else list(R.IMAGES)[:B]
@@ -189,11 +187,10 @@ def test_lattice_tables(cuda_dev, name, B, H, W, d, kind):
         per.append(R.lattice_tables(R.unpack(keys, 5, 12)))
         if b == 0:
             lat = crf._lattice_points(H, W, 5, R.BI_XY_STD, R.BI_RGB_STD, imgs[b], cuda_dev)
-            ev._csr(lat)
             _tables_equal(lat, per[0])
         del keys
     want, bases = R.concat(per)
-    got = ev._bilateral_lattice(x)
+    got = crf._bilateral_lattice(crf.prepare_image(f) for f in x)
     _tables_equal(got, want)
     print(f"{name}: M per frame {[p['M'] for p in per]}, N {H * W}, bases {bases.tolist()}")
 
@@ -216,52 +213,24 @@ FILTER = [("c4_piecewise", 1024, 2048, "piecewise", 27), ("320_noise", 320, 320,
           ("1x1", 1, 1, "noise", 5)]
 
 
-@pytest.mark.parametrize("name,H,W,kind,C", FILTER, ids=[f[0] for f in FILTER])
-def test_filter_atomic(cuda_dev, name, H, W, kind, C):
-    """stego_crf_splat_blur and stego_crf_norm (crf.cu) on the kernel's own lattices"""
-    from stego_b200 import crf
-    L = _lib()
-    lib = L.load()
-    img = R.image(kind, H, W, seed=H * W).to(cuda_dev)
-    rat = Ratios()
-    for d in (2, 5):
-        lat = crf._build_lattice(H, W, d, _sxy(d), R.BI_RGB_STD, img if d == 5 else None, cuda_dev)
-        l64 = _lat64(lat)
-        n, nb = R.norm(l64, bars=True)
-        rat.add(f"norm_d{d}", (lat.norm.double() - n).abs(), nb["bar"])
-        Q = torch.zeros(H * W, LD, device=cuda_dev)
-        Q[:, :C] = _probs(H * W, C, H + C, cuda_dev)
-        vals = torch.zeros(2, lat.M + 1, LD, device=cuda_dev)
-        L.check(lib.stego_crf_splat_blur(d, H * W, lat.M, C, L.ptr(lat.offset), L.ptr(lat.bary), L.ptr(lat.norm),
-                                         L.ptr(Q), L.ptr(lat.n1), L.ptr(lat.n2), L.ptr(vals[0]), L.ptr(vals[1]),
-                                         L.stream()), "stego_crf_splat_blur")
-        f = R.filter(l64, lat.norm.double()[:, None] * Q[:, :C].double(), bars=True)
-        got = vals[1 if d == 2 else 0, 1:, :C].double()
-        rat.add(f"blurred_d{d}", (got - f["passes"][-1]).abs(), f["err"][-1])
-        assert (vals[:, 1:, C:] == 0).all() and (vals[:, 0] == 0).all()
-        del lat, l64, f, vals, Q
-    print(f"{name}: {dict(rat)}")
-    rat.check(f"crf_filter_atomic_{name}")
-
-
-def _call_eval_norm(lat, dev):
+def _call_norm(lat, dev):
     L = _lib()
     v = torch.full((2, lat.M), float("nan"), device=dev)
     out = torch.empty(lat.N, device=dev)
-    L.check(L.load().stego_eval_crf_norm(lat.d, lat.N, lat.M, L.ptr(lat.offset), L.ptr(lat.bary), L.ptr(lat.rowptr),
-                                         L.ptr(lat.slots), L.ptr(lat.n1), L.ptr(lat.n2), L.ptr(v[0]), L.ptr(v[1]),
-                                         L.ptr(out), L.stream()), "stego_eval_crf_norm")
+    L.check(L.load().stego_crf_norm(lat.d, lat.N, lat.M, L.ptr(lat.offset), L.ptr(lat.bary), L.ptr(lat.rowptr),
+                                    L.ptr(lat.slots), L.ptr(lat.n1), L.ptr(lat.n2), L.ptr(v[0]), L.ptr(v[1]), L.ptr(out),
+                                    L.stream()), "stego_crf_norm")
     return v, out
 
 
-def _eval_setup(B, H, W, kinds, dev, seed=0):
-    """the gather path's lattices for B frames and the fp64 views of them: the position lattice repeated B times and
-    the concatenated bilateral lattice, both over B*N pixels"""
-    from stego_b200 import eval as ev
+def _setup(B, H, W, kinds, dev, seed=0):
+    """crf.py's lattices for B frames and the fp64 views of them: the position lattice repeated B times and the
+    concatenated bilateral lattice, both over B*N pixels"""
+    from stego_b200 import crf
     imgs = torch.stack([R.image(k, H, W, seed=seed + 7 * b) for b, k in enumerate(kinds)])
     x = R.normalised(imgs).to(dev)
-    lg = ev._position_lattice(H, W, dev)
-    lb = ev._bilateral_lattice(x)
+    lg = crf._position_lattice(H, W, dev)
+    lb = crf._bilateral_lattice(crf.prepare_image(f) for f in x)
     g1 = _lat64(lg)
     t = dict(d=2, N=H * W, M=lg.M, offset=g1["offset"], n1=g1["n1"], n2=g1["n2"], rowptr=lg.rowptr.long(),
              slots=lg.slots.long(), counts=g1["counts"])
@@ -270,21 +239,45 @@ def _eval_setup(B, H, W, kinds, dev, seed=0):
     return x, lg, lb, g64, _lat64(lb)
 
 
-def _call_eval_mf(B, N, n_lin, n_clu, n_iter, unary, Q, lg, lb, dev):
+def _call_mf(B, N, n_lin, n_clu, n_iter, unary, Q, lg, lb, dev):
+    """stego_crf_mean_field; n_clu = 0: one probe, rows of 32 floats (else 64)"""
     L = _lib()
-    vg = torch.full((2, B * lg.M, 64), float("nan"), device=dev)
-    vb = torch.full((2, lb.M, 64), float("nan"), device=dev)
+    ld = 64 if n_clu else LD
+    vg = torch.full((2, B * lg.M, ld), float("nan"), device=dev)
+    vb = torch.full((2, lb.M, ld), float("nan"), device=dev)
     lq = torch.empty(B, n_lin, N, device=dev)
-    cq = torch.empty(B, n_clu, N, device=dev)
+    cq = torch.empty(B, n_clu, N, device=dev) if n_clu else None
     lp = torch.empty(B, N, dtype=torch.uint8, device=dev)
-    cp = torch.empty(B, N, dtype=torch.uint8, device=dev)
+    cp = torch.empty(B, N, dtype=torch.uint8, device=dev) if n_clu else None
     p = L.ptr
-    L.check(L.load().stego_eval_crf_mean_field(
+    L.check(L.load().stego_crf_mean_field(
         B, N, n_lin, n_clu, n_iter, p(unary), p(Q), p(lg.offset), p(lg.bary), p(lg.rowptr), p(lg.slots), p(lg.n1),
         p(lg.n2), p(lg.norm), lg.M, p(lb.offset), p(lb.bary), p(lb.rowptr), p(lb.slots), p(lb.n1), p(lb.n2),
         p(lb.norm), lb.M, R.POS_W, R.BI_W, p(vg[0]), p(vg[1]), p(vb[0]), p(vb[1]), p(lq), p(cq), p(lp), p(cp), 0, 0, 0,
-        0, 0, L.stream()), "stego_eval_crf_mean_field")
+        0, 0, L.stream()), "stego_crf_mean_field")
     return vg, vb, lq, cq, lp, cp
+
+
+@pytest.mark.parametrize("name,H,W,kind,C", FILTER, ids=[f[0] for f in FILTER])
+def test_filter_one_probe(cuda_dev, name, H, W, kind, C):
+    """dense_crf's rows of 32 floats: the normalisation of both of its lattices (stego_crf_norm) and the last two blur
+    passes of each left in the scratch of stego_crf_mean_field(n_clu = 0, n_iter = 1)"""
+    N = H * W
+    _, lg, lb, g64, b64 = _setup(1, H, W, [kind], cuda_dev, seed=N)
+    rat = Ratios()
+    Q = torch.zeros(N, LD, device=cuda_dev)
+    Q[:, :C] = _probs(N, C, H + C, cuda_dev)
+    vg, vb, *_ = _call_mf(1, N, C, 0, 1, torch.zeros(N, LD, device=cuda_dev), Q, lg, lb, cuda_dev)
+    for lat, l64, v, last, tag in ((lg, g64, vg, 1, "d2"), (lb, b64, vb, 0, "d5")):
+        n, nb = R.norm(l64, bars=True)
+        rat.add(f"norm_{tag}", (lat.norm.double() - n).abs(), nb["bar"])
+        f = R.filter(l64, lat.norm.double()[:, None] * Q[:, :C].double(), bars=True)
+        rat.add(f"blurred_{tag}", (v[last, :, :C].double() - f["passes"][-1]).abs(), f["err"][-1])
+        rat.add(f"blurred_prev_{tag}", (v[1 - last, :, :C].double() - f["passes"][-2]).abs(), f["err"][-2])
+        assert (v[:, :, C:] == 0).all(), tag
+        del f
+    print(f"{name}: {dict(rat)}")
+    rat.check(f"crf_filter_one_probe_{name}")
 
 
 def _check_q(rat, tag, q, arg, ref, n):
@@ -308,15 +301,15 @@ EVAL_FILTER = [("320_piecewise_x16", 16, 320, 320, "piecewise", 27, 32), ("320_n
 
 
 @pytest.mark.parametrize("name,B,H,W,kind,n_lin,n_clu", EVAL_FILTER, ids=[e[0] for e in EVAL_FILTER])
-def test_filter_gather_and_update(cuda_dev, name, B, H, W, kind, n_lin, n_clu):
-    """stego_eval_crf_norm's scratch and norm, and stego_eval_crf_mean_field(n_iter=1): the last two blur passes of
-    both lattices left in val_g / tmp_g / val_b / tmp_b, the updated marginals and the argmax maps"""
+def test_filter_and_update_two_probes(cuda_dev, name, B, H, W, kind, n_lin, n_clu):
+    """stego_crf_norm's scratch and norm, and stego_crf_mean_field(n_iter=1) with two probes: the last two blur passes
+    of both lattices left in val_g / tmp_g / val_b / tmp_b, the updated marginals and the argmax maps"""
     N = H * W
     kinds = [kind] * B if kind else list(R.IMAGES)[:B]
-    x, lg, lb, g64, b64 = _eval_setup(B, H, W, kinds, cuda_dev, seed=N)
+    x, lg, lb, g64, b64 = _setup(B, H, W, kinds, cuda_dev, seed=N)
     rat = Ratios()
     for lat, l64, tag in ((lg, _lat64(lg), "g"), (lb, b64, "b")):
-        v, nrm = _call_eval_norm(lat, cuda_dev)
+        v, nrm = _call_norm(lat, cuda_dev)
         n, nb = R.norm(l64, bars=True)
         f = nb["filter"]
         last = 1 if lat.d == 2 else 0
@@ -331,7 +324,7 @@ def test_filter_gather_and_update(cuda_dev, name, B, H, W, kind, n_lin, n_clu):
         Q[:, lo:lo + n] = torch.softmax(torch.randn(B * N, n, generator=g) * 2, 1)
         unary[:, lo:lo + n] = R.unary_from_logits(torch.randn(B * N, n, generator=g) * 3)[0].float()
     Q, unary = Q.to(cuda_dev), unary.to(cuda_dev)
-    vg, vb, lq, cq, lp, cp = _call_eval_mf(B, N, n_lin, n_clu, 1, unary, Q.clone(), lg, lb, cuda_dev)
+    vg, vb, lq, cq, lp, cp = _call_mf(B, N, n_lin, n_clu, 1, unary, Q.clone(), lg, lb, cuda_dev)
     ng, nbn = lg.norm.double().repeat(B), lb.norm.double()
     # position values [B][Mg][64] of the B frames = one lattice over B*N pixels; passes 2 and 3 / 5 and 6 remain
     on = torch.zeros(64, dtype=torch.bool, device=cuda_dev)
@@ -376,9 +369,10 @@ def _q0_bar(Q32, U32, n):
 
 
 @pytest.mark.parametrize("name,H,W,kind,C,unary", UPDATE, ids=[u[0] for u in UPDATE])
-def test_update_from_fp64_chain(cuda_dev, name, H, W, kind, C, unary):
+def test_update_one_and_two_probes_from_fp64_chain(cuda_dev, name, H, W, kind, C, unary):
     """crf_unary_kernel and Q_0, then for k = 0..9: Q_k of the fp64 chain rounded to fp32 through one iteration of
-    stego_crf_splat_blur + stego_crf_update and of stego_eval_crf_mean_field(n_iter=1)"""
+    stego_crf_mean_field(n_iter=1) with one probe (dense_crf's rows of 32) and with two carrying the same classes
+    (fused_eval_crf's rows of 64); both give the same bits"""
     from stego_b200 import crf
     L = _lib()
     lib = L.load()
@@ -394,48 +388,28 @@ def test_update_from_fp64_chain(cuda_dev, name, H, W, kind, C, unary):
     assert (Ut[:, C:] == 0).all() and (Q0[:, C:] == 0).all()
     if unary == "uniform":
         assert (Q0[:, :C] == Q0[:, :1]).all() and (Ut[:, :C] == Ut[:, :1]).all()
-    lg = crf._build_lattice(H, W, 2, R.POS_XY_STD, 0.0, None, cuda_dev)
-    lb = crf._build_lattice(H, W, 5, R.BI_XY_STD, R.BI_RGB_STD, img, cuda_dev)
+    lg = crf._position_lattice(H, W, cuda_dev)
+    lb = crf._bilateral_lattice([img])
     g64, b64 = _lat64(lg), _lat64(lb)
     U32 = Ut[:, :C]
     seq = R.mean_field(U32, g64, b64, R.MAX_ITER, record=True)
-    # the gather path on the same frame: its own lattices, both probes carrying the same classes
-    from stego_b200 import eval as ev
-    x = R.normalised(img.cpu()[None]).to(cuda_dev)
-    eg, eb = ev._position_lattice(H, W, cuda_dev), ev._bilateral_lattice(x)
-    eg64, eb64 = _lat64(eg), _lat64(eb)
     eU = torch.zeros(N, 64, device=cuda_dev)
     eU[:, :C] = U32
     eU[:, 32:32 + C] = U32
-    vals_g = torch.empty(2, lg.M + 1, LD, device=cuda_dev)
-    vals_b = torch.empty(2, lb.M + 1, LD, device=cuda_dev)
     for k in range(R.MAX_ITER):
         Qk = torch.zeros(N, LD, device=cuda_dev)
         Qk[:, :C] = seq[k].float()
-        vals_g.zero_()
-        vals_b.zero_()
-        for lat, v in ((lg, vals_g), (lb, vals_b)):
-            L.check(lib.stego_crf_splat_blur(lat.d, N, lat.M, C, L.ptr(lat.offset), L.ptr(lat.bary), L.ptr(lat.norm),
-                                             L.ptr(Qk), L.ptr(lat.n1), L.ptr(lat.n2), L.ptr(v[0]), L.ptr(v[1]),
-                                             L.stream()), "stego_crf_splat_blur")
-        q_out = torch.empty(C, N, device=cuda_dev)
-        arg = torch.empty(N, dtype=torch.uint8, device=cuda_dev)
-        L.check(lib.stego_crf_update(L.ptr(Ut), L.ptr(lg.offset), L.ptr(lg.bary), L.ptr(vals_g[1]), L.ptr(lg.norm),
-                                     L.ptr(lb.offset), L.ptr(lb.bary), L.ptr(vals_b[0]), L.ptr(lb.norm), R.POS_W, R.BI_W,
-                                     L.ptr(Qk), L.ptr(q_out), L.ptr(arg), N, C, L.stream()), "stego_crf_update")
+        _, _, q1, _, a1, _ = _call_mf(1, N, C, 0, 1, Ut, Qk, lg, lb, cuda_dev)
         ref = R.update(U32, seq[k], g64, b64, lg.norm, lb.norm, bars=True)
-        _check_q(rat, "atomic", q_out.t(), arg, ref, C)
-        assert torch.equal(Qk[:, :C], q_out.t()) and (Qk[:, C:] == 0).all()
+        _check_q(rat, "one_probe", q1[0].t(), a1[0], ref, C)
         eQ = torch.zeros(N, 64, device=cuda_dev)
         eQ[:, :C] = seq[k].float()
         eQ[:, 32:32 + C] = seq[k].float()
-        _, _, lq, cq, lp, cp = _call_eval_mf(1, N, C, C, 1, eU, eQ, eg, eb, cuda_dev)
-        eref = R.update(U32, seq[k], eg64, eb64, eg.norm, eb.norm, bars=True)
-        _check_q(rat, "gather", lq[0].t(), lp[0], eref, C)
+        _, _, lq, cq, lp, cp = _call_mf(1, N, C, C, 1, eU, eQ, lg, lb, cuda_dev)
         assert torch.equal(lq, cq) and torch.equal(lp, cp)
+        assert torch.equal(q1, lq) and torch.equal(a1, lp)
         if unary == "uniform":
-            for q, a in ((q_out.t(), arg), (lq[0].t(), lp[0])):
-                assert (q == q[:, :1]).all() and (a == 0).all(), k
+            assert (q1 == q1[:, :1]).all() and (a1 == 0).all(), k
     print(f"{name}: {dict(rat)}")
     rat.check(f"crf_update_{name}")
 
@@ -508,7 +482,7 @@ CHAIN = [("c4", 1, 1024, 2048, "piecewise", 27, 27), ("320_x16", 16, 320, 320, "
 
 
 @pytest.mark.parametrize("name,B,H,W,kind,n_lin,n_clu", CHAIN, ids=[c[0] for c in CHAIN])
-def test_chain(cuda_dev, name, B, H, W, kind, n_lin, n_clu):
+def test_mean_field_chain(cuda_dev, name, B, H, W, kind, n_lin, n_clu):
     """crf.mean_field (dense_crf's ten iterations) per frame and fused_eval_crf for the batch against the fp64 chain
     on the same lattices (fp64 normalisation, fp64 unaries from the logits / from the probe table's unary)"""
     from stego_b200 import crf, eval as ev
@@ -516,8 +490,8 @@ def test_chain(cuda_dev, name, B, H, W, kind, n_lin, n_clu):
     kinds = [kind] * B
     imgs = torch.stack([R.image(k, H, W, seed=N + 7 * b) for b, k in enumerate(kinds)])
     rat = {}
-    # crf.cu: one frame at a time, class scores given at full resolution
-    lg = crf._build_lattice(H, W, 2, R.POS_XY_STD, 0.0, None, cuda_dev)
+    # dense_crf: one frame at a time, class scores given at full resolution
+    lg = crf._position_lattice(H, W, cuda_dev)
     g64 = _lat64(lg)
     for b in range(min(B, 2)):
         img = imgs[b].to(cuda_dev)
@@ -529,7 +503,7 @@ def test_chain(cuda_dev, name, B, H, W, kind, n_lin, n_clu):
         rat["dense_crf"] = max(rat.get("dense_crf", 0.0), _chain_check(f"{name} dense_crf frame {b}", got, want))
         assert torch.equal(arg.reshape(-1).long(), got.argmax(1))
         del q, want, got, lb
-    # eval_crf.cu: the batch in one call, from a low-resolution code
+    # fused_eval_crf: the batch in one call, from a low-resolution code
     from stego_b200.modules import ClusterLookup
     g = torch.Generator().manual_seed(N)
     C, h, w = 24, max(1, H // 8), max(1, W // 8)
@@ -552,7 +526,7 @@ def test_chain(cuda_dev, name, B, H, W, kind, n_lin, n_clu):
     L.check(L.load().stego_eval_crf_unary(L.ptr(xc), L.ptr(xf), ld, C, B, h, w, H, W, L.ptr(wl), L.ptr(bl), n_lin,
                                           L.ptr(cl), n_clu, 2.0, L.ptr(scratch), L.ptr(unary), L.ptr(Q), L.stream()),
               "stego_eval_crf_unary")
-    _, elg, elb, eg64, eb64 = _eval_setup(B, H, W, kinds, cuda_dev, seed=N)
+    _, elg, elb, eg64, eb64 = _setup(B, H, W, kinds, cuda_dev, seed=N)
     for lo, n, q, p, tag in ((0, n_lin, lq, lp, "lin"), (32, n_clu, cq, cp, "clu")):
         want = R.mean_field(unary[:, lo:lo + n], eg64, eb64)
         got = q.permute(0, 2, 3, 1).reshape(B * N, n)

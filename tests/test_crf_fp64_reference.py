@@ -80,7 +80,8 @@ def test_embedding_identities(name, H, W, d, sxy, kind):
 @pytest.mark.parametrize("d,kind", [(2, None), (5, "noise"), (5, "piecewise")])
 def test_tables_match_fixed_width_packing(d, kind):
     """The mixed-radix numbering is the order of stego_b200.crf's sorted fixed-width keys, neighbours included, and
-    the CSR list is the stable sort eval._csr makes; the concatenation matches eval._bilateral_lattice's bases."""
+    the CSR list is the stable sort crf._lattice_points makes; the concatenation matches crf._bilateral_lattice's
+    bases."""
     from stego_b200 import crf
     H, W = 23, 31
     _, f64, _ = _frame(H, W, d, 1.0 if d == 2 else 7.0, kind, seed=3)

@@ -46,7 +46,7 @@ def test_dense_crf_matches_oracle(cuda_dev, H, W, C, h, w):
     assert (want.argmax(0) != up.argmax(0).numpy()).mean() > 0.01
 
 
-def test_lattices_match_oracle(cuda_dev):
+def test_crf_lattices_match_oracle(cuda_dev):
     """Lattice construction (vertex de-duplication, barycentric weights, symmetric normalisation) for both kernels."""
     import crf_oracle as CO
     from stego_b200 import crf
@@ -57,7 +57,7 @@ def test_lattices_match_oracle(cuda_dev):
     assert (image_dev.cpu().numpy() == image).all()
     for d, feat in ((2, CO.gaussian_features(H, W, 1.0)), (5, CO.bilateral_features(image, 67.0, 3.0))):
         ok = CO.DenseKernel(feat)
-        lat = crf._build_lattice(H, W, d, 1.0 if d == 2 else 67.0, 0.0 if d == 2 else 3.0, image_dev if d == 5 else None, cuda_dev)
+        lat = crf._position_lattice(H, W, cuda_dev) if d == 2 else crf._bilateral_lattice([image_dev])
         assert lat.M == ok.lattice.M
         assert np.abs(lat.bary.cpu().numpy() - ok.lattice.bary).max() < 1e-4
         assert np.abs(lat.norm.cpu().numpy() / ok.norm - 1).max() < 1e-4
@@ -82,3 +82,16 @@ def test_batched_crf_full_frame_properties(cuda_dev):
     assert (q.sum(1) - 1).abs().max().item() < 1e-4
     assert torch.isfinite(q).all()
     assert (q.argmax(1) == logp.argmax(1)).float().mean().item() > 0.5
+
+
+def test_dense_crf_is_reproducible(cuda_dev):
+    """Two calls on the same input give bit-identical marginals and labels: every splat sums its lattice point's slots
+    in a fixed order (no float atomics).  A noise frame, so the bilateral lattice has many points with several slots."""
+    from stego_b200 import crf
+    H, W, C = 320, 320, 27
+    g = torch.Generator().manual_seed(11)
+    img = torch.randn(3, H, W, generator=g).to(cuda_dev)
+    logits = (torch.randn(C, 40, 40, generator=g) * 3).to(cuda_dev)
+    q1, a1 = crf.dense_crf(img, logits, want_argmax=True)
+    q2, a2 = crf.dense_crf(img, logits, want_argmax=True)
+    assert torch.equal(q1, q2) and torch.equal(a1, a2)

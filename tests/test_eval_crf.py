@@ -65,17 +65,21 @@ def test_other_shapes_are_refused():
     _refused(ValueError, "img", img=torch.randn(2, 4, 12, 16))
 
 
-def test_entry_points_declared_and_checking_arguments():
+def test_crf_entry_points_declared_and_checking_arguments():
     protos = _lib.header_prototypes()
-    for name in ("stego_eval_crf_unary", "stego_eval_crf_norm", "stego_eval_crf_mean_field"):
+    for name in ("stego_eval_crf_unary", "stego_crf_norm", "stego_crf_mean_field"):
         assert name in protos
     lib = _lib.load()
     n0 = _lib.launch_count()
     rc = lib.stego_eval_crf_unary(0, 0, 8, 8, 1, 2, 2, 4, 4, 0, 0, 5, 0, 5, 2.0, 0, 0, 0, 0)
     assert rc == -1 and "null pointer" in _lib.last_error()
-    rc = lib.stego_eval_crf_norm(3, 16, 4, *([0] * 9), 0)
+    rc = lib.stego_crf_norm(3, 16, 4, *([0] * 9), 0)
     assert rc == -1 and "bad args" in _lib.last_error()
-    rc = lib.stego_eval_crf_mean_field(1, 16, 33, 5, 10, *([0] * 9), 8, *([0] * 7), 8, 3.0, 4.0, *([0] * 9), 0, 0, 0,
-                                       0, 0)
-    assert rc == -1 and "unsupported" in _lib.last_error()
+    for n_lin, n_clu in ((33, 5), (5, 33), (5, -1)):
+        rc = lib.stego_crf_mean_field(1, 16, n_lin, n_clu, 10, *([0] * 9), 8, *([0] * 7), 8, 3.0, 4.0, *([0] * 9), 0, 0,
+                                      0, 0, 0)
+        assert rc == -1 and "unsupported" in _lib.last_error()
+    # one probe (n_clu = 0) passes the limits and stops at the missing buffers
+    rc = lib.stego_crf_mean_field(1, 16, 5, 0, 10, *([0] * 9), 8, *([0] * 7), 8, 3.0, 4.0, *([0] * 9), 0, 0, 0, 0, 0)
+    assert rc == -1 and "null pointer" in _lib.last_error()
     assert _lib.launch_count() == n0

@@ -1,4 +1,4 @@
-"""CRF-refined evaluation (stego_b200.eval.fused_eval_crf; csrc/eval_crf.cu, eval_crf_unary_kernel in
+"""CRF-refined evaluation (stego_b200.eval.fused_eval_crf; csrc/crf.cu, eval_crf_unary_kernel in
 csrc/eval_probes.cu) against
 
   * the CPU chain: the fp64 flip-TTA / upsampling / probes of tests/_probes_fp64.py, then the CPU restatement of the
