@@ -84,6 +84,11 @@ STEGO_API int stego_layernorm_bf16(const float* x, const float* gamma, const flo
  * [B][ntok][E] residual stream -> out fp32 [B][E] (+=; zero it first) = mean over the ntok-1 patch tokens of LayerNorm(x). */
 STEGO_API int stego_layernorm_gap(const float* x, const float* gamma, const float* beta, float* out, int B, int ntok,
                                   int E, float eps, void* stream);
+/* out fp32 [B][N] = x fp32 [B][K] . w^T + bias, w bf16 rows [N] at stride ldw (>= K, a multiple of 8), bias fp32 [N]
+ * or null; K a multiple of 8, x and w 16-byte aligned.  The key projection of the pooled LN1 outputs of the last block:
+ * the "KK" kNN descriptors (mean over patches of the keys, src/modules.py:98-101 + src/precompute_knns.py:19). */
+STEGO_API int stego_linear_rows_f32(const float* x, const void* w_bf16, int ldw, const float* bias, float* out, int B,
+                                    int N, int K, void* stream);
 /* Attention.forward (:78-90) without the projections: softmax(q k^T / sqrt(64)) v, fused (flash-style) on
  * wgmma; qkv [B][N][3E] bf16 packed q|k|v with heads contiguous inside each third, out [B][N][E] bf16. */
 STEGO_API int stego_attention_fwd(const void* qkv, void* out, int B, int N, int E, int heads, void* stream);

@@ -182,6 +182,39 @@ layernorm_gap_kernel(const float* __restrict__ x, const float* __restrict__ gamm
   }
 }
 
+// ---------------------------------------------------------------------------------------------
+// out[b][n] = x[b] . w[n] + bias[n]: fp32 rows against bf16 weight rows, one warp per output element, 16-byte loads of
+// 8 weights (and the 8 matching fp32 inputs) per lane, fp32 accumulation.  Used for the "KK" kNN descriptors: the mean
+// of the last block's keys is the key projection of the mean of its LN1 outputs (the projection is linear), so the
+// [B, hw, E] key map is never written.  Tiny (B x E x E): latency-bound, no shared memory.
+// ---------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256)
+linear_rows_f32_kernel(const float* __restrict__ x, const bf16* __restrict__ w, int ldw, const float* __restrict__ bias,
+                       float* __restrict__ out, int B, int N, int K) {
+  const long long o = 1ll * blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (o >= 1ll * B * N) return;
+  const int lane = threadIdx.x & 31;
+  const int b = static_cast<int>(o / N), n = static_cast<int>(o % N);
+  const float4* xr = reinterpret_cast<const float4*>(x + 1ll * b * K);
+  const uint4* wr = reinterpret_cast<const uint4*>(w + 1ll * n * ldw);
+  float acc = 0.f;
+  for (int c = lane; c < K / 8; c += 32) {
+    const uint4 wv = __ldg(wr + c);
+    const float4 x0 = __ldg(xr + 2 * c), x1 = __ldg(xr + 2 * c + 1);
+    const bf16* wb = reinterpret_cast<const bf16*>(&wv);
+    acc = fmaf(x0.x, __bfloat162float(wb[0]), acc);
+    acc = fmaf(x0.y, __bfloat162float(wb[1]), acc);
+    acc = fmaf(x0.z, __bfloat162float(wb[2]), acc);
+    acc = fmaf(x0.w, __bfloat162float(wb[3]), acc);
+    acc = fmaf(x1.x, __bfloat162float(wb[4]), acc);
+    acc = fmaf(x1.y, __bfloat162float(wb[5]), acc);
+    acc = fmaf(x1.z, __bfloat162float(wb[6]), acc);
+    acc = fmaf(x1.w, __bfloat162float(wb[7]), acc);
+  }
+  acc = warp_sum(acc);
+  if (lane == 0) out[o] = acc + (bias ? bias[n] : 0.f);
+}
+
 }  // namespace stego
 
 using namespace stego;
@@ -266,5 +299,25 @@ extern "C" int stego_layernorm_gap(const float* x, const float* gamma, const flo
       return STEGO_ERR_UNSUPPORTED;
   }
   STEGO_CHECK_LAUNCH("layernorm_gap_kernel");
+  return STEGO_OK;
+}
+
+// out fp32 [B][N] = x fp32 [B][K] . w bf16 [N][ldw]^T (+ bias fp32 [N]).
+extern "C" int stego_linear_rows_f32(const float* x, const void* w_bf16, int ldw, const float* bias, float* out, int B,
+                                     int N, int K, void* stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  STEGO_CHECK_ARG(x && w_bf16 && out, "stego_linear_rows_f32: null pointer");
+  STEGO_CHECK_ARG(B > 0 && N > 0 && K > 0 && K % 8 == 0, "stego_linear_rows_f32: bad sizes B=%d N=%d K=%d (K a multiple of 8)",
+                  B, N, K);
+  STEGO_CHECK_ARG(ldw >= K && ldw % 8 == 0, "stego_linear_rows_f32: ldw=%d (>= K, a multiple of 8)", ldw);
+  STEGO_CHECK_ARG((reinterpret_cast<uintptr_t>(x) & 15u) == 0 && (reinterpret_cast<uintptr_t>(w_bf16) & 15u) == 0,
+                  "stego_linear_rows_f32: x and w must be 16-byte aligned");
+  const long long outputs = 1ll * B * N;
+  const int warps = 8;
+  const long long blocks = (outputs + warps - 1) / warps;
+  STEGO_CHECK_ARG(blocks <= 0x7fffffffll, "stego_linear_rows_f32: B*N=%lld too large", outputs);
+  linear_rows_f32_kernel<<<static_cast<unsigned>(blocks), warps * 32, 0, stream>>>(
+      x, reinterpret_cast<const bf16*>(w_bf16), ldw, bias, out, B, N, K);
+  STEGO_CHECK_LAUNCH("linear_rows_f32_kernel");
   return STEGO_OK;
 }

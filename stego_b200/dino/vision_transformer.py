@@ -180,11 +180,12 @@ class VisionTransformer(nn.Module):
     # the kernel sequence
     # ------------------------------------------------------------------------------------------
     @torch.no_grad()
-    def forward_tokens(self, img: torch.Tensor, want_qkv: bool = False, taps: Optional["BlockTaps"] = None
-                       ) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
+    def forward_tokens(self, img: torch.Tensor, want_qkv: bool = False, taps: Optional["BlockTaps"] = None,
+                       stop_before_last: bool = False) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
         """Returns (x, qkv_last): x = fp32 residual stream [B*N, E] after the last block (before the
         final norm); qkv_last = packed bf16 [B*N, 3E] of the last block if requested.  `taps` collects values of
-        the last taps.n blocks (see BlockTaps); the block outputs are computed the same way with or without it."""
+        the last taps.n blocks (see BlockTaps); the block outputs are computed the same way with or without it.
+        stop_before_last: run blocks 0 .. depth-2 only; x is then the residual stream entering the last block."""
         if not img.is_cuda:
             raise RuntimeError("stego_b200: the DINO ViT forward only exists as sm_90a kernels (no CPU fallback)")
         w = self._prepared()
@@ -208,7 +209,7 @@ class VisionTransformer(nn.Module):
         Hd = hid.shape[1]
         blocks = w["blocks"]
         depth = len(blocks)
-        for i, bw in enumerate(blocks):
+        for i, bw in enumerate(blocks[:-1] if stop_before_last else blocks):
             tap = taps is not None and depth - i <= taps.n
             ops.layernorm(x, bw["n1w"], bw["n1b"], y, eps=bw["eps1"])
             ops.gemm(y, bw["qkv_w"], qkv, M=B * N, N=3 * E, K=E, bias=bw["qkv_b"])
@@ -236,27 +237,44 @@ class VisionTransformer(nn.Module):
         use_graph=True replays the whole kernel sequence (~110 launches) as ONE CUDA graph captured per input
         shape (the backbone is frozen and RNG-free).  The result then lives in a static buffer that the next
         replay overwrites: only for callers that consume it before calling again (the fused training step)."""
+        return self._tokens(img, use_graph, "feat")
+
+    @torch.no_grad()
+    def key_features(self, img: torch.Tensor, use_graph: bool = False) -> torch.Tensor:
+        """The last block's keys with the cls token dropped, tokens-major bf16 [B, hw, E], channels head-major
+        (head * 64 + d) — dino_feat_type "KK" of src/modules.py:98-101.  Blocks 0 .. depth-2 run as in patch_features;
+        the last block stops after LN1 and the key third of its qkv GEMM (no attention, proj, MLP or final norm).
+        The bits are those of the K third of the full block's packed qkv: the same LN1 rows, and the GEMM reads the
+        key rows of the packed weight (and bias) in place, with the same K loop per output element.
+        use_graph as in patch_features (a graph of its own per input shape)."""
+        return self._tokens(img, use_graph, "KK")
+
+    def _tokens(self, img, use_graph: bool, kind: str) -> torch.Tensor:
         if use_graph and (img[0] if isinstance(img, (list, tuple)) else img).is_cuda:
-            return self._graphed_patch_features(img)
+            return self._graphed(img, kind)
         if isinstance(img, (list, tuple)):
             img = torch.cat(list(img), 0)
-        return self._patch_features_eager(img)
+        return self._eager(img, kind)
 
-    def _graphed_patch_features(self, img) -> torch.Tensor:
+    def _eager(self, img: torch.Tensor, kind: str) -> torch.Tensor:
+        return self._patch_features_eager(img) if kind == "feat" else self._key_features_eager(img)
+
+    def _graphed(self, img, kind: str) -> torch.Tensor:
         """`img` may be a list of image batches: they are copied into consecutive slices of the graph's static
-        input (the fused step passes [img, img_pos] — no torch.cat of the two 19 MB batches)."""
+        input (the fused step passes [img, img_pos] — no torch.cat of the two 19 MB batches).  One graph per
+        (feature kind, input shape, device, dtype)."""
         from .. import _lib
         self._prepared()
         graphs = self._cache.setdefault("graphs", {})
         parts = list(img) if isinstance(img, (list, tuple)) else [img]
         shape = (sum(p.shape[0] for p in parts),) + tuple(parts[0].shape[1:])
         dt = torch.bfloat16 if all(p.dtype == torch.bfloat16 for p in parts) else torch.float32
-        key = (shape, parts[0].device.index, dt)
+        key = (kind, shape, parts[0].device.index, dt)
         if key not in graphs:
             img = torch.cat([p.to(dt) for p in parts], 0) if len(parts) > 1 else parts[0].to(dt)
-            self._patch_features_eager(img)  # warm-up: kernel attributes, pos-embed cache, allocator
+            self._eager(img, kind)  # warm-up: kernel attributes, pos-embed cache, allocator
             static_in = img.detach().contiguous().clone()
-            graphs[key] = (_lib.Graph(lambda: self._patch_features_eager(static_in)), static_in)
+            graphs[key] = (_lib.Graph(lambda: self._eager(static_in, kind)), static_in)
         g, static_in = graphs[key]
         off = 0
         for part in parts:
@@ -274,6 +292,17 @@ class VisionTransformer(nn.Module):
         ops.layernorm(x, w["nw"], w["nb"], out, eps=self.norm.eps, drop_cls_ntok=N)
         return out.view(B, N - 1, self.embed_dim)
 
+    def _key_features_eager(self, img: torch.Tensor) -> torch.Tensor:
+        B, E = img.shape[0], self.embed_dim
+        x, _ = self.forward_tokens(img, stop_before_last=True)
+        bw = self._prepared()["blocks"][-1]
+        N = x.shape[0] // B
+        y = torch.empty(B * (N - 1), E, dtype=torch.bfloat16, device=x.device)
+        ops.layernorm(x, bw["n1w"], bw["n1b"], y, eps=bw["eps1"], drop_cls_ntok=N)
+        out = torch.empty(B * (N - 1), E, dtype=torch.bfloat16, device=x.device)
+        ops.gemm(y, bw["qkv_w"][E:2 * E], out, M=B * (N - 1), N=E, K=E, bias=bw["qkv_b"][E:2 * E])
+        return out.view(B, N - 1, E)
+
     @torch.no_grad()
     def pooled_patch_features(self, img: torch.Tensor) -> torch.Tensor:
         """mean over the patch tokens of norm(last block) — `DinoFeaturizer(img)[0].mean([2, 3])` of
@@ -288,6 +317,23 @@ class VisionTransformer(nn.Module):
                                                    x.shape[0] // B, self.embed_dim, float(self.norm.eps), _lib.stream()),
                    "stego_layernorm_gap")
         return out
+
+    @torch.no_grad()
+    def pooled_key_features(self, img: torch.Tensor) -> torch.Tensor:
+        """mean over the patch tokens of the last block's keys — `DinoFeaturizer(img)[0].mean([2, 3])` with
+        dino_feat_type "KK" — fp32 [B, E].  The key projection is linear, so the mean of the keys is
+        mean_t LN1(x_t) . W_k^T + b_k: LN1 of the last block fused with the pooling (stego_layernorm_gap on the residual
+        stream entering that block), then one small projection (stego_linear_rows_f32) with the bf16 key weights the
+        key_features GEMM reads.  The [B, hw, E] key map is never written."""
+        from .. import _lib
+        B, E = img.shape[0], self.embed_dim
+        x, _ = self.forward_tokens(img, stop_before_last=True)
+        bw = self._prepared()["blocks"][-1]
+        pooled = torch.zeros(B, E, dtype=torch.float32, device=x.device)
+        lib = _lib.load()
+        _lib.check(lib.stego_layernorm_gap(_lib.ptr(x), _lib.ptr(bw["n1w"]), _lib.ptr(bw["n1b"]), _lib.ptr(pooled), B,
+                                           x.shape[0] // B, E, float(bw["eps1"]), _lib.stream()), "stego_layernorm_gap")
+        return ops.linear_rows_f32(pooled, bw["qkv_w"][E:2 * E], bw["qkv_b"][E:2 * E])
 
     def _all_tokens(self, img: torch.Tensor, want_qkv: bool = False):
         x, qkv = self.forward_tokens(img, want_qkv)

@@ -52,7 +52,7 @@ class FusedStep:
         return (img.is_cuda and seg.training and seg.net.training and cfg.correspondence_weight > 0
                 and not cfg.use_salience and seg.net.proj_type is not None
                 and cfg.rec_weight == 0 and cfg.aug_alignment_weight == 0 and cfg.crf_weight == 0
-                and cfg.neg_samples >= 1 and cfg.dino_feat_type == "feat"
+                and cfg.neg_samples >= 1 and cfg.dino_feat_type in ("feat", "KK")
                 and seg.linear_probe.weight.shape[0] <= 32 and seg.net.dim <= 96
                 and batch["label"].dtype in ops.LABEL_BYTES
                 and (not cfg.use_true_labels or (batch.get("label_pos") is not None and seg.n_classes <= 255

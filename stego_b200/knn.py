@@ -28,15 +28,21 @@ def knn_topk(feats: torch.Tensor, k: int = 30, return_values: bool = False
 
 
 def knn_descriptors(net, img: torch.Tensor) -> torch.Tensor:
-    """`model.forward(img).mean([2, 3])` of precompute_knns.py:19 for a `DinoFeaturizer` (feat_type "feat"), un-normalised
-    fp32 [B, E]: frozen ViT -> final LayerNorm + global average pool in one kernel.  In training mode with cfg.dropout the
+    """`model.forward(img).mean([2, 3])` of precompute_knns.py:19 for a `DinoFeaturizer`, un-normalised fp32 [B, E]:
+    frozen ViT -> global average pool of the teacher features the config selects, without writing the feature map —
+    "feat": final LayerNorm + pooling in one kernel; "KK": the last block's LN1 + pooling, then the key projection of the
+    pooled row (the mean of the keys, the projection being linear).  In training mode with cfg.dropout the
     reference's returned features carry the third Dropout2d mask (src/modules.py:115-116 — precompute_knns.py never calls
     .eval()); a per-(image, channel) scale commutes with the spatial mean, so the same noise tensors are drawn (all three,
     to keep the RNG stream of `net(img)`) and the last one is applied to the pooled vector."""
-    if net.feat_type != "feat":
-        raise RuntimeError("stego_b200.knn_descriptors: dino_feat_type 'feat' only")
+    if net.feat_type == "feat":
+        pool = net.model.pooled_patch_features
+    elif net.feat_type == "KK":
+        pool = net.model.pooled_key_features
+    else:
+        raise ValueError("Unknown feat type:{}".format(net.feat_type))
     net.model.eval()
-    pooled = net.model.pooled_patch_features(img)
+    pooled = pool(img)
     _, _, m3 = net.draw_masks(img.shape[0], img.device)
     if net.cfg.dropout and m3 is not None:
         pooled = pooled * m3

@@ -280,13 +280,19 @@ class DinoFeaturizer(nn.Module):
 
     # ---- fused internals -------------------------------------------------------------------------
     def backbone_tokens(self, img: torch.Tensor, use_graph: bool = False) -> torch.Tensor:
-        """Frozen ViT -> bf16 tokens-major features [B, hw, E] (cls dropped).  use_graph: replay the kernel
-        sequence as one CUDA graph (result is a static buffer valid until the next call)."""
+        """Frozen ViT -> bf16 tokens-major teacher features [B, hw, E] (cls dropped): the final-norm tokens for
+        dino_feat_type "feat", the last block's keys (head-major channels) for "KK" — the tensor forward() returns
+        as image_feat, which both training paths feed to the head and the correspondence loss.  use_graph: replay the
+        kernel sequence as one CUDA graph (result is a static buffer valid until the next call)."""
         self.model.eval()
         first = img[0] if isinstance(img, (list, tuple)) else img  # a list of batches is concatenated on the fly
         assert first.shape[2] % self.patch_size == 0
         assert first.shape[3] % self.patch_size == 0
-        return self.model.patch_features(img, use_graph=use_graph)
+        if self.feat_type == "feat":
+            return self.model.patch_features(img, use_graph=use_graph)
+        if self.feat_type == "KK":
+            return self.model.key_features(img, use_graph=use_graph)
+        raise ValueError("Unknown feat type:{}".format(self.feat_type))
 
     def draw_masks(self, batch: int, device):
         """Dropout2d noises in the reference's call order: cluster1 input, cluster2 input, returned feats."""
@@ -340,8 +346,11 @@ class DinoFeaturizer(nn.Module):
                 else:
                     tok = self.model.final_norm(self.model.block_taps(img, n).x[0], B)[:, 1:].contiguous()
             elif self.feat_type == "KK":
-                qkv = self.model.block_taps(img, n).qkv[0]  # packed bf16 [B*N, 3E]: k is the middle third
-                tok = qkv.view(B, fh * fw + 1, 3, -1)[:, 1:, 1].contiguous()  # [B, hw, heads*64], head-major
+                if n == 1:
+                    tok = self.model.key_features(img)  # [B, hw, heads*64] bf16, head-major; the last block stops at k
+                else:
+                    qkv = self.model.block_taps(img, n).qkv[0]  # packed bf16 [B*N, 3E]: k is the middle third
+                    tok = qkv.view(B, fh * fw + 1, 3, -1)[:, 1:, 1].contiguous()  # [B, hw, heads*64], head-major
             else:
                 raise ValueError("Unknown feat type:{}".format(self.feat_type))
         E = tok.shape[-1]

@@ -95,6 +95,22 @@ def layernorm(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, out: tor
     return out
 
 
+def linear_rows_f32(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """fp32 [B, K] . bf16 [N, K]^T (+ fp32 bias [N]) -> new fp32 [B, N] (stego_linear_rows_f32).  w may be a row slice
+    of a larger weight (inner dimension contiguous)."""
+    _lib.require_cuda(x, w, bias)
+    assert x.dtype == torch.float32 and x.dim() == 2 and x.is_contiguous()
+    assert w.dtype == torch.bfloat16 and w.dim() == 2 and w.stride(1) == 1 and w.shape[1] == x.shape[1]
+    if bias is not None:
+        assert bias.dtype == torch.float32 and bias.is_contiguous() and bias.numel() == w.shape[0]
+    B, K = x.shape
+    N = w.shape[0]
+    out = torch.empty(B, N, dtype=torch.float32, device=x.device)
+    _lib.check(_lib.load().stego_linear_rows_f32(_lib.ptr(x), _lib.ptr(w), w.stride(0), _lib.ptr(bias), _lib.ptr(out),
+                                                 B, N, K, _lib.stream()), "stego_linear_rows_f32")
+    return out
+
+
 def attention(qkv: torch.Tensor, out: torch.Tensor, B: int, N: int, E: int, heads: int) -> torch.Tensor:
     """Fused softmax(q k^T / 8) v on wgmma (stego_attention_fwd). qkv [B*N, 3E] bf16, out [B*N, E] bf16."""
     _lib.require_cuda(qkv, out)
