@@ -335,9 +335,13 @@ STEGO_API int stego_eval_probes(const float* code, const float* code_flip, long 
  *   normed = F.normalize(feats, dim=1);  sims = einsum("nf,mf->nm", normed, normed);  idx = topk(sims, k)[1]
  * fused: the [n][n] similarity matrix is never materialised (wgmma tiles in registers, bf16 hi/lo split = 3 passes,
  * per-row running top-k in the epilogue).  feats: fp32 [n][E] (un-normalised, e.g. GAP-pooled ViT features),
- * E a multiple of 64, 1 <= k <= 32.  planes_scratch: 2*n*E bf16 (16-byte aligned).  idx_out: int64 [n][k], sorted by
- * descending similarity (ties: lower index first; a row is its own nearest neighbour, as in the reference);
- * val_out: optional fp32 [n][k] similarities.
+ * E a multiple of 64, 1 <= k <= min(32, n).  planes_scratch: 2*n*E bf16 (16-byte aligned).  idx_out: int64 [n][k]:
+ * column 0 is the row's own index, always (the reference's loader, src/data.py:524, draws from columns 1..k as "not the
+ * image itself"; the similarity alone would not guarantee it: an exact duplicate ties with the row and a near duplicate's
+ * computed similarity can exceed the row's own 1 - O(2^-17); an all-zero row ties with everything at 0); columns 1..k-1
+ * are the other rows by (similarity descending, index ascending).
+ * val_out: optional fp32 [n][k] computed similarities of those indices (column 0: the row with itself, so columns
+ * 1..k-1 are non-increasing and column 1 may exceed column 0 by rounding).
  * ---------------------------------------------------------------------------------------------- */
 STEGO_API int stego_knn_topk(const float* feats, int n, int E, int k, void* planes_scratch, long long* idx_out,
                              float* val_out, void* stream);

@@ -10,11 +10,16 @@
 // private list, compared against a register threshold (an insert happens ~k ln(n/k) times per row, everything else
 // is one FSETP per similarity).  The two lists of a row are merged once per row block.
 //
+// Order of a row's k neighbours: the row itself first, whatever its computed self-similarity (the data loader reads
+// columns 1..k as "not the image itself", and an exact or near duplicate can reach or exceed the 1 - O(2^-17) the
+// three passes give the diagonal), then (similarity descending, index ascending).  The diagonal element is replaced by
+// +inf in the staged tile, so the scan and the merge need no special case; its computed value is reported.
+//
 //   knn_prep_kernel   : fp32 [n][E] -> L2-normalise (eps 1e-12 like F.normalize) -> bf16 hi / lo planes [2][n][E]
 //   knn_topk_kernel   : persistent CTAs, one 128-row query block at a time against all 128-column key tiles
 //       warpgroups 0,1  wgmma for query rows 0..63 / 64..127: 3 passes (hi.hi, hi.lo, lo.hi) x E/64 k-blocks per tile,
-//                       then the scan of those rows; after the last tile the row's k indices (descending similarity,
-//                       ties -> lower index first) are written as int64
+//                       then the scan of those rows; after the last tile the row's k indices (itself, then descending
+//                       similarity, ties -> lower index first) are written as int64
 //       warpgroup 2     TMA producer (A = query rows, B = key rows, both from the same planes tensor, 3-stage ring)
 #include "common.cuh"
 #include "host_util.h"
@@ -28,7 +33,9 @@ constexpr uint32_t KNN_STAGE_BYTES = KNN_A_BYTES + KNN_B_BYTES;
 constexpr int KNN_ST_LD = KNN_BM + 4;                   // transposed score tile [key col][query row], padded
 constexpr uint32_t KNN_ST_BYTES = KNN_BN * KNN_ST_LD * 4;
 constexpr uint32_t KNN_MERGE_BYTES = KNN_BM * KNN_MAXK * 8;  // second-half lists: [row][k] value + index
-constexpr size_t KNN_SMEM = size_t(KNN_STAGES) * KNN_STAGE_BYTES + KNN_ST_BYTES + KNN_MERGE_BYTES + 1024 + 256;
+constexpr uint32_t KNN_SELF_BYTES = KNN_BM * 4;               // computed self-similarity of every query row
+constexpr size_t KNN_SMEM =
+    size_t(KNN_STAGES) * KNN_STAGE_BYTES + KNN_ST_BYTES + KNN_MERGE_BYTES + KNN_SELF_BYTES + 1024 + 256;
 
 struct KnnParams {
   int n, E, k;
@@ -62,7 +69,8 @@ knn_topk_kernel(const __grid_constant__ CUtensorMap tmF, KnnParams p) {
   float* st = reinterpret_cast<float*>(smem + KNN_STAGES * KNN_STAGE_BYTES);
   float* merge_v = reinterpret_cast<float*>(smem + KNN_STAGES * KNN_STAGE_BYTES + KNN_ST_BYTES);
   int* merge_i = reinterpret_cast<int*>(merge_v + KNN_BM * KNN_MAXK);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + KNN_STAGES * KNN_STAGE_BYTES + KNN_ST_BYTES + KNN_MERGE_BYTES);
+  float* self_v = reinterpret_cast<float*>(merge_i + KNN_BM * KNN_MAXK);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(self_v + KNN_BM);
   uint64_t* empty_bar = full_bar + KNN_STAGES;
 
   const int warp = threadIdx.x >> 5;
@@ -158,6 +166,10 @@ knn_topk_kernel(const __grid_constant__ CUtensorMap tmF, KnnParams p) {
         st[col * KNN_ST_LD + r] = acc[t];
       }
       asm volatile("bar.sync %0, 128;\n" ::"r"(1 + mwg) : "memory");
+      if (ct == rb && half == mwg) {  // the diagonal sits in this thread's half: key column srow of the tile
+        self_v[srow] = st[srow * KNN_ST_LD + srow];
+        st[srow * KNN_ST_LD + srow] = INFINITY;
+      }
       const int col0 = ct * KNN_BN + half * 64;
 #pragma unroll 1
       for (int c = 0; c < 64; c += 32) {
@@ -183,7 +195,8 @@ knn_topk_kernel(const __grid_constant__ CUtensorMap tmF, KnnParams p) {
         }
       }
     }
-    // merge the two half lists of every row: (value desc, index asc), the order a single scan would produce
+    // merge the two half lists of every row: (value desc, index asc), the order a single scan would produce; the row
+    // itself (+inf) comes out first and takes its computed similarity back
     if (half == 1) {
       for (int i = 0; i < k; ++i) {
         merge_v[srow * KNN_MAXK + i] = tv[i];
@@ -198,7 +211,7 @@ knn_topk_kernel(const __grid_constant__ CUtensorMap tmF, KnnParams p) {
         const float vb = merge_v[srow * KNN_MAXK + ib];
         const int xb = merge_i[srow * KNN_MAXK + ib];
         const bool take_a = tv[ia] > vb || (tv[ia] == vb && ti[ia] >= 0 && (xb < 0 || ti[ia] < xb));
-        const float v = take_a ? tv[ia] : vb;
+        const float v = i == 0 ? self_v[srow] : (take_a ? tv[ia] : vb);
         const int x = take_a ? ti[ia] : xb;
         if (take_a) ++ia; else ++ib;
         p.idx_out[static_cast<size_t>(row) * k + i] = x;

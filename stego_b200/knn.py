@@ -12,8 +12,10 @@ from . import _lib
 def knn_topk(feats: torch.Tensor, k: int = 30, return_values: bool = False
              ) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
     """feats: [n, E] fp32 CUDA (un-normalised descriptors, e.g. `model(img).mean([2, 3])`, precompute_knns.py:19).
-    Returns int64 [n, k] neighbour indices by descending cosine similarity (each row contains itself, like the
-    reference's `torch.topk(einsum("nf,mf->nm", ...), 30)[1]`), and the similarities if requested."""
+    Returns int64 [n, k] neighbour indices of the reference's `torch.topk(einsum("nf,mf->nm", ...), 30)[1]` with the
+    order pinned: column 0 is the row's own index, always (also next to exact or near duplicates and for an all-zero
+    row — src/data.py:524 reads columns 1..k as "not the image itself"), columns 1..k-1 the other rows by (cosine
+    similarity descending, index ascending); and the fp32 similarities of those indices if requested."""
     _lib.require_cuda(feats)
     if feats.dim() != 2 or feats.dtype != torch.float32:
         raise RuntimeError("stego_b200.knn_topk: feats must be a 2-D fp32 tensor")

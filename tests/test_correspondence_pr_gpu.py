@@ -282,12 +282,12 @@ def test_correspondence_pr_step(cuda_dev):
     dev = cuda_dev
     steps = [make_batch(8, 224, dev, seed=20 + i) for i in range(2)]
     val = make_batch(8, 224, dev, seed=60)
-    runs = {}
-    for name in ("plain", "plain_again", "with_pr"):
+
+    def run(with_pr):
         model, _ = make_model("vit_small", dev, fused=True, seed=0)
         torch.manual_seed(777)
         losses = [model.training_step(steps[0], 0).item()]
-        if name == "with_pr":
+        if with_pr:
             fused = model._fused
             graph, key = fused.ws.graph, fused.key
             before = _train_state(model, dev)
@@ -321,14 +321,29 @@ def test_correspondence_pr_step(cuda_dev):
             assert int(metric.counts.sum()) == 2 * 8 * fs ** 4
             torch.cuda.set_rng_state(before["cuda_rng"], dev)  # the next step draws what it would have drawn
         losses.append(model.training_step(steps[1], 1).item())
-        runs[name] = (losses, _train_state(model, dev))
-    ref, again, pr = runs["plain"], runs["plain_again"], runs["with_pr"]
-    noise = max(float((ref[1][k].double() - again[1][k].double()).abs().max())
-                for k in ("param", "exp_avg", "exp_avg_sq"))
-    diff = max(float((ref[1][k].double() - pr[1][k].double()).abs().max()) for k in ("param", "exp_avg", "exp_avg_sq"))
-    print(f"run-to-run {noise:.3e}, with correspondence_pr_step {diff:.3e}")
+        return losses, _train_state(model, dev)
+
+    def dist(a, b):
+        return max(float((a[1][k].double() - b[1][k].double()).abs().max()) for k in ("param", "exp_avg", "exp_avg_sq"))
+
+    # The step's fp32 atomics make identical runs differ in the last bits, and the largest difference over the state
+    # takes few distinct values, some rare (1e-7, 6e-7 and 2e-6 have been seen on unchanged code): one pair of plain
+    # runs is too small a sample of the spread to hold the run with correspondence_pr_step to 4x of it.  The spread is
+    # the largest distance among the plain runs; while it does not cover that run, more plain runs are drawn, up to
+    # 16.  A step that left another RNG state behind would change every coordinate and dropout draw of the next one,
+    # which no number of plain runs reproduces.
+    plain = [run(False) for _ in range(2)]
+    pr = run(True)
+    while True:
+        noise = max(dist(a, b) for i, a in enumerate(plain) for b in plain[i + 1:])
+        diff = max(dist(a, pr) for a in plain)
+        if diff <= 4 * noise or len(plain) == 16:
+            break
+        plain.append(run(False))
+    print(f"run-to-run {noise:.3e} over {len(plain)} plain runs, with correspondence_pr_step {diff:.3e}")
+    ref = plain[0]
     assert torch.equal(ref[1]["cuda_rng"], pr[1]["cuda_rng"])
-    if noise == 0 and ref[0] == again[0]:
+    if noise == 0 and all(a[0] == ref[0] for a in plain):
         assert ref[0] == pr[0] and diff == 0
     else:
         assert diff <= 4 * noise

@@ -28,7 +28,7 @@ def test_knn_topk_matches_oracle(cuda_dev, n, E, k):
     idx, val = knn_topk(feats.to(cuda_dev), k, return_values=True)
     idx, val = idx.cpu(), val.cpu().double()
     assert idx.shape == (n, k) and idx.dtype == torch.long
-    assert (idx[:, 0] == torch.arange(n)).all()                              # a row is its own nearest neighbour
+    assert (idx[:, 0] == torch.arange(n)).all()                              # column 0 is the row itself, by contract
     assert (val[:, :-1] >= val[:, 1:]).all()                                 # sorted by descending similarity
     assert (val - want_val).abs().max().item() < 2e-5                        # the k best similarities, in order
     true_sims = (normed.double() @ normed.double().t()).gather(1, idx)       # returned indices really have those sims
