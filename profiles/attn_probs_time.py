@@ -11,43 +11,19 @@ Q K^T (2 x 2 B h N^2 64 FLOP) take under a quarter of that at the data-sheet bf1
 scale and again for the softmax: 20 B h N^2 bytes, five times the kernel's.
 """
 import argparse
-import json
 import os
-import subprocess
 import sys
 
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from _measure import card, emit, window_ms  # noqa: E402
 
 PEAK_TFLOPS, PEAK_TBS = 989.0, 3.35
 # config: (arch, batch, resolution, tokens N = (res / 8)^2 + 1, heads)
 CONFIGS = {"c1": ("vit_small", 32, 224, 785, 6), "c2": ("vit_base", 32, 320, 1601, 12),
            "c3": ("vit_base", 16, 448, 3137, 12)}
-
-
-def gpu_info():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader,nounits"],
-                       capture_output=True, text=True).stdout.strip().splitlines()[0]
-    name, plim, clk = [x.strip() for x in q.split(",")]
-    return dict(gpu=name, power_limit_w=float(plim), max_sm_clock_mhz=int(float(clk)))
-
-
-def time_ms(fn, min_window_s=0.5):
-    fn()
-    torch.cuda.synchronize()
-    s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    s.record()
-    fn()
-    e.record()
-    e.synchronize()
-    n = max(10, min(500, int(min_window_s * 1e3 / max(s.elapsed_time(e), 1e-3))))
-    s.record()
-    for _ in range(n):
-        fn()
-    e.record()
-    e.synchronize()
-    return s.elapsed_time(e) / n, n
+WINDOW = dict(warmup=1, min_window_s=0.5, min_iters=10, max_iters=500)
 
 
 def case(name, dev):
@@ -57,7 +33,7 @@ def case(name, dev):
     g = torch.Generator(device=dev).manual_seed(0)
     qkv = (2.0 * torch.randn(B * N, 3 * E, device=dev, generator=g)).to(torch.bfloat16)  # logit std about 4
     P = torch.empty(B, heads, N, N, device=dev)
-    t_k, n_k = time_ms(lambda: ops.attention_probs(qkv, P, B, N, E, heads))
+    t_k, n_k = window_ms(lambda: ops.attention_probs(qkv, P, B, N, E, heads), **WINDOW)
     x = qkv.view(B, N, 3, heads, 64).permute(2, 0, 3, 1, 4)
     q, k = x[0], x[1]
 
@@ -68,7 +44,7 @@ def case(name, dev):
     max_abs = (ref - P).abs().max().item()
     del ref
     torch.cuda.empty_cache()
-    t_e, n_e = time_ms(eager)
+    t_e, n_e = window_ms(eager, **WINDOW)
     torch.cuda.empty_cache()
     out_bytes = 4 * B * heads * N * N
     nbytes = out_bytes + 4 * B * N * E
@@ -90,20 +66,13 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--out", default=None, help="also write the JSON line to this file")
     args = ap.parse_args()
-    if not torch.cuda.is_available():
-        raise SystemExit("attn_probs_time.py needs a CUDA device")
     torch.backends.cuda.matmul.allow_tf32 = False
     dev = torch.device("cuda:0")
-    res = dict(gpu_info(), peaks=dict(bf16_tflops=PEAK_TFLOPS, hbm_tbs=PEAK_TBS), cases=[])
+    res = dict(card=card(), peaks=dict(bf16_tflops=PEAK_TFLOPS, hbm_tbs=PEAK_TBS), cases=[])
     for name in CONFIGS:
         res["cases"].append(case(name, dev))
-    res.update(gpu_info_after=gpu_info())
-    line = json.dumps(res)
-    print(line)
-    if args.out:
-        os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
-        with open(args.out, "w") as fh:
-            fh.write(line + "\n")
+    res["gpu_info_after"] = card()
+    emit(res, args.out)
 
 
 if __name__ == "__main__":

@@ -11,11 +11,8 @@ clock around a device synchronise (it ends on the host).  Prints one JSON object
 from __future__ import annotations
 
 import argparse
-import json
 import os
-import subprocess
 import sys
-import time
 
 import numpy as np
 import torch
@@ -23,9 +20,11 @@ import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from stego_b200 import corr, hist  # noqa: E402
 from stego_b200.config import make_cfg  # noqa: E402
+from _measure import card, emit, host_ms, window_ms  # noqa: E402
 
 B, H, E, D = 32, 28, 384, 70
 REPS = 20
+WINDOW = dict(warmup=3, min_window_s=0.0, min_iters=REPS, max_iters=REPS)
 
 
 def _inputs(fs, dev):
@@ -41,34 +40,22 @@ def _inputs(fs, dev):
     return spec, ft, ct
 
 
-def _time(fn):
-    for _ in range(3):
-        fn()
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    a.record()
-    for _ in range(REPS):
-        fn()
-    b.record()
-    b.synchronize()
-    return a.elapsed_time(b) / REPS * 1e3  # us
-
-
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--out", default=None)
     ap.add_argument("--materialise-max-fs", type=int, default=28)
     args = ap.parse_args()
     dev = torch.device("cuda:0")
-    smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                         capture_output=True, text=True).stdout.strip()
+    gpu = card()
     rows = []
     for fs in (11, 28, 56):
         spec, ft, ct = _inputs(fs, dev)
         partials, row_means = spec.scratch(B, dev)
         stats = torch.empty(spec.ncalls, 4, device=dev)
         h = hist.CdHistogram(spec, B, dev)
-        plain = _time(lambda: spec.forward(ft, ct, B, E, D, partials, row_means, stats))
-        with_h = _time(lambda: (spec.forward(ft, ct, B, E, D, partials, row_means, stats, hist=h), h.stage()))
+        plain = window_ms(lambda: spec.forward(ft, ct, B, E, D, partials, row_means, stats), **WINDOW)[0] * 1e3
+        with_h = window_ms(lambda: (spec.forward(ft, ct, B, E, D, partials, row_means, stats, hist=h), h.stage()),
+                           **WINDOW)[0] * 1e3
         row = dict(fs=fs, S=fs * fs, forward_us=round(plain, 1), forward_with_histograms_us=round(with_h, 1),
                    histogram_cost_us=round(with_h - plain, 1))
         S = fs * fs
@@ -77,24 +64,21 @@ def main():
         if fs <= args.materialise_max_fs:
             cd = torch.empty(spec.ncalls, B, S, S, device=dev)
             fdc = torch.empty_like(cd)
+
+            def materialise():
+                spec.forward(ft, ct, B, E, D, partials, row_means, stats, cd, fdc)
+                host = cd.cpu().numpy()
+                for vals in (host[0], host[1], host[2:]):
+                    np.histogram(vals.astype(np.float64), bins=hist.default_bins())
+
             spec.forward(ft, ct, B, E, D, partials, row_means, stats, cd, fdc)
-            torch.cuda.synchronize()
-            t0 = time.perf_counter()
-            spec.forward(ft, ct, B, E, D, partials, row_means, stats, cd, fdc)
-            host = cd.cpu().numpy()
-            for vals in (host[0], host[1], host[2:]):
-                np.histogram(vals.astype(np.float64), bins=hist.default_bins())
-            row["materialise_and_np_histogram_us"] = round((time.perf_counter() - t0) * 1e6, 1)
-            del cd, fdc, host
+            row["materialise_and_np_histogram_us"] = round(host_ms(materialise, 1) * 1e3, 1)
+            del cd, fdc
         else:
             row["materialise_and_np_histogram_us"] = "not measured (cd would take %.1f GB)" % (cd_bytes / 1e9)
         rows.append(row)
         torch.cuda.empty_cache()
-    out = dict(gpu=smi, shape=dict(B=B, code=H, E=E, D=D, neg_samples=5), reps=REPS, rows=rows)
-    print(json.dumps(out, indent=1))
-    if args.out:
-        with open(args.out, "w") as f:
-            json.dump(out, f, indent=1)
+    emit(dict(card=gpu, shape=dict(B=B, code=H, E=E, D=D, neg_samples=5), reps=REPS, rows=rows), args.out, indent=1)
 
 
 if __name__ == "__main__":

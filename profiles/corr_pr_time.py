@@ -16,9 +16,7 @@ from __future__ import annotations
 import argparse
 import json
 import os
-import subprocess
 import sys
-import time
 
 import numpy as np
 import torch
@@ -27,11 +25,13 @@ import torch.nn.functional as F
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from stego_b200 import _lib  # noqa: E402
 from stego_b200.correspondence import CorrespondencePR  # noqa: E402
+from _measure import card, emit, host_ms, window_ms  # noqa: E402
 
 CASES = [("c1", 32, 28, 384, 11), ("c1", 32, 28, 384, 28), ("c1", 32, 28, 384, 56),
          ("c2", 32, 40, 768, 11), ("c2", 32, 40, 768, 40)]
 D, N_CLASSES = 70, 27
 REPS, ROUNDS = 20, 3
+WINDOW = dict(warmup=0, min_window_s=0.0, min_iters=REPS, max_iters=REPS)
 REF_MAX_PAIRS = 1_000_000_000   # 3 x pairs: fd (two methods) and ld, fp32 (up to 4 GB), on the GPU and copied to the host
 SKLEARN_MAX_PAIRS = 20_000_000
 
@@ -66,19 +66,12 @@ def _reference(feats, code, label, c1, c2):
     return [t.cpu() for t in out]
 
 
-def _card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True).stdout.strip().splitlines()
-    return q[torch.cuda.current_device()] if q else torch.cuda.get_device_name()
-
-
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
-    assert torch.cuda.is_available(), "needs a CUDA device"
     dev = torch.device("cuda:0")
-    res = {"card": _card(), "reps": REPS, "rounds": ROUNDS, "cases": []}
+    res = {"card": card(), "reps": REPS, "rounds": ROUNDS, "cases": []}
     for shape, B, h, E, fs in CASES:
         x = _inputs(B, h, E, fs, dev)
         pairs = B * fs ** 4
@@ -93,18 +86,9 @@ def main():
             _reference(*x)
         ours, ref = [], []
         for _ in range(ROUNDS):
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-            for _ in range(REPS):
-                met.update(*x)
-            e1.record()
-            e1.synchronize()
-            ours.append(e0.elapsed_time(e1) / REPS)
+            ours.append(window_ms(lambda: met.update(*x), **WINDOW)[0])
             if do_ref:
-                torch.cuda.synchronize()
-                t0 = time.perf_counter()
-                fd_code, fd_feats, ld = _reference(*x)
-                ref.append((time.perf_counter() - t0) * 1e3)
+                ref.append(host_ms(lambda: _reference(*x), 1))
         row = dict(shape=shape, B=B, feature_samples=fs, E=E, D=D, pairs_per_method=pairs,
                    ours_ms=float(np.median(ours)), ours_ms_all=ours, ours_launches=launches,
                    ours_pairs_per_s=2 * pairs / (float(np.median(ours)) * 1e-3))
@@ -112,23 +96,22 @@ def main():
             row.update(reference_gpu_and_copy_ms=float(np.median(ref)), reference_ms_all=ref)
             if pairs <= SKLEARN_MAX_PAIRS:
                 from sklearn.metrics import average_precision_score
-                t0 = time.perf_counter()
-                p = fd_code.reshape(-1)
-                p = (p - p.min()) / (p - p.min()).max()
-                average_precision_score(ld.to(torch.int64).reshape(-1).numpy(), p.numpy())
-                row["reference_sklearn_ap_ms_per_method"] = (time.perf_counter() - t0) * 1e3
+                fd_code, _, ld = _reference(*x)
+
+                def sklearn_ap():
+                    p = fd_code.reshape(-1)
+                    p = (p - p.min()) / (p - p.min()).max()
+                    average_precision_score(ld.to(torch.int64).reshape(-1).numpy(), p.numpy())
+
+                row["reference_sklearn_ap_ms_per_method"] = host_ms(sklearn_ap, 1)
         else:
             row["reference"] = f"not run: fd and ld would be {3 * pairs * 4 / 1e9:.1f} GB"
         res["cases"].append(row)
         print(json.dumps(row), file=sys.stderr)
         del x, met
         torch.cuda.empty_cache()
-    res["card_after"] = _card()
-    line = json.dumps(res)
-    print(line)
-    if args.out:
-        with open(args.out, "w") as fh:
-            fh.write(json.dumps(res, indent=1) + "\n")
+    res["card_after"] = card()
+    emit(res, args.out, indent=1)
 
 
 if __name__ == "__main__":

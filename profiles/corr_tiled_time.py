@@ -12,42 +12,18 @@ Bytes: the operand tiles read once plus the loss's own scratch / gradient tiles.
 of FLOPs / 989 TFLOP/s (dense bf16) and bytes / 3.35 TB/s (H100 SXM data sheet, 700 W).
 """
 import argparse
-import json
 import os
-import subprocess
 import sys
 
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from _measure import call_ms, card, emit, window_ms  # noqa: E402
 
 PEAK_TFLOPS, PEAK_TBS = 989.0, 3.35
 CONFIGS = {"c1": ("vit_small", 384, 28, 32), "c2": ("vit_base", 768, 40, 32), "c3": ("vit_base", 768, 56, 16)}
 D, NEG = 70, 5
-
-
-def gpu_info():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader,nounits"],
-                       capture_output=True, text=True).stdout.strip().splitlines()[0]
-    name, plim, clk = [x.strip() for x in q.split(",")]
-    return dict(gpu=name, power_limit_w=float(plim), max_sm_clock_mhz=int(float(clk)))
-
-
-def time_ms(fn, min_window_s=0.3):
-    fn()
-    torch.cuda.synchronize()
-    s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    s.record()
-    fn()
-    e.record()
-    e.synchronize()
-    n = max(5, min(200, int(min_window_s * 1e3 / max(s.elapsed_time(e), 1e-3))))
-    s.record()
-    for _ in range(n):
-        fn()
-    e.record()
-    e.synchronize()
-    return s.elapsed_time(e) / n, n
+WINDOW = dict(warmup=1, min_window_s=0.3, min_iters=5, max_iters=200)
 
 
 def kernel_case(cfg_name, fs, dev):
@@ -91,10 +67,10 @@ def kernel_case(cfg_name, fs, dev):
                           spec.nslots, 1, st), "sample_bwd")
 
     fwd()
-    t_fwd, n_fwd = time_ms(fwd)
-    t_bwd, n_bwd = time_ms(bwd)
-    t_sf, _ = time_ms(sample_fwd)
-    t_sb, _ = time_ms(sample_bwd)
+    t_fwd, n_fwd = window_ms(fwd, **WINDOW)
+    t_bwd, n_bwd = window_ms(bwd, **WINDOW)
+    t_sf, _ = window_ms(sample_fwd, **WINDOW)
+    t_sb, _ = window_ms(sample_bwd, **WINDOW)
     nT = R // 128
     alg_fwd = B * K * 2 * S * S * (E + D)
     alg_bwd = B * K * 2 * S * S * 2 * D
@@ -152,14 +128,15 @@ def train_step_rate(fs, dev, steps, warmup):
         model.training_step(batch, i)
     model.flush()
     torch.cuda.synchronize()
-    s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    s.record()
-    for i in range(steps):
-        loss = model.training_step(batch, warmup + i)
-    model.flush()
-    e.record()
-    e.synchronize()
-    ms = s.elapsed_time(e) / steps
+
+    def timed_steps():
+        for i in range(steps):
+            loss = model.training_step(batch, warmup + i)
+        model.flush()
+        return loss
+
+    ms, loss = call_ms(timed_steps)
+    ms /= steps
     fused = model._fused is not None and model._fused.ws is not None and model._fused.ws.graph is not None
     out = dict(config="c1", fs=fs, batch=B, steps=steps, ms_per_step=round(ms, 3), images_per_s=round(B * 1e3 / ms, 1),
                fused_graph_path=bool(fused), loss=float(loss))
@@ -175,12 +152,10 @@ def main():
     ap.add_argument("--steps", type=int, default=40)
     ap.add_argument("--warmup", type=int, default=8)
     args = ap.parse_args()
-    if not torch.cuda.is_available():
-        raise SystemExit("corr_tiled_time.py needs a CUDA device")
     dev = torch.device("cuda:0")
     from stego_b200 import _lib
     _lib.load()
-    res = dict(gpu_info(), peaks=dict(bf16_tflops=PEAK_TFLOPS, hbm_tbs=PEAK_TBS), kernels=[], train_step=[])
+    res = dict(card=card(), peaks=dict(bf16_tflops=PEAK_TFLOPS, hbm_tbs=PEAK_TBS), kernels=[], train_step=[])
     cfgs = ["c1"] if args.quick else ["c1", "c2", "c3"]
     fss = [11, 16] if args.quick else [11, 16, 28, 40, 56]
     for c in cfgs:
@@ -188,13 +163,8 @@ def main():
             res["kernels"].append(kernel_case(c, fs, dev))
     for fs in ([11, 16] if args.quick else [11, 16, 28]):
         res["train_step"].append(train_step_rate(fs, dev, args.steps, args.warmup))
-    res.update(gpu_info_after=gpu_info())
-    line = json.dumps(res)
-    print(line)
-    if args.out:
-        os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
-        with open(args.out, "w") as fh:
-            fh.write(line + "\n")
+    res["gpu_info_after"] = card()
+    emit(res, args.out)
 
 
 if __name__ == "__main__":

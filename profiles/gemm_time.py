@@ -14,41 +14,17 @@ read once where there is one.  The floor is the larger of FLOPs / 989 TFLOP/s (d
 --root imports stego_b200 from another checkout (e.g. the parent commit, built) to compare kernels on one card.
 """
 import argparse
-import json
 import os
-import subprocess
 import sys
 
 import torch
 
+from _measure import card, emit, window_ms
+
 PEAK_TFLOPS, PEAK_TBS = 989.0, 3.35
 CONFIGS = {"c1": (384, 28, 64), "c2": (768, 40, 64), "c3": (768, 56, 32)}  # E, patches per side, backbone images
 D, P = 70, 72  # code width and its padded fp32 row
-
-
-def gpu_info():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader,nounits"],
-                       capture_output=True, text=True).stdout.strip().splitlines()[0]
-    name, plim, clk = [x.strip() for x in q.split(",")]
-    return dict(gpu=name, power_limit_w=float(plim), max_sm_clock_mhz=int(float(clk)))
-
-
-def time_ms(fn, min_window_s=0.3):
-    for _ in range(3):
-        fn()
-    torch.cuda.synchronize()
-    s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    s.record()
-    fn()
-    e.record()
-    e.synchronize()
-    n = max(10, int(min_window_s * 1e3 / max(s.elapsed_time(e), 1e-3)) + 1)
-    s.record()
-    for _ in range(n):
-        fn()
-    e.record()
-    e.synchronize()
-    return s.elapsed_time(e) / n, n
+WINDOW = dict(warmup=3, min_window_s=0.3, min_iters=10)
 
 
 def cases(cfg, dev):
@@ -114,14 +90,13 @@ def main():
     ap.add_argument("--root", default=os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
     args = ap.parse_args()
     sys.path.insert(0, os.path.abspath(args.root))
-    assert torch.cuda.is_available(), "gemm_time.py needs a CUDA device"
     dev = torch.device("cuda:0")
     torch.cuda.set_device(dev)
-    res = dict(info=gpu_info(), configs={})
+    res = dict(card=card(), configs={})
     for cfg in args.configs.split(","):
         rows, block_ms = [], 0.0
         for name, (flops, nbytes), fn in cases(cfg, dev):
-            ms, n = time_ms(fn)
+            ms, n = window_ms(fn, **WINDOW)
             t_floor = max(flops / (PEAK_TFLOPS * 1e12), nbytes / (PEAK_TBS * 1e12)) * 1e6
             bound = "tensor" if flops / PEAK_TFLOPS > nbytes / PEAK_TBS else "hbm"
             rows.append(dict(gemm=name, ms=round(ms, 4), launches=n, tflops=round(flops / ms / 1e9, 1),
@@ -131,11 +106,7 @@ def main():
                 block_ms += ms
         res["configs"][cfg] = dict(gemms=rows, vit_block_linears_ms=round(block_ms, 4))
         torch.cuda.empty_cache()
-    line = json.dumps(res)
-    print(line)
-    if args.out:
-        with open(args.out, "w") as fh:
-            fh.write(line + "\n")
+    emit(res, args.out)
 
 
 if __name__ == "__main__":

@@ -18,9 +18,7 @@ from __future__ import annotations
 import argparse
 import json
 import os
-import subprocess
 import sys
-import time
 
 import numpy as np
 import torch
@@ -31,17 +29,13 @@ sys.path.insert(0, os.path.join(ROOT, "oracle"))
 import heatmap_oracle as HO  # noqa: E402
 from stego_b200 import _lib, ops  # noqa: E402
 from stego_b200.correspondence import correspondence_heatmaps, get_heatmaps  # noqa: E402
+from _measure import card, emit, host_ms, window_ms  # noqa: E402
 
 HBM_BYTES_PER_S = 3.35e12  # H100 SXM data sheet
 REPS, ROUNDS = 20, 3
+WINDOW = dict(warmup=0, min_window_s=0.0, min_iters=REPS, max_iters=REPS)
 FIGURE = [[-.1, 0.0], [.5, .8], [-.7, -.7]]
 CASES = [("figure", 1, 3, 384, 64, 512), ("movie", 1, 280, 384, 64, 512), ("batch", 16, 16, 768, 40, 320)]
-
-
-def _card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True).stdout.strip().splitlines()
-    return q[torch.cuda.current_device()] if q else torch.cuda.get_device_name()
 
 
 def _points(name, B, P, dev):
@@ -63,16 +57,6 @@ def _feats(B, E, h, seed, dev):
     """fp32 NCHW view of tokens-major storage, as DinoFeaturizer returns it."""
     g = torch.Generator().manual_seed(seed)
     return torch.randn(B, h * h, E, generator=g).to(dev).view(B, h, h, E).permute(0, 3, 1, 2)
-
-
-def _events(fn, reps=REPS):
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(reps):
-        fn()
-    e1.record()
-    e1.synchronize()
-    return e0.elapsed_time(e1) / reps
 
 
 def _steps(f, t, qp, H, W):
@@ -104,9 +88,8 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
-    assert torch.cuda.is_available(), "needs a CUDA device"
     dev = torch.device("cuda:0")
-    res = {"card": _card(), "reps": REPS, "rounds": ROUNDS, "hbm_bytes_per_s_datasheet": HBM_BYTES_PER_S, "cases": []}
+    res = {"card": card(), "reps": REPS, "rounds": ROUNDS, "hbm_bytes_per_s_datasheet": HBM_BYTES_PER_S, "cases": []}
     for name, B, P, E, h, res_px in CASES:
         f, fp = _feats(B, E, h, 1, dev), _feats(B, E, h, 2, dev)
         qp = _points(name, B, P, dev)
@@ -123,10 +106,10 @@ def main():
         torch.cuda.synchronize()
         t_ours, t_ref, t_steps = [], [], {k: [] for k in steps}
         for _ in range(ROUNDS):
-            t_ours.append(_events(ours))
-            t_ref.append(_events(ref))
+            t_ours.append(window_ms(ours, **WINDOW)[0])
+            t_ref.append(window_ms(ref, **WINDOW)[0])
             for k, fn in steps.items():
-                t_steps[k].append(_events(fn))
+                t_steps[k].append(window_ms(fn, **WINDOW)[0])
         med = {k: float(np.median(v)) for k, v in t_steps.items()}
         row = dict(case=name, B=B, P=P, E=E, map=[h, h], size=list(size), max_abs_diff_vs_reference_fp32=err,
                    ours_ms=float(np.median(t_ours)), ours_ms_all=t_ours, reference_ms=float(np.median(t_ref)),
@@ -141,23 +124,17 @@ def main():
                 calls[0] += 1
                 return (f if calls[0] % 2 else fp), None
 
+            def ref_maps():
+                return [HO.heatmaps(f, t, qp, size, dtype=torch.float32)[0] for t in (f, fp)]
+
             get_heatmaps(net, img, img, qp)
             d_ours, d_ref, d_copy = [], [], []
             for _ in range(ROUNDS):
-                torch.cuda.synchronize()
-                t0 = time.perf_counter()
-                get_heatmaps(net, img, img, qp)
-                d_ours.append((time.perf_counter() - t0) * 1e3)
-                torch.cuda.synchronize()
-                t0 = time.perf_counter()
-                a = HO.heatmaps(f, f, qp, size, dtype=torch.float32)[0]
-                b = HO.heatmaps(f, fp, qp, size, dtype=torch.float32)[0]
-                torch.cuda.synchronize()
-                t1 = time.perf_counter()
-                a.cpu(), b.cpu()
-                t2 = time.perf_counter()
-                d_ref.append((t2 - t0) * 1e3)
-                d_copy.append((t2 - t1) * 1e3)
+                d_ours.append(host_ms(lambda: get_heatmaps(net, img, img, qp), 1))
+                d_ref.append(host_ms(lambda: [m.cpu() for m in ref_maps()], 1))
+                maps = ref_maps()  # the copies alone
+                d_copy.append(host_ms(lambda: [m.cpu() for m in maps], 1))
+                del maps
             row.update(drop_in_ours_ms=float(np.median(d_ours)), drop_in_ours_ms_all=d_ours,
                        drop_in_reference_ms=float(np.median(d_ref)), drop_in_reference_ms_all=d_ref,
                        drop_in_reference_copy_ms=float(np.median(d_copy)))
@@ -165,11 +142,8 @@ def main():
         print(json.dumps(row), file=sys.stderr)
         del f, fp, steps
         torch.cuda.empty_cache()
-    res["card_after"] = _card()
-    print(json.dumps(res))
-    if args.out:
-        with open(args.out, "w") as fh:
-            fh.write(json.dumps(res, indent=1) + "\n")
+    res["card_after"] = card()
+    emit(res, args.out, indent=1)
 
 
 if __name__ == "__main__":

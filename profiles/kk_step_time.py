@@ -10,9 +10,7 @@ CUDA events around each round, the overlapped parameter update flushed before th
 last block only to LN1 and the key third of its qkv GEMM; everything after the backbone is the same work.
 """
 import argparse
-import json
 import os
-import subprocess
 import sys
 
 import torch
@@ -20,16 +18,10 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "oracle"))
+from _measure import call_ms, card, emit  # noqa: E402
 
 N_CLASSES = 27
 SHAPES = {"c1": ("vit_small", 224, 32), "c2": ("vit_base", 320, 32)}
-
-
-def gpu_info():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader,nounits"],
-                       capture_output=True, text=True).stdout.strip().splitlines()[0]
-    name, plim, clk = [x.strip() for x in q.split(",")]
-    return dict(gpu=name, power_limit_w=float(plim), max_sm_clock_mhz=int(float(clk)))
 
 
 def step_case(name, dev, rounds=4, steps=20):
@@ -55,19 +47,17 @@ def step_case(name, dev, rounds=4, steps=20):
             m.training_step(batch, s)
         assert m._fused is not None and m._fused.ws.graph is not None, kind
         models[kind] = m
+
+    def run(m):
+        for i in range(steps):
+            m.training_step(batch, i)
+        m.flush()
+
     ms = {k: [] for k in kinds}
     for _ in range(rounds):
         for kind in kinds:
-            m = models[kind]
             torch.cuda.synchronize()
-            s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            s.record()
-            for i in range(steps):
-                m.training_step(batch, i)
-            m.flush()
-            e.record()
-            e.synchronize()
-            ms[kind].append(round(s.elapsed_time(e) / steps, 3))
+            ms[kind].append(round(call_ms(lambda: run(models[kind]))[0] / steps, 3))
     best = {k: min(v) for k, v in ms.items()}
     out = dict(shape=name, arch=arch, res=res, B=B, steps_per_round=steps, ms_per_step_feat=ms["feat"],
                ms_per_step_kk=ms["KK"], best_ms_feat=best["feat"], best_ms_kk=best["KK"],
@@ -84,14 +74,7 @@ def main():
     from stego_b200 import _lib
     _lib.load()
     dev = torch.device("cuda:0")
-    info = gpu_info()
-    res = dict(info, steps=[step_case(n, dev) for n in SHAPES], gpu_info_after=gpu_info())
-    line = json.dumps(res)
-    print(line)
-    if args.out:
-        os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
-        with open(args.out, "w") as fh:
-            fh.write(line + "\n")
+    emit(dict(card=card(), steps=[step_case(n, dev) for n in SHAPES], gpu_info_after=card()), args.out)
 
 
 if __name__ == "__main__":

@@ -18,16 +18,15 @@ from __future__ import annotations
 
 import argparse
 import ctypes
-import json
 import os
 import statistics
-import subprocess
 import sys
 
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from stego_b200 import _lib  # noqa: E402
+from _measure import call_ms, card, emit  # noqa: E402
 
 SHAPES = [(2975, 384, 20), (118287, 384, 10), (118287, 768, 10)]  # n, E, REPS
 K = 30
@@ -48,15 +47,6 @@ def _descriptors(n, E):
     return base[torch.randint(0, base.shape[0], (n,), generator=g)] + 0.35 * torch.randn(n, E, generator=g)
 
 
-def _timed(fn):
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    a.record()
-    out = fn()
-    b.record()
-    b.synchronize()
-    return a.elapsed_time(b), out
-
-
 def _reference_search(x):
     normed = torch.nn.functional.normalize(x, dim=1)
     step = normed.shape[0] // 16
@@ -73,8 +63,7 @@ def main():
     dev = torch.device("cuda:0")
     torch.backends.cuda.matmul.allow_tf32 = False
     torch.set_float32_matmul_precision("highest")
-    smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                         capture_output=True, text=True).stdout.strip()
+    gpu = card()
     libs = {"this": _lib.load()}
     if args.compare_lib:
         libs["compared"] = _bind(args.compare_lib)
@@ -93,7 +82,7 @@ def main():
             call(name)  # warm-up
         for _ in range(reps):
             for name in libs:  # alternating
-                times[name].append(_timed(lambda: call(name))[0])
+                times[name].append(call_ms(lambda: call(name))[0])
         flop = 3 * 2 * n * n * E
         row = dict(n=n, E=E, k=K, reps=reps, tensor_flop=flop)
         for name in libs:
@@ -104,17 +93,13 @@ def main():
             row["rows_with_different_indices"] = int((idx["this"] != idx["compared"]).any(1).sum())
         _reference_search(x[:max(16, n // 16)])  # warm-up: one slab's worth
         torch.cuda.synchronize()
-        ref_ms, ref_idx = _timed(lambda: _reference_search(x))
+        ref_ms, ref_idx = call_ms(lambda: _reference_search(x))
         row["torch_einsum_topk_fp32_ms"] = round(ref_ms, 1)
         row["rows_differing_from_torch_fp32"] = int((ref_idx != idx["this"]).any(1).sum())
         rows.append(row)
         del x, planes, idx, ref_idx
         torch.cuda.empty_cache()
-    out = dict(gpu=smi, k=K, compared=args.compare_label, rows=rows)
-    print(json.dumps(out, indent=1))
-    if args.out:
-        with open(args.out, "w") as f:
-            json.dump(out, f, indent=1)
+    emit(dict(card=gpu, k=K, compared=args.compare_label, rows=rows), args.out, indent=1)
 
 
 if __name__ == "__main__":

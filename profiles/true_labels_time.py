@@ -12,9 +12,7 @@ Prints one JSON line with the card name and power limit read in the same run.
     and on, alternated in one process.
 """
 import argparse
-import json
 import os
-import subprocess
 import sys
 
 import torch
@@ -23,34 +21,11 @@ import torch.nn.functional as F
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "oracle"))
+from _measure import call_ms, card, emit, window_ms  # noqa: E402
 
 N_CLASSES, FS, N_NEG = 27, 11, 5
 SHAPES = {"c1": (32, 224), "c2": (32, 320), "c3": (16, 448)}  # batch, label / image resolution
-
-
-def gpu_info():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader,nounits"],
-                       capture_output=True, text=True).stdout.strip().splitlines()[0]
-    name, plim, clk = [x.strip() for x in q.split(",")]
-    return dict(gpu=name, power_limit_w=float(plim), max_sm_clock_mhz=int(float(clk)))
-
-
-def time_ms(fn, min_window_s=0.5):
-    for _ in range(3):
-        fn()
-    torch.cuda.synchronize()
-    s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    s.record()
-    fn()
-    e.record()
-    e.synchronize()
-    n = max(10, int(min_window_s * 1e3 / max(s.elapsed_time(e), 1e-3)) + 1)
-    s.record()
-    for _ in range(n):
-        fn()
-    e.record()
-    e.synchronize()
-    return s.elapsed_time(e) / n, n
+WINDOW = dict(warmup=3, min_window_s=0.5, min_iters=10)
 
 
 def eager_signal(label, label_pos, c1, c2, perms):
@@ -76,9 +51,9 @@ def tiles_case(name, dev):
     perms = torch.stack([torch.randperm(B, generator=g) for _ in range(N_NEG)]).to(dev)
     spec = corr.make_spec(make_cfg())
     out = torch.empty(2, spec.nslots, B, spec.rows, corr.teacher_width(N_CLASSES + 1), dtype=torch.bfloat16, device=dev)
-    ours_ms, ours_n = time_ms(lambda: corr.build_label_tiles(label, label_pos, c1, c2, perms, spec, N_CLASSES,
-                                                             raw_perms=True, out=out))
-    eager_ms, eager_n = time_ms(lambda: eager_signal(label, label_pos, c1, c2, perms))
+    ours_ms, ours_n = window_ms(lambda: corr.build_label_tiles(label, label_pos, c1, c2, perms, spec, N_CLASSES,
+                                                               raw_perms=True, out=out), **WINDOW)
+    eager_ms, eager_n = window_ms(lambda: eager_signal(label, label_pos, c1, c2, perms), **WINDOW)
     C, S, px = N_CLASSES + 1, FS * FS, B * res * res
     eager_bytes = 2 * px * C * 8 + 2 * px * C * 4 + N_NEG * px * C * 4 + 2 * 7 * B * C * S * 4  # one_hot, float, gathers,
     ours_bytes = out.numel() * 2                                                             # samples + normalised
@@ -108,19 +83,17 @@ def step_case(dev, rounds=4, steps=30):
         for s in range(3):  # eager, capture, replay
             m.training_step(batch, s)
         models[on] = m
+
+    def run(m):
+        for i in range(steps):
+            m.training_step(batch, i)
+        m.flush()
+
     rates = {False: [], True: []}
     for _ in range(rounds):
         for on in (False, True):
-            m = models[on]
             torch.cuda.synchronize()
-            s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            s.record()
-            for i in range(steps):
-                m.training_step(batch, i)
-            m.flush()
-            e.record()
-            e.synchronize()
-            rates[on].append(round(B * steps / (s.elapsed_time(e) / 1e3), 1))
+            rates[on].append(round(B * steps / (call_ms(lambda: run(models[on]))[0] / 1e3), 1))
     assert models[True]._fused.step_idx == 3 + rounds * steps
     return dict(shape="c1", B=B, res=res, steps_per_round=steps, images_per_s_true_labels_off=rates[False],
                 images_per_s_true_labels_on=rates[True])
@@ -133,14 +106,8 @@ def main():
     from stego_b200 import _lib
     _lib.load()
     dev = torch.device("cuda:0")
-    info = gpu_info()
-    res = dict(info, tiles=[tiles_case(n, dev) for n in SHAPES], step=step_case(dev), gpu_info_after=gpu_info())
-    line = json.dumps(res)
-    print(line)
-    if args.out:
-        os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
-        with open(args.out, "w") as fh:
-            fh.write(line + "\n")
+    emit(dict(card=card(), tiles=[tiles_case(n, dev) for n in SHAPES], step=step_case(dev), gpu_info_after=card()),
+         args.out)
 
 
 if __name__ == "__main__":

@@ -10,9 +10,7 @@ is the reference's fp32 computation with torch's default math settings: the DINO
 with alpha None and argmax, and UnsupervisedMetrics.update's bincount for both probes (utils.py:219-229).
 """
 import argparse
-import json
 import os
-import subprocess
 import sys
 
 import torch
@@ -21,33 +19,10 @@ import torch.nn.functional as F
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "oracle"))
+from _measure import card, emit, window_ms  # noqa: E402
 
 B, RES, N_CLASSES, N_IMAGES = 16, 320, 27, 5
-
-
-def gpu_info():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader,nounits"],
-                       capture_output=True, text=True).stdout.strip().splitlines()[0]
-    name, plim, clk = [x.strip() for x in q.split(",")]
-    return dict(gpu=name, power_limit_w=float(plim), max_sm_clock_mhz=int(float(clk)))
-
-
-def time_ms(fn, min_window_s=1.0):
-    for _ in range(2):
-        fn()
-    torch.cuda.synchronize()
-    s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    s.record()
-    fn()
-    e.record()
-    e.synchronize()
-    n = max(5, min(200, int(min_window_s * 1e3 / max(s.elapsed_time(e), 1e-3))))
-    s.record()
-    for _ in range(n):
-        fn()
-    e.record()
-    e.synchronize()
-    return s.elapsed_time(e) / n, n
+WINDOW = dict(warmup=2, min_window_s=1.0, min_iters=5, max_iters=200)
 
 
 def eager_validation(sd, head, lin_w, lin_b, clusters, img, label, arch):
@@ -84,13 +59,13 @@ def case(arch, dev):
     img = torch.randn(B, 3, RES, RES, device=dev, generator=g)
     label = torch.randint(-1, N_CLASSES, (B, RES, RES), device=dev, generator=g)
     batch = dict(img=img, label=label)
-    t_ours, n_ours = time_ms(lambda: model.validation_step(batch, 0))
+    t_ours, n_ours = window_ms(lambda: model.validation_step(batch, 0), **WINDOW)
 
     sdd = {k: v.to(dev) for k, v in sd.items()}
     head = {k[len("net."):]: v.detach() for k, v in model.named_parameters() if k.startswith("net.cluster")}
     lw, lb = model.linear_probe.weight.detach(), model.linear_probe.bias.detach()
     cl = model.cluster_probe.clusters.detach()
-    t_eager, n_eager = time_ms(lambda: eager_validation(sdd, head, lw, lb, cl, img, label, arch))
+    t_eager, n_eager = window_ms(lambda: eager_validation(sdd, head, lw, lb, cl, img, label, arch), **WINDOW)
 
     # agreement of the two on this batch (bf16 ViT here, fp32 there: near-ties differ)
     model.linear_metrics.reset()
@@ -108,16 +83,8 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
-    if not torch.cuda.is_available():
-        raise SystemExit("profiles/validation_time.py: needs a CUDA device")
     dev = torch.device("cuda:0")
-    info = gpu_info()
-    res = dict(info, cases=[case(arch, dev) for arch in ("vit_small", "vit_base")], gpu_info_after=gpu_info())
-    line = json.dumps(res)
-    print(line)
-    if a.out:
-        with open(a.out, "w") as fh:
-            fh.write(line + "\n")
+    emit(dict(card=card(), cases=[case(arch, dev) for arch in ("vit_small", "vit_base")], gpu_info_after=card()), a.out)
 
 
 if __name__ == "__main__":
