@@ -411,14 +411,15 @@ STEGO_API int stego_crf_loss_bwd(const float* grad_out, const float* sel, const 
 
 /* ---- per-pixel cosine similarity <normalize(a), normalize(b)> over the channel axis and its backward: the arithmetic of the
  * optional reconstruction and augmentation-alignment terms (src/train_segmentation.py:183-199; F.normalize eps semantics of
- * src/modules.py:275-276).  a, b: fp32 [B, C, H, W] with arbitrary element strides; cosv / inva / invb: [B*H*W] floats. */
+ * src/modules.py:275-276).  a, b: fp32 [B, C, H, W] with arbitrary element strides; cosv / norma / normb: [B*H*W] floats,
+ * the cosine and the unclamped fp32 norms |a|, |b| the backward reads (it needs |a| >= eps, F.normalize's rule). */
 STEGO_API int stego_cosine_fwd(const float* a, long long a_sb, long long a_sc, long long a_sy, long long a_sx, const float* b,
                                long long b_sb, long long b_sc, long long b_sy, long long b_sx, int B, int C, int H, int W,
-                               float eps, float* cosv, float* inva, float* invb, void* stream);
+                               float eps, float* cosv, float* norma, float* normb, void* stream);
 /* grad_cos [B*H*W]; da / db (either may be null) are written with the strides of a / b. */
 STEGO_API int stego_cosine_bwd(const float* a, long long a_sb, long long a_sc, long long a_sy, long long a_sx, const float* b,
                                long long b_sb, long long b_sc, long long b_sy, long long b_sx, int B, int C, int H, int W,
-                               float eps, const float* cosv, const float* inva, const float* invb, const float* grad_cos,
+                               float eps, const float* cosv, const float* norma, const float* normb, const float* grad_cos,
                                float* da, float* db, void* stream);
 
 /* ---- data-parallel exchange over NVLink peer memory: gradient all-reduce fused into the Adam update (replaces the DDP

@@ -17,8 +17,8 @@ struct CosParams {
   int B, C, H, W;
   float eps;
   float* cosv;   // [B*H*W]
-  float* inva;   // [B*H*W] 1 / max(|a|, eps)
-  float* invb;
+  float* norma;  // [B*H*W] |a| in fp32, unclamped: the backward needs |a| >= eps, which 1 / max(|a|, eps) cannot tell
+  float* normb;
   const float* g;   // bwd: [B*H*W] upstream gradient of cosv
   float* da; float* db;  // bwd: same strides as a / b
 };
@@ -40,17 +40,20 @@ __global__ void __launch_bounds__(256) cosine_fwd_kernel(CosParams p) {
     sab = fmaf(va, vb, sab);
   }
   if (WARP) { saa = warp_sum(saa); sbb = warp_sum(sbb); sab = warp_sum(sab); }
-  const float ia = 1.0f / fmaxf(sqrtf(saa), p.eps), ib = 1.0f / fmaxf(sqrtf(sbb), p.eps);
+  const float na = sqrtf(saa), nb = sqrtf(sbb);
+  const float ia = 1.0f / fmaxf(na, p.eps), ib = 1.0f / fmaxf(nb, p.eps);
   if (!WARP || lane == 0) {
     p.cosv[pix] = sab * ia * ib;
-    p.inva[pix] = ia;
-    p.invb[pix] = ib;
+    p.norma[pix] = na;
+    p.normb[pix] = nb;
   }
 }
 
-// d cos / d a = ib * (ia * b - [|a| >= eps] * cos * ia^2 * a) ... written with the saved inverse norms:
+// d cos / d a = ib * (ia * b - [|a| >= eps] * cos * ia^2 * a) ... written with the saved norms, ia = 1 / max(|a|, eps)
+// recomputed from them (the forward's bits):
 //   a_hat = a * ia, b_hat = b * ib, cos = <a_hat, b_hat>
 //   |a| >= eps:  d cos / d a = ia * (b_hat - cos * a_hat)        |a| < eps (ia = 1/eps constant):  d cos / d a = ia * b_hat
+// F.normalize's clamp_min passes the gradient at |a| == eps too, which the inverse alone cannot tell from |a| < eps.
 template <bool WARP>
 __global__ void __launch_bounds__(256) cosine_bwd_kernel(CosParams p) {
   const long long npix = 1ll * p.B * p.H * p.W;
@@ -59,8 +62,9 @@ __global__ void __launch_bounds__(256) cosine_bwd_kernel(CosParams p) {
   if (pix >= npix) return;
   const int x = static_cast<int>(pix % p.W), y = static_cast<int>((pix / p.W) % p.H), b = static_cast<int>(pix / (1ll * p.W * p.H));
   const long long oa = b * p.a_sb + y * p.a_sy + x * p.a_sx, ob = b * p.b_sb + y * p.b_sy + x * p.b_sx;
-  const float g = p.g[pix], cs = p.cosv[pix], ia = p.inva[pix], ib = p.invb[pix];
-  const float ka = (ia < 1.0f / p.eps) ? cs : 0.f, kb = (ib < 1.0f / p.eps) ? cs : 0.f;  // clamped norm: no tangential term
+  const float g = p.g[pix], cs = p.cosv[pix], na = p.norma[pix], nb = p.normb[pix];
+  const float ia = 1.0f / fmaxf(na, p.eps), ib = 1.0f / fmaxf(nb, p.eps);
+  const float ka = (na >= p.eps) ? cs : 0.f, kb = (nb >= p.eps) ? cs : 0.f;  // clamped norm: no tangential term
   for (int c = WARP ? lane : 0; c < p.C; c += WARP ? 32 : 1) {
     const float ah = p.a[oa + c * p.a_sc] * ia, bh = p.b[ob + c * p.b_sc] * ib;
     if (p.da) p.da[oa + c * p.a_sc] = g * ia * (bh - ka * ah);
@@ -72,17 +76,17 @@ __global__ void __launch_bounds__(256) cosine_bwd_kernel(CosParams p) {
 
 using namespace stego;
 
-// cosv / inva / invb: [B*H*W] floats each (cosv is the result, the inverse norms are saved for the backward).
+// cosv / norma / normb: [B*H*W] floats each (cosv is the result, the unclamped fp32 norms are saved for the backward).
 extern "C" int stego_cosine_fwd(const float* a, long long a_sb, long long a_sc, long long a_sy, long long a_sx, const float* b,
                                 long long b_sb, long long b_sc, long long b_sy, long long b_sx, int B, int C, int H, int W,
-                                float eps, float* cosv, float* inva, float* invb, void* stream_) {
+                                float eps, float* cosv, float* norma, float* normb, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  STEGO_CHECK_ARG(a && b && cosv && inva && invb, "stego_cosine_fwd: null pointer");
+  STEGO_CHECK_ARG(a && b && cosv && norma && normb, "stego_cosine_fwd: null pointer");
   STEGO_CHECK_ARG(B > 0 && C > 0 && H > 0 && W > 0 && eps > 0.f, "stego_cosine_fwd: bad sizes");
   CosParams p;
   p.a = a; p.a_sb = a_sb; p.a_sc = a_sc; p.a_sy = a_sy; p.a_sx = a_sx;
   p.b = b; p.b_sb = b_sb; p.b_sc = b_sc; p.b_sy = b_sy; p.b_sx = b_sx;
-  p.B = B; p.C = C; p.H = H; p.W = W; p.eps = eps; p.cosv = cosv; p.inva = inva; p.invb = invb;
+  p.B = B; p.C = C; p.H = H; p.W = W; p.eps = eps; p.cosv = cosv; p.norma = norma; p.normb = normb;
   p.g = nullptr; p.da = nullptr; p.db = nullptr;
   const long long npix = 1ll * B * H * W;
   if (a_sc == 1 && b_sc == 1) {
@@ -97,16 +101,16 @@ extern "C" int stego_cosine_fwd(const float* a, long long a_sb, long long a_sc, 
 // grad_cos [B*H*W]; da / db (either may be null) are written with the strides of a / b.
 extern "C" int stego_cosine_bwd(const float* a, long long a_sb, long long a_sc, long long a_sy, long long a_sx, const float* b,
                                 long long b_sb, long long b_sc, long long b_sy, long long b_sx, int B, int C, int H, int W,
-                                float eps, const float* cosv, const float* inva, const float* invb, const float* grad_cos,
+                                float eps, const float* cosv, const float* norma, const float* normb, const float* grad_cos,
                                 float* da, float* db, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  STEGO_CHECK_ARG(a && b && cosv && inva && invb && grad_cos && (da || db), "stego_cosine_bwd: null pointer");
+  STEGO_CHECK_ARG(a && b && cosv && norma && normb && grad_cos && (da || db), "stego_cosine_bwd: null pointer");
   STEGO_CHECK_ARG(B > 0 && C > 0 && H > 0 && W > 0 && eps > 0.f, "stego_cosine_bwd: bad sizes");
   CosParams p;
   p.a = a; p.a_sb = a_sb; p.a_sc = a_sc; p.a_sy = a_sy; p.a_sx = a_sx;
   p.b = b; p.b_sb = b_sb; p.b_sc = b_sc; p.b_sy = b_sy; p.b_sx = b_sx;
   p.B = B; p.C = C; p.H = H; p.W = W; p.eps = eps;
-  p.cosv = const_cast<float*>(cosv); p.inva = const_cast<float*>(inva); p.invb = const_cast<float*>(invb);
+  p.cosv = const_cast<float*>(cosv); p.norma = const_cast<float*>(norma); p.normb = const_cast<float*>(normb);
   p.g = grad_cos; p.da = da; p.db = db;
   const long long npix = 1ll * B * H * W;
   if (a_sc == 1 && b_sc == 1) {

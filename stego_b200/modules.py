@@ -630,6 +630,17 @@ class NetWithActivations(torch.nn.Module):
         return activations
 
 
+def _overlapping(t: torch.Tensor) -> bool:
+    """True unless t's strides provably give every element its own address (each stride, in increasing order, exceeds
+    the span of the smaller ones).  Stride-0 broadcasts and other aliasing views are overlapping."""
+    span = 0
+    for st, sz in sorted((st, sz) for st, sz in zip(t.stride(), t.shape) if sz > 1):
+        if st <= span:
+            return True
+        span += (sz - 1) * st
+    return False
+
+
 class _PixelCosineFn(torch.autograd.Function):
     """cos[b, y, x] = <normalize(a)[b, :, y, x], normalize(b)[b, :, y, x]> (F.normalize eps 1e-10, modules.py:275-276): one
     read of each operand in the forward, one in the backward (csrc/cosine_loss.cu)."""
@@ -638,19 +649,21 @@ class _PixelCosineFn(torch.autograd.Function):
     def forward(ctx, a, b):
         _lib.require_cuda(a, b)
         lib = _lib.load()
-        a32, b32 = a.detach().float(), b.detach().float()
+        # the backward writes each gradient with its operand's strides, so an operand whose elements share memory (a
+        # broadcast prototype, stride 0) is made dense here: otherwise every pixel's gradient would land on the same floats
+        a32, b32 = (t.contiguous() if _overlapping(t) else t for t in (a.detach().float(), b.detach().float()))
         B, C, H, W = a32.shape
         assert b32.shape == a32.shape
         cosv = torch.empty(B, H, W, dtype=torch.float32, device=a.device)
-        inva, invb = torch.empty_like(cosv), torch.empty_like(cosv)
+        norma, normb = torch.empty_like(cosv), torch.empty_like(cosv)
         _lib.check(lib.stego_cosine_fwd(_lib.ptr(a32), *a32.stride(), _lib.ptr(b32), *b32.stride(), B, C, H, W, 1e-10,
-                                        _lib.ptr(cosv), _lib.ptr(inva), _lib.ptr(invb), _lib.stream()), "stego_cosine_fwd")
-        ctx.save_for_backward(a32, b32, cosv, inva, invb)
+                                        _lib.ptr(cosv), _lib.ptr(norma), _lib.ptr(normb), _lib.stream()), "stego_cosine_fwd")
+        ctx.save_for_backward(a32, b32, cosv, norma, normb)
         return cosv
 
     @staticmethod
     def backward(ctx, g):
-        a32, b32, cosv, inva, invb = ctx.saved_tensors
+        a32, b32, cosv, norma, normb = ctx.saved_tensors
         lib = _lib.load()
         B, C, H, W = a32.shape
         need_a, need_b = ctx.needs_input_grad
@@ -659,7 +672,7 @@ class _PixelCosineFn(torch.autograd.Function):
         if not (need_a or need_b):
             return None, None
         _lib.check(lib.stego_cosine_bwd(_lib.ptr(a32), *a32.stride(), _lib.ptr(b32), *b32.stride(), B, C, H, W, 1e-10,
-                                        _lib.ptr(cosv), _lib.ptr(inva), _lib.ptr(invb), _lib.ptr(g.float().contiguous()),
+                                        _lib.ptr(cosv), _lib.ptr(norma), _lib.ptr(normb), _lib.ptr(g.float().contiguous()),
                                         _lib.ptr(da), _lib.ptr(db), _lib.stream()), "stego_cosine_bwd")
         return da, db
 
