@@ -175,6 +175,33 @@ STEGO_API int stego_corr_loss_tiled_bwd(const void* feat_tiles, const void* code
                                         const float* stats, const float* row_means, const float* gscale,
                                         const float* gelem, const float* gcd, float* dtiles, void* stream);
 
+/* Salient sampling locations (cfg.use_salience; src/modules.py:298-311, 357-364, fed from train_segmentation.py:147-152)
+ * for both maps of a batch, in two launches.  salience / salience_pos: contiguous [B][H][W] masks of mask_bytes = 4
+ * (fp32, a pixel is salient when != 0: NaN is, -0 is not) or 1 (bool / uint8, != 0).  Unit u = map * B + b (map 0 =
+ * salience, 1 = salience_pos) is the u-th torch.randint call of the reference.  Which generator that call uses
+ * depends on the image: randint(count, (fs^2,)) runs on the CPU generator (the reference passes no device), and an
+ * image without nonzeros draws randint(H, (fs^2, 2)) on the CUDA generator.  So the caller reads the counts first.
+ * stego_salience_counts: counts [2B] int32 = the nonzeros of each unit's mask. */
+STEGO_API int stego_salience_counts(const void* salience, const void* salience_pos, int mask_bytes, int B, int H, int W,
+                                    int* counts, void* stream);
+/* stego_salience_coords: coords1 / coords2 [B][fs][fs][2] (may alias u_reg1 / u_reg2) = nz * keep + reg * (1 - keep)
+ * with nz = (x, y) * fl(1 / H) * 2 - 1 of the picked pixel, reg = u_reg * 2 - 1, keep = u_keep > 0.1f, each operation
+ * rounded once in fp32.  u_reg1 / u_reg2 [B][fs][fs][2] and u_keep [B][fs][fs]: the uniforms of the three torch.rand
+ * draws that follow the randint calls.
+ * draws_u32 [2B][2 fs^2] (element li of unit u at u * 2 fs^2 + li): for a unit with nonzeros, elements 0 .. fs^2 - 1
+ * pick the (draw % count)-th nonzero in row-major order (the CPU randint's values).  For an empty unit y, x = draw % H
+ * from elements 2 s, 2 s + 1, where the draws are Philox4x32-10 at (seed, offsets[u]), as torch's CUDA randint makes
+ * them (offsets: device int64 [2B], each a multiple of 4), or, with offsets null, the given elements (tests).
+ * scratch: stego_salience_scratch_bytes(B, H, W) bytes, 4-byte aligned (null when that is 0).
+ * Limits: B, H, W >= 1, H * W < 2^28 (torch's randint switches to 64-bit draws there), fs 1..64. */
+STEGO_API int stego_salience_coords(const void* salience, const void* salience_pos, int mask_bytes, int B, int H, int W,
+                                    int feature_samples, long long seed, const long long* offsets,
+                                    const void* draws_u32, const float* u_reg1, const float* u_reg2,
+                                    const float* u_keep, float* coords1, float* coords2, void* scratch, void* stream);
+/* Scratch bytes stego_salience_coords needs: 0 while an image's bitmap (ceil(H W / 32) words and their prefix) fits in
+ * the 96 KB of shared memory a CTA uses (H W <= 393 216), else 16 B ceil(H W / 32).  No CUDA call. */
+STEGO_API long long stego_salience_scratch_bytes(int B, int H, int W);
+
 /* ------------------------------------------------------------------------------------------------
  * TensorBoard histograms (SummaryWriter.add_histogram with its default bins="tensorflow")
  * ---------------------------------------------------------------------------------------------- */

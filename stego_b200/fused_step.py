@@ -8,8 +8,8 @@ path, each costing ~4 us of launch latency behind the frozen ViT.  Here
   * every buffer of the step lives in a workspace allocated once per input shape;
   * the *prologue* — everything that does not depend on the ViT output: the Dropout2d / coordinate / permutation
     draws (same torch RNG calls in the same order as the reference: net(img) x3 noises, net(img_pos) x3,
-    rand x2, randperm x neg_samples), the bf16 operand copies of the trainable head weights, and ONE memset of
-    all accumulate-into buffers (+ the flat gradient buffer) — runs on a side stream concurrently with the ViT graph;
+    rand x2 (with use_salience: the draws of salience.draw_into), randperm x neg_samples), the bf16 operand copies
+    of the trainable head weights, and ONE memset of all accumulate-into buffers (+ the flat gradient buffer) — runs on a side stream concurrently with the ViT graph;
   * forward and backward stages are called in order, weight gradients are accumulated straight into the flat
     gradient buffer (no per-parameter AccumulateGrad kernels), and the scalar loss arithmetic is one launch.
 
@@ -24,7 +24,7 @@ import ctypes
 
 import torch
 
-from . import _lib, corr, modules, ops, segmenter
+from . import _lib, corr, modules, ops, salience, segmenter
 
 
 def _round_up(a: int, b: int) -> int:
@@ -44,22 +44,25 @@ class FusedStep:
         self.side = None
         self.step_idx = 0
         self.update_done = None
+        self._masks = None  # use_salience: this step's (mask, mask_pos), read by the prologue
 
     # ------------------------------------------------------------------------------------------
     def supported(self, batch) -> bool:
         seg, cfg = self.seg, self.seg.cfg
         img = batch["img"]
         return (img.is_cuda and seg.training and seg.net.training and cfg.correspondence_weight > 0
-                and not cfg.use_salience and seg.net.proj_type is not None
+                and seg.net.proj_type is not None
                 and cfg.rec_weight == 0 and cfg.aug_alignment_weight == 0 and cfg.crf_weight == 0
                 and cfg.neg_samples >= 1 and cfg.dino_feat_type in ("feat", "KK")
                 and seg.linear_probe.weight.shape[0] <= 32 and seg.net.dim <= 96
                 and batch["label"].dtype in ops.LABEL_BYTES
                 and (not cfg.use_true_labels or (batch.get("label_pos") is not None and seg.n_classes <= 255
-                                                 and batch["label_pos"].dtype in ops.LABEL_BYTES)))
+                                                 and batch["label_pos"].dtype in ops.LABEL_BYTES))
+                and (not cfg.use_salience or salience.masks_supported(batch.get("mask"), batch.get("mask_pos"),
+                                                                      img.shape[0], img.device)))
 
     # ------------------------------------------------------------------------------------------
-    def _alloc(self, B, H, W, LH, LW, dev, label_dtype, label_pos_dtype):
+    def _alloc(self, B, H, W, LH, LW, dev, label_dtype, label_pos_dtype, mask_shape):
         seg, cfg, net = self.seg, self.seg.cfg, self.seg.net
         ws = _Workspace()
         E, D = net.n_feats, net.dim
@@ -78,6 +81,9 @@ class FusedStep:
         ws.c1 = torch.empty(B, spec.fs, spec.fs, 2, dtype=f32, device=dev)
         ws.c2 = torch.empty(B, spec.fs, spec.fs, 2, dtype=f32, device=dev)
         ws.perms = torch.empty(spec.n_neg, B, dtype=torch.long, device=dev)
+        # use_salience: the keep uniforms and, for maps too large for shared memory, the kernel's bitmap scratch
+        ws.keep = torch.empty(B, spec.fs, spec.fs, dtype=f32, device=dev) if mask_shape is not None else None
+        ws.sal_scratch = salience.scratch_for(B, *mask_shape[-2:], dev) if mask_shape is not None else None
         # head
         ws.x1 = torch.empty(M, E, dtype=bf, device=dev)
         ws.x2 = torch.empty(M, E, dtype=bf, device=dev) if nonlinear else None
@@ -138,8 +144,11 @@ class FusedStep:
                 ws.M2[sl].bernoulli_(keep).div_(keep)
             if ws.M3 is not None:
                 ws.M3[sl].bernoulli_(keep).div_(keep)
-        torch.rand(ws.c1.shape, out=ws.c1).mul_(2).sub_(1)  # modules.py:366-367
-        torch.rand(ws.c2.shape, out=ws.c2).mul_(2).sub_(1)
+        if ws.keep is not None:  # use_salience (modules.py:357-364): 2B randint calls, reg1, reg2, keep; one kernel
+            salience.draw_into(*self._masks, seg._spec.fs, ws.c1, ws.c2, ws.keep, ws.sal_scratch)
+        else:
+            torch.rand(ws.c1.shape, out=ws.c1).mul_(2).sub_(1)  # modules.py:366-367
+            torch.rand(ws.c2.shape, out=ws.c2).mul_(2).sub_(1)
         for i in range(ws.perms.shape[0]):                  # super_perm's randperm (modules.py:291-295)
             torch.randperm(B, device=ws.perms.device, dtype=torch.long, out=ws.perms[i])
         w1, _, wa, _, wb, _ = net.head_params()
@@ -211,12 +220,14 @@ class FusedStep:
         seg._flat.ensure_bound()  # parameters / .grad still are the views into the flat buffers the kernels write
         net_optim, linear_probe_optim, cluster_probe_optim = seg.optimizers()
         label_pos = batch["label_pos"] if cfg.use_true_labels else None
+        mask = batch["mask"] if cfg.use_salience else None
         # a new flat parameter buffer (or another label dtype) invalidates the captured graph
         key = (B, H, W, LH, LW, dev.index, id(seg._flat), label.dtype,
-               label_pos.dtype if label_pos is not None else None)
+               label_pos.dtype if label_pos is not None else None,
+               (tuple(mask.shape), mask.dtype, batch["mask_pos"].dtype) if mask is not None else None)
         if self.key != key:
             self.flush()
-            self.ws = self._alloc(B, H, W, LH, LW, dev, label.dtype, key[-1])
+            self.ws = self._alloc(B, H, W, LH, LW, dev, label.dtype, key[-2], key[-1][0] if mask is not None else None)
             self.key = key
             self.side = torch.cuda.Stream(device=dev)
         ws = self.ws
@@ -229,15 +240,25 @@ class FusedStep:
         #      prologue of this step.  The frozen ViT on the main stream depends on neither, so the whole update
         #      (the one collective of the data-parallel step included) is hidden under the next step's backbone.
         self.side.wait_stream(main)
-        with torch.cuda.stream(self.side):
-            self._prologue(ws)
-            ready = torch.cuda.Event()
-            ready.record(self.side)
+        self._masks = (batch["mask"], batch["mask_pos"]) if ws.keep is not None else None
+        ready = torch.cuda.Event()
+
+        def prologue():
+            with torch.cuda.stream(self.side):
+                self._prologue(ws)
+                ready.record(self.side)
+
+        # with use_salience the prologue waits on the host for the mask counts (salience.draw_into): it goes after the
+        # backbone is enqueued, so that wait overlaps the ViT (which draws nothing from the generators)
+        if ws.keep is None:
+            prologue()
 
         use_graph = bool(getattr(cfg, "cuda_graph", True)) and seg.profile_marks is None
         overlap = bool(getattr(cfg, "overlap_update", True)) and seg.profile_marks is None
         with torch.no_grad():
             tok_all = net.backbone_tokens([img, img_pos], use_graph=getattr(cfg, "cuda_graph", True))  # [2B,hw,E] bf16
+            if ws.keep is not None:
+                prologue()
             ws.label.copy_(label.reshape(B, LH, LW))
             if label_pos is not None:
                 ws.label_pos.copy_(label_pos.reshape(B, LH, LW))

@@ -402,8 +402,9 @@ class LitUnsupervisedSegmenter(nn.Module):
 
     # ---- the step ---------------------------------------------------------------------------------
     def training_step(self, batch, batch_idx):
-        """train_segmentation.py:112-245.  The shipped configuration (dino arch, correspondence loss, no salience /
-        rec / aug / crf terms) runs as the hand-scheduled kernel sequence of fused_step.FusedStep; anything else
+        """train_segmentation.py:112-245.  The shipped configuration (dino arch, correspondence loss, no rec / aug /
+        crf terms; use_salience, use_true_labels and "KK" included) runs as the hand-scheduled kernel sequence of
+        fused_step.FusedStep; anything else
         (or cfg.fused_step = False) takes the autograd-stitched path below.  Both compute the same step."""
         self._deliver_histograms()
         if getattr(self.cfg, "fused_step", True):
