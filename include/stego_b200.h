@@ -203,6 +203,29 @@ STEGO_API int stego_salience_coords(const void* salience, const void* salience_p
 STEGO_API long long stego_salience_scratch_bytes(int B, int H, int W);
 
 /* ------------------------------------------------------------------------------------------------
+ * Aug-alignment views (src/data.py:527-563 with the transforms of src/train_segmentation.py:408-416): img_aug and
+ * coord_aug of a batch, with torchvision's tensor arithmetic, in two launches.
+ * ---------------------------------------------------------------------------------------------- */
+/* Words per sample in the records of stego_aug_views (48).  No CUDA call. */
+STEGO_API int stego_aug_record_words(void);
+/* Scratch bytes stego_aug_views needs for B samples at output size `size`: fp64 partial sums of contrast's mean and an
+ * fp32 [B][3][size][size] intermediate.  No CUDA call. */
+STEGO_API long long stego_aug_scratch_bytes(int B, int size);
+/* img fp32 [B][3][H][W] at element strides (batch, channel, y, x), the normalised frames.  records: device int32
+ * [B][48], one per sample, drawn by the host (stego_b200/augment.py): word 0 flip, 1-4 the crop box (top, left, height,
+ * width) on the flipped frame, inside it; 5-8 ColorJitter's fn_idx; 9 grayscale; 10 blur; as fp32 bits: 11-12 the
+ * brightness factor b and fl(1 - b), 13-14 contrast, 15-16 saturation, 17 the hue factor, 18-42 the 5x5 Gaussian
+ * weights (row-major).  Outputs: img_aug fp32 [B][3][size][size] = flip, crop, antialiased bilinear resize
+ * (align_corners=False), the four jitter ops in fn_idx order (contrast blends with the mean of rgb_to_grayscale at that
+ * point of the chain), grayscale, 5x5 blur with reflect padding; coord_aug fp32 [B][size][size][2] = the same flip,
+ * crop and resize of meshgrid(linspace(-1, 1, H), linspace(-1, 1, W)) ("ij": element 0 varies along rows).
+ * scratch: stego_aug_scratch_bytes(B, size) bytes, 8-byte aligned.  B 1..65535, H, W >= 1, size 3..8192.  The means are
+ * summed in a fixed order: repeated calls return identical bits. */
+STEGO_API int stego_aug_views(const float* img, long long stride_b, long long stride_c, long long stride_y,
+                              long long stride_x, int B, int H, int W, int size, const int* records, void* scratch,
+                              float* img_aug, float* coord_aug, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * TensorBoard histograms (SummaryWriter.add_histogram with its default bins="tensorflow")
  * ---------------------------------------------------------------------------------------------- */
 /* The 1549 float64 bucket edges of torch's SummaryWriter.default_bins (edges, may be null) and the 1550 fp32
