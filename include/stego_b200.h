@@ -472,6 +472,22 @@ STEGO_API int stego_cosine_bwd(const float* a, long long a_sb, long long a_sc, l
                                float eps, const float* cosv, const float* norma, const float* normb, const float* grad_cos,
                                float* da, float* db, void* stream);
 
+/* ---- sampling half of the aug-alignment term (src/train_segmentation.py:189-199, src/modules.py:287-288): the code of
+ * img read at the view's coordinates, ahead of the cosine above.  coord_aug: fp32 [B][S][S][2] contiguous; code: fp32
+ * [B][C][h][h] with element strides (sb, sc, sy, sx).  grid [B][h][h][2] = F.interpolate(coord_aug.permute(0, 3, 1, 2), h,
+ * mode="bilinear", align_corners=False).permute(0, 2, 3, 1), ATen's arithmetic; sampled [B][C][h][h] contiguous =
+ * F.grid_sample(code, grid.permute(0, 2, 1, 3), padding_mode="border", align_corners=True), ATen's arithmetic. */
+STEGO_API int stego_aug_align_fwd(const float* coord_aug, int S, const float* code, long long sb, long long sc,
+                                  long long sy, long long sx, int B, int C, int h, float* grid, float* sampled,
+                                  void* stream);
+/* d(code) += the grid_sample backward of dsampled [B][C][h][h] contiguous at the forward's grid, by fp32 atomics
+ * (dcode strides as the forward's code). */
+STEGO_API int stego_aug_align_bwd(const float* grid, const float* dsampled, int B, int C, int h, float* dcode,
+                                  long long sb, long long sc, long long sy, long long sx, void* stream);
+/* loss[0] = -mean(cosv[0 .. n)) summed in fp64 in a fixed order (bit-reproducible); total[0] += weight * loss[0] when
+ * total is not null. */
+STEGO_API int stego_aug_align_loss(const float* cosv, long long n, float weight, float* loss, float* total, void* stream);
+
 /* ---- data-parallel exchange over NVLink peer memory: gradient all-reduce fused into the Adam update (replaces the DDP
  * all-reduce behind manual_backward + the three optimizer.step() calls, src/train_segmentation.py:227-230, 476).
  * Every rank allocates one peer-visible block [export 2 x n_pad floats | flags world x uint32], exchanges the 64-byte CUDA

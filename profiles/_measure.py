@@ -67,6 +67,19 @@ def window_ms(fn, *, warmup, min_window_s, min_iters, max_iters=None):
     return call_ms(window)[0] / n, n
 
 
+def enqueue_ms(fn, n):
+    """Host-clock time per call of n calls of fn, from an idle device to the return of the last call (no wait for the
+    device at the end): what the host spends issuing the work.  The device is synchronised afterwards."""
+    _require_device()
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    for _ in range(n):
+        fn()
+    t = (time.perf_counter() - t0) * 1e3 / n
+    torch.cuda.synchronize()
+    return t
+
+
 def host_ms(fn, n):
     """Host-clock time per call of n calls of fn, from an idle device to the synchronize after the last call; for
     work that ends on the host."""

@@ -102,6 +102,20 @@ def _check(img, seeds, size):
     return seeds
 
 
+def batch_seeds(seeds) -> list:
+    """batch["seed"] as B Python ints: a list, or a CPU integer tensor as a DataLoader collates one.  A CUDA tensor
+    raises, because reading it would synchronise with the device."""
+    if isinstance(seeds, torch.Tensor):
+        if seeds.is_cuda:
+            raise ValueError("stego_b200.augment: batch['seed'] must be a list or a CPU tensor (reading a CUDA tensor "
+                             "would synchronise with the device)")
+        if seeds.dtype.is_floating_point or seeds.dtype.is_complex or seeds.dtype == torch.bool or seeds.dim() != 1:
+            raise ValueError(f"stego_b200.augment: batch['seed'] must be a 1-d integer tensor, got {seeds.dtype} "
+                             f"{tuple(seeds.shape)}")
+        return seeds.tolist()
+    return list(seeds)
+
+
 def launch(img, records_dev, size, img_aug, coord_aug, scratch) -> None:
     """stego_aug_views on prepared operands: records int32 [B, 48] on the device, scratch of
     stego_aug_scratch_bytes bytes."""

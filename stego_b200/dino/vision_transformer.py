@@ -278,10 +278,16 @@ class VisionTransformer(nn.Module):
         g, static_in = graphs[key]
         off = 0
         for part in parts:
-            static_in[off:off + part.shape[0]].copy_(part)
+            if part.data_ptr() != static_in[off].data_ptr():  # a part built in place (graph_input) needs no copy
+                static_in[off:off + part.shape[0]].copy_(part)
             off += part.shape[0]
         g.replay()
         return g.result
+
+    def graph_input(self, kind: str, shape, device, dtype=torch.float32):
+        """The static input of the captured graph for (kind, shape), or None before that graph exists.  A caller may
+        build part of its batch straight into a slice of it and pass that slice back in its list of batches."""
+        return self._cache.get("graphs", {}).get((kind, tuple(shape), device.index, dtype), (None, None))[1]
 
     def _patch_features_eager(self, img: torch.Tensor) -> torch.Tensor:
         B = img.shape[0]

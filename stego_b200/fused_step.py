@@ -8,7 +8,8 @@ path, each costing ~4 us of launch latency behind the frozen ViT.  Here
   * every buffer of the step lives in a workspace allocated once per input shape;
   * the *prologue* — everything that does not depend on the ViT output: the Dropout2d / coordinate / permutation
     draws (same torch RNG calls in the same order as the reference: net(img) x3 noises, net(img_pos) x3,
-    rand x2 (with use_salience: the draws of salience.draw_into), randperm x neg_samples), the bf16 operand copies
+    rand x2 (with use_salience: the draws of salience.draw_into), randperm x neg_samples, and with the aug-alignment
+    term net(img_aug) x3), the bf16 operand copies
     of the trainable head weights, and ONE memset of all accumulate-into buffers (+ the flat gradient buffer) — runs on a side stream concurrently with the ViT graph;
   * forward and backward stages are called in order, weight gradients are accumulated straight into the flat
     gradient buffer (no per-parameter AccumulateGrad kernels), and the scalar loss arithmetic is one launch.
@@ -17,6 +18,11 @@ The stages are the functions the autograd nodes call (modules.pack_head_weights 
 cluster_lookup_forward / cluster_lookup_backward, corr.build_tiles / build_label_tiles / sample_norm_backward / LossSpec,
 segmenter.linear_probe_ce_step), given the workspace instead of per-call buffers: both paths launch the same kernels
 with the same arguments.  Only stego_step_losses is called from here alone.
+
+With cfg.aug_alignment_weight > 0 and batch["seed"] (train_segmentation.py:189-199) the step builds img_aug / coord_aug
+itself (augment: host draws on a forked CPU generator, one pinned upload, two launches, all before the backbone is
+enqueued), runs img, img_pos and img_aug through the backbone as ONE batch of 3B and the head over 3B rows; the term is
+modules.aug_sample_forward / cosine_forward / aug_loss and their backward, inside the tail graph.
 """
 from __future__ import annotations
 
@@ -24,7 +30,7 @@ import ctypes
 
 import torch
 
-from . import _lib, corr, modules, ops, salience, segmenter
+from . import _lib, augment, corr, modules, ops, salience, segmenter
 
 
 def _round_up(a: int, b: int) -> int:
@@ -52,7 +58,8 @@ class FusedStep:
         img = batch["img"]
         return (img.is_cuda and seg.training and seg.net.training and cfg.correspondence_weight > 0
                 and seg.net.proj_type is not None
-                and cfg.rec_weight == 0 and cfg.aug_alignment_weight == 0 and cfg.crf_weight == 0
+                and cfg.rec_weight == 0 and cfg.crf_weight == 0
+                and (cfg.aug_alignment_weight == 0 or self._aug_supported(batch))
                 and cfg.neg_samples >= 1 and cfg.dino_feat_type in ("feat", "KK")
                 and seg.linear_probe.weight.shape[0] <= 32 and seg.net.dim <= 96
                 and batch["label"].dtype in ops.LABEL_BYTES
@@ -61,23 +68,33 @@ class FusedStep:
                 and (not cfg.use_salience or salience.masks_supported(batch.get("mask"), batch.get("mask_pos"),
                                                                       img.shape[0], img.device)))
 
+    def _aug_supported(self, batch) -> bool:
+        """The aug-alignment term runs here when the step builds the views itself: seeds and no views, fp32 img at
+        cfg.res x cfg.res, seeds readable without a device synchronisation."""
+        img, seeds, res = batch["img"], batch.get("seed"), self.seg.cfg.res
+        return (seeds is not None and batch.get("img_aug") is None and batch.get("coord_aug") is None
+                and not (isinstance(seeds, torch.Tensor) and seeds.is_cuda)
+                and img.dtype == torch.float32 and img.dim() == 4 and tuple(img.shape[1:]) == (3, res, res))
+
     # ------------------------------------------------------------------------------------------
-    def _alloc(self, B, H, W, LH, LW, dev, label_dtype, label_pos_dtype, mask_shape):
+    def _alloc(self, B, H, W, LH, LW, dev, label_dtype, label_pos_dtype, mask_shape, aug):
         seg, cfg, net = self.seg, self.seg.cfg, self.seg.net
         ws = _Workspace()
         E, D = net.n_feats, net.dim
         fh, fw = H // net.patch_size, W // net.patch_size
         hw = fh * fw
-        M = 2 * B * hw
+        n_img = 3 if aug else 2  # backbone / head rows: img, img_pos (, img_aug)
+        M = n_img * B * hw
         P = _round_up(D, 8)
         spec = seg._spec
         f32, bf = torch.float32, torch.bfloat16
         nonlinear = net.proj_type == "nonlinear"
         ws.dims = (B, E, D, P, fh, fw, hw, M, nonlinear)
-        # RNG outputs
-        ws.M1 = torch.empty(2 * B, E, 1, 1, dtype=f32, device=dev)
-        ws.M2 = torch.empty(2 * B, E, 1, 1, dtype=f32, device=dev) if nonlinear else None
-        ws.M3 = torch.empty(2 * B, E, 1, 1, dtype=f32, device=dev) if cfg.dropout else None
+        ws.n_img = n_img
+        # RNG outputs (img_aug's third noise is drawn, as net(img_aug) draws it, and scales nothing)
+        ws.M1 = torch.empty(n_img * B, E, 1, 1, dtype=f32, device=dev)
+        ws.M2 = torch.empty(n_img * B, E, 1, 1, dtype=f32, device=dev) if nonlinear else None
+        ws.M3 = torch.empty(n_img * B, E, 1, 1, dtype=f32, device=dev) if cfg.dropout else None
         ws.c1 = torch.empty(B, spec.fs, spec.fs, 2, dtype=f32, device=dev)
         ws.c2 = torch.empty(B, spec.fs, spec.fs, 2, dtype=f32, device=dev)
         ws.perms = torch.empty(spec.n_neg, B, dtype=torch.long, device=dev)
@@ -120,6 +137,25 @@ class FusedStep:
         ws.eager_steps = 0
         ws.hist = None        # hist.CdHistogram and the tail graph that fills it, made on the first histogram step
         ws.hist_graph = None
+        ws.aug = aug
+        if aug:  # the aug-alignment term: the views, the sampled code of img, the cosine and its gradients
+            ws.img_aug = torch.empty(B, 3, H, W, dtype=f32, device=dev)  # used until the backbone graph exists
+            ws.coord_aug = torch.empty(B, H, W, 2, dtype=f32, device=dev)
+            # the view records go up through two pinned host buffers used in turn: one is refilled once the copy made
+            # from it two steps earlier has run (enqueued ahead of that step's backbone, so the wait is for work long
+            # done), and no pinned block is allocated per step
+            ws.rec_host = [torch.empty(B, augment.RECORD_WORDS, dtype=torch.int32).pin_memory() for _ in range(2)]
+            ws.rec_copied = [None, None]
+            ws.rec_dev = torch.empty(B, augment.RECORD_WORDS, dtype=torch.int32, device=dev)
+            ws.aug_scratch = torch.empty(-(-int(_lib.load().stego_aug_scratch_bytes(B, H)) // 8), dtype=torch.float64,
+                                         device=dev)
+            ws.grid = torch.empty(B, fh, fw, 2, dtype=f32, device=dev)
+            ws.sampled = torch.empty(B, D, fh, fw, dtype=f32, device=dev)
+            ws.dsampled = torch.empty(B, D, fh, fw, dtype=f32, device=dev)
+            ws.cosv, ws.norma, ws.normb = (torch.empty(B, fh, fw, dtype=f32, device=dev) for _ in range(3))
+            # d(loss)/d(cos) of loss += w * -(cos.mean()): autograd's fl(fl(-w) / N), one value per pixel
+            ws.dcos = torch.full((B, fh, fw), -float(cfg.aug_alignment_weight), dtype=f32, device=dev).div_(B * hw)
+            ws.aug_loss = torch.empty(1, dtype=f32, device=dev)
         # everything the kernels accumulate into: ONE buffer, ONE memset per step
         sizes = dict(dlogits=B * hw * 32, dtiles=spec.nslots * B * spec.rows * corr.DT_LD, dall=M * P,
                      dnc=n_clu * D, db_pad=P)
@@ -137,13 +173,17 @@ class FusedStep:
         seg, cfg, net = self.seg, self.seg.cfg, self.seg.net
         B, E, D, P, fh, fw, hw, M, nonlinear = ws.dims
         keep = 0.9  # Dropout2d(p=.1), modules.py:41
-        for half in (0, 1):  # net(img) then net(img_pos): cluster1 noise, cluster2 noise, returned-feature noise
-            sl = slice(half * B, (half + 1) * B)
+
+        def noises(i):  # the i-th net() call of the step: cluster1 noise, cluster2 noise, returned-feature noise
+            sl = slice(i * B, (i + 1) * B)
             ws.M1[sl].bernoulli_(keep).div_(keep)
             if nonlinear:
                 ws.M2[sl].bernoulli_(keep).div_(keep)
             if ws.M3 is not None:
                 ws.M3[sl].bernoulli_(keep).div_(keep)
+
+        noises(0)  # net(img)
+        noises(1)  # net(img_pos)
         if ws.keep is not None:  # use_salience (modules.py:357-364): 2B randint calls, reg1, reg2, keep; one kernel
             salience.draw_into(*self._masks, seg._spec.fs, ws.c1, ws.c2, ws.keep, ws.sal_scratch)
         else:
@@ -151,6 +191,8 @@ class FusedStep:
             torch.rand(ws.c2.shape, out=ws.c2).mul_(2).sub_(1)
         for i in range(ws.perms.shape[0]):                  # super_perm's randperm (modules.py:291-295)
             torch.randperm(B, device=ws.perms.device, dtype=torch.long, out=ws.perms[i])
+        if ws.aug:
+            noises(2)  # net(img_aug), after the correspondence loss (train_segmentation.py:189-190)
         w1, _, wa, _, wb, _ = net.head_params()
         modules.pack_head_weights(w1, wa, wb, ws.w1p, ws.wab, ws.wbp)
         ws.zbuf.zero_()
@@ -166,12 +208,15 @@ class FusedStep:
         spec = seg._spec
         params = net.head_params()
         _, b1, _, ba, _, bb = params
-        # [2B, C, h, w] views of the tokens-major features and of the padded code storage: img rows, then img_pos rows
-        feats = tok_all.view(2 * B, fh, fw, E).permute(0, 3, 1, 2)
-        code = ws.code.view(2 * B, fh, fw, P)[..., :D].permute(0, 3, 1, 2)
+        # [nB, C, h, w] views of the tokens-major features and of the padded code storage: img rows, then img_pos rows
+        # (, then img_aug rows)
+        n = ws.n_img
+        feats = tok_all.view(n * B, fh, fw, E).permute(0, 3, 1, 2)
+        code = ws.code.view(n * B, fh, fw, P)[..., :D].permute(0, 3, 1, 2)
+        img_rows, pos_rows, aug_rows = slice(0, B), slice(B, 2 * B), slice(2 * B, 3 * B)
 
         # ---- head forward (modules.py:108-111)
-        modules.head_forward(tok_all.reshape(M, E), ws.M1, ws.M2, 2 * B, hw, ws.x1, ws.x2, ws.hid, ws.code, ws.w1p, b1,
+        modules.head_forward(tok_all.reshape(M, E), ws.M1, ws.M2, n * B, hw, ws.x1, ws.x2, ws.hid, ws.code, ws.w1p, b1,
                              ws.wab, ba, ws.wbp, bb)
         seg._mark("head_forward")
 
@@ -180,12 +225,15 @@ class FusedStep:
             corr.build_label_tiles(ws.label, ws.label_pos, ws.c1, ws.c2, ws.perms, spec, seg.n_classes, raw_perms=True,
                                    out=ws.ftiles)
         else:
-            m3, p3 = (ws.M3[:B], ws.M3[B:]) if ws.M3 is not None else (None, None)
-            corr.build_tiles(feats[:B], feats[B:], ws.c1, ws.c2, ws.perms, spec, E, m3, p3, raw_perms=True,
+            m3, p3 = (ws.M3[img_rows], ws.M3[pos_rows]) if ws.M3 is not None else (None, None)
+            corr.build_tiles(feats[img_rows], feats[pos_rows], ws.c1, ws.c2, ws.perms, spec, E, m3, p3, raw_perms=True,
                              out=ws.ftiles)
-        corr.build_tiles(code[:B], code[B:], ws.c1, ws.c2, ws.perms, spec, corr.CODE_PAD, raw_perms=True,
+        corr.build_tiles(code[img_rows], code[pos_rows], ws.c1, ws.c2, ws.perms, spec, corr.CODE_PAD, raw_perms=True,
                          out=ws.ctiles)
         spec.forward(ws.ftiles, ws.ctiles, B, ws.ET, D, ws.partials, ws.row_means, ws.stats, hist=hist)
+        if ws.aug:  # -cosine(sample(code, coord), code_aug) (train_segmentation.py:189-199)
+            modules.aug_sample_forward(ws.coord_aug, code[img_rows], ws.grid, ws.sampled)
+            modules.cosine_forward(ws.sampled, code[aug_rows], ws.cosv, ws.norma, ws.normb)
         seg._mark("corr_loss_forward")
 
         # ---- probes on the detached code (train_segmentation.py:213-225): forward + backward in place
@@ -196,14 +244,21 @@ class FusedStep:
         _lib.check(_lib.load().stego_step_losses(_lib.ptr(ws.stats), spec.ncalls, ws.call_w, _lib.ptr(ws.lin_loss),
                                                  _lib.ptr(ws.clu_loss), _lib.ptr(ws.out4), _lib.stream()),
                    "stego_step_losses")
+        if ws.aug:  # loss/aug_alignment, and its weighted value onto the total
+            modules.aug_loss(ws.cosv, seg.cfg.aug_alignment_weight, ws.aug_loss, ws.out4)
         seg._mark("probes_forward")
 
         # ---- backward (manual_backward, :227)
         modules.cluster_lookup_backward(code[:B], cl, None, ws.one, ws.dnc, cl.grad)
         spec.backward(ws.ftiles, ws.ctiles, B, ws.ET, D, ws.stats, ws.row_means, ws.gscale, None, None, ws.dtiles)
         dall = ws.dall.view(M, P)
-        corr.sample_norm_backward(code[:B], code[B:], ws.c1, ws.c2, ws.perms, spec, ws.dtiles, dall[:B * hw],
-                                  dall[B * hw:], raw_perms=True)
+        corr.sample_norm_backward(code[img_rows], code[pos_rows], ws.c1, ws.c2, ws.perms, spec, ws.dtiles,
+                                  dall[:B * hw], dall[B * hw:2 * B * hw], raw_perms=True)
+        if ws.aug:  # d(code_aug) into the img_aug rows, d(sampled) scattered into the img rows
+            dcode = dall.view(n * B, fh, fw, P)[..., :D].permute(0, 3, 1, 2)
+            modules.cosine_backward(ws.sampled, code[aug_rows], ws.cosv, ws.norma, ws.normb, ws.dcos, ws.dsampled,
+                                    dcode[aug_rows])
+            modules.aug_sample_backward(ws.grid, ws.dsampled, dcode[img_rows])
         # head backward: d(code) [M, P] -> bias / weight gradients straight into the flat gradient buffer
         modules.head_backward(dall, ws.x1, ws.x2, ws.hid, ws.wbp, ws.dyb, ws.db_pad, ws.dh, ws.dhb,
                               *[p.grad if p is not None else None for p in params])
@@ -221,13 +276,18 @@ class FusedStep:
         net_optim, linear_probe_optim, cluster_probe_optim = seg.optimizers()
         label_pos = batch["label_pos"] if cfg.use_true_labels else None
         mask = batch["mask"] if cfg.use_salience else None
+        aug = cfg.aug_alignment_weight > 0
+        if aug:  # the host draws of the views come first: they overlap the previous step's work on the device
+            seeds = augment._check(img, augment.batch_seeds(batch["seed"]), cfg.res)
+            _, records = augment.draw_records(seeds, H, W)
         # a new flat parameter buffer (or another label dtype) invalidates the captured graph
         key = (B, H, W, LH, LW, dev.index, id(seg._flat), label.dtype,
                label_pos.dtype if label_pos is not None else None,
-               (tuple(mask.shape), mask.dtype, batch["mask_pos"].dtype) if mask is not None else None)
+               (tuple(mask.shape), mask.dtype, batch["mask_pos"].dtype) if mask is not None else None, aug)
         if self.key != key:
             self.flush()
-            self.ws = self._alloc(B, H, W, LH, LW, dev, label.dtype, key[-2], key[-1][0] if mask is not None else None)
+            self.ws = self._alloc(B, H, W, LH, LW, dev, label.dtype, key[-3], key[-2][0] if mask is not None else None,
+                                  aug)
             self.key = key
             self.side = torch.cuda.Stream(device=dev)
         ws = self.ws
@@ -256,7 +316,23 @@ class FusedStep:
         use_graph = bool(getattr(cfg, "cuda_graph", True)) and seg.profile_marks is None
         overlap = bool(getattr(cfg, "overlap_update", True)) and seg.profile_marks is None
         with torch.no_grad():
-            tok_all = net.backbone_tokens([img, img_pos], use_graph=getattr(cfg, "cuda_graph", True))  # [2B,hw,E] bf16
+            parts = [img, img_pos]
+            if aug:
+                # the views go straight into the backbone graph's input once that graph exists (no copy)
+                img_aug = ws.img_aug
+                if getattr(cfg, "cuda_graph", True):
+                    static_in = net.model.graph_input(net.feat_type, (3 * B, 3, H, W), dev)
+                    img_aug = static_in[2 * B:] if static_in is not None else img_aug
+                i = self.step_idx % 2
+                if ws.rec_copied[i] is not None:
+                    ws.rec_copied[i].synchronize()
+                ws.rec_host[i].copy_(records)
+                ws.rec_dev.copy_(ws.rec_host[i], non_blocking=True)
+                ws.rec_copied[i] = torch.cuda.Event()
+                ws.rec_copied[i].record(main)
+                augment.launch(img, ws.rec_dev, H, img_aug, ws.coord_aug, ws.aug_scratch)
+                parts.append(img_aug)
+            tok_all = net.backbone_tokens(parts, use_graph=getattr(cfg, "cuda_graph", True))  # [nB, hw, E] bf16
             if ws.keep is not None:
                 prologue()
             ws.label.copy_(label.reshape(B, LH, LW))
@@ -316,6 +392,8 @@ class FusedStep:
         seg.log('cd/neg_inter', out4[3])
         seg.log('loss/linear', ws.lin_loss[0])
         seg.log('loss/cluster', ws.clu_loss[0])
+        if ws.aug:
+            seg.log('loss/aug_alignment', ws.aug_loss[0])
         seg.log('loss/total', out4[0])
         self.step_idx += 1
         seg.global_step += 1

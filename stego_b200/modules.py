@@ -641,6 +641,50 @@ def _overlapping(t: torch.Tensor) -> bool:
     return False
 
 
+def cosine_forward(a, b, cosv, norma, normb) -> None:
+    """cosv [B, H, W] = <normalize(a), normalize(b)> over the channels of fp32 [B, C, H, W] views a, b (any strides),
+    and the unclamped norms the backward reads (csrc/cosine_loss.cu)."""
+    B, C, H, W = a.shape
+    _lib.check(_lib.load().stego_cosine_fwd(_lib.ptr(a), *a.stride(), _lib.ptr(b), *b.stride(), B, C, H, W, 1e-10,
+                                            _lib.ptr(cosv), _lib.ptr(norma), _lib.ptr(normb), _lib.stream()),
+               "stego_cosine_fwd")
+
+
+def cosine_backward(a, b, cosv, norma, normb, grad_cos, da, db) -> None:
+    """da / db (either may be None) = grad_cos [B, H, W] x d(cosv)/d(a) / d(b), written (not accumulated) with the
+    strides of a / b."""
+    B, C, H, W = a.shape
+    _lib.check(_lib.load().stego_cosine_bwd(_lib.ptr(a), *a.stride(), _lib.ptr(b), *b.stride(), B, C, H, W, 1e-10,
+                                            _lib.ptr(cosv), _lib.ptr(norma), _lib.ptr(normb), _lib.ptr(grad_cos),
+                                            _lib.ptr(da), _lib.ptr(db), _lib.stream()), "stego_cosine_bwd")
+
+
+def aug_sample_forward(coord_aug, code, grid, sampled) -> None:
+    """The sampling half of the aug-alignment term (train_segmentation.py:189-199): grid [B, h, h, 2] = coord_aug
+    [B, S, S, 2] (contiguous) resized to h x h as F.interpolate(bilinear, align_corners=False) does, and sampled
+    [B, C, h, h] (contiguous) = sample(code, grid) (modules.py:287-288) of the fp32 code [B, C, h, h] (any strides)."""
+    B, C, h, w = code.shape
+    if h != w or coord_aug.shape[1] != coord_aug.shape[2] or not coord_aug.is_contiguous():
+        raise ValueError(f"stego_b200.aug_sample_forward: square code and contiguous square coord_aug needed, got "
+                         f"{tuple(code.shape)} and {tuple(coord_aug.shape)}")
+    _lib.check(_lib.load().stego_aug_align_fwd(_lib.ptr(coord_aug), coord_aug.shape[1], _lib.ptr(code), *code.stride(),
+                                               B, C, h, _lib.ptr(grid), _lib.ptr(sampled), _lib.stream()),
+               "stego_aug_align_fwd")
+
+
+def aug_sample_backward(grid, dsampled, dcode) -> None:
+    """dcode [B, C, h, h] (the forward's code strides) += the grid_sample backward of dsampled at grid, by atomics."""
+    B, C, h, _ = dcode.shape
+    _lib.check(_lib.load().stego_aug_align_bwd(_lib.ptr(grid), _lib.ptr(dsampled), B, C, h, _lib.ptr(dcode),
+                                               *dcode.stride(), _lib.stream()), "stego_aug_align_bwd")
+
+
+def aug_loss(cosv, weight: float, loss, total=None) -> None:
+    """loss[0] = -cosv.mean() in a fixed summation order; total[0] += weight * loss[0] when total is given."""
+    _lib.check(_lib.load().stego_aug_align_loss(_lib.ptr(cosv), cosv.numel(), float(weight), _lib.ptr(loss),
+                                                _lib.ptr(total), _lib.stream()), "stego_aug_align_loss")
+
+
 class _PixelCosineFn(torch.autograd.Function):
     """cos[b, y, x] = <normalize(a)[b, :, y, x], normalize(b)[b, :, y, x]> (F.normalize eps 1e-10, modules.py:275-276): one
     read of each operand in the forward, one in the backward (csrc/cosine_loss.cu)."""
@@ -648,7 +692,6 @@ class _PixelCosineFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, a, b):
         _lib.require_cuda(a, b)
-        lib = _lib.load()
         # the backward writes each gradient with its operand's strides, so an operand whose elements share memory (a
         # broadcast prototype, stride 0) is made dense here: otherwise every pixel's gradient would land on the same floats
         a32, b32 = (t.contiguous() if _overlapping(t) else t for t in (a.detach().float(), b.detach().float()))
@@ -656,24 +699,19 @@ class _PixelCosineFn(torch.autograd.Function):
         assert b32.shape == a32.shape
         cosv = torch.empty(B, H, W, dtype=torch.float32, device=a.device)
         norma, normb = torch.empty_like(cosv), torch.empty_like(cosv)
-        _lib.check(lib.stego_cosine_fwd(_lib.ptr(a32), *a32.stride(), _lib.ptr(b32), *b32.stride(), B, C, H, W, 1e-10,
-                                        _lib.ptr(cosv), _lib.ptr(norma), _lib.ptr(normb), _lib.stream()), "stego_cosine_fwd")
+        cosine_forward(a32, b32, cosv, norma, normb)
         ctx.save_for_backward(a32, b32, cosv, norma, normb)
         return cosv
 
     @staticmethod
     def backward(ctx, g):
         a32, b32, cosv, norma, normb = ctx.saved_tensors
-        lib = _lib.load()
-        B, C, H, W = a32.shape
         need_a, need_b = ctx.needs_input_grad
         da = torch.empty_strided(a32.shape, a32.stride(), dtype=torch.float32, device=a32.device) if need_a else None
         db = torch.empty_strided(b32.shape, b32.stride(), dtype=torch.float32, device=b32.device) if need_b else None
         if not (need_a or need_b):
             return None, None
-        _lib.check(lib.stego_cosine_bwd(_lib.ptr(a32), *a32.stride(), _lib.ptr(b32), *b32.stride(), B, C, H, W, 1e-10,
-                                        _lib.ptr(cosv), _lib.ptr(norma), _lib.ptr(normb), _lib.ptr(g.float().contiguous()),
-                                        _lib.ptr(da), _lib.ptr(db), _lib.stream()), "stego_cosine_bwd")
+        cosine_backward(a32, b32, cosv, norma, normb, g.float().contiguous(), da, db)
         return da, db
 
 

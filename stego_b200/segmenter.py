@@ -185,6 +185,18 @@ def true_label_pos(batch) -> torch.Tensor:
     return batch["label_pos"]
 
 
+def aug_views_of(batch, res: int):
+    """(img_aug, coord_aug) of the aug-alignment term (train_segmentation.py:189-199): the caller's views when the batch
+    carries them, else built from batch["img"] (fp32, normalised) and the per-sample seeds batch["seed"] at res."""
+    if batch.get("img_aug") is not None or batch.get("coord_aug") is not None:
+        return batch["img_aug"], batch["coord_aug"]
+    if batch.get("seed") is None:
+        raise RuntimeError("stego_b200: cfg.aug_alignment_weight > 0 needs batch['seed'] (one seed per sample) or the "
+                           "views batch['img_aug'] / batch['coord_aug']")
+    from .augment import aug_alignment_views, batch_seeds
+    return aug_alignment_views(batch["img"], batch_seeds(batch["seed"]), res)
+
+
 # --------------------------------------------------------------------------------------------------
 # linear probe: 1x1 conv -> bilinear upsample -> masked CE, forward + backward in one fused call
 # --------------------------------------------------------------------------------------------------
@@ -402,10 +414,14 @@ class LitUnsupervisedSegmenter(nn.Module):
 
     # ---- the step ---------------------------------------------------------------------------------
     def training_step(self, batch, batch_idx):
-        """train_segmentation.py:112-245.  The shipped configuration (dino arch, correspondence loss, no rec / aug /
-        crf terms; use_salience, use_true_labels and "KK" included) runs as the hand-scheduled kernel sequence of
-        fused_step.FusedStep; anything else
-        (or cfg.fused_step = False) takes the autograd-stitched path below.  Both compute the same step."""
+        """train_segmentation.py:112-245.  The shipped configuration (dino arch, correspondence loss, no rec / crf
+        terms; use_salience, use_true_labels, "KK" and the aug-alignment term fed by batch["seed"] included) runs as the
+        hand-scheduled kernel sequence of fused_step.FusedStep; anything else (or cfg.fused_step = False) takes the
+        autograd-stitched path below.  Both compute the same step.
+
+        With cfg.aug_alignment_weight > 0 the batch carries either the views batch["img_aug"] / batch["coord_aug"]
+        (the autograd path, with them) or batch["seed"]: B ints, a list or a CPU tensor, from which the step builds
+        the views itself (augment.aug_alignment_views at cfg.res, from the fp32 batch["img"])."""
         self._deliver_histograms()
         if getattr(self.cfg, "fused_step", True):
             if self._fused is None:
@@ -427,6 +443,8 @@ class LitUnsupervisedSegmenter(nn.Module):
         img, img_pos, label = batch["img"], batch["img_pos"], batch["label"]
         B = img.shape[0]
         net = self.net
+        if cfg.aug_alignment_weight > 0:
+            img_aug, coord_aug = aug_views_of(batch, cfg.res)
         fh, fw = img.shape[2] // net.patch_size, img.shape[3] // net.patch_size
         use_pos = cfg.correspondence_weight > 0
 
@@ -503,8 +521,8 @@ class LitUnsupervisedSegmenter(nn.Module):
                 self.log('loss/rec', rec_loss)
                 loss = loss + cfg.rec_weight * rec_loss
             if cfg.aug_alignment_weight > 0:
-                _, code_aug = net(batch["img_aug"])
-                coord = F.interpolate(batch["coord_aug"].permute(0, 3, 1, 2), code_aug.shape[2], mode="bilinear",
+                _, code_aug = net(img_aug)
+                coord = F.interpolate(coord_aug.permute(0, 3, 1, 2), code_aug.shape[2], mode="bilinear",
                                       align_corners=False).permute(0, 2, 3, 1)
                 aug = -pixel_cosine(sample(code, coord), code_aug).mean()
                 self.log('loss/aug_alignment', aug)
