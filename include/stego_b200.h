@@ -47,6 +47,10 @@ STEGO_API long long stego_launch_count(void);
  *   row_div > 0 (patch-embed mode): output row r goes to r + r/row_div + 1 (skips the cls slot of
  *     each image) and the residual row is r % row_div + 1 (positional embedding broadcast).
  *   splits > 1 requires atomic_out = 1: split-K partial sums are atomically added into fp32 `out`.
+ *   atomic_out = 1 computes out += A . B^T only: a bias, act != 0 or a residual is refused.
+ *   Every leading dimension holds a whole row: lda >= K (a_mn_major: >= M), ldb >= K (b_mn_major: >= N),
+ *   ldo >= N and, with a residual, ldr >= N; a shorter one is refused.
+ *   A refused call returns a non-zero status before anything is launched and leaves `out` untouched.
  * ---------------------------------------------------------------------------------------------- */
 STEGO_API int stego_gemm_bf16(const void* A, int lda, int a_mn_major, const void* B, int ldb, int b_mn_major,
                               int M, int N, int K, void* out, int ldo, int out_bf16, const float* bias, int act,
@@ -55,7 +59,8 @@ STEGO_API int stego_gemm_bf16(const void* A, int lda, int a_mn_major, const void
 
 /* `batch` independent GEMMs of one shape in ONE launch: entry b reads A + b * a_batch_stride, B + b * b_batch_stride and
  * writes out + b * out_batch_stride (strides in elements; operand strides multiples of 8).  Rows past M / N of an entry
- * are zero-filled / clipped by TMA, so M and N need not be tile multiples.  This is `tensor_correlation`
+ * are zero-filled / clipped by TMA, so M and N need not be tile multiples; the leading dimensions follow the rules of
+ * stego_gemm_bf16.  This is `tensor_correlation`
  * (src/modules.py:283-284: einsum nchw,ncij->nhwij = one [hw, C] x [C, ij] GEMM per image) for ANY h w, i j — the dense
  * S = h w case of SURVEY.md 8(d) included — with the bf16 hi/lo split folded into K ([hi | lo | hi] . [hi | hi | lo]). */
 STEGO_API int stego_gemm_bf16_batched(const void* A, int lda, long long a_batch_stride, int a_mn_major, const void* B,

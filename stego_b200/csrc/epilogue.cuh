@@ -19,29 +19,13 @@ __device__ __forceinline__ float gelu_erf(float x) {
   return 0.5f * x * (1.0f + copysignf(erf_abs, x));
 }
 
-// MUFU-free variant for bf16 outputs: erf(z) = z * P(z^2) (degree-9 minimax fit on |z| <= 3.2, clamped beyond;
-// |abs err| < 8.2e-6, i.e. < 2e-5 on GELU — two orders below bf16 rounding).  The fc1 epilogue applies GELU to
-// 77 M elements per layer; two MUFU ops per element made it MUFU-bound (16 ops/clk/SM).
-__device__ __forceinline__ float gelu_erf_poly(float x) {
-  const float z = fminf(fabsf(x) * 0.70710678118654752f, 3.2f);
-  const float t = z * z;
-  float p = fmaf(t, -2.4003365851451727e-09f, 1.4192566410626377e-07f);
-  p = fmaf(p, t, -3.73997355423602e-06f);
-  p = fmaf(p, t, 5.846926586228758e-05f);
-  p = fmaf(p, t, -0.0006113043563036988f);
-  p = fmaf(p, t, 0.004584169635313263f);
-  p = fmaf(p, t, -0.025814482266624247f);
-  p = fmaf(p, t, 0.11186436329524356f);
-  p = fmaf(p, t, -0.37570728585235524f);
-  p = fmaf(p, t, 1.1283256165012454f);
-  const float e = fminf(p * z, 1.0f);
-  return 0.5f * x * (1.0f + copysignf(e, x));
-}
-
-// bf16-output GELU, eight elements in lock-step as four fp32 pairs, ~8 instructions per element instead of 13:
-//   erf(|x|/sqrt2) = xc * Q(xc^2), xc = min(|x|, 3.2*sqrt2), Q of degree 8 (minimax fit, |abs err| < 4.3e-5 in
-//   fp32 evaluation — two orders of magnitude below the bf16 rounding of the result), and
-//   gelu(x) = 0.5 x (1 + sign(x) erf(|x|/sqrt2)) = h + |h| * e with h = x/2.
+// bf16-output GELU, MUFU-free (the fc1 epilogue applies GELU to 77 M elements per layer; two MUFU ops per element
+// made it MUFU-bound), eight elements in lock-step as four fp32 pairs, ~9 instructions per element instead of 13:
+//   erf(|x|/sqrt2) ~ e = min(xc * Q(xc^2), 1), xc = min(|x|, 3.2*sqrt2), Q of degree 8 (minimax fit, |abs err| <
+//   4.3e-5 in fp32 evaluation), and gelu(x) = 0.5 x (1 + sign(x) erf(|x|/sqrt2)) = h + |h| * e with h = x/2.
+// The error on GELU is |h| times the erf error: at most ~1e-4 (near |x| = 4.5), an absolute error that does not grow
+// with |x|.  The cap matters: at the clamp xc * Q(xc^2) is 1 + 2.7e-5, which without it made every x below -4.19
+// positive, by an amount growing linearly in |x|.  With it, x below the clamp gives exactly 0 and x above exactly x.
 __device__ __forceinline__ void gelu_erf_poly8(float* x) {
   uint64_t xc[4], u[4], q[4];
 #pragma unroll
@@ -63,7 +47,9 @@ __device__ __forceinline__ void gelu_erf_poly8(float* x) {
 #undef STEGO_POLY_STEP
 #pragma unroll
   for (int j = 0; j < 4; ++j) {
-    const uint64_t e = mul_f32x2(q[j], xc[j]);
+    float e0, e1;
+    unpack_f32x2(mul_f32x2(q[j], xc[j]), e0, e1);
+    const uint64_t e = pack_f32x2(fminf(e0, 1.0f), fminf(e1, 1.0f));
     const float h0 = 0.5f * x[2 * j], h1 = 0.5f * x[2 * j + 1];
     const uint64_t r = fma_f32x2(pack_f32x2(fabsf(h0), fabsf(h1)), e, pack_f32x2(h0, h1));
     unpack_f32x2(r, x[2 * j], x[2 * j + 1]);

@@ -78,7 +78,7 @@ __device__ __forceinline__ void gemm_bias_act(float (&acc)[BN / 2], const GemmPa
     }
   }
   if (p.act == 1) {
-    // bf16 outputs take the MUFU-free polynomial (error far below the bf16 rounding), fp32 outputs the A-S erf
+    // bf16 outputs take the MUFU-free polynomial (absolute error ~1e-4), fp32 outputs the A-S erf (~5e-7)
     if (p.out_bf16) {
 #pragma unroll
       for (int j = 0; j < BN / 2; j += 8) gelu_erf_poly8(acc + j);
@@ -417,6 +417,16 @@ static int gemm_impl(const void* A, int lda, long long a_bs, int a_mn_major, con
   STEGO_CHECK_ARG(!(atomic_out && out_bf16), "stego_gemm_bf16: atomic output must be fp32");
   STEGO_CHECK_ARG(splits >= 1, "stego_gemm_bf16: splits=%d", splits);
   STEGO_CHECK_ARG(splits == 1 || atomic_out, "stego_gemm_bf16: split-K requires atomic_out");
+  // every split adds its partial sum into out: a bias would be added `splits` times, an activation would act on the
+  // partial sums, and the register epilogue's atomics have no residual term
+  STEGO_CHECK_ARG(!atomic_out || (bias == nullptr && act == 0 && residual == nullptr),
+                  "stego_gemm_bf16: atomic_out takes no bias, act or residual (bias=%p act=%d residual=%p)",
+                  (const void*)bias, act, (const void*)residual);
+  STEGO_CHECK_ARG(lda >= (a_mn_major ? M : K) && ldb >= (b_mn_major ? N : K),
+                  "stego_gemm_bf16: lda=%d / ldb=%d shorter than a row (M=%d N=%d K=%d, a_mn_major=%d b_mn_major=%d)",
+                  lda, ldb, M, N, K, a_mn_major, b_mn_major);
+  STEGO_CHECK_ARG(ldo >= N && (residual == nullptr || ldr >= N),
+                  "stego_gemm_bf16: ldo=%d / ldr=%d shorter than a row of N=%d", ldo, ldr, N);
   if (batch == 1) {  // any 16-byte-compatible value: the third coordinate is always 0
     a_bs = static_cast<long long>(a_mn_major ? K : M) * lda;
     b_bs = static_cast<long long>(b_mn_major ? K : N) * ldb;

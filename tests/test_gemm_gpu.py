@@ -131,9 +131,9 @@ def test_gemm_bad_args_raise(cuda_dev):
 
 @pytest.mark.parametrize("mode", ["residual_other", "bf16_out_residual", "atomic", "bias_misaligned"])
 def test_gemm_n1152_without_tma_epilogue(cuda_dev, mode):
-    """N = 1152 (the ViT-B qkv width) takes the wide 128x256 tile with a ragged last column tile; every epilogue
-    variant (residual != out, bf16 output + residual, atomic output, misaligned bias) must clip it correctly and the
-    tensor-map box must match the kernel actually launched (a mismatch hangs on the stage barrier)."""
+    """N = 1152 (the ViT-B qkv width) is nine 128x128 column tiles; every epilogue variant that bypasses the TMA
+    store (residual != out, bf16 output + residual, atomic output, misaligned bias) must write exactly the N columns
+    through the register epilogue."""
     from stego_b200 import ops
     torch.manual_seed(11)
     M, N, K = 300, 1152, 384
