@@ -109,7 +109,7 @@ STEGO_API int stego_attention_probs(const void* qkv, float* probs, int B, int N,
  * operand is always slot 0 and its B operand is slot_of_call[call].
  * Operand tiles: bf16 [2 planes (hi, lo)][nslots][B][R][Cpad] with R = ceil(feature_samples^2 / 128) * 128 rows
  * per (plane, slot, image), i.e. R = 128 for feature_samples <= 11; rows >= feature_samples^2 are zero.  Gradient
- * tiles: fp32 [nslots][B][R][72].
+ * tiles: fp32 [nslots][B][R][96] (one row holds all D <= 96 code channels).
  * ---------------------------------------------------------------------------------------------- */
 /* sample (:287-288) + norm (:275-276): bilinear border/align_corners=True gather at the coords, optional
  * per-(image,channel) scale (the Dropout2d noise of modules.py:116), L2 normalise (eps 1e-10), write
@@ -145,7 +145,7 @@ STEGO_API int stego_corr_loss_fwd(const void* feat_tiles, const void* code_tiles
                                   void* stream);
 /* Backward of the above wrt the normalised code tiles.  gscale [ncalls] = upstream gradient of each call's mean
  * loss; gelem / gcd (optional) = upstream gradients of the unreduced loss / cd elements [ncalls][B][S][S].
- * dtiles: fp32 [nslots][B][128][72], must be zero on entry, receives d(loss)/d(normalised sampled code). */
+ * dtiles: fp32 [nslots][B][128][96], must be zero on entry, receives d(loss)/d(normalised sampled code). */
 STEGO_API int stego_corr_loss_bwd(const void* feat_tiles, const void* code_tiles, int B, int feature_samples, int E,
                                   int D, int nslots, int ncalls, const int* slot_of_call_host,
                                   const float* shifts_host, int pointwise, int zero_clamp, int stabilize,
@@ -172,7 +172,7 @@ STEGO_API int stego_corr_loss_tiled_fwd(const void* feat_tiles, const void* code
                                         const float* shifts_host, int pointwise, int zero_clamp, int stabilize,
                                         float* row_partials, float* row_means, float* stats, float* cd_out,
                                         float* fdc_out, float* loss_out, void* stream);
-/* dtiles: fp32 [nslots][B][R][72], zero on entry.  Two passes recompute fd / cd per block: dB (all slots) then dA
+/* dtiles: fp32 [nslots][B][R][96], zero on entry.  Two passes recompute fd / cd per block: dB (all slots) then dA
  * (slot 0), each with one CTA owning its output rows. */
 STEGO_API int stego_corr_loss_tiled_bwd(const void* feat_tiles, const void* code_tiles, int B, int feature_samples,
                                         int E, int D, int nslots, int ncalls, const int* slot_of_call_host,

@@ -15,8 +15,9 @@ from . import _lib, ops
 
 CODE_PAD = 128   # code channels are zero-padded to two 64-wide k-blocks in the operand tiles
 TILE_ROWS = 128  # feature_samples^2 <= 128
-DT_LD = 72       # row stride of the gradient tiles
+DT_LD = 96       # row stride of the gradient tiles: one row holds every code channel (D <= 96)
 MAX_TILED_FS = 64  # the multi-tile kernels take feature_samples up to 64 (S = 4096 points per image)
+MAX_CALLS = 16     # loss calls per evaluation (intra, inter and one per negative): CL_MAX_CALLS of corr_loss.cu
 TEACHER_WIDTHS = (64, 128, 192, 256, 384, 768)  # operand-tile widths of the teacher signal the sampler takes
 
 
@@ -58,6 +59,9 @@ def _zeros_strided_like(t: torch.Tensor) -> torch.Tensor:
 def _describe(spec, cfg, n_neg: Optional[int]) -> None:
     spec.fs = int(cfg.feature_samples)
     spec.n_neg = int(cfg.neg_samples if n_neg is None else n_neg)
+    if not 0 <= spec.n_neg <= MAX_CALLS - 2:
+        raise RuntimeError(f"stego_b200: neg_samples={spec.n_neg} unsupported (0..{MAX_CALLS - 2}: the loss kernels take "
+                           f"{MAX_CALLS} calls)")
     spec.pointwise = bool(cfg.pointwise)
     spec.zero_clamp = bool(cfg.zero_clamp)
     spec.stabilize = bool(cfg.stabalize)

@@ -32,7 +32,7 @@ namespace stego {
 constexpr int CL_ROWS = 128;     // rows of one operand tile
 constexpr int CL_CODE_PAD = 128; // code channels padded to 2 k-blocks
 constexpr int CL_MAX_CALLS = 16;
-constexpr int CL_DT_LD = 72;     // row stride (floats) of the per-slot gradient tiles
+constexpr int CL_DT_LD = 96;     // row stride (floats) of the per-slot gradient tiles: every code channel (D <= 96)
 constexpr int CT_MAX_FS = 64;    // largest feature_samples (S = 4096 points per image)
 constexpr int CL_PR_BINS = 4096; // score bins of the precision-recall counts (STEGO_PR_BINS)
 

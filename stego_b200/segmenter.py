@@ -254,10 +254,20 @@ class LitUnsupervisedSegmenter(nn.Module):
     """train_segmentation.py:53-383 (the parts on the training hot path)."""
 
     def __init__(self, n_classes, cfg):
+        dim = cfg.dim if cfg.continuous else n_classes
+        # the limits of the probe and correspondence-loss kernels, checked before anything is drawn or built, so that an
+        # unsupported configuration fails here rather than part-way through its first training step
+        if not 1 <= dim <= 96:
+            raise RuntimeError(f"stego_b200: code dim {dim} unsupported (1..96)")
+        if not 1 <= n_classes <= 32:
+            raise RuntimeError(f"stego_b200: n_classes={n_classes} unsupported by the linear probe (1..32)")
+        if not 0 <= cfg.extra_clusters <= 64 - n_classes:
+            raise RuntimeError(f"stego_b200: n_classes + extra_clusters = {n_classes + cfg.extra_clusters} cluster "
+                               f"probe rows unsupported (<= 64)")
+        spec = corr.make_spec(cfg)
         super().__init__()
         self.cfg = cfg
         self.n_classes = n_classes
-        dim = cfg.dim if cfg.continuous else n_classes
         if cfg.arch == "dino":
             self.net = DinoFeaturizer(dim, cfg)
         elif cfg.arch == "feature-pyramid":
@@ -284,7 +294,7 @@ class LitUnsupervisedSegmenter(nn.Module):
         self.global_step = 0
         self.logged: Dict[str, torch.Tensor] = {}
         self._flat: Optional[FlatParams] = None
-        self._spec = corr.make_spec(cfg)
+        self._spec = spec
         self._fused = None
         self.profile_marks = None  # optional list: bench.py --breakdown collects (name, cuda event) pairs here
         # cd histograms every cfg.hist_freq steps (train_segmentation.py:144-146, 165-168) go to

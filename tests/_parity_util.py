@@ -34,14 +34,14 @@ def lr_of(name):
     return 5e-4 if name.startswith("net.") else 5e-3  # train_segmentation.py:379-381
 
 
-def make_model(arch, dev, fused=True, seed=0, **cfg_over):
+def make_model(arch, dev, fused=True, seed=0, n_classes=27, patch=8, **cfg_over):
     import stego_oracle as O
     from stego_b200.config import make_cfg
     from stego_b200.segmenter import LitUnsupervisedSegmenter
-    cfg = make_cfg(model_type=arch, random_backbone_init=True, fused_step=fused, **cfg_over)
+    cfg = make_cfg(model_type=arch, random_backbone_init=True, fused_step=fused, dino_patch_size=patch, **cfg_over)
     torch.manual_seed(seed)
-    model = LitUnsupervisedSegmenter(27, cfg).to(dev)
-    sd = O.perturb_vit_state(O.vit_random_state(arch, 8, seed=3))
+    model = LitUnsupervisedSegmenter(n_classes, cfg).to(dev)
+    sd = O.perturb_vit_state(O.vit_random_state(arch, patch, seed=3))
     model.net.model.load_state_dict(sd)
     model.train()
     model.configure_optimizers()

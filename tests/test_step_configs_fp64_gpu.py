@@ -1,0 +1,285 @@
+"""The hand-scheduled training step (fused_step.FusedStep) in the configurations it accepts beyond the shipped one:
+code widths 1..96, the linear head, dropout off, 3..32 classes with up to 64 cluster rows, patch 16, non-square frames,
+labels at another resolution, batches of 1 and 3, 1 and 14 negatives, and the loss's clamp / centring switches (the
+table in tests/_step_fp64.py).  Per row:
+
+  1. fused path   FusedStep.supported(batch), and _fused.step_idx advances on each step.
+  2. twin         the first step of an autograd twin (cfg.fused_step=False) from the same generator states leaves both
+                  generators where the fused step left them; the positive correspondence terms, their cd means and the
+                  cluster loss are bit-equal (both paths launch the same kernels on the same inputs, and those
+                  reductions run in a fixed order); the linear loss within 1e-6 (fp64 atomics in either order); every
+                  gradient within 3e-3 relative L2 (test_step_parity_gpu.py's bar: atomics in another order, the twin's
+                  own kink sides), except d(clusters) at D = 1, which is exactly 0 (a one-channel centroid normalises
+                  to +-1) and so is held to its absolute fp64 bar in check 3 only.
+  3. fp64         three steps (eager, capture, replay); the replayed step's own tensors against tests/_step_fp64.compose
+                  on the same backbone tokens, noises ws.M1 / M2 / M3, coordinates ws.c1 / c2, permutations ws.perms and
+                  the parameters snapshotted before the step, stage-wise (each stage from what the kernels before it
+                  computed), with the bars the stage tests derive:
+                    head forward   test_head_fp64_gpu._check_forward: x1 / x2 bit-exact, hid within gamma_{E+2} pre_abs
+                                   and one bf16 rounding, code within gamma_{E+3} code_abs, against the exact head within
+                                   6 * 2^-8 prop_abs;
+                    operand tiles  |hi + lo - n| <= E_n + 2^-16 (|n| + E_n) (test_corr_fp64_gpu.py), rows >= S and code
+                                   channels >= D exactly zero;
+                    call stats     E_loss and E_cd_mean of CorrRef;
+                    d(code)        CorrRef's backward bar on ws.dall, whose columns D..P stay exactly zero;
+                    logged terms   neg_inter: sum of the negatives' E_loss / n_neg + gamma_{ncalls} mean |loss_k|
+                                   (stego_step_losses, test_head_fp64_gpu.py section 7); total: sum_k w_k E_loss_k +
+                                   E_lin + E_clu + gamma_{ncalls+3} (sum |w_k loss_k| + |lin| + |clu|);
+                    linear probe   test_probes_fp64_gpu._lce_bars (loss, dW, db) + u |dW| for the final atomic;
+                    cluster probe  test_probes_fp64_gpu._cluster_check's argmax bars: E_ip = (2C + 16) u S, loss within
+                                   mean max_k E_ip + 32 u mean |max ip|, plus 2 max_k E_ip on the pixels whose fp64 top-2
+                                   margin is under 2 max_k E_ip (near ties); dnc within |gs| (L + C/2 + 6) u sum_p |x_hat|,
+                                   L the kernel's atomic chain, plus |gs x_hat| into every candidate row of a near tie;
+                                   dclusters through the normalise backward;
+                    head backward  from the step's d(code): test_fused_step_head_fp64's bars (colsum gamma_{40+blocks},
+                                   split-K wgrad gamma_{64 kbps + splits}, dh gamma_130), dyb and dhb bit-exact.
+  4. padding      ws.ctiles (torch.empty) is NaN-filled when the workspace is made: after the first step nothing logged
+                  or in the flat gradient buffer is NaN and channels D..128 of every code tile are zero; ws.code is
+                  allocated zero-filled and its columns D..P are still exactly zero after the replayed step.
+  5. update       the replayed step's Adam update of every group against _head_fp64.adam from the step's gradients
+                  and the moments before it (test_head_fp64_gpu._adam_ratios).
+
+Largest error / bar ratios go to $STEGO_PARITY_DIR when it is set.
+"""
+import os
+import sys
+
+import pytest
+import torch
+
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+import _corr_fp64 as RC  # noqa: E402
+import _head_fp64 as RH  # noqa: E402
+import _probes_fp64 as RP  # noqa: E402
+import _step_fp64 as S  # noqa: E402
+from _parity_util import rel  # noqa: E402
+from test_head_fp64_gpu import Ratios, _adam_ratios, _check_forward, _colsum_bar, _same_bits, _wgrad_bar  # noqa: E402
+from test_probes_fp64_gpu import _chain, _lce_bars  # noqa: E402
+
+pytestmark = pytest.mark.gpu
+U, G = RH.U, RH.gamma
+NAN = float("nan")
+
+
+def _snapshot(model, which):
+    model.flush()
+    sd = dict(model.named_parameters())
+    return {k: (sd[k].grad if which == "grad" else sd[k]).detach().clone() for k in S.names_of(model)}
+
+
+def _cluster_bars(r, loss, dcl, x, cl, dev):
+    """the step's cluster loss and d(clusters) (argmax mode, upstream gradient 1) against cluster_ref"""
+    B, C, P = x.shape
+    n = cl.shape[0]
+    ref = RP.cluster_ref(x, cl, None, 1.0)
+    ip, Sabs = ref["ip"], ref["S"]
+    E_ip = (2 * C + 16) * U * Sabs
+    Emax = E_ip.amax(1)
+    top = ip.amax(1)
+    near = (ip.topk(2, 1).values[:, 0] - ip.topk(2, 1).values[:, 1]) <= 2 * Emax
+    r["cluster_near_ties"] = int(near.sum())  # recorded, not a ratio
+    loss_bar = (Emax.mean() + 32 * U * top.abs().mean() + (2 * Emax * near.double()).mean()).item()
+    r.add("loss_cluster", loss, torch.tensor(ref["loss"].item()), torch.tensor(loss_bar))
+    xh, gs = ref["xh"], abs(ref["gs"])
+    L = _chain(B * P, dev, x.stride(1) == 1 and n <= 32)
+    cand = ((ip >= top[:, None] - 2 * Emax[:, None]) & near[:, None]).double()
+    D = gs * ((L + C / 2 + 6) * U * torch.einsum("bkp,bcp->kc", ref["dip"].abs(), xh.abs()) +
+              torch.einsum("bkp,bcp->kc", cand, xh.abs()))
+    cd, dnc, ch = cl.double(), ref["dnc"], ref["ch"]
+    nrm = cd.norm(dim=1, keepdim=True)
+    full = (D + ch.abs() * (ch.abs() * D).sum(1, keepdim=True)) / nrm.clamp_min(1e-12) + \
+        (C + 8) * U * (dnc.abs() + ch.abs() * (ch * dnc).sum(1, keepdim=True).abs()) / nrm.clamp_min(1e-12)
+    r.add("dclusters", dcl, ref["dcl"], torch.where(nrm > 1e-12, full, (D + U * dnc.abs()) / 1e-12) + 1e-300)
+
+
+def _fp64_replayed_step(r, model, batch, before, grads, dev):
+    """check 3 (and the ws.code / d(code) padding of check 4) on the replayed step's workspace"""
+    from stego_b200 import ops
+    ws, cfg = model._fused.ws, model.cfg
+    B, E, D, P, fh, fw, hw, M, nonlinear = ws.dims
+    n = model.n_classes
+    with torch.no_grad():  # the same backbone graph the step replayed, on the same images
+        tok = model.net.backbone_tokens([batch["img"], batch["img_pos"]], use_graph=True).reshape(M, E).clone()
+    w = {k: before.get(k) for k in S.HEAD}
+    assert _same_bits(ws.w1p[:D], w["net.cluster1.0.weight"].reshape(D, E).bfloat16())
+    assert (ws.w1p[D:] == 0).all()
+    if nonlinear:
+        assert _same_bits(ws.wab, w["net.cluster2.0.weight"].reshape(E, E).bfloat16())
+        assert _same_bits(ws.wbp[:D], w["net.cluster2.2.weight"].reshape(D, E).bfloat16())
+    M1 = ws.M1.view(2 * B, E)
+    M2 = ws.M2.view(2 * B, E) if nonlinear else None
+    M3 = ws.M3.view(2 * B, E) if ws.M3 is not None else None
+    assert (M3 is not None) == bool(cfg.dropout)
+    x = dict(f=tok, m1=M1, m2=M2, w1=w["net.cluster1.0.weight"], b1=w["net.cluster1.0.bias"],
+             wa=w["net.cluster2.0.weight"], ba=w["net.cluster2.0.bias"], wb=w["net.cluster2.2.weight"],
+             bb=w["net.cluster2.2.bias"])
+    # head forward stage-wise; also: ws.code's columns D..P are still exactly zero (pad=0)
+    _check_forward(r, dict(x1=ws.x1, x2=ws.x2, hid=ws.hid, code=ws.code), x, 2 * B, D, nonlinear, True, pad=0.0)
+
+    ref = S.compose(tok, B, fh, fw, M1, M2, M3, ws.c1, ws.c2, ws.perms, before, ws.label, cfg, n, hid=ws.hid,
+                    code=ws.code)
+    corr, stats = ref["corr"], ref["stats"]
+    Sn = corr.S
+    # operand tiles (the teacher tiles from the features, the code tiles from the step's code)
+    for name, tiles, vals, bars, C in (("ftiles", ws.ftiles, corr.fn, corr.fE, E), ("ctiles", ws.ctiles, corr.cn,
+                                                                                    corr.cE, D)):
+        assert torch.equal(tiles[:, :, :, Sn:], torch.zeros_like(tiles[:, :, :, Sn:])), (name, "rows >= S")
+        assert torch.equal(tiles[..., C:], torch.zeros_like(tiles[..., C:])), (name, "pad channels")
+        hl = tiles.double()[0] + tiles.double()[1]
+        for s in range(corr.nslots):
+            r.add(name, hl[s, :, :Sn, :C], vals[s], bars[s] + RC.SPLIT * (vals[s].abs() + bars[s]))
+    st = ws.stats.double().cpu()
+    for k, s in enumerate(stats):
+        r.add("call_loss", st[k, 0], torch.tensor(s["loss"]), torch.tensor(s["E_loss"]))
+        r.add("call_cd_mean", st[k, 1], torch.tensor(s["cd_mean"]), torch.tensor(s["E_cd_mean"]))
+    # d(code) of the correspondence loss, img rows then img_pos rows; the padding columns stay zero
+    dall = ws.dall.view(M, P)
+    assert (dall[:, D:] == 0).all(), "d(code) padding columns"
+    r.add("dcode", dall[:, :D], ref["dcode"], ref["dcode_bar"])
+    # linear probe (upstream gradient 1, accumulated from zero)
+    code4 = ws.code.view(2 * B, fh, fw, P)[..., :D].permute(0, 3, 1, 2)[:B]
+    LH, LW = ws.label.shape[-2:]
+    lin = ref["lin"]
+    lbar, dW_bar, db_bar = _lce_bars(code4, lin, n, LH, LW)
+    r.add("loss_linear", ws.lin_loss[0].cpu(), lin["loss"].cpu(), torch.tensor(lbar))
+    assert int(ws.lin_loss[1].item()) == lin["count"]
+    r.add("dW_linear", grads["linear_probe.weight"].reshape(n, D), lin["dW"], dW_bar + U * lin["dW"].abs())
+    r.add("db_linear", grads["linear_probe.bias"], lin["db"], db_bar + U * lin["db"].abs())
+    # cluster probe
+    _cluster_bars(r, ws.clu_loss[0].cpu(), grads["cluster_probe.clusters"], code4.reshape(B, D, hw),
+                  before["cluster_probe.clusters"], dev)
+    # the logged terms the step assembles (stego_step_losses)
+    logged = {k: float(v) for k, v in model.logged.items()}
+    cw, nn = S.call_weights(cfg), len(stats) - 2
+    L = ref["losses"]
+    neg_bar = sum(s["E_loss"] for s in stats[2:]) / nn + G(len(stats)) * sum(abs(s["loss"]) for s in stats[2:]) / nn
+    r.add("loss_neg_inter", torch.tensor(logged["loss/neg_inter"]), torch.tensor(L["neg_inter"]), torch.tensor(neg_bar))
+    for key, kk in (("loss/pos_intra", 0), ("loss/pos_inter", 1)):
+        assert logged[key] == float(st[kk, 0])
+    e_lin, e_clu = lbar, r.bars["loss_cluster"]
+    tot_bar = sum(c * s["E_loss"] for c, s in zip(cw, stats)) + e_lin + e_clu + \
+        G(len(stats) + 3) * (sum(abs(c * s["loss"]) for c, s in zip(cw, stats)) + abs(L["linear"]) + abs(L["cluster"]))
+    r.add("loss_total", torch.tensor(logged["loss/total"]), torch.tensor(L["total"]), torch.tensor(tot_bar))
+    # head backward from the step's own d(code)
+    hb = RH.head_backward(dall, ws.x1, ws.x2, ws.hid, ws.wbp, d=D, dh=ws.dh)
+    dyb = torch.zeros(M, 128, dtype=torch.bfloat16, device=dev)
+    dyb[:, :D] = dall[:, :D].bfloat16()
+    assert _same_bits(ws.dyb, dyb), "dyb"
+    sms = torch.cuda.get_device_properties(dev).multi_processor_count
+    wg_d, cs = _wgrad_bar(M, ops.wgrad_splits(M, D, E, sms)), _colsum_bar(M, True)
+    g = {k: grads[k].reshape(grads[k].shape[0], -1).squeeze(1) for k in S.HEAD if k in grads}
+    r.add("db_pad", ws.db_pad, hb["db"], cs * hb["db_abs"])
+    r.add("db1", g["net.cluster1.0.bias"], hb["db"][:D], cs * hb["db_abs"][:D])
+    r.add("dw1", g["net.cluster1.0.weight"], hb["dw1"], wg_d * hb["dw1_abs"])
+    if nonlinear:
+        assert _same_bits(ws.dhb, torch.where(ws.hid.float() > 0, ws.dh, 0.0).bfloat16()), "dhb"
+        wg_e = _wgrad_bar(M, ops.wgrad_splits(M, E, E, sms))
+        r.add("dbb", g["net.cluster2.2.bias"], hb["db"][:D], cs * hb["db_abs"][:D])
+        r.add("dwb", g["net.cluster2.2.weight"], hb["dwb"], wg_d * hb["dwb_abs"])
+        r.add("dh", ws.dh, hb["dh"], G(130) * hb["dh_abs"])
+        r.add("dba", g["net.cluster2.0.bias"], hb["dba"], cs * hb["dba_abs"])
+        r.add("dwa", g["net.cluster2.0.weight"], hb["dwa"], wg_e * hb["dwa_abs"])
+
+
+class StepRatios(Ratios):
+    """Ratios that also keep each scalar bar (the total's bar is built from the parts' bars) and counters"""
+
+    def __init__(self):
+        super().__init__()
+        self.bars = {}
+
+    def add(self, name, got, ref, bar):
+        if bar.numel() == 1:
+            self.bars[name] = float(bar)
+        return super().add(name, got, ref, bar)
+
+    def check(self, tag):
+        counts = {k: self.pop(k) for k in [k for k in self if k.endswith("_near_ties")]}
+        super().check(tag)
+        from _parity_util import record
+        record(tag + "_counts", counts)
+
+
+@pytest.mark.parametrize("name", list(S.CONFIGS))
+def test_step_config(cuda_dev, name, monkeypatch):
+    from stego_b200.fused_step import FusedStep
+    row = S.CONFIGS[name]
+    fused = S.make_model(row, cuda_dev, fused=True)
+    twin = S.make_model(row, cuda_dev, fused=False)
+    names = S.names_of(fused)
+    p0, p0t = _snapshot(fused, "param"), _snapshot(twin, "param")
+    for k in names:
+        assert torch.equal(p0[k], p0t[k]), k
+    batches = [S.make_batch(row, cuda_dev, seed=1), S.make_batch(row, cuda_dev, seed=2)]
+    # 1. the fused path takes every batch of the row
+    for b in batches:
+        assert FusedStep(fused).supported(b), name
+    # 4. the code tiles come from torch.empty: NaN in them must not survive the step
+    alloc = FusedStep._alloc
+
+    def nan_alloc(self, *a, **k):
+        ws = alloc(self, *a, **k)
+        ws.ctiles.fill_(NAN)
+        return ws
+    monkeypatch.setattr(FusedStep, "_alloc", nan_alloc)
+
+    torch.manual_seed(777)
+    gpu_state, cpu_state = torch.cuda.get_rng_state(cuda_dev), torch.get_rng_state()
+    fused.training_step(batches[0], 0)
+    g_f = _snapshot(fused, "grad")
+    torch.cuda.synchronize()
+    assert fused._fused.step_idx == 1
+    after_gpu, after_cpu = torch.cuda.get_rng_state(cuda_dev), torch.get_rng_state()
+    got = {k: v.detach().clone() for k, v in fused.logged.items()}
+    ws = fused._fused.ws
+    D = ws.dims[2]
+    assert all(torch.isfinite(v).all() for v in got.values()), got
+    assert torch.isfinite(fused._flat.grad).all() and torch.isfinite(fused._flat.param).all()
+    assert (ws.ctiles[..., D:] == 0).all(), "code tile channels D..128"
+
+    # 2. the autograd twin from the same generator states
+    torch.cuda.set_rng_state(gpu_state, cuda_dev)
+    torch.set_rng_state(cpu_state)
+    twin.training_step(batches[0], 0)
+    g_t = _snapshot(twin, "grad")
+    torch.cuda.synchronize()
+    assert twin._fused is None
+    assert torch.equal(torch.cuda.get_rng_state(cuda_dev), after_gpu), "CUDA generator consumption differs"
+    assert torch.equal(torch.get_rng_state(), after_cpu), "CPU generator consumption differs"
+    want = {k: v.detach().clone() for k, v in twin.logged.items()}
+    for key in ("loss/pos_intra", "loss/pos_inter", "cd/pos_intra", "cd/pos_inter", "loss/cluster"):
+        assert torch.equal(got[key], want[key]), (key, got[key].item(), want[key].item())
+    lin_f, lin_t = got["loss/linear"].item(), want["loss/linear"].item()
+    assert abs(lin_f - lin_t) <= 1e-6 * abs(lin_t), (lin_f, lin_t)
+    twin_rel = {k: rel(g_f[k], g_t[k]) for k in names}
+    for k in names:
+        if k == "cluster_probe.clusters" and D == 1:
+            # a one-channel centroid normalises to +-1 whatever its value: the exact gradient is 0 and both paths hold
+            # rounding noise, which the fp64 check below bounds absolutely
+            continue
+        assert twin_rel[k] < 3e-3, (k, twin_rel)
+
+    # 3. + 5. eager, capture, replay; the replayed step against fp64
+    fused.training_step(batches[1], 1)
+    assert fused._fused.step_idx == 2
+    before = _snapshot(fused, "param")  # flushes: the parameters the replayed step runs with
+    flat = fused._flat
+    state0 = [t.clone() for t in (flat.param, flat.exp_avg, flat.exp_avg_sq)]
+    steps0 = [o.steps for o in flat.optimizers]
+    fused.training_step(batches[0], 2)
+    grads = _snapshot(fused, "grad")  # flushes
+    torch.cuda.synchronize()
+    assert fused._fused.step_idx == 3
+    ws = fused._fused.ws
+    assert ws.graph is not None and ws.eager_steps == 1, "the compared step must be a graph replay"
+    r = StepRatios()
+    _fp64_replayed_step(r, fused, batches[0], before, grads, cuda_dev)
+    g_all = flat.grad.clone()
+    for grp, opt, s0 in zip(flat.groups, flat.optimizers, steps0):
+        sl = slice(grp.start, grp.start + grp.numel)
+        assert opt.steps == s0 + 1
+        _adam_ratios(r, [t[sl] for t in (state0[0], g_all, state0[1], state0[2])],
+                     [t[sl] for t in (flat.param, flat.exp_avg, flat.exp_avg_sq)], opt.steps, grp.lr, flat.grad_scale)
+    from _parity_util import record
+    record(f"step_configs_{name}_twin", twin_rel)
+    r.check(f"step_configs_fp64_{name}")
