@@ -111,13 +111,16 @@ class CorrRef:
 
     cfg: anything with pointwise, zero_clamp, stabalize, feature_samples, neg_samples and the three shifts.
     vec8: the feature tiles come from sample_norm_vec8_kernel (only the sum-of-squares chain length differs).
-    hi: the stabalize clamp bound, 0.8 in fp32 as the kernels hold it (the fp64 oracle clamps at 0.8 in fp64)."""
+    hi: the stabalize clamp bound, 0.8 in fp32 as the kernels hold it (the fp64 oracle clamps at 0.8 in fp64).
+    The teacher feats may lie on another grid than the code (the one-hot label maps of use_true_labels, at label
+    resolution): each is sampled with the taps of its own size, at the same normalised coordinates."""
 
     def __init__(self, feats, feats_pos, code, code_pos, coords1, coords2, perms, cfg, chan_scale=None,
                  chan_scale_pos=None, raw_perms=False, vec8=False, hi=HI):
         self.cfg = cfg
-        self.B, self.E, self.H, self.W = feats.shape
-        self.D = code.shape[1]
+        self.B, self.E = feats.shape[:2]
+        self.D, self.H, self.W = code.shape[1:]
+        FH, FW = feats.shape[2:]
         self.fs = int(cfg.feature_samples)
         self.S = self.fs * self.fs
         self.n_neg = int(cfg.neg_samples)
@@ -134,15 +137,16 @@ class CorrRef:
         ar = torch.arange(B, device=self.dev)
         pr = resolve_perms(perms, B, raw_perms) if self.n_neg else None
         t1, t2 = taps(coords1, self.H, self.W), taps(coords2, self.H, self.W)
+        f1, f2 = (t1, t2) if (FH, FW) == (self.H, self.W) else (taps(coords1, FH, FW), taps(coords2, FH, FW))
         self.code, self.code_pos = code, code_pos
-        # per slot: (image of each b, taps, feature source, code source, chan_scale)
-        self.slots = [(ar, t1, feats, code, chan_scale), (ar, t2, feats_pos, code_pos, chan_scale_pos)]
+        # per slot: (image of each b, code taps, feature source, code source, chan_scale, feature taps)
+        self.slots = [(ar, t1, feats, code, chan_scale, f1), (ar, t2, feats_pos, code_pos, chan_scale_pos, f2)]
         for k in range(self.n_neg):
-            self.slots.append((pr[k].to(self.dev), t2, feats, code, chan_scale))
+            self.slots.append((pr[k].to(self.dev), t2, feats, code, chan_scale, f2))
         Lf, Lc = chain_norm(self.E, vec8), chain_norm(self.D)
         self.fn, self.fE, self.cn, self.cE, self.cv, self.cA, self.cnrm = [], [], [], [], [], [], []
-        for img, (idx, w), fsrc, csrc, cs in self.slots:
-            v, A = gather_sample(fsrc, img, idx, w, cs)
+        for img, (idx, w), fsrc, csrc, cs, (fidx, fw) in self.slots:
+            v, A = gather_sample(fsrc, img, fidx, fw, cs)
             n, E, _ = normalise(v, A, Lf)
             self.fn.append(n)
             self.fE.append(E)
@@ -304,7 +308,7 @@ class CorrRef:
         z = lambda c: torch.zeros(B * HW, c, dtype=torch.float64, device=self.dev)  # pixel-major accumulators
         out, Eo, Ao, hits = ({False: z(c), True: z(c)} for c in (D, D, D, 1))
         self.dv, self.Edv = [], []
-        for s, (img, (idx, w), _, _, _) in enumerate(self.slots):
+        for s, (img, (idx, w), _, _, _, _) in enumerate(self.slots):
             v, A, nrm, gg, Eg_ = self.cv[s], self.cA[s], self.cnrm[s], g[s], Eg[s]
             delta = 5 * U * A
             den = nrm.clamp_min(EPS)
@@ -335,6 +339,7 @@ class CorrRef:
             bar = Eo[pos] + (hits[pos] + 2) * U * Ao[pos]
             res.append((nchw(out[pos]), nchw(bar)))
         self.hits = (nchw(hits[False]), nchw(hits[True]))
+        self.Ao = (nchw(Ao[False]), nchw(Ao[True]))  # sum |w dv| per element: what its fp32 accumulator rounds against
         return res
 
 

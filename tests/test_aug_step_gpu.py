@@ -15,7 +15,7 @@ Bars (u = 2^-24).  grid: ATen's lambdas are exact here (scale = 8), so each valu
 numbers of magnitude <= m = max|coord_aug|: 6 u m.  sampled, restated in fp64 at the kernel's own grid: the source
 position ((g + 1) / 2) (h - 1) is formed with three roundings, |dx| <= 3 u h; the weights (x1 - x)(y1 - y) then move by
 <= 2 (3 u h) + 3 u, and the sum of four products adds 4 u; with c = max|code| the bar is c (4 (6 u h + 3 u) + 4 u).
-d(code): each element is a sum of k contributions w g (k counted from the grid: _tap_counts) made in any order by the
+d(code): each element is a sum of k contributions w g (k counted from the grid: _step_fp64.tap_counts) made in any order by the
 atomics; with A the fp64 sum of |w g| (grid_sample's backward of |g|) the sum costs (k + 1) u A.  The weights are
 formed in fp32 from the fp32 position: each factor is off by <= 3 u h + 2 u, the product by <= (6 h + 8) u absolute
 (a weight near 0 has no relative bound), which adds k (6 h + 8) u max|g|.  d(code_aug) is the cosine
@@ -39,6 +39,7 @@ import torch
 import torch.nn.functional as F
 
 from _parity_util import NAMES, grads_of, make_batch, make_model, rel
+from _step_fp64 import aug_grid_bar, aug_sampled_bar, aug_scatter_bar
 
 pytestmark = pytest.mark.gpu
 U = 2.0 ** -24
@@ -107,24 +108,6 @@ def _torch_ref(coord, code):
     return grid, F.grid_sample(code, grid.permute(0, 2, 1, 3), padding_mode="border", align_corners=True)
 
 
-def _tap_counts(grid, h):
-    """[B, 1, h, h] -> how many non-zero-weight taps of the grid land on each code element (d(code)'s atomics)."""
-    g = grid.double().permute(0, 2, 1, 3)  # the point output (p, q) reads
-    x = (((g[..., 0] + 1) / 2) * (h - 1)).clamp(0, h - 1)
-    y = (((g[..., 1] + 1) / 2) * (h - 1)).clamp(0, h - 1)
-    x0, y0 = x.floor(), y.floor()
-    B = grid.shape[0]
-    cnt = torch.zeros(B, h * h, dtype=torch.float64, device=grid.device)
-    for dy in (0, 1):
-        for dx in (0, 1):
-            wx = (x - x0) if dx else (x0 + 1 - x)
-            wy = (y - y0) if dy else (y0 + 1 - y)
-            xi, yi = (x0 + dx).clamp(max=h - 1).long(), (y0 + dy).clamp(max=h - 1).long()
-            live = ((wx * wy) != 0) & (x0 + dx <= h - 1) & (y0 + dy <= h - 1)
-            cnt.scatter_add_(1, (yi * h + xi).reshape(B, -1), live.double().reshape(B, -1))
-    return cnt.view(B, 1, h, h)
-
-
 def _bits(t):
     return t.contiguous().view(torch.int32)
 
@@ -152,13 +135,11 @@ def test_kernels_vs_torch_and_fp64(cuda_dev, h, layout, coords):
     tgrid, tsampled = _torch_ref(coord, code)
     assert torch.equal(_bits(grid), _bits(tgrid)), int((_bits(grid) != _bits(tgrid)).sum())
     assert torch.equal(_bits(sampled), _bits(tsampled)), int((_bits(sampled) != _bits(tsampled)).sum())
-    c = code.abs().max().item()
-    sbar = c * (4 * (6 * U * h + 3 * U) + 4 * U)
+    sbar = aug_sampled_bar(code, h)
 
     # fp64 restatement
     g64 = F.interpolate(coord.double().permute(0, 3, 1, 2), h, mode="bilinear", align_corners=False).permute(0, 2, 3, 1)
-    m = coord.abs().max().item()
-    assert (grid.double() - g64).abs().max().item() <= 6 * U * m
+    assert (grid.double() - g64).abs().max().item() <= aug_grid_bar(coord)
     code64 = code.double().requires_grad_(True)
     s64 = F.grid_sample(code64, grid.double().permute(0, 2, 1, 3), padding_mode="border", align_corners=True)
     assert (sampled.double() - s64).abs().max().item() <= sbar
@@ -194,9 +175,7 @@ def test_kernels_vs_torch_and_fp64(cuda_dev, h, layout, coords):
     code64c = code.double().requires_grad_(True)
     sa = F.grid_sample(code64c, grid.double().permute(0, 2, 1, 3), padding_mode="border", align_corners=True)
     (sa * dsampled.double().abs()).sum().backward()
-    A = code64c.grad
-    k = _tap_counts(grid, h)
-    bar = (k + 1) * U * A + k * (6 * h + 8) * U * dsampled.abs().max().item() + 1e-30
+    bar = aug_scatter_bar(grid, code64c.grad, dsampled, h)
     err = (dcode.double() - code64b.grad).abs()
     assert bool((err <= bar).all()), float((err / bar).max())
     # and against torch's fp32 grid_sample backward (atomics in another order): the same bar

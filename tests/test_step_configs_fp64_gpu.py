@@ -50,9 +50,12 @@ import torch
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import _corr_fp64 as RC  # noqa: E402
 import _head_fp64 as RH  # noqa: E402
+import _loss_terms_fp64 as RL  # noqa: E402
 import _probes_fp64 as RP  # noqa: E402
 import _step_fp64 as S  # noqa: E402
 from _parity_util import rel  # noqa: E402
+from stego_b200 import hist as hist_mod  # noqa: E402
+from test_loss_terms_fp64_gpu import cos_bars  # noqa: E402
 from test_head_fp64_gpu import Ratios, _adam_ratios, _check_forward, _colsum_bar, _same_bits, _wgrad_bar  # noqa: E402
 from test_probes_fp64_gpu import _chain, _lce_bars  # noqa: E402
 
@@ -92,37 +95,53 @@ def _cluster_bars(r, loss, dcl, x, cl, dev):
     r.add("dclusters", dcl, ref["dcl"], torch.where(nrm > 1e-12, full, (D + U * dnc.abs()) / 1e-12) + 1e-300)
 
 
-def _fp64_replayed_step(r, model, batch, before, grads, dev):
-    """check 3 (and the ws.code / d(code) padding of check 4) on the replayed step's workspace"""
-    from stego_b200 import ops
+def _fp64_replayed_step(r, model, batch, before, grads, dev, hist=False):
+    """check 3 (and the ws.code / d(code) padding of check 4) on the replayed step's workspace; with the modes (see
+    tests/test_step_modes_fp64_gpu.py) also the label teacher tiles, the aug-alignment term over 3B rows and (hist) the
+    cd histograms the replayed histogram graph binned"""
+    from stego_b200 import augment, ops
     ws, cfg = model._fused.ws, model.cfg
     B, E, D, P, fh, fw, hw, M, nonlinear = ws.dims
+    nI = ws.n_img
     n = model.n_classes
+    parts = [batch["img"], batch["img_pos"]]
+    aug = None
+    if ws.aug:  # the views the step built from the seeds, bit for bit; the backbone graph read img_aug as its input
+        img_aug, coord_aug = augment.aug_alignment_views(batch["img"], augment.batch_seeds(batch["seed"]), cfg.res)
+        assert _same_bits(ws.coord_aug, coord_aug), "coord_aug"
+        static_in = model.net.model.graph_input(model.net.feat_type, (3 * B,) + tuple(batch["img"].shape[1:]), dev)
+        assert static_in is not None and _same_bits(static_in[2 * B:], img_aug), "img_aug"
+        parts.append(img_aug)
+        aug = dict(coord=ws.coord_aug, w=float(cfg.aug_alignment_weight), grid=ws.grid, dsampled=ws.dsampled)
     with torch.no_grad():  # the same backbone graph the step replayed, on the same images
-        tok = model.net.backbone_tokens([batch["img"], batch["img_pos"]], use_graph=True).reshape(M, E).clone()
+        tok = model.net.backbone_tokens(parts, use_graph=True).reshape(M, E).clone()
     w = {k: before.get(k) for k in S.HEAD}
     assert _same_bits(ws.w1p[:D], w["net.cluster1.0.weight"].reshape(D, E).bfloat16())
     assert (ws.w1p[D:] == 0).all()
     if nonlinear:
         assert _same_bits(ws.wab, w["net.cluster2.0.weight"].reshape(E, E).bfloat16())
         assert _same_bits(ws.wbp[:D], w["net.cluster2.2.weight"].reshape(D, E).bfloat16())
-    M1 = ws.M1.view(2 * B, E)
-    M2 = ws.M2.view(2 * B, E) if nonlinear else None
-    M3 = ws.M3.view(2 * B, E) if ws.M3 is not None else None
+    M1 = ws.M1.view(nI * B, E)
+    M2 = ws.M2.view(nI * B, E) if nonlinear else None
+    M3 = ws.M3.view(nI * B, E) if ws.M3 is not None else None
     assert (M3 is not None) == bool(cfg.dropout)
     x = dict(f=tok, m1=M1, m2=M2, w1=w["net.cluster1.0.weight"], b1=w["net.cluster1.0.bias"],
              wa=w["net.cluster2.0.weight"], ba=w["net.cluster2.0.bias"], wb=w["net.cluster2.2.weight"],
              bb=w["net.cluster2.2.bias"])
     # head forward stage-wise; also: ws.code's columns D..P are still exactly zero (pad=0)
-    _check_forward(r, dict(x1=ws.x1, x2=ws.x2, hid=ws.hid, code=ws.code), x, 2 * B, D, nonlinear, True, pad=0.0)
+    _check_forward(r, dict(x1=ws.x1, x2=ws.x2, hid=ws.hid, code=ws.code), x, nI * B, D, nonlinear, True, pad=0.0)
 
+    edges = torch.from_numpy(hist_mod.default_bins().copy()) if hist else None
     ref = S.compose(tok, B, fh, fw, M1, M2, M3, ws.c1, ws.c2, ws.perms, before, ws.label, cfg, n, hid=ws.hid,
-                    code=ws.code)
+                    code=ws.code, label_pos=ws.label_pos, aug=aug, hist_edges=edges)
     corr, stats = ref["corr"], ref["stats"]
     Sn = corr.S
-    # operand tiles (the teacher tiles from the features, the code tiles from the step's code)
-    for name, tiles, vals, bars, C in (("ftiles", ws.ftiles, corr.fn, corr.fE, E), ("ctiles", ws.ctiles, corr.cn,
-                                                                                    corr.cE, D)):
+    assert ws.ftiles.shape[-1] == ws.ET and corr.E == ws.ET
+    if ws.label_pos is not None:  # the one-hot teacher: channels n + 1 .. ET are exactly zero
+        assert torch.equal(ws.ftiles[..., n + 1:], torch.zeros_like(ws.ftiles[..., n + 1:])), "label tile channels"
+    # operand tiles (the teacher tiles from the features or labels, the code tiles from the step's code)
+    for name, tiles, vals, bars, C in (("ftiles", ws.ftiles, corr.fn, corr.fE, ws.ET), ("ctiles", ws.ctiles, corr.cn,
+                                                                                         corr.cE, D)):
         assert torch.equal(tiles[:, :, :, Sn:], torch.zeros_like(tiles[:, :, :, Sn:])), (name, "rows >= S")
         assert torch.equal(tiles[..., C:], torch.zeros_like(tiles[..., C:])), (name, "pad channels")
         hl = tiles.double()[0] + tiles.double()[1]
@@ -132,12 +151,38 @@ def _fp64_replayed_step(r, model, batch, before, grads, dev):
     for k, s in enumerate(stats):
         r.add("call_loss", st[k, 0], torch.tensor(s["loss"]), torch.tensor(s["E_loss"]))
         r.add("call_cd_mean", st[k, 1], torch.tensor(s["cd_mean"]), torch.tensor(s["E_cd_mean"]))
-    # d(code) of the correspondence loss, img rows then img_pos rows; the padding columns stay zero
+    # d(code): the correspondence loss's into the img and img_pos rows (plus the aug term's scatter into the img rows,
+    # and its cosine backward into the img_aug rows); the padding columns stay zero
     dall = ws.dall.view(M, P)
     assert (dall[:, D:] == 0).all(), "d(code) padding columns"
-    r.add("dcode", dall[:, :D], ref["dcode"], ref["dcode_bar"])
+    rows = slice(0, 2 * B * hw)
+    bar = ref["dcode_bar"][rows]
+    if ws.aug:
+        a = ref["aug"]
+        rm = lambda t: t.permute(0, 2, 3, 1).reshape(B * hw, -1)
+        code_img = ws.code.view(nI * B, fh, fw, P)[:B, ..., :D].permute(0, 3, 1, 2)
+        code_aug = ws.code.view(nI * B, fh, fw, P)[2 * B:, ..., :D].permute(0, 3, 1, 2)
+        r.add("aug_grid", ws.grid, a["grid"], torch.tensor(S.aug_grid_bar(ws.coord_aug), device=dev))
+        r.add("aug_sampled", ws.sampled, a["sampled"], torch.tensor(S.aug_sampled_bar(code_img, fh), device=dev))
+        cref = RL.pixel_cosine(ws.sampled, code_aug, ga=ws.dcos)
+        dcos_bar, cbars = cos_bars(cref, D, False, ws.dcos)
+        r.add("aug_cos", ws.cosv, cref["cos"], dcos_bar)
+        r.add("aug_dsampled", ws.dsampled, cref["da"], cbars["da"])
+        r.add("dcode_aug_rows", dall[2 * B * hw:, :D], rm(cref["db"]), rm(cbars["db"]))
+        aug_loss = float(ws.aug_loss[0])
+        assert aug_loss == float(torch.tensor(-ws.cosv.double().mean().item(), dtype=torch.float32))
+        e_aug = dcos_bar.mean().item() + U * abs(aug_loss)
+        r.add("loss_aug_alignment", torch.tensor(aug_loss), torch.tensor(-cref["cos"].mean().item()),
+              torch.tensor(e_aug))
+        assert float(model.logged["loss/aug_alignment"]) == aug_loss
+        # the scatter's bar, and the cross terms of sharing the img rows' fp32 accumulators with the correspondence
+        # loss's gather (k more additions onto its sum of |terms|, its hits more onto the scatter's)
+        k = S.tap_counts(ws.grid, fh)
+        sc = S.aug_scatter_bar(ws.grid, a["A"], ws.dsampled, fh) + k * U * corr.Ao[0] + corr.hits[0] * U * a["A"]
+        bar = torch.cat([rm(sc) + bar[:B * hw], bar[B * hw:]])
+    r.add("dcode", dall[rows, :D], ref["dcode"][rows], bar)
     # linear probe (upstream gradient 1, accumulated from zero)
-    code4 = ws.code.view(2 * B, fh, fw, P)[..., :D].permute(0, 3, 1, 2)[:B]
+    code4 = ws.code.view(nI * B, fh, fw, P)[..., :D].permute(0, 3, 1, 2)[:B]
     LH, LW = ws.label.shape[-2:]
     lin = ref["lin"]
     lbar, dW_bar, db_bar = _lce_bars(code4, lin, n, LH, LW)
@@ -148,7 +193,7 @@ def _fp64_replayed_step(r, model, batch, before, grads, dev):
     # cluster probe
     _cluster_bars(r, ws.clu_loss[0].cpu(), grads["cluster_probe.clusters"], code4.reshape(B, D, hw),
                   before["cluster_probe.clusters"], dev)
-    # the logged terms the step assembles (stego_step_losses)
+    # the logged terms the step assembles (stego_step_losses, then w * aug onto the total)
     logged = {k: float(v) for k, v in model.logged.items()}
     cw, nn = S.call_weights(cfg), len(stats) - 2
     L = ref["losses"]
@@ -158,9 +203,16 @@ def _fp64_replayed_step(r, model, batch, before, grads, dev):
         assert logged[key] == float(st[kk, 0])
     e_lin, e_clu = lbar, r.bars["loss_cluster"]
     tot_bar = sum(c * s["E_loss"] for c, s in zip(cw, stats)) + e_lin + e_clu + \
-        G(len(stats) + 3) * (sum(abs(c * s["loss"]) for c, s in zip(cw, stats)) + abs(L["linear"]) + abs(L["cluster"]))
-    r.add("loss_total", torch.tensor(logged["loss/total"]), torch.tensor(L["total"]), torch.tensor(tot_bar))
-    # head backward from the step's own d(code)
+        G(len(stats) + 5) * (sum(abs(c * s["loss"]) for c, s in zip(cw, stats)) + abs(L["linear"]) + abs(L["cluster"]))
+    want_total = L["total"]
+    if ws.aug:  # stage-wise: the step's own aug loss, weighted in fp32
+        wa = float(cfg.aug_alignment_weight)
+        want_total += wa * (aug_loss - L["aug_alignment"])
+        tot_bar += abs(wa) * e_aug + G(3) * abs(wa * aug_loss)
+    r.add("loss_total", torch.tensor(logged["loss/total"]), torch.tensor(want_total), torch.tensor(tot_bar))
+    if hist:
+        _hist_checks(r, ws.hist, ref["hist"])
+    # head backward from the step's own d(code), over all nB rows
     hb = RH.head_backward(dall, ws.x1, ws.x2, ws.hid, ws.wbp, d=D, dh=ws.dh)
     dyb = torch.zeros(M, 128, dtype=torch.bfloat16, device=dev)
     dyb[:, :D] = dall[:, :D].bfloat16()
@@ -179,6 +231,29 @@ def _fp64_replayed_step(r, model, batch, before, grads, dev):
         r.add("dh", ws.dh, hb["dh"], G(130) * hb["dh_abs"])
         r.add("dba", g["net.cluster2.0.bias"], hb["dba"], cs * hb["dba_abs"])
         r.add("dwa", g["net.cluster2.0.weight"], hb["dwa"], wg_e * hb["dwa_abs"])
+
+
+def _hist_checks(r, h, want):
+    """the counts the histogram graph binned against the fp64 binning: at every bucket edge, the number of elements
+    below it lies between those certainly below (cd + E_cd under the edge) and those possibly below (cd - E_cd under
+    it), so only elements within their cd bar of an edge may move; the group sizes exactly; min / max within max E_cd,
+    sum within sum E_cd, the sum of squares within sum E_cd (2 |cd| + E_cd), each plus fp64 summation slack"""
+    counts, stats = h.counts.cpu(), h.stats.cpu()
+    r["hist_ambiguous_near_ties"] = sum(g["ambiguous"] for g in want)
+    for gi, g in enumerate(want):
+        got = counts[gi]
+        assert int(got.sum()) == g["num"] == h.num[gi], (gi, int(got.sum()), g["num"])
+        cum = got.cumsum(0)
+        lo_ok = bool((g["hi"].cpu().cumsum(0) <= cum).all())
+        hi_ok = bool((cum <= g["lo"].cpu().cumsum(0)).all())
+        assert lo_ok and hi_ok, (gi, "histogram counts outside the fp64 edge brackets")
+        if g["ambiguous"] == 0:
+            assert torch.equal(got, g["counts"].cpu()), gi
+        slack = 1e-12 * g["abs_sum"]
+        r.add("hist_min", stats[gi, 0], torch.tensor(g["min"]), torch.tensor(g["E_minmax"]))
+        r.add("hist_max", stats[gi, 1], torch.tensor(g["max"]), torch.tensor(g["E_minmax"]))
+        r.add("hist_sum", stats[gi, 2], torch.tensor(g["sum"]), torch.tensor(g["E_sum"] + slack))
+        r.add("hist_sumsq", stats[gi, 3], torch.tensor(g["sumsq"]), torch.tensor(g["E_sumsq"] + 1e-12 * g["sumsq"]))
 
 
 class StepRatios(Ratios):
@@ -200,20 +275,34 @@ class StepRatios(Ratios):
         record(tag + "_counts", counts)
 
 
-@pytest.mark.parametrize("name", list(S.CONFIGS))
-def test_step_config(cuda_dev, name, monkeypatch):
+class _Recorder:
+    def __init__(self):
+        self.calls = []
+
+    def add_histogram_raw(self, tag, **kw):
+        self.calls.append((tag, kw))
+
+
+def run_row(row, tag, dev, monkeypatch):
+    """checks 1-5 on one row of tests/_step_fp64.py (CONFIGS or MODE_CONFIGS); returns the fused model, its batches and
+    the ratios.  hist rows get a logger: step 0 is eager, step 1 captures the histogram graph, step 2 replays it."""
+    from types import SimpleNamespace
+    from stego_b200 import augment
     from stego_b200.fused_step import FusedStep
-    row = S.CONFIGS[name]
-    fused = S.make_model(row, cuda_dev, fused=True)
-    twin = S.make_model(row, cuda_dev, fused=False)
+    fused = S.make_model(row, dev, fused=True)
+    twin = S.make_model(row, dev, fused=False)
+    hist = bool(row.get("hist"))
+    if hist:
+        for m in (fused, twin):
+            m.logger = SimpleNamespace(experiment=_Recorder())
     names = S.names_of(fused)
     p0, p0t = _snapshot(fused, "param"), _snapshot(twin, "param")
     for k in names:
         assert torch.equal(p0[k], p0t[k]), k
-    batches = [S.make_batch(row, cuda_dev, seed=1), S.make_batch(row, cuda_dev, seed=2)]
+    batches = [S.make_batch(row, dev, seed=1), S.make_batch(row, dev, seed=2)]
     # 1. the fused path takes every batch of the row
     for b in batches:
-        assert FusedStep(fused).supported(b), name
+        assert FusedStep(fused).supported(b), tag
     # 4. the code tiles come from torch.empty: NaN in them must not survive the step
     alloc = FusedStep._alloc
 
@@ -224,28 +313,37 @@ def test_step_config(cuda_dev, name, monkeypatch):
     monkeypatch.setattr(FusedStep, "_alloc", nan_alloc)
 
     torch.manual_seed(777)
-    gpu_state, cpu_state = torch.cuda.get_rng_state(cuda_dev), torch.get_rng_state()
+    gpu_state, cpu_state = torch.cuda.get_rng_state(dev), torch.get_rng_state()
     fused.training_step(batches[0], 0)
     g_f = _snapshot(fused, "grad")
     torch.cuda.synchronize()
     assert fused._fused.step_idx == 1
-    after_gpu, after_cpu = torch.cuda.get_rng_state(cuda_dev), torch.get_rng_state()
+    after_gpu, after_cpu = torch.cuda.get_rng_state(dev), torch.get_rng_state()
     got = {k: v.detach().clone() for k, v in fused.logged.items()}
     ws = fused._fused.ws
     D = ws.dims[2]
+    coords = (ws.c1.clone(), ws.c2.clone())
     assert all(torch.isfinite(v).all() for v in got.values()), got
     assert torch.isfinite(fused._flat.grad).all() and torch.isfinite(fused._flat.param).all()
     assert (ws.ctiles[..., D:] == 0).all(), "code tile channels D..128"
+    if ws.aug:  # before the backbone graph exists the views are built into ws.img_aug
+        img_aug, coord_aug = augment.aug_alignment_views(batches[0]["img"], batches[0]["seed"], fused.cfg.res)
+        assert _same_bits(ws.img_aug, img_aug) and _same_bits(ws.coord_aug, coord_aug), "aug views"
 
-    # 2. the autograd twin from the same generator states
-    torch.cuda.set_rng_state(gpu_state, cuda_dev)
+    # 2. the autograd twin from the same generator states, its coordinates recorded where it draws them
+    drawn = []
+    lossfn = twin.contrastive_corr_loss_fn
+    orig_draw = lossfn.draw_coords
+    monkeypatch.setattr(lossfn, "draw_coords", lambda *a: drawn.append(orig_draw(*a)) or drawn[-1])
+    torch.cuda.set_rng_state(gpu_state, dev)
     torch.set_rng_state(cpu_state)
     twin.training_step(batches[0], 0)
     g_t = _snapshot(twin, "grad")
     torch.cuda.synchronize()
     assert twin._fused is None
-    assert torch.equal(torch.cuda.get_rng_state(cuda_dev), after_gpu), "CUDA generator consumption differs"
+    assert torch.equal(torch.cuda.get_rng_state(dev), after_gpu), "CUDA generator consumption differs"
     assert torch.equal(torch.get_rng_state(), after_cpu), "CPU generator consumption differs"
+    assert len(drawn) == 1 and all(_same_bits(a, b) for a, b in zip(coords, drawn[0])), "coordinates differ"
     want = {k: v.detach().clone() for k, v in twin.logged.items()}
     for key in ("loss/pos_intra", "loss/pos_inter", "cd/pos_intra", "cd/pos_inter", "loss/cluster"):
         assert torch.equal(got[key], want[key]), (key, got[key].item(), want[key].item())
@@ -262,6 +360,9 @@ def test_step_config(cuda_dev, name, monkeypatch):
     # 3. + 5. eager, capture, replay; the replayed step against fp64
     fused.training_step(batches[1], 1)
     assert fused._fused.step_idx == 2
+    ws = fused._fused.ws
+    graphs = (ws.graph, ws.hist_graph)
+    assert (graphs[1] if hist else graphs[0]) is not None and (graphs[0] if hist else graphs[1]) is None
     before = _snapshot(fused, "param")  # flushes: the parameters the replayed step runs with
     flat = fused._flat
     state0 = [t.clone() for t in (flat.param, flat.exp_avg, flat.exp_avg_sq)]
@@ -270,16 +371,22 @@ def test_step_config(cuda_dev, name, monkeypatch):
     grads = _snapshot(fused, "grad")  # flushes
     torch.cuda.synchronize()
     assert fused._fused.step_idx == 3
-    ws = fused._fused.ws
-    assert ws.graph is not None and ws.eager_steps == 1, "the compared step must be a graph replay"
+    assert fused._fused.ws is ws and (ws.graph, ws.hist_graph) == graphs and ws.eager_steps == 1, \
+        "the compared step must replay the graph the step before captured"
     r = StepRatios()
-    _fp64_replayed_step(r, fused, batches[0], before, grads, cuda_dev)
+    _fp64_replayed_step(r, fused, batches[0], before, grads, dev, hist=hist)
     g_all = flat.grad.clone()
     for grp, opt, s0 in zip(flat.groups, flat.optimizers, steps0):
         sl = slice(grp.start, grp.start + grp.numel)
         assert opt.steps == s0 + 1
         _adam_ratios(r, [t[sl] for t in (state0[0], g_all, state0[1], state0[2])],
                      [t[sl] for t in (flat.param, flat.exp_avg, flat.exp_avg_sq)], opt.steps, grp.lr, flat.grad_scale)
+    return dict(fused=fused, batches=batches, ratios=r, twin_rel=twin_rel)
+
+
+@pytest.mark.parametrize("name", list(S.CONFIGS))
+def test_step_config(cuda_dev, name, monkeypatch):
+    out = run_row(S.CONFIGS[name], name, cuda_dev, monkeypatch)
     from _parity_util import record
-    record(f"step_configs_{name}_twin", twin_rel)
-    r.check(f"step_configs_fp64_{name}")
+    record(f"step_configs_{name}_twin", out["twin_rel"])
+    out["ratios"].check(f"step_configs_fp64_{name}")
