@@ -77,6 +77,12 @@ STEGO_API int stego_vit_patchify(const float* img, void* out_bf16, int B, int H,
 /* Same, for an image batch already held in bf16 (the precision the fp32 variant rounds to): half the input bytes. */
 STEGO_API int stego_vit_patchify_bf16(const void* img_bf16, void* out_bf16, int B, int H, int W, int patch,
                                       void* stream);
+/* Flip-TTA im2col (eval_segmentation.py:124-125): the rows of 2B images from img [B][3][H][W] (fp32, or bf16 with
+ * img_is_bf16 = 1) -> rows [2B*(H/p)*(W/p)][3*p*p] bf16.  Images 0..B-1 are img, images B..2B-1 are img.flip(3): their
+ * patch column px reads source patch W/p-1-px with its pixel columns reversed.  Bit-identical to stego_vit_patchify of
+ * the two batches; same argument rules (p = 8 or 16, W % 8 == 0, 16-byte aligned img). */
+STEGO_API int stego_vit_patchify_tta(const void* img, int img_is_bf16, void* out_bf16, int B, int H, int W, int patch,
+                                     void* stream);
 /* prepare_tokens (:203-207): x[b][0][:] = cls_token + pos_embed[0] (fp32 residual stream [B][ntok][E]). */
 STEGO_API int stego_vit_cls_rows(float* x, const float* cls_token, const float* pos_embed, int B, int ntok, int E,
                                  void* stream);

@@ -1,5 +1,6 @@
 // Bandwidth-bound pieces of the frozen DINO ViT forward (reference: src/dino/vision_transformer.py):
-//   patchify      : NCHW fp32 image -> im2col rows [B*hw][3*P*P] bf16  (PatchEmbed conv, :127-131, as a GEMM operand)
+//   patchify      : NCHW fp32 image -> im2col rows [B*hw][3*P*P] bf16  (PatchEmbed conv, :127-131, as a GEMM operand),
+//                   optionally followed by the rows of the mirrored images (flip-TTA)
 //   cls rows      : x[b,0,:] = cls_token + pos_embed[0]                 (prepare_tokens, :203-207)
 //   layernorm     : fp32 residual stream -> bf16 GEMM operand            (Block norm1/norm2 :107,111; final norm :234)
 // The residual stream is kept in fp32 (the reference computes in fp32); GEMM operands are bf16.
@@ -12,11 +13,16 @@ namespace stego {
 // ---------------------------------------------------------------------------------------------
 // patchify: one thread per (patch, channel, ky): reads P contiguous pixels, writes P bf16.
 // column order c*P*P + ky*P + kx == flattening of the conv weight [E][3][P][P].
+// MIRROR: the rows of 2B images are written, images B..2B-1 being img.flip(3) (the flip-TTA frames of
+// eval_segmentation.py:125): patch column px reads source patch fw-1-px with its P pixels in reverse order, so the
+// mirrored batch is never materialised.  The values are the same bits as patchify of the flipped image.
 // ---------------------------------------------------------------------------------------------
-template <int P, typename T>
+__device__ __forceinline__ uint32_t swap_bf16x2(uint32_t v) { return __byte_perm(v, 0, 0x1032); }
+
+template <int P, typename T, bool MIRROR>
 __global__ void patchify_kernel(const T* __restrict__ img, bf16* __restrict__ out, int B, int H, int W) {
   const int fh = H / P, fw = W / P;
-  const long long total = 1ll * B * fh * fw * 3 * P;
+  const long long total = 1ll * (MIRROR ? 2 * B : B) * fh * fw * 3 * P;
   const long long idx = 1ll * blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= total) return;
   const int ky = idx % P;
@@ -25,24 +31,28 @@ __global__ void patchify_kernel(const T* __restrict__ img, bf16* __restrict__ ou
   const int px = patch % fw;
   const int py = (patch / fw) % fh;
   const int b = patch / (1ll * fw * fh);
-  const T* src = img + ((1ll * b * 3 + c) * H + (py * P + ky)) * W + px * P;
+  const bool flip = MIRROR && b >= B;
+  const int sb = flip ? b - B : b, sx = flip ? fw - 1 - px : px;
+  const T* src = img + ((1ll * sb * 3 + c) * H + (py * P + ky)) * W + sx * P;
   bf16* dst = out + patch * (3 * P * P) + c * P * P + ky * P;
   static_assert(P == 8 || P == 16, "patch size");
 #pragma unroll
   for (int v = 0; v < P / 8; ++v) {
+    const int sv = flip ? P / 8 - 1 - v : v;  // 8-pixel group of the source; reversed inside below when flipped
+    uint4 w;
     if constexpr (sizeof(T) == 2) {
       // bf16 image (already the precision the GEMM operand has): a straight 16-byte copy
-      *reinterpret_cast<uint4*>(dst + v * 8) = *reinterpret_cast<const uint4*>(src + v * 8);
+      w = *reinterpret_cast<const uint4*>(src + sv * 8);
     } else {
-      const float4 a = *reinterpret_cast<const float4*>(src + v * 8);
-      const float4 b4 = *reinterpret_cast<const float4*>(src + v * 8 + 4);
-      uint4 w;
+      const float4 a = *reinterpret_cast<const float4*>(src + sv * 8);
+      const float4 b4 = *reinterpret_cast<const float4*>(src + sv * 8 + 4);
       w.x = pack_bf16x2(a.x, a.y);
       w.y = pack_bf16x2(a.z, a.w);
       w.z = pack_bf16x2(b4.x, b4.y);
       w.w = pack_bf16x2(b4.z, b4.w);
-      *reinterpret_cast<uint4*>(dst + v * 8) = w;
     }
+    if (flip) w = make_uint4(swap_bf16x2(w.w), swap_bf16x2(w.z), swap_bf16x2(w.y), swap_bf16x2(w.x));
+    *reinterpret_cast<uint4*>(dst + v * 8) = w;
   }
 }
 
@@ -219,38 +229,46 @@ linear_rows_f32_kernel(const float* __restrict__ x, const bf16* __restrict__ w, 
 
 using namespace stego;
 
+template <bool MIRROR>
 static int launch_patchify(const void* img, int img_is_bf16, void* out_bf16, int B, int H, int W, int patch,
                            cudaStream_t stream) {
-  STEGO_CHECK_ARG(img && out_bf16, "stego_vit_patchify: null pointer");
-  STEGO_CHECK_ARG(patch == 8 || patch == 16, "stego_vit_patchify: patch size %d unsupported (8 or 16)", patch);
-  STEGO_CHECK_ARG(B > 0 && H % patch == 0 && W % patch == 0 && W % 8 == 0, "stego_vit_patchify: bad image %dx%dx%d", B, H, W);
-  STEGO_CHECK_ARG((reinterpret_cast<uintptr_t>(img) & 15u) == 0, "stego_vit_patchify: image not 16-byte aligned");
-  const long long total = 1ll * B * (H / patch) * (W / patch) * 3 * patch;
+  const char* name = MIRROR ? "stego_vit_patchify_tta" : "stego_vit_patchify";
+  STEGO_CHECK_ARG(img && out_bf16, "%s: null pointer", name);
+  STEGO_CHECK_ARG(patch == 8 || patch == 16, "%s: patch size %d unsupported (8 or 16)", name, patch);
+  STEGO_CHECK_ARG(B > 0 && H % patch == 0 && W % patch == 0 && W % 8 == 0, "%s: bad image %dx%dx%d", name, B, H, W);
+  STEGO_CHECK_ARG((reinterpret_cast<uintptr_t>(img) & 15u) == 0, "%s: image not 16-byte aligned", name);
+  const long long total = 1ll * (MIRROR ? 2 * B : B) * (H / patch) * (W / patch) * 3 * patch;
   const int threads = 256;
   const int blocks = (int)((total + threads - 1) / threads);
   bf16* out = reinterpret_cast<bf16*>(out_bf16);
   if (img_is_bf16) {
     const bf16* im = reinterpret_cast<const bf16*>(img);
-    if (patch == 8) patchify_kernel<8, bf16><<<blocks, threads, 0, stream>>>(im, out, B, H, W);
-    else patchify_kernel<16, bf16><<<blocks, threads, 0, stream>>>(im, out, B, H, W);
+    if (patch == 8) patchify_kernel<8, bf16, MIRROR><<<blocks, threads, 0, stream>>>(im, out, B, H, W);
+    else patchify_kernel<16, bf16, MIRROR><<<blocks, threads, 0, stream>>>(im, out, B, H, W);
   } else {
     const float* im = reinterpret_cast<const float*>(img);
-    if (patch == 8) patchify_kernel<8, float><<<blocks, threads, 0, stream>>>(im, out, B, H, W);
-    else patchify_kernel<16, float><<<blocks, threads, 0, stream>>>(im, out, B, H, W);
+    if (patch == 8) patchify_kernel<8, float, MIRROR><<<blocks, threads, 0, stream>>>(im, out, B, H, W);
+    else patchify_kernel<16, float, MIRROR><<<blocks, threads, 0, stream>>>(im, out, B, H, W);
   }
   STEGO_CHECK_LAUNCH("patchify_kernel");
   return STEGO_OK;
 }
 
 extern "C" int stego_vit_patchify(const float* img, void* out_bf16, int B, int H, int W, int patch, void* stream_) {
-  return launch_patchify(img, 0, out_bf16, B, H, W, patch, reinterpret_cast<cudaStream_t>(stream_));
+  return launch_patchify<false>(img, 0, out_bf16, B, H, W, patch, reinterpret_cast<cudaStream_t>(stream_));
 }
 
 // Same im2col for an image batch that is already bf16 (the GEMM operand precision): results are bit-identical to
 // feeding the fp32 image whenever the fp32 image holds bf16-representable values, and the H2D copy is half the size.
 extern "C" int stego_vit_patchify_bf16(const void* img_bf16, void* out_bf16, int B, int H, int W, int patch,
                                        void* stream_) {
-  return launch_patchify(img_bf16, 1, out_bf16, B, H, W, patch, reinterpret_cast<cudaStream_t>(stream_));
+  return launch_patchify<false>(img_bf16, 1, out_bf16, B, H, W, patch, reinterpret_cast<cudaStream_t>(stream_));
+}
+
+// The rows of the 2B images [img ; img.flip(3)] from the B images of img (fp32, or bf16 with img_is_bf16 = 1).
+extern "C" int stego_vit_patchify_tta(const void* img, int img_is_bf16, void* out_bf16, int B, int H, int W, int patch,
+                                      void* stream_) {
+  return launch_patchify<true>(img, img_is_bf16, out_bf16, B, H, W, patch, reinterpret_cast<cudaStream_t>(stream_));
 }
 
 extern "C" int stego_vit_cls_rows(float* x, const float* cls_token, const float* pos_embed, int B, int ntok, int E,

@@ -181,24 +181,28 @@ class VisionTransformer(nn.Module):
     # ------------------------------------------------------------------------------------------
     @torch.no_grad()
     def forward_tokens(self, img: torch.Tensor, want_qkv: bool = False, taps: Optional["BlockTaps"] = None,
-                       stop_before_last: bool = False) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
+                       stop_before_last: bool = False, mirror: bool = False
+                       ) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
         """Returns (x, qkv_last): x = fp32 residual stream [B*N, E] after the last block (before the
         final norm); qkv_last = packed bf16 [B*N, 3E] of the last block if requested.  `taps` collects values of
         the last taps.n blocks (see BlockTaps); the block outputs are computed the same way with or without it.
-        stop_before_last: run blocks 0 .. depth-2 only; x is then the residual stream entering the last block."""
+        stop_before_last: run blocks 0 .. depth-2 only; x is then the residual stream entering the last block.
+        mirror: run the 2B images [img ; img.flip(3)] (flip-TTA) from the B images of img, the mirrored ones read by the
+        patchify kernel (stego_vit_patchify_tta); x then holds 2B*N rows."""
         if not img.is_cuda:
             raise RuntimeError("stego_b200: the DINO ViT forward only exists as sm_90a kernels (no CPU fallback)")
         w = self._prepared()
         # bf16 images are taken as they are (patchify rounds fp32 images to bf16 anyway: same operand bits)
         img = (img if img.dtype == torch.bfloat16 else img.float()).contiguous()
         B, _, H, W = img.shape
+        B = 2 * B if mirror else B
         p = self.patch_embed.patch_size
         E, heads = self.embed_dim, self.num_heads
         hw = (H // p) * (W // p)
         N = hw + 1
         dev = img.device
         pos = self._pos_for(H, W)
-        rows = ops.patchify(img, p)
+        rows = ops.patchify_tta(img, p) if mirror else ops.patchify(img, p)
         x = torch.empty(B * N, E, dtype=torch.float32, device=dev)
         ops.gemm(rows, w["pe_w"], x, M=B * hw, N=E, K=3 * p * p, bias=w["pe_b"], residual=pos, row_div=hw)
         ops.cls_rows(x, w["cls"], pos, B, N)
@@ -230,26 +234,31 @@ class VisionTransformer(nn.Module):
         return x, (qkv if want_qkv else None)
 
     @torch.no_grad()
-    def patch_features(self, img: torch.Tensor, use_graph: bool = False) -> torch.Tensor:
+    def patch_features(self, img: torch.Tensor, use_graph: bool = False, mirror: bool = False) -> torch.Tensor:
         """norm(last block) with the cls token dropped, tokens-major bf16 [B, hw, E] — the tensor STEGO's
         DinoFeaturizer builds at src/modules.py:97, in the K-major layout the correlation GEMM wants.
 
         use_graph=True replays the whole kernel sequence (~110 launches) as ONE CUDA graph captured per input
         shape (the backbone is frozen and RNG-free).  The result then lives in a static buffer that the next
-        replay overwrites: only for callers that consume it before calling again (the fused training step)."""
-        return self._tokens(img, use_graph, "feat")
+        replay overwrites: only for callers that consume it before calling again (the fused training step).
+
+        mirror=True returns [2B, hw, E]: the features of img, then those of img.flip(3), from one pass over 2B images
+        whose mirrored half the patchify kernel reads from img (flip-TTA, eval_segmentation.py:124-125).  Its graph is
+        cached under a key of its own and holds B frames as its static input."""
+        return self._tokens(img, use_graph, "feat", mirror)
 
     @torch.no_grad()
-    def key_features(self, img: torch.Tensor, use_graph: bool = False) -> torch.Tensor:
+    def key_features(self, img: torch.Tensor, use_graph: bool = False, mirror: bool = False) -> torch.Tensor:
         """The last block's keys with the cls token dropped, tokens-major bf16 [B, hw, E], channels head-major
         (head * 64 + d) — dino_feat_type "KK" of src/modules.py:98-101.  Blocks 0 .. depth-2 run as in patch_features;
         the last block stops after LN1 and the key third of its qkv GEMM (no attention, proj, MLP or final norm).
         The bits are those of the K third of the full block's packed qkv: the same LN1 rows, and the GEMM reads the
         key rows of the packed weight (and bias) in place, with the same K loop per output element.
-        use_graph as in patch_features (a graph of its own per input shape)."""
-        return self._tokens(img, use_graph, "KK")
+        use_graph and mirror as in patch_features (a graph of its own per input shape and mirror flag)."""
+        return self._tokens(img, use_graph, "KK", mirror)
 
-    def _tokens(self, img, use_graph: bool, kind: str) -> torch.Tensor:
+    def _tokens(self, img, use_graph: bool, kind: str, mirror: bool = False) -> torch.Tensor:
+        kind = kind + "+mirror" if mirror else kind  # "feat", "KK", "feat+mirror", "KK+mirror": one graph cache key each
         if use_graph and (img[0] if isinstance(img, (list, tuple)) else img).is_cuda:
             return self._graphed(img, kind)
         if isinstance(img, (list, tuple)):
@@ -257,7 +266,10 @@ class VisionTransformer(nn.Module):
         return self._eager(img, kind)
 
     def _eager(self, img: torch.Tensor, kind: str) -> torch.Tensor:
-        return self._patch_features_eager(img) if kind == "feat" else self._key_features_eager(img)
+        mirror = kind.endswith("+mirror")
+        if kind.startswith("feat"):
+            return self._patch_features_eager(img, mirror)
+        return self._key_features_eager(img, mirror)
 
     def _graphed(self, img, kind: str) -> torch.Tensor:
         """`img` may be a list of image batches: they are copied into consecutive slices of the graph's static
@@ -289,18 +301,18 @@ class VisionTransformer(nn.Module):
         build part of its batch straight into a slice of it and pass that slice back in its list of batches."""
         return self._cache.get("graphs", {}).get((kind, tuple(shape), device.index, dtype), (None, None))[1]
 
-    def _patch_features_eager(self, img: torch.Tensor) -> torch.Tensor:
-        B = img.shape[0]
-        x, _ = self.forward_tokens(img)
+    def _patch_features_eager(self, img: torch.Tensor, mirror: bool = False) -> torch.Tensor:
+        B = img.shape[0] * (2 if mirror else 1)
+        x, _ = self.forward_tokens(img, mirror=mirror)
         w = self._prepared()
         N = x.shape[0] // B
         out = torch.empty(B * (N - 1), self.embed_dim, dtype=torch.bfloat16, device=x.device)
         ops.layernorm(x, w["nw"], w["nb"], out, eps=self.norm.eps, drop_cls_ntok=N)
         return out.view(B, N - 1, self.embed_dim)
 
-    def _key_features_eager(self, img: torch.Tensor) -> torch.Tensor:
-        B, E = img.shape[0], self.embed_dim
-        x, _ = self.forward_tokens(img, stop_before_last=True)
+    def _key_features_eager(self, img: torch.Tensor, mirror: bool = False) -> torch.Tensor:
+        B, E = img.shape[0] * (2 if mirror else 1), self.embed_dim
+        x, _ = self.forward_tokens(img, stop_before_last=True, mirror=mirror)
         bw = self._prepared()["blocks"][-1]
         N = x.shape[0] // B
         y = torch.empty(B * (N - 1), E, dtype=torch.bfloat16, device=x.device)

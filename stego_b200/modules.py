@@ -279,19 +279,20 @@ class DinoFeaturizer(nn.Module):
                                    torch.nn.Conv2d(in_channels, self.dim, (1, 1)))
 
     # ---- fused internals -------------------------------------------------------------------------
-    def backbone_tokens(self, img: torch.Tensor, use_graph: bool = False) -> torch.Tensor:
+    def backbone_tokens(self, img: torch.Tensor, use_graph: bool = False, mirror: bool = False) -> torch.Tensor:
         """Frozen ViT -> bf16 tokens-major teacher features [B, hw, E] (cls dropped): the final-norm tokens for
         dino_feat_type "feat", the last block's keys (head-major channels) for "KK" — the tensor forward() returns
         as image_feat, which both training paths feed to the head and the correspondence loss.  use_graph: replay the
-        kernel sequence as one CUDA graph (result is a static buffer valid until the next call)."""
+        kernel sequence as one CUDA graph (result is a static buffer valid until the next call).  mirror: [2B, hw, E],
+        the tokens of img and then of img.flip(3) from one pass (VisionTransformer.patch_features)."""
         self.model.eval()
         first = img[0] if isinstance(img, (list, tuple)) else img  # a list of batches is concatenated on the fly
         assert first.shape[2] % self.patch_size == 0
         assert first.shape[3] % self.patch_size == 0
         if self.feat_type == "feat":
-            return self.model.patch_features(img, use_graph=use_graph)
+            return self.model.patch_features(img, use_graph=use_graph, mirror=mirror)
         if self.feat_type == "KK":
-            return self.model.key_features(img, use_graph=use_graph)
+            return self.model.key_features(img, use_graph=use_graph, mirror=mirror)
         raise ValueError("Unknown feat type:{}".format(self.feat_type))
 
     def draw_masks(self, batch: int, device):

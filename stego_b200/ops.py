@@ -78,6 +78,18 @@ def patchify(img: torch.Tensor, patch: int) -> torch.Tensor:
     return out
 
 
+def patchify_tta(img: torch.Tensor, patch: int) -> torch.Tensor:
+    """Flip-TTA im2col rows [2B*hw, 3*p*p] bf16 of img [B, 3, H, W] (fp32 or bf16): the rows of img, then those of
+    img.flip(3), which is never materialised (stego_vit_patchify_tta)."""
+    _lib.require_cuda(img)
+    assert img.dtype in (torch.float32, torch.bfloat16) and img.is_contiguous() and img.shape[1] == 3
+    B, _, H, W = img.shape
+    out = torch.empty(2 * B * (H // patch) * (W // patch), 3 * patch * patch, dtype=torch.bfloat16, device=img.device)
+    _lib.check(_lib.load().stego_vit_patchify_tta(_lib.ptr(img), int(img.dtype == torch.bfloat16), _lib.ptr(out), B, H, W,
+                                                  patch, _lib.stream()), "stego_vit_patchify_tta")
+    return out
+
+
 def cls_rows(x: torch.Tensor, cls_token: torch.Tensor, pos_embed: torch.Tensor, B: int, ntok: int) -> None:
     E = x.shape[-1]
     _lib.check(_lib.load().stego_vit_cls_rows(_lib.ptr(x), _lib.ptr(cls_token), _lib.ptr(pos_embed), B, ntok, E,

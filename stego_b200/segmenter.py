@@ -19,6 +19,7 @@ shard; only gradients cross ranks (averaged).
 """
 from __future__ import annotations
 
+import contextlib
 from typing import Dict, List, Optional, Sequence
 
 import torch
@@ -566,6 +567,19 @@ class LitUnsupervisedSegmenter(nn.Module):
         return loss
 
     # ---- validation -------------------------------------------------------------------------------
+    @contextlib.contextmanager
+    def _net_in_eval_mode(self):
+        """The net in eval mode inside the block, every module's train / eval mode restored on exit (also on an error):
+        there is no Trainer to call `.train()` afterwards, and the hand-scheduled step only runs on a net in training
+        mode."""
+        modes = [(m, m.training) for m in self.net.modules()]
+        self.net.eval()
+        try:
+            yield
+        finally:
+            for m, mode in modes:
+                m.training = mode
+
     def validation_step(self, batch, batch_idx):
         """train_segmentation.py:254-275: the eval-mode net, then upsampling to the label size, both probes, both
         argmaxes and both `UnsupervisedMetrics.update` calls as ONE fused_probe_log_probs pass (the upsampled code is
@@ -580,18 +594,12 @@ class LitUnsupervisedSegmenter(nn.Module):
         self.flush()
         img, label = batch["img"], batch["label"]
         n_images = getattr(self.cfg, "n_images", 5)
-        modes = [(m, m.training) for m in self.net.modules()]
-        self.net.eval()
-        try:
-            with torch.no_grad():
-                _, code = self.net(img)
-                out = fused_probe_log_probs(code, self.linear_probe, self.cluster_probe, label.shape[-2:], 2.0,
-                                            want_log_probs=False, want_argmax=n_images > 0, label=label,
-                                            linear_confusion=self.linear_metrics.stats,
-                                            cluster_confusion=self.cluster_metrics.stats)
-        finally:
-            for m, mode in modes:
-                m.training = mode
+        with self._net_in_eval_mode(), torch.no_grad():
+            _, code = self.net(img)
+            out = fused_probe_log_probs(code, self.linear_probe, self.cluster_probe, label.shape[-2:], 2.0,
+                                        want_log_probs=False, want_argmax=n_images > 0, label=label,
+                                        linear_confusion=self.linear_metrics.stats,
+                                        cluster_confusion=self.cluster_metrics.stats)
         none = torch.empty(0, *label.shape[-2:], dtype=torch.long)
         return {"img": img[:n_images].detach().cpu(),
                 "linear_preds": out[2][:n_images].long().cpu() if n_images > 0 else none,
@@ -608,19 +616,105 @@ class LitUnsupervisedSegmenter(nn.Module):
         and workspace alone and restores the net's train / eval modes on exit.  Nothing is copied to the host."""
         self.flush()
         img, label = batch["img"], batch["label"]
-        modes = [(m, m.training) for m in self.net.modules()]
-        self.net.eval()
-        try:
-            with torch.no_grad():
-                feats, code = self.net(img)
-                fs = int(self.cfg.feature_samples)
-                coord_shape = [img.shape[0], fs, fs, 2]
-                coords1 = torch.rand(coord_shape, device=img.device) * 2 - 1
-                coords2 = torch.rand(coord_shape, device=img.device) * 2 - 1
-                metric.update(feats, code, label, coords1, coords2)
-        finally:
-            for m, mode in modes:
-                m.training = mode
+        with self._net_in_eval_mode(), torch.no_grad():
+            feats, code = self.net(img)
+            fs = int(self.cfg.feature_samples)
+            coord_shape = [img.shape[0], fs, fs, 2]
+            coords1 = torch.rand(coord_shape, device=img.device) * 2 - 1
+            coords2 = torch.rand(coord_shape, device=img.device) * 2 - 1
+            metric.update(feats, code, label, coords1, coords2)
+
+    def eval_step(self, batch, run_crf: bool = False, want_probs: bool = False) -> Dict[str, torch.Tensor]:
+        """The evaluation loop body of eval_segmentation.py:122-141 (also demo_segmentation.py:57-78, plot_potsdam.py:44-57)
+        for one batch of frames:
+
+            code = (net(img)[1] + net(img.flip(3))[1].flip(3)) / 2
+            code = F.interpolate(code, size, mode='bilinear', align_corners=False)
+            linear_probs  = torch.log_softmax(linear_probe(code), dim=1)
+            cluster_probs = cluster_probe(code, 2, log_probs=True)
+            preds = batched_crf(img, probs).argmax(1) if run_crf else probs.argmax(1)     # for both probes
+            test_linear_metrics.update(linear_preds, label); test_cluster_metrics.update(cluster_preds, label)
+
+        batch["img"]: the normalised frames [B, 3, H, W], fp32 or bf16, CUDA.  batch["label"] (optional): [B, H', W'],
+        uint8 with 255 = ignore, int32 or int64; with it both `final/` confusion matrices (test_linear_metrics.stats,
+        test_cluster_metrics.stats) are accumulated in the same pass, and `compute()` stays the caller's call.  The output
+        size is the label's (eval_segmentation, plot_potsdam), or the frames' without a label (demo_segmentation); with
+        run_crf the label must have the frames' size (the dense CRF runs at image resolution, fused_eval_crf).
+
+        The frame and its mirror go through the frozen ViT as one batch of 2B, the mirrored frames read in place by the
+        patchify kernel and the whole backbone replayed as one CUDA graph per frame shape (cached beside the training
+        step's graphs, never replacing them).  The eval-mode head (no dropout noise) runs once over the 2B rows, then
+        fused_probe_log_probs (or fused_eval_crf with run_crf) takes the two halves of the code as code / code_flipped.
+
+        Returns dict(linear_preds, cluster_preds), uint8 [B, H', W'] on the device; with want_probs also
+        linear_probs / cluster_probs fp32 [B, n, H', W']: the log-probabilities without CRF, the CRF marginals with it.
+        Like validation_step it waits for the previous step's parameter update, draws no random numbers, leaves the
+        training step's workspace, graphs and parameters alone and restores the net's train / eval modes on exit.
+        Configurations the fused eval kernels do not take (proj_type None: a code of E > 96 channels; more than 32
+        cluster-probe rows) and CPU tensors are refused before anything is enqueued."""
+        from .eval import fused_eval_crf, fused_probe_log_probs
+        img, label = batch["img"], batch.get("label")
+        self._check_eval_args(img, label, run_crf)
+        self.flush()
+        net = self.net
+        B, fh, fw = img.shape[0], img.shape[2] // net.patch_size, img.shape[3] // net.patch_size
+        stats = dict(linear_confusion=self.test_linear_metrics.stats, cluster_confusion=self.test_cluster_metrics.stats) \
+            if label is not None else {}
+        with self._net_in_eval_mode(), torch.no_grad():
+            tok = net.backbone_tokens(img, use_graph=getattr(self.cfg, "cuda_graph", True), mirror=True)  # [2B, hw, E]
+            code_all = net.head_code(tok, None, None, fh, fw)  # [2B, dim, h, w]
+            code, code_flipped = code_all[:B], code_all[B:]
+            if run_crf:
+                out = fused_eval_crf(code, self.linear_probe, self.cluster_probe, img, 2.0, code_flipped=code_flipped,
+                                     label=label, want_marginals=want_probs, **stats)
+                preds, probs = out[:2], out[2:]
+            else:
+                size = label.shape[-2:] if label is not None else img.shape[-2:]
+                out = fused_probe_log_probs(code, self.linear_probe, self.cluster_probe, size, 2.0,
+                                            want_log_probs=want_probs, want_argmax=True, code_flipped=code_flipped,
+                                            label=label, **stats)
+                preds, probs = out[2:], out[:2]
+        result = dict(linear_preds=preds[0], cluster_preds=preds[1])
+        if want_probs:
+            result.update(linear_probs=probs[0], cluster_probs=probs[1])
+        return result
+
+    def _check_eval_args(self, img, label, run_crf: bool) -> None:
+        """eval_step's arguments against the rules of the kernels it calls, shapes and limits first (ValueError), the
+        device last (RuntimeError), so that nothing is enqueued for a call that would fail part-way."""
+        from .eval import _check_crf_args
+        net = self.net
+        p = net.patch_size
+        if img.dim() != 4 or img.shape[1] != 3 or img.shape[0] < 1 or img.dtype not in (torch.float32, torch.bfloat16):
+            raise ValueError(f"eval_step: img must be fp32 or bf16 [B, 3, H, W], got {img.dtype} {tuple(img.shape)}")
+        B, _, H, W = img.shape
+        # the patchify rules (stego_vit_patchify_tta): patch 8 or 16, whole patches, rows of a multiple of 8 pixels
+        if p not in (8, 16) or H % p or W % p or W % 8:
+            raise ValueError(f"eval_step: a {H}x{W} frame is not whole {p}x{p} patches with W a multiple of 8 "
+                             f"(patch 8 or 16)")
+        if net.proj_type is None:
+            raise ValueError(f"eval_step: projection_type None gives a code of {net.n_feats} channels; the fused "
+                             f"evaluation probes take at most 96")
+        n_lin, n_clu = self.linear_probe.weight.shape[0], self.cluster_probe.clusters.shape[0]
+        if n_lin > 32 or n_clu > 32:
+            raise ValueError(f"eval_step: {n_lin} linear-probe classes / {n_clu} cluster-probe rows unsupported by the "
+                             f"fused evaluation probes (at most 32 each)")
+        if label is not None:
+            if label.dtype not in ops.LABEL_BYTES:
+                raise ValueError(f"eval_step: label dtype {label.dtype} unsupported (uint8, int32 or int64)")
+            Hl, Wl = label.shape[-2:]
+            if label.dim() < 2 or label.numel() != B * Hl * Wl:
+                raise ValueError(f"eval_step: label {tuple(label.shape)} is not one [H, W] map per frame of {B}")
+            if Hl < H // p or Wl < W // p:
+                raise ValueError(f"eval_step: label {Hl}x{Wl} is smaller than the code {H // p}x{W // p} "
+                                 f"(upsampling only)")
+        if run_crf:
+            # fused_eval_crf's own checks (label at the frames' size, ...), on a stand-in of the code's shape
+            stub = torch.empty(1, device=img.device).expand(B, net.dim, H // p, W // p)
+            stats = (self.test_linear_metrics.stats, self.test_cluster_metrics.stats) if label is not None else (None, None)
+            _check_crf_args(stub, self.linear_probe, self.cluster_probe, img, stub, label, *stats)
+        _lib.require_cuda(img, label, self.linear_probe.weight, self.cluster_probe.clusters,
+                          self.test_linear_metrics.stats, self.test_cluster_metrics.stats, net.cluster1[0].weight)
 
     def validation_epoch_end(self, outputs=None) -> Dict[str, float]:
         """train_segmentation.py:277-283, 361-371 without the figures: sum both confusion matrices over the ranks (what
