@@ -499,6 +499,50 @@ STEGO_API int stego_aug_align_bwd(const float* grid, const float* dsampled, int 
  * total is not null. */
 STEGO_API int stego_aug_align_loss(const float* cosv, long long n, float weight, float* loss, float* total, void* stream);
 
+/* ---- reconstruction term of the training step (src/train_segmentation.py:183-187): cos = <normalize(decoder(code)),
+ * normalize(feat * m3)> per pixel, the decoder a 1x1 conv D -> E in fp32, never written out.  code: fp32 rows [M][ldc]
+ * (first D <= 96 columns); feat: bf16 rows [M][ldf] (first E columns); m3: fp32 [M / hw][E] per-image channel scale, or
+ * null; weight [E][D], bias [E] fp32.  cosv / nr / nf: [M] floats, the cosine and the unclamped norms |r|, |f|. */
+STEGO_API int stego_rec_fwd(const float* code, long long ldc, const void* feat, long long ldf, const float* m3, int hw,
+                            const float* weight, const float* bias, long long M, int E, int D, float* cosv, float* nr,
+                            float* nf, void* stream);
+/* Bytes of the scratch stego_rec_bwd needs on the current device (per-CTA dW / db partials; 0 for bad sizes). */
+STEGO_API long long stego_rec_scratch_bytes(long long M, int E, int D);
+/* Backward with the forward's inputs and outputs; dcos [1] is d loss / d cos of every pixel.  dcode [M][ldd] (first D
+ * columns) is ACCUMULATED into (each row by one CTA, no atomics); dweight [E][D] and dbias [E] are WRITTEN, the rows
+ * summed in a fixed order (bit-reproducible). */
+STEGO_API int stego_rec_bwd(const float* code, long long ldc, const void* feat, long long ldf, const float* m3, int hw,
+                            const float* weight, const float* bias, long long M, int E, int D, const float* cosv,
+                            const float* nr, const float* nf, const float* dcos, float* dcode, long long ldd,
+                            float* scratch, long long scratch_bytes, float* dweight, float* dbias, void* stream);
+
+/* ---- contrastive CRF term of the training step (src/train_segmentation.py:201-208):
+ * crf_loss_fn(resize(img, S), normalize(resize(code, S))).mean() with resize = F.interpolate(bilinear,
+ * align_corners=False), evaluated at the n sampled points of the S x S maps only (coords [2][n] int64: rows, then
+ * columns).  The taps follow ATen's arithmetic, so the resized values are bit-equal to torch's at those points.
+ * Workspace, NP = round_up(n, 64): gsel [B][NP][4] and sel / dsel [B][C][NP] floats, pos [NP][2] ints, nrm [B][NP]
+ * floats, tile_sum [B][NP/64][NP/64] doubles.
+ * Guidance: img fp32 [B][Cg <= 3][H][W] (element strides) -> gsel, pos. */
+STEGO_API int stego_crf_guidance(const float* img, long long sb, long long sc, long long sy, long long sx, int Cg, int H,
+                                 int W, const long long* coords, int B, int n, int S, float* gsel, int* pos, void* stream);
+/* code fp32 [B][C <= 80][h][w] (element strides) -> raw (the resized code at the samples, [B][C][NP]), sel (raw
+ * normalised over the channels), nrm (the unclamped norms), and the fixed-order
+ * fp64 sum of every 64 x 64 tile of -(Gram x pairwise kernel) in tile_sum (no [B][n][n] output). */
+STEGO_API int stego_crf_mean_fwd(const float* code, long long sb, long long sc, long long sy, long long sx, int C, int h,
+                                 int w, const long long* coords, int B, int n, int S, float alpha, float beta, float gamma,
+                                 float w1, float w2, float shift, const float* gsel, const int* pos, float* raw,
+                                 float* sel, float* nrm, double* tile_sum, void* stream);
+/* loss[0] = the mean of the B n^2 outputs, from tile_sum in a fixed order; total[0] += weight * loss[0] when total is
+ * not null. */
+STEGO_API int stego_crf_mean_loss(const double* tile_sum, int B, int n, float weight, float* loss, float* total,
+                                  void* stream);
+/* d code (strides as given) += the mean's gradient for the upstream gradient gscalar[0] of every output, through the
+ * Gram x kernel product, F.normalize and the bilinear taps, by fp32 atomics; dsel is scratch. */
+STEGO_API int stego_crf_mean_bwd(const float* gscalar, const float* sel, const float* nrm, const float* gsel,
+                                 const int* pos, const long long* coords, int B, int C, int n, int h, int w, int S,
+                                 float alpha, float beta, float gamma, float w1, float w2, float shift, float* dsel,
+                                 float* dcode, long long sb, long long sc, long long sy, long long sx, void* stream);
+
 /* ---- data-parallel exchange over NVLink peer memory: gradient all-reduce fused into the Adam update (replaces the DDP
  * all-reduce behind manual_backward + the three optimizer.step() calls, src/train_segmentation.py:227-230, 476).
  * Every rank allocates one peer-visible block [export 2 x n_pad floats | flags world x uint32], exchanges the 64-byte CUDA

@@ -24,6 +24,8 @@ TRAIN_DEFAULTS = dict(
     fused_step=True,   # hand-scheduled training step (fused_step.py) instead of the autograd-stitched one
     overlap_update=True,  # parameter update on the side stream under the next step's backbone
     p2p_update=True,   # N > 1: gradient all-reduce fused into Adam over NVLink peer memory (NCCL all-reduce as the fallback)
+    fused_rec_crf=False,  # rec_weight / crf_weight > 0 on the hand-scheduled step (fp32 img and dim <= 80 for the CRF
+                          # term) instead of the autograd-stitched one
 )
 
 

@@ -4,12 +4,12 @@
 //     sampled = F.grid_sample(code, coord.permute(0, 2, 1, 3), padding_mode="border", align_corners=True)
 //     aug_alignment = -cosine(sampled, code_aug).mean()
 // The resize of the two coordinate channels is evaluated only at the h x h points grid_sample reads, with ATen's
-// upsample_bilinear2d arithmetic (src_index of probe_common.cuh); the taps are grid_sample's (grid_taps of taps.cuh),
+// upsample_bilinear2d arithmetic (resize.cuh); the taps are grid_sample's (grid_taps of taps.cuh),
 // accumulated in ATen's order, so both match torch's CUDA results bit for bit.  Output pixel (p, q) reads grid point
 // (q, p): the permute(0, 2, 1, 3).
 // The cosine and its gradients are stego_cosine_fwd / _bwd; the backward here scatters d(sampled) into d(code) with
 // the same taps, and stego_aug_align_loss is the fixed-order mean (the logged term repeats bit for bit).
-#include "probe_common.cuh"
+#include "resize.cuh"
 #include "taps.cuh"
 #include "host_util.h"
 
@@ -25,13 +25,6 @@ struct AugAlignParams {
   float* sampled;          // [B][C][h][h] contiguous (fwd: written; bwd: d(sampled), read)
 };
 
-// grid[b][i][j][c] = channel c of the resized coordinates at (i, j): ATen upsample_bilinear2d_out_frame's expression
-__device__ __forceinline__ float resize_at(const float* cb, int S, int y0, int y1, float ly, int x0, int x1, float lx, int c) {
-  const float h1l = ly, h0l = 1.f - ly, w1l = lx, w0l = 1.f - lx;
-  auto at = [&](int y, int x) { return cb[(static_cast<long long>(y) * S + x) * 2 + c]; };
-  return h0l * (w0l * at(y0, x0) + w1l * at(y0, x1)) + h1l * (w0l * at(y1, x0) + w1l * at(y1, x1));
-}
-
 // One thread per output pixel (b, p, q); consecutive threads take consecutive q, so the NCHW stores coalesce.
 __global__ void __launch_bounds__(256) aug_align_fwd_kernel(AugAlignParams p) {
   const long long npix = 1ll * p.B * p.h * p.h;
@@ -40,16 +33,14 @@ __global__ void __launch_bounds__(256) aug_align_fwd_kernel(AugAlignParams p) {
   const int q = static_cast<int>(pix % p.h), pp = static_cast<int>((pix / p.h) % p.h), b = static_cast<int>(pix / (1ll * p.h * p.h));
   // this thread writes grid point (i, j) = (pp, q) and samples with grid point (q, pp)
   const float* cb = p.coord_aug + static_cast<long long>(b) * p.S * p.S * 2;
-  int y0, y1, x0, x1;
-  float ly, lx;
-  src_index(pp, p.scale, p.S, y0, y1, ly);
-  src_index(q, p.scale, p.S, x0, x1, lx);
+  // grid[b][i][j][c] = channel c of the resized coordinates at (i, j)
+  auto chan = [&](int c) { return [=](int y, int x) { return cb[(static_cast<long long>(y) * p.S + x) * 2 + c]; }; };
+  ResizeTaps rt = resize_taps(pp, q, p.scale, p.scale, p.S, p.S);
   float* gw = p.grid + ((static_cast<long long>(b) * p.h + pp) * p.h + q) * 2;
-  gw[0] = resize_at(cb, p.S, y0, y1, ly, x0, x1, lx, 0);
-  gw[1] = resize_at(cb, p.S, y0, y1, ly, x0, x1, lx, 1);
-  src_index(q, p.scale, p.S, y0, y1, ly);
-  src_index(pp, p.scale, p.S, x0, x1, lx);
-  const float gx = resize_at(cb, p.S, y0, y1, ly, x0, x1, lx, 0), gy = resize_at(cb, p.S, y0, y1, ly, x0, x1, lx, 1);
+  gw[0] = resize_at(rt, chan(0));
+  gw[1] = resize_at(rt, chan(1));
+  rt = resize_taps(q, pp, p.scale, p.scale, p.S, p.S);
+  const float gx = resize_at(rt, chan(0)), gy = resize_at(rt, chan(1));
   const Taps t = grid_taps(gx, gy, p.h, p.h);
   auto off = [&](int i) { return static_cast<long long>(i / p.h) * p.sy + static_cast<long long>(i % p.h) * p.sx; };
   const float* base = p.code + static_cast<long long>(b) * p.sb;

@@ -7,6 +7,7 @@
 // and once in the backward.  Inputs are fp32 with arbitrary element strides: channels-last views (what DinoFeaturizer
 // returns, channel stride 1) take the warp-per-pixel path, anything else the thread-per-pixel path.
 #include "common.cuh"
+#include "cosine.cuh"
 #include "host_util.h"
 
 namespace stego {
@@ -49,11 +50,7 @@ __global__ void __launch_bounds__(256) cosine_fwd_kernel(CosParams p) {
   }
 }
 
-// d cos / d a = ib * (ia * b - [|a| >= eps] * cos * ia^2 * a) ... written with the saved norms, ia = 1 / max(|a|, eps)
-// recomputed from them (the forward's bits):
-//   a_hat = a * ia, b_hat = b * ib, cos = <a_hat, b_hat>
-//   |a| >= eps:  d cos / d a = ia * (b_hat - cos * a_hat)        |a| < eps (ia = 1/eps constant):  d cos / d a = ia * b_hat
-// F.normalize's clamp_min passes the gradient at |a| == eps too, which the inverse alone cannot tell from |a| < eps.
+// the gradient formulas are CosineGrad's (cosine.cuh)
 template <bool WARP>
 __global__ void __launch_bounds__(256) cosine_bwd_kernel(CosParams p) {
   const long long npix = 1ll * p.B * p.H * p.W;
@@ -63,12 +60,11 @@ __global__ void __launch_bounds__(256) cosine_bwd_kernel(CosParams p) {
   const int x = static_cast<int>(pix % p.W), y = static_cast<int>((pix / p.W) % p.H), b = static_cast<int>(pix / (1ll * p.W * p.H));
   const long long oa = b * p.a_sb + y * p.a_sy + x * p.a_sx, ob = b * p.b_sb + y * p.b_sy + x * p.b_sx;
   const float g = p.g[pix], cs = p.cosv[pix], na = p.norma[pix], nb = p.normb[pix];
-  const float ia = 1.0f / fmaxf(na, p.eps), ib = 1.0f / fmaxf(nb, p.eps);
-  const float ka = (na >= p.eps) ? cs : 0.f, kb = (nb >= p.eps) ? cs : 0.f;  // clamped norm: no tangential term
+  const CosineGrad cg(cs, na, nb, p.eps);
   for (int c = WARP ? lane : 0; c < p.C; c += WARP ? 32 : 1) {
-    const float ah = p.a[oa + c * p.a_sc] * ia, bh = p.b[ob + c * p.b_sc] * ib;
-    if (p.da) p.da[oa + c * p.a_sc] = g * ia * (bh - ka * ah);
-    if (p.db) p.db[ob + c * p.b_sc] = g * ib * (ah - kb * bh);
+    const float va = p.a[oa + c * p.a_sc], vb = p.b[ob + c * p.b_sc];
+    if (p.da) p.da[oa + c * p.a_sc] = cg.da(g, va, vb);
+    if (p.db) p.db[ob + c * p.b_sc] = cg.db(g, va, vb);
   }
 }
 

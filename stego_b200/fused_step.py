@@ -23,6 +23,12 @@ With cfg.aug_alignment_weight > 0 and batch["seed"] (train_segmentation.py:189-1
 itself (augment: host draws on a forked CPU generator, one pinned upload, two launches, all before the backbone is
 enqueued), runs img, img_pos and img_aug through the backbone as ONE batch of 3B and the head over 3B rows; the term is
 modules.aug_sample_forward / cosine_forward / aug_loss and their backward, inside the tail graph.
+
+With cfg.fused_rec_crf the reconstruction term (cfg.rec_weight, train_segmentation.py:183-187) and the CRF term
+(cfg.crf_weight, :201-208) run here too: modules.rec_forward / rec_backward (the decoder output never leaves the
+kernel) and modules.crf_forward / crf_loss / crf_backward (only the n sampled points of the 56 x 56 maps), inside the
+tail graph.  The CRF coordinates are drawn by the prologue after everything else, as the term's two randint calls come
+last in the reference; its image guidance is sampled by one eager launch per step, so the graph bakes no caller pointer.
 """
 from __future__ import annotations
 
@@ -58,7 +64,7 @@ class FusedStep:
         img = batch["img"]
         return (img.is_cuda and seg.training and seg.net.training and cfg.correspondence_weight > 0
                 and seg.net.proj_type is not None
-                and cfg.rec_weight == 0 and cfg.crf_weight == 0
+                and self._rec_crf_supported(batch)
                 and (cfg.aug_alignment_weight == 0 or self._aug_supported(batch))
                 and cfg.neg_samples >= 1 and cfg.dino_feat_type in ("feat", "KK")
                 and seg.linear_probe.weight.shape[0] <= 32 and seg.net.dim <= 96
@@ -76,8 +82,17 @@ class FusedStep:
                 and not (isinstance(seeds, torch.Tensor) and seeds.is_cuda)
                 and img.dtype == torch.float32 and img.dim() == 4 and tuple(img.shape[1:]) == (3, res, res))
 
+    def _rec_crf_supported(self, batch) -> bool:
+        """The reconstruction / CRF terms run here only with cfg.fused_rec_crf; the CRF term needs the fp32 image (its
+        guidance) and a code of at most 80 channels (stego_crf_loss_*)."""
+        cfg = self.seg.cfg
+        if cfg.rec_weight == 0 and cfg.crf_weight == 0:
+            return True
+        return bool(getattr(cfg, "fused_rec_crf", False)) and (
+            cfg.crf_weight == 0 or (batch["img"].dtype == torch.float32 and self.seg.net.dim <= 80))
+
     # ------------------------------------------------------------------------------------------
-    def _alloc(self, B, H, W, LH, LW, dev, label_dtype, label_pos_dtype, mask_shape, aug):
+    def _alloc(self, B, H, W, LH, LW, dev, label_dtype, label_pos_dtype, mask_shape, aug, rec, crf):
         seg, cfg, net = self.seg, self.seg.cfg, self.seg.net
         ws = _Workspace()
         E, D = net.n_feats, net.dim
@@ -156,6 +171,26 @@ class FusedStep:
             # d(loss)/d(cos) of loss += w * -(cos.mean()): autograd's fl(fl(-w) / N), one value per pixel
             ws.dcos = torch.full((B, fh, fw), -float(cfg.aug_alignment_weight), dtype=f32, device=dev).div_(B * hw)
             ws.aug_loss = torch.empty(1, dtype=f32, device=dev)
+        ws.rec, ws.crf = rec, crf
+        if rec:  # the reconstruction term: per-pixel cosine and norms, its gradient, the decoder-gradient partials
+            ws.rec_cos, ws.rec_nr, ws.rec_nf = (torch.empty(B * hw, dtype=f32, device=dev) for _ in range(3))
+            ws.rec_dcos = torch.full((1,), -float(cfg.rec_weight), dtype=f32, device=dev).div_(B * hw)  # as ws.dcos
+            ws.rec_loss = torch.empty(1, dtype=f32, device=dev)
+            ws.rec_scratch = modules.rec_scratch(B * hw, E, D, dev)
+        if crf:  # the CRF term: the coordinates, the sampled guidance and code, the tile sums
+            n = seg.crf_loss_fn.n_samples
+            NP = _round_up(n, 64)
+            ws.crf_coords = torch.empty(2, n, dtype=torch.long, device=dev)
+            ws.crf_gsel = torch.empty(B, NP, 4, dtype=f32, device=dev)
+            ws.crf_pos = torch.empty(NP, 2, dtype=torch.int32, device=dev)
+            ws.crf_raw = torch.empty(B, D, NP, dtype=f32, device=dev)
+            ws.crf_sel = torch.empty(B, D, NP, dtype=f32, device=dev)
+            ws.crf_dsel = torch.empty(B, D, NP, dtype=f32, device=dev)
+            ws.crf_nrm = torch.empty(B, NP, dtype=f32, device=dev)
+            ws.crf_tiles = torch.empty(B, NP // 64, NP // 64, dtype=torch.float64, device=dev)
+            # d(loss)/d(out) of loss += w * out.mean(): autograd's fl(fl(w) / (B n^2)), the same for every output
+            ws.crf_g = torch.full((1,), float(cfg.crf_weight), dtype=f32, device=dev).div_(B * n * n)
+            ws.crf_loss = torch.empty(1, dtype=f32, device=dev)
         # everything the kernels accumulate into: ONE buffer, ONE memset per step
         sizes = dict(dlogits=B * hw * 32, dtiles=spec.nslots * B * spec.rows * corr.DT_LD, dall=M * P,
                      dnc=n_clu * D, db_pad=P)
@@ -193,6 +228,9 @@ class FusedStep:
             torch.randperm(B, device=ws.perms.device, dtype=torch.long, out=ws.perms[i])
         if ws.aug:
             noises(2)  # net(img_aug), after the correspondence loss (train_segmentation.py:189-190)
+        if ws.crf:  # ContrastiveCRFLoss.draw_coords on the 56 x 56 maps: rows, then columns (train_segmentation.py:201-208)
+            for i in range(2):
+                torch.randint(0, modules.CRF_SIDE, (1, ws.crf_coords.shape[1]), out=ws.crf_coords[i:i + 1])
         w1, _, wa, _, wb, _ = net.head_params()
         modules.pack_head_weights(w1, wa, wb, ws.w1p, ws.wab, ws.wbp)
         ws.zbuf.zero_()
@@ -234,6 +272,15 @@ class FusedStep:
         if ws.aug:  # -cosine(sample(code, coord), code_aug) (train_segmentation.py:189-199)
             modules.aug_sample_forward(ws.coord_aug, code[img_rows], ws.grid, ws.sampled)
             modules.cosine_forward(ws.sampled, code[aug_rows], ws.cosv, ws.norma, ws.normb)
+        m3_img = ws.M3[img_rows] if ws.M3 is not None else None
+        dec = seg.decoder
+        if ws.rec:  # -cosine(decoder(code), feats * m3) (train_segmentation.py:183-187)
+            modules.rec_forward(ws.code[:B * hw], tok_all[:B].reshape(B * hw, E), m3_img, hw, dec.weight, dec.bias,
+                                ws.rec_cos, ws.rec_nr, ws.rec_nf)
+        if ws.crf:  # crf_loss_fn(resize(img, 56), norm(resize(code, 56))) at the samples (train_segmentation.py:201-208)
+            crf_p = modules.crf_params(seg.crf_loss_fn)
+            modules.crf_forward(code[img_rows], ws.crf_coords, crf_p, ws.crf_gsel, ws.crf_pos, ws.crf_raw, ws.crf_sel,
+                                ws.crf_nrm, ws.crf_tiles)
         seg._mark("corr_loss_forward")
 
         # ---- probes on the detached code (train_segmentation.py:213-225): forward + backward in place
@@ -244,8 +291,12 @@ class FusedStep:
         _lib.check(_lib.load().stego_step_losses(_lib.ptr(ws.stats), spec.ncalls, ws.call_w, _lib.ptr(ws.lin_loss),
                                                  _lib.ptr(ws.clu_loss), _lib.ptr(ws.out4), _lib.stream()),
                    "stego_step_losses")
+        if ws.rec:  # loss/rec, and its weighted value onto the total
+            modules.aug_loss(ws.rec_cos, seg.cfg.rec_weight, ws.rec_loss, ws.out4)
         if ws.aug:  # loss/aug_alignment, and its weighted value onto the total
             modules.aug_loss(ws.cosv, seg.cfg.aug_alignment_weight, ws.aug_loss, ws.out4)
+        if ws.crf:  # loss/crf, and its weighted value onto the total
+            modules.crf_loss(ws.crf_tiles, ws.crf_coords.shape[1], seg.cfg.crf_weight, ws.crf_loss, ws.out4)
         seg._mark("probes_forward")
 
         # ---- backward (manual_backward, :227)
@@ -254,11 +305,18 @@ class FusedStep:
         dall = ws.dall.view(M, P)
         corr.sample_norm_backward(code[img_rows], code[pos_rows], ws.c1, ws.c2, ws.perms, spec, ws.dtiles,
                                   dall[:B * hw], dall[B * hw:2 * B * hw], raw_perms=True)
+        dcode = dall.view(n * B, fh, fw, P)[..., :D].permute(0, 3, 1, 2)
         if ws.aug:  # d(code_aug) into the img_aug rows, d(sampled) scattered into the img rows
-            dcode = dall.view(n * B, fh, fw, P)[..., :D].permute(0, 3, 1, 2)
             modules.cosine_backward(ws.sampled, code[aug_rows], ws.cosv, ws.norma, ws.normb, ws.dcos, ws.dsampled,
                                     dcode[aug_rows])
             modules.aug_sample_backward(ws.grid, ws.dsampled, dcode[img_rows])
+        if ws.rec:  # d(code) into the img rows; the decoder's gradient straight into the flat gradient buffer
+            modules.rec_backward(ws.code[:B * hw], tok_all[:B].reshape(B * hw, E), m3_img, hw, dec.weight, dec.bias,
+                                 ws.rec_cos, ws.rec_nr, ws.rec_nf, ws.rec_dcos, dall[:B * hw], ws.rec_scratch,
+                                 dec.weight.grad, dec.bias.grad)
+        if ws.crf:  # d(code) scattered into the img rows
+            modules.crf_backward(ws.crf_g, ws.crf_sel, ws.crf_nrm, ws.crf_gsel, ws.crf_pos, ws.crf_coords, crf_p,
+                                 ws.crf_dsel, dcode[img_rows])
         # head backward: d(code) [M, P] -> bias / weight gradients straight into the flat gradient buffer
         modules.head_backward(dall, ws.x1, ws.x2, ws.hid, ws.wbp, ws.dyb, ws.db_pad, ws.dh, ws.dhb,
                               *[p.grad if p is not None else None for p in params])
@@ -277,17 +335,18 @@ class FusedStep:
         label_pos = batch["label_pos"] if cfg.use_true_labels else None
         mask = batch["mask"] if cfg.use_salience else None
         aug = cfg.aug_alignment_weight > 0
+        rec, crf = cfg.rec_weight > 0, cfg.crf_weight > 0  # supported() admitted them only with cfg.fused_rec_crf
         if aug:  # the host draws of the views come first: they overlap the previous step's work on the device
             seeds = augment._check(img, augment.batch_seeds(batch["seed"]), cfg.res)
             _, records = augment.draw_records(seeds, H, W)
         # a new flat parameter buffer (or another label dtype) invalidates the captured graph
         key = (B, H, W, LH, LW, dev.index, id(seg._flat), label.dtype,
                label_pos.dtype if label_pos is not None else None,
-               (tuple(mask.shape), mask.dtype, batch["mask_pos"].dtype) if mask is not None else None, aug)
+               (tuple(mask.shape), mask.dtype, batch["mask_pos"].dtype) if mask is not None else None, aug, rec, crf)
         if self.key != key:
             self.flush()
-            self.ws = self._alloc(B, H, W, LH, LW, dev, label.dtype, key[-3], key[-2][0] if mask is not None else None,
-                                  aug)
+            self.ws = self._alloc(B, H, W, LH, LW, dev, label.dtype, key[-5], key[-4][0] if mask is not None else None,
+                                  aug, rec, crf)
             self.key = key
             self.side = torch.cuda.Stream(device=dev)
         ws = self.ws
@@ -339,6 +398,8 @@ class FusedStep:
             if label_pos is not None:
                 ws.label_pos.copy_(label_pos.reshape(B, LH, LW))
             main.wait_event(ready)
+            if ws.crf:  # the guidance from this step's img, outside the tail graph (which bakes no caller pointer)
+                modules.crf_guidance(img, ws.crf_coords, ws.crf_gsel, ws.crf_pos)
             seg._mark("vit_forward")
             if seg.should_log_hist():
                 # histogram steps replay a tail graph of their own (captured the first time one is needed), so the
@@ -392,8 +453,12 @@ class FusedStep:
         seg.log('cd/neg_inter', out4[3])
         seg.log('loss/linear', ws.lin_loss[0])
         seg.log('loss/cluster', ws.clu_loss[0])
+        if ws.rec:
+            seg.log('loss/rec', ws.rec_loss[0])
         if ws.aug:
             seg.log('loss/aug_alignment', ws.aug_loss[0])
+        if ws.crf:
+            seg.log('loss/crf', ws.crf_loss[0])
         seg.log('loss/total', out4[0])
         self.step_idx += 1
         seg.global_step += 1

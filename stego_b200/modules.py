@@ -686,6 +686,80 @@ def aug_loss(cosv, weight: float, loss, total=None) -> None:
                                                 _lib.ptr(total), _lib.stream()), "stego_aug_align_loss")
 
 
+def rec_scratch(M: int, E: int, D: int, device) -> torch.Tensor:
+    """The per-CTA decoder-gradient partials rec_backward needs for M pixel rows on `device` (sized from its grid)."""
+    with torch.cuda.device(device):
+        nbytes = int(_lib.load().stego_rec_scratch_bytes(M, E, D))
+    return torch.empty(-(-nbytes // 4), dtype=torch.float32, device=device)
+
+
+def rec_forward(code, feat, m3, hw: int, weight, bias, cosv, nr, nf) -> None:
+    """The reconstruction term (train_segmentation.py:183-187) over M pixel rows: cosv [M] = <normalize(decoder(code)),
+    normalize(feat * m3)>, and the unclamped norms nr = |decoder(code)|, nf = |feat * m3| the backward reads
+    (csrc/rec_loss.cu; the decoder output is never written).  code: fp32 [M, >= D] rows; feat: bf16 [M, E] rows;
+    m3: fp32 [M / hw, E...] per-image channel scale or None; weight / bias: the decoder's [E, D, 1, 1] / [E]."""
+    M, E, D = feat.shape[0], weight.shape[0], weight.shape[1]
+    _lib.check(_lib.load().stego_rec_fwd(_lib.ptr(code), code.stride(0), _lib.ptr(feat), feat.stride(0), _lib.ptr(m3), hw,
+                                         _lib.ptr(weight), _lib.ptr(bias), M, E, D, _lib.ptr(cosv), _lib.ptr(nr),
+                                         _lib.ptr(nf), _lib.stream()), "stego_rec_fwd")
+
+
+def rec_backward(code, feat, m3, hw: int, weight, bias, cosv, nr, nf, dcos, dcode, scratch, dweight, dbias) -> None:
+    """dcode [M, >= D] rows += the term's code gradient for d loss / d cos = dcos[0]; dweight / dbias (the decoder's
+    shapes) are written, summed over the rows in a fixed order."""
+    M, E, D = feat.shape[0], weight.shape[0], weight.shape[1]
+    _lib.check(_lib.load().stego_rec_bwd(_lib.ptr(code), code.stride(0), _lib.ptr(feat), feat.stride(0), _lib.ptr(m3), hw,
+                                         _lib.ptr(weight), _lib.ptr(bias), M, E, D, _lib.ptr(cosv), _lib.ptr(nr),
+                                         _lib.ptr(nf), _lib.ptr(dcos), _lib.ptr(dcode), dcode.stride(0),
+                                         _lib.ptr(scratch), scratch.numel() * 4, _lib.ptr(dweight), _lib.ptr(dbias),
+                                         _lib.stream()), "stego_rec_bwd")
+
+
+CRF_SIDE = 56  # the CRF term works on resize(., 56) (train_segmentation.py:201-208)
+
+
+def crf_params(fn) -> tuple:
+    """(alpha, beta, gamma, w1, w2, shift) of a ContrastiveCRFLoss, as the kernels take them."""
+    return tuple(float(v) for v in (fn.alpha, fn.beta, fn.gamma, fn.w1, fn.w2, fn.shift))
+
+
+def crf_guidance(img, coords, gsel, pos) -> None:
+    """The CRF term's guidance: gsel [B, NP, 4] = resize(img, 56) (fp32 [B, <= 3, H, W], any strides) at the samples
+    coords [2, n], pos [NP, 2] their positions (csrc/crf_loss.cu)."""
+    B, Cg, H, W = img.shape
+    _lib.check(_lib.load().stego_crf_guidance(_lib.ptr(img), *img.stride(), Cg, H, W, _lib.ptr(coords), B,
+                                              coords.shape[1], CRF_SIDE, _lib.ptr(gsel), _lib.ptr(pos), _lib.stream()),
+               "stego_crf_guidance")
+
+
+def crf_forward(code, coords, params, gsel, pos, raw, sel, nrm, tile_sum) -> None:
+    """The CRF term's forward on the code (fp32 [B, C, h, w], any strides): raw [B, C, NP] = resize(code, 56) at the
+    samples, sel = normalize(raw) over the channels, nrm [B, NP] the norms, tile_sum [B, NP/64, NP/64] the fp64 sums of
+    -(Gram x pairwise kernel)."""
+    B, C, h, w = code.shape
+    _lib.check(_lib.load().stego_crf_mean_fwd(_lib.ptr(code), *code.stride(), C, h, w, _lib.ptr(coords), B,
+                                              coords.shape[1], CRF_SIDE, *params, _lib.ptr(gsel), _lib.ptr(pos),
+                                              _lib.ptr(raw), _lib.ptr(sel), _lib.ptr(nrm), _lib.ptr(tile_sum),
+                                              _lib.stream()),
+               "stego_crf_mean_fwd")
+
+
+def crf_loss(tile_sum, n: int, weight: float, loss, total=None) -> None:
+    """loss[0] = the mean of the B n^2 outputs from tile_sum, in a fixed order; total[0] += weight * loss[0] if given."""
+    _lib.check(_lib.load().stego_crf_mean_loss(_lib.ptr(tile_sum), tile_sum.shape[0], n, float(weight), _lib.ptr(loss),
+                                               _lib.ptr(total), _lib.stream()), "stego_crf_mean_loss")
+
+
+def crf_backward(gscalar, sel, nrm, gsel, pos, coords, params, dsel, dcode) -> None:
+    """dcode [B, C, h, w] (any strides) += the gradient of the mean for the upstream gradient gscalar[0] of every output,
+    by atomics; dsel [B, C, NP] is scratch."""
+    B, C, h, w = dcode.shape
+    _lib.check(_lib.load().stego_crf_mean_bwd(_lib.ptr(gscalar), _lib.ptr(sel), _lib.ptr(nrm), _lib.ptr(gsel),
+                                              _lib.ptr(pos), _lib.ptr(coords), B, C, coords.shape[1], h, w, CRF_SIDE,
+                                              *params, _lib.ptr(dsel), _lib.ptr(dcode), *dcode.stride(), _lib.stream()),
+               "stego_crf_mean_bwd")
+
+
 class _PixelCosineFn(torch.autograd.Function):
     """cos[b, y, x] = <normalize(a)[b, :, y, x], normalize(b)[b, :, y, x]> (F.normalize eps 1e-10, modules.py:275-276): one
     read of each operand in the forward, one in the backward (csrc/cosine_loss.cu)."""

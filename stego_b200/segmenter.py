@@ -426,9 +426,9 @@ class LitUnsupervisedSegmenter(nn.Module):
     # ---- the step ---------------------------------------------------------------------------------
     def training_step(self, batch, batch_idx):
         """train_segmentation.py:112-245.  The shipped configuration (dino arch, correspondence loss, no rec / crf
-        terms; use_salience, use_true_labels, "KK" and the aug-alignment term fed by batch["seed"] included) runs as the
-        hand-scheduled kernel sequence of fused_step.FusedStep; anything else (or cfg.fused_step = False) takes the
-        autograd-stitched path below.  Both compute the same step.
+        terms; use_salience, use_true_labels, "KK" and the aug-alignment term fed by batch["seed"] included, and the rec /
+        crf terms with cfg.fused_rec_crf) runs as the hand-scheduled kernel sequence of fused_step.FusedStep; anything
+        else (or cfg.fused_step = False) takes the autograd-stitched path below.  Both compute the same step.
 
         With cfg.aug_alignment_weight > 0 the batch carries either the views batch["img_aug"] / batch["coord_aug"]
         (the autograd path, with them) or batch["seed"]: B ints, a list or a CPU tensor, from which the step builds
