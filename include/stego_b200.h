@@ -390,6 +390,18 @@ STEGO_API int stego_eval_probes(const float* code, const float* code_flip, long 
                                 float* clu_log_probs, unsigned char* lin_argmax, unsigned char* clu_argmax,
                                 const void* label, int label_bytes, int n_label_classes, long long* lin_confusion,
                                 long long* clu_confusion, void* stream);
+/* stego_eval_probes with its outputs placed in a mosaic of tiles (plot_potsdam.py:65-81): frame b is tile tile0 + b of a
+ * tile_rows x tiles_per_row grid, in row-major tile order, and its pixel (y, x) goes to row
+ * ((tile0 + b) / tiles_per_row) * H + y, column ((tile0 + b) % tiles_per_row) * W + x of a plane of row pitch `pitch`
+ * (>= tiles_per_row * W): argmax maps [tile_rows*H][pitch] uint8, log-probabilities [n][tile_rows*H][pitch] fp32.
+ * label stays [B][H][W] (the B tiles' own labels); the confusion counts are those of stego_eval_probes. */
+STEGO_API int stego_eval_probes_mosaic(const float* code, const float* code_flip, long long ld_code, int C, int B, int h,
+                                       int w, int H, int W, const float* lin_weight, const float* lin_bias, int n_lin,
+                                       const float* clusters, int n_clu, float alpha, float* lr_scratch,
+                                       float* lin_log_probs, float* clu_log_probs, unsigned char* lin_argmax,
+                                       unsigned char* clu_argmax, const void* label, int label_bytes,
+                                       int n_label_classes, long long* lin_confusion, long long* clu_confusion,
+                                       int tile0, int tile_rows, int tiles_per_row, long long pitch, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * k-nearest-neighbour descriptors (SURVEY.md 8(f) rank 1; src/precompute_knns.py:15-21, 83-96):
@@ -453,6 +465,15 @@ STEGO_API int stego_eval_crf_unary(const float* code, const float* code_flip, lo
                                    int H, int W, const float* lin_weight, const float* lin_bias, int n_lin,
                                    const float* clusters, int n_clu, float alpha, float* lr_scratch, float* unary, float* Q,
                                    void* stream);
+/* stego_eval_crf_unary with the rows placed in a mosaic (the addressing of stego_eval_probes_mosaic: pixel (y, x) of
+ * frame b is row ((tile0 + b) / tiles_per_row * H + y) * pitch + (tile0 + b) % tiles_per_row * W + x).  probes = 3:
+ * rows of both probes (64 floats); 1 or 2: rows of 32 floats of the linear or the cluster probe alone
+ * (stego_crf_mean_field's one-probe rows). */
+STEGO_API int stego_eval_crf_unary_mosaic(const float* code, const float* code_flip, long long ld_code, int C, int B,
+                                          int h, int w, int H, int W, const float* lin_weight, const float* lin_bias,
+                                          int n_lin, const float* clusters, int n_clu, float alpha, float* lr_scratch,
+                                          float* unary, float* Q, int probes, int tile0, int tile_rows,
+                                          int tiles_per_row, long long pitch, void* stream);
 
 /* ---- contrastive CRF loss (optional training term; replaces ContrastiveCRFLoss.forward, src/modules.py:449-469, and its
  * autograd backward).  guidance [B, Cg <= 3, H, W] and clusters [B, C <= 80, H, W] are fp32 with arbitrary element strides;

@@ -47,6 +47,14 @@ def _pack(coords: torch.Tensor, d: int, bits: int) -> torch.Tensor:
     return key
 
 
+def lattice_key_bound(H: int, W: int, d: int, sxy: float, srgb: float = 0.0) -> Tuple[float, int]:
+    """(bound, limit): stego_crf_lattice's bound on the lattice coordinates of an H x W frame and the largest value its
+    packed keys hold (60 // d bits per coordinate, biased); the kernel refuses a frame with bound >= limit.  The same
+    arithmetic as crf.cu, so a caller can refuse such a frame before it launches anything."""
+    fmax = max(W, H) / sxy * 2 + (3 * 255.0 / srgb if d == 5 else 0.0)
+    return (d + 1) * 0.8165 * fmax + 2 * (d + 1), 1 << (60 // d - 1)
+
+
 def _lattice_points(H: int, W: int, d: int, sxy: float, srgb: float, image_u8: Optional[torch.Tensor], dev) -> _Lattice:
     """Lattice construction without the normalisation: the embedding of every pixel is a kernel; de-duplicating the
     vertex keys and finding the blur neighbours are a sort and binary searches (torch.unique / searchsorted).  The
@@ -101,13 +109,16 @@ def _norm(lat: _Lattice) -> None:
 _POSITION_LATTICES: Dict[Tuple[int, int, int], _Lattice] = {}
 
 
-def _position_lattice(H: int, W: int, dev) -> _Lattice:
+def _position_lattice(H: int, W: int, dev, cache: bool = True) -> _Lattice:
     """The Gaussian kernel's lattice of an H x W frame with its normalisation, cached per frame size: it depends on
-    pixel positions only, so every frame of that size shares it."""
+    pixel positions only, so every frame of that size shares it.  cache=False builds it for the caller alone (a scene
+    mosaic's lattice takes GBs and would stay for the life of the process); a cached copy is still reused."""
     key = (H, W, dev.index)
     if key not in _POSITION_LATTICES:
         lat = _lattice_points(H, W, 2, POS_XY_STD, 0.0, None, dev)
         _norm(lat)
+        if not cache:
+            return lat
         _POSITION_LATTICES[key] = lat
     return _POSITION_LATTICES[key]
 
@@ -140,6 +151,24 @@ def _bilateral_lattice(images_u8: Iterable[torch.Tensor]) -> _Lattice:
                                [torch.full((1,), B * slots_per_frame, dtype=torch.int32, device=dev)])
     _norm(out)
     return out
+
+
+def _free_device_memory(dev) -> int:
+    """Bytes a new allocation on dev can take: the device's free memory plus what torch's caching allocator holds
+    unused."""
+    free, _ = torch.cuda.mem_get_info(dev)
+    return int(free) + int(torch.cuda.memory_reserved(dev) - torch.cuda.memory_allocated(dev))
+
+
+def check_value_buffers(Mg: int, Mb: int, row: int, dev, what: str) -> None:
+    """Refuses a mean field whose value buffers (val / tmp of both lattices: 2 (Mg + Mb) rows of `row` fp32) do not fit
+    the free device memory, with a RuntimeError that names the sizes, instead of failing inside the allocation."""
+    need = 2 * (Mg + Mb) * row * 4
+    free = _free_device_memory(dev)
+    if need > free:
+        raise RuntimeError(f"{what}: the mean field's value buffers need {need / 2**30:.2f} GiB (position lattice {Mg} "
+                           f"points, bilateral lattice {Mb} points, rows of {row} floats, two buffers each) but "
+                           f"{free / 2**30:.2f} GiB of device memory is free")
 
 
 _IMAGENET_STATS: Dict[torch.device, Tuple[torch.Tensor, torch.Tensor]] = {}

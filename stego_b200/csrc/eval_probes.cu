@@ -119,6 +119,22 @@ eval_prep_kernel(EvalPrepParams p) {
   }
 }
 
+// Output addressing of a mosaic of tiles (eval_scene): frame b of a launch is tile tile0 + b of a grid of `cols` tiles
+// per row, and its pixel (Y, X) sits at row ((tile0 + b) / cols) * H + Y, column ((tile0 + b) % cols) * W + X of one
+// plane of row pitch `pitch` per map (and per class of the log-probabilities, planes `plane` floats apart).
+struct EvMosaic {
+  int tile0, cols;
+  long long pitch, plane;
+};
+
+// Pixel (Y, X) of frame b: frame-major [B][H][W] without a mosaic, else its place in the mosaic plane
+template <bool MOSAIC>
+__device__ __forceinline__ long long ev_out_pix(const EvMosaic& m, int H, int W, int b, int Y, int X) {
+  if (!MOSAIC) return (1ll * b * H + Y) * W + X;
+  const int tile = m.tile0 + b;
+  return (1ll * (tile / m.cols) * H + Y) * m.pitch + 1ll * (tile % m.cols) * W + X;
+}
+
 struct EvalProbeParams {
   const float* lr;   // [B*h*w][EV_LD]
   int B, h, w, H, W, n_lin, n_clu;
@@ -133,6 +149,7 @@ struct EvalProbeParams {
   int n_cls;               // label classes: a pixel counts when 0 <= label < n_cls and pred < n_cls (utils.py:222)
   unsigned long long* lin_conf;  // [n_lin][n_cls] += counts of (pred, actual), or null
   unsigned long long* clu_conf;  // [n_clu][n_cls]
+  EvMosaic mosaic;               // output addressing of eval_probe*_kernel<.., true>
 };
 
 // Output tile of a CTA: 64 x 4 pixels, thread = pixel, x fastest (coalesced plane writes).  (Measured and rejected in
@@ -240,6 +257,7 @@ __device__ __forceinline__ void ev_cluster(const float* slr, int bw, const EvCor
   }
 }
 
+template <bool MOSAIC>
 __global__ void __launch_bounds__(EVT_W* EVT_H)
 eval_probe_kernel(EvalProbeParams p) {
   extern __shared__ float slr[];  // [box_h*box_w][EV_LD]
@@ -255,8 +273,10 @@ eval_probe_kernel(EvalProbeParams p) {
   int lin_pred = -1, clu_pred = -1;
   if (active) {
     const EvCorners e = ev_corners(slr, t, p.h, p.w, Y, X);
-    const long long plane = 1ll * p.H * p.W;
+    // log-probability planes: [B][n][H][W], or one mosaic plane per class
+    const long long plane = MOSAIC ? p.mosaic.plane : 1ll * p.H * p.W;
     const long long pix = 1ll * Y * p.W + X;
+    const long long opix = ev_out_pix<MOSAIC>(p.mosaic, p.H, p.W, b, Y, X);
     // ---- linear probe: log_softmax of the interpolated logits
     if (p.lin_logp || p.lin_arg) {
       float z[32];
@@ -264,14 +284,14 @@ eval_probe_kernel(EvalProbeParams p) {
       int arg;
       ev_linear(e, p.n_lin, z, mx, arg);
       lin_pred = arg;
-      if (p.lin_arg) p.lin_arg[b * plane + pix] = static_cast<unsigned char>(arg);
+      if (p.lin_arg) p.lin_arg[opix] = static_cast<unsigned char>(arg);
       if (p.lin_logp) {
         float se = 0.f;
 #pragma unroll
         for (int k = 0; k < 32; ++k)
           if (k < p.n_lin) se += __expf(z[k] - mx);
         const float lse = mx + __logf(se);
-        float* o = p.lin_logp + (1ll * b * p.n_lin) * plane + pix;
+        float* o = p.lin_logp + (MOSAIC ? opix : (1ll * b * p.n_lin) * plane + pix);
 #pragma unroll
         for (int k = 0; k < 32; ++k)
           if (k < p.n_lin) o[k * plane] = z[k] - lse;
@@ -284,7 +304,7 @@ eval_probe_kernel(EvalProbeParams p) {
       int arg;
       ev_cluster(slr, t.bw, e, p.n_clu, z, mx, arg);
       clu_pred = arg;
-      if (p.clu_arg) p.clu_arg[b * plane + pix] = static_cast<unsigned char>(arg);
+      if (p.clu_arg) p.clu_arg[opix] = static_cast<unsigned char>(arg);
       if (p.clu_logp) {
         float m2 = -INFINITY;
 #pragma unroll
@@ -295,7 +315,7 @@ eval_probe_kernel(EvalProbeParams p) {
         for (int k = 0; k < 32; ++k)
           if (k < p.n_clu) se += __expf(z[k] * p.alpha - m2);
         const float lse = m2 + __logf(se);
-        float* o = p.clu_logp + (1ll * b * p.n_clu) * plane + pix;
+        float* o = p.clu_logp + (MOSAIC ? opix : (1ll * b * p.n_clu) * plane + pix);
 #pragma unroll
         for (int k = 0; k < 32; ++k)
           if (k < p.n_clu) o[k * plane] = z[k] * p.alpha - lse;
@@ -359,10 +379,17 @@ struct EvalCrfUnaryParams {
   const float* lr;  // [B*h*w][EV_LD]
   int B, h, w, H, W, n_lin, n_clu;
   float alpha;
-  float* unary;     // [B*H*W][EVC_LD]
-  float* Q;         // [B*H*W][EVC_LD]
+  float* unary;     // [B*H*W][32 per probe], or one row per mosaic pixel
+  float* Q;         // same rows
+  EvMosaic mosaic;  // row addressing of eval_crf_unary_kernel<.., true>: row = the pixel's place in the mosaic
 };
 
+// PROBES: which probes the rows hold, EV_PROBE_LIN | EV_PROBE_CLU.  Both: rows of EVC_LD floats, linear then cluster;
+// one: rows of 32 floats of that probe alone, the layout of dense_crf's one-probe rows, which halves the mean field's
+// value buffers when only one probe is wanted
+constexpr int EV_PROBE_LIN = 1, EV_PROBE_CLU = 2;
+
+template <int PROBES, bool MOSAIC>
 __global__ void __launch_bounds__(EVT_W* EVT_H)
 eval_crf_unary_kernel(EvalCrfUnaryParams p) {
   extern __shared__ float slr[];  // [box_h*box_w][EV_LD]
@@ -371,18 +398,25 @@ eval_crf_unary_kernel(EvalCrfUnaryParams p) {
   const int X = t.X0 + (threadIdx.x % EVT_W), Y = t.Y0 + (threadIdx.x / EVT_W);
   if (X >= p.W || Y >= p.H) return;
   const EvCorners e = ev_corners(slr, t, p.h, p.w, Y, X);
-  const long long row = (1ll * t.b * p.H + Y) * p.W + X;
-  float* u_row = p.unary + row * EVC_LD;
-  float* q_row = p.Q + row * EVC_LD;
+  const long long row = ev_out_pix<MOSAIC>(p.mosaic, p.H, p.W, t.b, Y, X);
+  constexpr int LD = PROBES == (EV_PROBE_LIN | EV_PROBE_CLU) ? EVC_LD : 32;
+  float* u_row = p.unary + row * LD;
+  float* q_row = p.Q + row * LD;
   float z[32];
   float mx;
   int arg;
-  ev_linear(e, p.n_lin, z, mx, arg);
-  ev_crf_half_rows(z, p.n_lin, u_row, q_row);
-  ev_cluster(slr, t.bw, e, p.n_clu, z, mx, arg);
+  if (PROBES & EV_PROBE_LIN) {
+    ev_linear(e, p.n_lin, z, mx, arg);
+    ev_crf_half_rows(z, p.n_lin, u_row, q_row);
+    u_row += 32;
+    q_row += 32;
+  }
+  if (PROBES & EV_PROBE_CLU) {
+    ev_cluster(slr, t.bw, e, p.n_clu, z, mx, arg);
 #pragma unroll
-  for (int k = 0; k < 32; ++k) z[k] *= p.alpha;
-  ev_crf_half_rows(z, p.n_clu, u_row + 32, q_row + 32);
+    for (int k = 0; k < 32; ++k) z[k] *= p.alpha;
+    ev_crf_half_rows(z, p.n_clu, u_row, q_row);
+  }
 }
 
 
@@ -453,7 +487,7 @@ __device__ __forceinline__ void ev4_probe(const float* ea, const float* eb, cons
   }
 }
 
-template <int NL, int NC>
+template <int NL, int NC, bool MOSAIC>
 __global__ void __launch_bounds__(EV4_TW* EV4_ROWS, 2)
 eval_probe_vec4_kernel(EvalProbeParams p) {
   extern __shared__ __align__(16) float slr[];  // [box_h*box_w][EV_LD]
@@ -499,15 +533,18 @@ eval_probe_vec4_kernel(EvalProbeParams p) {
     const float* eb = slr + (y0 * bw + x1) * EV_LD;
     const float* ec = slr + (y1 * bw + x0) * EV_LD;
     const float* ed = slr + (y1 * bw + x1) * EV_LD;
-    const long long plane = 1ll * p.H * p.W;
+    const long long plane = 1ll * p.H * p.W;  // one frame's pixels (the label's layout)
     const long long pix = 1ll * Y * p.W + X;
+    // outputs: [B][n][H][W] log-probabilities and [B][H][W] maps, or their places in the mosaic
+    const long long oplane = MOSAIC ? p.mosaic.plane : plane;
+    const long long opix = ev_out_pix<MOSAIC>(p.mosaic, p.H, p.W, b, Y, X);
     int lin_pred[4] = {-1, -1, -1, -1}, clu_pred[4] = {-1, -1, -1, -1};
     float one[4] = {1.f, 1.f, 1.f, 1.f};
     if (p.lin_logp || p.lin_arg) {
-      ev4_probe<NL, false>(ea, eb, ec, ed, ly, lx, one, p.lin_logp ? p.lin_logp + (1ll * b * NL) * plane + pix : nullptr,
-                           plane, lin_pred);
+      float* out = p.lin_logp ? p.lin_logp + (MOSAIC ? opix : (1ll * b * NL) * plane + pix) : nullptr;
+      ev4_probe<NL, false>(ea, eb, ec, ed, ly, lx, one, out, oplane, lin_pred);
       if (p.lin_arg)
-        *reinterpret_cast<uchar4*>(p.lin_arg + b * plane + pix) =
+        *reinterpret_cast<uchar4*>(p.lin_arg + opix) =
             make_uchar4((unsigned char)lin_pred[0], (unsigned char)lin_pred[1], (unsigned char)lin_pred[2], (unsigned char)lin_pred[3]);
     }
     if (p.clu_logp || p.clu_arg) {
@@ -528,10 +565,10 @@ eval_probe_vec4_kernel(EvalProbeParams p) {
         const double n2 = wx0 * (wx0 * ll + 2.0 * wx * lr) + wx * wx * rr;
         scale[j] = p.alpha / fmaxf(sqrtf(fmaxf(static_cast<float>(n2), 0.f)), 1e-12f);
       }
-      ev4_probe<NC, true>(ea + 32, eb + 32, ec + 32, ed + 32, ly, lx, scale,
-                          p.clu_logp ? p.clu_logp + (1ll * b * NC) * plane + pix : nullptr, plane, clu_pred);
+      float* out = p.clu_logp ? p.clu_logp + (MOSAIC ? opix : (1ll * b * NC) * plane + pix) : nullptr;
+      ev4_probe<NC, true>(ea + 32, eb + 32, ec + 32, ed + 32, ly, lx, scale, out, oplane, clu_pred);
       if (p.clu_arg)
-        *reinterpret_cast<uchar4*>(p.clu_arg + b * plane + pix) =
+        *reinterpret_cast<uchar4*>(p.clu_arg + opix) =
             make_uchar4((unsigned char)clu_pred[0], (unsigned char)clu_pred[1], (unsigned char)clu_pred[2], (unsigned char)clu_pred[3]);
     }
     if (want_conf) {
@@ -562,24 +599,22 @@ static int launch_eval_prep(const float* code, const float* code_flip, long long
   return STEGO_OK;
 }
 
-// code: tokens-major low-res code [B*h*w][ld_code] fp32 (what DinoFeaturizer produces); outputs at [H][W].
-// code_flip: the code of the horizontally flipped images (flip-TTA) or null.  lr_scratch: [B*h*w][80] floats, 16-byte aligned.
-// label + confusion outputs (int64, accumulated): optional.  Any output pointer may be null.
-extern "C" int stego_eval_probes(const float* code, const float* code_flip, long long ld_code, int C, int B, int h, int w,
-                                 int H, int W, const float* lin_weight, const float* lin_bias, int n_lin,
-                                 const float* clusters, int n_clu, float alpha, float* lr_scratch, float* lin_log_probs,
-                                 float* clu_log_probs, unsigned char* lin_argmax, unsigned char* clu_argmax,
-                                 const void* label, int label_bytes, int n_label_classes, long long* lin_confusion,
-                                 long long* clu_confusion, void* stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  STEGO_CHECK_ARG(code && lin_weight && lin_bias && clusters && lr_scratch, "stego_eval_probes: null pointer");
-  STEGO_CHECK_ARG((reinterpret_cast<uintptr_t>(lr_scratch) & 7u) == 0, "stego_eval_probes: lr_scratch not 8-byte aligned");
+// The probe pass of stego_eval_probes / stego_eval_probes_mosaic (m: null for frame-major outputs); `who` names the
+// entry in errors.
+static int eval_probes(const char* who, const float* code, const float* code_flip, long long ld_code, int C, int B,
+                       int h, int w, int H, int W, const float* lin_weight, const float* lin_bias, int n_lin,
+                       const float* clusters, int n_clu, float alpha, float* lr_scratch, float* lin_log_probs,
+                       float* clu_log_probs, unsigned char* lin_argmax, unsigned char* clu_argmax, const void* label,
+                       int label_bytes, int n_label_classes, long long* lin_confusion, long long* clu_confusion,
+                       const EvMosaic* m, cudaStream_t stream) {
+  STEGO_CHECK_ARG(code && lin_weight && lin_bias && clusters && lr_scratch, "%s: null pointer", who);
+  STEGO_CHECK_ARG((reinterpret_cast<uintptr_t>(lr_scratch) & 7u) == 0, "%s: lr_scratch not 8-byte aligned", who);
   STEGO_CHECK_ARG(C > 0 && C <= 96 && n_lin > 0 && n_lin <= 32 && n_clu > 0 && n_clu <= 32,
-                  "stego_eval_probes: C=%d n_lin=%d n_clu=%d unsupported (C <= 96, classes <= 32)", C, n_lin, n_clu);
-  STEGO_CHECK_ARG(B > 0 && h > 0 && w > 0 && H >= h && W >= w, "stego_eval_probes: bad sizes (upsampling only)");
+                  "%s: C=%d n_lin=%d n_clu=%d unsupported (C <= 96, classes <= 32)", who, C, n_lin, n_clu);
+  STEGO_CHECK_ARG(B > 0 && h > 0 && w > 0 && H >= h && W >= w, "%s: bad sizes (upsampling only)", who);
   STEGO_CHECK_ARG(!label || ((label_bytes == 8 || label_bytes == 4 || label_bytes == 1) && n_label_classes > 0 &&
                              n_label_classes <= 32 && (lin_confusion || clu_confusion)),
-                  "stego_eval_probes: confusion counts need label_bytes in {8,4,1}, n_label_classes <= 32 and an output");
+                  "%s: confusion counts need label_bytes in {8,4,1}, n_label_classes <= 32 and an output", who);
   int rc;
   if ((rc = launch_eval_prep(code, code_flip, ld_code, C, B, h, w, lin_weight, lin_bias, n_lin, clusters, n_clu,
                              lr_scratch, stream)) != STEGO_OK)
@@ -590,9 +625,11 @@ extern "C" int stego_eval_probes(const float* code, const float* code_flip, long
   p.label = label; p.label_bytes = label_bytes; p.n_cls = n_label_classes;
   p.lin_conf = reinterpret_cast<unsigned long long*>(lin_confusion);
   p.clu_conf = reinterpret_cast<unsigned long long*>(clu_confusion);
+  p.mosaic = m ? *m : EvMosaic{0, 1, W, 1ll * H * W};
   // four pixels per thread when a group of four x-adjacent pixels always shares its two source columns: integer
-  // horizontal factor that is a multiple of 8 (every patch-8 / patch-16 model evaluated at the label resolution)
-  const bool vec4 = n_lin == 27 && n_clu == 27 && W % w == 0 && (W / w) % 8 == 0 &&
+  // horizontal factor that is a multiple of 8 (every patch-8 / patch-16 model evaluated at the label resolution).  In a
+  // mosaic a group stays 16-byte aligned when the pitch is a multiple of 4 (W is a multiple of 8 here).
+  const bool vec4 = n_lin == 27 && n_clu == 27 && W % w == 0 && (W / w) % 8 == 0 && (!m || m->pitch % 4 == 0) &&
                     (!lin_log_probs || (reinterpret_cast<uintptr_t>(lin_log_probs) & 15) == 0) &&
                     (!clu_log_probs || (reinterpret_cast<uintptr_t>(clu_log_probs) & 15) == 0) &&
                     (!lin_argmax || (reinterpret_cast<uintptr_t>(lin_argmax) & 3) == 0) &&
@@ -602,18 +639,123 @@ extern "C" int stego_eval_probes(const float* code, const float* code_flip, long
   p.box_h = src_span_max(tile_h, h, H);
   p.box_w = src_span_max(tile_w, w, W);
   const size_t smem = (size_t)p.box_h * p.box_w * EV_LD * sizeof(float);
-  STEGO_CHECK_ARG(smem <= 200 * 1024, "stego_eval_probes: upsample ratio needs %zu B of shared memory", smem);
+  STEGO_CHECK_ARG(smem <= 200 * 1024, "%s: upsample ratio needs %zu B of shared memory", who, smem);
   const long long tiles = 1ll * B * ((H + tile_h - 1) / tile_h) * ((W + tile_w - 1) / tile_w);
-  STEGO_CHECK_ARG(tiles < (1ll << 31), "stego_eval_probes: too many tiles");
+  STEGO_CHECK_ARG(tiles < (1ll << 31), "%s: too many tiles", who);
   if (vec4) {
-    if ((rc = opt_in_smem<eval_probe_vec4_kernel<27, 27>>(smem, "eval_probe_vec4_kernel")) != STEGO_OK) return rc;
-    eval_probe_vec4_kernel<27, 27><<<(unsigned)tiles, EV4_TW * EV4_ROWS, smem, stream>>>(p);
+    if (m) {
+      if ((rc = opt_in_smem<eval_probe_vec4_kernel<27, 27, true>>(smem, "eval_probe_vec4_kernel")) != STEGO_OK) return rc;
+      eval_probe_vec4_kernel<27, 27, true><<<(unsigned)tiles, EV4_TW * EV4_ROWS, smem, stream>>>(p);
+    } else {
+      if ((rc = opt_in_smem<eval_probe_vec4_kernel<27, 27, false>>(smem, "eval_probe_vec4_kernel")) != STEGO_OK) return rc;
+      eval_probe_vec4_kernel<27, 27, false><<<(unsigned)tiles, EV4_TW * EV4_ROWS, smem, stream>>>(p);
+    }
     STEGO_CHECK_LAUNCH("eval_probe_vec4_kernel");
     return STEGO_OK;
   }
-  if ((rc = opt_in_smem<eval_probe_kernel>(smem, "eval_probe_kernel")) != STEGO_OK) return rc;
-  eval_probe_kernel<<<(unsigned)tiles, EVT_W * EVT_H, smem, stream>>>(p);
+  if (m) {
+    if ((rc = opt_in_smem<eval_probe_kernel<true>>(smem, "eval_probe_kernel")) != STEGO_OK) return rc;
+    eval_probe_kernel<true><<<(unsigned)tiles, EVT_W * EVT_H, smem, stream>>>(p);
+  } else {
+    if ((rc = opt_in_smem<eval_probe_kernel<false>>(smem, "eval_probe_kernel")) != STEGO_OK) return rc;
+    eval_probe_kernel<false><<<(unsigned)tiles, EVT_W * EVT_H, smem, stream>>>(p);
+  }
   STEGO_CHECK_LAUNCH("eval_probe_kernel");
+  return STEGO_OK;
+}
+
+// The mosaic of a launch: B tiles from tile0 in a grid of tile_rows x tiles_per_row tiles of H x W pixels, rows of
+// `pitch` elements (at least tiles_per_row * W)
+static int check_mosaic(const char* who, int B, int H, int W, int tile0, int tile_rows, int tiles_per_row,
+                        long long pitch, EvMosaic& m) {
+  STEGO_CHECK_ARG(tile_rows > 0 && tiles_per_row > 0 && tile0 >= 0 && B > 0 &&
+                  1ll * tile0 + B <= 1ll * tile_rows * tiles_per_row && pitch >= 1ll * tiles_per_row * W,
+                  "%s: tiles [%d, %d) do not fit a %d x %d grid of pitch %lld (at least %lld)", who, tile0, tile0 + B,
+                  tile_rows, tiles_per_row, pitch, 1ll * tiles_per_row * W);
+  m.tile0 = tile0; m.cols = tiles_per_row; m.pitch = pitch; m.plane = 1ll * tile_rows * H * pitch;
+  return STEGO_OK;
+}
+
+// code: tokens-major low-res code [B*h*w][ld_code] fp32 (what DinoFeaturizer produces); outputs at [H][W].
+// code_flip: the code of the horizontally flipped images (flip-TTA) or null.  lr_scratch: [B*h*w][80] floats, 16-byte aligned.
+// label + confusion outputs (int64, accumulated): optional.  Any output pointer may be null.
+extern "C" int stego_eval_probes(const float* code, const float* code_flip, long long ld_code, int C, int B, int h, int w,
+                                 int H, int W, const float* lin_weight, const float* lin_bias, int n_lin,
+                                 const float* clusters, int n_clu, float alpha, float* lr_scratch, float* lin_log_probs,
+                                 float* clu_log_probs, unsigned char* lin_argmax, unsigned char* clu_argmax,
+                                 const void* label, int label_bytes, int n_label_classes, long long* lin_confusion,
+                                 long long* clu_confusion, void* stream_) {
+  return eval_probes("stego_eval_probes", code, code_flip, ld_code, C, B, h, w, H, W, lin_weight, lin_bias, n_lin,
+                     clusters, n_clu, alpha, lr_scratch, lin_log_probs, clu_log_probs, lin_argmax, clu_argmax, label,
+                     label_bytes, n_label_classes, lin_confusion, clu_confusion, nullptr,
+                     reinterpret_cast<cudaStream_t>(stream_));
+}
+
+// stego_eval_probes with the outputs placed in a mosaic (check_mosaic): argmax maps [tile_rows*H][pitch] uint8,
+// log-probabilities [n][tile_rows*H][pitch] fp32.  The label and the confusion counts are as in stego_eval_probes.
+extern "C" int stego_eval_probes_mosaic(const float* code, const float* code_flip, long long ld_code, int C, int B, int h,
+                                        int w, int H, int W, const float* lin_weight, const float* lin_bias, int n_lin,
+                                        const float* clusters, int n_clu, float alpha, float* lr_scratch,
+                                        float* lin_log_probs, float* clu_log_probs, unsigned char* lin_argmax,
+                                        unsigned char* clu_argmax, const void* label, int label_bytes,
+                                        int n_label_classes, long long* lin_confusion, long long* clu_confusion,
+                                        int tile0, int tile_rows, int tiles_per_row, long long pitch, void* stream_) {
+  EvMosaic m;
+  int rc;
+  if ((rc = check_mosaic("stego_eval_probes_mosaic", B, H, W, tile0, tile_rows, tiles_per_row, pitch, m)) != STEGO_OK)
+    return rc;
+  return eval_probes("stego_eval_probes_mosaic", code, code_flip, ld_code, C, B, h, w, H, W, lin_weight, lin_bias, n_lin,
+                     clusters, n_clu, alpha, lr_scratch, lin_log_probs, clu_log_probs, lin_argmax, clu_argmax, label,
+                     label_bytes, n_label_classes, lin_confusion, clu_confusion, &m,
+                     reinterpret_cast<cudaStream_t>(stream_));
+}
+
+template <int PROBES, bool MOSAIC>
+static int launch_crf_unary(const EvalCrfUnaryParams& p, long long tiles, size_t smem, cudaStream_t stream) {
+  int rc;
+  if ((rc = opt_in_smem<eval_crf_unary_kernel<PROBES, MOSAIC>>(smem, "eval_crf_unary_kernel")) != STEGO_OK) return rc;
+  eval_crf_unary_kernel<PROBES, MOSAIC><<<(unsigned)tiles, EVT_W * EVT_H, smem, stream>>>(p);
+  return STEGO_OK;
+}
+
+template <int PROBES>
+static int launch_crf_unary(const EvalCrfUnaryParams& p, bool mosaic, long long tiles, size_t smem, cudaStream_t stream) {
+  return mosaic ? launch_crf_unary<PROBES, true>(p, tiles, smem, stream)
+                : launch_crf_unary<PROBES, false>(p, tiles, smem, stream);
+}
+
+// The unary pass of stego_eval_crf_unary / stego_eval_crf_unary_mosaic (m: null for frame-major rows); probes
+// EV_PROBE_LIN | EV_PROBE_CLU (rows of 64 floats) or one of them (rows of 32).
+static int eval_crf_unary(const char* who, const float* code, const float* code_flip, long long ld_code, int C, int B,
+                          int h, int w, int H, int W, const float* lin_weight, const float* lin_bias, int n_lin,
+                          const float* clusters, int n_clu, float alpha, float* lr_scratch, float* unary, float* Q,
+                          int probes, const EvMosaic* m, cudaStream_t stream) {
+  STEGO_CHECK_ARG(code && lin_weight && lin_bias && clusters && lr_scratch && unary && Q, "%s: null pointer", who);
+  STEGO_CHECK_ARG((reinterpret_cast<uintptr_t>(lr_scratch) & 7u) == 0 && (reinterpret_cast<uintptr_t>(unary) & 15u) == 0 &&
+                  (reinterpret_cast<uintptr_t>(Q) & 15u) == 0,
+                  "%s: lr_scratch must be 8-byte aligned, unary and Q 16-byte aligned", who);
+  STEGO_CHECK_ARG(C > 0 && C <= 96 && n_lin > 0 && n_lin <= 32 && n_clu > 0 && n_clu <= 32,
+                  "%s: C=%d n_lin=%d n_clu=%d unsupported (C <= 96, classes <= 32)", who, C, n_lin, n_clu);
+  STEGO_CHECK_ARG(B > 0 && h > 0 && w > 0 && H >= h && W >= w, "%s: bad sizes (upsampling only)", who);
+  STEGO_CHECK_ARG(probes >= 1 && probes <= 3, "%s: probes = %d (1: linear, 2: cluster, 3: both)", who, probes);
+  const int box_h = src_span_max(EVT_H, h, H), box_w = src_span_max(EVT_W, w, W);
+  const size_t smem = (size_t)box_h * box_w * EV_LD * sizeof(float);
+  STEGO_CHECK_ARG(smem <= 200 * 1024, "%s: upsample ratio needs %zu B of shared memory", who, smem);
+  const long long tiles = 1ll * B * ((H + EVT_H - 1) / EVT_H) * ((W + EVT_W - 1) / EVT_W);
+  STEGO_CHECK_ARG(tiles < (1ll << 31), "%s: too many tiles", who);
+  int rc;
+  if ((rc = launch_eval_prep(code, code_flip, ld_code, C, B, h, w, lin_weight, lin_bias, n_lin, clusters, n_clu,
+                             lr_scratch, stream)) != STEGO_OK)
+    return rc;
+  EvalCrfUnaryParams p;
+  p.lr = lr_scratch; p.B = B; p.h = h; p.w = w; p.H = H; p.W = W; p.n_lin = n_lin; p.n_clu = n_clu; p.alpha = alpha;
+  p.unary = unary; p.Q = Q;
+  p.mosaic = m ? *m : EvMosaic{0, 1, W, 1ll * H * W};
+  if (probes == (EV_PROBE_LIN | EV_PROBE_CLU)) rc = launch_crf_unary<EV_PROBE_LIN | EV_PROBE_CLU>(p, m, tiles, smem, stream);
+  else if (probes == EV_PROBE_LIN) rc = launch_crf_unary<EV_PROBE_LIN>(p, m, tiles, smem, stream);
+  else rc = launch_crf_unary<EV_PROBE_CLU>(p, m, tiles, smem, stream);
+  if (rc != STEGO_OK) return rc;
+  STEGO_CHECK_LAUNCH("eval_crf_unary_kernel");
   return STEGO_OK;
 }
 
@@ -623,28 +765,25 @@ extern "C" int stego_eval_crf_unary(const float* code, const float* code_flip, l
                                     int H, int W, const float* lin_weight, const float* lin_bias, int n_lin,
                                     const float* clusters, int n_clu, float alpha, float* lr_scratch, float* unary, float* Q,
                                     void* stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  STEGO_CHECK_ARG(code && lin_weight && lin_bias && clusters && lr_scratch && unary && Q, "stego_eval_crf_unary: null pointer");
-  STEGO_CHECK_ARG((reinterpret_cast<uintptr_t>(lr_scratch) & 7u) == 0 && (reinterpret_cast<uintptr_t>(unary) & 15u) == 0 &&
-                  (reinterpret_cast<uintptr_t>(Q) & 15u) == 0,
-                  "stego_eval_crf_unary: lr_scratch must be 8-byte aligned, unary and Q 16-byte aligned");
-  STEGO_CHECK_ARG(C > 0 && C <= 96 && n_lin > 0 && n_lin <= 32 && n_clu > 0 && n_clu <= 32,
-                  "stego_eval_crf_unary: C=%d n_lin=%d n_clu=%d unsupported (C <= 96, classes <= 32)", C, n_lin, n_clu);
-  STEGO_CHECK_ARG(B > 0 && h > 0 && w > 0 && H >= h && W >= w, "stego_eval_crf_unary: bad sizes (upsampling only)");
-  const int box_h = src_span_max(EVT_H, h, H), box_w = src_span_max(EVT_W, w, W);
-  const size_t smem = (size_t)box_h * box_w * EV_LD * sizeof(float);
-  STEGO_CHECK_ARG(smem <= 200 * 1024, "stego_eval_crf_unary: upsample ratio needs %zu B of shared memory", smem);
-  const long long tiles = 1ll * B * ((H + EVT_H - 1) / EVT_H) * ((W + EVT_W - 1) / EVT_W);
-  STEGO_CHECK_ARG(tiles < (1ll << 31), "stego_eval_crf_unary: too many tiles");
+  return eval_crf_unary("stego_eval_crf_unary", code, code_flip, ld_code, C, B, h, w, H, W, lin_weight, lin_bias, n_lin,
+                        clusters, n_clu, alpha, lr_scratch, unary, Q, EV_PROBE_LIN | EV_PROBE_CLU, nullptr,
+                        reinterpret_cast<cudaStream_t>(stream_));
+}
+
+// stego_eval_crf_unary with the rows placed in a mosaic (check_mosaic): pixel (Y, X) of frame b is row
+// ((tile0 + b) / tiles_per_row * H + Y) * pitch + (tile0 + b) % tiles_per_row * W + X of unary and Q.  probes: 3 for
+// rows of both probes (64 floats, linear then cluster), 1 or 2 for rows of 32 floats of the linear or the cluster
+// probe alone.
+extern "C" int stego_eval_crf_unary_mosaic(const float* code, const float* code_flip, long long ld_code, int C, int B,
+                                           int h, int w, int H, int W, const float* lin_weight, const float* lin_bias,
+                                           int n_lin, const float* clusters, int n_clu, float alpha, float* lr_scratch,
+                                           float* unary, float* Q, int probes, int tile0, int tile_rows,
+                                           int tiles_per_row, long long pitch, void* stream_) {
+  EvMosaic m;
   int rc;
-  if ((rc = launch_eval_prep(code, code_flip, ld_code, C, B, h, w, lin_weight, lin_bias, n_lin, clusters, n_clu,
-                             lr_scratch, stream)) != STEGO_OK)
+  if ((rc = check_mosaic("stego_eval_crf_unary_mosaic", B, H, W, tile0, tile_rows, tiles_per_row, pitch, m)) != STEGO_OK)
     return rc;
-  if ((rc = opt_in_smem<eval_crf_unary_kernel>(smem, "eval_crf_unary_kernel")) != STEGO_OK) return rc;
-  EvalCrfUnaryParams p;
-  p.lr = lr_scratch; p.B = B; p.h = h; p.w = w; p.H = H; p.W = W; p.n_lin = n_lin; p.n_clu = n_clu; p.alpha = alpha;
-  p.unary = unary; p.Q = Q;
-  eval_crf_unary_kernel<<<(unsigned)tiles, EVT_W * EVT_H, smem, stream>>>(p);
-  STEGO_CHECK_LAUNCH("eval_crf_unary_kernel");
-  return STEGO_OK;
+  return eval_crf_unary("stego_eval_crf_unary_mosaic", code, code_flip, ld_code, C, B, h, w, H, W, lin_weight, lin_bias,
+                        n_lin, clusters, n_clu, alpha, lr_scratch, unary, Q, probes, &m,
+                        reinterpret_cast<cudaStream_t>(stream_));
 }

@@ -679,34 +679,185 @@ class LitUnsupervisedSegmenter(nn.Module):
             result.update(linear_probs=probs[0], cluster_probs=probs[1])
         return result
 
-    def _check_eval_args(self, img, label, run_crf: bool) -> None:
+    def eval_scene(self, tiles: torch.Tensor, grid: Sequence[int], label: Optional[torch.Tensor] = None,
+                   run_crf: bool = False, probes: Sequence[str] = ("linear", "cluster"), want_probs: bool = False,
+                   map_clusters: bool = False, chunk: int = 64) -> Dict[str, torch.Tensor]:
+        """A scene evaluated from its tiles and stitched into one mosaic (plot_potsdam.py:44-83):
+
+            for each chunk of tiles: eval_step's loop body (flip-TTA code, upsampling, probes, metric updates)
+            stitch: tile i goes to tile row i // C, tile column i % C of an R t x C t mosaic
+            probs = dense_crf(mosaic image, mosaic probs) if run_crf          # one CRF across the tile seams
+            preds = test_cluster_metrics.map_clusters(probs.argmax(0)) if map_clusters
+
+        tiles: the normalised frames [R*C, 3, t, t'], fp32 or bf16, CUDA, in row-major tile order; grid = (R, C).  label
+        (optional): [R*C, t, t'], uint8 with 255 = ignore, int32 or int64.  probes: the probes to evaluate, "linear"
+        and / or "cluster".  Returns `<probe>_preds` uint8 [R t, C t'] per probe and, with want_probs,
+        `<probe>_probs` fp32 [n, R t, C t']: the log-probabilities without the CRF, the CRF marginals with it.
+
+        The tiles go through the backbone `chunk` at a time, each frame with its mirror in one pass as in eval_step
+        (two graph shapes at most: the full chunk and the tail), and the probe kernels write straight into the mosaic.
+        Without run_crf the confusion matrices (test_linear_metrics / test_cluster_metrics.stats) are updated per tile
+        and the outputs are bit-equal to eval_step per chunk, stitched.  With run_crf the chunks write the CRF's unary
+        rows of the mosaic, the stitched image is embedded once and one mean field runs over the whole mosaic; the
+        confusion counts are those of its predictions against the stitched label.  One probe (plot_potsdam's
+        probes=("cluster",), or the linear probe alone) runs rows of that probe only: 32 floats a pixel instead of 64,
+        half the CRF's memory and filtering work.  The mosaic's position lattice is built for the call, not cached,
+        unless the grid is a single tile.  A CRF mosaic must fit the lattice's packed keys (a longer side of at most
+        about 5380 pixels: Potsdam's 4800² scene fits, its native 6000² does not) and its int32 slot ids.
+
+        map_clusters: the cluster predictions mapped to classes by test_cluster_metrics' Hungarian assignment
+        (UnsupervisedMetrics.map_clusters; unmatched extra clusters become 255); the metric's compute() must have run.
+        Every argument is checked before the first launch (ValueError for shapes and limits, RuntimeError for CPU
+        tensors), and the mean field's value buffers are checked against the free device memory before it is
+        enqueued (RuntimeError naming the sizes)."""
+        from . import crf
+        from .eval import _probe_codes, _probe_tables
+        R, C, n_tiles, H, W, probes = self._check_scene_args(tiles, grid, label, run_crf, probes, map_clusters, chunk)
+        self.flush()
+        tiles = tiles.detach().contiguous()
+        lib = _lib.load()
+        net = self.net
+        dev = tiles.device
+        p = net.patch_size
+        h, w = H // p, W // p
+        HH, WW = R * H, C * W
+        lin_on, clu_on = "linear" in probes, "cluster" in probes
+        n_lin, n_clu = self.linear_probe.weight.shape[0], self.cluster_probe.clusters.shape[0]
+        wl, bl, cl = _probe_tables(self.linear_probe, self.cluster_probe, net.dim)
+        scratch = torch.empty(min(chunk, n_tiles) * h * w, 80, dtype=torch.float32, device=dev)  # eval_probes.cu EV_LD
+        lin_stats = self.test_linear_metrics.stats if label is not None and lin_on else None
+        clu_stats = self.test_cluster_metrics.stats if label is not None and clu_on else None
+        out = {}
+        if run_crf:
+            row = 32 * len(probes)  # rows of both probes (linear, then cluster), or of the one requested
+            unary = torch.empty(HH * WW, row, dtype=torch.float32, device=dev)
+            Q = torch.empty(HH * WW, row, dtype=torch.float32, device=dev)
+        else:
+            lab, lab_bytes = ops.probe_label(label, n_tiles, H, W) if label is not None else (None, 0)
+            preds = {k: torch.empty(HH, WW, dtype=torch.uint8, device=dev) for k in probes}
+            probs = {k: torch.empty(n, HH, WW, dtype=torch.float32, device=dev)
+                     for k, n in (("linear", n_lin), ("cluster", n_clu)) if k in probes} if want_probs else {}
+        with self._net_in_eval_mode(), torch.no_grad():
+            for t0 in range(0, n_tiles, chunk):
+                img = tiles[t0:t0 + chunk]
+                B = img.shape[0]
+                tok = net.backbone_tokens(img, use_graph=getattr(self.cfg, "cuda_graph", True), mirror=True)
+                code_all = net.head_code(tok, None, None, h, w)  # [2B, dim, h, w]
+                x, xf, ld = _probe_codes(code_all[:B], code_all[B:])
+                if run_crf:
+                    _lib.check(lib.stego_eval_crf_unary_mosaic(
+                        _lib.ptr(x), _lib.ptr(xf), ld, net.dim, B, h, w, H, W, _lib.ptr(wl), _lib.ptr(bl), n_lin,
+                        _lib.ptr(cl), n_clu, 2.0, _lib.ptr(scratch), _lib.ptr(unary), _lib.ptr(Q), int(lin_on) + 2 * int(clu_on), t0, R, C, WW,
+                        _lib.stream()), "stego_eval_crf_unary_mosaic")
+                else:
+                    _lib.check(lib.stego_eval_probes_mosaic(
+                        _lib.ptr(x), _lib.ptr(xf), ld, net.dim, B, h, w, H, W, _lib.ptr(wl), _lib.ptr(bl), n_lin,
+                        _lib.ptr(cl), n_clu, 2.0, _lib.ptr(scratch), _lib.ptr(probs.get("linear")),
+                        _lib.ptr(probs.get("cluster")), _lib.ptr(preds.get("linear")), _lib.ptr(preds.get("cluster")),
+                        _lib.ptr(lab[t0:] if lab is not None else None), lab_bytes, n_lin if lab is not None else 0,
+                        _lib.ptr(lin_stats), _lib.ptr(clu_stats), t0, R, C, WW, _lib.stream()),
+                        "stego_eval_probes_mosaic")
+        if run_crf:
+            image = crf.prepare_image(tiles.view(R, C, 3, H, W).permute(2, 0, 3, 1, 4).reshape(3, HH, WW))
+            lg = crf._position_lattice(HH, WW, dev, cache=n_tiles == 1)
+            lb = crf._bilateral_lattice([image])
+            crf.check_value_buffers(lg.M, lb.M, row, dev, "eval_scene")
+            val_g = torch.empty(2, lg.M, row, dtype=torch.float32, device=dev)
+            val_b = torch.empty(2, lb.M, row, dtype=torch.float32, device=dev)
+            lab, lab_bytes = (None, 0)
+            if label is not None:
+                lab, lab_bytes = ops.probe_label(label.reshape(R, C, H, W).permute(0, 2, 1, 3), 1, HH, WW)
+            preds = {k: torch.empty(HH, WW, dtype=torch.uint8, device=dev) for k in probes}
+            probs = {k: torch.empty(n, HH, WW, dtype=torch.float32, device=dev)
+                     for k, n in (("linear", n_lin), ("cluster", n_clu)) if k in probes} if want_probs else {}
+            # the mean field's two probe slots in row order; one probe (either) takes the first slot
+            slots = [(k, n, st) for k, n, st in (("linear", n_lin, lin_stats), ("cluster", n_clu, clu_stats)) if k in probes]
+            (first, n0, conf0), (second, n1, conf1) = slots[0], (slots[1] if len(slots) == 2 else (None, 0, None))
+            _lib.check(lib.stego_crf_mean_field(
+                1, HH * WW, n0, n1, crf.MAX_ITER, _lib.ptr(unary), _lib.ptr(Q),
+                _lib.ptr(lg.offset), _lib.ptr(lg.bary), _lib.ptr(lg.rowptr), _lib.ptr(lg.slots), _lib.ptr(lg.n1),
+                _lib.ptr(lg.n2), _lib.ptr(lg.norm), lg.M,
+                _lib.ptr(lb.offset), _lib.ptr(lb.bary), _lib.ptr(lb.rowptr), _lib.ptr(lb.slots), _lib.ptr(lb.n1),
+                _lib.ptr(lb.n2), _lib.ptr(lb.norm), lb.M, float(crf.POS_W), float(crf.Bi_W),
+                _lib.ptr(val_g[0]), _lib.ptr(val_g[1]), _lib.ptr(val_b[0]), _lib.ptr(val_b[1]),
+                _lib.ptr(probs.get(first)), _lib.ptr(probs.get(second)), _lib.ptr(preds[first]),
+                _lib.ptr(preds.get(second)), _lib.ptr(lab), lab_bytes, n_lin if lab is not None else 0,
+                _lib.ptr(conf0), _lib.ptr(conf1), _lib.stream()), "stego_crf_mean_field")
+        for k in probes:
+            out[f"{k}_preds"] = preds[k]
+            if want_probs:
+                out[f"{k}_probs"] = probs[k]
+        if map_clusters:
+            lut = self.test_cluster_metrics.map_clusters(torch.arange(n_clu, device=dev)).to(torch.uint8)
+            out["cluster_preds"] = lut[out["cluster_preds"].int()]
+        return out
+
+    def _check_scene_args(self, tiles, grid, label, run_crf, probes, map_clusters, chunk):
+        """eval_scene's own rules, then eval_step's on the tiles as one batch (shapes and limits: ValueError; CPU
+        tensors last: RuntimeError).  Returns (R, C, n_tiles, H, W, probes as a tuple)."""
+        if tiles.dim() != 4:
+            raise ValueError(f"eval_scene: tiles must be [R*C, 3, H, W], got {tuple(tiles.shape)}")
+        n_tiles, _, H, W = tiles.shape
+        try:
+            R, C = (int(g) for g in grid)
+        except (TypeError, ValueError):
+            raise ValueError(f"eval_scene: grid must be (rows, columns), got {grid!r}") from None
+        if R < 1 or C < 1 or R * C != n_tiles:
+            raise ValueError(f"eval_scene: a {R} x {C} grid does not hold the {n_tiles} tiles")
+        probes = tuple(probes)
+        if not probes or len(set(probes)) != len(probes) or not set(probes) <= {"linear", "cluster"}:
+            raise ValueError(f"eval_scene: probes must be \"linear\" and / or \"cluster\", got {probes!r}")
+        if isinstance(chunk, bool) or not isinstance(chunk, int) or chunk < 1:
+            raise ValueError(f"eval_scene: chunk must be a positive int, got {chunk!r}")
+        if label is not None and tuple(label.shape) != (n_tiles, H, W):
+            raise ValueError(f"eval_scene: label {tuple(label.shape)} is not one {H}x{W} map per tile of {n_tiles}")
+        if run_crf:
+            from . import crf
+            if 6 * R * H * C * W >= 1 << 31:
+                raise ValueError(f"eval_scene: a {R * H}x{C * W} mosaic has more lattice slots than the CRF's int32 "
+                                 f"slot ids hold (6 per pixel, < 2^31)")
+            bound, limit = crf.lattice_key_bound(R * H, C * W, 5, crf.Bi_XY_STD, crf.Bi_RGB_STD)
+            if bound >= limit:
+                raise ValueError(f"eval_scene: a {R * H}x{C * W} mosaic's bilateral lattice coordinates reach "
+                                 f"{bound:.0f}, beyond the {limit} its packed keys hold (a longer side of at most "
+                                 f"about 5380 pixels)")
+        if map_clusters:
+            if "cluster" not in probes:
+                raise ValueError("eval_scene: map_clusters needs the cluster probe")
+            if not hasattr(self.test_cluster_metrics, "assignments"):
+                raise ValueError("eval_scene: map_clusters needs test_cluster_metrics.compute() to have run (its "
+                                 "Hungarian assignment)")
+        self._check_eval_args(tiles, label, run_crf, who="eval_scene")
+        return R, C, n_tiles, H, W, probes
+
+    def _check_eval_args(self, img, label, run_crf: bool, who: str = "eval_step") -> None:
         """eval_step's arguments against the rules of the kernels it calls, shapes and limits first (ValueError), the
         device last (RuntimeError), so that nothing is enqueued for a call that would fail part-way."""
         from .eval import _check_crf_args
         net = self.net
         p = net.patch_size
         if img.dim() != 4 or img.shape[1] != 3 or img.shape[0] < 1 or img.dtype not in (torch.float32, torch.bfloat16):
-            raise ValueError(f"eval_step: img must be fp32 or bf16 [B, 3, H, W], got {img.dtype} {tuple(img.shape)}")
+            raise ValueError(f"{who}: img must be fp32 or bf16 [B, 3, H, W], got {img.dtype} {tuple(img.shape)}")
         B, _, H, W = img.shape
         # the patchify rules (stego_vit_patchify_tta): patch 8 or 16, whole patches, rows of a multiple of 8 pixels
         if p not in (8, 16) or H % p or W % p or W % 8:
-            raise ValueError(f"eval_step: a {H}x{W} frame is not whole {p}x{p} patches with W a multiple of 8 "
+            raise ValueError(f"{who}: a {H}x{W} frame is not whole {p}x{p} patches with W a multiple of 8 "
                              f"(patch 8 or 16)")
         if net.proj_type is None:
-            raise ValueError(f"eval_step: projection_type None gives a code of {net.n_feats} channels; the fused "
+            raise ValueError(f"{who}: projection_type None gives a code of {net.n_feats} channels; the fused "
                              f"evaluation probes take at most 96")
         n_lin, n_clu = self.linear_probe.weight.shape[0], self.cluster_probe.clusters.shape[0]
         if n_lin > 32 or n_clu > 32:
-            raise ValueError(f"eval_step: {n_lin} linear-probe classes / {n_clu} cluster-probe rows unsupported by the "
+            raise ValueError(f"{who}: {n_lin} linear-probe classes / {n_clu} cluster-probe rows unsupported by the "
                              f"fused evaluation probes (at most 32 each)")
         if label is not None:
             if label.dtype not in ops.LABEL_BYTES:
-                raise ValueError(f"eval_step: label dtype {label.dtype} unsupported (uint8, int32 or int64)")
+                raise ValueError(f"{who}: label dtype {label.dtype} unsupported (uint8, int32 or int64)")
             Hl, Wl = label.shape[-2:]
             if label.dim() < 2 or label.numel() != B * Hl * Wl:
-                raise ValueError(f"eval_step: label {tuple(label.shape)} is not one [H, W] map per frame of {B}")
+                raise ValueError(f"{who}: label {tuple(label.shape)} is not one [H, W] map per frame of {B}")
             if Hl < H // p or Wl < W // p:
-                raise ValueError(f"eval_step: label {Hl}x{Wl} is smaller than the code {H // p}x{W // p} "
+                raise ValueError(f"{who}: label {Hl}x{Wl} is smaller than the code {H // p}x{W // p} "
                                  f"(upsampling only)")
         if run_crf:
             # fused_eval_crf's own checks (label at the frames' size, ...), on a stand-in of the code's shape
