@@ -369,6 +369,23 @@ STEGO_API int stego_linear_probe_ce(const float* code, long long ld_code, int C,
                                     int n_classes, const void* label, int label_bytes, int B, int h, int w, int H,
                                     int Wimg, float* logits_scratch, float* dlogits_scratch, float* partials_scratch,
                                     float* loss_out, float grad_loss, float* dW, float* db, void* stream);
+/* stego_linear_probe_ce for a wide code: the backbone's C = 384 / 768 channels (projection_type None).  Same arguments
+ * plus dfix_scratch, int64 [B*h*w][32] zeroed by the caller (needed with dlogits_scratch): the logit gradient is
+ * accumulated there as exact fixed-point integers, and dW / db are reduced over the rows in a fixed order, so two
+ * identical calls give bit-identical results. */
+STEGO_API int stego_linear_probe_ce_wide(const float* code, long long ld_code, int C, const float* W, const float* bias,
+                                         int n_classes, const void* label, int label_bytes, int B, int h, int w, int H,
+                                         int Wimg, float* logits_scratch, float* dlogits_scratch,
+                                         long long* dfix_scratch, float* partials_scratch, float* loss_out,
+                                         float grad_loss, float* dW, float* db, void* stream);
+/* The training step's ClusterLookup (alpha None, src/train_segmentation.py:221-223) on a wide code: the backbone's
+ * C = 384 / 768 channels (projection_type None), x [rows][ld_x] fp32 tokens-major, clusters [n][C] with n <= 64.
+ * loss_out[0] = -mean_r max_k <x_r / |x_r|, c_k / |c_k|>; with dclusters (and dnc_scratch [n][C], zeroed by the
+ * caller) also dclusters += d loss_out[0] / d clusters.  Scratch: assign_scratch int32 [rows], inv_scratch fp32
+ * [rows], partials_scratch >= 16*SMs floats.  Every reduction over rows has a fixed order (no atomics). */
+STEGO_API int stego_cluster_lookup_wide(const float* x, long long ld_x, long long rows, int C, const float* clusters,
+                                        int n_classes, int* assign_scratch, float* inv_scratch, float* partials_scratch,
+                                        float* loss_out, float* dnc_scratch, float* dclusters, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Fused evaluation probes (src/eval_segmentation.py:128-131, BASELINE.json configs[4]):
@@ -474,6 +491,36 @@ STEGO_API int stego_eval_crf_unary_mosaic(const float* code, const float* code_f
                                           int n_lin, const float* clusters, int n_clu, float alpha, float* lr_scratch,
                                           float* unary, float* Q, int probes, int tile0, int tile_rows,
                                           int tiles_per_row, long long pitch, void* stream);
+
+/* ---- wide codes (projection_type None, the DINO baseline: the probes on the backbone's features) ---------------------
+ * The four eval entries above also take C = 384 or 768 (fp32 code).  The _bf16 entries below are the same four with
+ * a bf16 code and code_flip, C = 384 or 768 only: the backbone's tokens read in place, e.g. the two halves of the
+ * [2B, h*w, E] mirrored tokens.  Every other width is refused. */
+STEGO_API int stego_eval_probes_bf16(const void* code, const void* code_flip, long long ld_code, int C, int B, int h,
+                                     int w, int H, int W, const float* lin_weight, const float* lin_bias, int n_lin,
+                                     const float* clusters, int n_clu, float alpha, float* lr_scratch,
+                                     float* lin_log_probs, float* clu_log_probs, unsigned char* lin_argmax,
+                                     unsigned char* clu_argmax, const void* label, int label_bytes,
+                                     int n_label_classes, long long* lin_confusion, long long* clu_confusion,
+                                     void* stream);
+STEGO_API int stego_eval_probes_mosaic_bf16(const void* code, const void* code_flip, long long ld_code, int C, int B,
+                                            int h, int w, int H, int W, const float* lin_weight, const float* lin_bias,
+                                            int n_lin, const float* clusters, int n_clu, float alpha,
+                                            float* lr_scratch, float* lin_log_probs, float* clu_log_probs,
+                                            unsigned char* lin_argmax, unsigned char* clu_argmax, const void* label,
+                                            int label_bytes, int n_label_classes, long long* lin_confusion,
+                                            long long* clu_confusion, int tile0, int tile_rows, int tiles_per_row,
+                                            long long pitch, void* stream);
+STEGO_API int stego_eval_crf_unary_bf16(const void* code, const void* code_flip, long long ld_code, int C, int B, int h,
+                                        int w, int H, int W, const float* lin_weight, const float* lin_bias, int n_lin,
+                                        const float* clusters, int n_clu, float alpha, float* lr_scratch, float* unary,
+                                        float* Q, void* stream);
+STEGO_API int stego_eval_crf_unary_mosaic_bf16(const void* code, const void* code_flip, long long ld_code, int C, int B,
+                                               int h, int w, int H, int W, const float* lin_weight,
+                                               const float* lin_bias, int n_lin, const float* clusters, int n_clu,
+                                               float alpha, float* lr_scratch, float* unary, float* Q, int probes,
+                                               int tile0, int tile_rows, int tiles_per_row, long long pitch,
+                                               void* stream);
 
 /* ---- contrastive CRF loss (optional training term; replaces ContrastiveCRFLoss.forward, src/modules.py:449-469, and its
  * autograd backward).  guidance [B, Cg <= 3, H, W] and clusters [B, C <= 80, H, W] are fp32 with arbitrary element strides;

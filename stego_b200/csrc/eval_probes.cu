@@ -119,6 +119,91 @@ eval_prep_kernel(EvalPrepParams p) {
   }
 }
 
+// ---- wide codes: the backbone's 384 / 768 channels (projection_type None, the DINO baseline) ------------------------
+// The same EV_LD cells as eval_prep_kernel, with the channels in K tiles instead of three registers per lane.  A CTA
+// takes PW_ROWS low-res pixels at a time:
+//   * dots: wide_tile_dots of the (flip-averaged) code with the probe table [32 linear weights | 32 normalised
+//     centroids];
+//   * Gram entries: warp per pixel, lanes = channels, fp64 products and sums as in eval_prep_kernel.
+// The code is read tokens-major in fp32 or bf16 (the backbone's own tokens: no fp32 copy of the feature map).
+
+template <typename T>
+struct EvalPrepWideParams {
+  const T* code;       // [B*h*w][ld] tokens-major
+  const T* code_flip;  // flipped image's code (same layout) or null
+  long long ld;
+  int B, h, w, C;
+  const float* W;
+  const float* bias;
+  int n_lin;
+  const float* clusters;
+  int n_clu;
+  float* lr;  // [B*h*w][EV_LD]
+};
+
+__device__ __forceinline__ float ev_f32(float v) { return v; }
+__device__ __forceinline__ float ev_f32(__nv_bfloat16 v) { return __bfloat162float(v); }
+
+// Channel c of low-res pixel (y + dy, x + dx), row r = (b, y, x), flip-averaged as eval_prep_kernel does (the caller
+// checks that the pixel exists)
+template <typename T>
+__device__ __forceinline__ float ev_code_at(const EvalPrepWideParams<T>& p, long long r, int x, int dy, int dx, int c) {
+  float v = ev_f32(p.code[(r + 1ll * dy * p.w + dx) * p.ld + c]);
+  if (p.code_flip)
+    v = 0.5f * (v + ev_f32(p.code_flip[(r - x + (p.w - 1 - x) + 1ll * dy * p.w - dx) * p.ld + c]));
+  return v;
+}
+
+template <typename T>
+__global__ void __launch_bounds__(256, 2)
+eval_prep_wide_kernel(EvalPrepWideParams<T> p) {
+  __shared__ __align__(16) float sX[PW_ROWS * PW_SX];
+  __shared__ float sW[PW_KC * 64];
+  __shared__ float sinv[32];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  centroid_inv_norms(p.clusters, p.n_clu, p.C, sinv);
+  __syncthreads();
+  const long long rows = 1ll * p.B * p.h * p.w;
+  const int o = threadIdx.x & 63, rg = threadIdx.x >> 6;  // output column, pixel group (16 pixels)
+  for (long long r0 = 1ll * blockIdx.x * PW_ROWS; r0 < rows; r0 += 1ll * gridDim.x * PW_ROWS) {
+    float acc[16], unused = 0.f;
+    const float b0 = (o < p.n_lin) ? p.bias[o] : 0.f;
+#pragma unroll
+    for (int i = 0; i < 16; ++i) acc[i] = b0;
+    wide_tile_dots<false>([&](long long r, int c) { return ev_code_at(p, r, static_cast<int>(r % p.w), 0, 0, c); }, rows, r0,
+                   p.C, [&](int c, int k) {
+                     if (k < 32) return k < p.n_lin ? p.W[1ll * k * p.C + c] : 0.f;
+                     return k - 32 < p.n_clu ? p.clusters[1ll * (k - 32) * p.C + c] * sinv[k - 32] : 0.f;
+                   }, sX, sW, acc, unused);
+#pragma unroll
+    for (int i = 0; i < 16; ++i) {
+      const long long r = r0 + rg * 16 + i;
+      if (r < rows) p.lr[r * EV_LD + o] = acc[i];
+    }
+    // Gram entries with the right, down, down-right and down-left neighbours
+    for (int rr = warp; rr < PW_ROWS; rr += 8) {
+      const long long r = r0 + rr;
+      if (r >= rows) break;
+      const int x = static_cast<int>(r % p.w), y = static_cast<int>((r / p.w) % p.h);
+      const bool hr = x + 1 < p.w, hd = y + 1 < p.h, hl = x > 0;
+      double g0 = 0.0, g1 = 0.0, g2 = 0.0, g3 = 0.0, g4 = 0.0;
+      for (int c = lane; c < p.C; c += 32) {
+        const double v = ev_code_at(p, r, x, 0, 0, c);
+        g0 = fma(v, v, g0);
+        if (hr) g1 = fma(v, (double)ev_code_at(p, r, x, 0, 1, c), g1);
+        if (hd) g2 = fma(v, (double)ev_code_at(p, r, x, 1, 0, c), g2);
+        if (hd && hr) g3 = fma(v, (double)ev_code_at(p, r, x, 1, 1, c), g3);
+        if (hd && hl) g4 = fma(v, (double)ev_code_at(p, r, x, 1, -1, c), g4);
+      }
+      g0 = warp_sum_f64(g0); g1 = warp_sum_f64(g1); g2 = warp_sum_f64(g2); g3 = warp_sum_f64(g3); g4 = warp_sum_f64(g4);
+      if (lane == 0) {
+        double* og = reinterpret_cast<double*>(p.lr + r * EV_LD + EV_G);
+        og[EV_SS] = g0; og[EV_R] = g1; og[EV_D] = g2; og[EV_DR] = g3; og[EV_DL] = g4;
+      }
+    }
+  }
+}
+
 // Output addressing of a mosaic of tiles (eval_scene): frame b of a launch is tile tile0 + b of a grid of `cols` tiles
 // per row, and its pixel (Y, X) sits at row ((tile0 + b) / cols) * H + Y, column ((tile0 + b) % cols) * W + X of one
 // plane of row pitch `pitch` per map (and per class of the log-probabilities, planes `plane` floats apart).
@@ -584,10 +669,41 @@ eval_probe_vec4_kernel(EvalProbeParams p) {
 
 using namespace stego;
 
-// eval_prep_kernel over the B*h*w low-res pixels (arguments checked by the caller)
-static int launch_eval_prep(const float* code, const float* code_flip, long long ld_code, int C, int B, int h, int w,
-                            const float* lin_weight, const float* lin_bias, int n_lin, const float* clusters, int n_clu,
-                            float* lr_scratch, cudaStream_t stream) {
+// The code widths the eval entries take: the projection head's (1..96, fp32) or the backbone's (384 / 768, the code
+// of projection_type None, fp32 or bf16)
+static bool eval_code_ok(int C, int code_bytes) {
+  if (C == 384 || C == 768) return code_bytes == 4 || code_bytes == 2;
+  return C > 0 && C <= 96 && code_bytes == 4;
+}
+
+template <typename T>
+static int launch_eval_prep_wide(const void* code, const void* code_flip, long long ld_code, int C, int B, int h, int w,
+                                 const float* lin_weight, const float* lin_bias, int n_lin, const float* clusters,
+                                 int n_clu, float* lr_scratch, cudaStream_t stream) {
+  EvalPrepWideParams<T> q;
+  q.code = static_cast<const T*>(code); q.code_flip = static_cast<const T*>(code_flip); q.ld = ld_code;
+  q.B = B; q.h = h; q.w = w; q.C = C; q.W = lin_weight; q.bias = lin_bias; q.n_lin = n_lin; q.clusters = clusters;
+  q.n_clu = n_clu; q.lr = lr_scratch;
+  const long long tiles = (1ll * B * h * w + PW_ROWS - 1) / PW_ROWS;
+  const long long cap = 2ll * num_sms();
+  eval_prep_wide_kernel<T><<<(unsigned)(tiles < cap ? tiles : cap), 256, 0, stream>>>(q);
+  STEGO_CHECK_LAUNCH("eval_prep_wide_kernel");
+  return STEGO_OK;
+}
+
+// eval_prep_kernel over the B*h*w low-res pixels, or eval_prep_wide_kernel for the backbone's widths (arguments checked
+// by the caller: eval_code_ok)
+static int launch_eval_prep(const void* code_, const void* code_flip_, int code_bytes, long long ld_code, int C, int B,
+                            int h, int w, const float* lin_weight, const float* lin_bias, int n_lin,
+                            const float* clusters, int n_clu, float* lr_scratch, cudaStream_t stream) {
+  if (C > 96) {
+    return code_bytes == 2 ? launch_eval_prep_wide<__nv_bfloat16>(code_, code_flip_, ld_code, C, B, h, w, lin_weight,
+                                                                   lin_bias, n_lin, clusters, n_clu, lr_scratch, stream)
+                           : launch_eval_prep_wide<float>(code_, code_flip_, ld_code, C, B, h, w, lin_weight, lin_bias,
+                                                          n_lin, clusters, n_clu, lr_scratch, stream);
+  }
+  const float* code = static_cast<const float*>(code_);
+  const float* code_flip = static_cast<const float*>(code_flip_);
   EvalPrepParams q;
   q.code = code; q.code_flip = code_flip; q.ld = ld_code; q.B = B; q.h = h; q.w = w; q.C = C; q.W = lin_weight; q.bias = lin_bias;
   q.n_lin = n_lin; q.clusters = clusters; q.n_clu = n_clu; q.lr = lr_scratch;
@@ -601,23 +717,24 @@ static int launch_eval_prep(const float* code, const float* code_flip, long long
 
 // The probe pass of stego_eval_probes / stego_eval_probes_mosaic (m: null for frame-major outputs); `who` names the
 // entry in errors.
-static int eval_probes(const char* who, const float* code, const float* code_flip, long long ld_code, int C, int B,
-                       int h, int w, int H, int W, const float* lin_weight, const float* lin_bias, int n_lin,
-                       const float* clusters, int n_clu, float alpha, float* lr_scratch, float* lin_log_probs,
-                       float* clu_log_probs, unsigned char* lin_argmax, unsigned char* clu_argmax, const void* label,
-                       int label_bytes, int n_label_classes, long long* lin_confusion, long long* clu_confusion,
-                       const EvMosaic* m, cudaStream_t stream) {
+static int eval_probes(const char* who, const void* code, const void* code_flip, int code_bytes, long long ld_code,
+                       int C, int B, int h, int w, int H, int W, const float* lin_weight, const float* lin_bias,
+                       int n_lin, const float* clusters, int n_clu, float alpha, float* lr_scratch,
+                       float* lin_log_probs, float* clu_log_probs, unsigned char* lin_argmax,
+                       unsigned char* clu_argmax, const void* label, int label_bytes, int n_label_classes,
+                       long long* lin_confusion, long long* clu_confusion, const EvMosaic* m, cudaStream_t stream) {
   STEGO_CHECK_ARG(code && lin_weight && lin_bias && clusters && lr_scratch, "%s: null pointer", who);
   STEGO_CHECK_ARG((reinterpret_cast<uintptr_t>(lr_scratch) & 7u) == 0, "%s: lr_scratch not 8-byte aligned", who);
-  STEGO_CHECK_ARG(C > 0 && C <= 96 && n_lin > 0 && n_lin <= 32 && n_clu > 0 && n_clu <= 32,
-                  "%s: C=%d n_lin=%d n_clu=%d unsupported (C <= 96, classes <= 32)", who, C, n_lin, n_clu);
+  STEGO_CHECK_ARG(eval_code_ok(C, code_bytes) && n_lin > 0 && n_lin <= 32 && n_clu > 0 && n_clu <= 32,
+                  "%s: C=%d (%d-byte code) n_lin=%d n_clu=%d unsupported (C <= 96 fp32, or 384 / 768 fp32 or bf16; "
+                  "classes <= 32)", who, C, code_bytes, n_lin, n_clu);
   STEGO_CHECK_ARG(B > 0 && h > 0 && w > 0 && H >= h && W >= w, "%s: bad sizes (upsampling only)", who);
   STEGO_CHECK_ARG(!label || ((label_bytes == 8 || label_bytes == 4 || label_bytes == 1) && n_label_classes > 0 &&
                              n_label_classes <= 32 && (lin_confusion || clu_confusion)),
                   "%s: confusion counts need label_bytes in {8,4,1}, n_label_classes <= 32 and an output", who);
   int rc;
-  if ((rc = launch_eval_prep(code, code_flip, ld_code, C, B, h, w, lin_weight, lin_bias, n_lin, clusters, n_clu,
-                             lr_scratch, stream)) != STEGO_OK)
+  if ((rc = launch_eval_prep(code, code_flip, code_bytes, ld_code, C, B, h, w, lin_weight, lin_bias, n_lin, clusters,
+                             n_clu, lr_scratch, stream)) != STEGO_OK)
     return rc;
   EvalProbeParams p;
   p.lr = lr_scratch; p.B = B; p.h = h; p.w = w; p.H = H; p.W = W; p.n_lin = n_lin; p.n_clu = n_clu; p.alpha = alpha;
@@ -685,7 +802,7 @@ extern "C" int stego_eval_probes(const float* code, const float* code_flip, long
                                  float* clu_log_probs, unsigned char* lin_argmax, unsigned char* clu_argmax,
                                  const void* label, int label_bytes, int n_label_classes, long long* lin_confusion,
                                  long long* clu_confusion, void* stream_) {
-  return eval_probes("stego_eval_probes", code, code_flip, ld_code, C, B, h, w, H, W, lin_weight, lin_bias, n_lin,
+  return eval_probes("stego_eval_probes", code, code_flip, 4, ld_code, C, B, h, w, H, W, lin_weight, lin_bias, n_lin,
                      clusters, n_clu, alpha, lr_scratch, lin_log_probs, clu_log_probs, lin_argmax, clu_argmax, label,
                      label_bytes, n_label_classes, lin_confusion, clu_confusion, nullptr,
                      reinterpret_cast<cudaStream_t>(stream_));
@@ -704,7 +821,7 @@ extern "C" int stego_eval_probes_mosaic(const float* code, const float* code_fli
   int rc;
   if ((rc = check_mosaic("stego_eval_probes_mosaic", B, H, W, tile0, tile_rows, tiles_per_row, pitch, m)) != STEGO_OK)
     return rc;
-  return eval_probes("stego_eval_probes_mosaic", code, code_flip, ld_code, C, B, h, w, H, W, lin_weight, lin_bias, n_lin,
+  return eval_probes("stego_eval_probes_mosaic", code, code_flip, 4, ld_code, C, B, h, w, H, W, lin_weight, lin_bias, n_lin,
                      clusters, n_clu, alpha, lr_scratch, lin_log_probs, clu_log_probs, lin_argmax, clu_argmax, label,
                      label_bytes, n_label_classes, lin_confusion, clu_confusion, &m,
                      reinterpret_cast<cudaStream_t>(stream_));
@@ -726,16 +843,17 @@ static int launch_crf_unary(const EvalCrfUnaryParams& p, bool mosaic, long long 
 
 // The unary pass of stego_eval_crf_unary / stego_eval_crf_unary_mosaic (m: null for frame-major rows); probes
 // EV_PROBE_LIN | EV_PROBE_CLU (rows of 64 floats) or one of them (rows of 32).
-static int eval_crf_unary(const char* who, const float* code, const float* code_flip, long long ld_code, int C, int B,
-                          int h, int w, int H, int W, const float* lin_weight, const float* lin_bias, int n_lin,
+static int eval_crf_unary(const char* who, const void* code, const void* code_flip, int code_bytes, long long ld_code,
+                          int C, int B, int h, int w, int H, int W, const float* lin_weight, const float* lin_bias, int n_lin,
                           const float* clusters, int n_clu, float alpha, float* lr_scratch, float* unary, float* Q,
                           int probes, const EvMosaic* m, cudaStream_t stream) {
   STEGO_CHECK_ARG(code && lin_weight && lin_bias && clusters && lr_scratch && unary && Q, "%s: null pointer", who);
   STEGO_CHECK_ARG((reinterpret_cast<uintptr_t>(lr_scratch) & 7u) == 0 && (reinterpret_cast<uintptr_t>(unary) & 15u) == 0 &&
                   (reinterpret_cast<uintptr_t>(Q) & 15u) == 0,
                   "%s: lr_scratch must be 8-byte aligned, unary and Q 16-byte aligned", who);
-  STEGO_CHECK_ARG(C > 0 && C <= 96 && n_lin > 0 && n_lin <= 32 && n_clu > 0 && n_clu <= 32,
-                  "%s: C=%d n_lin=%d n_clu=%d unsupported (C <= 96, classes <= 32)", who, C, n_lin, n_clu);
+  STEGO_CHECK_ARG(eval_code_ok(C, code_bytes) && n_lin > 0 && n_lin <= 32 && n_clu > 0 && n_clu <= 32,
+                  "%s: C=%d (%d-byte code) n_lin=%d n_clu=%d unsupported (C <= 96 fp32, or 384 / 768 fp32 or bf16; "
+                  "classes <= 32)", who, C, code_bytes, n_lin, n_clu);
   STEGO_CHECK_ARG(B > 0 && h > 0 && w > 0 && H >= h && W >= w, "%s: bad sizes (upsampling only)", who);
   STEGO_CHECK_ARG(probes >= 1 && probes <= 3, "%s: probes = %d (1: linear, 2: cluster, 3: both)", who, probes);
   const int box_h = src_span_max(EVT_H, h, H), box_w = src_span_max(EVT_W, w, W);
@@ -744,8 +862,8 @@ static int eval_crf_unary(const char* who, const float* code, const float* code_
   const long long tiles = 1ll * B * ((H + EVT_H - 1) / EVT_H) * ((W + EVT_W - 1) / EVT_W);
   STEGO_CHECK_ARG(tiles < (1ll << 31), "%s: too many tiles", who);
   int rc;
-  if ((rc = launch_eval_prep(code, code_flip, ld_code, C, B, h, w, lin_weight, lin_bias, n_lin, clusters, n_clu,
-                             lr_scratch, stream)) != STEGO_OK)
+  if ((rc = launch_eval_prep(code, code_flip, code_bytes, ld_code, C, B, h, w, lin_weight, lin_bias, n_lin, clusters,
+                             n_clu, lr_scratch, stream)) != STEGO_OK)
     return rc;
   EvalCrfUnaryParams p;
   p.lr = lr_scratch; p.B = B; p.h = h; p.w = w; p.H = H; p.W = W; p.n_lin = n_lin; p.n_clu = n_clu; p.alpha = alpha;
@@ -765,7 +883,7 @@ extern "C" int stego_eval_crf_unary(const float* code, const float* code_flip, l
                                     int H, int W, const float* lin_weight, const float* lin_bias, int n_lin,
                                     const float* clusters, int n_clu, float alpha, float* lr_scratch, float* unary, float* Q,
                                     void* stream_) {
-  return eval_crf_unary("stego_eval_crf_unary", code, code_flip, ld_code, C, B, h, w, H, W, lin_weight, lin_bias, n_lin,
+  return eval_crf_unary("stego_eval_crf_unary", code, code_flip, 4, ld_code, C, B, h, w, H, W, lin_weight, lin_bias, n_lin,
                         clusters, n_clu, alpha, lr_scratch, unary, Q, EV_PROBE_LIN | EV_PROBE_CLU, nullptr,
                         reinterpret_cast<cudaStream_t>(stream_));
 }
@@ -783,7 +901,65 @@ extern "C" int stego_eval_crf_unary_mosaic(const float* code, const float* code_
   int rc;
   if ((rc = check_mosaic("stego_eval_crf_unary_mosaic", B, H, W, tile0, tile_rows, tiles_per_row, pitch, m)) != STEGO_OK)
     return rc;
-  return eval_crf_unary("stego_eval_crf_unary_mosaic", code, code_flip, ld_code, C, B, h, w, H, W, lin_weight, lin_bias,
+  return eval_crf_unary("stego_eval_crf_unary_mosaic", code, code_flip, 4, ld_code, C, B, h, w, H, W, lin_weight, lin_bias,
                         n_lin, clusters, n_clu, alpha, lr_scratch, unary, Q, probes, &m,
+                        reinterpret_cast<cudaStream_t>(stream_));
+}
+
+// The four entries above with a bf16 code (and code_flip): the backbone's tokens at 384 or 768 channels, read in place
+extern "C" int stego_eval_probes_bf16(const void* code, const void* code_flip, long long ld_code, int C, int B, int h,
+                                      int w, int H, int W, const float* lin_weight, const float* lin_bias, int n_lin,
+                                      const float* clusters, int n_clu, float alpha, float* lr_scratch,
+                                      float* lin_log_probs, float* clu_log_probs, unsigned char* lin_argmax,
+                                      unsigned char* clu_argmax, const void* label, int label_bytes,
+                                      int n_label_classes, long long* lin_confusion, long long* clu_confusion,
+                                      void* stream_) {
+  return eval_probes("stego_eval_probes_bf16", code, code_flip, 2, ld_code, C, B, h, w, H, W, lin_weight, lin_bias,
+                     n_lin, clusters, n_clu, alpha, lr_scratch, lin_log_probs, clu_log_probs, lin_argmax, clu_argmax,
+                     label, label_bytes, n_label_classes, lin_confusion, clu_confusion, nullptr,
+                     reinterpret_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int stego_eval_probes_mosaic_bf16(const void* code, const void* code_flip, long long ld_code, int C, int B,
+                                             int h, int w, int H, int W, const float* lin_weight, const float* lin_bias,
+                                             int n_lin, const float* clusters, int n_clu, float alpha,
+                                             float* lr_scratch, float* lin_log_probs, float* clu_log_probs,
+                                             unsigned char* lin_argmax, unsigned char* clu_argmax, const void* label,
+                                             int label_bytes, int n_label_classes, long long* lin_confusion,
+                                             long long* clu_confusion, int tile0, int tile_rows, int tiles_per_row,
+                                             long long pitch, void* stream_) {
+  EvMosaic m;
+  int rc;
+  if ((rc = check_mosaic("stego_eval_probes_mosaic_bf16", B, H, W, tile0, tile_rows, tiles_per_row, pitch, m)) !=
+      STEGO_OK)
+    return rc;
+  return eval_probes("stego_eval_probes_mosaic_bf16", code, code_flip, 2, ld_code, C, B, h, w, H, W, lin_weight,
+                     lin_bias, n_lin, clusters, n_clu, alpha, lr_scratch, lin_log_probs, clu_log_probs, lin_argmax,
+                     clu_argmax, label, label_bytes, n_label_classes, lin_confusion, clu_confusion, &m,
+                     reinterpret_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int stego_eval_crf_unary_bf16(const void* code, const void* code_flip, long long ld_code, int C, int B, int h,
+                                         int w, int H, int W, const float* lin_weight, const float* lin_bias, int n_lin,
+                                         const float* clusters, int n_clu, float alpha, float* lr_scratch, float* unary,
+                                         float* Q, void* stream_) {
+  return eval_crf_unary("stego_eval_crf_unary_bf16", code, code_flip, 2, ld_code, C, B, h, w, H, W, lin_weight, lin_bias,
+                        n_lin, clusters, n_clu, alpha, lr_scratch, unary, Q, EV_PROBE_LIN | EV_PROBE_CLU, nullptr,
+                        reinterpret_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int stego_eval_crf_unary_mosaic_bf16(const void* code, const void* code_flip, long long ld_code, int C,
+                                                int B, int h, int w, int H, int W, const float* lin_weight,
+                                                const float* lin_bias, int n_lin, const float* clusters, int n_clu,
+                                                float alpha, float* lr_scratch, float* unary, float* Q, int probes,
+                                                int tile0, int tile_rows, int tiles_per_row, long long pitch,
+                                                void* stream_) {
+  EvMosaic m;
+  int rc;
+  if ((rc = check_mosaic("stego_eval_crf_unary_mosaic_bf16", B, H, W, tile0, tile_rows, tiles_per_row, pitch, m)) !=
+      STEGO_OK)
+    return rc;
+  return eval_crf_unary("stego_eval_crf_unary_mosaic_bf16", code, code_flip, 2, ld_code, C, B, h, w, H, W, lin_weight,
+                        lin_bias, n_lin, clusters, n_clu, alpha, lr_scratch, unary, Q, probes, &m,
                         reinterpret_cast<cudaStream_t>(stream_));
 }

@@ -1,6 +1,7 @@
 // Device (and one host) helpers shared by the training probes (probes.cu) and the fused evaluation probes
 // (eval_probes.cu): bilinear source indices and the low-res box a tile of output pixels reads, label reads,
-// centroid normalisation, the warp-per-pixel channel broadcast and the per-CTA confusion histogram.
+// centroid normalisation, the warp-per-pixel channel broadcast, the K-tiled dots of wide codes and the per-CTA
+// confusion histogram.
 #pragma once
 #include "common.cuh"
 
@@ -100,6 +101,54 @@ __device__ __forceinline__ void conf_hist_flush(const ConfHist& hist, unsigned l
     const int probe = i >> 10, pred = (i >> 5) & 31, act = i & 31;
     unsigned long long* dst = probe ? clu_conf : lin_conf;
     if (dst && act < n_cls && pred < (probe ? n_clu : n_lin)) atomicAdd(dst + pred * n_cls + act, (unsigned long long)cnt);
+  }
+}
+
+// ---- wide codes: the backbone's 384 / 768 channels (projection_type None, the DINO baseline) --------------------------
+// A pixel's channels no longer fit the registers of the warp-per-pixel kernels; the dot products run as 32-channel K
+// tiles through shared memory instead, PW_ROWS pixels per CTA of 256 threads.
+constexpr int PW_ROWS = 64, PW_KC = 32, PW_SX = PW_KC + 4;  // sX row stride: 16-byte rows, offset banks
+
+// acc[i] += sum_c xat(r0 + 16 rg + i, c) * table(c, o) for the thread's output column o = tid & 63 and pixel group
+// rg = tid >> 6, sequential fp32 FMAs in channel order; with kSumSq, ss (threads < 64) += sum_c xat(r0 + tid, c)^2.  xat(r, c): channel
+// c of pixel r < rows; table(c, o): the probe table's column o.  C % 32 == 0; sX [PW_ROWS][PW_SX] (16-byte aligned) and
+// sT [PW_KC][64] are the caller's shared memory.
+// sinv[k] = 1 / max(|c_k|, 1e-12) for the centroids clusters [n][C], as normalize_centroids computes the norms (a warp
+// per centroid, 8 warps); the caller synchronises
+__device__ __forceinline__ void centroid_inv_norms(const float* clusters, int n, int C, float* sinv) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  for (int k = warp; k < n; k += 8) {
+    float ss = 0.f;
+    for (int c = lane; c < C; c += 32) { const float v = clusters[1ll * k * C + c]; ss += v * v; }
+    ss = warp_sum(ss);
+    if (lane == 0) sinv[k] = 1.0f / fmaxf(sqrtf(ss), 1e-12f);
+  }
+}
+
+template <bool kSumSq, typename XFn, typename TableFn>
+__device__ __forceinline__ void wide_tile_dots(XFn xat, long long rows, long long r0, int C, TableFn table, float* sX,
+                                               float* sT, float (&acc)[16], float& ss) {
+  const int o = threadIdx.x & 63, rg = threadIdx.x >> 6;
+  for (int c0 = 0; c0 < C; c0 += PW_KC) {
+    __syncthreads();  // the previous K tile has been read
+    for (int i = threadIdx.x; i < PW_ROWS * PW_KC; i += blockDim.x) {
+      const int rr = i / PW_KC, c = i % PW_KC;
+      const long long r = r0 + rr;
+      sX[rr * PW_SX + c] = (r < rows) ? xat(r, c0 + c) : 0.f;
+    }
+    for (int i = threadIdx.x; i < PW_KC * 64; i += blockDim.x) sT[i] = table(c0 + (i >> 6), i & 63);
+    __syncthreads();
+    if (kSumSq && threadIdx.x < PW_ROWS)
+      for (int c = 0; c < PW_KC; ++c) ss = fmaf(sX[threadIdx.x * PW_SX + c], sX[threadIdx.x * PW_SX + c], ss);
+#pragma unroll
+    for (int c = 0; c < PW_KC; c += 4) {
+      const float w0 = sT[c * 64 + o], w1 = sT[(c + 1) * 64 + o], w2 = sT[(c + 2) * 64 + o], w3 = sT[(c + 3) * 64 + o];
+#pragma unroll
+      for (int i = 0; i < 16; ++i) {
+        const float4 v = *reinterpret_cast<const float4*>(&sX[(rg * 16 + i) * PW_SX + c]);
+        acc[i] = fmaf(v.w, w3, fmaf(v.z, w2, fmaf(v.y, w1, fmaf(v.x, w0, acc[i]))));
+      }
+    }
   }
 }
 

@@ -265,6 +265,7 @@ struct LinearCEParams {
   int label_bytes;
   int B, h, w, H, W, n;
   float* dlogits;        // [B*h*w][LP_LD] unnormalised gradient (atomics), or null (loss only)
+  unsigned long long* dfix;  // linear_ce_kernel<true>: the gradient as int64 fixed point (LCE_FIX_SCALE) instead
   double* acc;           // [2]: loss sum, valid count (zeroed before the launch)
   int tiles_y, tiles_x, box_h, box_w;
 };
@@ -278,7 +279,12 @@ constexpr int LCE_TILE = 16;  // hi-res pixels per tile side (256 threads = one 
 //      G[cy][cx][k] = sum_Y wy[Y][cy] T[Y][cx][k], each a conflict-free shared-memory reduction.
 //   3. one global atomic per (box cell, class) of the tile.
 constexpr int LCE_SLD = 33;  // smem stride of one box cell (odd: lanes reading different cells hit different banks)
+// kFixed: the tiles' contributions to a cell are added as int64 multiples of 2^-40 (every contribution is at most the
+// tile's 256 pixel gradients in [-1, 1], far inside the range), and integer adds do not depend on their order: the
+// gradient is the same bit for bit from run to run, where float atomics are not
+constexpr double LCE_FIX_SCALE = 1099511627776.0;  // 2^40
 
+template <bool kFixed>
 __global__ void __launch_bounds__(256)
 linear_ce_kernel(LinearCEParams p) {
   extern __shared__ float sm[];
@@ -422,9 +428,18 @@ linear_ce_kernel(LinearCEParams p) {
       float acc = 0.f;
 #pragma unroll
       for (int yy = 0; yy < LCE_TILE; ++yy) acc = fmaf(swy[yy * bhm + cy], sT[(yy * bwm + cx) * n + k], acc);
-      if (acc != 0.f) atomicAdd(p.dlogits + (base + 1ll * (by0 + cy) * p.w + bx0 + cx) * LP_LD + k, acc);
+      if (acc == 0.f) continue;
+      const long long idx = (base + 1ll * (by0 + cy) * p.w + bx0 + cx) * LP_LD + k;
+      if (kFixed) atomicAdd(p.dfix + idx, static_cast<unsigned long long>(__double2ll_rn(acc * LCE_FIX_SCALE)));
+      else atomicAdd(p.dlogits + idx, acc);
     }
   }
+}
+
+// dlogits[i] = dfix[i] * 2^-40 (linear_ce_kernel<true>'s fixed-point gradient)
+__global__ void fixed_to_float_kernel(const unsigned long long* __restrict__ dfix, float* __restrict__ out, long long n) {
+  for (long long i = 1ll * blockIdx.x * blockDim.x + threadIdx.x; i < n; i += 1ll * gridDim.x * blockDim.x)
+    out[i] = static_cast<float>(static_cast<double>(static_cast<long long>(dfix[i])) * (1.0 / LCE_FIX_SCALE));
 }
 
 // out[0] = loss_sum / count ; out[1] = count
@@ -471,6 +486,195 @@ linear_wgrad_kernel(const float* __restrict__ dlogits, const float* __restrict__
     for (int r = 0; r < LW_ROWS; ++r) acc += sdl[r * 32 + threadIdx.x];
     atomicAdd(db + threadIdx.x, acc * s);
   }
+}
+
+// ---------------------------------------------------------------------------------------------
+// wide codes: the backbone's 384 / 768 channels (projection_type None, the DINO baseline)
+// ---------------------------------------------------------------------------------------------
+// The kernels above keep a pixel's channels in registers (<= 96).  At the backbone's widths the dots run as K tiles
+// (wide_tile_dots), and every reduction over rows (dW, db, d clusters) is one CTA per output tile walking all rows in a
+// fixed order: no atomics, so two identical steps are bit-identical.
+static bool wide_dim(int C) { return C == 384 || C == 768; }
+
+// logits[r][k] = bias[k] + code[r] . W[k]  (k < n <= 32; zeros up to LP_LD), as linear_logits_kernel
+__global__ void __launch_bounds__(256, 2)
+linear_logits_wide_kernel(const float* __restrict__ code, long long ld_code, int C, const float* __restrict__ W,
+                          const float* __restrict__ bias, int n, float* __restrict__ logits, long long rows) {
+  __shared__ __align__(16) float sX[PW_ROWS * PW_SX];
+  __shared__ float sT[PW_KC * 64];
+  const int o = threadIdx.x & 63, rg = threadIdx.x >> 6;
+  for (long long r0 = 1ll * blockIdx.x * PW_ROWS; r0 < rows; r0 += 1ll * gridDim.x * PW_ROWS) {
+    float acc[16], ss = 0.f;
+    const float b0 = (o < n) ? bias[o] : 0.f;
+#pragma unroll
+    for (int i = 0; i < 16; ++i) acc[i] = b0;
+    wide_tile_dots<false>([&](long long r, int c) { return code[r * ld_code + c]; }, rows, r0, C,
+                   [&](int c, int k) { return k < n ? W[1ll * k * C + c] : 0.f; }, sX, sT, acc, ss);
+    if (o < LP_LD) {
+#pragma unroll
+      for (int i = 0; i < 16; ++i) {
+        const long long r = r0 + rg * 16 + i;
+        if (r < rows) logits[r * LP_LD + o] = acc[i];
+      }
+    }
+  }
+}
+
+// ClusterLookup with alpha None on wide rows: ip[r][k] = <x_r / |x_r|, c_k / |c_k|>, assign[r] = first argmax,
+// inv[r] = 1 / max(|x_r|, 1e-12), loss_partials[cta] = sum of the CTA's max ip (the loss is minus their mean)
+__global__ void __launch_bounds__(256, 2)
+cluster_wide_fwd_kernel(const float* __restrict__ x, long long ld, long long rows, int C,
+                        const float* __restrict__ clusters, int n, int* __restrict__ assign, float* __restrict__ inv,
+                        float* __restrict__ loss_partials) {
+  __shared__ __align__(16) float sX[PW_ROWS * PW_SX];
+  __shared__ float sT[PW_KC * 64];
+  __shared__ float sD[PW_ROWS * 65];
+  __shared__ float sinv[64], sss[PW_ROWS], sred[8];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int o = threadIdx.x & 63, rg = threadIdx.x >> 6;
+  centroid_inv_norms(clusters, n, C, sinv);
+  __syncthreads();
+  float loss_acc = 0.f;
+  for (long long r0 = 1ll * blockIdx.x * PW_ROWS; r0 < rows; r0 += 1ll * gridDim.x * PW_ROWS) {
+    float acc[16], ss = 0.f;
+#pragma unroll
+    for (int i = 0; i < 16; ++i) acc[i] = 0.f;
+    wide_tile_dots<true>([&](long long r, int c) { return x[r * ld + c]; }, rows, r0, C,
+                   [&](int c, int k) { return k < n ? clusters[1ll * k * C + c] * sinv[k] : 0.f; }, sX, sT, acc, ss);
+#pragma unroll
+    for (int i = 0; i < 16; ++i) sD[(rg * 16 + i) * 65 + o] = acc[i];
+    if (threadIdx.x < PW_ROWS) sss[threadIdx.x] = ss;
+    __syncthreads();
+    for (int rr = warp; rr < PW_ROWS; rr += 8) {
+      const long long r = r0 + rr;
+      if (r >= rows) break;
+      const float iv = 1.0f / fmaxf(sqrtf(sss[rr]), 1e-12f);
+      const float ip0 = (lane < n) ? sD[rr * 65 + lane] * iv : -INFINITY;
+      const float ip1 = (lane + 32 < n) ? sD[rr * 65 + lane + 32] * iv : -INFINITY;
+      const float best = warp_max(fmaxf(ip0, ip1));
+      const unsigned lo = __ballot_sync(0xffffffffu, ip0 == best), hi = __ballot_sync(0xffffffffu, ip1 == best);
+      const int arg = lo ? __ffs(lo) - 1 : 32 + __ffs(hi) - 1;  // first maximum, like torch.argmax
+      if (lane == 0) {
+        loss_acc += best;
+        assign[r] = arg;
+        inv[r] = iv;
+      }
+    }
+  }
+  if (lane == 0) sred[warp] = loss_acc;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float t = 0.f;
+    for (int w = 0; w < 8; ++w) t += sred[w];
+    loss_partials[blockIdx.x] = t;
+  }
+}
+
+// out[k][c] += s * sum_r coef(r, k) x[r][c] for the CTA's 32 rows k = 32 blockIdx.y + kk (< n) and 4 channels
+// c = 4 blockIdx.x + cc; the CTA with blockIdx.x == C / 4 takes the constant channel 1 instead and adds into
+// out_sum[k].  coef: G[r][k] (row stride 32: the linear probe's dlogits) or, with assign, inv[r] where assign[r] == k (the
+// one-hot gradient of ClusterLookup's alpha None loss).  s = scale / count[0] (0 when count[0] == 0: no valid label, a
+// zero gradient) or, without count, scale.  Rows in a fixed order: thread row group rg takes rows rg, rg + 64, ... of
+// each 256-row tile, and the 64 groups' sums are added in order at the end.  Narrow channel blocks give the
+// C / 4 + 1 CTAs that keep the walk over every row short.
+struct WideWgradParams {
+  const float* x;
+  long long ld, rows;
+  int C, n;
+  const float* G;
+  const int* assign;
+  const float* inv;
+  const float* count;
+  float scale;
+  float* out;      // [n][C]
+  float* out_sum;  // [n] or null
+};
+
+constexpr int PWG_ROWS = 256, PWG_C = 4, PWG_SG = 36;  // rows per tile, channels per CTA, sG row stride
+
+__global__ void __launch_bounds__(256)
+wide_wgrad_kernel(WideWgradParams p) {
+  __shared__ __align__(16) float sG[PWG_ROWS * PWG_SG];
+  __shared__ float sXc[PWG_ROWS * PWG_C];
+  __shared__ float sRed[32 * PWG_C];
+  const int cc = threadIdx.x & (PWG_C - 1), rg = threadIdx.x / PWG_C;  // channel of the CTA's 4, row group of 64
+  const bool ones = blockIdx.x * PWG_C >= p.C;
+  const int k0 = blockIdx.y * 32;
+  float acc[32];
+#pragma unroll
+  for (int k = 0; k < 32; ++k) acc[k] = 0.f;
+  for (long long r0 = 0; r0 < p.rows; r0 += PWG_ROWS) {
+    // the tile's loads are all issued before the first shared store (a load per iteration would wait on each)
+    float gv[PWG_ROWS * 32 / 256], xs[PWG_ROWS * PWG_C / 256];
+#pragma unroll
+    for (int j = 0; j < PWG_ROWS * 32 / 256; ++j) {
+      const int i = threadIdx.x + 256 * j, rr = i >> 5, k = i & 31;
+      const long long r = r0 + rr;
+      gv[j] = 0.f;
+      if (r < p.rows && k0 + k < p.n) {
+        if (p.assign) gv[j] = (p.assign[r] == k0 + k) ? p.inv[r] : 0.f;
+        else gv[j] = p.G[r * LP_LD + k0 + k];
+      }
+    }
+#pragma unroll
+    for (int j = 0; j < PWG_ROWS * PWG_C / 256; ++j) {
+      const int i = threadIdx.x + 256 * j, rr = i / PWG_C, ci = i % PWG_C;
+      const long long r = r0 + rr;
+      xs[j] = 0.f;
+      if (r < p.rows) xs[j] = ones ? (ci == 0 ? 1.f : 0.f) : p.x[r * p.ld + blockIdx.x * PWG_C + ci];
+    }
+    __syncthreads();  // the previous tile has been read
+#pragma unroll
+    for (int j = 0; j < PWG_ROWS * 32 / 256; ++j) {
+      const int i = threadIdx.x + 256 * j;
+      sG[(i >> 5) * PWG_SG + (i & 31)] = gv[j];
+    }
+#pragma unroll
+    for (int j = 0; j < PWG_ROWS * PWG_C / 256; ++j) sXc[threadIdx.x + 256 * j] = xs[j];
+    __syncthreads();
+#pragma unroll
+    for (int j = 0; j < PWG_ROWS / 64; ++j) {
+      const int rr = rg + 64 * j;
+      const float xv = sXc[rr * PWG_C + cc];
+#pragma unroll
+      for (int k = 0; k < 32; k += 4) {
+        const float4 g = *reinterpret_cast<const float4*>(&sG[rr * PWG_SG + k]);
+        acc[k] = fmaf(g.x, xv, acc[k]);
+        acc[k + 1] = fmaf(g.y, xv, acc[k + 1]);
+        acc[k + 2] = fmaf(g.z, xv, acc[k + 2]);
+        acc[k + 3] = fmaf(g.w, xv, acc[k + 3]);
+      }
+    }
+  }
+  for (int g = 0; g < 64; ++g) {  // the row groups' partial sums, in order
+    __syncthreads();
+    if (rg == g)
+#pragma unroll
+      for (int k = 0; k < 32; ++k) sRed[k * PWG_C + cc] = (g == 0) ? acc[k] : sRed[k * PWG_C + cc] + acc[k];
+  }
+  __syncthreads();
+  float s = p.scale;
+  if (p.count) s = p.count[0] > 0.f ? p.scale / p.count[0] : 0.f;
+  if (threadIdx.x < 32 * PWG_C) {
+    const int k = threadIdx.x / PWG_C, ci = threadIdx.x % PWG_C;
+    if (k0 + k < p.n) {
+      if (!ones) p.out[1ll * (k0 + k) * p.C + blockIdx.x * PWG_C + ci] += s * sRed[threadIdx.x];
+      else if (ci == 0 && p.out_sum) p.out_sum[k0 + k] += s * sRed[threadIdx.x];
+    }
+  }
+}
+
+static int launch_wide_wgrad(const WideWgradParams& p, cudaStream_t stream) {
+  const dim3 grid(p.C / PWG_C + (p.out_sum ? 1 : 0), (p.n + 31) / 32);
+  wide_wgrad_kernel<<<grid, 256, 0, stream>>>(p);
+  STEGO_CHECK_LAUNCH("wide_wgrad_kernel");
+  return STEGO_OK;
+}
+
+static unsigned wide_row_grid(long long rows) {
+  const long long tiles = (rows + PW_ROWS - 1) / PW_ROWS;
+  const long long cap = 2ll * num_sms();
+  return (unsigned)(tiles < cap ? tiles : cap);
 }
 
 }  // namespace stego
@@ -565,29 +769,37 @@ extern "C" int stego_cluster_lookup_bwd(const float* x, long long stride_b, long
 //   loss_out[0] = CE mean over valid pixels, loss_out[1] = number of valid pixels
 //   logits_scratch / dlogits_scratch: [B*h*w][32] floats (dlogits zeroed by the caller; null = forward only)
 //   dW / db: accumulated (+=) with grad_loss * d(loss)/d(.)
-extern "C" int stego_linear_probe_ce(const float* code, long long ld_code, int C, const float* W, const float* bias,
-                                     int n_classes, const void* label, int label_bytes, int B, int h, int w, int H,
-                                     int Wimg, float* logits_scratch, float* dlogits_scratch, float* partials_scratch,
-                                     float* loss_out, float grad_loss, float* dW, float* db, void* stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  STEGO_CHECK_ARG(code && W && bias && label && logits_scratch && partials_scratch && loss_out,
-                  "stego_linear_probe_ce: null pointer");
-  STEGO_CHECK_ARG(C > 0 && C <= PR_MAX_DIM && n_classes > 0 && n_classes <= LP_LD,
-                  "stego_linear_probe_ce: C=%d n=%d unsupported", C, n_classes);
-  STEGO_CHECK_ARG(label_bytes == 8 || label_bytes == 4 || label_bytes == 1, "stego_linear_probe_ce: label_bytes=%d (8, 4 or 1)", label_bytes);
-  STEGO_CHECK_ARG(!dlogits_scratch || (dW && db), "stego_linear_probe_ce: backward needs dW and db");
+// The linear probe step of stego_linear_probe_ce (C <= 96; dfix null) and stego_linear_probe_ce_wide (C = 384 / 768;
+// the gradient accumulated in the int64 fixed point of dfix, so that dW / db are the same bit for bit run to run)
+static int linear_probe_ce(const char* who, const float* code, long long ld_code, int C, const float* W,
+                           const float* bias, int n_classes, const void* label, int label_bytes, int B, int h, int w,
+                           int H, int Wimg, float* logits_scratch, float* dlogits_scratch,
+                           unsigned long long* dfix_scratch, float* partials_scratch, float* loss_out, float grad_loss,
+                           float* dW, float* db, cudaStream_t stream) {
+  const bool wide = wide_dim(C);
+  STEGO_CHECK_ARG(code && W && bias && label && logits_scratch && partials_scratch && loss_out, "%s: null pointer", who);
+  STEGO_CHECK_ARG(n_classes > 0 && n_classes <= LP_LD, "%s: C=%d n=%d unsupported (n <= %d)", who, C, n_classes, LP_LD);
+  STEGO_CHECK_ARG(label_bytes == 8 || label_bytes == 4 || label_bytes == 1, "%s: label_bytes=%d (8, 4 or 1)", who,
+                  label_bytes);
+  STEGO_CHECK_ARG(!dlogits_scratch || (dW && db), "%s: backward needs dW and db", who);
+  STEGO_CHECK_ARG(!wide || !dlogits_scratch || dfix_scratch, "%s: the backward needs dfix_scratch", who);
   const long long rows = 1ll * B * h * w;
-  {
+  if (wide) {
+    linear_logits_wide_kernel<<<wide_row_grid(rows), 256, 0, stream>>>(code, ld_code, C, W, bias, n_classes,
+                                                                       logits_scratch, rows);
+    STEGO_CHECK_LAUNCH("linear_logits_wide_kernel");
+  } else {
     long long g = (rows + 7) / 8;
     const long long capg = 16ll * num_sms();
     linear_logits_kernel<<<(unsigned)(g < capg ? g : capg), 256, (size_t)C * 32 * sizeof(float), stream>>>(
         code, ld_code, C, W, bias, n_classes, logits_scratch, rows);
+    STEGO_CHECK_LAUNCH("linear_logits_kernel");
   }
-  STEGO_CHECK_LAUNCH("linear_logits_kernel");
   LinearCEParams p;
   p.logits = logits_scratch; p.label = label; p.label_bytes = label_bytes; p.B = B; p.h = h; p.w = w; p.H = H; p.W = Wimg; p.n = n_classes;
   p.dlogits = dlogits_scratch;
-  STEGO_CHECK_ARG((reinterpret_cast<uintptr_t>(partials_scratch) & 7u) == 0, "stego_linear_probe_ce: scratch not 8-byte aligned");
+  p.dfix = wide ? dfix_scratch : nullptr;
+  STEGO_CHECK_ARG((reinterpret_cast<uintptr_t>(partials_scratch) & 7u) == 0, "%s: scratch not 8-byte aligned", who);
   p.acc = reinterpret_cast<double*>(partials_scratch);
   p.tiles_y = (H + LCE_TILE - 1) / LCE_TILE;
   p.tiles_x = (Wimg + LCE_TILE - 1) / LCE_TILE;
@@ -596,18 +808,29 @@ extern "C" int stego_linear_probe_ce(const float* code, long long ld_code, int C
   const size_t region = std::max((size_t)LCE_TILE * p.box_w * n_classes, (size_t)LCE_TILE * p.box_h * LCE_SLD);
   const size_t ce_smem = ((size_t)p.box_h * p.box_w * LCE_SLD + 256 * (size_t)n_classes + region +
                           (size_t)LCE_TILE * (p.box_w + p.box_h)) * sizeof(float);
-  STEGO_CHECK_ARG(ce_smem <= 200 * 1024, "stego_linear_probe_ce: upsample ratio %dx%d -> %dx%d needs %zu B of smem", h, w, H, Wimg, ce_smem);
-  int rc = opt_in_smem<linear_ce_kernel>(ce_smem, "linear_ce_kernel");
+  STEGO_CHECK_ARG(ce_smem <= 200 * 1024, "%s: upsample ratio %dx%d -> %dx%d needs %zu B of smem", who, h, w, H, Wimg, ce_smem);
+  int rc = wide ? opt_in_smem<linear_ce_kernel<true>>(ce_smem, "linear_ce_kernel")
+                : opt_in_smem<linear_ce_kernel<false>>(ce_smem, "linear_ce_kernel");
   if (rc != STEGO_OK) return rc;
   {
     cudaError_t e = cudaMemsetAsync(partials_scratch, 0, 2 * sizeof(double), stream);
     if (e != cudaSuccess) return cuda_fail(e, "cudaMemsetAsync(linear_ce acc)");
   }
   const int grid = B * p.tiles_y * p.tiles_x;
-  linear_ce_kernel<<<grid, 256, ce_smem, stream>>>(p);
+  if (wide && dlogits_scratch) linear_ce_kernel<true><<<grid, 256, ce_smem, stream>>>(p);
+  else linear_ce_kernel<false><<<grid, 256, ce_smem, stream>>>(p);
   STEGO_CHECK_LAUNCH("linear_ce_kernel");
   linear_ce_finish_kernel<<<1, 1, 0, stream>>>(p.acc, loss_out);
   STEGO_CHECK_LAUNCH("linear_ce_finish_kernel");
+  if (dlogits_scratch && wide) {
+    const long long n = rows * LP_LD;
+    const long long cap = 8ll * num_sms();
+    const long long g = (n + 255) / 256;
+    fixed_to_float_kernel<<<(unsigned)(g < cap ? g : cap), 256, 0, stream>>>(dfix_scratch, dlogits_scratch, n);
+    STEGO_CHECK_LAUNCH("fixed_to_float_kernel");
+    WideWgradParams wg{code, ld_code, rows, C, n_classes, dlogits_scratch, nullptr, nullptr, loss_out + 1, grad_loss, dW, db};
+    return launch_wide_wgrad(wg, stream);
+  }
   if (dlogits_scratch) {
     const unsigned blocks = (unsigned)((rows + LW_ROWS - 1) / LW_ROWS);
     const size_t wsmem = (size_t)(LW_ROWS * 32 + LW_ROWS * C) * sizeof(float);
@@ -616,5 +839,61 @@ extern "C" int stego_linear_probe_ce(const float* code, long long ld_code, int C
                                                         grad_loss, dW, db);
     STEGO_CHECK_LAUNCH("linear_wgrad_kernel");
   }
+  return STEGO_OK;
+}
+
+extern "C" int stego_linear_probe_ce(const float* code, long long ld_code, int C, const float* W, const float* bias,
+                                     int n_classes, const void* label, int label_bytes, int B, int h, int w, int H,
+                                     int Wimg, float* logits_scratch, float* dlogits_scratch, float* partials_scratch,
+                                     float* loss_out, float grad_loss, float* dW, float* db, void* stream_) {
+  STEGO_CHECK_ARG(C > 0 && C <= PR_MAX_DIM && n_classes > 0 && n_classes <= LP_LD,
+                  "stego_linear_probe_ce: C=%d n=%d unsupported", C, n_classes);
+  return linear_probe_ce("stego_linear_probe_ce", code, ld_code, C, W, bias, n_classes, label, label_bytes, B, h, w, H,
+                         Wimg, logits_scratch, dlogits_scratch, nullptr, partials_scratch, loss_out, grad_loss, dW, db,
+                         reinterpret_cast<cudaStream_t>(stream_));
+}
+
+// stego_linear_probe_ce for a wide code (C = 384 / 768: projection_type None); dfix_scratch: int64 [B*h*w][32], zeroed by
+// the caller, needed with dlogits_scratch.  Every reduction has a fixed order or is exact: bit-identical run to run.
+extern "C" int stego_linear_probe_ce_wide(const float* code, long long ld_code, int C, const float* W, const float* bias,
+                                          int n_classes, const void* label, int label_bytes, int B, int h, int w, int H,
+                                          int Wimg, float* logits_scratch, float* dlogits_scratch, long long* dfix_scratch,
+                                          float* partials_scratch, float* loss_out, float grad_loss, float* dW, float* db,
+                                          void* stream_) {
+  STEGO_CHECK_ARG(wide_dim(C), "stego_linear_probe_ce_wide: C=%d unsupported (384 or 768)", C);
+  return linear_probe_ce("stego_linear_probe_ce_wide", code, ld_code, C, W, bias, n_classes, label, label_bytes, B, h, w,
+                         H, Wimg, logits_scratch, dlogits_scratch, reinterpret_cast<unsigned long long*>(dfix_scratch),
+                         partials_scratch, loss_out, grad_loss, dW, db, reinterpret_cast<cudaStream_t>(stream_));
+}
+
+// ClusterLookup's alpha None loss (the training step's cluster probe, train_segmentation.py:221-223) and, optionally,
+// its gradient in one call for a wide code (C = 384 or 768: projection_type None).  x [rows][ld_x] fp32 tokens-major;
+// clusters [n][C], n <= 64.  loss_out[0] = -mean_r max_k <x_r / |x_r|, c_k / |c_k|>.  Scratch: assign_scratch int32 and
+// inv_scratch fp32, [rows] each; partials_scratch: 16 * SMs floats.  With dclusters: dclusters [n][C] += d loss_out[0] /
+// d clusters, through dnc_scratch [n][C] (zeroed by the caller).  Deterministic: no atomics.
+extern "C" int stego_cluster_lookup_wide(const float* x, long long ld_x, long long rows, int C, const float* clusters,
+                                         int n_classes, int* assign_scratch, float* inv_scratch,
+                                         float* partials_scratch, float* loss_out, float* dnc_scratch,
+                                         float* dclusters, void* stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  STEGO_CHECK_ARG(x && clusters && assign_scratch && inv_scratch && partials_scratch && loss_out && rows > 0,
+                  "stego_cluster_lookup_wide: bad args");
+  STEGO_CHECK_ARG(wide_dim(C) && ld_x >= C, "stego_cluster_lookup_wide: C=%d (384 or 768), ld_x=%lld", C, ld_x);
+  STEGO_CHECK_ARG(n_classes > 0 && n_classes <= PR_MAX_CLASSES, "stego_cluster_lookup_wide: n_classes %d unsupported (<= %d)",
+                  n_classes, PR_MAX_CLASSES);
+  STEGO_CHECK_ARG(!dclusters || dnc_scratch, "stego_cluster_lookup_wide: the gradient needs dnc_scratch");
+  const unsigned grid = wide_row_grid(rows);
+  cluster_wide_fwd_kernel<<<grid, 256, 0, stream>>>(x, ld_x, rows, C, clusters, n_classes, assign_scratch, inv_scratch,
+                                                    partials_scratch);
+  STEGO_CHECK_LAUNCH("cluster_wide_fwd_kernel");
+  sum_partials_kernel<<<1, 256, 0, stream>>>(partials_scratch, (int)grid, (float)(-1.0 / (double)rows), loss_out);
+  STEGO_CHECK_LAUNCH("sum_partials_kernel");
+  if (!dclusters) return STEGO_OK;
+  WideWgradParams g{x, ld_x, rows, C, n_classes, nullptr, assign_scratch, inv_scratch, nullptr,
+                    (float)(-1.0 / (double)rows), dnc_scratch, nullptr};
+  int rc;
+  if ((rc = launch_wide_wgrad(g, stream)) != STEGO_OK) return rc;
+  cluster_norm_bwd_kernel<<<n_classes, 32, 0, stream>>>(clusters, dnc_scratch, dclusters, n_classes, C);
+  STEGO_CHECK_LAUNCH("cluster_norm_bwd_kernel");
   return STEGO_OK;
 }

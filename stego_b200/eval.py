@@ -27,7 +27,8 @@ def fused_probe_log_probs(code: torch.Tensor, linear_probe: torch.nn.Module, clu
                           want_argmax: bool = False, code_flipped: Optional[torch.Tensor] = None,
                           label: Optional[torch.Tensor] = None, linear_confusion: Optional[torch.Tensor] = None,
                           cluster_confusion: Optional[torch.Tensor] = None):
-    """code: low-res [B, C, h, w] (any strides, CUDA).  Returns (linear_log_probs, cluster_log_probs) [B,n,H,W]
+    """code: low-res [B, C, h, w] (any strides, CUDA; C <= 96, or 384 / 768 for projection_type None, where a bf16
+    tokens-major code is read in place).  Returns (linear_log_probs, cluster_log_probs) [B,n,H,W]
     fp32, and with want_argmax also (linear_argmax, cluster_argmax) uint8 [B,H,W].
 
     code_flipped: the code of `img.flip(dims=[3])` — the kernel then evaluates the flip-TTA average
@@ -41,7 +42,7 @@ def fused_probe_log_probs(code: torch.Tensor, linear_probe: torch.nn.Module, clu
     H, W = int(size[0]), int(size[1])
     if code_flipped is not None:
         assert code_flipped.shape == code.shape
-    x, xf, ld = _probe_codes(code, code_flipped)
+    x, xf, ld, bf16 = _eval_codes(code, code_flipped)
     wl, bl, cl = _probe_tables(linear_probe, cluster_probe, C)
     n_lin, n_clu = wl.shape[0], cl.shape[0]
     dev = code.device
@@ -60,14 +61,25 @@ def fused_probe_log_probs(code: torch.Tensor, linear_probe: torch.nn.Module, clu
                 assert t.dtype == torch.int64 and t.is_contiguous() and tuple(t.shape) == (n, n_cls)
         if linear_confusion is None and cluster_confusion is None:
             raise ValueError("label given without a confusion matrix to accumulate into")
-    rc = _lib.load().stego_eval_probes(_lib.ptr(x), _lib.ptr(xf), ld, C, B, h, w, H, W, _lib.ptr(wl), _lib.ptr(bl), n_lin,
+    entry = _lib.load().stego_eval_probes_bf16 if bf16 else _lib.load().stego_eval_probes
+    rc = entry(_lib.ptr(x), _lib.ptr(xf), ld, C, B, h, w, H, W, _lib.ptr(wl), _lib.ptr(bl), n_lin,
                                        _lib.ptr(cl), n_clu, float(alpha), _lib.ptr(scratch), _lib.ptr(lin), _lib.ptr(clu),
                                        _lib.ptr(la), _lib.ptr(ca), _lib.ptr(lab), lab_bytes, n_cls,
                                        _lib.ptr(linear_confusion), _lib.ptr(cluster_confusion), _lib.stream())
-    _lib.check(rc, "stego_eval_probes")
+    _lib.check(rc, "stego_eval_probes_bf16" if bf16 else "stego_eval_probes")
     if want_argmax:
         return lin, clu, la, ca
     return lin, clu
+
+
+# the code widths of projection_type None (the backbone's own features): the probe kernels also read them in bf16
+WIDE_DIMS = (384, 768)
+
+
+def _tokens_major_bf16(t: torch.Tensor) -> bool:
+    B, _, h, w = t.shape
+    return (t.dtype == torch.bfloat16 and t.stride(1) == 1 and t.stride(2) == w * t.stride(3)
+            and (B == 1 or t.stride(0) == h * w * t.stride(3)))
 
 
 def _probe_codes(code: torch.Tensor, code_flipped: Optional[torch.Tensor]):
@@ -82,6 +94,15 @@ def _probe_codes(code: torch.Tensor, code_flipped: Optional[torch.Tensor]):
             x = x.permute(0, 2, 3, 1).contiguous().permute(0, 3, 1, 2)
             ld = x.stride(3)
     return x, xf, ld
+
+
+def _eval_codes(code: torch.Tensor, code_flipped: Optional[torch.Tensor]):
+    """(x, xf, ld, bf16): _probe_codes, except that bf16 tokens-major views of 384 / 768 channels with one row stride
+    (the backbone's tokens) stay bf16 (bf16 = True), read in place by the probe kernels."""
+    if (code.shape[1] in WIDE_DIMS and _tokens_major_bf16(code) and
+            (code_flipped is None or (_tokens_major_bf16(code_flipped) and code_flipped.stride(3) == code.stride(3)))):
+        return code.detach(), None if code_flipped is None else code_flipped.detach(), code.stride(3), True
+    return (*_probe_codes(code, code_flipped), False)
 
 
 def _probe_tables(linear_probe: torch.nn.Module, cluster_probe: torch.nn.Module, C: int):
@@ -110,8 +131,9 @@ def _check_crf_args(code, linear_probe, cluster_probe, img, code_flipped, label,
     B, C, h, w = code.shape
     H, W = int(img.shape[2]), int(img.shape[3])
     n_lin, n_clu = int(linear_probe.weight.shape[0]), int(cluster_probe.clusters.shape[0])
-    if not (0 < C <= 96 and 0 < n_lin <= 32 and 0 < n_clu <= 32):
-        raise ValueError(f"fused_eval_crf: C={C}, n_lin={n_lin}, n_clu={n_clu} unsupported (C <= 96, classes <= 32)")
+    if not ((0 < C <= 96 or C in WIDE_DIMS) and 0 < n_lin <= 32 and 0 < n_clu <= 32):
+        raise ValueError(f"fused_eval_crf: C={C}, n_lin={n_lin}, n_clu={n_clu} unsupported (C <= 96 or 384 / 768, "
+                         f"classes <= 32)")
     if linear_probe.weight[0].numel() != C or cluster_probe.clusters.shape[1] != C:
         raise ValueError(f"fused_eval_crf: probes of {linear_probe.weight[0].numel()} / {cluster_probe.clusters.shape[1]} "
                          f"channels for a code of {C}")
@@ -151,7 +173,8 @@ def fused_eval_crf(code: torch.Tensor, linear_probe: torch.nn.Module, cluster_pr
         clu_pred = stack([dense_crf(img[b], cluster_probs[b]) for b]).argmax(1)
         linear_metrics.update(lin_pred, label); cluster_metrics.update(clu_pred, label)
 
-    code: low-res [B, C, h, w] (C <= 96, any strides); img: the normalised frames [B, 3, H, W]; both CUDA.  Returns
+    code: low-res [B, C, h, w] (C <= 96 or 384 / 768, any strides; a bf16 tokens-major code of 384 / 768 channels is
+    read in place); img: the normalised frames [B, 3, H, W]; both CUDA.  Returns
     (lin_pred, clu_pred) uint8 [B, H, W], the argmax of each probe's CRF marginals (lowest index on ties), and with
     want_marginals also (lin_Q [B, n_lin, H, W], clu_Q [B, n_clu, H, W]) fp32.  label [B, H, W] (uint8 with 255 =
     ignore, int32 or int64; the spatial size of img) with int64 `linear_confusion [n_lin, n_lin]` /
@@ -169,14 +192,15 @@ def fused_eval_crf(code: torch.Tensor, linear_probe: torch.nn.Module, cluster_pr
     lib = _lib.load()
     dev = code.device
     N = H * W
-    x, xf, ld = _probe_codes(code, code_flipped)
+    x, xf, ld, bf16 = _eval_codes(code, code_flipped)
     wl, bl, cl = _probe_tables(linear_probe, cluster_probe, C)
     scratch = torch.empty(B * h * w, 80, dtype=torch.float32, device=dev)  # eval_probes.cu EV_LD
     unary = torch.empty(B * N, _CRF_LD, dtype=torch.float32, device=dev)
     Q = torch.empty(B * N, _CRF_LD, dtype=torch.float32, device=dev)
-    _lib.check(lib.stego_eval_crf_unary(_lib.ptr(x), _lib.ptr(xf), ld, C, B, h, w, H, W, _lib.ptr(wl), _lib.ptr(bl), n_lin,
-                                        _lib.ptr(cl), n_clu, float(alpha), _lib.ptr(scratch), _lib.ptr(unary), _lib.ptr(Q),
-                                        _lib.stream()), "stego_eval_crf_unary")
+    name = "stego_eval_crf_unary_bf16" if bf16 else "stego_eval_crf_unary"
+    _lib.check(getattr(lib, name)(_lib.ptr(x), _lib.ptr(xf), ld, C, B, h, w, H, W, _lib.ptr(wl), _lib.ptr(bl), n_lin,
+                                  _lib.ptr(cl), n_clu, float(alpha), _lib.ptr(scratch), _lib.ptr(unary), _lib.ptr(Q),
+                                  _lib.stream()), name)
     lg = crf._position_lattice(H, W, dev)
     lb = crf._bilateral_lattice(crf.prepare_image(frame) for frame in img.detach())
     val_g = torch.empty(2, B * lg.M, _CRF_LD, dtype=torch.float32, device=dev)

@@ -324,6 +324,14 @@ class DinoFeaturizer(nn.Module):
         store = _HeadFn.apply(feat_tok.reshape(B * hw, E), m1, m2, B, hw, *self.head_params())
         return store.view(B, fh, fw, -1)[..., :self.dim].permute(0, 3, 1, 2)
 
+    def eval_code(self, feat_tok: torch.Tensor, fh: int, fw: int) -> torch.Tensor:
+        """The eval-mode code [B, C, h, w] of tokens-major features: the head's, or with projection_type None the
+        features themselves (modules.py:108-113), as a bf16 view of feat_tok that the probe kernels read in place."""
+        if self.proj_type is not None:
+            return self.head_code(feat_tok, None, None, fh, fw)
+        B, _, E = feat_tok.shape
+        return feat_tok.view(B, fh, fw, E).permute(0, 3, 1, 2)
+
     # ---- reference entry point -------------------------------------------------------------------
     def forward(self, img, n=1, return_class_feat=False):
         self.model.eval()
@@ -472,6 +480,38 @@ class _ClusterLookupFn(torch.autograd.Function):
         g = (g_loss if g_loss is not None else torch.zeros((), device=xf.device)).to(torch.float32).reshape(1).contiguous()
         cluster_lookup_backward(xf, cl, ctx.alpha, g, dnc, dcl)
         return None, dcl.reshape(ctx.shape), None, None, None
+
+
+class _ClusterLookupWideFn(torch.autograd.Function):
+    """ClusterLookup's alpha None loss (the training step's cluster probe) on a wide code: the backbone's 384 / 768
+    channels of projection_type None.  Loss and gradient come from one call of stego_cluster_lookup_wide (fixed-order
+    reductions); backward scales the gradient by the upstream one."""
+
+    @staticmethod
+    def forward(ctx, x, clusters):
+        B, C, H, W = x.shape
+        n = clusters.shape[0]
+        dev = x.device
+        xt = ops.tokens_major(x)
+        rows = B * H * W
+        cl = clusters.detach().float().contiguous()
+        loss = torch.empty(2, dtype=torch.float32, device=dev)
+        dnc = torch.zeros(n, C, dtype=torch.float32, device=dev)
+        dcl = torch.zeros(n, C, dtype=torch.float32, device=dev)
+        assign = torch.empty(rows, dtype=torch.int32, device=dev)
+        inv = torch.empty(rows, dtype=torch.float32, device=dev)
+        _lib.check(_lib.load().stego_cluster_lookup_wide(
+            _lib.ptr(xt), xt.stride(3), rows, C, _lib.ptr(cl), n, _lib.ptr(assign), _lib.ptr(inv),
+            _lib.ptr(ops.probe_scratch(dev)), _lib.ptr(loss), _lib.ptr(dnc), _lib.ptr(dcl), _lib.stream()),
+            "stego_cluster_lookup_wide")
+        ctx.save_for_backward(dcl)
+        ctx.shape = clusters.shape
+        return loss[0]
+
+    @staticmethod
+    def backward(ctx, g):
+        (dcl,) = ctx.saved_tensors
+        return None, (dcl * g).reshape(ctx.shape)
 
 
 class ClusterLookup(nn.Module):

@@ -28,7 +28,7 @@ import torch.nn.functional as F
 
 from . import _lib, corr, ops
 from .modules import ClusterLookup, ContrastiveCorrelationLoss, ContrastiveCRFLoss, DinoFeaturizer, \
-    FeaturePyramidNet, _ClusterLookupFn, norm, pixel_cosine, sample
+    FeaturePyramidNet, _ClusterLookupFn, _ClusterLookupWideFn, norm, pixel_cosine, sample
 
 
 # --------------------------------------------------------------------------------------------------
@@ -207,7 +207,16 @@ def linear_probe_ce_step(x, weight, bias, label, logits, dlogits, partials, loss
     += grad_scale * gradient.  dlogits, dW and db are accumulated into and must arrive zeroed."""
     B, C, h, w = x.shape
     H, W = label.shape[-2], label.shape[-1]
-    _lib.check(_lib.load().stego_linear_probe_ce(
+    lib = _lib.load()
+    if C > 96:  # the backbone's width (projection_type None): exact fixed-point logit gradient, bit-reproducible dW / db
+        dfix = torch.zeros(B * h * w, 32, dtype=torch.int64, device=x.device) if dlogits is not None else None
+        _lib.check(lib.stego_linear_probe_ce_wide(
+            _lib.ptr(x), x.stride(3), C, _lib.ptr(weight), _lib.ptr(bias), weight.shape[0], _lib.ptr(label),
+            ops.LABEL_BYTES[label.dtype], B, h, w, H, W, _lib.ptr(logits), _lib.ptr(dlogits), _lib.ptr(dfix),
+            _lib.ptr(partials), _lib.ptr(loss), grad_scale, _lib.ptr(dW), _lib.ptr(db), _lib.stream()),
+            "stego_linear_probe_ce_wide")
+        return
+    _lib.check(lib.stego_linear_probe_ce(
         _lib.ptr(x), x.stride(3), C, _lib.ptr(weight), _lib.ptr(bias), weight.shape[0], _lib.ptr(label),
         ops.LABEL_BYTES[label.dtype], B, h, w, H, W, _lib.ptr(logits), _lib.ptr(dlogits), _lib.ptr(partials),
         _lib.ptr(loss), grad_scale, _lib.ptr(dW), _lib.ptr(db), _lib.stream()), "stego_linear_probe_ce")
@@ -221,8 +230,9 @@ class _LinearProbeCEFn(torch.autograd.Function):
         B, C, h, w = code_nchw.shape
         n = weight.shape[0]
         dev = code_nchw.device
-        if n > 32 or C > 96:
-            raise RuntimeError(f"stego_b200 linear probe: n_classes={n} (<=32) / dim={C} (<=96) unsupported")
+        if n > 32 or not (C <= 96 or C in (384, 768)):
+            raise RuntimeError(f"stego_b200 linear probe: n_classes={n} (<=32) / dim={C} (<=96, or 384 / 768) "
+                               f"unsupported")
         rows = B * h * w
         lab, _ = ops.probe_label(label, B, label.shape[-2], label.shape[-1])
         logits = torch.empty(rows, 32, dtype=torch.float32, device=dev)
@@ -257,9 +267,14 @@ class LitUnsupervisedSegmenter(nn.Module):
     def __init__(self, n_classes, cfg):
         dim = cfg.dim if cfg.continuous else n_classes
         # the limits of the probe and correspondence-loss kernels, checked before anything is drawn or built, so that an
-        # unsupported configuration fails here rather than part-way through its first training step
-        if not 1 <= dim <= 96:
-            raise RuntimeError(f"stego_b200: code dim {dim} unsupported (1..96)")
+        # unsupported configuration fails here rather than part-way through its first training step.  The one wider
+        # code is the DINO baseline's: projection_type None, where the code is the backbone's features
+        # (modules.py:108-113) and dim their width
+        n_feats = 384 if cfg.model_type == "vit_small" else 768
+        baseline = cfg.arch == "dino" and cfg.projection_type is None and cfg.continuous and dim == n_feats
+        if not (1 <= dim <= 96 or baseline):
+            raise RuntimeError(f"stego_b200: code dim {dim} unsupported (1..96, or the backbone's {n_feats} with "
+                               f"projection_type None)")
         if not 1 <= n_classes <= 32:
             raise RuntimeError(f"stego_b200: n_classes={n_classes} unsupported by the linear probe (1..32)")
         if not 0 <= cfg.extra_clusters <= 64 - n_classes:
@@ -432,7 +447,14 @@ class LitUnsupervisedSegmenter(nn.Module):
 
         With cfg.aug_alignment_weight > 0 the batch carries either the views batch["img_aug"] / batch["coord_aug"]
         (the autograd path, with them) or batch["seed"]: B ints, a list or a CPU tensor, from which the step builds
-        the views itself (augment.aug_alignment_views at cfg.res, from the fp32 batch["img"])."""
+        the views itself (augment.aug_alignment_views at cfg.res, from the fp32 batch["img"]).
+
+        projection_type None (the DINO baseline, dim = the backbone's width, correspondence_weight 0) trains the probes
+        alone on the autograd path: the backbone on img, its features as the code, the wide probe kernels, Adam."""
+        if self.net.proj_type is None:
+            self._check_baseline_step()
+            self._deliver_histograms()
+            return self._training_step_autograd(batch, batch_idx)
         self._deliver_histograms()
         if getattr(self.cfg, "fused_step", True):
             if self._fused is None:
@@ -441,6 +463,22 @@ class LitUnsupervisedSegmenter(nn.Module):
             if self._fused.supported(batch):
                 return self._fused.run(batch)
         return self._training_step_autograd(batch, batch_idx)
+
+    def _check_baseline_step(self) -> None:
+        """The DINO baseline's step (projection_type None): the probes on the backbone's features, dim its width, with
+        no term that needs a code-side gradient or a code-side kernel beyond 96 channels.  Checked before anything is
+        enqueued."""
+        cfg, net = self.cfg, self.net
+        if net.dim != net.n_feats:
+            raise ValueError(f"stego_b200: projection_type None makes the code the backbone's {net.n_feats} channels, "
+                             f"but dim is {net.dim}: the reference cannot run this configuration")
+        if cfg.correspondence_weight > 0:
+            raise ValueError("stego_b200: projection_type None trains the probes alone; correspondence_weight > 0 has "
+                             "no parameter to train (set it to 0, as the DINO baseline does)")
+        for name in ("rec_weight", "aug_alignment_weight", "crf_weight"):
+            if getattr(cfg, name) > 0:
+                raise ValueError(f"stego_b200: {name} > 0 with projection_type None is unsupported (its kernels take "
+                                 f"codes of at most 96 channels)")
 
     def _training_step_autograd(self, batch, batch_idx):
         cfg = self.cfg
@@ -472,7 +510,10 @@ class LitUnsupervisedSegmenter(nn.Module):
             M1, M2 = cat(m1, p1), cat(m2, p2)
         else:
             M1, M2, p3 = m1, m2, None
-        code_all = net.head_code(tok_all, M1, M2, fh, fw)  # [2B, dim, h, w]
+        if net.proj_type is None:  # the DINO baseline: the code is the features (modules.py:108-113)
+            code_all = tok_all.float().view(-1, fh, fw, tok_all.shape[-1]).permute(0, 3, 1, 2)
+        else:
+            code_all = net.head_code(tok_all, M1, M2, fh, fw)  # [2B, dim, h, w]
         code = code_all[:B]
         E = tok_all.shape[-1]
         feats = tok_all[:B].view(B, fh, fw, E).permute(0, 3, 1, 2)  # NCHW view, bf16, channel stride 1
@@ -549,7 +590,10 @@ class LitUnsupervisedSegmenter(nn.Module):
         linear_loss = linear_probe_ce(detached_code, self.linear_probe.weight, self.linear_probe.bias, label)
         loss = loss + linear_loss
         self.log('loss/linear', linear_loss)
-        cluster_loss, _, _ = _ClusterLookupFn.apply(detached_code, self.cluster_probe.clusters, None, False, False)
+        if net.dim > 96:
+            cluster_loss = _ClusterLookupWideFn.apply(detached_code, self.cluster_probe.clusters)
+        else:
+            cluster_loss, _, _ = _ClusterLookupFn.apply(detached_code, self.cluster_probe.clusters, None, False, False)
         loss = loss + cluster_loss
         self.log('loss/cluster', cluster_loss)
         self.log('loss/total', loss)
@@ -650,8 +694,10 @@ class LitUnsupervisedSegmenter(nn.Module):
         linear_probs / cluster_probs fp32 [B, n, H', W']: the log-probabilities without CRF, the CRF marginals with it.
         Like validation_step it waits for the previous step's parameter update, draws no random numbers, leaves the
         training step's workspace, graphs and parameters alone and restores the net's train / eval modes on exit.
-        Configurations the fused eval kernels do not take (proj_type None: a code of E > 96 channels; more than 32
-        cluster-probe rows) and CPU tensors are refused before anything is enqueued."""
+        With projection_type None (the DINO baseline, dim = the backbone's width) the code is the mirrored bf16 tokens
+        themselves, read in place by the probe kernels.  Configurations the fused eval kernels do not take
+        (projection_type None with another dim; more than 32 cluster-probe rows) and CPU tensors are refused before
+        anything is enqueued."""
         from .eval import fused_eval_crf, fused_probe_log_probs
         img, label = batch["img"], batch.get("label")
         self._check_eval_args(img, label, run_crf)
@@ -662,7 +708,7 @@ class LitUnsupervisedSegmenter(nn.Module):
             if label is not None else {}
         with self._net_in_eval_mode(), torch.no_grad():
             tok = net.backbone_tokens(img, use_graph=getattr(self.cfg, "cuda_graph", True), mirror=True)  # [2B, hw, E]
-            code_all = net.head_code(tok, None, None, fh, fw)  # [2B, dim, h, w]
+            code_all = net.eval_code(tok, fh, fw)  # [2B, dim, h, w]
             code, code_flipped = code_all[:B], code_all[B:]
             if run_crf:
                 out = fused_eval_crf(code, self.linear_probe, self.cluster_probe, img, 2.0, code_flipped=code_flipped,
@@ -711,7 +757,7 @@ class LitUnsupervisedSegmenter(nn.Module):
         tensors), and the mean field's value buffers are checked against the free device memory before it is
         enqueued (RuntimeError naming the sizes)."""
         from . import crf
-        from .eval import _probe_codes, _probe_tables
+        from .eval import _eval_codes, _probe_tables
         R, C, n_tiles, H, W, probes = self._check_scene_args(tiles, grid, label, run_crf, probes, map_clusters, chunk)
         self.flush()
         tiles = tiles.detach().contiguous()
@@ -742,21 +788,22 @@ class LitUnsupervisedSegmenter(nn.Module):
                 img = tiles[t0:t0 + chunk]
                 B = img.shape[0]
                 tok = net.backbone_tokens(img, use_graph=getattr(self.cfg, "cuda_graph", True), mirror=True)
-                code_all = net.head_code(tok, None, None, h, w)  # [2B, dim, h, w]
-                x, xf, ld = _probe_codes(code_all[:B], code_all[B:])
+                code_all = net.eval_code(tok, h, w)  # [2B, dim, h, w]
+                x, xf, ld, bf16 = _eval_codes(code_all[:B], code_all[B:])
+                sfx = "_bf16" if bf16 else ""
                 if run_crf:
-                    _lib.check(lib.stego_eval_crf_unary_mosaic(
+                    _lib.check(getattr(lib, "stego_eval_crf_unary_mosaic" + sfx)(
                         _lib.ptr(x), _lib.ptr(xf), ld, net.dim, B, h, w, H, W, _lib.ptr(wl), _lib.ptr(bl), n_lin,
                         _lib.ptr(cl), n_clu, 2.0, _lib.ptr(scratch), _lib.ptr(unary), _lib.ptr(Q), int(lin_on) + 2 * int(clu_on), t0, R, C, WW,
-                        _lib.stream()), "stego_eval_crf_unary_mosaic")
+                        _lib.stream()), "stego_eval_crf_unary_mosaic" + sfx)
                 else:
-                    _lib.check(lib.stego_eval_probes_mosaic(
+                    _lib.check(getattr(lib, "stego_eval_probes_mosaic" + sfx)(
                         _lib.ptr(x), _lib.ptr(xf), ld, net.dim, B, h, w, H, W, _lib.ptr(wl), _lib.ptr(bl), n_lin,
                         _lib.ptr(cl), n_clu, 2.0, _lib.ptr(scratch), _lib.ptr(probs.get("linear")),
                         _lib.ptr(probs.get("cluster")), _lib.ptr(preds.get("linear")), _lib.ptr(preds.get("cluster")),
                         _lib.ptr(lab[t0:] if lab is not None else None), lab_bytes, n_lin if lab is not None else 0,
                         _lib.ptr(lin_stats), _lib.ptr(clu_stats), t0, R, C, WW, _lib.stream()),
-                        "stego_eval_probes_mosaic")
+                        "stego_eval_probes_mosaic" + sfx)
         if run_crf:
             image = crf.prepare_image(tiles.view(R, C, 3, H, W).permute(2, 0, 3, 1, 4).reshape(3, HH, WW))
             lg = crf._position_lattice(HH, WW, dev, cache=n_tiles == 1)
@@ -843,9 +890,9 @@ class LitUnsupervisedSegmenter(nn.Module):
         if p not in (8, 16) or H % p or W % p or W % 8:
             raise ValueError(f"{who}: a {H}x{W} frame is not whole {p}x{p} patches with W a multiple of 8 "
                              f"(patch 8 or 16)")
-        if net.proj_type is None:
-            raise ValueError(f"{who}: projection_type None gives a code of {net.n_feats} channels; the fused "
-                             f"evaluation probes take at most 96")
+        if net.proj_type is None and net.dim != net.n_feats:
+            raise ValueError(f"{who}: projection_type None gives a code of {net.n_feats} channels, and the probes were "
+                             f"built for dim={net.dim}: the DINO baseline needs dim={net.n_feats}")
         n_lin, n_clu = self.linear_probe.weight.shape[0], self.cluster_probe.clusters.shape[0]
         if n_lin > 32 or n_clu > 32:
             raise ValueError(f"{who}: {n_lin} linear-probe classes / {n_clu} cluster-probe rows unsupported by the "
