@@ -435,6 +435,17 @@ STEGO_API int stego_eval_probes_mosaic(const float* code, const float* code_flip
  * ---------------------------------------------------------------------------------------------- */
 STEGO_API int stego_knn_topk(const float* feats, int n, int E, int k, void* planes_scratch, long long* idx_out,
                              float* val_out, void* stream);
+/* The two stages of stego_knn_topk, for a search split over row ranges (e.g. one range per device of a node).
+ * stego_knn_prep: feats fp32 [n][E] -> the L2-normalised bf16 hi / lo planes [2][n][E] (16-byte aligned) that
+ * stego_knn_topk builds in its planes_scratch.
+ * stego_knn_topk_rows: the search of query rows [row0, row0 + nrows) only, over the prepared planes of ALL n descriptors,
+ * against every key tile in stego_knn_topk's order.  row0 must be a multiple of 128 (the query row block),
+ * 1 <= nrows, row0 + nrows <= n.  idx_out / val_out: [nrows][k], row r holding query row row0 + r; the self-first rule
+ * uses the absolute row index.  A row's result depends only on that row and the fixed key-tile order, so the
+ * concatenation of any split into such ranges is bit-identical to stego_knn_topk. */
+STEGO_API int stego_knn_prep(const float* feats, int n, int E, void* planes, void* stream);
+STEGO_API int stego_knn_topk_rows(const void* planes, int n, int E, int k, int row0, int nrows, long long* idx_out,
+                                  float* val_out, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Dense CRF post-processing (BASELINE.json configs[4]; src/crf.py:22-45 -> pydensecrf, third-party, parity UNPINNED:

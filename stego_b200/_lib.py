@@ -9,6 +9,7 @@ import ctypes
 import gc
 import os
 import re
+import threading
 from typing import Dict, List, Tuple
 
 import torch
@@ -84,11 +85,36 @@ def launch_count() -> int:
     return int(load().stego_launch_count()) + replayed_launches
 
 
+# One capture at a time in the process: a capture turns the garbage collector off process-wide (below), and a capture in
+# torch's global error mode is invalidated by another thread's unsafe calls.  The multi-device paths capture from the
+# calling thread, one device after another; nn.DataParallel replicas never capture (their forwards run eagerly).
+_CAPTURE_LOCK = threading.Lock()
+
+
+# One side stream per device to capture on.  torch.cuda.graph's default capture stream is one stream for the whole
+# process, made on whichever device was current at the first capture, and entering it switches the current device to
+# that one: a graph captured for another device would record its kernels in the first device's context.
+_CAPTURE_STREAMS: Dict[int, torch.cuda.Stream] = {}
+
+
+def capture_stream(device: torch.device) -> torch.cuda.Stream:
+    """The side stream captures on `device` use (made on first use; callers hold _CAPTURE_LOCK)."""
+    if device.index not in _CAPTURE_STREAMS:
+        _CAPTURE_STREAMS[device.index] = torch.cuda.Stream(device=device)
+    return _CAPTURE_STREAMS[device.index]
+
+
 class Graph:
-    """`fn()` captured as one CUDA graph on the current stream, with its result; `replay` counts the graph's launches
-    of this library in replayed_launches (stego_launch_count does not see them)."""
+    """`fn()` captured as one CUDA graph on the current device (on that device's capture stream, ordered after its current
+    stream), with its result; `replay` launches it on that device's current stream and counts the graph's launches of
+    this library in replayed_launches (stego_launch_count does not see them)."""
 
     def __init__(self, fn):
+        self.device = torch.device("cuda", torch.cuda.current_device())
+        with _CAPTURE_LOCK, torch.cuda.device(self.device):
+            self._capture(fn)
+
+    def _capture(self, fn):
         torch.cuda.synchronize()
         # A dead graph in a reference cycle (a model's graphs hold closures over the model) is destroyed by whichever
         # garbage-collector pass finds it.  Destroying a graph is not permitted while a stream is capturing and
@@ -99,7 +125,7 @@ class Graph:
         try:
             self.graph = torch.cuda.CUDAGraph()
             n0 = load().stego_launch_count()
-            with torch.cuda.graph(self.graph):
+            with torch.cuda.graph(self.graph, stream=capture_stream(self.device)):
                 self.result = fn()
             self.launches = load().stego_launch_count() - n0
         finally:
@@ -108,7 +134,11 @@ class Graph:
 
     def replay(self) -> None:
         global replayed_launches
-        self.graph.replay()
+        if torch.cuda.current_device() == self.device.index:
+            self.graph.replay()
+        else:
+            with torch.cuda.device(self.device):
+                self.graph.replay()
         replayed_launches += self.launches
 
 

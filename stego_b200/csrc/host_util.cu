@@ -25,30 +25,36 @@ static std::atomic<long long> g_launches{0};
 void count_launch() { g_launches.fetch_add(1, std::memory_order_relaxed); }
 long long launch_count() { return g_launches.load(std::memory_order_relaxed); }
 
+std::mutex& opt_in_mutex() {
+  static std::mutex m;
+  return m;
+}
+
+// SM count of the current device, cached per device ordinal (the grids of persistent kernels are sized by it).
 int num_sms() {
-  static int cached = 0;
-  if (cached == 0) {
-    int dev = 0, n = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) return 132;
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) return 132;
-    cached = n;
-  }
-  return cached;
+  static std::atomic<int> cached[kMaxCachedDevices];
+  int dev = 0, n = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess) return 132;
+  const bool cacheable = dev >= 0 && dev < kMaxCachedDevices;
+  if (cacheable && (n = cached[dev].load(std::memory_order_relaxed)) > 0) return n;
+  if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) return 132;
+  if (cacheable) cached[dev].store(n, std::memory_order_relaxed);
+  return n;
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
+// The driver entry point is process-wide (not per device); resolved once, thread-safely.
 static EncodeTiledFn encode_fn() {
-  static EncodeTiledFn fn = nullptr;
-  if (!fn) {
+  static const EncodeTiledFn fn = []() -> EncodeTiledFn {
     void* p = nullptr;
     cudaDriverEntryPointQueryResult q;
     cudaError_t e = cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q);
     if (e != cudaSuccess || q != cudaDriverEntryPointSuccess || !p) return nullptr;
-    fn = reinterpret_cast<EncodeTiledFn>(p);
-  }
+    return reinterpret_cast<EncodeTiledFn>(p);
+  }();
   return fn;
 }
 

@@ -5,6 +5,9 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <atomic>
+#include <mutex>
+
 namespace stego {
 
 // status codes returned by every extern "C" entry point
@@ -28,16 +31,32 @@ int make_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t*
 int make_tmap_f32(CUtensorMap* out, const void* base, int rank, const uint64_t* dims,
                   const uint64_t* strides_bytes, const uint32_t* box);
 
-// Lets Kernel launch with `bytes` of dynamic shared memory: above the 48 KB default that takes an opt-in, set
-// again only when a launch asks for more than before.  Returns STEGO_OK, or cuda_fail(e, what).
+// Device ordinals whose per-device state (shared-memory opt-ins, SM counts) is cached; a process that sees more
+// devices than this still works, it sets the attribute / queries the count on every call for the ordinals beyond.
+constexpr int kMaxCachedDevices = 64;
+
+// Serialises the opt-in slow path of every kernel (rare: once per kernel, device and size increase).
+std::mutex& opt_in_mutex();
+
+// Lets Kernel launch with `bytes` of dynamic shared memory on the current device: above the 48 KB default that takes
+// an opt-in.  A function attribute belongs to the current device's context, so the configured size is kept per device
+// ordinal and set again only when a launch on that device asks for more than before.  Safe from any host thread: the
+// check is one atomic load, and the attribute is raised under a mutex so that a smaller concurrent request can never
+// lower it below a size already recorded.  Returns STEGO_OK, or cuda_fail(e, what).
 template <auto Kernel>
 int opt_in_smem(size_t bytes, const char* what) {
-  static size_t configured = 0;
-  if (bytes > 48 * 1024 && bytes > configured) {
-    cudaError_t e = cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
-    if (e != cudaSuccess) return cuda_fail(e, what);
-    configured = bytes;
-  }
+  static std::atomic<size_t> configured[kMaxCachedDevices];
+  if (bytes <= 48 * 1024) return STEGO_OK;
+  int dev = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e != cudaSuccess) return cuda_fail(e, what);
+  const bool cached = dev >= 0 && dev < kMaxCachedDevices;
+  if (cached && configured[dev].load(std::memory_order_acquire) >= bytes) return STEGO_OK;
+  std::lock_guard<std::mutex> lock(opt_in_mutex());
+  if (cached && configured[dev].load(std::memory_order_relaxed) >= bytes) return STEGO_OK;
+  e = cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+  if (e != cudaSuccess) return cuda_fail(e, what);
+  if (cached) configured[dev].store(bytes, std::memory_order_release);
   return STEGO_OK;
 }
 

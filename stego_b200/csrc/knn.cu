@@ -39,8 +39,9 @@ constexpr size_t KNN_SMEM =
 
 struct KnnParams {
   int n, E, k;
-  long long* idx_out;  // [n][k]
-  float* val_out;      // [n][k] or null
+  int row0, row_end;   // query rows [row0, row_end) are searched; row0 a multiple of KNN_BM
+  long long* idx_out;  // [row_end - row0][k], row r holding query row row0 + r
+  float* val_out;      // the same shape, or null
 };
 
 __global__ void knn_prep_kernel(const float* __restrict__ x, bf16* __restrict__ planes, int n, int E) {
@@ -75,7 +76,8 @@ knn_topk_kernel(const __grid_constant__ CUtensorMap tmF, KnnParams p) {
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const int row_blocks = (p.n + KNN_BM - 1) / KNN_BM;
+  const int rb0 = p.row0 / KNN_BM;
+  const int rb_end = (p.row_end + KNN_BM - 1) / KNN_BM;
   const int col_tiles = (p.n + KNN_BN - 1) / KNN_BN;
   const int nkb = p.E / KNN_BK;
   const int ksteps = 3 * nkb;  // pass 0: A hi x B hi, pass 1: A hi x B lo, pass 2: A lo x B hi
@@ -95,7 +97,7 @@ knn_topk_kernel(const __grid_constant__ CUtensorMap tmF, KnnParams p) {
     warpgroup_reg_dealloc<40>();
     if (warp == 8 && lane == 0) {
       uint32_t stage = 0, phase = 0;
-      for (int rb = blockIdx.x; rb < row_blocks; rb += gridDim.x) {
+      for (int rb = rb0 + blockIdx.x; rb < rb_end; rb += gridDim.x) {
         for (int ct = 0; ct < col_tiles; ++ct) {
           for (int ks = 0; ks < ksteps; ++ks) {
             const int pass = ks / nkb, kb = ks - pass * nkb;
@@ -131,7 +133,7 @@ knn_topk_kernel(const __grid_constant__ CUtensorMap tmF, KnnParams p) {
   float tv[KNN_MAXK];  // sorted descending; dynamic indexing -> local memory (touched only on inserts)
   int ti[KNN_MAXK];
   float acc[KNN_BN / 2];
-  for (int rb = blockIdx.x; rb < row_blocks; rb += gridDim.x) {
+  for (int rb = rb0 + blockIdx.x; rb < rb_end; rb += gridDim.x) {
 #pragma unroll 1
     for (int i = 0; i < KNN_MAXK; ++i) { tv[i] = -INFINITY; ti[i] = -1; }
     float thr = -INFINITY;  // similarity of the current k-th neighbour
@@ -205,7 +207,8 @@ knn_topk_kernel(const __grid_constant__ CUtensorMap tmF, KnnParams p) {
     }
     asm volatile("bar.sync %0, 128;\n" ::"r"(1 + mwg) : "memory");
     const int row = rb * KNN_BM + srow;
-    if (half == 0 && row < p.n) {
+    if (half == 0 && row < p.row_end) {
+      const size_t out_row = static_cast<size_t>(row - p.row0);
       int ia = 0, ib = 0;
       for (int i = 0; i < k; ++i) {
         const float vb = merge_v[srow * KNN_MAXK + ib];
@@ -214,8 +217,8 @@ knn_topk_kernel(const __grid_constant__ CUtensorMap tmF, KnnParams p) {
         const float v = i == 0 ? self_v[srow] : (take_a ? tv[ia] : vb);
         const int x = take_a ? ti[ia] : xb;
         if (take_a) ++ia; else ++ib;
-        p.idx_out[static_cast<size_t>(row) * k + i] = x;
-        if (p.val_out) p.val_out[static_cast<size_t>(row) * k + i] = v;
+        p.idx_out[out_row * k + i] = x;
+        if (p.val_out) p.val_out[out_row * k + i] = v;
       }
     }
     asm volatile("bar.sync %0, 128;\n" ::"r"(1 + mwg) : "memory");  // merge buffer free for the next row block
@@ -227,27 +230,51 @@ knn_topk_kernel(const __grid_constant__ CUtensorMap tmF, KnnParams p) {
 using namespace stego;
 
 // C-ABI: see include/stego_b200.h for the contract.
-extern "C" int stego_knn_topk(const float* feats, int n, int E, int k, void* planes_scratch, long long* idx_out,
-                              float* val_out, void* stream_) {
+extern "C" int stego_knn_prep(const float* feats, int n, int E, void* planes, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  STEGO_CHECK_ARG(feats && planes_scratch && idx_out, "stego_knn_topk: null pointer");
-  STEGO_CHECK_ARG(n > 0 && E > 0 && E % KNN_BK == 0, "stego_knn_topk: E=%d must be a positive multiple of 64", E);
-  STEGO_CHECK_ARG(k >= 1 && k <= KNN_MAXK && k <= n, "stego_knn_topk: k=%d (1..%d, <= n)", k, KNN_MAXK);
-  STEGO_CHECK_ARG((reinterpret_cast<uintptr_t>(planes_scratch) & 15u) == 0, "stego_knn_topk: planes_scratch not 16-byte aligned");
-  knn_prep_kernel<<<(n + 7) / 8, 256, 0, stream>>>(feats, reinterpret_cast<bf16*>(planes_scratch), n, E);
+  STEGO_CHECK_ARG(feats && planes, "stego_knn_prep: null pointer");
+  STEGO_CHECK_ARG(n > 0 && E > 0 && E % KNN_BK == 0, "stego_knn_prep: n=%d, E=%d must be a positive multiple of 64", n, E);
+  STEGO_CHECK_ARG((reinterpret_cast<uintptr_t>(planes) & 15u) == 0, "stego_knn_prep: planes not 16-byte aligned");
+  knn_prep_kernel<<<(n + 7) / 8, 256, 0, stream>>>(feats, reinterpret_cast<bf16*>(planes), n, E);
   STEGO_CHECK_LAUNCH("knn_prep_kernel launch");
+  return STEGO_OK;
+}
+
+extern "C" int stego_knn_topk_rows(const void* planes, int n, int E, int k, int row0, int nrows, long long* idx_out,
+                                   float* val_out, void* stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  STEGO_CHECK_ARG(planes && idx_out, "stego_knn_topk_rows: null pointer");
+  STEGO_CHECK_ARG(n > 0 && E > 0 && E % KNN_BK == 0, "stego_knn_topk_rows: n=%d, E=%d must be a positive multiple of 64",
+                  n, E);
+  STEGO_CHECK_ARG(k >= 1 && k <= KNN_MAXK && k <= n, "stego_knn_topk_rows: k=%d (1..%d, <= n)", k, KNN_MAXK);
+  STEGO_CHECK_ARG(row0 >= 0 && row0 % KNN_BM == 0, "stego_knn_topk_rows: row0=%d must be a non-negative multiple of %d",
+                  row0, KNN_BM);
+  STEGO_CHECK_ARG(nrows >= 1 && (long long)row0 + nrows <= n, "stego_knn_topk_rows: rows [%d, %lld) not within n=%d",
+                  row0, (long long)row0 + nrows, n);
+  STEGO_CHECK_ARG((reinterpret_cast<uintptr_t>(planes) & 15u) == 0, "stego_knn_topk_rows: planes not 16-byte aligned");
   CUtensorMap tm;
   uint64_t dims[3] = {(uint64_t)E, (uint64_t)n, 2};
   uint64_t str[2] = {(uint64_t)E * 2, (uint64_t)n * E * 2};
   uint32_t box[3] = {64, 128, 1};  // KNN_BM = KNN_BN = 128 rows
-  int rc = make_tmap_bf16(&tm, planes_scratch, 3, dims, str, box);
+  int rc = make_tmap_bf16(&tm, planes, 3, dims, str, box);
   if (rc != STEGO_OK) return rc;
   if ((rc = opt_in_smem<knn_topk_kernel>(KNN_SMEM, "knn_topk_kernel")) != STEGO_OK) return rc;
   KnnParams p;
-  p.n = n; p.E = E; p.k = k; p.idx_out = idx_out; p.val_out = val_out;
-  const int row_blocks = (n + KNN_BM - 1) / KNN_BM;
+  p.n = n; p.E = E; p.k = k; p.row0 = row0; p.row_end = row0 + nrows; p.idx_out = idx_out; p.val_out = val_out;
+  const int row_blocks = (nrows + KNN_BM - 1) / KNN_BM;
   const int grid = row_blocks < num_sms() ? row_blocks : num_sms();
   knn_topk_kernel<<<grid, KNN_THREADS, KNN_SMEM, stream>>>(tm, p);
   STEGO_CHECK_LAUNCH("knn_topk_kernel launch");
   return STEGO_OK;
+}
+
+extern "C" int stego_knn_topk(const float* feats, int n, int E, int k, void* planes_scratch, long long* idx_out,
+                              float* val_out, void* stream) {
+  STEGO_CHECK_ARG(feats && planes_scratch && idx_out, "stego_knn_topk: null pointer");
+  STEGO_CHECK_ARG(n > 0 && E > 0 && E % KNN_BK == 0, "stego_knn_topk: E=%d must be a positive multiple of 64", E);
+  STEGO_CHECK_ARG(k >= 1 && k <= KNN_MAXK && k <= n, "stego_knn_topk: k=%d (1..%d, <= n)", k, KNN_MAXK);
+  STEGO_CHECK_ARG((reinterpret_cast<uintptr_t>(planes_scratch) & 15u) == 0, "stego_knn_topk: planes_scratch not 16-byte aligned");
+  int rc = stego_knn_prep(feats, n, E, planes_scratch, stream);
+  if (rc != STEGO_OK) return rc;
+  return stego_knn_topk_rows(planes_scratch, n, E, k, 0, n, idx_out, val_out, stream);
 }

@@ -14,6 +14,7 @@ src/modules.py:30-32), so there is no backward and dropout / drop-path are ident
 from __future__ import annotations
 
 import math
+import threading
 from functools import partial
 from typing import Dict, List, Optional, Tuple
 
@@ -21,6 +22,18 @@ import torch
 import torch.nn as nn
 
 from .. import ops
+
+# Guards the prepared-weight caches: nn.DataParallel runs its replicas' forwards in threads of their own.
+_PREPARE_LOCK = threading.RLock()
+
+
+def _to_device(w, dev):
+    """A copy of the prepared weights (nested dicts / lists of tensors and floats) on `dev`."""
+    if isinstance(w, dict):
+        return {k: _to_device(v, dev) for k, v in w.items()}
+    if isinstance(w, list):
+        return [_to_device(v, dev) for v in w]
+    return w.to(dev) if isinstance(w, torch.Tensor) else w
 
 
 class Mlp(nn.Module):
@@ -117,34 +130,60 @@ class VisionTransformer(nn.Module):
     def _weights_key(self):
         return tuple((p.data_ptr(), p._version) for p in self.parameters())
 
-    def _prepared(self):
-        """bf16 copies of the GEMM weights and fp32 biases / LN params (cached while weights are unchanged)."""
-        key = self._weights_key()
-        if self._cache.get("key") != key:
-            dev = self.cls_token.device
-            E = self.embed_dim
-            w = {}
-            w["pe_w"] = self.patch_embed.proj.weight.detach().reshape(E, -1).to(torch.bfloat16).contiguous()
-            w["pe_b"] = self.patch_embed.proj.bias.detach().float().contiguous()
-            w["cls"] = self.cls_token.detach().float().reshape(E).contiguous()
-            blocks = []
-            for blk in self.blocks:
-                def f32(t, n):
-                    return t.detach().float().contiguous() if t is not None else torch.zeros(n, device=dev)
-                blocks.append(dict(
-                    n1w=f32(blk.norm1.weight, E), n1b=f32(blk.norm1.bias, E), eps1=blk.norm1.eps,
-                    qkv_w=blk.attn.qkv.weight.detach().to(torch.bfloat16).contiguous(),
-                    qkv_b=f32(blk.attn.qkv.bias, 3 * E),
-                    proj_w=blk.attn.proj.weight.detach().to(torch.bfloat16).contiguous(),
-                    proj_b=f32(blk.attn.proj.bias, E),
-                    n2w=f32(blk.norm2.weight, E), n2b=f32(blk.norm2.bias, E), eps2=blk.norm2.eps,
-                    fc1_w=blk.mlp.fc1.weight.detach().to(torch.bfloat16).contiguous(), fc1_b=f32(blk.mlp.fc1.bias, blk.mlp.fc1.out_features),
-                    fc2_w=blk.mlp.fc2.weight.detach().to(torch.bfloat16).contiguous(), fc2_b=f32(blk.mlp.fc2.bias, E)))
-            w["blocks"] = blocks
-            w["nw"] = self.norm.weight.detach().float().contiguous()
-            w["nb"] = self.norm.bias.detach().float().contiguous()
-            self._cache = {"key": key, "w": w, "pos": {}}
-        return self._cache["w"]
+    def _replicate_for_data_parallel(self):
+        """nn.DataParallel's replica: it keeps a reference to this module, whose per-device cache of prepared weights it
+        reads and fills (keyed by this module's parameters, not the replica's freshly broadcast copies)."""
+        replica = super()._replicate_for_data_parallel()
+        replica.__dict__["_master"] = self._root()
+        return replica
+
+    def _root(self) -> "VisionTransformer":
+        """The module whose caches this one uses: itself, or for a DataParallel replica the module replicated."""
+        return self.__dict__.get("_master", self)
+
+    def _prepared(self, device=None):
+        """bf16 copies of the GEMM weights and fp32 biases / LN params on `device` (default: the parameters'), cached
+        while the weights are unchanged.  One cache, on the module itself (for a DataParallel replica: on the module it
+        was replicated from), keyed by that module's parameters' (data_ptr, _version): an in-place update or a new
+        parameter invalidates every device's entry.  Another device's entry is the parameters' device's, copied: the
+        same bits on every device, and a DataParallel call costs a copy per device the first time, not a re-cast."""
+        master = self._root()
+        home = master.cls_token.device
+        dev = home if device is None else torch.device(device)
+        with _PREPARE_LOCK:  # DataParallel replicas prepare from their own threads
+            key = master._weights_key()
+            if master._cache.get("key") != key:
+                master._cache = {"key": key, "w": {}, "pos": {}}
+            ws = master._cache["w"]
+            if home not in ws:
+                ws[home] = master._prepare_weights(home)
+            if dev not in ws:
+                ws[dev] = _to_device(ws[home], dev)
+            return ws[dev]
+
+    def _prepare_weights(self, dev):
+        E = self.embed_dim
+        w = {}
+        w["pe_w"] = self.patch_embed.proj.weight.detach().reshape(E, -1).to(torch.bfloat16).contiguous()
+        w["pe_b"] = self.patch_embed.proj.bias.detach().float().contiguous()
+        w["cls"] = self.cls_token.detach().float().reshape(E).contiguous()
+        blocks = []
+        for blk in self.blocks:
+            def f32(t, n):
+                return t.detach().float().contiguous() if t is not None else torch.zeros(n, device=dev)
+            blocks.append(dict(
+                n1w=f32(blk.norm1.weight, E), n1b=f32(blk.norm1.bias, E), eps1=blk.norm1.eps,
+                qkv_w=blk.attn.qkv.weight.detach().to(torch.bfloat16).contiguous(),
+                qkv_b=f32(blk.attn.qkv.bias, 3 * E),
+                proj_w=blk.attn.proj.weight.detach().to(torch.bfloat16).contiguous(),
+                proj_b=f32(blk.attn.proj.bias, E),
+                n2w=f32(blk.norm2.weight, E), n2b=f32(blk.norm2.bias, E), eps2=blk.norm2.eps,
+                fc1_w=blk.mlp.fc1.weight.detach().to(torch.bfloat16).contiguous(), fc1_b=f32(blk.mlp.fc1.bias, blk.mlp.fc1.out_features),
+                fc2_w=blk.mlp.fc2.weight.detach().to(torch.bfloat16).contiguous(), fc2_b=f32(blk.mlp.fc2.bias, E)))
+        w["blocks"] = blocks
+        w["nw"] = self.norm.weight.detach().float().contiguous()
+        w["nb"] = self.norm.bias.detach().float().contiguous()
+        return w
 
     def interpolate_pos_encoding(self, x, w, h):
         """vision_transformer.py:176-196: bicubic resize of the patch position embeddings (with the
@@ -164,17 +203,25 @@ class VisionTransformer(nn.Module):
         grid = grid.permute(0, 2, 3, 1).reshape(1, -1, dim)
         return torch.cat((self.pos_embed[:, :1], grid), dim=1)
 
-    def _pos_for(self, H: int, W: int) -> torch.Tensor:
-        self._prepared()
-        cache = self._cache["pos"]
-        if (H, W) not in cache:
-            p = self.patch_embed.patch_size
-            ntok = (H // p) * (W // p) + 1
-            with torch.no_grad():
-                dummy = torch.empty(1, ntok, self.embed_dim, device="meta")
-                pos = self.interpolate_pos_encoding(dummy, H, W)
-            cache[(H, W)] = pos.detach().float().reshape(ntok, self.embed_dim).contiguous()
-        return cache[(H, W)]
+    def _pos_for(self, H: int, W: int, device=None) -> torch.Tensor:
+        """The position embeddings of an H x W frame on `device`: computed on the parameters' device, copied to the
+        others (the same bits everywhere; cached per resolution and device with the prepared weights)."""
+        master = self._root()
+        home = master.cls_token.device
+        dev = home if device is None else torch.device(device)
+        self._prepared(dev)
+        with _PREPARE_LOCK:
+            cache = master._cache["pos"]
+            if (H, W, home) not in cache:
+                p = master.patch_embed.patch_size
+                ntok = (H // p) * (W // p) + 1
+                with torch.no_grad():
+                    dummy = torch.empty(1, ntok, master.embed_dim, device="meta")
+                    pos = master.interpolate_pos_encoding(dummy, H, W)
+                cache[(H, W, home)] = pos.detach().float().reshape(ntok, master.embed_dim).contiguous()
+            if (H, W, dev) not in cache:
+                cache[(H, W, dev)] = cache[(H, W, home)].to(dev)
+            return cache[(H, W, dev)]
 
     # ------------------------------------------------------------------------------------------
     # the kernel sequence
@@ -191,7 +238,7 @@ class VisionTransformer(nn.Module):
         patchify kernel (stego_vit_patchify_tta); x then holds 2B*N rows."""
         if not img.is_cuda:
             raise RuntimeError("stego_b200: the DINO ViT forward only exists as sm_90a kernels (no CPU fallback)")
-        w = self._prepared()
+        w = self._prepared(img.device)
         # bf16 images are taken as they are (patchify rounds fp32 images to bf16 anyway: same operand bits)
         img = (img if img.dtype == torch.bfloat16 else img.float()).contiguous()
         B, _, H, W = img.shape
@@ -201,7 +248,7 @@ class VisionTransformer(nn.Module):
         hw = (H // p) * (W // p)
         N = hw + 1
         dev = img.device
-        pos = self._pos_for(H, W)
+        pos = self._pos_for(H, W, dev)
         rows = ops.patchify_tta(img, p) if mirror else ops.patchify(img, p)
         x = torch.empty(B * N, E, dtype=torch.float32, device=dev)
         ops.gemm(rows, w["pe_w"], x, M=B * hw, N=E, K=3 * p * p, bias=w["pe_b"], residual=pos, row_div=hw)
@@ -276,9 +323,9 @@ class VisionTransformer(nn.Module):
         input (the fused step passes [img, img_pos] — no torch.cat of the two 19 MB batches).  One graph per
         (feature kind, input shape, device, dtype)."""
         from .. import _lib
-        self._prepared()
-        graphs = self._cache.setdefault("graphs", {})
         parts = list(img) if isinstance(img, (list, tuple)) else [img]
+        self._prepared(parts[0].device)
+        graphs = self._root()._cache.setdefault("graphs", {})
         shape = (sum(p.shape[0] for p in parts),) + tuple(parts[0].shape[1:])
         dt = torch.bfloat16 if all(p.dtype == torch.bfloat16 for p in parts) else torch.float32
         key = (kind, shape, parts[0].device.index, dt)
@@ -286,7 +333,8 @@ class VisionTransformer(nn.Module):
             img = torch.cat([p.to(dt) for p in parts], 0) if len(parts) > 1 else parts[0].to(dt)
             self._eager(img, kind)  # warm-up: kernel attributes, pos-embed cache, allocator
             static_in = img.detach().contiguous().clone()
-            graphs[key] = (_lib.Graph(lambda: self._eager(static_in, kind)), static_in)
+            with torch.cuda.device(static_in.device):  # captured on the input's device, whichever is current
+                graphs[key] = (_lib.Graph(lambda: self._eager(static_in, kind)), static_in)
         g, static_in = graphs[key]
         off = 0
         for part in parts:
@@ -299,12 +347,12 @@ class VisionTransformer(nn.Module):
     def graph_input(self, kind: str, shape, device, dtype=torch.float32):
         """The static input of the captured graph for (kind, shape), or None before that graph exists.  A caller may
         build part of its batch straight into a slice of it and pass that slice back in its list of batches."""
-        return self._cache.get("graphs", {}).get((kind, tuple(shape), device.index, dtype), (None, None))[1]
+        return self._root()._cache.get("graphs", {}).get((kind, tuple(shape), device.index, dtype), (None, None))[1]
 
     def _patch_features_eager(self, img: torch.Tensor, mirror: bool = False) -> torch.Tensor:
         B = img.shape[0] * (2 if mirror else 1)
         x, _ = self.forward_tokens(img, mirror=mirror)
-        w = self._prepared()
+        w = self._prepared(x.device)
         N = x.shape[0] // B
         out = torch.empty(B * (N - 1), self.embed_dim, dtype=torch.bfloat16, device=x.device)
         ops.layernorm(x, w["nw"], w["nb"], out, eps=self.norm.eps, drop_cls_ntok=N)
@@ -313,7 +361,7 @@ class VisionTransformer(nn.Module):
     def _key_features_eager(self, img: torch.Tensor, mirror: bool = False) -> torch.Tensor:
         B, E = img.shape[0] * (2 if mirror else 1), self.embed_dim
         x, _ = self.forward_tokens(img, stop_before_last=True, mirror=mirror)
-        bw = self._prepared()["blocks"][-1]
+        bw = self._prepared(x.device)["blocks"][-1]
         N = x.shape[0] // B
         y = torch.empty(B * (N - 1), E, dtype=torch.bfloat16, device=x.device)
         ops.layernorm(x, bw["n1w"], bw["n1b"], y, eps=bw["eps1"], drop_cls_ntok=N)
@@ -329,7 +377,7 @@ class VisionTransformer(nn.Module):
         from .. import _lib
         B = img.shape[0]
         x, _ = self.forward_tokens(img)
-        w = self._prepared()
+        w = self._prepared(x.device)
         out = torch.zeros(B, self.embed_dim, dtype=torch.float32, device=x.device)
         _lib.check(_lib.load().stego_layernorm_gap(_lib.ptr(x), _lib.ptr(w["nw"]), _lib.ptr(w["nb"]), _lib.ptr(out), B,
                                                    x.shape[0] // B, self.embed_dim, float(self.norm.eps), _lib.stream()),
@@ -346,7 +394,7 @@ class VisionTransformer(nn.Module):
         from .. import _lib
         B, E = img.shape[0], self.embed_dim
         x, _ = self.forward_tokens(img, stop_before_last=True)
-        bw = self._prepared()["blocks"][-1]
+        bw = self._prepared(x.device)["blocks"][-1]
         pooled = torch.zeros(B, E, dtype=torch.float32, device=x.device)
         lib = _lib.load()
         _lib.check(lib.stego_layernorm_gap(_lib.ptr(x), _lib.ptr(bw["n1w"]), _lib.ptr(bw["n1b"]), _lib.ptr(pooled), B,
@@ -376,7 +424,7 @@ class VisionTransformer(nn.Module):
 
     def final_norm(self, x: torch.Tensor, B: int) -> torch.Tensor:
         """The final LayerNorm of a residual stream [B*N, E] fp32 -> bf16 [B, N, E]."""
-        w = self._prepared()
+        w = self._prepared(x.device)
         out = torch.empty(x.shape[0], self.embed_dim, dtype=torch.bfloat16, device=x.device)
         ops.layernorm(x, w["nw"], w["nb"], out, eps=self.norm.eps)
         return out.view(B, -1, self.embed_dim)

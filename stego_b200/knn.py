@@ -2,30 +2,77 @@
 loop of the reference's `src/precompute_knns.py:83-96`, which produces the `nns_*.npz` files `img_pos` is drawn from."""
 from __future__ import annotations
 
-from typing import Optional, Tuple
+from typing import List, Optional, Sequence, Tuple
 
 import torch
 
 from . import _lib
+from .devices import DeviceLike, check_devices, split
+
+KNN_ROW_BLOCK = 128  # knn.cu KNN_BM: a row range of stego_knn_topk_rows starts on a multiple of it
 
 
-def knn_topk(feats: torch.Tensor, k: int = 30, return_values: bool = False
-             ) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
+def knn_topk(feats: torch.Tensor, k: int = 30, return_values: bool = False,
+             devices: Optional[Sequence[DeviceLike]] = None) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
     """feats: [n, E] fp32 CUDA (un-normalised descriptors, e.g. `model(img).mean([2, 3])`, precompute_knns.py:19).
     Returns int64 [n, k] neighbour indices of the reference's `torch.topk(einsum("nf,mf->nm", ...), 30)[1]` with the
     order pinned: column 0 is the row's own index, always (also next to exact or near duplicates and for an all-zero
     row — src/data.py:524 reads columns 1..k as "not the image itself"), columns 1..k-1 the other rows by (cosine
-    similarity descending, index ascending); and the fp32 similarities of those indices if requested."""
+    similarity descending, index ascending); and the fp32 similarities of those indices if requested.
+
+    devices: several GPUs of the node, the first being feats' device (see stego_b200.devices.check_devices).  The
+    normalised descriptors are prepared once on it and copied to the others; each device searches a contiguous range of
+    128-row blocks against all n rows and the results are gathered on the first device.  A row's result depends only on
+    the row and the fixed key-tile order, so the output is bit-identical to the single-device call."""
+    devs = check_devices(devices, feats.device, "knn_topk")
     _lib.require_cuda(feats)
     if feats.dim() != 2 or feats.dtype != torch.float32:
         raise RuntimeError("stego_b200.knn_topk: feats must be a 2-D fp32 tensor")
     feats = feats.contiguous()
     n, E = feats.shape
+    if devs is not None:
+        if n < 1 or E < 1 or E % 64 or not 1 <= k <= min(32, n):
+            raise ValueError(f"knn_topk: n={n}, E={E}, k={k} unsupported (E a positive multiple of 64, 1 <= k <= "
+                             f"min(32, n))")
+        ranges = split(n, len(devs), KNN_ROW_BLOCK)
+        return _knn_topk_sharded(feats, k, return_values, [(d, r0, r1) for d, (r0, r1) in zip(devs, ranges)])
     planes = torch.empty(2, n, E, dtype=torch.bfloat16, device=feats.device)
     idx = torch.empty(n, k, dtype=torch.long, device=feats.device)
     vals = torch.empty(n, k, dtype=torch.float32, device=feats.device) if return_values else None
     rc = _lib.load().stego_knn_topk(_lib.ptr(feats), n, E, k, _lib.ptr(planes), _lib.ptr(idx), _lib.ptr(vals), _lib.stream())
     _lib.check(rc, "stego_knn_topk")
+    return idx, vals
+
+
+def _knn_topk_sharded(feats: torch.Tensor, k: int, return_values: bool, shards: List[Tuple[torch.device, int, int]]
+                      ) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
+    """knn_topk over query-row ranges [r0, r1) (r0 a multiple of 128), one per (device, r0, r1) entry, launched from the
+    calling thread one device after another.  The first entry runs on feats' device and writes into the outputs in
+    place; every other entry gets its own copy of the planes and its own outputs, copied back into the first device's
+    (the copies are ordered on the devices' current streams; no host synchronisation)."""
+    lib = _lib.load()
+    n, E = feats.shape
+    primary = feats.device
+    planes = torch.empty(2, n, E, dtype=torch.bfloat16, device=primary)
+    _lib.check(lib.stego_knn_prep(_lib.ptr(feats), n, E, _lib.ptr(planes), _lib.stream()), "stego_knn_prep")
+    idx = torch.empty(n, k, dtype=torch.long, device=primary)
+    vals = torch.empty(n, k, dtype=torch.float32, device=primary) if return_values else None
+    for i, (dev, r0, r1) in enumerate(shards):
+        if r1 <= r0:
+            continue
+        with torch.cuda.device(dev):
+            if i == 0:
+                pl, out_i, out_v = planes, idx[r0:r1], vals[r0:r1] if return_values else None
+            else:
+                pl = planes.to(dev)
+                out_i = torch.empty(r1 - r0, k, dtype=torch.long, device=dev)
+                out_v = torch.empty(r1 - r0, k, dtype=torch.float32, device=dev) if return_values else None
+            _lib.check(lib.stego_knn_topk_rows(_lib.ptr(pl), n, E, k, r0, r1 - r0, _lib.ptr(out_i), _lib.ptr(out_v),
+                                               _lib.stream()), "stego_knn_topk_rows")
+            if i > 0:
+                idx[r0:r1].copy_(out_i)
+                if return_values:
+                    vals[r0:r1].copy_(out_v)
     return idx, vals
 
 
@@ -51,14 +98,27 @@ def knn_descriptors(net, img: torch.Tensor) -> torch.Tensor:
     return pooled
 
 
-def precompute_knns(net, batches, k: int = 30) -> torch.Tensor:
+def precompute_knns(net, batches, k: int = 30, devices: Optional[Sequence[DeviceLike]] = None) -> torch.Tensor:
     """The device-side body of precompute_knns.py:83-96: descriptors of every image (`batches` yields image tensors or
-    dicts with an "img" entry, like the reference's loader), cosine-similarity top-k over the whole set."""
+    dicts with an "img" entry, like the reference's loader), cosine-similarity top-k over the whole set.
+
+    devices: several GPUs of the node, the first being the net's device.  Batch i's descriptors are computed on
+    devices[i % len(devices)] (the frozen ViT's prepared weights are cached per device), gathered in loader order on
+    the first device, and the search runs as knn_topk(..., devices=devices).  The result equals the single-device one;
+    the exception is a net in training mode with cfg.dropout, whose Dropout2d noise each device draws from its own
+    generator (as nn.DataParallel does)."""
+    primary = next(net.parameters()).device
+    devs = check_devices(devices, primary, "precompute_knns")
     feats = []
-    for pack in batches:
+    for i, pack in enumerate(batches):
         img = pack["img"] if isinstance(pack, dict) else pack
-        feats.append(knn_descriptors(net, img.to(next(net.parameters()).device)))
-    idx, _ = knn_topk(torch.cat(feats, 0), k)
+        if devs is None:
+            feats.append(knn_descriptors(net, img.to(primary)))
+            continue
+        dev = devs[i % len(devs)]
+        with torch.cuda.device(dev):
+            feats.append(knn_descriptors(net, img.to(dev)).to(primary))
+    idx, _ = knn_topk(torch.cat(feats, 0), k, devices=devs)
     return idx
 
 

@@ -317,18 +317,20 @@ class DinoFeaturizer(nn.Module):
         ca, cb = self.cluster2[0], self.cluster2[2]
         return c1.weight, c1.bias, ca.weight, ca.bias, cb.weight, cb.bias
 
-    def head_code(self, feat_tok: torch.Tensor, m1, m2, fh: int, fw: int) -> torch.Tensor:
-        """cluster1 (+ cluster2) on tokens-major features -> code [B, dim, h, w] (view of padded storage)."""
+    def head_code(self, feat_tok: torch.Tensor, m1, m2, fh: int, fw: int, params=None) -> torch.Tensor:
+        """cluster1 (+ cluster2) on tokens-major features -> code [B, dim, h, w] (view of padded storage).  params: the
+        head_params() tuple to use instead of the module's own (e.g. their copies on feat_tok's device)."""
         B, hw, E = feat_tok.shape
         m2 = m2 if self.proj_type == "nonlinear" else None
-        store = _HeadFn.apply(feat_tok.reshape(B * hw, E), m1, m2, B, hw, *self.head_params())
+        store = _HeadFn.apply(feat_tok.reshape(B * hw, E), m1, m2, B, hw, *(params or self.head_params()))
         return store.view(B, fh, fw, -1)[..., :self.dim].permute(0, 3, 1, 2)
 
-    def eval_code(self, feat_tok: torch.Tensor, fh: int, fw: int) -> torch.Tensor:
+    def eval_code(self, feat_tok: torch.Tensor, fh: int, fw: int, params=None) -> torch.Tensor:
         """The eval-mode code [B, C, h, w] of tokens-major features: the head's, or with projection_type None the
-        features themselves (modules.py:108-113), as a bf16 view of feat_tok that the probe kernels read in place."""
+        features themselves (modules.py:108-113), as a bf16 view of feat_tok that the probe kernels read in place.
+        params as in head_code."""
         if self.proj_type is not None:
-            return self.head_code(feat_tok, None, None, fh, fw)
+            return self.head_code(feat_tok, None, None, fh, fw, params)
         B, _, E = feat_tok.shape
         return feat_tok.view(B, fh, fw, E).permute(0, 3, 1, 2)
 

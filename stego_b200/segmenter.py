@@ -20,6 +20,7 @@ shard; only gradients cross ranks (averaged).
 from __future__ import annotations
 
 import contextlib
+from types import SimpleNamespace
 from typing import Dict, List, Optional, Sequence
 
 import torch
@@ -27,6 +28,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from . import _lib, corr, ops
+from .devices import DeviceLike, check_devices, split
 from .modules import ClusterLookup, ContrastiveCorrelationLoss, ContrastiveCRFLoss, DinoFeaturizer, \
     FeaturePyramidNet, _ClusterLookupFn, _ClusterLookupWideFn, norm, pixel_cosine, sample
 
@@ -668,7 +670,8 @@ class LitUnsupervisedSegmenter(nn.Module):
             coords2 = torch.rand(coord_shape, device=img.device) * 2 - 1
             metric.update(feats, code, label, coords1, coords2)
 
-    def eval_step(self, batch, run_crf: bool = False, want_probs: bool = False) -> Dict[str, torch.Tensor]:
+    def eval_step(self, batch, run_crf: bool = False, want_probs: bool = False,
+                  devices: Optional[Sequence[DeviceLike]] = None) -> Dict[str, torch.Tensor]:
         """The evaluation loop body of eval_segmentation.py:122-141 (also demo_segmentation.py:57-78, plot_potsdam.py:44-57)
         for one batch of frames:
 
@@ -697,10 +700,24 @@ class LitUnsupervisedSegmenter(nn.Module):
         With projection_type None (the DINO baseline, dim = the backbone's width) the code is the mirrored bf16 tokens
         themselves, read in place by the probe kernels.  Configurations the fused eval kernels do not take
         (projection_type None with another dim; more than 32 cluster-probe rows) and CPU tensors are refused before
-        anything is enqueued."""
-        from .eval import fused_eval_crf, fused_probe_log_probs
+        anything is enqueued.
+
+        devices: several GPUs of the node, the first being the frames' and the model's device (see
+        stego_b200.devices.check_devices; None or one device is the single-device call).  The B frames are split into
+        contiguous, nearly equal slices, one per device (devices without a frame stay idle); each device runs the
+        loop body above on its slice with its own backbone graph, copies of the head and probe parameters and its own
+        int64 confusion counts, which are added into the two `stats` on the first device.  The outputs are gathered
+        there in the shapes above.  Every frame's results are independent of the rest of the batch and the counts are
+        integer sums, so the outputs and both confusion matrices are bit-equal to the single-device call.  Launches go
+        out from the calling thread, device after device; the host synchronises only where the single-device call does
+        (once per frame with run_crf)."""
         img, label = batch["img"], batch.get("label")
+        devs = self._check_devices(devices, img, "eval_step")
         self._check_eval_args(img, label, run_crf)
+        if devs is not None:
+            return self._eval_step_sharded(img, label, run_crf, want_probs,
+                                           [(d, b0, b1) for d, (b0, b1) in zip(devs, split(img.shape[0], len(devs)))])
+        from .eval import fused_eval_crf, fused_probe_log_probs
         self.flush()
         net = self.net
         B, fh, fw = img.shape[0], img.shape[2] // net.patch_size, img.shape[3] // net.patch_size
@@ -725,9 +742,93 @@ class LitUnsupervisedSegmenter(nn.Module):
             result.update(linear_probs=probs[0], cluster_probs=probs[1])
         return result
 
+    def _check_devices(self, devices, img, who: str):
+        """check_devices against the inputs' device, which must also be the model's."""
+        devs = check_devices(devices, img.device, who)
+        model_dev = self.net.cluster1[0].weight.device
+        if devs is not None and model_dev != devs[0]:
+            raise ValueError(f"{who}: the model is on {model_dev}, the first device is {devs[0]}")
+        return devs
+
+    def _device_params(self, dev: torch.device, primary: bool):
+        """(head parameters, linear probe, cluster probe) for evaluation on `dev`: the modules' own on the primary,
+        copies elsewhere.  The copies are made on every call (a few MB at most): the hand-scheduled training step
+        writes the parameters through raw pointers, which no version counter sees, so a cache could not tell an
+        update."""
+        if primary:
+            return self.net.head_params(), self.linear_probe, self.cluster_probe
+        head = tuple(None if t is None else t.detach().to(dev) for t in self.net.head_params())
+        lin = SimpleNamespace(weight=self.linear_probe.weight.detach().to(dev),
+                              bias=self.linear_probe.bias.detach().to(dev))
+        clu = SimpleNamespace(clusters=self.cluster_probe.clusters.detach().to(dev))
+        return head, lin, clu
+
+    def _eval_step_sharded(self, img, label, run_crf: bool, want_probs: bool, shards) -> Dict[str, torch.Tensor]:
+        """eval_step over frame slices [b0, b1), one per (device, b0, b1) entry, the first entry on img's device.  Every
+        device first runs the backbone and the head on its slice, then the probes (or the CRF, whose per-frame host
+        synchronisations then find the other devices' backbones already running), and copies its outputs and counts to
+        the first device on the devices' current streams.  With the CRF, each frame's lattice build still waits on the
+        host for its device, and these waits run one after another on the calling thread: only the devices' GPU work
+        overlaps."""
+        from .eval import fused_eval_crf, fused_probe_log_probs
+        self.flush()
+        net = self.net
+        primary = img.device
+        B, fh, fw = img.shape[0], img.shape[2] // net.patch_size, img.shape[3] // net.patch_size
+        size = tuple(label.shape[-2:]) if label is not None else tuple(img.shape[-2:])
+        n_lin, n_clu = self.linear_probe.weight.shape[0], self.cluster_probe.clusters.shape[0]
+        lab_all = label.reshape(B, *size) if label is not None else None
+        preds = [torch.empty(B, *size, dtype=torch.uint8, device=primary) for _ in range(2)]
+        probs = [torch.empty(B, n, *size, dtype=torch.float32, device=primary) for n in (n_lin, n_clu)] \
+            if want_probs else []
+        metrics = (self.test_linear_metrics, self.test_cluster_metrics)
+        use_graph = getattr(self.cfg, "cuda_graph", True)
+        work = []
+        with self._net_in_eval_mode(), torch.no_grad():
+            for i, (dev, b0, b1) in enumerate(shards):
+                if b1 <= b0:
+                    continue
+                with torch.cuda.device(dev):
+                    first = i == 0
+                    x = img[b0:b1] if first else img[b0:b1].to(dev)
+                    lab = None if label is None else (lab_all[b0:b1] if first else lab_all[b0:b1].to(dev))
+                    head, lin, clu = self._device_params(dev, first)
+                    tok = net.backbone_tokens(x, use_graph=use_graph, mirror=True)  # [2b, hw, E]
+                    code_all = net.eval_code(tok, fh, fw, head)
+                    if any(d == dev for d, c0, c1 in shards[i + 1:] if c1 > c0):
+                        code_all = code_all.clone()  # the graph's output buffer is reused by the next slice's replay
+                    stats = {}
+                    if label is not None:
+                        conf = [m.stats if first else torch.zeros_like(m.stats, device=dev) for m in metrics]
+                        stats = dict(linear_confusion=conf[0], cluster_confusion=conf[1])
+                    work.append((first, dev, b0, b1, x, lab, code_all, lin, clu, stats))
+            for first, dev, b0, b1, x, lab, code_all, lin, clu, stats in work:
+                with torch.cuda.device(dev):
+                    code, code_flipped = code_all[:b1 - b0], code_all[b1 - b0:]
+                    if run_crf:
+                        out = fused_eval_crf(code, lin, clu, x, 2.0, code_flipped=code_flipped, label=lab,
+                                             want_marginals=want_probs, **stats)
+                        p, q = out[:2], out[2:]
+                    else:
+                        out = fused_probe_log_probs(code, lin, clu, size, 2.0, want_log_probs=want_probs,
+                                                    want_argmax=True, code_flipped=code_flipped, label=lab, **stats)
+                        p, q = out[2:], out[:2]
+                    for k in range(2):
+                        preds[k][b0:b1].copy_(p[k])
+                        if want_probs:
+                            probs[k][b0:b1].copy_(q[k])
+                    if stats and not first:
+                        for m, c in zip(metrics, (stats["linear_confusion"], stats["cluster_confusion"])):
+                            m.stats.add_(c.to(primary))
+        result = dict(linear_preds=preds[0], cluster_preds=preds[1])
+        if want_probs:
+            result.update(linear_probs=probs[0], cluster_probs=probs[1])
+        return result
+
     def eval_scene(self, tiles: torch.Tensor, grid: Sequence[int], label: Optional[torch.Tensor] = None,
                    run_crf: bool = False, probes: Sequence[str] = ("linear", "cluster"), want_probs: bool = False,
-                   map_clusters: bool = False, chunk: int = 64) -> Dict[str, torch.Tensor]:
+                   map_clusters: bool = False, chunk: int = 64,
+                   devices: Optional[Sequence[DeviceLike]] = None) -> Dict[str, torch.Tensor]:
         """A scene evaluated from its tiles and stitched into one mosaic (plot_potsdam.py:44-83):
 
             for each chunk of tiles: eval_step's loop body (flip-TTA code, upsampling, probes, metric updates)
@@ -755,10 +856,31 @@ class LitUnsupervisedSegmenter(nn.Module):
         (UnsupervisedMetrics.map_clusters; unmatched extra clusters become 255); the metric's compute() must have run.
         Every argument is checked before the first launch (ValueError for shapes and limits, RuntimeError for CPU
         tensors), and the mean field's value buffers are checked against the free device memory before it is
-        enqueued (RuntimeError naming the sizes)."""
+        enqueued (RuntimeError naming the sizes).
+
+        devices: several GPUs of the node, the first being the tiles' and the model's device (see
+        stego_b200.devices.check_devices; None or one device is the single-device call).  The grid's tile rows are
+        split into contiguous, nearly equal bands, one per device.  Each other device evaluates its band's tiles,
+        `chunk` at a time, into a staging band laid out as those mosaic rows (predictions, log-probabilities or the
+        CRF's unary rows), which is then copied into the first device's mosaic in one contiguous copy per plane; its
+        confusion counts go to int64 counts of its own, added into the first device's.  The outputs and both confusion
+        matrices are bit-equal to the single-device call.  With run_crf the one mean field over the mosaic still runs
+        on the first device alone; it is most of a large cluster-only scene's time (DESIGN.md §10), which bounds
+        what more devices gain there."""
+        devs = self._check_devices(devices, tiles, "eval_scene")
+        R, C, n_tiles, H, W, probes = self._check_scene_args(tiles, grid, label, run_crf, probes, map_clusters, chunk)
+        dev = tiles.device
+        bands = [(dev, 0, R)] if devs is None else [(d, r0, r1) for d, (r0, r1) in zip(devs, split(R, len(devs)))]
+        return self._eval_scene_bands(tiles, label, run_crf, probes, want_probs, map_clusters, chunk, R, C, n_tiles, H,
+                                      W, bands)
+
+    def _eval_scene_bands(self, tiles, label, run_crf, probes, want_probs, map_clusters, chunk, R, C, n_tiles, H, W,
+                          bands) -> Dict[str, torch.Tensor]:
+        """eval_scene over bands of tile rows [r0, r1), one per (device, r0, r1) entry, the first entry on the tiles'
+        device and writing the mosaic in place, every other one into a staging band of its own that is copied into the
+        first device's mosaic."""
         from . import crf
         from .eval import _eval_codes, _probe_tables
-        R, C, n_tiles, H, W, probes = self._check_scene_args(tiles, grid, label, run_crf, probes, map_clusters, chunk)
         self.flush()
         tiles = tiles.detach().contiguous()
         lib = _lib.load()
@@ -769,41 +891,82 @@ class LitUnsupervisedSegmenter(nn.Module):
         HH, WW = R * H, C * W
         lin_on, clu_on = "linear" in probes, "cluster" in probes
         n_lin, n_clu = self.linear_probe.weight.shape[0], self.cluster_probe.clusters.shape[0]
-        wl, bl, cl = _probe_tables(self.linear_probe, self.cluster_probe, net.dim)
-        scratch = torch.empty(min(chunk, n_tiles) * h * w, 80, dtype=torch.float32, device=dev)  # eval_probes.cu EV_LD
+        metrics = {"linear": self.test_linear_metrics, "cluster": self.test_cluster_metrics}
+        use_graph = getattr(self.cfg, "cuda_graph", True)
+        out = {}
+        row = 32 * len(probes)  # CRF rows of both probes (linear, then cluster), or of the one requested
+
+        def mosaic(d, rows):  # the outputs of `rows` tile rows on device d
+            if run_crf:
+                return dict(unary=torch.empty(rows * H * WW, row, dtype=torch.float32, device=d),
+                            Q=torch.empty(rows * H * WW, row, dtype=torch.float32, device=d))
+            return dict(preds={k: torch.empty(rows * H, WW, dtype=torch.uint8, device=d) for k in probes},
+                        probs={k: torch.empty(n, rows * H, WW, dtype=torch.float32, device=d)
+                               for k, n in (("linear", n_lin), ("cluster", n_clu)) if k in probes} if want_probs else {})
+
+        full = mosaic(dev, R)
+        with self._net_in_eval_mode(), torch.no_grad():
+            for i, (d, r0, r1) in enumerate(bands):
+                if r1 <= r0:
+                    continue
+                first = i == 0
+                with torch.cuda.device(d):
+                    bt0, bt1 = r0 * C, r1 * C  # the band's tiles
+                    band_tiles = tiles[bt0:bt1] if first else tiles[bt0:bt1].to(d)
+                    dst = full if first else mosaic(d, r1 - r0)
+                    head, lin_p, clu_p = self._device_params(d, first)
+                    wl, bl, cl = _probe_tables(lin_p, clu_p, net.dim)
+                    scratch = torch.empty(min(chunk, bt1 - bt0) * h * w, 80, dtype=torch.float32, device=d)  # EV_LD
+                    stats = {k: None for k in ("linear", "cluster")}
+                    lab, lab_bytes = None, 0
+                    if label is not None and not run_crf:
+                        lab, lab_bytes = ops.probe_label(label[bt0:bt1] if first else label[bt0:bt1].to(d),
+                                                         bt1 - bt0, H, W)
+                        stats = {k: (metrics[k].stats if first else torch.zeros_like(metrics[k].stats, device=d))
+                                 if k in probes else None for k in stats}
+                    for c0 in range(0, bt1 - bt0, chunk):
+                        img = band_tiles[c0:c0 + chunk]
+                        B = img.shape[0]
+                        t0 = c0 if not first else bt0 + c0  # tile index within the band's mosaic rows
+                        tok = net.backbone_tokens(img, use_graph=use_graph, mirror=True)
+                        code_all = net.eval_code(tok, h, w, head)  # [2B, dim, h, w]
+                        x, xf, ld, bf16 = _eval_codes(code_all[:B], code_all[B:])
+                        sfx = "_bf16" if bf16 else ""
+                        rows_here = R if first else r1 - r0
+                        if run_crf:
+                            _lib.check(getattr(lib, "stego_eval_crf_unary_mosaic" + sfx)(
+                                _lib.ptr(x), _lib.ptr(xf), ld, net.dim, B, h, w, H, W, _lib.ptr(wl), _lib.ptr(bl), n_lin,
+                                _lib.ptr(cl), n_clu, 2.0, _lib.ptr(scratch), _lib.ptr(dst["unary"]), _lib.ptr(dst["Q"]),
+                                int(lin_on) + 2 * int(clu_on), t0, rows_here, C, WW, _lib.stream()),
+                                "stego_eval_crf_unary_mosaic" + sfx)
+                        else:
+                            _lib.check(getattr(lib, "stego_eval_probes_mosaic" + sfx)(
+                                _lib.ptr(x), _lib.ptr(xf), ld, net.dim, B, h, w, H, W, _lib.ptr(wl), _lib.ptr(bl), n_lin,
+                                _lib.ptr(cl), n_clu, 2.0, _lib.ptr(scratch), _lib.ptr(dst["probs"].get("linear")),
+                                _lib.ptr(dst["probs"].get("cluster")), _lib.ptr(dst["preds"].get("linear")),
+                                _lib.ptr(dst["preds"].get("cluster")), _lib.ptr(lab[c0:] if lab is not None else None),
+                                lab_bytes, n_lin if lab is not None else 0, _lib.ptr(stats["linear"]),
+                                _lib.ptr(stats["cluster"]), t0, rows_here, C, WW, _lib.stream()),
+                                "stego_eval_probes_mosaic" + sfx)
+                    if first:
+                        continue
+                    y0, y1 = r0 * H, r1 * H  # the band's mosaic rows: one contiguous block per plane
+                    if run_crf:
+                        for k in ("unary", "Q"):
+                            full[k][y0 * WW:y1 * WW].copy_(dst[k])
+                    else:
+                        for k in probes:
+                            full["preds"][k][y0:y1].copy_(dst["preds"][k])
+                            for c in range(dst["probs"][k].shape[0] if want_probs else 0):
+                                full["probs"][k][c, y0:y1].copy_(dst["probs"][k][c])
+                            if stats[k] is not None:
+                                metrics[k].stats.add_(stats[k].to(dev))
         lin_stats = self.test_linear_metrics.stats if label is not None and lin_on else None
         clu_stats = self.test_cluster_metrics.stats if label is not None and clu_on else None
-        out = {}
         if run_crf:
-            row = 32 * len(probes)  # rows of both probes (linear, then cluster), or of the one requested
-            unary = torch.empty(HH * WW, row, dtype=torch.float32, device=dev)
-            Q = torch.empty(HH * WW, row, dtype=torch.float32, device=dev)
+            unary, Q = full["unary"], full["Q"]
         else:
-            lab, lab_bytes = ops.probe_label(label, n_tiles, H, W) if label is not None else (None, 0)
-            preds = {k: torch.empty(HH, WW, dtype=torch.uint8, device=dev) for k in probes}
-            probs = {k: torch.empty(n, HH, WW, dtype=torch.float32, device=dev)
-                     for k, n in (("linear", n_lin), ("cluster", n_clu)) if k in probes} if want_probs else {}
-        with self._net_in_eval_mode(), torch.no_grad():
-            for t0 in range(0, n_tiles, chunk):
-                img = tiles[t0:t0 + chunk]
-                B = img.shape[0]
-                tok = net.backbone_tokens(img, use_graph=getattr(self.cfg, "cuda_graph", True), mirror=True)
-                code_all = net.eval_code(tok, h, w)  # [2B, dim, h, w]
-                x, xf, ld, bf16 = _eval_codes(code_all[:B], code_all[B:])
-                sfx = "_bf16" if bf16 else ""
-                if run_crf:
-                    _lib.check(getattr(lib, "stego_eval_crf_unary_mosaic" + sfx)(
-                        _lib.ptr(x), _lib.ptr(xf), ld, net.dim, B, h, w, H, W, _lib.ptr(wl), _lib.ptr(bl), n_lin,
-                        _lib.ptr(cl), n_clu, 2.0, _lib.ptr(scratch), _lib.ptr(unary), _lib.ptr(Q), int(lin_on) + 2 * int(clu_on), t0, R, C, WW,
-                        _lib.stream()), "stego_eval_crf_unary_mosaic" + sfx)
-                else:
-                    _lib.check(getattr(lib, "stego_eval_probes_mosaic" + sfx)(
-                        _lib.ptr(x), _lib.ptr(xf), ld, net.dim, B, h, w, H, W, _lib.ptr(wl), _lib.ptr(bl), n_lin,
-                        _lib.ptr(cl), n_clu, 2.0, _lib.ptr(scratch), _lib.ptr(probs.get("linear")),
-                        _lib.ptr(probs.get("cluster")), _lib.ptr(preds.get("linear")), _lib.ptr(preds.get("cluster")),
-                        _lib.ptr(lab[t0:] if lab is not None else None), lab_bytes, n_lin if lab is not None else 0,
-                        _lib.ptr(lin_stats), _lib.ptr(clu_stats), t0, R, C, WW, _lib.stream()),
-                        "stego_eval_probes_mosaic" + sfx)
+            preds, probs = full["preds"], full["probs"]
         if run_crf:
             image = crf.prepare_image(tiles.view(R, C, 3, H, W).permute(2, 0, 3, 1, 4).reshape(3, HH, WW))
             lg = crf._position_lattice(HH, WW, dev, cache=n_tiles == 1)
