@@ -9,7 +9,7 @@ No CPU fallback: CUDA tensors only.
 """
 from __future__ import annotations
 
-from typing import Dict, Iterable, Optional, Tuple
+from typing import Dict, Iterable, Optional, Sequence, Tuple
 
 import torch
 import torch.nn.functional as F
@@ -171,6 +171,29 @@ def check_value_buffers(Mg: int, Mb: int, row: int, dev, what: str) -> None:
                            f"{free / 2**30:.2f} GiB of device memory is free")
 
 
+def _launch_mean_field(B: int, N: int, lg: _Lattice, lb: _Lattice, unary: torch.Tensor, Q: torch.Tensor,
+                       slots: Sequence[tuple], n_iter: int = MAX_ITER, label: Optional[torch.Tensor] = None,
+                       n_classes: int = 0) -> None:
+    """stego_crf_mean_field over B frames of N pixels: lg the position lattice of one frame (shared by the B frames), lb
+    the frames' bilateral lattice, unary / Q rows of 32 floats per slot.  slots: one or two probe slots in row order,
+    (n, marginals [B, n, N], argmax [B, N], int64 confusion), each output optional; the confusion counts are taken
+    against label ([B, N] as ops.probe_label gives it) for classes below n_classes.  The value buffers, [2, B * lg.M, row]
+    and [2, lb.M, row], are allocated here."""
+    (n0, q0, p0, c0), (n1, q1, p1, c1) = slots[0], (slots[1] if len(slots) == 2 else (0, None, None, None))
+    row = _LD * len(slots)
+    val_g = torch.empty(2, B * lg.M, row, dtype=torch.float32, device=unary.device)
+    val_b = torch.empty(2, lb.M, row, dtype=torch.float32, device=unary.device)
+    _lib.check(_lib.load().stego_crf_mean_field(
+        B, N, n0, n1, n_iter, _lib.ptr(unary), _lib.ptr(Q),
+        _lib.ptr(lg.offset), _lib.ptr(lg.bary), _lib.ptr(lg.rowptr), _lib.ptr(lg.slots), _lib.ptr(lg.n1), _lib.ptr(lg.n2),
+        _lib.ptr(lg.norm), lg.M,
+        _lib.ptr(lb.offset), _lib.ptr(lb.bary), _lib.ptr(lb.rowptr), _lib.ptr(lb.slots), _lib.ptr(lb.n1), _lib.ptr(lb.n2),
+        _lib.ptr(lb.norm), lb.M, float(POS_W), float(Bi_W),
+        _lib.ptr(val_g[0]), _lib.ptr(val_g[1]), _lib.ptr(val_b[0]), _lib.ptr(val_b[1]), _lib.ptr(q0), _lib.ptr(q1),
+        _lib.ptr(p0), _lib.ptr(p1), _lib.ptr(label), 0 if label is None else label.element_size(), n_classes,
+        _lib.ptr(c0), _lib.ptr(c1), _lib.stream()), "stego_crf_mean_field")
+
+
 _IMAGENET_STATS: Dict[torch.device, Tuple[torch.Tensor, torch.Tensor]] = {}
 
 
@@ -206,16 +229,7 @@ def mean_field(logits_full: torch.Tensor, image_u8: torch.Tensor, n_iter: int = 
     q_out = torch.empty(C, H, W, dtype=torch.float32, device=dev)
     arg = torch.empty(H, W, dtype=torch.uint8, device=dev) if want_argmax else None
     if n_iter > 0:
-        vg = torch.empty(2, lg.M, _LD, dtype=torch.float32, device=dev)
-        vb = torch.empty(2, lb.M, _LD, dtype=torch.float32, device=dev)
-        _lib.check(lib.stego_crf_mean_field(
-            1, N, C, 0, n_iter, _lib.ptr(unary), _lib.ptr(Q),
-            _lib.ptr(lg.offset), _lib.ptr(lg.bary), _lib.ptr(lg.rowptr), _lib.ptr(lg.slots), _lib.ptr(lg.n1),
-            _lib.ptr(lg.n2), _lib.ptr(lg.norm), lg.M,
-            _lib.ptr(lb.offset), _lib.ptr(lb.bary), _lib.ptr(lb.rowptr), _lib.ptr(lb.slots), _lib.ptr(lb.n1),
-            _lib.ptr(lb.n2), _lib.ptr(lb.norm), lb.M, float(POS_W), float(Bi_W),
-            _lib.ptr(vg[0]), _lib.ptr(vg[1]), _lib.ptr(vb[0]), _lib.ptr(vb[1]), _lib.ptr(q_out), 0, _lib.ptr(arg), 0,
-            0, 0, 0, 0, 0, _lib.stream()), "stego_crf_mean_field")
+        _launch_mean_field(1, N, lg, lb, unary, Q, [(C, q_out, arg, None)], n_iter)
     else:
         q_out.copy_(Q[:, :C].t().reshape(C, H, W))
         if want_argmax:

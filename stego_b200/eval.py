@@ -42,31 +42,25 @@ def fused_probe_log_probs(code: torch.Tensor, linear_probe: torch.nn.Module, clu
     H, W = int(size[0]), int(size[1])
     if code_flipped is not None:
         assert code_flipped.shape == code.shape
-    x, xf, ld, bf16 = _eval_codes(code, code_flipped)
-    wl, bl, cl = _probe_tables(linear_probe, cluster_probe, C)
-    n_lin, n_clu = wl.shape[0], cl.shape[0]
+    codes = _eval_codes(code, code_flipped)
+    tables = _probe_tables(linear_probe, cluster_probe, C)
+    n_lin, n_clu = tables[0].shape[0], tables[2].shape[0]
     dev = code.device
-    scratch = torch.empty(B * h * w, 80, dtype=torch.float32, device=dev)  # eval_probes.cu EV_LD
+    scratch = torch.empty(B * h * w, _EV_LD, dtype=torch.float32, device=dev)
     lin = torch.empty(B, n_lin, H, W, dtype=torch.float32, device=dev) if want_log_probs else None
     clu = torch.empty(B, n_clu, H, W, dtype=torch.float32, device=dev) if want_log_probs else None
     la = torch.empty(B, H, W, dtype=torch.uint8, device=dev) if want_argmax else None
     ca = torch.empty(B, H, W, dtype=torch.uint8, device=dev) if want_argmax else None
-    lab, lab_bytes, n_cls = None, 0, 0
+    lab = None
     if label is not None:
         _lib.require_cuda(label, linear_confusion, cluster_confusion)
-        lab, lab_bytes = ops.probe_label(label, B, H, W)
-        n_cls = n_lin
+        lab, _ = ops.probe_label(label, B, H, W)
         for t, n in ((linear_confusion, n_lin), (cluster_confusion, n_clu)):
             if t is not None:
-                assert t.dtype == torch.int64 and t.is_contiguous() and tuple(t.shape) == (n, n_cls)
+                assert t.dtype == torch.int64 and t.is_contiguous() and tuple(t.shape) == (n, n_lin)
         if linear_confusion is None and cluster_confusion is None:
             raise ValueError("label given without a confusion matrix to accumulate into")
-    entry = _lib.load().stego_eval_probes_bf16 if bf16 else _lib.load().stego_eval_probes
-    rc = entry(_lib.ptr(x), _lib.ptr(xf), ld, C, B, h, w, H, W, _lib.ptr(wl), _lib.ptr(bl), n_lin,
-                                       _lib.ptr(cl), n_clu, float(alpha), _lib.ptr(scratch), _lib.ptr(lin), _lib.ptr(clu),
-                                       _lib.ptr(la), _lib.ptr(ca), _lib.ptr(lab), lab_bytes, n_cls,
-                                       _lib.ptr(linear_confusion), _lib.ptr(cluster_confusion), _lib.stream())
-    _lib.check(rc, "stego_eval_probes_bf16" if bf16 else "stego_eval_probes")
+    _launch_probes(codes, tables, H, W, alpha, scratch, lin, clu, la, ca, lab, linear_confusion, cluster_confusion)
     if want_argmax:
         return lin, clu, la, ca
     return lin, clu
@@ -111,6 +105,44 @@ def _probe_tables(linear_probe: torch.nn.Module, cluster_probe: torch.nn.Module,
     bl = linear_probe.bias.detach().float().contiguous()
     cl = cluster_probe.clusters.detach().float().contiguous()
     return wl, bl, cl
+
+
+_EV_LD = 80  # eval_probes.cu EV_LD: floats per low-res pixel of the probe kernels' scratch
+
+
+def _launch_probes(codes, tables, H: int, W: int, alpha: float, scratch: torch.Tensor, lin_log_probs, clu_log_probs,
+                   lin_argmax, clu_argmax, label=None, lin_confusion=None, clu_confusion=None, mosaic=None) -> None:
+    """One stego_eval_probes[_mosaic][_bf16] pass, the entry picked from the code's dtype and the placement.  codes:
+    _eval_codes' (x, xf, ld, bf16) of a [B, C, h, w] code; tables: _probe_tables'; scratch [B*h*w, 80] fp32.  The
+    outputs are the caller's tensors, each optional: log-probabilities [B, n, H, W], argmax maps [B, H, W] uint8 and,
+    with label ([B, H, W] as ops.probe_label gives it), the int64 confusion counts.  mosaic: None for those frame
+    layouts, or (tile0, tile_rows, tiles_per_row, pitch): the outputs are mosaic planes (stego_eval_probes_mosaic)."""
+    x, xf, ld, bf16 = codes
+    wl, bl, cl = tables
+    B, C, h, w = x.shape
+    name = "stego_eval_probes" + ("_mosaic" if mosaic else "") + ("_bf16" if bf16 else "")
+    _lib.check(getattr(_lib.load(), name)(
+        _lib.ptr(x), _lib.ptr(xf), ld, C, B, h, w, H, W, _lib.ptr(wl), _lib.ptr(bl), wl.shape[0], _lib.ptr(cl),
+        cl.shape[0], float(alpha), _lib.ptr(scratch), _lib.ptr(lin_log_probs), _lib.ptr(clu_log_probs),
+        _lib.ptr(lin_argmax), _lib.ptr(clu_argmax), _lib.ptr(label), 0 if label is None else label.element_size(),
+        0 if label is None else wl.shape[0], _lib.ptr(lin_confusion), _lib.ptr(clu_confusion), *(mosaic or ()),
+        _lib.stream()), name)
+
+
+def _launch_crf_unary(codes, tables, H: int, W: int, alpha: float, scratch: torch.Tensor, unary: torch.Tensor,
+                      Q: torch.Tensor, mosaic=None, probes: int = 3) -> None:
+    """One stego_eval_crf_unary[_mosaic][_bf16] pass, the entry picked as in _launch_probes: the CRF's unary and initial
+    Q rows into the caller's unary / Q, [B*H*W, 64] fp32 for frames.  mosaic: (tile0, tile_rows, tiles_per_row, pitch),
+    the rows placed in a mosaic (stego_eval_crf_unary_mosaic), whose rows hold probes = 3 (both, 64 floats), 1 (the
+    linear probe, 32) or 2 (the cluster probe, 32)."""
+    x, xf, ld, bf16 = codes
+    wl, bl, cl = tables
+    B, C, h, w = x.shape
+    name = "stego_eval_crf_unary" + ("_mosaic" if mosaic else "") + ("_bf16" if bf16 else "")
+    _lib.check(getattr(_lib.load(), name)(
+        _lib.ptr(x), _lib.ptr(xf), ld, C, B, h, w, H, W, _lib.ptr(wl), _lib.ptr(bl), wl.shape[0], _lib.ptr(cl),
+        cl.shape[0], float(alpha), _lib.ptr(scratch), _lib.ptr(unary), _lib.ptr(Q),
+        *((probes, *mosaic) if mosaic else ()), _lib.stream()), name)
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -189,39 +221,38 @@ def fused_eval_crf(code: torch.Tensor, linear_probe: torch.nn.Module, cluster_pr
     seen (its cached position lattice).  Everything is checked before the first launch."""
     B, C, h, w, H, W, n_lin, n_clu = _check_crf_args(code, linear_probe, cluster_probe, img, code_flipped, label,
                                                       linear_confusion, cluster_confusion)
-    lib = _lib.load()
     dev = code.device
-    N = H * W
-    x, xf, ld, bf16 = _eval_codes(code, code_flipped)
-    wl, bl, cl = _probe_tables(linear_probe, cluster_probe, C)
-    scratch = torch.empty(B * h * w, 80, dtype=torch.float32, device=dev)  # eval_probes.cu EV_LD
-    unary = torch.empty(B * N, _CRF_LD, dtype=torch.float32, device=dev)
-    Q = torch.empty(B * N, _CRF_LD, dtype=torch.float32, device=dev)
-    name = "stego_eval_crf_unary_bf16" if bf16 else "stego_eval_crf_unary"
-    _lib.check(getattr(lib, name)(_lib.ptr(x), _lib.ptr(xf), ld, C, B, h, w, H, W, _lib.ptr(wl), _lib.ptr(bl), n_lin,
-                                  _lib.ptr(cl), n_clu, float(alpha), _lib.ptr(scratch), _lib.ptr(unary), _lib.ptr(Q),
-                                  _lib.stream()), name)
-    lg = crf._position_lattice(H, W, dev)
-    lb = crf._bilateral_lattice(crf.prepare_image(frame) for frame in img.detach())
-    val_g = torch.empty(2, B * lg.M, _CRF_LD, dtype=torch.float32, device=dev)
-    val_b = torch.empty(2, lb.M, _CRF_LD, dtype=torch.float32, device=dev)
     lin_pred = torch.empty(B, H, W, dtype=torch.uint8, device=dev)
     clu_pred = torch.empty(B, H, W, dtype=torch.uint8, device=dev)
     lin_q = torch.empty(B, n_lin, H, W, dtype=torch.float32, device=dev) if want_marginals else None
     clu_q = torch.empty(B, n_clu, H, W, dtype=torch.float32, device=dev) if want_marginals else None
-    lab, lab_bytes = (None, 0) if label is None else ops.probe_label(label, B, H, W)
-    _lib.check(lib.stego_crf_mean_field(
-        B, N, n_lin, n_clu, crf.MAX_ITER, _lib.ptr(unary), _lib.ptr(Q),
-        _lib.ptr(lg.offset), _lib.ptr(lg.bary), _lib.ptr(lg.rowptr), _lib.ptr(lg.slots), _lib.ptr(lg.n1), _lib.ptr(lg.n2),
-        _lib.ptr(lg.norm), lg.M,
-        _lib.ptr(lb.offset), _lib.ptr(lb.bary), _lib.ptr(lb.rowptr), _lib.ptr(lb.slots), _lib.ptr(lb.n1), _lib.ptr(lb.n2),
-        _lib.ptr(lb.norm), lb.M, float(crf.POS_W), float(crf.Bi_W),
-        _lib.ptr(val_g[0]), _lib.ptr(val_g[1]), _lib.ptr(val_b[0]), _lib.ptr(val_b[1]), _lib.ptr(lin_q), _lib.ptr(clu_q),
-        _lib.ptr(lin_pred), _lib.ptr(clu_pred), _lib.ptr(lab), lab_bytes, n_lin if label is not None else 0,
-        _lib.ptr(linear_confusion), _lib.ptr(cluster_confusion), _lib.stream()), "stego_crf_mean_field")
+    lab = None if label is None else ops.probe_label(label, B, H, W)[0]
+    _crf_pass(_eval_codes(code, code_flipped), _probe_tables(linear_probe, cluster_probe, C), img, alpha, lin_pred,
+              clu_pred, lin_q, clu_q, lab, linear_confusion, cluster_confusion)
     if want_marginals:
         return lin_pred, clu_pred, lin_q, clu_q
     return lin_pred, clu_pred
+
+
+def _crf_pass(codes, tables, img: torch.Tensor, alpha: float, lin_pred, clu_pred, lin_q, clu_q, label=None,
+              lin_confusion=None, clu_confusion=None) -> None:
+    """fused_eval_crf's work on checked arguments, into the caller's outputs (marginals and confusion counts optional):
+    both probes' unary rows of the B frames img [B, 3, H, W], their lattices (one host sync per frame) and one mean
+    field.  codes, tables and label as in _launch_probes."""
+    B, _, H, W = img.shape
+    N = H * W
+    _, _, h, w = codes[0].shape
+    dev = codes[0].device
+    scratch = torch.empty(B * h * w, _EV_LD, dtype=torch.float32, device=dev)
+    unary = torch.empty(B * N, _CRF_LD, dtype=torch.float32, device=dev)
+    Q = torch.empty(B * N, _CRF_LD, dtype=torch.float32, device=dev)
+    _launch_crf_unary(codes, tables, H, W, alpha, scratch, unary, Q)
+    lg = crf._position_lattice(H, W, dev)
+    lb = crf._bilateral_lattice(crf.prepare_image(frame) for frame in img.detach())
+    n_lin, n_clu = tables[0].shape[0], tables[2].shape[0]
+    crf._launch_mean_field(B, N, lg, lb, unary, Q, [(n_lin, lin_q, lin_pred, lin_confusion),
+                                                    (n_clu, clu_q, clu_pred, clu_confusion)],
+                           label=label, n_classes=0 if label is None else n_lin)
 
 
 class UnsupervisedMetrics:

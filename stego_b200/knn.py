@@ -30,18 +30,13 @@ def knn_topk(feats: torch.Tensor, k: int = 30, return_values: bool = False,
         raise RuntimeError("stego_b200.knn_topk: feats must be a 2-D fp32 tensor")
     feats = feats.contiguous()
     n, E = feats.shape
-    if devs is not None:
-        if n < 1 or E < 1 or E % 64 or not 1 <= k <= min(32, n):
-            raise ValueError(f"knn_topk: n={n}, E={E}, k={k} unsupported (E a positive multiple of 64, 1 <= k <= "
-                             f"min(32, n))")
-        ranges = split(n, len(devs), KNN_ROW_BLOCK)
-        return _knn_topk_sharded(feats, k, return_values, [(d, r0, r1) for d, (r0, r1) in zip(devs, ranges)])
-    planes = torch.empty(2, n, E, dtype=torch.bfloat16, device=feats.device)
-    idx = torch.empty(n, k, dtype=torch.long, device=feats.device)
-    vals = torch.empty(n, k, dtype=torch.float32, device=feats.device) if return_values else None
-    rc = _lib.load().stego_knn_topk(_lib.ptr(feats), n, E, k, _lib.ptr(planes), _lib.ptr(idx), _lib.ptr(vals), _lib.stream())
-    _lib.check(rc, "stego_knn_topk")
-    return idx, vals
+    # several devices are refused here, before any launch; on one device the C entries refuse bad sizes themselves
+    if devs is not None and (n < 1 or E < 1 or E % 64 or not 1 <= k <= min(32, n)):
+        raise ValueError(f"knn_topk: n={n}, E={E}, k={k} unsupported (E a positive multiple of 64, 1 <= k <= "
+                         f"min(32, n))")
+    devs = devs or [feats.device]
+    ranges = split(n, len(devs), KNN_ROW_BLOCK)
+    return _knn_topk_sharded(feats, k, return_values, [(d, r0, r1) for d, (r0, r1) in zip(devs, ranges)])
 
 
 def _knn_topk_sharded(feats: torch.Tensor, k: int, return_values: bool, shards: List[Tuple[torch.device, int, int]]
@@ -108,16 +103,13 @@ def precompute_knns(net, batches, k: int = 30, devices: Optional[Sequence[Device
     the exception is a net in training mode with cfg.dropout, whose Dropout2d noise each device draws from its own
     generator (as nn.DataParallel does)."""
     primary = next(net.parameters()).device
-    devs = check_devices(devices, primary, "precompute_knns")
+    devs = check_devices(devices, primary, "precompute_knns") or [primary]
     feats = []
     for i, pack in enumerate(batches):
         img = pack["img"] if isinstance(pack, dict) else pack
-        if devs is None:
-            feats.append(knn_descriptors(net, img.to(primary)))
-            continue
-        dev = devs[i % len(devs)]
-        with torch.cuda.device(dev):
-            feats.append(knn_descriptors(net, img.to(dev)).to(primary))
+        img = img.to(devs[i % len(devs)])
+        with torch.cuda.device_of(img):
+            feats.append(knn_descriptors(net, img).to(primary))
     idx, _ = knn_topk(torch.cat(feats, 0), k, devices=devs)
     return idx
 

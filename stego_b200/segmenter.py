@@ -691,7 +691,8 @@ class LitUnsupervisedSegmenter(nn.Module):
         The frame and its mirror go through the frozen ViT as one batch of 2B, the mirrored frames read in place by the
         patchify kernel and the whole backbone replayed as one CUDA graph per frame shape (cached beside the training
         step's graphs, never replacing them).  The eval-mode head (no dropout noise) runs once over the 2B rows, then
-        fused_probe_log_probs (or fused_eval_crf with run_crf) takes the two halves of the code as code / code_flipped.
+        the probe pass of fused_probe_log_probs (or that of fused_eval_crf with run_crf) takes the two halves of the code
+        as code / code_flipped and writes the returned tensors in place.
 
         Returns dict(linear_preds, cluster_preds), uint8 [B, H', W'] on the device; with want_probs also
         linear_probs / cluster_probs fp32 [B, n, H', W']: the log-probabilities without CRF, the CRF marginals with it.
@@ -712,35 +713,10 @@ class LitUnsupervisedSegmenter(nn.Module):
         out from the calling thread, device after device; the host synchronises only where the single-device call does
         (once per frame with run_crf)."""
         img, label = batch["img"], batch.get("label")
-        devs = self._check_devices(devices, img, "eval_step")
+        devs = self._check_devices(devices, img, "eval_step") or [img.device]
         self._check_eval_args(img, label, run_crf)
-        if devs is not None:
-            return self._eval_step_sharded(img, label, run_crf, want_probs,
-                                           [(d, b0, b1) for d, (b0, b1) in zip(devs, split(img.shape[0], len(devs)))])
-        from .eval import fused_eval_crf, fused_probe_log_probs
-        self.flush()
-        net = self.net
-        B, fh, fw = img.shape[0], img.shape[2] // net.patch_size, img.shape[3] // net.patch_size
-        stats = dict(linear_confusion=self.test_linear_metrics.stats, cluster_confusion=self.test_cluster_metrics.stats) \
-            if label is not None else {}
-        with self._net_in_eval_mode(), torch.no_grad():
-            tok = net.backbone_tokens(img, use_graph=getattr(self.cfg, "cuda_graph", True), mirror=True)  # [2B, hw, E]
-            code_all = net.eval_code(tok, fh, fw)  # [2B, dim, h, w]
-            code, code_flipped = code_all[:B], code_all[B:]
-            if run_crf:
-                out = fused_eval_crf(code, self.linear_probe, self.cluster_probe, img, 2.0, code_flipped=code_flipped,
-                                     label=label, want_marginals=want_probs, **stats)
-                preds, probs = out[:2], out[2:]
-            else:
-                size = label.shape[-2:] if label is not None else img.shape[-2:]
-                out = fused_probe_log_probs(code, self.linear_probe, self.cluster_probe, size, 2.0,
-                                            want_log_probs=want_probs, want_argmax=True, code_flipped=code_flipped,
-                                            label=label, **stats)
-                preds, probs = out[2:], out[:2]
-        result = dict(linear_preds=preds[0], cluster_preds=preds[1])
-        if want_probs:
-            result.update(linear_probs=probs[0], cluster_probs=probs[1])
-        return result
+        return self._eval_step_sharded(img, label, run_crf, want_probs,
+                                       [(d, b0, b1) for d, (b0, b1) in zip(devs, split(img.shape[0], len(devs)))])
 
     def _check_devices(self, devices, img, who: str):
         """check_devices against the inputs' device, which must also be the model's."""
@@ -764,13 +740,14 @@ class LitUnsupervisedSegmenter(nn.Module):
         return head, lin, clu
 
     def _eval_step_sharded(self, img, label, run_crf: bool, want_probs: bool, shards) -> Dict[str, torch.Tensor]:
-        """eval_step over frame slices [b0, b1), one per (device, b0, b1) entry, the first entry on img's device.  Every
-        device first runs the backbone and the head on its slice, then the probes (or the CRF, whose per-frame host
-        synchronisations then find the other devices' backbones already running), and copies its outputs and counts to
-        the first device on the devices' current streams.  With the CRF, each frame's lattice build still waits on the
-        host for its device, and these waits run one after another on the calling thread: only the devices' GPU work
-        overlaps."""
-        from .eval import fused_eval_crf, fused_probe_log_probs
+        """eval_step, its arguments checked, over frame slices [b0, b1), one per (device, b0, b1) entry, the first entry
+        on img's device.  Every device first runs the backbone and the head on its slice, then the probes (or the CRF,
+        whose per-frame host synchronisations then find the other devices' backbones already running).  The first
+        entry's kernels write its slice of the outputs and the confusion counts in place; every other device writes
+        outputs and counts of its own, copied to the first device on the devices' current streams.  With the CRF, each
+        frame's lattice build still waits on the host for its device, and these waits run one after another on the
+        calling thread: only the devices' GPU work overlaps."""
+        from .eval import _crf_pass, _EV_LD, _eval_codes, _launch_probes, _probe_tables
         self.flush()
         net = self.net
         primary = img.device
@@ -780,7 +757,7 @@ class LitUnsupervisedSegmenter(nn.Module):
         lab_all = label.reshape(B, *size) if label is not None else None
         preds = [torch.empty(B, *size, dtype=torch.uint8, device=primary) for _ in range(2)]
         probs = [torch.empty(B, n, *size, dtype=torch.float32, device=primary) for n in (n_lin, n_clu)] \
-            if want_probs else []
+            if want_probs else [None, None]
         metrics = (self.test_linear_metrics, self.test_cluster_metrics)
         use_graph = getattr(self.cfg, "cuda_graph", True)
         work = []
@@ -797,28 +774,30 @@ class LitUnsupervisedSegmenter(nn.Module):
                     code_all = net.eval_code(tok, fh, fw, head)
                     if any(d == dev for d, c0, c1 in shards[i + 1:] if c1 > c0):
                         code_all = code_all.clone()  # the graph's output buffer is reused by the next slice's replay
-                    stats = {}
+                    conf = [None, None]
                     if label is not None:
                         conf = [m.stats if first else torch.zeros_like(m.stats, device=dev) for m in metrics]
-                        stats = dict(linear_confusion=conf[0], cluster_confusion=conf[1])
-                    work.append((first, dev, b0, b1, x, lab, code_all, lin, clu, stats))
-            for first, dev, b0, b1, x, lab, code_all, lin, clu, stats in work:
+                    work.append((first, dev, b0, b1, x, lab, code_all, lin, clu, conf))
+            for first, dev, b0, b1, x, lab, code_all, lin, clu, conf in work:
                 with torch.cuda.device(dev):
-                    code, code_flipped = code_all[:b1 - b0], code_all[b1 - b0:]
+                    n = b1 - b0
+                    outs = [t if t is None else t[b0:b1] for t in (*preds, *probs)]  # this slice's outputs
+                    dst = outs if first else [t if t is None else torch.empty_like(t, device=dev) for t in outs]
+                    codes = _eval_codes(code_all[:n], code_all[n:])
+                    tables = _probe_tables(lin, clu, net.dim)
+                    lab = None if lab is None else ops.probe_label(lab, n, *size)[0]
                     if run_crf:
-                        out = fused_eval_crf(code, lin, clu, x, 2.0, code_flipped=code_flipped, label=lab,
-                                             want_marginals=want_probs, **stats)
-                        p, q = out[:2], out[2:]
+                        _crf_pass(codes, tables, x, 2.0, *dst, lab, *conf)
                     else:
-                        out = fused_probe_log_probs(code, lin, clu, size, 2.0, want_log_probs=want_probs,
-                                                    want_argmax=True, code_flipped=code_flipped, label=lab, **stats)
-                        p, q = out[2:], out[:2]
-                    for k in range(2):
-                        preds[k][b0:b1].copy_(p[k])
-                        if want_probs:
-                            probs[k][b0:b1].copy_(q[k])
-                    if stats and not first:
-                        for m, c in zip(metrics, (stats["linear_confusion"], stats["cluster_confusion"])):
+                        scratch = torch.empty(n * fh * fw, _EV_LD, dtype=torch.float32, device=dev)
+                        _launch_probes(codes, tables, *size, 2.0, scratch, *dst[2:], *dst[:2], lab, *conf)
+                    if first:
+                        continue
+                    for t, s in zip(outs, dst):
+                        if t is not None:
+                            t.copy_(s)
+                    if label is not None:
+                        for m, c in zip(metrics, conf):
                             m.stats.add_(c.to(primary))
         result = dict(linear_preds=preds[0], cluster_preds=preds[1])
         if want_probs:
@@ -867,12 +846,10 @@ class LitUnsupervisedSegmenter(nn.Module):
         matrices are bit-equal to the single-device call.  With run_crf the one mean field over the mosaic still runs
         on the first device alone; it is most of a large cluster-only scene's time (DESIGN.md §10), which bounds
         what more devices gain there."""
-        devs = self._check_devices(devices, tiles, "eval_scene")
+        devs = self._check_devices(devices, tiles, "eval_scene") or [tiles.device]
         R, C, n_tiles, H, W, probes = self._check_scene_args(tiles, grid, label, run_crf, probes, map_clusters, chunk)
-        dev = tiles.device
-        bands = [(dev, 0, R)] if devs is None else [(d, r0, r1) for d, (r0, r1) in zip(devs, split(R, len(devs)))]
         return self._eval_scene_bands(tiles, label, run_crf, probes, want_probs, map_clusters, chunk, R, C, n_tiles, H,
-                                      W, bands)
+                                      W, [(d, r0, r1) for d, (r0, r1) in zip(devs, split(R, len(devs)))])
 
     def _eval_scene_bands(self, tiles, label, run_crf, probes, want_probs, map_clusters, chunk, R, C, n_tiles, H, W,
                           bands) -> Dict[str, torch.Tensor]:
@@ -880,10 +857,9 @@ class LitUnsupervisedSegmenter(nn.Module):
         device and writing the mosaic in place, every other one into a staging band of its own that is copied into the
         first device's mosaic."""
         from . import crf
-        from .eval import _eval_codes, _probe_tables
+        from .eval import _EV_LD, _eval_codes, _launch_crf_unary, _launch_probes, _probe_tables
         self.flush()
         tiles = tiles.detach().contiguous()
-        lib = _lib.load()
         net = self.net
         dev = tiles.device
         p = net.patch_size
@@ -915,13 +891,12 @@ class LitUnsupervisedSegmenter(nn.Module):
                     band_tiles = tiles[bt0:bt1] if first else tiles[bt0:bt1].to(d)
                     dst = full if first else mosaic(d, r1 - r0)
                     head, lin_p, clu_p = self._device_params(d, first)
-                    wl, bl, cl = _probe_tables(lin_p, clu_p, net.dim)
-                    scratch = torch.empty(min(chunk, bt1 - bt0) * h * w, 80, dtype=torch.float32, device=d)  # EV_LD
+                    tables = _probe_tables(lin_p, clu_p, net.dim)
+                    scratch = torch.empty(min(chunk, bt1 - bt0) * h * w, _EV_LD, dtype=torch.float32, device=d)
                     stats = {k: None for k in ("linear", "cluster")}
-                    lab, lab_bytes = None, 0
+                    lab = None
                     if label is not None and not run_crf:
-                        lab, lab_bytes = ops.probe_label(label[bt0:bt1] if first else label[bt0:bt1].to(d),
-                                                         bt1 - bt0, H, W)
+                        lab, _ = ops.probe_label(label[bt0:bt1] if first else label[bt0:bt1].to(d), bt1 - bt0, H, W)
                         stats = {k: (metrics[k].stats if first else torch.zeros_like(metrics[k].stats, device=d))
                                  if k in probes else None for k in stats}
                     for c0 in range(0, bt1 - bt0, chunk):
@@ -930,24 +905,16 @@ class LitUnsupervisedSegmenter(nn.Module):
                         t0 = c0 if not first else bt0 + c0  # tile index within the band's mosaic rows
                         tok = net.backbone_tokens(img, use_graph=use_graph, mirror=True)
                         code_all = net.eval_code(tok, h, w, head)  # [2B, dim, h, w]
-                        x, xf, ld, bf16 = _eval_codes(code_all[:B], code_all[B:])
-                        sfx = "_bf16" if bf16 else ""
-                        rows_here = R if first else r1 - r0
+                        codes = _eval_codes(code_all[:B], code_all[B:])
+                        placement = (t0, R if first else r1 - r0, C, WW)
                         if run_crf:
-                            _lib.check(getattr(lib, "stego_eval_crf_unary_mosaic" + sfx)(
-                                _lib.ptr(x), _lib.ptr(xf), ld, net.dim, B, h, w, H, W, _lib.ptr(wl), _lib.ptr(bl), n_lin,
-                                _lib.ptr(cl), n_clu, 2.0, _lib.ptr(scratch), _lib.ptr(dst["unary"]), _lib.ptr(dst["Q"]),
-                                int(lin_on) + 2 * int(clu_on), t0, rows_here, C, WW, _lib.stream()),
-                                "stego_eval_crf_unary_mosaic" + sfx)
+                            _launch_crf_unary(codes, tables, H, W, 2.0, scratch, dst["unary"], dst["Q"], placement,
+                                              probes=int(lin_on) + 2 * int(clu_on))
                         else:
-                            _lib.check(getattr(lib, "stego_eval_probes_mosaic" + sfx)(
-                                _lib.ptr(x), _lib.ptr(xf), ld, net.dim, B, h, w, H, W, _lib.ptr(wl), _lib.ptr(bl), n_lin,
-                                _lib.ptr(cl), n_clu, 2.0, _lib.ptr(scratch), _lib.ptr(dst["probs"].get("linear")),
-                                _lib.ptr(dst["probs"].get("cluster")), _lib.ptr(dst["preds"].get("linear")),
-                                _lib.ptr(dst["preds"].get("cluster")), _lib.ptr(lab[c0:] if lab is not None else None),
-                                lab_bytes, n_lin if lab is not None else 0, _lib.ptr(stats["linear"]),
-                                _lib.ptr(stats["cluster"]), t0, rows_here, C, WW, _lib.stream()),
-                                "stego_eval_probes_mosaic" + sfx)
+                            _launch_probes(codes, tables, H, W, 2.0, scratch, dst["probs"].get("linear"),
+                                           dst["probs"].get("cluster"), dst["preds"].get("linear"),
+                                           dst["preds"].get("cluster"), None if lab is None else lab[c0:],
+                                           stats["linear"], stats["cluster"], placement)
                     if first:
                         continue
                     y0, y1 = r0 * H, r1 * H  # the band's mosaic rows: one contiguous block per plane
@@ -961,38 +928,24 @@ class LitUnsupervisedSegmenter(nn.Module):
                                 full["probs"][k][c, y0:y1].copy_(dst["probs"][k][c])
                             if stats[k] is not None:
                                 metrics[k].stats.add_(stats[k].to(dev))
-        lin_stats = self.test_linear_metrics.stats if label is not None and lin_on else None
-        clu_stats = self.test_cluster_metrics.stats if label is not None and clu_on else None
-        if run_crf:
-            unary, Q = full["unary"], full["Q"]
-        else:
-            preds, probs = full["preds"], full["probs"]
         if run_crf:
             image = crf.prepare_image(tiles.view(R, C, 3, H, W).permute(2, 0, 3, 1, 4).reshape(3, HH, WW))
             lg = crf._position_lattice(HH, WW, dev, cache=n_tiles == 1)
             lb = crf._bilateral_lattice([image])
             crf.check_value_buffers(lg.M, lb.M, row, dev, "eval_scene")
-            val_g = torch.empty(2, lg.M, row, dtype=torch.float32, device=dev)
-            val_b = torch.empty(2, lb.M, row, dtype=torch.float32, device=dev)
-            lab, lab_bytes = (None, 0)
+            lab = None
             if label is not None:
-                lab, lab_bytes = ops.probe_label(label.reshape(R, C, H, W).permute(0, 2, 1, 3), 1, HH, WW)
+                lab, _ = ops.probe_label(label.reshape(R, C, H, W).permute(0, 2, 1, 3), 1, HH, WW)
             preds = {k: torch.empty(HH, WW, dtype=torch.uint8, device=dev) for k in probes}
             probs = {k: torch.empty(n, HH, WW, dtype=torch.float32, device=dev)
                      for k, n in (("linear", n_lin), ("cluster", n_clu)) if k in probes} if want_probs else {}
-            # the mean field's two probe slots in row order; one probe (either) takes the first slot
-            slots = [(k, n, st) for k, n, st in (("linear", n_lin, lin_stats), ("cluster", n_clu, clu_stats)) if k in probes]
-            (first, n0, conf0), (second, n1, conf1) = slots[0], (slots[1] if len(slots) == 2 else (None, 0, None))
-            _lib.check(lib.stego_crf_mean_field(
-                1, HH * WW, n0, n1, crf.MAX_ITER, _lib.ptr(unary), _lib.ptr(Q),
-                _lib.ptr(lg.offset), _lib.ptr(lg.bary), _lib.ptr(lg.rowptr), _lib.ptr(lg.slots), _lib.ptr(lg.n1),
-                _lib.ptr(lg.n2), _lib.ptr(lg.norm), lg.M,
-                _lib.ptr(lb.offset), _lib.ptr(lb.bary), _lib.ptr(lb.rowptr), _lib.ptr(lb.slots), _lib.ptr(lb.n1),
-                _lib.ptr(lb.n2), _lib.ptr(lb.norm), lb.M, float(crf.POS_W), float(crf.Bi_W),
-                _lib.ptr(val_g[0]), _lib.ptr(val_g[1]), _lib.ptr(val_b[0]), _lib.ptr(val_b[1]),
-                _lib.ptr(probs.get(first)), _lib.ptr(probs.get(second)), _lib.ptr(preds[first]),
-                _lib.ptr(preds.get(second)), _lib.ptr(lab), lab_bytes, n_lin if lab is not None else 0,
-                _lib.ptr(conf0), _lib.ptr(conf1), _lib.stream()), "stego_crf_mean_field")
+            # the mean field's probe slots in row order; one probe (either) takes the first slot
+            slots = [(n, probs.get(k), preds[k], None if lab is None else metrics[k].stats)
+                     for k, n in (("linear", n_lin), ("cluster", n_clu)) if k in probes]
+            crf._launch_mean_field(1, HH * WW, lg, lb, full["unary"], full["Q"], slots, label=lab,
+                                   n_classes=0 if lab is None else n_lin)
+        else:
+            preds, probs = full["preds"], full["probs"]
         for k in probes:
             out[f"{k}_preds"] = preds[k]
             if want_probs:
