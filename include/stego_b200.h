@@ -237,6 +237,27 @@ STEGO_API int stego_aug_views(const float* img, long long stride_b, long long st
                               float* img_aug, float* coord_aug, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Loader frames and labels (src/utils.py:165-183 get_transform: Resize(res, NEAREST), CenterCrop(res), then ToTensor +
+ * Normalize or ToTargetTensor and a data set's remap) from decoded images of any size, one launch each.
+ * staging: one buffer of `bytes` bytes, built by the host (stego_b200/frames.py):
+ *   bytes [0, 32 B): int64 records [B][4] = {byte offset of the image in staging, H, W, first table word};
+ *   bytes [32 B, 32 B + 4 table_words): int32 tables, per record res source rows then res source columns (Pillow's
+ *     nearest-neighbour index with the crop offset folded in; -1 = Pillow's fill value 0);
+ *   after them the images, uint8 row-major: H x W x 3 RGB (frames) or H x W (labels), each at its record's offset.
+ * staging_host: a host copy of at least the records and tables, read to check every record, table entry and image
+ * extent before the launch; staging_dev: the device copy (8-byte aligned) the kernel reads.  B 1..65535, res 1..8192,
+ * H, W 1..2^20; out 16-byte aligned.  The host reads nothing back and the call never synchronises. */
+/* out fp32 [B][3][res][res] = ((float)x / 255 - mean[c]) / std[c] of the gathered byte, each operation an IEEE fp32
+ * division / subtraction (torchvision's ToTensor then Normalize on the CPU, bit for bit). */
+STEGO_API int stego_frames_rgb8(const void* staging_host, const void* staging_dev, long long bytes,
+                                long long table_words, int B, int res, float mean0, float mean1, float mean2,
+                                float std0, float std1, float std2, float* out, void* stream);
+/* out int64 [B][res][res] = lut[id] of the gathered label byte, or id itself when lut is null.  lut: device int64 [256],
+ * 8-byte aligned. */
+STEGO_API int stego_labels_u8(const void* staging_host, const void* staging_dev, long long bytes,
+                              long long table_words, int B, int res, const long long* lut, long long* out, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * TensorBoard histograms (SummaryWriter.add_histogram with its default bins="tensorflow")
  * ---------------------------------------------------------------------------------------------- */
 /* The 1549 float64 bucket edges of torch's SummaryWriter.default_bins (edges, may be null) and the 1550 fp32
