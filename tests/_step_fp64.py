@@ -1,7 +1,8 @@
 """The training-step configurations the hand-scheduled step accepts beyond the shipped one (ROWS) and its optional modes
-alone and crossed with them (MODE_ROWS), their model and batch builders, and the float64 composition of one training
-step from the existing references, shared by tests/test_step_configs_fp64_gpu.py, tests/test_step_modes_fp64_gpu.py and
-tests/test_step_fp64_reference.py.
+alone and crossed with them (MODE_ROWS), both with the reconstruction and CRF terms (REC_CRF_ROWS), their model and
+batch builders, and the float64 composition of one training
+step from the existing references, shared by tests/test_step_configs_fp64_gpu.py, tests/test_step_modes_fp64_gpu.py,
+tests/test_step_rec_crf_fp64_gpu.py and tests/test_step_fp64_reference.py.
 
 The composition chains the stage references: _head_fp64.head_forward (cluster1 + cluster2, or cluster1 alone for the
 linear head), _corr_fp64.CorrRef (the correspondence loss on the returned features, Dropout2d-scaled by the third noise
@@ -98,9 +99,69 @@ MODE_ROWS = {
 }
 MODE_CONFIGS = {name: {**BASE, "labels": "int64", "masks": None, "hist": False, **row} for name, row in MODE_ROWS.items()}
 
-HEAD = ["net.cluster1.0.weight", "net.cluster1.0.bias", "net.cluster2.0.weight", "net.cluster2.0.bias",
+# The reconstruction and CRF terms (cfg.fused_rec_crf) on ROWS' configurations and the modes: each base row with the
+# reconstruction term alone ("rec"), the CRF term alone ("crf") and both ("both"); the CRF term only where its kernels
+# take the code (at most 80 channels), and crf_samples rows only with it.
+REC, CRF = dict(rec_weight=0.7, fused_rec_crf=True), dict(crf_weight=0.5, fused_rec_crf=True)
+_REC_CRF_BASE = {
+    "plain": {},
+    "no_dropout": dict(cfg=dict(dropout=False)),          # m3 = None in the reconstruction kernels
+    "linear_no_dropout": dict(cfg=dict(projection_type="linear", dropout=False)),
+    "linear_head": dict(cfg=dict(projection_type="linear")),
+    "dim1": dict(cfg=dict(dim=1)),
+    "dim27": dict(cfg=dict(dim=27)),
+    "dim65": dict(cfg=dict(dim=65)),
+    "dim80": dict(cfg=dict(dim=80)),                      # the most channels the CRF kernels take
+    "dim96": dict(cfg=dict(dim=96)),                      # reconstruction only
+    "patch16_s": dict(patch=16),                          # 14 x 14 code: the CRF resize upsamples 4x
+    "patch16_b": dict(arch="vit_base", patch=16, frame=(320, 320)),
+    "vitb8_320": dict(arch="vit_base", frame=(320, 320)),  # 40 x 40 code, E = 768
+    "nonsquare": dict(frame=(224, 320)),                  # 28 x 40 code: scale_h != scale_w
+    "nonsquare_labels": dict(frame=(224, 320), label=(112, 150)),
+    "B1": dict(B=1),
+    "B3": dict(B=3),
+    "neg_max": dict(cfg=dict(neg_samples=14)),
+    "extra6": dict(cfg=dict(extra_clusters=6)),
+    "classes32_extra32": dict(n_classes=32, cfg=dict(extra_clusters=32)),
+    "fs16": dict(cfg=dict(feature_samples=16)),
+    "fs28_neg14": dict(cfg=dict(feature_samples=28, neg_samples=14)),
+    "tl": dict(cfg=TL),
+    "sal": dict(masks="fp32", cfg=SAL),
+    "kk": dict(cfg=KK),
+    "aug": dict(cfg=AUG),                                 # the aug scatter shares the img rows' accumulators
+    "hist": dict(hist=True, cfg={}),                      # the histogram graph replays with the terms
+    "crf_samples1": dict(cfg=dict(crf_samples=1)),
+    "crf_samples64": dict(cfg=dict(crf_samples=64)),      # one full 64-sample tile
+    "crf_samples65": dict(cfg=dict(crf_samples=65)),      # a second tile with one sample
+    "everything": dict(B=3, masks="fp32", hist=True, terms=("both",),
+                       cfg=dict(KK, **TL, **SAL, **AUG, feature_samples=16, dim=27)),
+}
+
+
+def _rec_crf_rows():
+    rows = {}
+    for name, row in _REC_CRF_BASE.items():
+        row = dict(row)
+        cfg, only = row.pop("cfg", {}), row.pop("terms", None)
+        for terms, over in (("rec", REC), ("crf", CRF), ("both", dict(REC, **CRF))):
+            if only is not None and terms not in only:
+                continue
+            if "crf_weight" in over and cfg.get("dim", 70) > 80:
+                continue
+            if "crf_weight" not in over and "crf_samples" in cfg:
+                continue
+            rows[f"{name}_{terms}"] = dict(row, cfg=dict(cfg, **over))
+    return rows
+
+
+REC_CRF_ROWS = _rec_crf_rows()
+REC_CRF_CONFIGS = {name: {**BASE, "labels": "int64", "masks": None, "hist": False, **row}
+                   for name, row in REC_CRF_ROWS.items()}
+
+HEAD =["net.cluster1.0.weight", "net.cluster1.0.bias", "net.cluster2.0.weight", "net.cluster2.0.bias",
         "net.cluster2.2.weight", "net.cluster2.2.bias"]
 PROBES = ["linear_probe.weight", "linear_probe.bias", "cluster_probe.clusters"]
+DECODER = ["decoder.weight", "decoder.bias"]
 
 
 def make_model(row, dev, fused=True, seed=0):
@@ -146,9 +207,10 @@ def make_batch(row, dev, seed=1):
 
 
 def names_of(model):
-    """the trainable parameters of the step, in NAMES order (the linear head has no cluster2)"""
+    """the trainable parameters of the step, in NAMES order (the linear head has no cluster2), then the decoder when
+    the reconstruction term trains it"""
     have = dict(model.named_parameters())
-    return [k for k in HEAD + PROBES if k in have]
+    return [k for k in HEAD + PROBES if k in have] + (DECODER if model.cfg.rec_weight > 0 else [])
 
 
 def loss_cfg(cfg):

@@ -44,6 +44,38 @@ def test_supported_truth_table():
         assert m.supported(_batch(seed=False)) and m.supported(_batch(seed=False, dtype=torch.bfloat16))
 
 
+def test_rec_crf_rows_take_the_fused_step(monkeypatch):
+    """Every batch of tests/_step_fp64.py's REC_CRF_ROWS goes to the fused step, so the GPU rows check the kernels they
+    name; a configuration the step refuses belongs with the refusals above.  The salience rows' masks are CPU tensors
+    here: their check stands in for salience.masks_supported (the mode rows test the real one on the GPU) and only
+    asserts the [B, 1, H, W] frame-sized pair."""
+    import _step_fp64 as S
+    from stego_b200 import fused_step
+    from stego_b200.config import make_cfg
+    from stego_b200.segmenter import LitUnsupervisedSegmenter
+    from test_aug_step import _CudaImg
+
+    def masks_ok(mask, mask_pos, B, device):
+        return tuple(mask.shape) == tuple(mask_pos.shape) == (B, 1) + tuple(frame)
+    monkeypatch.setattr(fused_step.salience, "masks_supported", masks_ok)
+    assert {n.rsplit("_", 1)[1] for n in S.REC_CRF_ROWS} == {"rec", "crf", "both"}
+    for name, row in S.REC_CRF_CONFIGS.items():
+        cfg = dict(row["cfg"])
+        if cfg.get("aug_alignment_weight", 0) > 0:
+            cfg["res"] = row["frame"][0]
+        if row["hist"]:
+            cfg["hist_freq"] = 1
+        model = LitUnsupervisedSegmenter(row["n_classes"], make_cfg(model_type=row["arch"], random_backbone_init=True,
+                                                                    dino_patch_size=row["patch"], **cfg))
+        model.train()
+        assert model.cfg.fused_rec_crf and (model.cfg.rec_weight > 0 or model.cfg.crf_weight > 0), name
+        frame = row["frame"]
+        for seed in (1, 2):
+            b = S.make_batch(row, "cpu", seed=seed)
+            b["img"] = _CudaImg(b["img"].shape)
+            assert fused_step.FusedStep(model).supported(b), name
+
+
 def test_default_is_off():
     from stego_b200.config import TRAIN_DEFAULTS
     assert TRAIN_DEFAULTS["fused_rec_crf"] is False

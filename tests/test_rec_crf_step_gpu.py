@@ -30,10 +30,23 @@ crf (the stego_crf_mean_* entry points of csrc/crf_loss.cu):
   * dcode against fp64 through the same chain from the kernel's raw: test_loss_terms_fp64_gpu.crf_bwd_bar gives the
     bar of d sel for the uniform upstream gradient; F.normalize's backward dv = (dsel - k sel <sel, dsel>) / den carries
     (|d dsel| + |d sel| sum|sel dsel| + |sel| |d dot|) / den plus (eN + gamma_3) of its own terms, with
-    |d dot| <= sum (|d sel| |dsel| + |sel| |d dsel|) + eS sum |sel dsel|; the tap weights are fp32 products of fp32
-    lambdas (4 u in_size + 2u each), and a pixel reached r times gets r atomics: gamma_r of its |contributions| and
-    2^-125 per atomic (crf_dcode_bar).
+    |d dot| <= sum (|d sel| |dsel| + |sel| |d dsel|) + eS sum |sel dsel|.  The tap weights are fp32 products a' b'
+    of fp32 lambdas, each off by an ABSOLUTE d = 4 u in_size + 2 u from the fp64 a, b in [0, 1]; so
+    |a' b' - a b| <= d (a + b) + d^2 + u <= 2 d + d^2 + u, however small a b is.  And where the fp64 source position
+    lies within d of an integer, the fp32 one may fall on its other side: the kernel then taps the next pixel out
+    (i0 - 1 or i1 + 1) with a weight <= d.  So the weight error is bounded over the 4 x 4 box [y0 - 1, y0 + 2] x
+    [x0 - 1, x0 + 2] of every sample (clipped to the map), each pixel of it by (2 d + d^2 + u)(|dv| + |d dv|), and a
+    pixel gets at most r atomics, r the samples whose box holds it: gamma_r of its |contributions| and 2^-125 per
+    atomic (crf_dcode_bar).  With a non-dyadic scale (40 / 56, 60 / 56) a weight of a few 1e-7 lands on a pixel whose
+    fp64 weight is 0: a bar relative to a b does not hold there (a 60 x 84 code, 64 samples, 80 channels, went to 1.4
+    times such a bar).
   * the fused step's peak memory over a step stays below B n^2 4 bytes (no [B, n, n] tensor).
+
+Kernel edges: rec with m3 = None (the step with dropout off) at E = 384 / 768, D = 1 / 70 / 96, bit-equal to an
+all-ones m3; rec at the non-square frames' hw = 28 x 40 and 14 x 20 with M = B hw, B = 1 / 3; CRF codes of 28 x 40,
+40 x 28, 14 x 20 and 60 x 84 (a downsampling resize), C = 1 / 15 / 16 / 27 / 70 / 80 in NCHW and channels-last strides
+(both of ATen's bilinear kernels), guidance 224 x 320 or its transpose, n = 1 / 64 / 65 / 1000.  The same terms inside
+the replayed step, stage by stage across the step's configurations: tests/test_step_rec_crf_fp64_gpu.py.
 
 Step (switch on) against an autograd twin (switch off, no TF32) from the same generator states, at ViT-S/8 224² and
 ViT-B/8 320² (B = 32) and at ViT-S/8 224² (B = 8) crossed with the aug seeds, use_salience, use_true_labels, "KK",
@@ -120,20 +133,16 @@ def rec_bars(ref, code, W, M, D, E, dcos):
                 db=dr_bar.sum(0) + G(M) * dr.abs().sum(0))
 
 
-@pytest.mark.parametrize("E", [384, 768])
-@pytest.mark.parametrize("D", [1, 8, 70, 96])
-@pytest.mark.parametrize("edge", [False, True])
-def test_rec_kernels_vs_fp64(cuda_dev, E, D, edge):
-    """M = 3 x 337 rows (not a multiple of the CTA's 32), m3 with zeros; with edge, a pixel with r = 0 and one with
-    f = 0 (the eps clamps)."""
-    hw, M = 337, 3 * 337
-    code, feat, m3, W, b = _rec_inputs(E, D, M, hw, cuda_dev, seed=E + D + edge, edge=edge)
+def _rec_check(code, feat, m3, W, b, hw, tag, edge=False):
+    """one forward and backward against rec_term at rec_bars; the decoder gradient repeats bit for bit"""
+    M, E, D = feat.shape[0], W.shape[0], W.shape[1]
     dcos = float(torch.tensor(-0.7, dtype=torch.float32) / M)
-    cosv, nr, nf, dcode, dW, db = _rec_run(code, feat, m3, W, b, hw, dcos)
+    out = _rec_run(code, feat, m3, W, b, hw, dcos)
+    cosv, nr, nf, dcode, dW, db = out
     again = _rec_run(code, feat, m3, W, b, hw, dcos)
     assert torch.equal(dW, again[4]) and torch.equal(db, again[5]), "decoder gradient not bit-reproducible"
     assert torch.equal(dcode, again[3])
-    m3r = m3.repeat_interleave(hw, 0)[:M]
+    m3r = m3.repeat_interleave(hw, 0)[:M] if m3 is not None else None
     ref = RC.rec_term(code[:, :D], feat, m3r, W.view(E, D), b, dcos)
     bars = rec_bars(ref, code, W, M, D, E, dcos)
     rat = Ratios()
@@ -146,7 +155,43 @@ def test_rec_kernels_vs_fp64(cuda_dev, E, D, edge):
     assert (dcode[:, D:] == 0).all(), "padding columns written"
     if edge:
         assert nr[3].item() == 0 and nf[5].item() == 0 and cosv[3].item() == 0 and cosv[5].item() == 0
-    rat.check(f"rec_E{E}_D{D}_{'edge' if edge else 'rand'}")
+    rat.check(tag)
+    return out
+
+
+@pytest.mark.parametrize("E", [384, 768])
+@pytest.mark.parametrize("D", [1, 8, 70, 96])
+@pytest.mark.parametrize("edge", [False, True])
+def test_rec_kernels_vs_fp64(cuda_dev, E, D, edge):
+    """M = 3 x 337 rows (not a multiple of the CTA's 32), m3 with zeros; with edge, a pixel with r = 0 and one with
+    f = 0 (the eps clamps)."""
+    hw, M = 337, 3 * 337
+    code, feat, m3, W, b = _rec_inputs(E, D, M, hw, cuda_dev, seed=E + D + edge, edge=edge)
+    _rec_check(code, feat, m3, W, b, hw, f"rec_E{E}_D{D}_{'edge' if edge else 'rand'}", edge)
+
+
+@pytest.mark.parametrize("E", [384, 768])
+@pytest.mark.parametrize("D", [1, 70, 96])
+def test_rec_kernels_without_m3(cuda_dev, E, D):
+    """m3 = None (the step with dropout off) against rec_term without a mask, and bit-equal to an all-ones m3: f = feat
+    * 1.0 is exact in fp32, and nothing else reads m3."""
+    hw, M = 337, 3 * 337
+    code, feat, m3, W, b = _rec_inputs(E, D, M, hw, cuda_dev, seed=7 * E + D, edge=True)
+    none = _rec_check(code, feat, None, W, b, hw, f"rec_nom3_E{E}_D{D}", edge=True)
+    ones = _rec_run(code, feat, torch.ones_like(m3), W, b, hw, float(torch.tensor(-0.7, dtype=torch.float32) / M))
+    for name, a, o in zip(("cos", "nr", "nf", "dcode", "dW", "db"), none, ones):
+        assert torch.equal(a, o), f"m3 = None differs from an all-ones m3 in {name}"
+
+
+@pytest.mark.parametrize("E,D", [(384, 70), (768, 96)])
+@pytest.mark.parametrize("hw", [28 * 40, 14 * 20])
+@pytest.mark.parametrize("B", [1, 3])
+def test_rec_kernels_nonsquare(cuda_dev, E, D, hw, B):
+    """The step's non-square frames (28 x 40 at ViT-S/8 224 x 320, 14 x 20 at patch 16): M = B hw rows, a per-image m3
+    switching at every multiple of hw (280 is not a multiple of the CTA's 32 rows)."""
+    M = B * hw
+    code, feat, m3, W, b = _rec_inputs(E, D, M, hw, cuda_dev, seed=hw + B + D, edge=False)
+    _rec_check(code, feat, m3, W, b, hw, f"rec_E{E}_D{D}_hw{hw}_B{B}")
 
 
 # ================================================================================================
@@ -214,7 +259,22 @@ def _taps64(coords, h, w):
     return ((y0, x0, (1 - ly) * (1 - lx)), (y0, x1, (1 - ly) * lx), (y1, x0, ly * (1 - lx)), (y1, x1, ly * lx))
 
 
-def _scatter_taps(v, coords, h, w, weights=True):
+def scatter_box(v, coords, h, w):
+    """v [B, C, n] added to every pixel of each sample's 4 x 4 box [y0 - 1, y0 + 2] x [x0 - 1, x0 + 2] (clipped to the
+    [B, C, h, w] map): the pixels the kernel's fp32 taps can land on"""
+    B, C, _ = v.shape
+    y0 = RC.resize_taps(coords[0], h, 56)[0]
+    x0 = RC.resize_taps(coords[1], w, 56)[0]
+    out = torch.zeros(B, C, h * w, dtype=torch.float64, device=v.device)
+    for dy in range(-1, 3):
+        for dx in range(-1, 3):
+            yi, xi = y0 + dy, x0 + dx
+            ok = ((yi >= 0) & (yi < h) & (xi >= 0) & (xi < w)).double()
+            out.index_add_(2, yi.clamp(0, h - 1) * w + xi.clamp(0, w - 1), v * ok)
+    return out.view(B, C, h, w)
+
+
+def scatter_taps(v, coords, h, w, weights=True):
     """v [B, C, n] scattered into [B, C, h, w] through the bilinear taps (weights=False: count the nonzero taps)"""
     B, C, _ = v.shape
     out = torch.zeros(B, C, h * w, dtype=torch.float64, device=v.device)
@@ -240,11 +300,13 @@ def crf_dcode_bar(run, ref, ds, coords, code, n, h, w):
     ddot = (selbar * dsel.abs() + sel.abs() * dsel_bar).sum(1, keepdim=True) + eS * dotabs
     dv = (dsel - sel * (sel * dsel).sum(1, keepdim=True)) / den
     dv_bar = (dsel_bar + selbar * dotabs + sel.abs() * ddot) / den + (eN + G(3)) * (dsel.abs() + sel.abs() * dotabs) / den
-    werr = 2 * (4 * U * max(h, w) + 2 * U)  # each fp32 tap weight: two factors, each off by 4 u in_size + 2 u
-    r = _scatter_taps(torch.ones_like(dv), coords, h, w, weights=False)  # atomics per pixel
+    d = 4 * U * max(h, w) + 2 * U  # each fp32 lambda (and 1 - lambda): absolute error
+    werr = 2 * d + d * d + U        # |a' b' - a b| for a, b in [0, 1], on every pixel of the sample's box
+    wbox = werr * scatter_box(dv.abs() + dv_bar, coords, h, w)
+    r = scatter_box(torch.ones_like(dv), coords, h, w)  # atomics per pixel, at most
     gr = r * U / (1 - r * U)
-    return (_scatter_taps(dv_bar, coords, h, w) + werr * _scatter_taps(dv.abs(), coords, h, w) +
-            gr * _scatter_taps(dv.abs() + dv_bar, coords, h, w) + r * 2 * 2.0 ** -126)
+    return (scatter_taps(dv_bar, coords, h, w) + wbox + gr * (scatter_taps(dv.abs() + dv_bar, coords, h, w) + wbox) +
+            r * 2 * 2.0 ** -126)
 
 
 def dcode_from_raw(raw64, run, coords, p32, shape):
@@ -257,32 +319,24 @@ def dcode_from_raw(raw64, run, coords, p32, shape):
     dsel = torch.einsum("zab,zkb->zka", -2 * run["g"].double().item() * ref["s"], sel)
     k = torch.where(nv >= EPS, (sel * dsel).sum(1), torch.zeros_like(nv))
     dv = (dsel - sel * k[:, None]) / nv.clamp_min(EPS)[:, None]
-    return _scatter_taps(dv, coords, h, w), ref
+    ref["dv"] = dv
+    return scatter_taps(dv, coords, h, w), ref
 
 
-@pytest.mark.parametrize("h,S", [(28, 224), (40, 320), (56, 448)])
-@pytest.mark.parametrize("n", [1, 63, 64, 65, 1000, 2000])
-@pytest.mark.parametrize("C", [1, 70, 80])
-def test_crf_kernels_vs_torch_and_fp64(cuda_dev, h, S, n, C):
-    gen = torch.Generator().manual_seed(h * 7 + n + C)
-    B = 2
-    img = ((torch.rand(B, 3, S, S, generator=gen) - torch.tensor(R.MEAN).view(1, 3, 1, 1)) /
-           torch.tensor(R.STD).view(1, 3, 1, 1)).to(cuda_dev)
-    code_cl = torch.randn(B, h, h, C + 2, generator=gen).to(cuda_dev)  # channels-last with padding, as the step's
-    code = code_cl[..., :C].permute(0, 3, 1, 2)
-    coords = _crf_coords(n, gen).to(cuda_dev)
+def _crf_check(img, code, coords, tag):
+    """the CRF kernels on one code map (any strides) and guidance image: the resized samples bit-equal to torch CUDA's
+    F.interpolate read at them; sel, the norms, the loss and d(code) at crf_bars / crf_dcode_bar"""
+    B, C, h, w = code.shape
+    n = coords.shape[1]
     p32 = R.fp32_params(R.PARAMS)
-    w = 0.5
-    run = _crf_run(img, code, coords, p32, w)
+    wt = 0.5
+    run = _crf_run(img, code, coords, p32, wt)
     # the resized samples are torch's, bit for bit
     rs = lambda t: F.interpolate(t, 56, mode="bilinear", align_corners=False)
     ys, xs = coords[0], coords[1]
     assert torch.equal(run["raw"], rs(code)[:, :, ys, xs]), "resized code differs from F.interpolate"
     assert torch.equal(run["gsel"], rs(img)[:, :, ys, xs].permute(0, 2, 1)), "resized image differs from F.interpolate"
     assert torch.equal(run["pos"].long(), coords.t())
-    if n == 1000:  # an NCHW-contiguous code: ATen's other kernel (the same for fewer than 16 channels)
-        flat = code.contiguous()
-        assert torch.equal(_crf_run(img, flat, coords, p32, w)["raw"], rs(flat)[:, :, ys, xs])
     rat = Ratios()
     raw64 = run["raw"].double()
     nv = raw64.norm(dim=1)
@@ -291,17 +345,66 @@ def test_crf_kernels_vs_torch_and_fp64(cuda_dev, h, S, n, C):
     eN = eS / 2 + eS ** 2 + G(2)
     rat.add("sel", run["sel"], sel64, sel64.abs() * (eN + U) + 2.0 ** -149)
     rat.add("nrm", run["nrm"], nv, nv * eS)
-    bar, loss64, e2e, ref, ds = crf_loss_bars(run, coords, p32, C, code, h, h)
+    bar, loss64, e2e, ref, ds = crf_loss_bars(run, coords, p32, C, code, h, w)
     rat.add("loss", run["loss"], loss64, bar)
-    rat.add("total", run["total"], w * loss64, w * bar + U * abs(w) * loss64.abs() + 2 * U * abs(w * loss64))
-    full = RC.crf_term(img, code, coords, p32, w)
+    rat.add("total", run["total"], wt * loss64, wt * bar + U * abs(wt) * loss64.abs() + 2 * U * abs(wt * loss64))
+    full = RC.crf_term(img, code, coords, p32, wt)
     rat.add("loss_e2e", run["loss"], full["loss"], bar + e2e)
     # dcode through the chain from the kernel's own raw
     want, ref_raw = dcode_from_raw(raw64, run, coords, p32, code.shape)
     _, ds_raw = crf_bars(ref_raw, C, p32)
-    rat.add("dcode", run["dcode"], want, crf_dcode_bar(run, ref_raw, ds_raw, coords, code, n, h, h))
-    rat.check(f"crf_h{h}_n{n}_C{C}")
+    rat.add("dcode", run["dcode"], want, crf_dcode_bar(run, ref_raw, ds_raw, coords, code, n, h, w))
+    rat.check(tag)
+    return run
 
+
+def _crf_image(B, H, W, gen, dev):
+    return ((torch.rand(B, 3, H, W, generator=gen) - torch.tensor(R.MEAN).view(1, 3, 1, 1)) /
+            torch.tensor(R.STD).view(1, 3, 1, 1)).to(dev)
+
+
+def _crf_code(B, C, h, w, layout, gen, dev):
+    """[B, C, h, w]: "channels_last" is the step's layout (channels innermost, rows padded by two channels), "nchw"
+    contiguous"""
+    if layout == "channels_last":
+        return torch.randn(B, h, w, C + 2, generator=gen).to(dev)[..., :C].permute(0, 3, 1, 2)
+    return torch.randn(B, C, h, w, generator=gen).to(dev)
+
+
+@pytest.mark.parametrize("h,S", [(28, 224), (40, 320), (56, 448)])
+@pytest.mark.parametrize("n", [1, 63, 64, 65, 1000, 2000])
+@pytest.mark.parametrize("C", [1, 70, 80])
+def test_crf_kernels_vs_torch_and_fp64(cuda_dev, h, S, n, C):
+    gen = torch.Generator().manual_seed(h * 7 + n + C)
+    B = 2
+    img = _crf_image(B, S, S, gen, cuda_dev)
+    code = _crf_code(B, C, h, h, "channels_last", gen, cuda_dev)
+    coords = _crf_coords(n, gen).to(cuda_dev)
+    _crf_check(img, code, coords, f"crf_h{h}_n{n}_C{C}")
+    if n == 1000:  # an NCHW-contiguous code: ATen's other kernel (the same for fewer than 16 channels)
+        flat = code.contiguous()
+        rs = lambda t: F.interpolate(t, 56, mode="bilinear", align_corners=False)
+        run = _crf_run(img, flat, coords, R.fp32_params(R.PARAMS), 0.5)
+        assert torch.equal(run["raw"], rs(flat)[:, :, coords[0], coords[1]])
+
+
+@pytest.mark.parametrize("h,w", [(28, 40), (40, 28), (14, 20), (60, 84)])
+@pytest.mark.parametrize("C", [1, 15, 16, 27, 70, 80])
+@pytest.mark.parametrize("layout", ["nchw", "channels_last"])
+@pytest.mark.parametrize("n", [1, 64, 65, 1000])
+def test_crf_kernels_nonsquare(cuda_dev, h, w, C, layout, n):
+    """Non-square code maps (28 x 40 and its transpose: ViT-S/8 at 224 x 320 and 320 x 224; 14 x 20: patch 16) and one
+    with both sides above 56, which the resize to 56 x 56 downsamples; the guidance image 224 x 320 or its transpose,
+    as the code.  Channel counts on both sides of ATen's channels-last switch at 16, each in both layouts, so both
+    restatements of ATen's bilinear kernel run; 1, 64 and 65 samples (one, a full and a second 64-sample tile) and the
+    default 1000."""
+    gen = torch.Generator().manual_seed(h * 1000 + w * 10 + C + n)
+    B = 2
+    H, W = (224, 320) if w > h else (320, 224)
+    img = _crf_image(B, H, W, gen, cuda_dev)
+    code = _crf_code(B, C, h, w, layout, gen, cuda_dev)
+    coords = _crf_coords(n, gen).to(cuda_dev)
+    _crf_check(img, code, coords, f"crf_{h}x{w}_n{n}_C{C}_{layout}")
 
 
 # ================================================================================================

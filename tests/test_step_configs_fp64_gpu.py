@@ -33,6 +33,8 @@ table in tests/_step_fp64.py).  Per row:
                                    dclusters through the normalise backward;
                     head backward  from the step's d(code): test_fused_step_head_fp64's bars (colsum gamma_{40+blocks},
                                    split-K wgrad gamma_{64 kbps + splits}, dh gamma_130), dyb and dhb bit-exact.
+                    rec / crf      with the reconstruction and CRF terms, their stages and their share of the img
+                                   rows' d(code) (_rec_crf_stages, _cross_bar; tests/test_step_rec_crf_fp64_gpu.py).
   4. padding      ws.ctiles (torch.empty) is NaN-filled when the workspace is made: after the first step nothing logged
                   or in the flat gradient buffer is NaN and channels D..128 of every code tile are zero; ws.code is
                   allocated zero-filled and its columns D..P are still exactly zero after the replayed step.
@@ -46,16 +48,19 @@ import sys
 
 import pytest
 import torch
+import torch.nn.functional as F
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import _corr_fp64 as RC  # noqa: E402
 import _head_fp64 as RH  # noqa: E402
 import _loss_terms_fp64 as RL  # noqa: E402
 import _probes_fp64 as RP  # noqa: E402
+import _rec_crf_fp64 as RRC  # noqa: E402
 import _step_fp64 as S  # noqa: E402
 from _parity_util import rel  # noqa: E402
 from stego_b200 import hist as hist_mod  # noqa: E402
-from test_loss_terms_fp64_gpu import cos_bars  # noqa: E402
+from test_loss_terms_fp64_gpu import cos_bars, crf_bars  # noqa: E402
+from test_rec_crf_step_gpu import crf_dcode_bar, crf_loss_bars, dcode_from_raw, rec_bars, scatter_box, scatter_taps  # noqa: E402,E501
 from test_head_fp64_gpu import Ratios, _adam_ratios, _check_forward, _colsum_bar, _same_bits, _wgrad_bar  # noqa: E402
 from test_probes_fp64_gpu import _chain, _lce_bars  # noqa: E402
 
@@ -93,6 +98,96 @@ def _cluster_bars(r, loss, dcl, x, cl, dev):
     full = (D + ch.abs() * (ch.abs() * D).sum(1, keepdim=True)) / nrm.clamp_min(1e-12) + \
         (C + 8) * U * (dnc.abs() + ch.abs() * (ch * dnc).sum(1, keepdim=True).abs()) / nrm.clamp_min(1e-12)
     r.add("dclusters", dcl, ref["dcl"], torch.where(nrm > 1e-12, full, (D + U * dnc.abs()) / 1e-12) + 1e-300)
+
+
+def _rec_crf_stages(r, model, batch, before, grads, tok, M3):
+    """The reconstruction and CRF terms of the replayed step, stage-wise on its own inputs (see
+    tests/test_step_rec_crf_fp64_gpu.py).  Returns the terms' fp64 d(code) of the img rows [B hw, D], its bar, the
+    (roundings, sum of |contributions|) each term adds to those rows' fp32 accumulators, and per term (weight, fp64
+    loss, its bar, the step's loss)."""
+    from stego_b200 import modules
+    ws, cfg = model._fused.ws, model.cfg
+    B, E, D, P, fh, fw, hw, M, nonlinear = ws.dims
+    dev = ws.code.device
+    N = B * hw
+    rm = lambda t: t.permute(0, 2, 3, 1).reshape(N, -1)
+    want = torch.zeros(N, D, dtype=torch.float64, device=dev)
+    bar = torch.zeros_like(want)
+    acc, losses = [], {}
+    if ws.rec:  # -cosine(decoder(code), feats * m3) on the img rows, with the decoder the step ran with
+        W, b = before["decoder.weight"], before["decoder.bias"]
+        code = ws.code[:N]
+        m3 = M3[:B].repeat_interleave(hw, 0) if M3 is not None else None
+        # d loss / d cos = -w / (B hw): fl(-w) times an fp32 reciprocal on the device, three roundings
+        dcos = ws.rec_dcos.item()
+        assert abs(dcos + float(cfg.rec_weight) / N) <= G(3) * float(cfg.rec_weight) / N, "d loss / d cos of rec"
+        ref = RRC.rec_term(code[:, :D], tok[:N], m3, W.view(E, D), b, dcos)
+        bars = rec_bars(ref, code, W, N, D, E, dcos)
+        for k in ("cos", "nr", "nf"):
+            r.add("rec_" + k, getattr(ws, "rec_" + k), ref[k], bars[k])
+        loss = float(ws.rec_loss[0])
+        assert loss == float(torch.tensor(-ws.rec_cos.double().mean().item(), dtype=torch.float32))
+        assert float(model.logged["loss/rec"]) == loss
+        e = bars["cos"].mean().item() + U * abs(loss)
+        r.add("loss_rec", torch.tensor(loss), torch.tensor(ref["loss"].item()), torch.tensor(e))
+        r.add("dW_decoder", grads["decoder.weight"].view(E, D), ref["dW"], bars["dW"])
+        r.add("db_decoder", grads["decoder.bias"], ref["db"], bars["db"])
+        want += ref["dcode"]
+        bar += bars["dcode"]
+        # one fp32 add of each 64-channel chunk's partial onto the row's accumulator
+        acc.append((-(-E // 64), ref["dr"].abs() @ W.double().view(E, D).abs() + bars["dcode"]))
+        losses["rec"] = (float(cfg.rec_weight), ref["loss"].item(), e, loss)
+    if ws.crf:  # crf_loss_fn(resize(img, 56), normalize(resize(code, 56))) at this step's samples
+        coords = ws.crf_coords
+        n = coords.shape[1]
+        ys, xs = coords[0], coords[1]
+        img = batch["img"]
+        code = ws.code.view(ws.n_img * B, fh, fw, P)[:B, ..., :D].permute(0, 3, 1, 2)  # the step's strides
+        rs = lambda t: F.interpolate(t, modules.CRF_SIDE, mode="bilinear", align_corners=False)
+        w = float(cfg.crf_weight)
+        # d loss / d out = w / (B n^2) of the mean: fl(w) times an fp32 reciprocal on the device, three roundings
+        g = ws.crf_g
+        assert abs(g.item() - w / (B * n * n)) <= G(3) * w / (B * n * n), "d loss / d out of the CRF term"
+        run = dict(gsel=ws.crf_gsel[:, :n, :3], raw=ws.crf_raw[:, :, :n], sel=ws.crf_sel[:, :, :n],
+                   nrm=ws.crf_nrm[:, :n], g=g)
+        # the guidance ran outside the graph, on the coordinates the replayed prologue drew
+        assert torch.equal(run["gsel"], rs(img)[:, :, ys, xs].permute(0, 2, 1)), "crf_gsel differs from F.interpolate"
+        assert torch.equal(run["raw"], rs(code)[:, :, ys, xs]), "crf_raw differs from F.interpolate"
+        assert torch.equal(ws.crf_pos[:n].long(), coords.t())
+        p32 = RL.fp32_params(modules.crf_params(model.crf_loss_fn))
+        raw64 = run["raw"].double()
+        nv = raw64.norm(dim=1)
+        sel64 = raw64 / nv.clamp_min(RL.EPS32)[:, None]
+        eS = G(-(-D // 32) + 5)
+        eN = eS / 2 + eS ** 2 + G(2)
+        r.add("crf_sel", run["sel"], sel64, sel64.abs() * (eN + U) + 2.0 ** -149)
+        r.add("crf_nrm", run["nrm"], nv, nv * eS)
+        cbar, loss64, e2e, _, _ = crf_loss_bars(run, coords, p32, D, code, fh, fw)
+        loss = float(ws.crf_loss[0])
+        assert float(model.logged["loss/crf"]) == loss
+        r.add("loss_crf", torch.tensor(loss), loss64.cpu(), cbar.cpu())
+        full = RRC.crf_term(img, code, coords, p32, w)
+        r.add("loss_crf_e2e", torch.tensor(loss), full["loss"].cpu(), (cbar + e2e).cpu())
+        dc, ref_raw = dcode_from_raw(raw64, run, coords, p32, code.shape)
+        _, ds_raw = crf_bars(ref_raw, D, p32)
+        cb = crf_dcode_bar(run, ref_raw, ds_raw, coords, code, n, fh, fw)
+        want += rm(dc)
+        bar += rm(cb)
+        # at most one atomic per sample whose fp32 taps can land on the element (crf_dcode_bar's box)
+        cnt = scatter_box(torch.ones_like(ref_raw["dv"]), coords, fh, fw)
+        acc.append((rm(cnt), rm(scatter_taps(ref_raw["dv"].abs(), coords, fh, fw) + cb)))
+        losses["crf"] = (w, loss64.item(), cbar.item(), loss)
+    return want, bar, acc, losses
+
+
+def _cross_bar(old, new):
+    """The cross terms of several stages accumulating into the same fp32 d(code) elements: each stage's bar covers the
+    roundings of its own additions against its own sum of |contributions|; each of its k additions onto the shared
+    accumulator rounds against the others' sums too, u (A_all - A_own) per addition.  old: the (k, A) of the stages
+    whose cross terms are already in the bar (among themselves), new: those added here."""
+    A_new = sum(A for _, A in new)
+    A_all = A_new + sum(A for _, A in old)
+    return sum(k * U * A_new for k, _ in old) + sum(k * U * (A_all - A) for k, A in new)
 
 
 def _fp64_replayed_step(r, model, batch, before, grads, dev, hist=False):
@@ -157,9 +252,11 @@ def _fp64_replayed_step(r, model, batch, before, grads, dev, hist=False):
     assert (dall[:, D:] == 0).all(), "d(code) padding columns"
     rows = slice(0, 2 * B * hw)
     bar = ref["dcode_bar"][rows]
+    want = ref["dcode"][rows]
+    rm = lambda t: t.permute(0, 2, 3, 1).reshape(B * hw, -1)
+    old = [(rm(corr.hits[0]), rm(corr.Ao[0]))]  # the correspondence loss's gather into the img rows
     if ws.aug:
         a = ref["aug"]
-        rm = lambda t: t.permute(0, 2, 3, 1).reshape(B * hw, -1)
         code_img = ws.code.view(nI * B, fh, fw, P)[:B, ..., :D].permute(0, 3, 1, 2)
         code_aug = ws.code.view(nI * B, fh, fw, P)[2 * B:, ..., :D].permute(0, 3, 1, 2)
         r.add("aug_grid", ws.grid, a["grid"], torch.tensor(S.aug_grid_bar(ws.coord_aug), device=dev))
@@ -180,7 +277,14 @@ def _fp64_replayed_step(r, model, batch, before, grads, dev, hist=False):
         k = S.tap_counts(ws.grid, fh)
         sc = S.aug_scatter_bar(ws.grid, a["A"], ws.dsampled, fh) + k * U * corr.Ao[0] + corr.hits[0] * U * a["A"]
         bar = torch.cat([rm(sc) + bar[:B * hw], bar[B * hw:]])
-    r.add("dcode", dall[rows, :D], ref["dcode"][rows], bar)
+        old.append((rm(k), rm(a["A"])))
+    rc_losses = {}
+    if ws.rec or ws.crf:  # their d(code) joins the img rows' accumulators, with the cross terms of sharing them
+        rc_want, rc_bar, new, rc_losses = _rec_crf_stages(r, model, batch, before, grads, tok, M3)
+        img = slice(0, B * hw)
+        want = torch.cat([want[img] + rc_want, want[B * hw:]])
+        bar = torch.cat([bar[img] + rc_bar + _cross_bar(old, new), bar[B * hw:]])
+    r.add("dcode", dall[rows, :D], want, bar)
     # linear probe (upstream gradient 1, accumulated from zero)
     code4 = ws.code.view(nI * B, fh, fw, P)[..., :D].permute(0, 3, 1, 2)[:B]
     LH, LW = ws.label.shape[-2:]
@@ -202,9 +306,18 @@ def _fp64_replayed_step(r, model, batch, before, grads, dev, hist=False):
     for key, kk in (("loss/pos_intra", 0), ("loss/pos_inter", 1)):
         assert logged[key] == float(st[kk, 0])
     e_lin, e_clu = lbar, r.bars["loss_cluster"]
-    tot_bar = sum(c * s["E_loss"] for c, s in zip(cw, stats)) + e_lin + e_clu + \
-        G(len(stats) + 5) * (sum(abs(c * s["loss"]) for c, s in zip(cw, stats)) + abs(L["linear"]) + abs(L["cluster"]))
+    # w * rec and w * crf: each fl(w l) added onto the running total, one more rounding of it per term (the sum
+    # below then also counts the terms' and the aug term's sizes), and the fp64 loss off by its bar
+    extra = len(rc_losses)
+    terms_abs = sum(abs(c * s["loss"]) for c, s in zip(cw, stats)) + abs(L["linear"]) + abs(L["cluster"])
+    if extra:
+        terms_abs += sum(abs(wt * got) for wt, _, _, got in rc_losses.values())
+        terms_abs += abs(float(cfg.aug_alignment_weight) * aug_loss) if ws.aug else 0.0
+    tot_bar = sum(c * s["E_loss"] for c, s in zip(cw, stats)) + e_lin + e_clu + G(len(stats) + 5 + extra) * terms_abs
     want_total = L["total"]
+    for wt, l64, e, got in rc_losses.values():
+        want_total += wt * l64
+        tot_bar += abs(wt) * e + U * abs(wt * got)
     if ws.aug:  # stage-wise: the step's own aug loss, weighted in fp32
         wa = float(cfg.aug_alignment_weight)
         want_total += wa * (aug_loss - L["aug_alignment"])
@@ -354,6 +467,11 @@ def run_row(row, tag, dev, monkeypatch):
         if k == "cluster_probe.clusters" and D == 1:
             # a one-channel centroid normalises to +-1 whatever its value: the exact gradient is 0 and both paths hold
             # rounding noise, which the fp64 check below bounds absolutely
+            continue
+        if k.startswith("net.") and D == 1 and fused.cfg.crf_weight > 0:
+            # likewise each CRF sample normalises to +-1: the exact d(code) of the CRF term is 0, which the fused
+            # backward gives exactly (sel dsel sel = dsel), while autograd's F.normalize backward leaves a rounding of
+            # dsel / |v| (6e-3 relative L2 of the head gradients); the fp64 check below holds the fused step's
             continue
         assert twin_rel[k] < 3e-3, (k, twin_rel)
 
