@@ -21,6 +21,8 @@
 //   * registers: paired stores straight from the accumulator fragments, for what TMA cannot express: split-K atomics,
 //     the patch-embed row remap, a residual other than the output, outputs (or rows of N outputs) not 16-byte aligned.
 // Operand tiles are 128 x 64 bf16 (A and B); accumulation fp32.
+// Large GEMMs with K <= 384 (the ViT-S qkv, proj, fc1) run gemm_bf16_resident_kernel instead, which keeps each CTA's
+// 128-column block of B in shared memory and streams only A.
 #include <stdlib.h>
 #include <string.h>
 
@@ -160,7 +162,7 @@ __device__ __forceinline__ void gemm_store_regs(const float (&acc)[BN / 2], cons
 // chunk c - 1.  Every chunk is its own bulk group: before buffer reuse the issuing thread waits only until the store
 // two chunks back has READ its buffer.  Rows past M and columns past N are clipped by TMA.  The named barrier (one
 // per warpgroup, 128 threads) only orders the warpgroup's own staging writes against its issuing thread.
-template <bool kBf16>
+template <bool kBf16, int kBufs = 2>
 __device__ __forceinline__ void gemm_store_tma(const float (&acc)[2][GEMM_BN / 2], const GemmParams& p,
                                                const CUtensorMap* tm_out, uint32_t stage, int bar_id, bool issuer,
                                                int m0, int n0, int tb) {
@@ -171,8 +173,8 @@ __device__ __forceinline__ void gemm_store_tma(const float (&acc)[2][GEMM_BN / 2
   const uint32_t swz = (lane >> 2) & 7;  // row & 7 of every row this thread holds
 #pragma unroll
   for (int ch = 0; ch < GEMM_BN / kCols; ++ch) {
-    const uint32_t buf = stage + (ch & 1) * GEMM_CHUNK_BYTES;
-    if (issuer) tma_wait_group_read<1>();
+    const uint32_t buf = stage + (ch % kBufs) * GEMM_CHUNK_BYTES;
+    if (issuer) tma_wait_group_read<kBufs - 1>();
     named_bar_sync(bar_id, 128);
     // this thread's rows are 16 wq + lane / 4 + {0, 8, 64, 72}, all with the same row & 7
     const uint32_t rbase = buf + (16 * wq + (lane >> 2)) * 128u;
@@ -396,6 +398,157 @@ static int launch_gemm_epi(bool tma_epi, const CUtensorMap& tmA, const CUtensorM
   return launch_gemm<6, A_MN, B_MN, false>(tmA, tmB, tmOut, p, stream);
 }
 
+// Resident-weight variant for K <= GEMM_RES_MAX_K, both operands K-major, batch 1, TMA epilogue.  Every tile of
+// gemm_bf16_kernel streams a 128 x 64 A box and a 128 x 64 B box per k-block; here each CTA owns one 128-column block
+// tn of the output, loads B[tn] ([128 cols][K], ceil(K / 64) SWIZZLE_128B boxes) into shared memory once, and the
+// ring carries only A boxes: half the L2-to-SM bytes per tile.  The CTAs sharing column tn walk the row tiles
+// tm = blockIdx.x / tiles_n, strided by their count, so the CTAs of all columns advance through A together and A's
+// re-reads (once per column) hit L2.  Warp roles, the ping-pong hand-over and the epilogue are gemm_bf16_kernel's; each
+// output element sees the same k16 wgmma sequence, so the results are bit-identical to it.
+constexpr int GEMM_RES_MAX_K = 384;
+constexpr uint32_t GEMM_RES_BOX_BYTES = GEMM_BM * GEMM_BK * 2;  // one 128 x 64 bf16 box, A or B: 16 KB
+constexpr uint32_t GEMM_RES_B_BYTES = (GEMM_RES_MAX_K / GEMM_BK) * GEMM_RES_BOX_BYTES;
+
+//
+// Shared memory: 96 KB of B, then either 4 A stages and two 16 KB staging buffers per MMA warpgroup (kBufs = 2), or 6
+// A stages and one buffer per warpgroup (kBufs = 1).  At the c1 shapes on an H100 the deeper ring made the GELU / ReLU
+// GEMMs 4-7 % faster and the plain bf16 / fp32 x += ones slower (their stores serialise on the single buffer).
+template <int kStages, int kBufs>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+gemm_bf16_resident_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                          const __grid_constant__ CUtensorMap tmOut, GemmParams p) {
+  constexpr uint32_t BOX = GEMM_RES_BOX_BYTES;
+
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* sb = smem;                                  // B column block: box kb at kb * 16 KB
+  uint8_t* sa = smem + GEMM_RES_B_BYTES;               // A ring
+  uint8_t* staging = sa + kStages * BOX;               // kBufs 16 KB chunk buffers per MMA warpgroup
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(staging + 2 * kBufs * GEMM_CHUNK_BYTES);
+  uint64_t* empty_bar = full_bar + kStages;
+  uint64_t* turn_bar = empty_bar + kStages;  // turn_bar[w]: MMA warpgroup w may start its next mainloop
+  uint64_t* b_bar = turn_bar + 2;            // the B column block has landed
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const int wg = warp >> 2;  // 0 producer, 1..2 MMA warpgroups
+
+  const int tiles_m = (p.M + GEMM_BM - 1) / GEMM_BM;
+  const int tiles_n = (p.N + GEMM_BN - 1) / GEMM_BN;
+  const int num_kb = (p.K + GEMM_BK - 1) / GEMM_BK;  // K tail: TMA zero-fills out-of-bounds
+  // the host launches at least tiles_n CTAs, so every column block has one
+  const int tn = static_cast<int>(blockIdx.x) % tiles_n;
+  const int tm_start = static_cast<int>(blockIdx.x) / tiles_n;
+  const int tm_step = (static_cast<int>(gridDim.x) - tn + tiles_n - 1) / tiles_n;  // CTAs that own column tn
+
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmA);
+    tma_prefetch_desc(&tmB);
+    tma_prefetch_desc(&tmOut);
+    for (int s = 0; s < kStages; ++s) {
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], 1);  // every stage is consumed by exactly one MMA warpgroup
+    }
+    mbar_init(&turn_bar[0], 1);
+    mbar_init(&turn_bar[1], 1);
+    mbar_init(b_bar, 1);
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  if (wg == 0) {
+    // ===================== TMA producer =====================
+    warpgroup_reg_dealloc<40>();
+    if (threadIdx.x == 0) {
+      mbar_arrive_expect_tx(b_bar, num_kb * BOX);
+      for (int kb = 0; kb < num_kb; ++kb) tma_load_3d(sb + kb * BOX, &tmB, b_bar, kb * GEMM_BK, tn * GEMM_BN, 0);
+      uint32_t stage = 0, phase = 0;
+      for (int tm = tm_start; tm < tiles_m; tm += tm_step) {
+        for (int kb = 0; kb < num_kb; ++kb) {
+          mbar_wait(&empty_bar[stage], phase ^ 1u);
+          mbar_arrive_expect_tx(&full_bar[stage], BOX);
+          tma_load_3d(sa + stage * BOX, &tmA, &full_bar[stage], kb * GEMM_BK, tm * GEMM_BM, 0);
+          if (++stage == kStages) { stage = 0; phase ^= 1u; }
+        }
+      }
+    }
+  } else {
+    // ===================== MMA warpgroups =====================
+    warpgroup_reg_alloc<232>();
+    const int mwg = wg - 1;  // owns the CTA's tiles i with i % 2 == mwg
+    constexpr uint32_t DESC_HI = smem_desc_hi_sw128(1024);
+    constexpr uint32_t KSTEP = 32u >> 4;     // low-word step per k16 slice (K-major)
+    constexpr uint32_t A_HALF = 8192u >> 4;  // rows 64.. of the A tile
+    const uint32_t a_lo0 = smem_desc_lo(smem_u32(sa), 8192u);
+    const uint32_t b_lo0 = smem_desc_lo(smem_u32(sb), 8192u);
+    const bool leader = (threadIdx.x & 127) == 0;
+    uint32_t stage = 0, phase = 0;
+    float acc[2][GEMM_BN / 2];
+    mbar_wait(b_bar, 0);
+    int i = 0;
+    for (int tm = tm_start; tm < tiles_m; tm += tm_step, ++i) {
+      if ((i & 1) != mwg) {  // the partner's tile: its k-blocks pass through the ring in between
+        ring_advance<kStages>(stage, phase, num_kb);
+        continue;
+      }
+      if (i > 0) mbar_wait(&turn_bar[mwg], ((i - 1) >> 1) & 1);  // as in gemm_bf16_kernel
+#pragma unroll
+      for (int j = 0; j < GEMM_BN / 2; ++j) { acc[0][j] = 0.f; acc[1][j] = 0.f; }
+      uint32_t prev_stage = 0;
+      for (int kb = 0; kb < num_kb; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t a_lo = a_lo0 + stage * (BOX >> 4);
+        const uint32_t b_lo = b_lo0 + kb * (BOX >> 4);
+        fence_operands(acc[0]);
+        fence_operands(acc[1]);
+        wgmma_fence();
+#pragma unroll
+        for (uint32_t k = 0; k < GEMM_BK / 16; ++k) {
+          const uint64_t db = smem_desc_join(b_lo + k * KSTEP, DESC_HI);
+#pragma unroll
+          for (uint32_t h = 0; h < 2; ++h)
+            wgmma_ss<GEMM_BN, 0, 0>(acc[h], smem_desc_join(a_lo + h * A_HALF + k * KSTEP, DESC_HI), db, 1u);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();  // the previous k-block's MMAs have retired: its A slot is reusable
+        if (kb > 0 && leader) mbar_arrive(&empty_bar[prev_stage]);
+        prev_stage = stage;
+        if (++stage == kStages) { stage = 0; phase ^= 1u; }
+      }
+      if (leader) mbar_arrive(&turn_bar[mwg ^ 1]);  // hand the tensor cores to the partner
+      wgmma_wait<0>();
+      fence_operands(acc[0]);
+      fence_operands(acc[1]);
+      if (leader) mbar_arrive(&empty_bar[prev_stage]);
+      const int col_base = tn * GEMM_BN + 2 * (lane & 3);
+      gemm_bias_act<GEMM_BN>(acc[0], p, col_base);
+      gemm_bias_act<GEMM_BN>(acc[1], p, col_base);
+      const uint32_t st = smem_u32(staging) + mwg * kBufs * GEMM_CHUNK_BYTES;
+      if (p.out_bf16) gemm_store_tma<true, kBufs>(acc, p, &tmOut, st, 1 + mwg, leader, tm * GEMM_BM, tn * GEMM_BN, 0);
+      else gemm_store_tma<false, kBufs>(acc, p, &tmOut, st, 1 + mwg, leader, tm * GEMM_BM, tn * GEMM_BN, 0);
+    }
+    if (leader) tma_wait_group<0>();  // every store has completed before the CTA (and its smem) goes away
+  }
+}
+
+template <int kStages, int kBufs>
+static int launch_gemm_resident_kernel(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmOut,
+                                       const GemmParams& p, int grid, cudaStream_t stream) {
+  constexpr size_t smem = GEMM_RES_B_BYTES + kStages * GEMM_RES_BOX_BYTES + 2 * kBufs * GEMM_CHUNK_BYTES + 1024 + 256;
+  static_assert(smem <= 232448, "exceeds the 227 KB of shared memory a CTA can opt into");
+  constexpr auto kern = gemm_bf16_resident_kernel<kStages, kBufs>;
+  if (const int rc = opt_in_smem<kern>(smem, "gemm_bf16_resident_kernel"); rc != STEGO_OK) return rc;
+  kern<<<grid, GEMM_THREADS, smem, stream>>>(tmA, tmB, tmOut, p);
+  STEGO_CHECK_LAUNCH("gemm_bf16_resident_kernel launch");
+  return STEGO_OK;
+}
+
+static int launch_gemm_resident(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmOut,
+                                const GemmParams& p, int grid, cudaStream_t stream) {
+  if (p.act != 0) return launch_gemm_resident_kernel<6, 1>(tmA, tmB, tmOut, p, grid, stream);
+  return launch_gemm_resident_kernel<4, 2>(tmA, tmB, tmOut, p, grid, stream);
+}
+
 }  // namespace stego
 
 using namespace stego;
@@ -485,6 +638,14 @@ static int gemm_impl(const void* A, int lda, long long a_bs, int a_mn_major, con
   } else {
     memset(&tmOut, 0, sizeof(tmOut));  // unused by the register epilogue
   }
+  // The resident-weight kernel needs its B column block to fit in shared memory (K <= 384) and enough tiles per CTA
+  // (>= 4 per SM) to amortise loading it; one CTA per SM, at least one per column block.
+  const int tiles_n = (N + GEMM_BN - 1) / GEMM_BN;
+  const long long tiles = static_cast<long long>((M + GEMM_BM - 1) / GEMM_BM) * tiles_n;
+  const int sms = num_sms();
+  if (batch == 1 && !a_mn_major && !b_mn_major && tma_epi && K <= GEMM_RES_MAX_K && tiles >= 4LL * sms &&
+      tiles_n <= sms)
+    return launch_gemm_resident(tmA, tmB, tmOut, p, sms, stream);
   if (!a_mn_major && !b_mn_major) return launch_gemm_epi<false, false>(tma_epi, tmA, tmB, tmOut, p, stream);
   if (!a_mn_major && b_mn_major) return launch_gemm_epi<false, true>(tma_epi, tmA, tmB, tmOut, p, stream);
   if (a_mn_major && b_mn_major) return launch_gemm_epi<true, true>(tma_epi, tmA, tmB, tmOut, p, stream);
