@@ -256,6 +256,29 @@ STEGO_API int stego_frames_rgb8(const void* staging_host, const void* staging_de
  * 8-byte aligned. */
 STEGO_API int stego_labels_u8(const void* staging_host, const void* staging_dev, long long bytes,
                               long long table_words, int B, int res, const long long* lut, long long* out, void* stream);
+/* Resident training store (stego_b200/dataset.py ResidentDataset): the same staging layout and gather, with the raw
+ * bytes written into rows r0 .. r0 + B of an n-row uint8 store, no normalisation and no table: [n][3][res][res] images
+ * (stego_frames_store_rgb8) or [n][res][res] label maps (stego_labels_store_u8).  store: 16-byte aligned, device memory
+ * or pinned host memory (written through its mapped address).  0 <= r0 <= n - B. */
+STEGO_API int stego_frames_store_rgb8(const void* staging_host, const void* staging_dev, long long bytes,
+                                      long long table_words, int B, int res, unsigned char* store, long long n,
+                                      long long r0, void* stream);
+STEGO_API int stego_labels_store_u8(const void* staging_host, const void* staging_dev, long long bytes,
+                                    long long table_words, int B, int res, unsigned char* store, long long n,
+                                    long long r0, void* stream);
+/* `count` samples from the resident store, sample s being row index[s]: images uint8 [n][3][res][res] and labels uint8
+ * [n][res][res] (null: every pixel reads id 0), each device memory or pinned host memory, 16-byte aligned.
+ *   img [count][3][res][res]: ((float)x / 255 - mean[c]) / std[c] as stego_frames_rgb8 computes it; fp32, or its
+ *     bf16 round when out_bf16 = 1;
+ *   label int64 [count][res][res] = lut[byte], lut: device int64 [256];
+ *   mask [count][res][res]: mask_kind 0 = bool (label == -1) (CroppedDataset), 1 = fp32 (label > 0) (DirectoryDataset).
+ * index: int64 [count] in pinned host memory, checked on the host (0 <= index[s] < n) and read by the kernel through its
+ * mapped address, so it must stay unchanged until the launch has run.  count 1..65535, res 1..8192; outputs 16-byte
+ * aligned.  One launch; the call never synchronises and reads nothing back from the device. */
+STEGO_API int stego_dataset_batch(const unsigned char* images, const unsigned char* labels, long long n, int res,
+                                  const long long* index, int count, const long long* lut, float mean0, float mean1,
+                                  float mean2, float std0, float std1, float std2, int out_bf16, int mask_kind,
+                                  void* img, long long* label, void* mask, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * TensorBoard histograms (SummaryWriter.add_histogram with its default bins="tensorflow")

@@ -9,11 +9,15 @@
 // Each output pixel is then one gather: no resized intermediate is written, and only the source pixels the output
 // needs are read.  A table entry of -1 is a pixel Pillow leaves at its fill value 0.
 //
-// frames_rgb8_kernel: one thread per 4 output pixels of a row, all three channels; the value is
+// frames_rgb8_kernel<Op>: one thread per 4 output pixels of a row, all three channels.  FrameOut writes
 //   ((float)x / 255 - mean[c]) / std[c], ToTensor's div(255) then Normalize's sub_ and div_, each rounded as torch
-//   rounds it on the CPU (true divisions, no contraction).  float4 stores when res % 4 == 0.
-// labels_u8_kernel: the same gather on one byte per pixel, then the optional 256-entry int64 table (shared memory),
-//   written as int64; two 16-byte stores per thread when res % 4 == 0.
+//   rounds it on the CPU (true divisions, no contraction); float4 stores when res % 4 == 0.  StoreOut writes the raw
+//   bytes into row r0 + b of a resident store (stego_b200/dataset.py).
+// labels_u8_kernel<Op>: the same gather on one byte per pixel, then the optional 256-entry int64 table (shared memory);
+//   LabelOut writes int64 (two 16-byte stores per thread when res % 4 == 0), StoreOut the raw bytes.
+// dataset_batch_kernel: a training batch from the resident store, one sample per blockIdx.y and 16 bytes per thread:
+//   the frame through the same normalisation as FrameOut (fp32, or the bf16 round of it), the label through a
+//   256-entry int64 table, and the data set's mask of that label.
 #include "common.cuh"
 #include "host_util.h"
 
@@ -45,37 +49,92 @@ __device__ __forceinline__ void gather(const FrameArgs& a, int b, int y, int x0,
   }
 }
 
-__global__ void __launch_bounds__(FR_THREADS) frames_rgb8_kernel(FrameArgs a, float m0, float m1, float m2, float s0,
-                                                                  float s1, float s2, float* out) {
+// ToTensor's div(255) then Normalize's sub_ and div_ of one byte, each an IEEE fp32 operation: the one definition both
+// the loader frames and the resident-store batches use.
+__device__ __forceinline__ float normalize_u8(unsigned x, float mean, float stdv) {
+  return __fdiv_rn(__fsub_rn(__fdiv_rn(static_cast<float>(x), 255.0f), mean), stdv);
+}
+
+struct Norm {
+  float mean[3], stdv[3];
+};
+
+// Output ops of the gather kernels: put(b, c, y, x0, v) writes output pixels (y, x0 .. x0 + FR_PIX) of channel c of
+// image b, v[k] being the gathered byte (frames) or its table value (labels); pixels past res are not written.
+struct FrameOut {  // fp32 [B][3][res][res], normalised
+  Norm n;
+  float* out;
+  int res;
+  __device__ __forceinline__ void put(int b, int c, int y, int x0, const unsigned (&x)[FR_PIX]) const {
+    float v[FR_PIX];
+#pragma unroll
+    for (int k = 0; k < FR_PIX; ++k) v[k] = normalize_u8(x[k], n.mean[c], n.stdv[c]);
+    const size_t plane = static_cast<size_t>(res) * res;
+    float* o = out + (static_cast<size_t>(b) * 3 + c) * plane + static_cast<size_t>(y) * res + x0;
+    if ((res & (FR_PIX - 1)) == 0) {
+      *reinterpret_cast<float4*>(o) = make_float4(v[0], v[1], v[2], v[3]);
+    } else {
+#pragma unroll
+      for (int k = 0; k < FR_PIX; ++k)
+        if (x0 + k < res) o[k] = v[k];
+    }
+  }
+};
+
+struct LabelOut {  // int64 [B][res][res]
+  long long* out;
+  int res;
+  __device__ __forceinline__ void put(int b, int, int y, int x0, const long long (&v)[FR_PIX]) const {
+    long long* o = out + (static_cast<size_t>(b) * res + y) * res + x0;
+    if ((res & (FR_PIX - 1)) == 0) {
+      reinterpret_cast<longlong2*>(o)[0] = make_longlong2(v[0], v[1]);
+      reinterpret_cast<longlong2*>(o)[1] = make_longlong2(v[2], v[3]);
+    } else {
+#pragma unroll
+      for (int k = 0; k < FR_PIX; ++k)
+        if (x0 + k < res) o[k] = v[k];
+    }
+  }
+};
+
+struct StoreOut {  // uint8 rows [n][channels][res][res] of a resident store; image b goes to row r0 + b
+  unsigned char* out;
+  long long r0;
+  int channels, res;
+  template <typename T>
+  __device__ __forceinline__ void put(int b, int c, int y, int x0, const T (&v)[FR_PIX]) const {
+    const size_t plane = static_cast<size_t>(res) * res;
+    unsigned char* o = out + (static_cast<size_t>(r0 + b) * channels + c) * plane + static_cast<size_t>(y) * res + x0;
+    if ((res & (FR_PIX - 1)) == 0) {
+      *reinterpret_cast<uchar4*>(o) = make_uchar4(static_cast<unsigned char>(v[0]), static_cast<unsigned char>(v[1]),
+                                                  static_cast<unsigned char>(v[2]), static_cast<unsigned char>(v[3]));
+    } else {
+#pragma unroll
+      for (int k = 0; k < FR_PIX; ++k)
+        if (x0 + k < res) o[k] = static_cast<unsigned char>(v[k]);
+    }
+  }
+};
+
+template <class Op>
+__global__ void __launch_bounds__(FR_THREADS) frames_rgb8_kernel(FrameArgs a, Op op) {
   const int b = blockIdx.y;
   const int idx = blockIdx.x * FR_THREADS + threadIdx.x;
   if (idx >= a.res * a.quads) return;
   const int y = idx / a.quads, x0 = (idx - y * a.quads) * FR_PIX;
   const unsigned char* src[FR_PIX];
   gather<3>(a, b, y, x0, src);
-  const float mean[3] = {m0, m1, m2}, stdv[3] = {s0, s1, s2};
-  const size_t plane = static_cast<size_t>(a.res) * a.res;
-  float* o = out + static_cast<size_t>(b) * 3 * plane + static_cast<size_t>(y) * a.res + x0;
 #pragma unroll
   for (int c = 0; c < 3; ++c) {
-    float v[FR_PIX];
+    unsigned x[FR_PIX];
 #pragma unroll
-    for (int k = 0; k < FR_PIX; ++k) {
-      const float x = src[k] ? static_cast<float>(src[k][c]) : 0.0f;
-      v[k] = __fdiv_rn(__fsub_rn(__fdiv_rn(x, 255.0f), mean[c]), stdv[c]);
-    }
-    float* oc = o + c * plane;
-    if ((a.res & (FR_PIX - 1)) == 0) {
-      *reinterpret_cast<float4*>(oc) = make_float4(v[0], v[1], v[2], v[3]);
-    } else {
-#pragma unroll
-      for (int k = 0; k < FR_PIX; ++k)
-        if (x0 + k < a.res) oc[k] = v[k];
-    }
+    for (int k = 0; k < FR_PIX; ++k) x[k] = src[k] ? src[k][c] : 0u;
+    op.put(b, c, y, x0, x);
   }
 }
 
-__global__ void __launch_bounds__(FR_THREADS) labels_u8_kernel(FrameArgs a, const long long* lut, long long* out) {
+template <class Op>
+__global__ void __launch_bounds__(FR_THREADS) labels_u8_kernel(FrameArgs a, const long long* lut, Op op) {
   __shared__ long long table[256];
   if (lut) {
     for (int i = threadIdx.x; i < 256; i += FR_THREADS) table[i] = lut[i];
@@ -93,14 +152,125 @@ __global__ void __launch_bounds__(FR_THREADS) labels_u8_kernel(FrameArgs a, cons
     const int id = src[k] ? *src[k] : 0;
     v[k] = lut ? table[id] : id;
   }
-  long long* o = out + (static_cast<size_t>(b) * a.res + y) * a.res + x0;
-  if ((a.res & (FR_PIX - 1)) == 0) {
-    reinterpret_cast<longlong2*>(o)[0] = make_longlong2(v[0], v[1]);
-    reinterpret_cast<longlong2*>(o)[1] = make_longlong2(v[2], v[3]);
+  op.put(b, 0, y, x0, v);
+}
+
+// ---- training batches from a resident store ------------------------------------------------------------------------
+constexpr int DB_THREADS = 256, DB_BYTES = 16;  // 16 store bytes (one 16-byte load) per thread
+enum : int { MASK_IS_IGNORE = 0, MASK_IS_POSITIVE = 1 };  // bool (label == -1), CroppedDataset; fp32 (label > 0)
+
+struct BatchArgs {
+  const unsigned char* images;  // [n][3][res][res]
+  const unsigned char* labels;  // [n][res][res], or null: every pixel reads id 0
+  const long long* index;       // [count] store rows
+  const long long* lut;         // [256]
+  Norm n;
+  void* img;                    // [count][3][res][res] fp32 or bf16
+  long long* label;             // [count][res][res]
+  void* mask;                   // [count][res][res] bool or fp32
+  int res, img_chunks, lab_chunks;
+};
+
+__device__ __forceinline__ void store16(float* o, const float (&v)[DB_BYTES]) {
+#pragma unroll
+  for (int k = 0; k < DB_BYTES; k += 4) *reinterpret_cast<float4*>(o + k) = make_float4(v[k], v[k + 1], v[k + 2], v[k + 3]);
+}
+__device__ __forceinline__ void store16(bf16* o, const float (&v)[DB_BYTES]) {
+#pragma unroll
+  for (int k = 0; k < DB_BYTES; k += 8) {
+    uint4 w;
+    __nv_bfloat162* h = reinterpret_cast<__nv_bfloat162*>(&w);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) h[j] = __floats2bfloat162_rn(v[k + 2 * j], v[k + 2 * j + 1]);
+    *reinterpret_cast<uint4*>(o + k) = w;
+  }
+}
+__device__ __forceinline__ void put1(float* o, float v) { *o = v; }
+__device__ __forceinline__ void put1(bf16* o, float v) { *o = __float2bfloat16_rn(v); }
+
+// The 16 bytes at element e0 of a row of `len` bytes (fewer past its end), as 16-byte loads when rows are 16-byte
+// multiples (res % 4 == 0), byte loads otherwise.
+__device__ __forceinline__ void load16(const unsigned char* row, long long e0, long long len, bool vec,
+                                       unsigned (&x)[DB_BYTES]) {
+  if (vec) {
+    const uint4 w = *reinterpret_cast<const uint4*>(row + e0);
+    const unsigned words[4] = {w.x, w.y, w.z, w.w};
+#pragma unroll
+    for (int k = 0; k < DB_BYTES; ++k) x[k] = (words[k >> 2] >> (8 * (k & 3))) & 0xffu;
   } else {
 #pragma unroll
-    for (int k = 0; k < FR_PIX; ++k)
-      if (x0 + k < a.res) o[k] = v[k];
+    for (int k = 0; k < DB_BYTES; ++k) x[k] = e0 + k < len ? row[e0 + k] : 0u;
+  }
+}
+
+template <typename T, int MASK>
+__global__ void __launch_bounds__(DB_THREADS) dataset_batch_kernel(BatchArgs a) {
+  __shared__ long long table[256];
+  __shared__ long long row_of;
+  for (int i = threadIdx.x; i < 256; i += DB_THREADS) table[i] = a.lut[i];
+  if (threadIdx.x == 0) row_of = a.index[blockIdx.y];  // one read of the (possibly host-resident) index record
+  __syncthreads();
+  const int s = blockIdx.y;
+  const long long row = row_of;
+  const long long plane = static_cast<long long>(a.res) * a.res;
+  const bool vec = (a.res & 3) == 0;  // then every plane is a multiple of 16 bytes
+  const int chunk = blockIdx.x * DB_THREADS + threadIdx.x;
+  unsigned x[DB_BYTES];
+  if (chunk < a.img_chunks) {
+    const long long e0 = static_cast<long long>(chunk) * DB_BYTES, len = 3 * plane;
+    load16(a.images + row * len, e0, len, vec, x);
+    T* o = static_cast<T*>(a.img) + s * len + e0;
+    if (vec) {  // the 16 elements lie in one channel plane
+      const int c = static_cast<int>(e0 / plane);
+      float v[DB_BYTES];
+#pragma unroll
+      for (int k = 0; k < DB_BYTES; ++k) v[k] = normalize_u8(x[k], a.n.mean[c], a.n.stdv[c]);
+      store16(o, v);
+    } else {
+#pragma unroll
+      for (int k = 0; k < DB_BYTES; ++k) {
+        if (e0 + k >= len) break;
+        const int c = static_cast<int>((e0 + k) / plane);
+        put1(o + k, normalize_u8(x[k], a.n.mean[c], a.n.stdv[c]));
+      }
+    }
+  } else if (chunk - a.img_chunks < a.lab_chunks) {
+    const long long e0 = static_cast<long long>(chunk - a.img_chunks) * DB_BYTES;
+    if (a.labels) {
+      load16(a.labels + row * plane, e0, plane, vec, x);
+    } else {
+#pragma unroll
+      for (int k = 0; k < DB_BYTES; ++k) x[k] = 0u;
+    }
+    long long v[DB_BYTES];
+#pragma unroll
+    for (int k = 0; k < DB_BYTES; ++k) v[k] = table[x[k]];
+    long long* lo = a.label + s * plane + e0;
+    if (vec) {
+#pragma unroll
+      for (int k = 0; k < DB_BYTES; k += 2) *reinterpret_cast<longlong2*>(lo + k) = make_longlong2(v[k], v[k + 1]);
+      if (MASK == MASK_IS_IGNORE) {
+        unsigned w[4] = {0u, 0u, 0u, 0u};
+#pragma unroll
+        for (int k = 0; k < DB_BYTES; ++k) w[k >> 2] |= static_cast<unsigned>(v[k] == -1) << (8 * (k & 3));
+        *reinterpret_cast<uint4*>(static_cast<unsigned char*>(a.mask) + s * plane + e0) = make_uint4(w[0], w[1], w[2], w[3]);
+      } else {
+        float m[DB_BYTES];
+#pragma unroll
+        for (int k = 0; k < DB_BYTES; ++k) m[k] = v[k] > 0 ? 1.0f : 0.0f;
+        store16(static_cast<float*>(a.mask) + s * plane + e0, m);
+      }
+    } else {
+#pragma unroll
+      for (int k = 0; k < DB_BYTES; ++k) {
+        if (e0 + k >= plane) break;
+        lo[k] = v[k];
+        if (MASK == MASK_IS_IGNORE)
+          static_cast<unsigned char*>(a.mask)[s * plane + e0 + k] = v[k] == -1;
+        else
+          static_cast<float*>(a.mask)[s * plane + e0 + k] = v[k] > 0 ? 1.0f : 0.0f;
+      }
+    }
   }
 }
 
@@ -146,6 +316,38 @@ static dim3 frames_grid(const FrameArgs& a, int B) {
   return dim3(static_cast<unsigned>((static_cast<long long>(a.res) * a.quads + FR_THREADS - 1) / FR_THREADS), B);
 }
 
+
+// The address a kernel reads or writes `p` through: `p` itself for device memory, the mapped device pointer of pinned
+// (page-locked) host memory.  Pageable host memory is refused.
+static int device_view(const char* who, const char* what, const void* p, const void** dev, bool* on_host) {
+  cudaPointerAttributes attr;
+  const cudaError_t e = cudaPointerGetAttributes(&attr, p);
+  if (e != cudaSuccess) return cuda_fail(e, who);
+  if (attr.type == cudaMemoryTypeDevice || attr.type == cudaMemoryTypeManaged) {
+    *dev = p;
+    *on_host = false;
+    return STEGO_OK;
+  }
+  STEGO_CHECK_ARG(attr.type == cudaMemoryTypeHost && attr.devicePointer,
+                  "%s: %s is neither device memory nor pinned host memory", who, what);
+  *dev = attr.devicePointer;
+  *on_host = true;
+  return STEGO_OK;
+}
+
+// Checks a store-build call (rows r0 .. r0 + B of an n-row store, 16-byte aligned) and resolves the store's address.
+static int check_store(const char* who, unsigned char* store, long long n, long long r0, int B, unsigned char** dev) {
+  STEGO_CHECK_ARG(store, "%s: null store", who);
+  STEGO_CHECK_ARG(reinterpret_cast<uintptr_t>(store) % 16 == 0, "%s: store must be 16-byte aligned", who);
+  STEGO_CHECK_ARG(n >= 1 && r0 >= 0 && r0 <= n - B, "%s: rows %lld .. %lld of a %lld-row store", who, r0, r0 + B, n);
+  const void* d = nullptr;
+  bool on_host = false;
+  const int rc = device_view(who, "store", store, &d, &on_host);
+  if (rc != STEGO_OK) return rc;
+  *dev = static_cast<unsigned char*>(const_cast<void*>(d));
+  return STEGO_OK;
+}
+
 }  // namespace stego
 
 using namespace stego;
@@ -160,7 +362,8 @@ extern "C" int stego_frames_rgb8(const void* staging_host, const void* staging_d
   FrameArgs a;
   const int rc = check_staging("stego_frames_rgb8", staging_host, staging_dev, bytes, B, res, table_words, 3, a);
   if (rc != STEGO_OK) return rc;
-  frames_rgb8_kernel<<<frames_grid(a, B), FR_THREADS, 0, stream>>>(a, mean0, mean1, mean2, std0, std1, std2, out);
+  const FrameOut op{{{mean0, mean1, mean2}, {std0, std1, std2}}, out, res};
+  frames_rgb8_kernel<<<frames_grid(a, B), FR_THREADS, 0, stream>>>(a, op);
   STEGO_CHECK_LAUNCH("frames_rgb8_kernel launch");
   return STEGO_OK;
 }
@@ -175,7 +378,100 @@ extern "C" int stego_labels_u8(const void* staging_host, const void* staging_dev
   FrameArgs a;
   const int rc = check_staging("stego_labels_u8", staging_host, staging_dev, bytes, B, res, table_words, 1, a);
   if (rc != STEGO_OK) return rc;
-  labels_u8_kernel<<<frames_grid(a, B), FR_THREADS, 0, stream>>>(a, lut, out);
+  labels_u8_kernel<<<frames_grid(a, B), FR_THREADS, 0, stream>>>(a, lut, LabelOut{out, res});
   STEGO_CHECK_LAUNCH("labels_u8_kernel launch");
+  return STEGO_OK;
+}
+
+extern "C" int stego_frames_store_rgb8(const void* staging_host, const void* staging_dev, long long bytes,
+                                       long long table_words, int B, int res, unsigned char* store, long long n,
+                                       long long r0, void* stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  FrameArgs a;
+  int rc = check_staging("stego_frames_store_rgb8", staging_host, staging_dev, bytes, B, res, table_words, 3, a);
+  if (rc != STEGO_OK) return rc;
+  unsigned char* dev = nullptr;
+  rc = check_store("stego_frames_store_rgb8", store, n, r0, B, &dev);
+  if (rc != STEGO_OK) return rc;
+  frames_rgb8_kernel<<<frames_grid(a, B), FR_THREADS, 0, stream>>>(a, StoreOut{dev, r0, 3, res});
+  STEGO_CHECK_LAUNCH("frames_rgb8_kernel<StoreOut> launch");
+  return STEGO_OK;
+}
+
+extern "C" int stego_labels_store_u8(const void* staging_host, const void* staging_dev, long long bytes,
+                                     long long table_words, int B, int res, unsigned char* store, long long n,
+                                     long long r0, void* stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  FrameArgs a;
+  int rc = check_staging("stego_labels_store_u8", staging_host, staging_dev, bytes, B, res, table_words, 1, a);
+  if (rc != STEGO_OK) return rc;
+  unsigned char* dev = nullptr;
+  rc = check_store("stego_labels_store_u8", store, n, r0, B, &dev);
+  if (rc != STEGO_OK) return rc;
+  labels_u8_kernel<<<frames_grid(a, B), FR_THREADS, 0, stream>>>(a, nullptr, StoreOut{dev, r0, 1, res});
+  STEGO_CHECK_LAUNCH("labels_u8_kernel<StoreOut> launch");
+  return STEGO_OK;
+}
+
+extern "C" int stego_dataset_batch(const unsigned char* images, const unsigned char* labels, long long n, int res,
+                                   const long long* index, int count, const long long* lut, float mean0, float mean1,
+                                   float mean2, float std0, float std1, float std2, int out_bf16, int mask_kind,
+                                   void* img, long long* label, void* mask, void* stream_) {
+  static const char* who = "stego_dataset_batch";
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  STEGO_CHECK_ARG(images && index && lut && img && label && mask, "%s: null pointer", who);
+  STEGO_CHECK_ARG(n >= 1, "%s: n=%lld rows", who, n);
+  STEGO_CHECK_ARG(res >= 1 && res <= 8192, "%s: res=%d (1..8192)", who, res);
+  STEGO_CHECK_ARG(count >= 1 && count <= 65535, "%s: count=%d (1..65535)", who, count);
+  STEGO_CHECK_ARG(out_bf16 == 0 || out_bf16 == 1, "%s: out_bf16=%d (0 or 1)", who, out_bf16);
+  STEGO_CHECK_ARG(mask_kind == MASK_IS_IGNORE || mask_kind == MASK_IS_POSITIVE, "%s: mask_kind=%d (0 or 1)", who,
+                  mask_kind);
+  STEGO_CHECK_ARG(reinterpret_cast<uintptr_t>(images) % 16 == 0 && reinterpret_cast<uintptr_t>(labels) % 16 == 0,
+                  "%s: the stores must be 16-byte aligned", who);
+  STEGO_CHECK_ARG(reinterpret_cast<uintptr_t>(lut) % 8 == 0, "%s: lut must be 8-byte aligned", who);
+  STEGO_CHECK_ARG(reinterpret_cast<uintptr_t>(img) % 16 == 0 && reinterpret_cast<uintptr_t>(label) % 16 == 0 &&
+                      reinterpret_cast<uintptr_t>(mask) % 16 == 0,
+                  "%s: outputs must be 16-byte aligned", who);
+  BatchArgs a;
+  bool on_host = false;
+  const void* d = nullptr;
+  int rc = device_view(who, "index", index, &d, &on_host);
+  if (rc != STEGO_OK) return rc;
+  STEGO_CHECK_ARG(on_host, "%s: index must be pinned host memory (it is checked on the host)", who);
+  for (int i = 0; i < count; ++i)
+    STEGO_CHECK_ARG(index[i] >= 0 && index[i] < n, "%s: index[%d]=%lld outside the %lld-row store", who, i, index[i],
+                    n);
+  a.index = static_cast<const long long*>(d);
+  rc = device_view(who, "images", images, &d, &on_host);
+  if (rc != STEGO_OK) return rc;
+  a.images = static_cast<const unsigned char*>(d);
+  a.labels = nullptr;
+  if (labels) {
+    rc = device_view(who, "labels", labels, &d, &on_host);
+    if (rc != STEGO_OK) return rc;
+    a.labels = static_cast<const unsigned char*>(d);
+  }
+  a.lut = lut;
+  a.n = Norm{{mean0, mean1, mean2}, {std0, std1, std2}};
+  a.img = img;
+  a.label = label;
+  a.mask = mask;
+  a.res = res;
+  const long long plane = static_cast<long long>(res) * res;
+  a.img_chunks = static_cast<int>((3 * plane + DB_BYTES - 1) / DB_BYTES);
+  a.lab_chunks = static_cast<int>((plane + DB_BYTES - 1) / DB_BYTES);
+  const dim3 grid(static_cast<unsigned>((a.img_chunks + a.lab_chunks + DB_THREADS - 1) / DB_THREADS), count);
+  if (out_bf16) {
+    if (mask_kind == MASK_IS_IGNORE)
+      dataset_batch_kernel<bf16, MASK_IS_IGNORE><<<grid, DB_THREADS, 0, stream>>>(a);
+    else
+      dataset_batch_kernel<bf16, MASK_IS_POSITIVE><<<grid, DB_THREADS, 0, stream>>>(a);
+  } else {
+    if (mask_kind == MASK_IS_IGNORE)
+      dataset_batch_kernel<float, MASK_IS_IGNORE><<<grid, DB_THREADS, 0, stream>>>(a);
+    else
+      dataset_batch_kernel<float, MASK_IS_POSITIVE><<<grid, DB_THREADS, 0, stream>>>(a);
+  }
+  STEGO_CHECK_LAUNCH("dataset_batch_kernel launch");
   return STEGO_OK;
 }

@@ -1,0 +1,431 @@
+"""A training set kept resident on the GPU (or in pinned host memory): frames, labels and kNN positives of every step
+gathered in one launch, the batches of the reference's training loader bit for bit.
+
+The reference trains from `ContrastiveSegDataset` (src/data.py:419-565) over `CroppedDataset` (the five-crop sets) or
+`DirectoryDataset`, read with get_transform(res, ., "center"): a nearest resize and a centre crop, with no randomness.
+Its host workers open and decode the anchor and its kNN positive for every sample of every step.  The frames are a
+function of the index alone, so `ResidentDataset` decodes each file once, runs the transform once on the GPU (the
+gather of stego_b200/frames.py, writing the raw bytes: stego_frames_store_rgb8 / stego_labels_store_u8) and keeps
+
+    images uint8 [n, 3, res, res] and labels uint8 [n, res, res]: 4 * res^2 bytes per sample (200,704 B at 224^2),
+
+on the device (location="cuda") or in pinned host memory read over PCIe (location="host").  Each step is then one
+launch (stego_dataset_batch) that gathers the 2B rows of its anchors and positives, normalises the frames with the
+arithmetic of load_frames, maps the label bytes through the class's remap and writes its mask.
+
+What is drawn per step is drawn on the host, in the reference's order and from private generators (`Sampler`): the
+shuffle order (RandomSampler, or DistributedSampler with set_epoch), and per sample the data set's numpy seed, the
+neighbour rank and the aug seed, with the numpy streams of DataLoader(num_workers=W) workers.  The global numpy,
+`random` and torch generators never move; in particular torch.manual_seed is never called, so the CUDA generators the
+training step's dropout draws from are untouched.
+"""
+from __future__ import annotations
+
+import math
+import os
+
+import numpy as np
+import torch
+from PIL import Image
+from torch.utils.data import DataLoader, Dataset
+
+from . import _lib, frames
+
+KINDS = ("cropped", "directory")
+LOCATIONS = ("cuda", "host")
+MASK_IS_IGNORE, MASK_IS_POSITIVE = 0, 1  # stego_dataset_batch's mask_kind: CroppedDataset's, DirectoryDataset's
+SEED_HIGH = 2147483647                    # np.random.randint(2147483647), src/data.py:102, 387, 527
+RRC_SCALE, RRC_RATIO = (0.8, 1.0), (3.0 / 4.0, 4.0 / 3.0)  # the geometric aug of src/train_segmentation.py:408-411
+REFUSED = {"cocostuff3": "Coco", "cocostuff15": "Coco", "cocostuff27": "Coco (uncropped)", "cityscapes": "CityscapesSeg",
+           "potsdam": "Potsdam", "potsdamraw": "PotsdamRaw"}
+
+
+def _generate_state(base_seed: int, worker_id: int) -> list:
+    """The four uint32 words a DataLoader worker seeds numpy with (torch/utils/data/_utils/worker.py _generate_state,
+    a SeedSequence-style hash of [worker_id, base_seed low, base_seed high, 0])."""
+    mask = 0xFFFFFFFF
+    mult_a, mult_b, mix_l, mix_r, shift = 0x931E8875, 0x58F38DED, 0xCA01F9DD, 0x4973F715, 16
+    hash_a = 0x43B0D7E5
+
+    def hashed(value):
+        nonlocal hash_a
+        value = (value ^ hash_a) & mask
+        hash_a = (hash_a * mult_a) & mask
+        value = (value * hash_a) & mask
+        return (value ^ (value >> shift)) & mask
+
+    def mix(x, y):
+        r = (((mix_l * x) & mask) - ((mix_r * y) & mask)) & mask
+        return (r ^ (r >> shift)) & mask
+
+    pool = [hashed(v) for v in (worker_id, base_seed & mask, base_seed >> 32, 0)]
+    for i_src in range(4):
+        for i_dst in range(4):
+            if i_src != i_dst:
+                pool[i_dst] = mix(pool[i_dst], hashed(pool[i_src]))
+    hash_b, state = 0x8B51F9DD, []
+    for v in pool:
+        v = (v ^ hash_b) & mask
+        hash_b = (hash_b * mult_b) & mask
+        v = (v * hash_b) & mask
+        state.append((v ^ (v >> shift)) & mask)
+    return state
+
+
+def _draw_int64(g: torch.Generator) -> int:
+    """torch.empty((), dtype=torch.int64).random_(): the DataLoader's base seed and RandomSampler's epoch seed."""
+    return int(torch.empty((), dtype=torch.int64).random_(generator=g).item())
+
+
+def _after_geometric_aug(seed: int, res: int) -> torch.Tensor:
+    """The CPU generator state a single-process reference loader leaves after a sample whose aug seed is `seed`: its
+    last draws are the geometric pair on coord (src/data.py:559-560): RandomHorizontalFlip, then RandomResizedCrop on
+    [2, res, res].  Made on a forked default generator, so the caller's state is unchanged."""
+    import torchvision.transforms as T
+    with torch.random.fork_rng(devices=[]):
+        torch.default_generator.manual_seed(seed)
+        torch.rand(1)
+        T.RandomResizedCrop.get_params(torch.empty(1, 1, 1).expand(2, res, res), list(RRC_SCALE), list(RRC_RATIO))
+        return torch.get_rng_state()
+
+
+class Sampler:
+    """The host draws of the reference's training loader, `DataLoader(ContrastiveSegDataset(...), batch_size,
+    shuffle=True, num_workers=loader_workers)` after seed_everything(seed), per batch: (ind, ind_pos, seed) int64
+    arrays.  Iterating gives one iterator per epoch.
+
+    - Order: RandomSampler, seeded per epoch from the main process's torch generator (drawn after the DataLoader
+      iterator's base seed); with world_size > 1, DistributedSampler(shuffle=True, seed=seed) with set_epoch(epoch) and
+      its padding.  The last batch may be partial.
+    - Per sample, from the numpy stream of the process that loads it: dataset[ind]'s np.random.randint, whose
+      torch.manual_seed seeds the neighbour rank torch.randint(1, num_neighbors + 1, []); then dataset[ind_pos]'s draw
+      and the aug seed.
+    - loader_workers = 0: one numpy stream for the whole run (np.random.seed(seed)), and the main torch generator is
+      the one the samples reseed: each epoch's seeds follow the state its last sample's geometric aug draws leave
+      (src/train_segmentation.py:408-429).  W >= 1: a fresh worker set per epoch; worker w seeds numpy with
+      _generate_state(base_seed, w), and batch i goes to worker i % W.
+    """
+
+    def __init__(self, nns, batch_size: int, num_neighbors: int, seed: int, loader_workers: int = 0, rank: int = 0,
+                 world_size: int = 1, res: int = 224):
+        self.nns = nns
+        self.n = nns.shape[0]
+        self.batch_size, self.num_neighbors, self.seed = batch_size, num_neighbors, seed
+        self.workers, self.rank, self.world_size, self.res = loader_workers, rank, world_size, res
+        self.main = torch.Generator()
+        self.main.manual_seed(seed)
+        self.np_main = np.random.RandomState(seed)
+        self.epoch = 0
+        self._open = None
+
+    def __iter__(self):
+        return self
+
+    def __next__(self):
+        if self._open is not None and self.workers == 0:
+            for _ in self._open:  # the next epoch starts from the state this one's last sample leaves
+                pass
+        base = _draw_int64(self.main)
+        order = self.order()
+        self._open = self._epoch(order, base)
+        self.epoch += 1
+        return self._open
+
+    def order(self) -> list:
+        """This epoch's sample order (this rank's share with world_size > 1)."""
+        if self.world_size == 1:
+            g = torch.Generator()
+            g.manual_seed(_draw_int64(self.main))
+            return torch.randperm(self.n, generator=g).tolist()
+        g = torch.Generator()
+        g.manual_seed(self.seed + self.epoch)
+        indices = torch.randperm(self.n, generator=g).tolist()
+        num_samples = math.ceil(self.n / self.world_size)
+        total = num_samples * self.world_size
+        pad = total - len(indices)
+        indices += indices[:pad] if pad <= len(indices) else (indices * math.ceil(pad / len(indices)))[:pad]
+        return indices[self.rank:total:self.world_size]
+
+    def _epoch(self, order: list, base: int):
+        B = self.batch_size
+        streams = ([self.np_main] if self.workers == 0 else
+                   [np.random.RandomState(_generate_state(base, w)) for w in range(self.workers)])
+        g = torch.Generator()
+        aug_seed = None
+        for i, start in enumerate(range(0, len(order), B)):
+            rs = streams[i % len(streams)]
+            ind = order[start:start + B]
+            pos, seeds = [], []
+            for j in ind:
+                g.manual_seed(int(rs.randint(SEED_HIGH)))
+                k = int(torch.randint(low=1, high=self.num_neighbors + 1, size=[], generator=g))
+                pos.append(int(self.nns[j][k]))
+                rs.randint(SEED_HIGH)
+                aug_seed = int(rs.randint(SEED_HIGH))
+                seeds.append(aug_seed)
+            if self.workers == 0 and start + B >= len(order):
+                self.main.set_state(_after_geometric_aug(aug_seed, self.res))
+            yield (np.asarray(ind, dtype=np.int64), np.asarray(pos, dtype=np.int64), np.asarray(seeds, dtype=np.int64))
+
+
+def _check_int(value, name: str, lo: int, hi: int, who: str) -> int:
+    if isinstance(value, bool) or not isinstance(value, (int, np.integer)) or not lo <= value <= hi:
+        raise ValueError(f"stego_b200.dataset.{who}: {name}={value!r} (an int in {lo}..{hi})")
+    return int(value)
+
+
+class _Files(Dataset):
+    """(image array, label array or None) per index, decoded as the reference's class opens them."""
+
+    def __init__(self, images: list, labels, convert: bool):
+        self.images, self.labels, self.convert = images, labels, convert
+
+    def __getitem__(self, index):
+        with Image.open(self.images[index]) as im:
+            img = np.asarray(im.convert("RGB") if self.convert else im)
+        if self.labels is None:
+            return img, None
+        with Image.open(self.labels[index]) as im:
+            return img, np.asarray(im)
+
+    def __len__(self):
+        return len(self.images)
+
+
+def _as_list(batch):
+    return batch
+
+
+class ResidentDataset:
+    """The training set of a CroppedDataset (kind="cropped") or DirectoryDataset (kind="directory") resident in memory.
+
+    n samples at res: 4 * res^2 bytes each (3 * res^2 of image, res^2 of label), 200,704 B at 224^2.  location="cuda"
+    keeps them in device memory, location="host" in pinned host memory that the batch kernel reads over PCIe; the
+    caller chooses from the set's size.  Rows are filled in order by `append` (or the `cropped` / `directory`
+    constructors); `frames` and `batches` need all n."""
+
+    def __init__(self, n: int, res: int, kind: str = "cropped", location: str = "cuda", has_labels: bool = True):
+        who = "ResidentDataset"
+        if kind in REFUSED:
+            raise ValueError(f"stego_b200.dataset.{who}: {kind!r} is read by {REFUSED[kind]}, which is not a training "
+                             f"set class; load_frames / load_labels build its batches")
+        if kind not in KINDS:
+            raise ValueError(f"stego_b200.dataset.{who}: kind={kind!r} (\"cropped\" or \"directory\")")
+        if location not in LOCATIONS:
+            raise ValueError(f"stego_b200.dataset.{who}: location={location!r} (\"cuda\" or \"host\")")
+        if kind == "cropped" and not has_labels:
+            raise ValueError(f"stego_b200.dataset.{who}: a CroppedDataset always has labels")
+        self.n = _check_int(n, "n", 1, 1 << 40, who)
+        self.res = _check_int(res, "res", 1, 8192, who)
+        self.kind, self.location, self.has_labels = kind, location, bool(has_labels)
+        self.device = frames._require_cuda(who)
+        shape = (self.n, 3, self.res, self.res)
+        if location == "cuda":
+            self.images = torch.empty(shape, dtype=torch.uint8, device=self.device)
+            self.labels = (torch.empty(self.n, self.res, self.res, dtype=torch.uint8, device=self.device)
+                           if has_labels else None)
+        else:
+            self.images = torch.empty(shape, dtype=torch.uint8, pin_memory=True)
+            self.labels = torch.empty(self.n, self.res, self.res, dtype=torch.uint8, pin_memory=True) if has_labels else None
+        # CroppedDataset: label = byte - 1; DirectoryDataset: the byte, or -1 everywhere without a label folder
+        ids = torch.arange(256, dtype=torch.int64)
+        lut = ids - 1 if kind == "cropped" else (ids if has_labels else torch.full((256,), -1, dtype=torch.int64))
+        self._lut = lut.to(self.device)
+        self.count = 0
+        # pinned index records, used in turn: one is refilled once the launch that read it two steps earlier has run
+        self._ring = [torch.empty(0, dtype=torch.int64), torch.empty(0, dtype=torch.int64)]
+        self._ring_done = [None, None]
+        self._slot = 0
+
+    @property
+    def nbytes(self) -> int:
+        return 4 * self.n * self.res * self.res if self.has_labels else 3 * self.n * self.res * self.res
+
+    def append(self, images, labels=None) -> None:
+        """Transform and store the next len(images) samples: images as load_frames takes them (uint8 H x W x 3), labels
+        as load_labels (uint8 H x W), one per image (None without labels).  One build launch per store; the caller is
+        not synchronised."""
+        who = "ResidentDataset.append"
+        arrays = frames._as_arrays(images, 3, who)
+        if self.has_labels:
+            if labels is None:
+                raise ValueError(f"stego_b200.dataset.{who}: this store keeps labels; pass one label map per image")
+            label_arrays = frames._as_arrays(labels, 1, who)
+            if len(label_arrays) != len(arrays):
+                raise ValueError(f"stego_b200.dataset.{who}: {len(label_arrays)} label maps for {len(arrays)} images")
+        elif labels is not None:
+            raise ValueError(f"stego_b200.dataset.{who}: this store was made with has_labels=False")
+        B = len(arrays)
+        if self.count + B > self.n:
+            raise ValueError(f"stego_b200.dataset.{who}: {B} samples after {self.count} overflow the {self.n}-row store")
+        lib = _lib.load()
+        with torch.cuda.device(self.device):
+            staging, words, _ = frames._stage(arrays, self.res, "center")
+            staged = staging.to(self.device, non_blocking=True)
+            _lib.check(lib.stego_frames_store_rgb8(staging.data_ptr(), _lib.ptr(staged), staging.numel(), words, B,
+                                                   self.res, _lib.ptr(self.images), self.n, self.count, _lib.stream()),
+                       "stego_frames_store_rgb8")
+            if self.has_labels:
+                staging, words, _ = frames._stage(label_arrays, self.res, "center")
+                staged = staging.to(self.device, non_blocking=True)
+                _lib.check(lib.stego_labels_store_u8(staging.data_ptr(), _lib.ptr(staged), staging.numel(), words, B,
+                                                     self.res, _lib.ptr(self.labels), self.n, self.count,
+                                                     _lib.stream()), "stego_labels_store_u8")
+        self.count += B
+
+    @classmethod
+    def _from_files(cls, images, labels, convert, res, kind, location, batch_size, num_workers):
+        store = cls(len(images), res, kind, location, has_labels=labels is not None)
+        loader = DataLoader(_Files(images, labels, convert), batch_size, shuffle=False, num_workers=num_workers,
+                            collate_fn=_as_list)
+        for batch in loader:
+            store.append([b[0] for b in batch], [b[1] for b in batch] if labels is not None else None)
+        return store
+
+    @classmethod
+    def cropped(cls, root: str, dataset_name: str, crop_type: str, crop_ratio, image_set: str, res: int,
+                location: str = "cuda", batch_size: int = 64, num_workers: int = 0) -> "ResidentDataset":
+        """CroppedDataset(root, dataset_name, crop_type, crop_ratio, image_set, ...) (src/data.py:370-400): the files
+        {root}/cropped/{dataset_name}_{crop_type}_crop_{crop_ratio}/img/{image_set}/{i}.jpg (converted to RGB) and
+        label/{image_set}/{i}.png, decoded once in DataLoader(num_workers) workers."""
+        base = os.path.join(root, "cropped", "{}_{}_crop_{}".format(dataset_name, crop_type, crop_ratio))
+        img_dir, label_dir = os.path.join(base, "img", image_set), os.path.join(base, "label", image_set)
+        n = len(os.listdir(img_dir))
+        if n != len(os.listdir(label_dir)):
+            raise ValueError(f"stego_b200.dataset.ResidentDataset.cropped: {n} images but "
+                             f"{len(os.listdir(label_dir))} label files under {base}")
+        images = [os.path.join(img_dir, f"{i}.jpg") for i in range(n)]
+        labels = [os.path.join(label_dir, f"{i}.png") for i in range(n)]
+        return cls._from_files(images, labels, True, res, "cropped", location, batch_size, num_workers)
+
+    @classmethod
+    def directory(cls, root: str, path: str, image_set: str, res: int, location: str = "cuda", batch_size: int = 64,
+                  num_workers: int = 0) -> "ResidentDataset":
+        """DirectoryDataset(root, path, image_set, ...) (src/data.py:75-118): sorted listdir of {root}/{path}/imgs/
+        {image_set} and, when {root}/{path}/labels exists, of labels/{image_set}; the images are read as they are
+        (no convert), so they must decode to RGB."""
+        base = os.path.join(root, path)
+        img_dir, label_dir = os.path.join(base, "imgs", image_set), os.path.join(base, "labels", image_set)
+        names = sorted(os.listdir(img_dir))
+        if not names:
+            raise ValueError(f"stego_b200.dataset.ResidentDataset.directory: no images in {img_dir}")
+        labels = None
+        if os.path.exists(os.path.join(base, "labels")):
+            label_names = sorted(os.listdir(label_dir))
+            if len(label_names) != len(names):
+                raise ValueError(f"stego_b200.dataset.ResidentDataset.directory: {len(names)} images but "
+                                 f"{len(label_names)} label files")
+            labels = [os.path.join(label_dir, f) for f in label_names]
+        images = [os.path.join(img_dir, f) for f in names]
+        return cls._from_files(images, labels, False, res, "directory", location, batch_size, num_workers)
+
+    # ---- reading --------------------------------------------------------------------------------------------------
+    def _require_full(self, who: str) -> None:
+        if self.count != self.n:
+            raise ValueError(f"stego_b200.dataset.{who}: the store holds {self.count} of its {self.n} samples")
+
+    def _record(self, index: np.ndarray) -> torch.Tensor:
+        """The next pinned index record holding `index`, reused once the launch that read it last has run."""
+        if self._ring[0].numel() < index.size:  # both records grow together, once their readers have run
+            for j in (0, 1):
+                if self._ring_done[j] is not None:
+                    self._ring_done[j].synchronize()
+                self._ring[j] = torch.empty(index.size, dtype=torch.int64, pin_memory=True)
+        i = self._slot
+        self._slot ^= 1
+        if self._ring_done[i] is not None:
+            self._ring_done[i].synchronize()
+        self._ring[i].numpy()[:index.size] = index
+        return i
+
+    def _gather(self, index: np.ndarray, dtype) -> tuple:
+        """(img, label, mask) of the store rows `index`, one launch on the current stream."""
+        count, res = index.size, self.res
+        with torch.cuda.device(self.device):
+            i = self._record(index)
+            img = torch.empty(count, 3, res, res, dtype=dtype, device=self.device)
+            label = torch.empty(count, res, res, dtype=torch.int64, device=self.device)
+            mask_dtype = torch.bool if self.kind == "cropped" else torch.float32
+            mask = torch.empty(count, res, res, dtype=mask_dtype, device=self.device)
+            _lib.check(_lib.load().stego_dataset_batch(
+                _lib.ptr(self.images), _lib.ptr(self.labels), self.n, res, self._ring[i].data_ptr(), count,
+                _lib.ptr(self._lut), *frames.MEAN, *frames.STD, int(dtype == torch.bfloat16),
+                MASK_IS_IGNORE if self.kind == "cropped" else MASK_IS_POSITIVE, _lib.ptr(img), _lib.ptr(label),
+                _lib.ptr(mask), _lib.stream()), "stego_dataset_batch")
+            done = torch.cuda.Event()
+            done.record()
+            self._ring_done[i] = done
+        return img, label, mask
+
+    def _shaped(self, label, mask):
+        """The shapes the reference's classes return, batched: CroppedDataset label [B, res, res] and mask
+        [B, 1, res, res]; DirectoryDataset label and mask [B, 1, res, res] with a label folder, [B, res, res] without."""
+        B, res = label.shape[0], self.res
+        if self.kind == "cropped":
+            return label, mask.view(B, 1, res, res)
+        if self.has_labels:
+            return label.view(B, 1, res, res), mask.view(B, 1, res, res)
+        return label, mask
+
+    def frames(self, batch_size: int, dtype=torch.float32):
+        """Batches {"img", "label", "mask"} of the samples in index order: get_transform(res, ., "center") of each
+        image, as a shuffle=False loader yields them (precompute_knns(net, store.frames(b)) runs on them unchanged)."""
+        who = "ResidentDataset.frames"
+        self._require_full(who)
+        batch_size = _check_int(batch_size, "batch_size", 1, 65535, who)
+        self._check_dtype(dtype, who)
+        for start in range(0, self.n, batch_size):
+            img, label, mask = self._gather(np.arange(start, min(start + batch_size, self.n), dtype=np.int64), dtype)
+            label, mask = self._shaped(label, mask)
+            yield dict(img=img, label=label, mask=mask)
+
+    @staticmethod
+    def _check_dtype(dtype, who: str) -> None:
+        if dtype not in (torch.float32, torch.bfloat16):
+            raise ValueError(f"stego_b200.dataset.{who}: dtype={dtype} (torch.float32 or torch.bfloat16)")
+
+    def batches(self, nns, batch_size: int, num_neighbors: int, seed: int, loader_workers: int = 0, rank: int = 0,
+                world_size: int = 1, dtype=torch.float32, res: int = None):
+        """The training loader: an iterator over epochs, each yielding the dicts training_step takes, those of
+        DataLoader(ContrastiveSegDataset(..., mask=True, pos_images=True, pos_labels=True), batch_size, shuffle=True,
+        num_workers=loader_workers) after seed_everything(seed) (the draws: `Sampler`).
+
+        ind, ind_pos (int64) and seed (B aug seeds, int64, from which the fused step builds the aug views) are CPU
+        tensors; img, img_pos (dtype), label, label_pos, mask and mask_pos are on the store's device, one launch per
+        step on the current stream with fresh outputs.  The host runs at most two steps ahead of the device.
+
+        nns: the kNN table [n, k] (precompute_knns), host array or tensor; num_neighbors 1 .. k - 1.  res, if given,
+        must be the store's."""
+        who = "ResidentDataset.batches"
+        self._require_full(who)
+        if res is not None and res != self.res:
+            raise ValueError(f"stego_b200.dataset.{who}: res={res!r} but the store holds {self.res}^2 frames")
+        self._check_dtype(dtype, who)
+        nns = np.asarray(nns.detach().cpu() if isinstance(nns, torch.Tensor) else nns)
+        if nns.ndim != 2 or not np.issubdtype(nns.dtype, np.integer):
+            raise ValueError(f"stego_b200.dataset.{who}: nns must be an integer table [n, k], got {nns.dtype} "
+                             f"{nns.shape}")
+        if nns.shape[0] != self.n:
+            raise ValueError(f"stego_b200.dataset.{who}: nns has {nns.shape[0]} rows for a {self.n}-sample store")
+        if nns.size and (nns.min() < 0 or nns.max() >= self.n):
+            raise ValueError(f"stego_b200.dataset.{who}: nns holds indices outside 0..{self.n - 1}")
+        if nns.shape[1] < 2:
+            raise ValueError(f"stego_b200.dataset.{who}: nns has {nns.shape[1]} column(s); a positive needs 2 or more")
+        batch_size = _check_int(batch_size, "batch_size", 1, 32767, who)
+        num_neighbors = _check_int(num_neighbors, "num_neighbors", 1, nns.shape[1] - 1, who)
+        seed = _check_int(seed, "seed", 0, (1 << 32) - 1, who)
+        loader_workers = _check_int(loader_workers, "loader_workers", 0, 1024, who)
+        world_size = _check_int(world_size, "world_size", 1, 1 << 20, who)
+        rank = _check_int(rank, "rank", 0, world_size - 1, who)
+        sampler = Sampler(nns, batch_size, num_neighbors, seed, loader_workers, rank, world_size, self.res)
+        for epoch in sampler:
+            yield self._epoch(epoch, dtype)
+
+    def _epoch(self, plan, dtype):
+        for ind, pos, seeds in plan:
+            B = ind.size
+            img, label, mask = self._gather(np.concatenate([ind, pos]), dtype)
+            label, mask = self._shaped(label, mask)
+            yield dict(ind=torch.from_numpy(ind), img=img[:B], img_pos=img[B:], ind_pos=torch.from_numpy(pos),
+                       label=label[:B], label_pos=label[B:], mask=mask[:B], mask_pos=mask[B:],
+                       seed=torch.from_numpy(seeds))
