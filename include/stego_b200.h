@@ -279,6 +279,13 @@ STEGO_API int stego_dataset_batch(const unsigned char* images, const unsigned ch
                                   const long long* index, int count, const long long* lut, float mean0, float mean1,
                                   float mean2, float std0, float std1, float std2, int out_bf16, int mask_kind,
                                   void* img, long long* label, void* mask, void* stream);
+/* A batch of a resident evaluation set (stego_b200/evalset.py EvalSet): stego_dataset_batch's arguments, store and
+ * contract, with a third mask rule for mask_kind 2 = bool (label >= 0) (Coco).  mask_kind 0 is CityscapesSeg's and
+ * 1 Potsdam's / PotsdamRaw's.  One launch; the call never synchronises and reads nothing back from the device. */
+STEGO_API int stego_evalset_batch(const unsigned char* images, const unsigned char* labels, long long n, int res,
+                                  const long long* index, int count, const long long* lut, float mean0, float mean1,
+                                  float mean2, float std0, float std1, float std2, int out_bf16, int mask_kind,
+                                  void* img, long long* label, void* mask, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * TensorBoard histograms (SummaryWriter.add_histogram with its default bins="tensorflow")

@@ -17,7 +17,8 @@
 //   LabelOut writes int64 (two 16-byte stores per thread when res % 4 == 0), StoreOut the raw bytes.
 // dataset_batch_kernel: a training batch from the resident store, one sample per blockIdx.y and 16 bytes per thread:
 //   the frame through the same normalisation as FrameOut (fp32, or the bf16 round of it), the label through a
-//   256-entry int64 table, and the data set's mask of that label.
+//   256-entry int64 table, and the data set's mask of that label.  The evaluation-set batches (stego_evalset_batch,
+//   stego_b200/evalset.py) are the same kernel with a third mask rule, bool (label >= 0) for Coco.
 #include "common.cuh"
 #include "host_util.h"
 
@@ -157,7 +158,9 @@ __global__ void __launch_bounds__(FR_THREADS) labels_u8_kernel(FrameArgs a, cons
 
 // ---- training batches from a resident store ------------------------------------------------------------------------
 constexpr int DB_THREADS = 256, DB_BYTES = 16;  // 16 store bytes (one 16-byte load) per thread
-enum : int { MASK_IS_IGNORE = 0, MASK_IS_POSITIVE = 1 };  // bool (label == -1), CroppedDataset; fp32 (label > 0)
+// bool (label == -1): CroppedDataset, CityscapesSeg; fp32 (label > 0): DirectoryDataset, Potsdam, PotsdamRaw;
+// bool (label >= 0): Coco (evaluation sets only)
+enum : int { MASK_IS_IGNORE = 0, MASK_IS_POSITIVE = 1, MASK_IS_NONNEG = 2 };
 
 struct BatchArgs {
   const unsigned char* images;  // [n][3][res][res]
@@ -249,10 +252,11 @@ __global__ void __launch_bounds__(DB_THREADS) dataset_batch_kernel(BatchArgs a) 
     if (vec) {
 #pragma unroll
       for (int k = 0; k < DB_BYTES; k += 2) *reinterpret_cast<longlong2*>(lo + k) = make_longlong2(v[k], v[k + 1]);
-      if (MASK == MASK_IS_IGNORE) {
+      if (MASK != MASK_IS_POSITIVE) {
         unsigned w[4] = {0u, 0u, 0u, 0u};
 #pragma unroll
-        for (int k = 0; k < DB_BYTES; ++k) w[k >> 2] |= static_cast<unsigned>(v[k] == -1) << (8 * (k & 3));
+        for (int k = 0; k < DB_BYTES; ++k)
+          w[k >> 2] |= static_cast<unsigned>(MASK == MASK_IS_IGNORE ? v[k] == -1 : v[k] >= 0) << (8 * (k & 3));
         *reinterpret_cast<uint4*>(static_cast<unsigned char*>(a.mask) + s * plane + e0) = make_uint4(w[0], w[1], w[2], w[3]);
       } else {
         float m[DB_BYTES];
@@ -267,6 +271,8 @@ __global__ void __launch_bounds__(DB_THREADS) dataset_batch_kernel(BatchArgs a) 
         lo[k] = v[k];
         if (MASK == MASK_IS_IGNORE)
           static_cast<unsigned char*>(a.mask)[s * plane + e0 + k] = v[k] == -1;
+        else if (MASK == MASK_IS_NONNEG)
+          static_cast<unsigned char*>(a.mask)[s * plane + e0 + k] = v[k] >= 0;
         else
           static_cast<float*>(a.mask)[s * plane + e0 + k] = v[k] > 0 ? 1.0f : 0.0f;
       }
@@ -348,6 +354,72 @@ static int check_store(const char* who, unsigned char* store, long long n, long 
   return STEGO_OK;
 }
 
+
+// The checks and the launch of stego_dataset_batch (mask kinds 0 and 1) and stego_evalset_batch (0, 1 and 2).
+static int batch_launch(const char* who, int max_mask_kind, const unsigned char* images, const unsigned char* labels,
+                        long long n, int res, const long long* index, int count, const long long* lut, const Norm& norm,
+                        int out_bf16, int mask_kind, void* img, long long* label, void* mask, cudaStream_t stream) {
+  STEGO_CHECK_ARG(images && index && lut && img && label && mask, "%s: null pointer", who);
+  STEGO_CHECK_ARG(n >= 1, "%s: n=%lld rows", who, n);
+  STEGO_CHECK_ARG(res >= 1 && res <= 8192, "%s: res=%d (1..8192)", who, res);
+  STEGO_CHECK_ARG(count >= 1 && count <= 65535, "%s: count=%d (1..65535)", who, count);
+  STEGO_CHECK_ARG(out_bf16 == 0 || out_bf16 == 1, "%s: out_bf16=%d (0 or 1)", who, out_bf16);
+  STEGO_CHECK_ARG(mask_kind >= 0 && mask_kind <= max_mask_kind, "%s: mask_kind=%d (0..%d)", who, mask_kind,
+                  max_mask_kind);
+  STEGO_CHECK_ARG(reinterpret_cast<uintptr_t>(images) % 16 == 0 && reinterpret_cast<uintptr_t>(labels) % 16 == 0,
+                  "%s: the stores must be 16-byte aligned", who);
+  STEGO_CHECK_ARG(reinterpret_cast<uintptr_t>(lut) % 8 == 0, "%s: lut must be 8-byte aligned", who);
+  STEGO_CHECK_ARG(reinterpret_cast<uintptr_t>(img) % 16 == 0 && reinterpret_cast<uintptr_t>(label) % 16 == 0 &&
+                      reinterpret_cast<uintptr_t>(mask) % 16 == 0,
+                  "%s: outputs must be 16-byte aligned", who);
+  BatchArgs a;
+  bool on_host = false;
+  const void* d = nullptr;
+  int rc = device_view(who, "index", index, &d, &on_host);
+  if (rc != STEGO_OK) return rc;
+  STEGO_CHECK_ARG(on_host, "%s: index must be pinned host memory (it is checked on the host)", who);
+  for (int i = 0; i < count; ++i)
+    STEGO_CHECK_ARG(index[i] >= 0 && index[i] < n, "%s: index[%d]=%lld outside the %lld-row store", who, i, index[i],
+                    n);
+  a.index = static_cast<const long long*>(d);
+  rc = device_view(who, "images", images, &d, &on_host);
+  if (rc != STEGO_OK) return rc;
+  a.images = static_cast<const unsigned char*>(d);
+  a.labels = nullptr;
+  if (labels) {
+    rc = device_view(who, "labels", labels, &d, &on_host);
+    if (rc != STEGO_OK) return rc;
+    a.labels = static_cast<const unsigned char*>(d);
+  }
+  a.lut = lut;
+  a.n = norm;
+  a.img = img;
+  a.label = label;
+  a.mask = mask;
+  a.res = res;
+  const long long plane = static_cast<long long>(res) * res;
+  a.img_chunks = static_cast<int>((3 * plane + DB_BYTES - 1) / DB_BYTES);
+  a.lab_chunks = static_cast<int>((plane + DB_BYTES - 1) / DB_BYTES);
+  const dim3 grid(static_cast<unsigned>((a.img_chunks + a.lab_chunks + DB_THREADS - 1) / DB_THREADS), count);
+  if (out_bf16) {
+    if (mask_kind == MASK_IS_IGNORE)
+      dataset_batch_kernel<bf16, MASK_IS_IGNORE><<<grid, DB_THREADS, 0, stream>>>(a);
+    else if (mask_kind == MASK_IS_POSITIVE)
+      dataset_batch_kernel<bf16, MASK_IS_POSITIVE><<<grid, DB_THREADS, 0, stream>>>(a);
+    else
+      dataset_batch_kernel<bf16, MASK_IS_NONNEG><<<grid, DB_THREADS, 0, stream>>>(a);
+  } else {
+    if (mask_kind == MASK_IS_IGNORE)
+      dataset_batch_kernel<float, MASK_IS_IGNORE><<<grid, DB_THREADS, 0, stream>>>(a);
+    else if (mask_kind == MASK_IS_POSITIVE)
+      dataset_batch_kernel<float, MASK_IS_POSITIVE><<<grid, DB_THREADS, 0, stream>>>(a);
+    else
+      dataset_batch_kernel<float, MASK_IS_NONNEG><<<grid, DB_THREADS, 0, stream>>>(a);
+  }
+  STEGO_CHECK_LAUNCH("dataset_batch_kernel launch");
+  return STEGO_OK;
+}
+
 }  // namespace stego
 
 using namespace stego;
@@ -416,62 +488,17 @@ extern "C" int stego_labels_store_u8(const void* staging_host, const void* stagi
 extern "C" int stego_dataset_batch(const unsigned char* images, const unsigned char* labels, long long n, int res,
                                    const long long* index, int count, const long long* lut, float mean0, float mean1,
                                    float mean2, float std0, float std1, float std2, int out_bf16, int mask_kind,
-                                   void* img, long long* label, void* mask, void* stream_) {
-  static const char* who = "stego_dataset_batch";
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  STEGO_CHECK_ARG(images && index && lut && img && label && mask, "%s: null pointer", who);
-  STEGO_CHECK_ARG(n >= 1, "%s: n=%lld rows", who, n);
-  STEGO_CHECK_ARG(res >= 1 && res <= 8192, "%s: res=%d (1..8192)", who, res);
-  STEGO_CHECK_ARG(count >= 1 && count <= 65535, "%s: count=%d (1..65535)", who, count);
-  STEGO_CHECK_ARG(out_bf16 == 0 || out_bf16 == 1, "%s: out_bf16=%d (0 or 1)", who, out_bf16);
-  STEGO_CHECK_ARG(mask_kind == MASK_IS_IGNORE || mask_kind == MASK_IS_POSITIVE, "%s: mask_kind=%d (0 or 1)", who,
-                  mask_kind);
-  STEGO_CHECK_ARG(reinterpret_cast<uintptr_t>(images) % 16 == 0 && reinterpret_cast<uintptr_t>(labels) % 16 == 0,
-                  "%s: the stores must be 16-byte aligned", who);
-  STEGO_CHECK_ARG(reinterpret_cast<uintptr_t>(lut) % 8 == 0, "%s: lut must be 8-byte aligned", who);
-  STEGO_CHECK_ARG(reinterpret_cast<uintptr_t>(img) % 16 == 0 && reinterpret_cast<uintptr_t>(label) % 16 == 0 &&
-                      reinterpret_cast<uintptr_t>(mask) % 16 == 0,
-                  "%s: outputs must be 16-byte aligned", who);
-  BatchArgs a;
-  bool on_host = false;
-  const void* d = nullptr;
-  int rc = device_view(who, "index", index, &d, &on_host);
-  if (rc != STEGO_OK) return rc;
-  STEGO_CHECK_ARG(on_host, "%s: index must be pinned host memory (it is checked on the host)", who);
-  for (int i = 0; i < count; ++i)
-    STEGO_CHECK_ARG(index[i] >= 0 && index[i] < n, "%s: index[%d]=%lld outside the %lld-row store", who, i, index[i],
-                    n);
-  a.index = static_cast<const long long*>(d);
-  rc = device_view(who, "images", images, &d, &on_host);
-  if (rc != STEGO_OK) return rc;
-  a.images = static_cast<const unsigned char*>(d);
-  a.labels = nullptr;
-  if (labels) {
-    rc = device_view(who, "labels", labels, &d, &on_host);
-    if (rc != STEGO_OK) return rc;
-    a.labels = static_cast<const unsigned char*>(d);
-  }
-  a.lut = lut;
-  a.n = Norm{{mean0, mean1, mean2}, {std0, std1, std2}};
-  a.img = img;
-  a.label = label;
-  a.mask = mask;
-  a.res = res;
-  const long long plane = static_cast<long long>(res) * res;
-  a.img_chunks = static_cast<int>((3 * plane + DB_BYTES - 1) / DB_BYTES);
-  a.lab_chunks = static_cast<int>((plane + DB_BYTES - 1) / DB_BYTES);
-  const dim3 grid(static_cast<unsigned>((a.img_chunks + a.lab_chunks + DB_THREADS - 1) / DB_THREADS), count);
-  if (out_bf16) {
-    if (mask_kind == MASK_IS_IGNORE)
-      dataset_batch_kernel<bf16, MASK_IS_IGNORE><<<grid, DB_THREADS, 0, stream>>>(a);
-    else
-      dataset_batch_kernel<bf16, MASK_IS_POSITIVE><<<grid, DB_THREADS, 0, stream>>>(a);
-  } else {
-    if (mask_kind == MASK_IS_IGNORE)
-      dataset_batch_kernel<float, MASK_IS_IGNORE><<<grid, DB_THREADS, 0, stream>>>(a);
-    else
-      dataset_batch_kernel<float, MASK_IS_POSITIVE><<<grid, DB_THREADS, 0, stream>>>(a);
-  }
-  STEGO_CHECK_LAUNCH("dataset_batch_kernel launch");
-  return STEGO_OK;
+                                   void* img, long long* label, void* mask, void* stream) {
+  return batch_launch("stego_dataset_batch", MASK_IS_POSITIVE, images, labels, n, res, index, count, lut,
+                      Norm{{mean0, mean1, mean2}, {std0, std1, std2}}, out_bf16, mask_kind, img, label, mask,
+                      reinterpret_cast<cudaStream_t>(stream));
+}
+
+extern "C" int stego_evalset_batch(const unsigned char* images, const unsigned char* labels, long long n, int res,
+                                   const long long* index, int count, const long long* lut, float mean0, float mean1,
+                                   float mean2, float std0, float std1, float std2, int out_bf16, int mask_kind,
+                                   void* img, long long* label, void* mask, void* stream) {
+  return batch_launch("stego_evalset_batch", MASK_IS_NONNEG, images, labels, n, res, index, count, lut,
+                      Norm{{mean0, mean1, mean2}, {std0, std1, std2}}, out_bf16, mask_kind, img, label, mask,
+                      reinterpret_cast<cudaStream_t>(stream));
 }

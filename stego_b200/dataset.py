@@ -72,6 +72,15 @@ def _generate_state(base_seed: int, worker_id: int) -> list:
     return state
 
 
+def shard(indices: list, rank: int, world_size: int) -> list:
+    """Rank `rank`'s share of `indices` as DistributedSampler(drop_last=False) deals it: the list padded with its own
+    head to a multiple of world_size, then every world_size-th entry from position rank."""
+    total = math.ceil(len(indices) / world_size) * world_size
+    pad = total - len(indices)
+    indices = indices + (indices[:pad] if pad <= len(indices) else (indices * math.ceil(pad / len(indices)))[:pad])
+    return indices[rank:total:world_size]
+
+
 def _draw_int64(g: torch.Generator) -> int:
     """torch.empty((), dtype=torch.int64).random_(): the DataLoader's base seed and RandomSampler's epoch seed."""
     return int(torch.empty((), dtype=torch.int64).random_(generator=g).item())
@@ -139,12 +148,7 @@ class Sampler:
             return torch.randperm(self.n, generator=g).tolist()
         g = torch.Generator()
         g.manual_seed(self.seed + self.epoch)
-        indices = torch.randperm(self.n, generator=g).tolist()
-        num_samples = math.ceil(self.n / self.world_size)
-        total = num_samples * self.world_size
-        pad = total - len(indices)
-        indices += indices[:pad] if pad <= len(indices) else (indices * math.ceil(pad / len(indices)))[:pad]
-        return indices[self.rank:total:self.world_size]
+        return shard(torch.randperm(self.n, generator=g).tolist(), self.rank, self.world_size)
 
     def _epoch(self, order: list, base: int):
         B = self.batch_size
@@ -196,7 +200,117 @@ def _as_list(batch):
     return batch
 
 
-class ResidentDataset:
+class _Store:
+    """n uint8 rows of res x res frames (and label maps) in device or pinned host memory, filled in order by `append`
+    and read by one gather launch per batch: what ResidentDataset and evalset.EvalSet share.  A subclass sets the batch
+    entry, its mask rule and the label table, and calls _allocate once its own arguments are checked."""
+
+    _PREFIX = "stego_b200.dataset"
+    _ENTRY = "stego_dataset_batch"
+
+    def _allocate(self, n: int, res: int, location: str, has_labels: bool, lut: torch.Tensor) -> None:
+        self.n, self.res, self.location, self.has_labels = n, res, location, bool(has_labels)
+        self.device = frames._require_cuda(type(self).__name__)
+        shape = (self.n, 3, self.res, self.res)
+        if location == "cuda":
+            self.images = torch.empty(shape, dtype=torch.uint8, device=self.device)
+            self.labels = (torch.empty(self.n, self.res, self.res, dtype=torch.uint8, device=self.device)
+                           if has_labels else None)
+        else:
+            self.images = torch.empty(shape, dtype=torch.uint8, pin_memory=True)
+            self.labels = torch.empty(self.n, self.res, self.res, dtype=torch.uint8, pin_memory=True) if has_labels else None
+        self._lut = lut.to(self.device)
+        self.count = 0
+        # pinned index records, used in turn: one is refilled once the launch that read it two steps earlier has run
+        self._ring = [torch.empty(0, dtype=torch.int64), torch.empty(0, dtype=torch.int64)]
+        self._ring_done = [None, None]
+        self._slot = 0
+
+    @property
+    def nbytes(self) -> int:
+        return 4 * self.n * self.res * self.res if self.has_labels else 3 * self.n * self.res * self.res
+
+    def append(self, images, labels=None) -> None:
+        """Transform and store the next len(images) samples: images as load_frames takes them (uint8 H x W x 3), labels
+        as load_labels (uint8 H x W), one per image (None without labels).  One build launch per store; the caller is
+        not synchronised."""
+        who = f"{type(self).__name__}.append"
+        arrays = frames._as_arrays(images, 3, who)
+        if self.has_labels:
+            if labels is None:
+                raise ValueError(f"{self._PREFIX}.{who}: this store keeps labels; pass one label map per image")
+            label_arrays = frames._as_arrays(labels, 1, who)
+            if len(label_arrays) != len(arrays):
+                raise ValueError(f"{self._PREFIX}.{who}: {len(label_arrays)} label maps for {len(arrays)} images")
+        elif labels is not None:
+            raise ValueError(f"{self._PREFIX}.{who}: this store was made with has_labels=False")
+        B = len(arrays)
+        if self.count + B > self.n:
+            raise ValueError(f"{self._PREFIX}.{who}: {B} samples after {self.count} overflow the {self.n}-row store")
+        lib = _lib.load()
+        with torch.cuda.device(self.device):
+            staging, words, _ = frames._stage(arrays, self.res, "center")
+            staged = staging.to(self.device, non_blocking=True)
+            _lib.check(lib.stego_frames_store_rgb8(staging.data_ptr(), _lib.ptr(staged), staging.numel(), words, B,
+                                                   self.res, _lib.ptr(self.images), self.n, self.count, _lib.stream()),
+                       "stego_frames_store_rgb8")
+            if self.has_labels:
+                staging, words, _ = frames._stage(label_arrays, self.res, "center")
+                staged = staging.to(self.device, non_blocking=True)
+                _lib.check(lib.stego_labels_store_u8(staging.data_ptr(), _lib.ptr(staged), staging.numel(), words, B,
+                                                     self.res, _lib.ptr(self.labels), self.n, self.count,
+                                                     _lib.stream()), "stego_labels_store_u8")
+        self.count += B
+
+    def _fill(self, files: Dataset, batch_size: int, num_workers: int) -> None:
+        """Append every (image, label or None) item of `files`, decoded in DataLoader(num_workers) workers."""
+        loader = DataLoader(files, batch_size, shuffle=False, num_workers=num_workers, collate_fn=_as_list)
+        for batch in loader:
+            self.append([b[0] for b in batch], [b[1] for b in batch] if self.has_labels else None)
+
+    # ---- reading --------------------------------------------------------------------------------------------------
+    def _require_full(self, who: str) -> None:
+        if self.count != self.n:
+            raise ValueError(f"{self._PREFIX}.{who}: the store holds {self.count} of its {self.n} samples")
+
+    def _record(self, index: np.ndarray) -> torch.Tensor:
+        """The next pinned index record holding `index`, reused once the launch that read it last has run."""
+        if self._ring[0].numel() < index.size:  # both records grow together, once their readers have run
+            for j in (0, 1):
+                if self._ring_done[j] is not None:
+                    self._ring_done[j].synchronize()
+                self._ring[j] = torch.empty(index.size, dtype=torch.int64, pin_memory=True)
+        i = self._slot
+        self._slot ^= 1
+        if self._ring_done[i] is not None:
+            self._ring_done[i].synchronize()
+        self._ring[i].numpy()[:index.size] = index
+        return i
+
+    def _gather(self, index: np.ndarray, dtype) -> tuple:
+        """(img, label, mask) of the store rows `index`, one launch on the current stream."""
+        count, res = index.size, self.res
+        with torch.cuda.device(self.device):
+            i = self._record(index)
+            img = torch.empty(count, 3, res, res, dtype=dtype, device=self.device)
+            label = torch.empty(count, res, res, dtype=torch.int64, device=self.device)
+            mask_dtype = torch.float32 if self._mask_kind == MASK_IS_POSITIVE else torch.bool
+            mask = torch.empty(count, res, res, dtype=mask_dtype, device=self.device)
+            _lib.check(getattr(_lib.load(), self._ENTRY)(
+                _lib.ptr(self.images), _lib.ptr(self.labels), self.n, res, self._ring[i].data_ptr(), count,
+                _lib.ptr(self._lut), *frames.MEAN, *frames.STD, int(dtype == torch.bfloat16), self._mask_kind,
+                _lib.ptr(img), _lib.ptr(label), _lib.ptr(mask), _lib.stream()), self._ENTRY)
+            done = torch.cuda.Event()
+            done.record()
+            self._ring_done[i] = done
+        return img, label, mask
+
+    def _check_dtype(self, dtype, who: str) -> None:
+        if dtype not in (torch.float32, torch.bfloat16):
+            raise ValueError(f"{self._PREFIX}.{who}: dtype={dtype} (torch.float32 or torch.bfloat16)")
+
+
+class ResidentDataset(_Store):
     """The training set of a CroppedDataset (kind="cropped") or DirectoryDataset (kind="directory") resident in memory.
 
     n samples at res: 4 * res^2 bytes each (3 * res^2 of image, res^2 of label), 200,704 B at 224^2.  location="cuda"
@@ -215,71 +329,19 @@ class ResidentDataset:
             raise ValueError(f"stego_b200.dataset.{who}: location={location!r} (\"cuda\" or \"host\")")
         if kind == "cropped" and not has_labels:
             raise ValueError(f"stego_b200.dataset.{who}: a CroppedDataset always has labels")
-        self.n = _check_int(n, "n", 1, 1 << 40, who)
-        self.res = _check_int(res, "res", 1, 8192, who)
-        self.kind, self.location, self.has_labels = kind, location, bool(has_labels)
-        self.device = frames._require_cuda(who)
-        shape = (self.n, 3, self.res, self.res)
-        if location == "cuda":
-            self.images = torch.empty(shape, dtype=torch.uint8, device=self.device)
-            self.labels = (torch.empty(self.n, self.res, self.res, dtype=torch.uint8, device=self.device)
-                           if has_labels else None)
-        else:
-            self.images = torch.empty(shape, dtype=torch.uint8, pin_memory=True)
-            self.labels = torch.empty(self.n, self.res, self.res, dtype=torch.uint8, pin_memory=True) if has_labels else None
+        n = _check_int(n, "n", 1, 1 << 40, who)
+        res = _check_int(res, "res", 1, 8192, who)
+        self.kind = kind
+        self._mask_kind = MASK_IS_IGNORE if kind == "cropped" else MASK_IS_POSITIVE
         # CroppedDataset: label = byte - 1; DirectoryDataset: the byte, or -1 everywhere without a label folder
         ids = torch.arange(256, dtype=torch.int64)
         lut = ids - 1 if kind == "cropped" else (ids if has_labels else torch.full((256,), -1, dtype=torch.int64))
-        self._lut = lut.to(self.device)
-        self.count = 0
-        # pinned index records, used in turn: one is refilled once the launch that read it two steps earlier has run
-        self._ring = [torch.empty(0, dtype=torch.int64), torch.empty(0, dtype=torch.int64)]
-        self._ring_done = [None, None]
-        self._slot = 0
-
-    @property
-    def nbytes(self) -> int:
-        return 4 * self.n * self.res * self.res if self.has_labels else 3 * self.n * self.res * self.res
-
-    def append(self, images, labels=None) -> None:
-        """Transform and store the next len(images) samples: images as load_frames takes them (uint8 H x W x 3), labels
-        as load_labels (uint8 H x W), one per image (None without labels).  One build launch per store; the caller is
-        not synchronised."""
-        who = "ResidentDataset.append"
-        arrays = frames._as_arrays(images, 3, who)
-        if self.has_labels:
-            if labels is None:
-                raise ValueError(f"stego_b200.dataset.{who}: this store keeps labels; pass one label map per image")
-            label_arrays = frames._as_arrays(labels, 1, who)
-            if len(label_arrays) != len(arrays):
-                raise ValueError(f"stego_b200.dataset.{who}: {len(label_arrays)} label maps for {len(arrays)} images")
-        elif labels is not None:
-            raise ValueError(f"stego_b200.dataset.{who}: this store was made with has_labels=False")
-        B = len(arrays)
-        if self.count + B > self.n:
-            raise ValueError(f"stego_b200.dataset.{who}: {B} samples after {self.count} overflow the {self.n}-row store")
-        lib = _lib.load()
-        with torch.cuda.device(self.device):
-            staging, words, _ = frames._stage(arrays, self.res, "center")
-            staged = staging.to(self.device, non_blocking=True)
-            _lib.check(lib.stego_frames_store_rgb8(staging.data_ptr(), _lib.ptr(staged), staging.numel(), words, B,
-                                                   self.res, _lib.ptr(self.images), self.n, self.count, _lib.stream()),
-                       "stego_frames_store_rgb8")
-            if self.has_labels:
-                staging, words, _ = frames._stage(label_arrays, self.res, "center")
-                staged = staging.to(self.device, non_blocking=True)
-                _lib.check(lib.stego_labels_store_u8(staging.data_ptr(), _lib.ptr(staged), staging.numel(), words, B,
-                                                     self.res, _lib.ptr(self.labels), self.n, self.count,
-                                                     _lib.stream()), "stego_labels_store_u8")
-        self.count += B
+        self._allocate(n, res, location, has_labels, lut)
 
     @classmethod
     def _from_files(cls, images, labels, convert, res, kind, location, batch_size, num_workers):
         store = cls(len(images), res, kind, location, has_labels=labels is not None)
-        loader = DataLoader(_Files(images, labels, convert), batch_size, shuffle=False, num_workers=num_workers,
-                            collate_fn=_as_list)
-        for batch in loader:
-            store.append([b[0] for b in batch], [b[1] for b in batch] if labels is not None else None)
+        store._fill(_Files(images, labels, convert), batch_size, num_workers)
         return store
 
     @classmethod
@@ -319,44 +381,6 @@ class ResidentDataset:
         images = [os.path.join(img_dir, f) for f in names]
         return cls._from_files(images, labels, False, res, "directory", location, batch_size, num_workers)
 
-    # ---- reading --------------------------------------------------------------------------------------------------
-    def _require_full(self, who: str) -> None:
-        if self.count != self.n:
-            raise ValueError(f"stego_b200.dataset.{who}: the store holds {self.count} of its {self.n} samples")
-
-    def _record(self, index: np.ndarray) -> torch.Tensor:
-        """The next pinned index record holding `index`, reused once the launch that read it last has run."""
-        if self._ring[0].numel() < index.size:  # both records grow together, once their readers have run
-            for j in (0, 1):
-                if self._ring_done[j] is not None:
-                    self._ring_done[j].synchronize()
-                self._ring[j] = torch.empty(index.size, dtype=torch.int64, pin_memory=True)
-        i = self._slot
-        self._slot ^= 1
-        if self._ring_done[i] is not None:
-            self._ring_done[i].synchronize()
-        self._ring[i].numpy()[:index.size] = index
-        return i
-
-    def _gather(self, index: np.ndarray, dtype) -> tuple:
-        """(img, label, mask) of the store rows `index`, one launch on the current stream."""
-        count, res = index.size, self.res
-        with torch.cuda.device(self.device):
-            i = self._record(index)
-            img = torch.empty(count, 3, res, res, dtype=dtype, device=self.device)
-            label = torch.empty(count, res, res, dtype=torch.int64, device=self.device)
-            mask_dtype = torch.bool if self.kind == "cropped" else torch.float32
-            mask = torch.empty(count, res, res, dtype=mask_dtype, device=self.device)
-            _lib.check(_lib.load().stego_dataset_batch(
-                _lib.ptr(self.images), _lib.ptr(self.labels), self.n, res, self._ring[i].data_ptr(), count,
-                _lib.ptr(self._lut), *frames.MEAN, *frames.STD, int(dtype == torch.bfloat16),
-                MASK_IS_IGNORE if self.kind == "cropped" else MASK_IS_POSITIVE, _lib.ptr(img), _lib.ptr(label),
-                _lib.ptr(mask), _lib.stream()), "stego_dataset_batch")
-            done = torch.cuda.Event()
-            done.record()
-            self._ring_done[i] = done
-        return img, label, mask
-
     def _shaped(self, label, mask):
         """The shapes the reference's classes return, batched: CroppedDataset label [B, res, res] and mask
         [B, 1, res, res]; DirectoryDataset label and mask [B, 1, res, res] with a label folder, [B, res, res] without."""
@@ -367,22 +391,21 @@ class ResidentDataset:
             return label.view(B, 1, res, res), mask.view(B, 1, res, res)
         return label, mask
 
-    def frames(self, batch_size: int, dtype=torch.float32):
+    def frames(self, batch_size: int, dtype=torch.float32, rank: int = 0, world_size: int = 1):
         """Batches {"img", "label", "mask"} of the samples in index order: get_transform(res, ., "center") of each
-        image, as a shuffle=False loader yields them (precompute_knns(net, store.frames(b)) runs on them unchanged)."""
+        image, as a shuffle=False loader yields them (precompute_knns(net, store.frames(b)) runs on them unchanged).
+        With world_size > 1, rank `rank`'s samples of DistributedSampler(shuffle=False), padding included."""
         who = "ResidentDataset.frames"
         self._require_full(who)
         batch_size = _check_int(batch_size, "batch_size", 1, 65535, who)
         self._check_dtype(dtype, who)
-        for start in range(0, self.n, batch_size):
-            img, label, mask = self._gather(np.arange(start, min(start + batch_size, self.n), dtype=np.int64), dtype)
+        world_size = _check_int(world_size, "world_size", 1, 1 << 20, who)
+        rank = _check_int(rank, "rank", 0, world_size - 1, who)
+        order = np.asarray(shard(list(range(self.n)), rank, world_size), dtype=np.int64)
+        for start in range(0, order.size, batch_size):
+            img, label, mask = self._gather(order[start:start + batch_size], dtype)
             label, mask = self._shaped(label, mask)
             yield dict(img=img, label=label, mask=mask)
-
-    @staticmethod
-    def _check_dtype(dtype, who: str) -> None:
-        if dtype not in (torch.float32, torch.bfloat16):
-            raise ValueError(f"stego_b200.dataset.{who}: dtype={dtype} (torch.float32 or torch.bfloat16)")
 
     def batches(self, nns, batch_size: int, num_neighbors: int, seed: int, loader_workers: int = 0, rank: int = 0,
                 world_size: int = 1, dtype=torch.float32, res: int = None):

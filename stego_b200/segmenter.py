@@ -636,21 +636,46 @@ class LitUnsupervisedSegmenter(nn.Module):
         graphs and workspace alone.  The net's train / eval modes are restored on exit: there is no Trainer to call
         `.train()` afterwards, and the hand-scheduled step only runs on a net in training mode.  Returns the
         reference's preview dict on the CPU (first cfg.n_images entries, int64 predictions)."""
-        from .eval import fused_probe_log_probs
-        self.flush()
         img, label = batch["img"], batch["label"]
         n_images = getattr(self.cfg, "n_images", 5)
-        with self._net_in_eval_mode(), torch.no_grad():
-            _, code = self.net(img)
-            out = fused_probe_log_probs(code, self.linear_probe, self.cluster_probe, label.shape[-2:], 2.0,
-                                        want_log_probs=False, want_argmax=n_images > 0, label=label,
-                                        linear_confusion=self.linear_metrics.stats,
-                                        cluster_confusion=self.cluster_metrics.stats)
+        out = self._validation_counts(img, label, n_images > 0)
         none = torch.empty(0, *label.shape[-2:], dtype=torch.long)
         return {"img": img[:n_images].detach().cpu(),
                 "linear_preds": out[2][:n_images].long().cpu() if n_images > 0 else none,
                 "cluster_preds": out[3][:n_images].long().cpu() if n_images > 0 else none,
                 "label": label[:n_images].detach().cpu()}
+
+    def _validation_counts(self, img, label, want_argmax: bool):
+        """validation_step's device work: the eval-mode net, both probes and both confusion-count updates."""
+        from .eval import fused_probe_log_probs
+        self.flush()
+        with self._net_in_eval_mode(), torch.no_grad():
+            _, code = self.net(img)
+            return fused_probe_log_probs(code, self.linear_probe, self.cluster_probe, label.shape[-2:], 2.0,
+                                         want_log_probs=False, want_argmax=want_argmax, label=label,
+                                         linear_confusion=self.linear_metrics.stats,
+                                         cluster_confusion=self.cluster_metrics.stats)
+
+    def validate(self, store, batch_size: int, rank: int = 0, world_size: int = 1) -> Dict[str, float]:
+        """One validation pass over a resident set (evalset.EvalSet or dataset.ResidentDataset): validation_step over
+        store.frames(batch_size, rank=rank, world_size=world_size), i.e. the batches of the reference's shuffle=False
+        validation loader (rank r's DistributedSampler shard with world_size > 1), then validation_epoch_end, whose
+        metric dict is returned (the counts are summed over the ranks when a process group is up).
+
+        Only the first batch goes through validation_step itself; the rest run its device work without the preview
+        copy, so the host does not wait on the device between batches.  The first batch's preview dict is kept as
+        `self.last_validation_preview`."""
+        from .dataset import ResidentDataset
+        from .evalset import EvalSet
+        if not isinstance(store, (EvalSet, ResidentDataset)):
+            raise ValueError(f"validate: store must be an EvalSet or a ResidentDataset, got {type(store).__name__}")
+        kw = dict(mask=False) if isinstance(store, EvalSet) else {}
+        for i, batch in enumerate(store.frames(batch_size, rank=rank, world_size=world_size, **kw)):
+            if i == 0:
+                self.last_validation_preview = self.validation_step(batch, 0)
+            else:
+                self._validation_counts(batch["img"], batch["label"], True)  # the probe pass counts from its argmax
+        return self.validation_epoch_end([])
 
     def correspondence_pr_step(self, batch, metric) -> None:
         """plot_pr_curves.py:126-142 (LitRecalibrator.validation_step) for the two methods this package has: the head's
