@@ -288,6 +288,35 @@ STEGO_API int stego_evalset_batch(const unsigned char* images, const unsigned ch
                                   void* img, long long* label, void* mask, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Cropped training sets (src/crop_datasets.py:114-124 then CroppedDataset, src/data.py:370-400): crop windows of
+ * decoded originals through the JPEG round trip of Pillow's default save (baseline, quality 75, 4:2:0, islow DCT)
+ * and its decode, then the store build of stego_frames_store_rgb8, in two launches.  Integer arithmetic throughout.
+ * staging: one buffer of `bytes` bytes, built by the host (stego_b200/crops.py):
+ *   bytes [0, 72 count): int64 records [count][9] = {byte offset of the crop's source image, source H, source W, top,
+ *     left, crop height h, crop width w, first table word, workspace byte offset};
+ *   then int32 tables (table_words words), per record res source rows then res source columns inside the crop (the
+ *     index tables of get_transform(res, False, "center") for an h x w image; -1 = Pillow's fill value 0);
+ *   then the source images, uint8 H x W x 3 RGB, each at its record's offset.
+ * staging_host: a host copy read to check every record, window, table entry and extent before the launch;
+ * staging_dev: the device copy (8-byte aligned).  count 1..65535.  workspace: device memory, h w + 2 ceil(h / 2)
+ * ceil(w / 2) bytes per crop at its record's offset (decoded luma [h][w], then Cb and Cr [ceil(h/2)][ceil(w/2)]).
+ * The calls never synchronise and read nothing back. */
+/* The codec: per 16 x 16 MCU of each crop (grid relative to the crop's origin, edges replicated as libjpeg pads),
+ * RGB -> YCbCr, h2v2 downsampling, FDCT, quantisation, dequantisation and IDCT of its 6 blocks; writes the decoded
+ * planes into the workspace.  The tables are not read (table_words may be 0). */
+STEGO_API int stego_jpeg_crops_codec(const void* staging_host, const void* staging_dev, long long bytes,
+                                     long long table_words, int count, unsigned char* workspace,
+                                     long long workspace_bytes, void* stream);
+/* The store rows of the decoded crops: crop k's frame (res 1..8192) is gathered through its tables, each pixel
+ * rebuilt from the workspace with the decoder's chroma upsampling ("fancy" h2v2; 2 x 2 replication when
+ * ceil(w / 2) <= 2) and YCbCr -> RGB, and written as raw bytes into row r0 + k of the uint8 store [n][3][res][res]
+ * (16-byte aligned, device memory or pinned host memory).  0 <= r0 <= n - count. */
+STEGO_API int stego_jpeg_crops_store_rgb8(const void* staging_host, const void* staging_dev, long long bytes,
+                                          long long table_words, int count, int res, const unsigned char* workspace,
+                                          long long workspace_bytes, unsigned char* store, long long n, long long r0,
+                                          void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * TensorBoard histograms (SummaryWriter.add_histogram with its default bins="tensorflow")
  * ---------------------------------------------------------------------------------------------- */
 /* The 1549 float64 bucket edges of torch's SummaryWriter.default_bins (edges, may be null) and the 1550 fp32

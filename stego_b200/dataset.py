@@ -361,6 +361,23 @@ class ResidentDataset(_Store):
         return cls._from_files(images, labels, True, res, "cropped", location, batch_size, num_workers)
 
     @classmethod
+    def crops(cls, root: str, dataset_name: str, crop_type: str, crop_ratio, image_set: str, res: int,
+              location: str = "cuda", batch_size: int = 64, num_workers: int = 0,
+              fine_to_coarse=None) -> "ResidentDataset":
+        """The store `cropped(root, dataset_name, crop_type, crop_ratio, image_set, res, location)` reads from the tree
+        the reference's crop_datasets.py writes, built straight from the uncropped originals (stego_b200/crops.py):
+        dataset_name "cocostuff27" (Coco, subset None; val: 7) or "cityscapes" (CityscapesSeg), crop_type "five" or
+        "random".  Each original is decoded once in DataLoader(num_workers) workers, max(1, batch_size // 5) originals
+        (their 5x crops: about batch_size rows) per build launch; its five crops go through the JPEG round trip of
+        Pillow's default save and decode on the GPU.  The
+        rows, frames() and batches() equal those of `cropped` on the written tree byte for byte; the label rows hold
+        the source's raw bytes, read through the class's table.  fine_to_coarse: Coco's {fine id: coarse id} table
+        (cocostuff27 only)."""
+        from . import crops
+        return crops.build_store(cls, root, dataset_name, crop_type, crop_ratio, image_set, res, location, batch_size,
+                                 num_workers, fine_to_coarse)
+
+    @classmethod
     def directory(cls, root: str, path: str, image_set: str, res: int, location: str = "cuda", batch_size: int = 64,
                   num_workers: int = 0) -> "ResidentDataset":
         """DirectoryDataset(root, path, image_set, ...) (src/data.py:75-118): sorted listdir of {root}/{path}/imgs/
