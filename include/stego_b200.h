@@ -286,6 +286,30 @@ STEGO_API int stego_evalset_batch(const unsigned char* images, const unsigned ch
                                   const long long* index, int count, const long long* lut, float mean0, float mean1,
                                   float mean2, float std0, float std1, float std2, int out_bf16, int mask_kind,
                                   void* img, long long* label, void* mask, void* stream);
+/* Ragged store build (stego_b200/dataset.py, crop="random"): the whole T.Resize(res, NEAREST) output of each image, no
+ * crop, written as a uint8 row [channels][oh][ow] of a flat store of store_bytes bytes.  The staging layout of
+ * stego_frames_rgb8 with 7-word records {byte offset of the image in staging, H, W, first table word, oh, ow, byte
+ * offset of the row in the store} and, per record, oh source rows then ow source columns.  channels 3 (H x W x 3 RGB
+ * images) or 1 (H x W label maps, raw bytes).  Every record, table entry, image extent and row extent is checked on
+ * staging_host before the launch.  store: device memory or pinned host memory.  One launch; never synchronises. */
+STEGO_API int stego_store_rows_u8(const void* staging_host, const void* staging_dev, long long bytes,
+                                  long long table_words, int B, int channels, unsigned char* store,
+                                  long long store_bytes, void* stream);
+/* A batch of res x res windows of a ragged store: stego_evalset_batch's outputs, table and mask kinds 0..2, with
+ * sample s read from the window record[s] = {row, image top, image left, label top, label left} (int64 [count][5]).
+ * rows: int64 [n][6] = {image byte offset, oh, ow, label byte offset, lh, lw}; row i's image is uint8 [3][oh][ow] at its
+ * offset in `images` (image_bytes long) and its label uint8 [lh][lw] in `labels` (label_bytes long; null: every pixel
+ * reads id 0).  Both stores 16-byte aligned and a multiple of 16 bytes long, device or pinned host memory.  rows and
+ * record are pinned host memory: every record entry is checked on the host against the row table (0 <= row < n, the
+ * windows inside their image and label, the rows inside their stores), then the kernel reads both through their mapped
+ * addresses, so they must stay unchanged until the launch has run.  One launch; the call never synchronises and reads
+ * nothing back from the device. */
+STEGO_API int stego_store_batch_window(const unsigned char* images, long long image_bytes,
+                                       const unsigned char* labels, long long label_bytes, const long long* rows,
+                                       long long n, int res, const long long* record, int count,
+                                       const long long* lut, float mean0, float mean1, float mean2, float std0,
+                                       float std1, float std2, int out_bf16, int mask_kind, void* img,
+                                       long long* label, void* mask, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Cropped training sets (src/crop_datasets.py:114-124 then CroppedDataset, src/data.py:370-400): crop windows of

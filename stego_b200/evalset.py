@@ -35,7 +35,7 @@ import torch
 from PIL import Image
 from torch.utils.data import Dataset
 
-from .dataset import LOCATIONS, MASK_IS_IGNORE, MASK_IS_POSITIVE, _check_int, _Store, shard
+from .dataset import LOCATIONS, MASK_IS_IGNORE, MASK_IS_POSITIVE, _check_int, _Store, image_size, shard
 
 COCO_KINDS = ("cocostuff27", "cocostuff15", "cocostuff3")
 KINDS = COCO_KINDS + ("cityscapes", "potsdam", "potsdamraw")
@@ -189,16 +189,35 @@ def read_mat(image_path: str, label_path: str) -> tuple:
     return img, gt
 
 
+def source_sizes(images: list, labels: list, reader: str) -> np.ndarray:
+    """int64 [n, 4]: each image's height, width and its label map's, from the file headers (scipy's whosmat for the
+    .mat tiles; a missing gt file is the image's size): the row sizes a crop="random" store is made with."""
+    from scipy.io import whosmat
+    out = []
+    for image, label in zip(images, labels):
+        if reader == "pil":
+            out.append(image_size(image) + image_size(label))
+            continue
+        hw = next(shape[:2] for name, shape, _ in whosmat(image) if name == "img")
+        lhw = next((shape[:2] for name, shape, _ in whosmat(label) if name == "gt"), hw) if os.path.exists(label) else hw
+        out.append(tuple(hw) + tuple(lhw))
+    return np.array(out, dtype=np.int64).reshape(-1, 4)
+
+
 class EvalSet(_Store):
-    """An evaluation set of one of KINDS resident in memory, n samples at res (4 * res^2 bytes each).
+    """An evaluation set of one of KINDS resident in memory, n samples at res (4 * res^2 bytes each with crop "center"
+    or None; with "random" each row's whole Resize(res) output).
 
     Rows are filled in order by `append` (images uint8 H x W x 3, label maps uint8 H x W) or built from the files by
-    the `coco` / `cityscapes` / `potsdam` / `potsdamraw` constructors; `frames` needs all n."""
+    the `coco` / `cityscapes` / `potsdam` / `potsdamraw` constructors; `frames` and `batches` need all n.  `batches`
+    is the training loader of ContrastiveSegDataset(root, kind, None, "train", ...) (dataset._Store.batches), crop the
+    loader's (train_config.yml loader_crop_type)."""
 
     _PREFIX = "stego_b200.evalset"
     _ENTRY = "stego_evalset_batch"
 
-    def __init__(self, n: int, res: int, kind: str, location: str = "cuda", fine_to_coarse=None):
+    def __init__(self, n: int, res: int, kind: str, location: str = "cuda", fine_to_coarse=None, crop="center",
+                 sizes=None):
         who = "EvalSet"
         if kind not in KINDS:
             _fail(who, f"kind={kind!r} (one of {', '.join(KINDS)}); the five-crop and directory sets are "
@@ -211,50 +230,60 @@ class EvalSet(_Store):
         self.kind = kind
         self._mask_kind = (MASK_IS_NONNEG if kind in COCO_KINDS else MASK_IS_IGNORE if kind == "cityscapes" else
                            MASK_IS_POSITIVE)
-        self._allocate(n, res, location, True, lut)
+        self._allocate(n, res, location, True, lut, crop, sizes)
 
     @classmethod
-    def _from_files(cls, images, labels, reader, res, kind, location, batch_size, num_workers, fine_to_coarse=None):
+    def _from_files(cls, images, labels, reader, res, kind, location, batch_size, num_workers, fine_to_coarse=None,
+                    crop="center"):
         if not images:
             _fail(f"EvalSet.{kind}", "the listing names no files")
         if len(images) != len(labels):
             _fail(f"EvalSet.{kind}", f"{len(images)} images but {len(labels)} label files")
-        store = cls(len(images), res, kind, location, fine_to_coarse)
+        sizes = source_sizes(images, labels, reader) if crop == "random" else None
+        store = cls(len(images), res, kind, location, fine_to_coarse, crop, sizes)
         store._fill(_EvalFiles(images, labels, reader), batch_size, num_workers)
         return store
 
     @classmethod
     def coco(cls, root: str, kind: str, image_set: str, res: int, fine_to_coarse, location: str = "cuda",
-             batch_size: int = 64, num_workers: int = 0) -> "EvalSet":
+             batch_size: int = 64, num_workers: int = 0, crop="center") -> "EvalSet":
         """ContrastiveSegDataset(root, kind, None, image_set, ...)'s Coco (`coco_files`), decoded once in
         DataLoader(num_workers) workers."""
         images, labels = coco_files(root, kind, image_set)
-        return cls._from_files(images, labels, "pil", res, kind, location, batch_size, num_workers, fine_to_coarse)
+        return cls._from_files(images, labels, "pil", res, kind, location, batch_size, num_workers, fine_to_coarse,
+                               crop)
 
     @classmethod
     def cityscapes(cls, root: str, image_set: str, res: int, location: str = "cuda", batch_size: int = 64,
-                   num_workers: int = 0) -> "EvalSet":
+                   num_workers: int = 0, crop="center") -> "EvalSet":
         """ContrastiveSegDataset(root, "cityscapes", None, image_set, ...)'s CityscapesSeg (`cityscapes_files`)."""
         images, labels = cityscapes_files(root, image_set)
-        return cls._from_files(images, labels, "pil", res, "cityscapes", location, batch_size, num_workers)
+        return cls._from_files(images, labels, "pil", res, "cityscapes", location, batch_size, num_workers, crop=crop)
 
     @classmethod
     def potsdam(cls, root: str, image_set: str, res: int, location: str = "cuda", batch_size: int = 64,
-                num_workers: int = 0) -> "EvalSet":
+                num_workers: int = 0, crop="center") -> "EvalSet":
         """ContrastiveSegDataset(root, "potsdam", None, image_set, ...)'s Potsdam (`potsdam_files`, `read_mat`)."""
         images, labels = potsdam_files(root, image_set)
-        return cls._from_files(images, labels, "mat", res, "potsdam", location, batch_size, num_workers)
+        return cls._from_files(images, labels, "mat", res, "potsdam", location, batch_size, num_workers, crop=crop)
 
     @classmethod
     def potsdamraw(cls, root: str, res: int, location: str = "cuda", batch_size: int = 64,
-                   num_workers: int = 0) -> "EvalSet":
+                   num_workers: int = 0, crop="center") -> "EvalSet":
         """ContrastiveSegDataset(root, "potsdamraw", None, ...)'s PotsdamRaw (`potsdamraw_files`, `read_mat`)."""
         images, labels = potsdamraw_files(root)
-        return cls._from_files(images, labels, "mat", res, "potsdamraw", location, batch_size, num_workers)
+        return cls._from_files(images, labels, "mat", res, "potsdamraw", location, batch_size, num_workers, crop=crop)
 
     # ---- reading --------------------------------------------------------------------------------------------------
+    def _shaped(self, label, mask):
+        """The class's per-sample shapes, batched: label [B, res, res]; mask [B, 1, res, res] for CityscapesSeg,
+        [B, res, res] otherwise."""
+        return label, mask.unsqueeze(1) if self.kind == "cityscapes" else mask
+
     def frames(self, batch_size: int, dtype=torch.float32, mask: bool = True, rank: int = 0, world_size: int = 1):
-        """The batches of DataLoader(ContrastiveSegDataset(..., mask=mask), batch_size, shuffle=False): dicts of ind
+        """The batches of DataLoader(ContrastiveSegDataset(..., mask=mask), batch_size, shuffle=False) with
+        get_transform(res, ., "center") (a crop="random" store yields the centre windows, crop None the squashed
+        frames): dicts of ind
         (int64, CPU), img (dtype), label (int64 [B, res, res]) and with `mask` the class's mask (Coco: bool
         [B, res, res]; CityscapesSeg: bool [B, 1, res, res]; Potsdam, PotsdamRaw: fp32 [B, res, res]), on the store's
         device.  With world_size > 1, rank `rank`'s samples of DistributedSampler(shuffle=False), padding included.
@@ -271,5 +300,5 @@ class EvalSet(_Store):
             img, label, m = self._gather(ind, dtype)
             batch = dict(ind=torch.from_numpy(ind), img=img, label=label)
             if mask:
-                batch["mask"] = m.unsqueeze(1) if self.kind == "cityscapes" else m
+                batch["mask"] = self._shaped(label, m)[1]
             yield batch

@@ -21,6 +21,7 @@ from . import _lib
 
 MEAN, STD = (0.485, 0.456, 0.406), (0.229, 0.224, 0.225)  # src/utils.py:140 normalize (ImageNet statistics)
 REC_WORDS = 4  # int64 words per record: byte offset, H, W, first table word
+ROW_REC_WORDS = 7  # stego_store_rows_u8's records: those four, then the output's height, width and store byte offset
 CROPS = ("center", None)
 
 
@@ -116,18 +117,28 @@ def _require_cuda(who: str) -> torch.device:
     return torch.device("cuda", torch.cuda.current_device())
 
 
-def _stage(arrays, res: int, crop, lut=None):
+def _stage(arrays, res: int, crop, lut=None, dest=None):
     """The pinned staging buffer: records, index tables (one per distinct image size), the LUT, then the image bytes.
+    crop "random" stages the whole Resize(res) output of each image (no crop) for stego_store_rows_u8: 7-word records
+    ending with (oh, ow, dest[i]), dest[i] being image i's byte offset in the ragged store.
     Returns (host uint8 tensor, table words, byte offset of the LUT or None)."""
     B = len(arrays)
-    tables, table_of = [], {}
+    tables, table_of, words = [], {}, 0
     for x in arrays:
         key = x.shape[:2]
         if key not in table_of:
-            table_of[key] = res * len(tables)  # rows then columns: res words each
-            tables.extend(index_tables(key[0], key[1], res, crop))
+            table_of[key] = words  # output rows then output columns
+            if crop == "random":
+                oh, ow = output_size(key[0], key[1], res, "center")
+                pair = (pillow_nearest_index(key[0], oh).astype(np.int32),
+                        pillow_nearest_index(key[1], ow).astype(np.int32))
+            else:
+                pair = index_tables(key[0], key[1], res, crop)
+            tables.extend(pair)
+            words += pair[0].size + pair[1].size
     table = np.concatenate(tables)
-    head = 8 * REC_WORDS * B
+    rec_words = ROW_REC_WORDS if crop == "random" else REC_WORDS
+    head = 8 * rec_words * B
     pos = head + 4 * table.size
     lut_at = None
     if lut is not None:
@@ -141,6 +152,9 @@ def _stage(arrays, res: int, crop, lut=None):
     buf = staging.numpy()
     rec = np.array([(off, x.shape[0], x.shape[1], table_of[x.shape[:2]]) for off, x in zip(offsets, arrays)],
                    dtype=np.int64)
+    if crop == "random":
+        sizes = [output_size(x.shape[0], x.shape[1], res, "center") for x in arrays]
+        rec = np.concatenate([rec, np.array(sizes, dtype=np.int64), np.asarray(dest, dtype=np.int64)[:, None]], 1)
     buf[:head] = rec.reshape(-1).view(np.uint8)
     buf[head:head + 4 * table.size] = table.view(np.uint8)
     if lut is not None:
